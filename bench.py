@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""bench.py -- acquisition candidates/sec (+ suggest() ms) at n=4096, d=32 on N B200s of one node.
+"""bench.py -- acquisition candidates/sec (+ suggest() ms) at n=4096, d=32 on N H100s of one node.
 
     python bench.py --gpus 1 --steps 20 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference ...        # the reference's CPU path (oracle port) on the host cores
+    python bench.py --gpus 1 --steps 20 --warmup 3 --dump-outputs DIR   # + what the last timed step computed, as .npy
 
 Metric (BASELINE.json): "acquisition candidates/sec + suggest() ms at n=4096 d=32; 1/2/4/8 GPU".
 One STEP = one pass of the scoring hot path over one candidate batch: fused posterior (mu, sigma^2) + MACE
@@ -20,6 +21,11 @@ Extra keys: `parity` (mu / sigma / objectives / front of a 2368-candidate sample
 cores, N = 1), `guard_flagged_frac` (rows the precision guard re-contracted on the FP32 pipe), `dense_regime` (a second
 workload, n=4096 d=8, where most candidates sit inside the data and the guard fires), `suggest` (suggest() ms with the
 fit / scoring split), `roofline`, `cpu_baseline`.
+
+--dump-outputs DIR (rank 0) writes, after the timed steps, what the last timed device step computed: the global front a
+caller receives (front_ids, front_objectives [K, 3], front_mu_sigma [K, 2]) and the per-candidate results of rank 0's
+shard (objectives [R, 3], mu [R], var [R] at the rows candidate_rows; every row while the four arrays stay under 48 MiB,
+otherwise a fixed seeded sample).  Inputs depend only on the arguments, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -44,10 +50,7 @@ N_OBS, DIM, Q = 4096, 32, 8
 KERNEL = "matern32"
 M_HEADLINE = 10000            # north-star suggest() workload: q=8, 10k candidates
 M_PER_GPU = 131072            # BASELINE config 5 shard size (1M candidates / 8 GPUs); weak scaling keeps it fixed
-# dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of the dominant kernel (32768 x 4096 chunk) from the committed
-# `ncu --set full` capture under profiles/ (r02_vnorm_h16_kernel_ncu_full_32768x4096.txt).  Algorithmic operand bytes per
-# launch: 32768*4096*4 (K* h0/h1) + 4096*4096*4/2 (Linv h0/h1, lower half) = 5.7e8.
-TRAFFIC_FILE = os.path.join(ROOT, "profiles", "r02_vnorm_h16_traffic.json")
+DUMP_BYTES = 48 << 20         # per-candidate arrays written by --dump-outputs (all rows below this, else a seeded sample)
 
 
 def synth(n, d, seed, fn="hartmann6"):
@@ -75,7 +78,7 @@ def candidates(m, d, seed):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     def __init__(self, index):
         self.index = index
@@ -150,11 +153,27 @@ def host_threads() -> int:
 
 
 def peaks():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        p = json.load(open(path))
-        return float(p["bf16_tflops"]), float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json, burst bf16)"
-    return 1590.0, 6650.0, "fallback (B200_PROFILING.md)"
+    """Dense FP16 tensor rate and HBM3 bandwidth from NVIDIA's H100 SXM data sheet (700 W part; a card with a lower power
+    limit may not reach them)."""
+    return 989.0, 3350.0, "H100 SXM data sheet (dense FP16, HBM3)"
+
+
+def dump_outputs(dirname, front, scored):
+    """--dump-outputs: the last timed step's front (ids, objectives, mu / sigma) and rank 0's per-candidate results"""
+    os.makedirs(dirname, exist_ok=True)
+    gid, F, ms = front
+    np.save(os.path.join(dirname, "front_ids.npy"), gid.numpy().astype(np.float64))
+    np.save(os.path.join(dirname, "front_objectives.npy"), F.numpy().astype(np.float32))
+    np.save(os.path.join(dirname, "front_mu_sigma.npy"), ms.numpy().astype(np.float32))
+    Fa, mu, var = (t.reshape(t.shape[0], -1).cpu() for t in scored)
+    m = Fa.shape[0]
+    rows = torch.arange(m)
+    if m * 6 * 4 > DUMP_BYTES:
+        rows = torch.randperm(m, generator=torch.Generator().manual_seed(0))[:DUMP_BYTES // 24].sort().values
+    np.save(os.path.join(dirname, "candidate_rows.npy"), rows.numpy().astype(np.float64))
+    np.save(os.path.join(dirname, "objectives.npy"), Fa[rows].numpy().astype(np.float32))
+    np.save(os.path.join(dirname, "mu.npy"), mu[rows].reshape(-1).numpy().astype(np.float32))
+    np.save(os.path.join(dirname, "var.npy"), var[rows].reshape(-1).numpy().astype(np.float32))
 
 
 # ------------------------------------------------------------------------------------------ CPU reference path
@@ -249,6 +268,7 @@ def main():
     ap.add_argument("--no-suggest", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-dense", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     args = ap.parse_args()
     steps, warmup = args.steps, max(args.warmup, 3)
     rank = int(os.environ.get("RANK", "0"))
@@ -285,7 +305,7 @@ def main():
         print(json.dumps(line))
         return
 
-    # ---------------------------------------------------------------- B200 arm
+    # ---------------------------------------------------------------- CUDA arm
     import torch.distributed as dist
     import hebo_b200
     from hebo_b200 import _lib, dist as hdist
@@ -345,7 +365,7 @@ def main():
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
         return float(t.item()), wall
 
-    def run_workload(n, d, seed, m, k_steps, k_warm, profile, fn="hartmann6"):
+    def run_workload(n, d, seed, m, k_steps, k_warm, profile, fn="hartmann6", dump=False):
         """fit on rank 0 (+ broadcast), then time the device step and the end-to-end step over m candidates per rank"""
         X, y = synth(n, d, seed, fn)
         yt = hebo_y_transform(y)
@@ -367,11 +387,19 @@ def main():
         lo = rank * m
         Xs_host = candidates(m, d, 1000 + rank).pin_memory()
         Xs_dev = Xs_host.to(dev)
+        last = {}
+
+        def score_dev(x):
+            # the library's default scoring call of sharded_score_front, keeping a reference to the per-candidate results
+            last["scored"] = gp.predict_mace(x, tau, kappa, 1e-4, None, None, seed=7 + lo, return_mu_var=True, device_out=True)
+            return last["scored"]
 
         def step_dev():
             # fused posterior + MACE over this rank's shard, device front, fixed-capacity pack, (N > 1: ONE all-gather + device
             # merge); everything is enqueued, nothing waits for the host
-            return hdist.sharded_score_front(gp, Xs_dev, lo, tau, kappa, 1e-4, seed=7, capacity=CAP, overlap=world > 1)
+            last["front"] = hdist.sharded_score_front(gp, Xs_dev, lo, tau, kappa, 1e-4, seed=7, capacity=CAP, overlap=world > 1,
+                                                      score_fn=score_dev)
+            return last["front"]
 
         def step_e2e():
             # the same work fed from HOST buffers: pinned candidates in (uploaded chunk by chunk under the scoring by the
@@ -395,15 +423,20 @@ def main():
             lib.hb_profile_enable(0)
         gs = (C.c_uint64 * 2)()
         lib.hb_guard_stats(gs, 1)
+        outputs = None
+        if dump and k_steps > 0:
+            outputs = (front_read(last["front"]), tuple(t.cpu() for t in last["scored"]))
         e2e_ms, _ = timed(step_e2e, k_steps)
         t_region1 = time.perf_counter()
         front = front_read(step_dev())
         return dict(gp=gp, X=X, yt=yt, tau=tau, kappa=kappa, total_ms=total_ms, wall_ms=wall_ms, e2e_ms=e2e_ms, launches=launches,
                     kms=kms.value, kn=kn.value, guard_frac=(gs[1] / gs[0]) if gs[0] else 0.0, fit_ms=fit_ms, region=(t_region0, t_region1),
-                    front_size=int(front[0].numel()))
+                    front_size=int(front[0].numel()), outputs=outputs)
 
     m = args.m_per_gpu
-    w = run_workload(N_OBS, DIM, 1234 + 5, m, steps, warmup, True)
+    w = run_workload(N_OBS, DIM, 1234 + 5, m, steps, warmup, True, dump=args.dump_outputs is not None and rank == 0)
+    if w["outputs"] is not None:
+        dump_outputs(args.dump_outputs, *w["outputs"])
     if rank == 0 and sampler.proc is not None:
         sampler.window(*w["region"])
     clocks = sampler.stop() if rank == 0 else None
@@ -434,18 +467,15 @@ def main():
     flop_per_launch = flop_per_cand * m / n_chunks
     k_avg_ms = w["kms"] / max(1, w["kn"])
     achieved = flop_per_launch / (k_avg_ms / 1e3) / 1e12 if k_avg_ms > 0 else None
-    traffic = None
-    if os.path.exists(TRAFFIC_FILE):
-        traffic = json.load(open(TRAFFIC_FILE)).get("dram_bytes_per_launch")
     roofline = {"bound": "tensor",
-                "kernel": "vnorm_h16_kernel (posterior variance V = K* Linv^T, row ||.||^2; tcgen05 cta_group::2 kind::f16 on a "
+                "kernel": "vnorm_h16_kernel (posterior variance V = K* Linv^T, row ||.||^2; wgmma f16 on a "
                           "two-level fp16 operand split, fp32 accumulate)",
                 "achieved": achieved, "peak": bf16_peak, "unit": "TFLOP/s", "frac": (achieved / bf16_peak) if achieved else None,
-                "traffic": traffic, "peak_source": which, "launches_timed": w["kn"], "avg_launch_ms": k_avg_ms,
+                "peak_source": which, "launches_timed": w["kn"], "avg_launch_ms": k_avg_ms,
                 "candidates_per_launch": m // n_chunks, "share_of_step": w["kms"] / w["total_ms"] if w["total_ms"] > 0 else None,
                 "note": "algorithmic flops = n^2 per candidate (triangular trsm form). The kernel issues 3 fp16 MMAs (h0*h0, h0*h1, "
-                        "h1*h0) per algorithmic MAC for ~2^-22 operand precision, so frac <= 1/3 of the measured bf16 peak by "
-                        "construction; tensor-pipe busy % is in profiles/"}
+                        "h1*h0) per algorithmic MAC for ~2^-22 operand precision, so frac <= 1/3 of the data-sheet peak by "
+                        "construction"}
 
     # ---- suggest() ms at the north-star point (n=4096, d=32, q=8, 10k candidates), fit/score split
     suggest = None

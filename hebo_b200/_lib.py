@@ -105,7 +105,7 @@ def lib():
         if not available():
             raise HeboB200Error(
                 f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a).  hebo_b200 has no CPU fallback.")
+                "(nvcc, sm_90a).  hebo_b200 has no CPU fallback.")
         handle = C.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(handle, name)

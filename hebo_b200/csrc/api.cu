@@ -444,7 +444,7 @@ int32_t hb_factorize_ex(const float *Xt, const int32_t *Xe, const float *y, int6
   float jitter = 0.0f;
   for (;;) {   // gp.py:140-157 jitter escalation of predict()
     // the prediction state is built ONCE per fit: keep it on the FP32 SIMT pipe (round-to-nearest accumulation);
-    // the 3xTF32 tensor path (TMEM accumulation is not RN, ~5e-6 relative) is used for the 100 gradient epochs only
+    // the 3xTF32 tensor path (the tensor cores' fp32 accumulation is not RN) is used for the 100 gradient epochs only
     s = factor_once(Xt, n, np, sp, raw, kern, noise_diag, jitter, w, st, /*allow_tc=*/false);
     if (s != HB_OK) return s;
     HB_CUDA(cudaMemcpyAsync(&hs->info, w.info, sizeof(int32_t), cudaMemcpyDeviceToHost, st));

@@ -14,7 +14,7 @@
 //                           -> one K = 64 update of the next diagonal tile -- with the last two links fused into the
 //                           diagonal task (the trsm result feeds the update straight from shared memory).
 //   after the block     : A[r, c >= ce] -= P P^T  with K = 512 -- the one large dense contraction of the
-//                         factorisation: tcgen05 3xTF32 (fit_tc.cu) in the fit loop, FP32 SIMT core otherwise.
+//                         factorisation: wgmma 3xTF32 (fit_tc.cu) in the fit loop, FP32 SIMT core otherwise.
 // This is what gpytorch's psd_safe_cholesky does through LAPACK potrf for HEBO/hebo/models/gp/gp.py:112-113,148.
 // `info` follows LAPACK: j > 0 = leading minor j not positive definite (first failing pivot wins).
 #include <limits.h>
@@ -621,7 +621,7 @@ int launch_cholesky(float *A, int64_t np, float *ws, int32_t *info, cudaStream_t
     }
     if (ce == np) break;
     timer.mark(1, st);
-    if (tc) {   // outer update on the tensor cores (tcgen05 3xTF32, fit_tc.cu)
+    if (tc) {   // outer update on the tensor cores (wgmma 3xTF32, fit_tc.cu)
       const int s = launch_chol_outer_update_tc(A, np, cb, ce, *tc, st);
       if (s != HB_OK) return s;
     } else {    // everything right of the block, K = block width

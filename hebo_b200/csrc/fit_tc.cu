@@ -1,4 +1,4 @@
-// Tensor-core (tcgen05, 3xTF32) versions of the n^3-class stages of one MLL epoch, expressed as tile tables for
+// Tensor-core (wgmma, 3xTF32) versions of the n^3-class stages of one MLL epoch, expressed as tile tables for
 // the generic kernel in tcgemm.cu.  Everything is arranged so that BOTH operands of every product are K-major:
 // next to Linv (lower) its transpose U = Linv^T (upper) is maintained, products are formed so that the output is
 // the operand the next stage needs, and the epilogue writes the hi/lo split (and the transposed split) directly.
@@ -20,16 +20,6 @@
 
 namespace hb {
 
-// cta_group::2 pair kernel (tcgemm2.cu) for every stage with >= 256-row structure; HEBO_B200_TC_1CTA=1 = the 1-CTA kernel
-static bool use_pairs() {
-  static int v = -1;
-  if (v < 0) {
-    const char *e = getenv("HEBO_B200_TC_1CTA");
-    v = (e && e[0] == '1') ? 0 : 1;
-  }
-  return v == 1;
-}
-
 // tables live in device memory: the current device is part of the key (a process may drive more than one GPU)
 static inline uint64_t table_key(int op, int64_t np, int64_t p1, int64_t p2) {
   int dev = 0;
@@ -44,21 +34,15 @@ int launch_chol_outer_update_tc(float *A, int64_t np, int64_t cb, int64_t ce, co
   int s = launch_split_region(A + ce * np + cb, np, tc.P_hi + ce * K, tc.P_lo + ce * K, K, np - ce, K, st);
   if (s != HB_OK) return s;
   chol_timer_mark(2, st);
-  const bool pairs = use_pairs();
   int ntiles = 0;
-  const uint64_t key = table_key(pairs ? 17 : 1, np, cb, ce);
+  const uint64_t key = table_key(1, np, cb, ce);
   const TcTile *tiles = tc_table_lookup(key, &ntiles);
   if (!tiles) {
     std::vector<TcTile> host;
     for (int64_t c0 = ce; c0 < np; c0 += 256)          // widest (longest) tile columns first
-      if (pairs) {                                      // c0 is a multiple of 256: 256-row pair tiles from the diagonal down
-        for (int64_t r0 = c0; r0 < np; r0 += 256)
-          host.push_back(TcTile{(int)r0, 0, (int)c0, 0, 0, (int)K, (int)r0, (int)c0, (r0 + GT < np) ? 3 : 1});
-      } else {
-        for (int64_t r0 = (c0 / GT) * GT; r0 < np; r0 += GT) {
-          if (c0 >= r0 + GT) continue;                  // tile entirely above the diagonal
-          host.push_back(TcTile{(int)r0, 0, (int)c0, 0, 0, (int)K, (int)r0, (int)c0});
-        }
+      for (int64_t r0 = (c0 / GT) * GT; r0 < np; r0 += GT) {
+        if (c0 >= r0 + GT) continue;                    // tile entirely above the diagonal
+        host.push_back(TcTile{(int)r0, 0, (int)c0, 0, 0, (int)K, (int)r0, (int)c0});
       }
     tiles = tc_table_store(key, host, &ntiles);
     if (!tiles) return HB_ERR_CUDA;
@@ -70,7 +54,7 @@ int launch_chol_outer_update_tc(float *A, int64_t np, int64_t cb, int64_t ce, co
   epi.ldc = np;
   epi.r0 = (int)ce;
   epi.ncols = (int)np;
-  return pairs ? launch_tcgemm2(P, P, tiles, ntiles, epi, st) : launch_tcgemm(P, P, 256, tiles, ntiles, epi, st);
+  return launch_tcgemm(P, P, 256, tiles, ntiles, epi, st);
 }
 
 // ------------------------------------------------------------------------------------------ triangular inverse
@@ -167,32 +151,15 @@ int launch_tri_inverse_tc(const float *L, int64_t np, float *Linv, const TcBuffe
   TcOperand opT{tc.T_hi, tc.T_lo, (uint64_t)np, (uint64_t)np, (uint64_t)np};
   for (int64_t b = GT; b < np; b *= 2) {
     const int bn = b >= 256 ? 256 : 128;
-    const bool pairs = use_pairs() && b >= 256;
     for (int phase = 0; phase < 2; ++phase) {
       int ntiles = 0;
-      const uint64_t key = table_key((pairs ? 18 : 2) + phase, np, b, 0);
+      const uint64_t key = table_key(2 + phase, np, b, 0);
       const TcTile *tiles = tc_table_lookup(key, &ntiles);
       if (!tiles) {
         std::vector<TcTile> host;
         for (int64_t s0 = 0; s0 + b < np; s0 += 2 * b) {
           const int64_t s2 = (np - s0 - b) < b ? (np - s0 - b) : b;
-          if (pairs) {
-            // 256-row pair tiles.  The shared k range is the union of the two halves' ranges; the extra part multiplies
-            // entries of the triangular factors that are stored as exact zeros.
-            if (phase == 0) {
-              for (int64_t c = 0; c < b; c += 256)
-                for (int64_t r = 0; r < s2; r += 256)
-                  host.push_back(TcTile{(int)(s0 + c), (int)s0, (int)(s0 + b + r), (int)s0, (int)c, (int)b, (int)(s0 + c),
-                                        (int)(s0 + b + r), 3});
-            } else {
-              for (int64_t r = ((s2 - 1) / 256) * 256; r >= 0; r -= 256)      // longest k ranges first
-                for (int64_t c = 0; c < b; c += 256) {
-                  const int64_t kend = (r + 256) < s2 ? (r + 256) : s2;
-                  host.push_back(TcTile{(int)(s0 + b + r), (int)(s0 + b), (int)(s0 + c), (int)(s0 + b), 0, (int)kend,
-                                        (int)(s0 + b + r), (int)(s0 + c), (r + GT < s2) ? 3 : 1});
-                }
-            }
-          } else if (phase == 0) {
+          if (phase == 0) {
             // Tt[c][r] = sum_{k >= c} U[s0+c][s0+k] * L[s0+b+r][s0+k]
             for (int64_t c = 0; c < b; c += GT)
               for (int64_t r = 0; r < s2; r += bn)
@@ -220,7 +187,7 @@ int launch_tri_inverse_tc(const float *L, int64_t np, float *Linv, const TcBuffe
         epi.sign = 1.0f;
         epi.C_hi = tc.T_hi;
         epi.C_lo = tc.T_lo;
-        s = pairs ? launch_tcgemm2(opU, opL, tiles, ntiles, epi, st) : launch_tcgemm(opU, opL, bn, tiles, ntiles, epi, st);
+        s = launch_tcgemm(opU, opL, bn, tiles, ntiles, epi, st);
       } else {
         epi.sign = -1.0f;
         epi.C = Linv;
@@ -228,7 +195,7 @@ int launch_tri_inverse_tc(const float *L, int64_t np, float *Linv, const TcBuffe
         epi.C_lo = tc.Linv_lo;
         epi.Ct_hi = tc.U_hi;
         epi.Ct_lo = tc.U_lo;
-        s = pairs ? launch_tcgemm2(opLinv, opT, tiles, ntiles, epi, st) : launch_tcgemm(opLinv, opT, bn, tiles, ntiles, epi, st);
+        s = launch_tcgemm(opLinv, opT, bn, tiles, ntiles, epi, st);
       }
       if (s != HB_OK) return s;
     }
@@ -239,21 +206,14 @@ int launch_tri_inverse_tc(const float *L, int64_t np, float *Linv, const TcBuffe
 // ------------------------------------------------------------------------------------------ K^-1 = U U^T
 int launch_kinv_tc(int64_t np, float *Kinv, const TcBuffers &tc, cudaStream_t st) {
   if (np <= 0 || np % GT != 0) return HB_ERR_INVALID;
-  const bool pairs = use_pairs();
   int ntiles = 0;
-  const uint64_t key = table_key(pairs ? 20 : 4, np, 0, 0);
+  const uint64_t key = table_key(4, np, 0, 0);
   const TcTile *tiles = tc_table_lookup(key, &ntiles);
   if (!tiles) {
     std::vector<TcTile> host;
-    if (pairs) {   // 256-row pair tiles; U[r][k] = 0 for k < r, so the second half ignores the first 128 k of the union
-      for (int64_t r0 = 0; r0 < np; r0 += 256)
-        for (int64_t c0 = 0; c0 <= r0; c0 += 256)
-          host.push_back(TcTile{(int)r0, 0, (int)c0, 0, (int)r0, (int)np, (int)r0, (int)c0, (r0 + GT < np) ? 3 : 1});
-    } else {
-      for (int64_t r0 = 0; r0 < np; r0 += GT)               // small r0 = long k range first
-        for (int64_t c0 = 0; c0 < r0 + GT; c0 += 256)
-          host.push_back(TcTile{(int)r0, 0, (int)c0, 0, (int)r0, (int)np, (int)r0, (int)c0});
-    }
+    for (int64_t r0 = 0; r0 < np; r0 += GT)                 // small r0 = long k range first
+      for (int64_t c0 = 0; c0 < r0 + GT; c0 += 256)
+        host.push_back(TcTile{(int)r0, 0, (int)c0, 0, (int)r0, (int)np, (int)r0, (int)c0});
     tiles = tc_table_store(key, host, &ntiles);
     if (!tiles) return HB_ERR_CUDA;
   }
@@ -264,7 +224,7 @@ int launch_kinv_tc(int64_t np, float *Kinv, const TcBuffers &tc, cudaStream_t st
   epi.C = Kinv;
   epi.ldc = np;
   epi.ncols = (int)np;
-  return pairs ? launch_tcgemm2(opU, opU, tiles, ntiles, epi, st) : launch_tcgemm(opU, opU, 256, tiles, ntiles, epi, st);
+  return launch_tcgemm(opU, opU, 256, tiles, ntiles, epi, st);
 }
 
 }  // namespace hb

@@ -93,7 +93,7 @@ int guard_stats(unsigned long long *out, int reset);
 int launch_mace_only(const float *mu, const float *var, int64_t m, float noise_var, float tau, float kappa, float eps,
                      const float *xi1, const float *xi2, uint64_t seed, float *F, cudaStream_t st);
 
-// fp16 two-level split tensor path of the posterior (vnorm_h16.cu: tcgen05 / TMEM / TMA)
+// fp16 two-level split tensor path of the posterior (vnorm_h16.cu: wgmma / TMA / mbarrier)
 int kstar_groups(int64_t np);
 int launch_kstar_plain(const float *xs, const int32_t *xe, int64_t mc, const ModelSpec &sp, const float *tab_s,
                        const float *x_mul, const float *x_add, const float *Zt,

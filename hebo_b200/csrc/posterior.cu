@@ -175,8 +175,8 @@ __global__ void __launch_bounds__(GTHREADS, 2) vnorm_kernel(const float *__restr
 }
 
 // ---- precision guard of the tensor path ------------------------------------------------------------------
-// sigma^2 = s - ||v||^2 cancels when a candidate sits on the data; the tensor cores' fp32 accumulation in TMEM is
-// not round-to-nearest (measured ~5e-6 relative on ||v||^2), which would exceed the 1e-4 sigma criterion once
+// sigma^2 = s - ||v||^2 cancels when a candidate sits on the data; the tensor cores' fp32 accumulation is
+// not round-to-nearest, which would exceed the 1e-4 sigma criterion once
 // sigma^2 < ~s/40.  Rows whose variance falls below theta * s (default 0.12) are therefore flagged and their ||v||^2 is
 // recomputed on the FP32 SIMT pipe from the same operands (K* = hi + lo); typical BO batches flag few rows, a
 // batch that sits entirely on the data degrades gracefully to the SIMT contraction.
@@ -432,10 +432,10 @@ int launch_posterior_mace(const float *Xs, const int32_t *Xe_s, int64_t m, int64
   if ((size_t)ws_bytes < posterior_ws_bytes(np, d, m_chunk)) return HB_ERR_INVALID;
   const size_t dyn = (size_t)sp.dtot() * (KS_ROWS + 1) * sizeof(float);
   if (dyn > 30 * 1024) return HB_ERR_INVALID;   // d + De <= 232 with the static 16 KB tile
-  const int64_t mc_pad_max = round_up(m_chunk, 2 * GT);   // 256: one CTA pair of the 2-SM tensor path
+  const int64_t mc_pad_max = round_up(m_chunk, 2 * GT);
   const int ncg = (int)ceil_div(np, KS_GROUP);
   const int nt = (int)(np / GT);
-  const bool tensor = Linv_hi != nullptr && Linv_lo != nullptr;   // tcgen05 path (two-level fp16 split), else FP32 SIMT
+  const bool tensor = Linv_hi != nullptr && Linv_lo != nullptr;   // wgmma path (two-level fp16 split), else FP32 SIMT
   const bool h16 = tensor;
   // workspace: the K* chunk (KS: fp32 rows of the SIMT / guard passes; KS2: the fp16 two-level split h0 | h1 of the
   // tensor path), the mean partials and the per-chunk partial-sum buffers.  (Building chunk i+1 on a side stream under
@@ -475,10 +475,10 @@ int launch_posterior_mace(const float *Xs, const int32_t *Xe_s, int64_t m, int64
     if (tensor) {
       const __half *kh0 = reinterpret_cast<const __half *>(KS2), *kh1 = kh0 + mc_pad_max * np;
       const int s = launch_vnorm_h16(kh0, kh1, mc_pad_max, reinterpret_cast<const __half *>(Linv_hi),
-                                     reinterpret_cast<const __half *>(Linv_lo), Linv_lo + np * np / 2, hyp, np, round_up(mc, 2 * GT),
+                                     reinterpret_cast<const __half *>(Linv_lo), Linv_lo + np * np / 2, hyp, np, mc_pad,
                                      mc_pad_max, vpart, st);
       if (s != HB_OK) return s;
-      nslots = (int)ceil_div(np, 256);
+      nslots = (int)ceil_div(np, 128);
       HB_CUDA(cudaMemsetAsync(fixcount, 0, sizeof(int32_t), st));
       guard_kernel<<<(int)ceil_div(mc, 256), 256, 0, st>>>(vpart, nslots, mc, mc_pad_max, hyp, guard_theta(), fixmap, fixlist, fixcount);
       const dim3 gf((unsigned)nt, (unsigned)(mc_pad / GT));

@@ -1,22 +1,17 @@
-// Shared device / host helpers of the tcgen05 kernels (vnorm_h16.cu, tcgemm.cu, tcgemm2.cu): mbarrier, TMA, UMMA commit,
-// TMEM load, shared-memory descriptors, the cuTensorMapEncodeTiled entry point and per-device one-time initialisation.
-// One copy instead of one per pipeline variant.  sm_100a only.
+// Shared device / host helpers of the Hopper tensor-core kernels (tcgemm.cu, vnorm_h16.cu): mbarrier, TMA, wgmma
+// shared-memory descriptors and instructions, and the cuTensorMapEncodeTiled entry point.  One copy instead of one per
+// kernel.  sm_90a only.
 //
-// Pipeline protocol shared by the three kernels (persistent, warp-specialised CTAs; a CTA pair for cta_group::2):
-//   warp 0 / lane 0  TMA producer   per k-block: wait empty[stage] -> (leader) arrive.expect_tx on full[stage] -> issue the
-//                                   cp.async.bulk.tensor loads of this CTA's operand boxes, completing on the LEADER's
-//                                   full[stage] (pair kernels: both CTAs' bytes land on one barrier, peer bit cleared in
-//                                   the barrier address)
-//   warp 1 / lane 0  MMA issuer     (leader CTA only) per tile: wait tempty (epilogue has drained the accumulators) ->
-//                                   per k-block: wait full[stage] -> tcgen05.mma over the swizzled smem descriptors ->
-//                                   tcgen05.commit on empty[stage] (multicast to both CTAs: frees the stage when the
-//                                   MMAs retire) -> after the last k-block tcgen05.commit on tfull
-//   warp 2           TMEM owner     tcgen05.alloc before / dealloc after the cluster-wide syncs
-//   warps 4..7       epilogue       wait tfull -> tcgen05.ld 32x32b (thread = accumulator row, warp q owns TMEM lanes
-//                                   32q..32q+31) -> arithmetic / stores -> arrive on the leader's tempty
-// Stage barriers carry one phase bit per ring wrap, accumulator barriers one per tile; every wait is bounded
-// (mbar_wait traps instead of hanging the GPU).  tcgen05.fence::before/after_thread_sync bracket every hand-over
-// between the async proxy (TMA, MMA) and generic-proxy code.
+// Pipeline protocol shared by the two kernels (persistent, warp-specialised CTAs of three warpgroups, 128-row tiles):
+//   warpgroup 0, thread 0   TMA producer  per k-block: wait empty[stage] -> arrive.expect_tx on full[stage] -> issue the
+//                                         cp.async.bulk.tensor loads of the stage's operand boxes (SWIZZLE_128B)
+//   warpgroups 1 and 2      consumers     each owns 64 rows of the tile and its fp32 accumulators in registers; per
+//                                         k-block: wait full[stage] -> wgmma.mma_async over the swizzled smem
+//                                         descriptors -> commit group -> wait until the PREVIOUS group has retired ->
+//                                         every thread arrives on empty[previous stage]; after the tile's last k-block
+//                                         wait for all groups, release the last stage and run the epilogue from registers
+//                                         while the producer already fills the ring for the next tile
+// Stage barriers carry one phase bit per ring wrap; every wait is bounded (mbar_wait traps instead of hanging the GPU).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -26,6 +21,7 @@ namespace hb {
 namespace tc {
 
 constexpr uint32_t SPIN_LIMIT = 1u << 26;
+constexpr int CONSUMER_THREADS = 256;   // two consumer warpgroups: the arrival count of every empty[stage] barrier
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -56,82 +52,116 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     if (++spins > SPIN_LIMIT) __trap();
   }
 }
+__device__ __forceinline__ void mbar_init_fence() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 
-// ---- single-CTA forms (tcgemm.cu)
-__device__ __forceinline__ void tma_load_2d_1cta(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c_inner, int c_outer) {
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c_inner, int c_outer) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
       "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c_inner), "r"(c_outer)
       : "memory");
 }
-__device__ __forceinline__ void umma_commit_1cta(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
 
-// ---- CTA-pair forms (cta_group::2: vnorm_h16.cu, tcgemm2.cu)
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c_inner, int c_outer) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c_inner), "r"(c_outer)
-      : "memory");
-}
-// commit of the pair's MMAs, arriving on the barrier at this offset in BOTH CTAs
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-               "h"((uint16_t)3)
-               : "memory");
-}
-// arrive on the barrier at this offset in the LEADER CTA (rank 0) from either CTA
-__device__ __forceinline__ void mbar_arrive_leader(uint32_t bar) {
-  asm volatile(
-      "{\n\t.reg .b32 rem;\n\t"
-      "mapa.shared::cluster.u32 rem, %0, 0;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [rem];\n\t}" ::"r"(bar)
-      : "memory");
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  __syncwarp();   // role lanes rejoin their warps before the cluster-wide barrier
-  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// K-major operand tile in the canonical SWIZZLE_128B layout TMA writes: 128-byte rows, 8-row groups 1024 B apart
+// K-major operand tile in the canonical SWIZZLE_128B layout TMA writes: 128-byte rows, 8-row groups 1024 B apart.  The
+// tile start must be 1024-byte aligned (base offset 0); a k step inside the swizzle row advances the start address.
 __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);   // start address, 16-byte units
-  d |= (uint64_t)1 << 16;                   // leading byte offset (ignored for swizzled K-major)
+  d |= (uint64_t)1 << 16;                   // leading byte offset (unused for swizzled K-major)
   d |= (uint64_t)(1024 >> 4) << 32;         // stride byte offset between 8-row groups
-  d |= (uint64_t)1 << 46;                   // descriptor version 1 (sm_100)
-  d |= (uint64_t)2 << 61;                   // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                   // SWIZZLE_128B
   return d;
 }
 
-// 32 lanes x 32 columns of fp32 accumulators -> registers (thread = TMEM lane = tile row)
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  tmem_ld32_nowait(taddr, r);
-  tmem_ld_wait();
+// keeps the compiler from moving accumulator accesses across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
 #pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x N] += A[64 x K] B[N x K]^T, both operands K-major in shared memory, fp32 accumulators in registers.  Register i
+// of thread (warp w of the warpgroup, lane l) holds row 16 w + l / 4 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (l % 4) + (i & 1).
+__device__ __forceinline__ void wgmma_tf32_n256(float (&d)[128], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+      "}, %128, %129, p, 1, 1;\n\t"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]),
+        "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]),
+        "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]),
+        "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]),
+        "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]),
+        "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]),
+        "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]),
+        "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]),
+        "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(1));
+}
+__device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1;\n\t"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(1));
+}
+__device__ __forceinline__ void wgmma_f16_n128(float (&d)[64], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1, 0, 0;\n\t"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(1));
 }
 
 // 3xTF32 operand split: hi = rn_tf32(x), lo = x - hi (exact)

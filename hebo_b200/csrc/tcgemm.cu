@@ -3,12 +3,12 @@
 //     C[tile] (op)= sum_{k in [kbeg, kend)} A[a_row + r][a_k0 + k] * B[b_row + c][b_k0 + k]
 //
 // Both operands K-major fp32, given as hi/lo split pairs (hi = rn_tf32(x), lo = x - hi).  Same machinery as
-// vnorm_h16.cu (protocol: tc_common.cuh) -- TMA SWIZZLE_128B boxes, mbarrier full/empty ring, tcgen05.mma kind::tf32 with fp32 accumulators in
-// TMEM (double buffered), warp-specialised persistent CTAs -- but driven by a TILE TABLE (built once per problem
-// size on the host, cached on the device) so triangular k-ranges, batched sub-problems and odd shapes need no
-// device-side index arithmetic, and with a store epilogue that can emit, from one TMEM read:
-//     fp32 C, the hi/lo split of C, and the hi/lo split of C^T (lanes = rows, so the transposed store is the
-//     perfectly coalesced one) -- or subtract the product from C in place (Cholesky trailing update).
+// vnorm_h16.cu (protocol: tc_common.cuh) -- TMA SWIZZLE_128B boxes, mbarrier full/empty ring, wgmma.mma_async kind tf32
+// with fp32 accumulators in registers, warp-specialised persistent CTAs -- but driven by a TILE TABLE (built once per
+// problem size on the host, cached on the device) so triangular k-ranges, batched sub-problems and odd shapes need no
+// device-side index arithmetic, and with a store epilogue that can emit, from the accumulator registers:
+//     fp32 C, the hi/lo split of C, and the hi/lo split of C^T -- or subtract the product from C in place (Cholesky
+//     trailing update).
 // Users: Cholesky outer trailing update (cholesky.cu), triangular inverse levels and K^-1 = U U^T (linalg.cu).
 #include <cuda.h>
 
@@ -23,18 +23,10 @@ namespace hb {
 namespace tcg {
 using namespace hb::tc;
 
-constexpr int BM = 128;
-constexpr int BK = 32;
-constexpr int UK = 8;
+constexpr int BM = 128;            // rows per tile: two consumer warpgroups of 64
+constexpr int BK = 32;             // fp32 elements per k-block = one 128-byte swizzle row
+constexpr int UK = 8;              // wgmma K for tf32
 
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
 template <int BN>
 struct Cfg {
   static constexpr int STAGES = (BN == 256) ? 2 : 3;
@@ -42,50 +34,46 @@ struct Cfg {
   static constexpr uint32_t B_BYTES = BN * BK * 4;
   static constexpr uint32_t STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
   static constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
-  static constexpr uint32_t TMEM_COLS = 2 * BN;
-  static constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
+  static constexpr int ACC = BN / 2;                       // accumulator registers per consumer thread
 };
 
 template <int BN>
-__global__ void __launch_bounds__(256, 1)
+__device__ __forceinline__ void mma3(float (&acc)[BN / 2], uint64_t da_hi, uint64_t da_lo, uint64_t db_hi, uint64_t db_lo) {
+  if constexpr (BN == 256) {
+    wgmma_tf32_n256(acc, da_hi, db_hi);
+    wgmma_tf32_n256(acc, da_hi, db_lo);
+    wgmma_tf32_n256(acc, da_lo, db_hi);
+  } else {
+    wgmma_tf32_n128(acc, da_hi, db_hi);
+    wgmma_tf32_n128(acc, da_hi, db_lo);
+    wgmma_tf32_n128(acc, da_lo, db_hi);
+  }
+}
+
+template <int BN>
+__global__ void __launch_bounds__(384, 1)
 tcgemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
               const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
               const TcTile *__restrict__ tiles, int ntiles, TcEpilogue epi) {
   using C = Cfg<BN>;
   extern __shared__ unsigned char smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;
-  const uint32_t bars = base + C::STAGES * C::STAGE_BYTES;
-  const uint32_t full_bar = bars;
-  const uint32_t empty_bar = bars + 8 * C::STAGES;
-  const uint32_t tfull_bar = bars + 16 * C::STAGES;
-  const uint32_t tempty_bar = tfull_bar + 16;
-  const uint32_t tmem_slot = tempty_bar + 16;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // SWIZZLE_128B tiles need 1024-byte alignment
+  const uint32_t full_bar = base + C::STAGES * C::STAGE_BYTES;
+  const uint32_t empty_bar = full_bar + 8 * C::STAGES;
+  const int wg = threadIdx.x >> 7;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(full_bar + 8 * s, 1);
-      mbar_init(empty_bar + 8 * s, 1);
+      mbar_init(empty_bar + 8 * s, CONSUMER_THREADS);
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar + 8 * a, 1);
-      mbar_init(tempty_bar + 8 * a, 128);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init_fence();
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(C::TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
-  if (warp == 0 && lane == 0) {
+  if (wg == 0) {
+    // ------------------------------------------------------------------ TMA producer
+    if (threadIdx.x != 0) return;
     int stage = 0;
     uint32_t phase = 0;
     for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
@@ -95,122 +83,100 @@ tcgemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constan
         const uint32_t sb = base + stage * C::STAGE_BYTES;
         const uint32_t fb = full_bar + 8 * stage;
         mbar_expect_tx(fb, C::STAGE_BYTES);
-        tma_load_2d_1cta(sb, &map_a_hi, fb, tl.a_k0 + k0, tl.a_row);
-        tma_load_2d_1cta(sb + C::A_BYTES, &map_a_lo, fb, tl.a_k0 + k0, tl.a_row);
-        tma_load_2d_1cta(sb + 2 * C::A_BYTES, &map_b_hi, fb, tl.b_k0 + k0, tl.b_row);
-        tma_load_2d_1cta(sb + 2 * C::A_BYTES + C::B_BYTES, &map_b_lo, fb, tl.b_k0 + k0, tl.b_row);
+        tma_load_2d(sb, &map_a_hi, fb, tl.a_k0 + k0, tl.a_row);
+        tma_load_2d(sb + C::A_BYTES, &map_a_lo, fb, tl.a_k0 + k0, tl.a_row);
+        tma_load_2d(sb + 2 * C::A_BYTES, &map_b_hi, fb, tl.b_k0 + k0, tl.b_row);
+        tma_load_2d(sb + 2 * C::A_BYTES + C::B_BYTES, &map_b_lo, fb, tl.b_k0 + k0, tl.b_row);
         if (++stage == C::STAGES) {
           stage = 0;
           phase ^= 1u;
         }
       }
     }
-  } else if (warp == 1 && lane == 0) {
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++it) {
-      const TcTile tl = tiles[t];
-      const int acc = it & 1;
-      const uint32_t acc_phase = (uint32_t)(it >> 1) & 1u;
-      mbar_wait(tempty_bar + 8 * acc, acc_phase ^ 1u);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + (uint32_t)(acc * BN);
-      uint32_t accumulate = 0;
-      for (int k0 = tl.kbeg; k0 < tl.kend; k0 += BK) {
-        mbar_wait(full_bar + 8 * stage, phase);
-        tc_fence_after();
-        const uint32_t sb = base + stage * C::STAGE_BYTES;
-        const uint64_t da_hi = make_sw128_desc(sb);
-        const uint64_t da_lo = make_sw128_desc(sb + C::A_BYTES);
-        const uint64_t db_hi = make_sw128_desc(sb + 2 * C::A_BYTES);
-        const uint64_t db_lo = make_sw128_desc(sb + 2 * C::A_BYTES + C::B_BYTES);
-#pragma unroll
-        for (int k = 0; k < BK / UK; ++k) {
-          const uint64_t adv = (uint64_t)((k * UK * 4) >> 4);
-          umma_tf32(tmem_d, da_hi + adv, db_hi + adv, C::IDESC, accumulate);
-          umma_tf32(tmem_d, da_hi + adv, db_lo + adv, C::IDESC, 1u);
-          umma_tf32(tmem_d, da_lo + adv, db_hi + adv, C::IDESC, 1u);
-          accumulate = 1u;
-        }
-        umma_commit_1cta(empty_bar + 8 * stage);
-        if (++stage == C::STAGES) {
-          stage = 0;
-          phase ^= 1u;
-        }
-      }
-      umma_commit_1cta(tfull_bar + 8 * acc);
-    }
-  } else if (warp >= 4) {
-    const int q = warp & 3;
-    int it = 0;
-    for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++it) {
-      const TcTile tl = tiles[t];
-      const int acc = it & 1;
-      const uint32_t acc_phase = (uint32_t)(it >> 1) & 1u;
-      const int64_t row = (int64_t)tl.c_row + q * 32 + lane;
-      mbar_wait(tfull_bar + 8 * acc, acc_phase);           // tables never contain empty k ranges
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN);
-#pragma unroll 1
-      for (int c = 0; c < BN; c += 32) {
-        float v[32];
-        tmem_ld32(taddr + (uint32_t)c, v);
-        const int64_t col0 = (int64_t)tl.c_col + c;
-        if (col0 >= epi.ncols) continue;                     // tile overhangs the matrix edge
-        if (epi.mode == TC_EPI_RMW_SUB) {
-          if (row >= epi.r0 && col0 >= epi.r0) {
-            float4 *p = reinterpret_cast<float4 *>(epi.C + row * epi.ldc + col0);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              float4 cv = p[i];
-              cv.x -= v[4 * i + 0];
-              cv.y -= v[4 * i + 1];
-              cv.z -= v[4 * i + 2];
-              cv.w -= v[4 * i + 3];
-              p[i] = cv;
-            }
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] *= epi.sign;
-          if (epi.C) {
-            float4 *p = reinterpret_cast<float4 *>(epi.C + row * epi.ldc + col0);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) p[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-          }
-          if (epi.C_hi || epi.Ct_hi) {
-            float h[32], l[32];
-#pragma unroll
-            for (int i = 0; i < 32; ++i) split1(v[i], h[i], l[i]);
-            if (epi.C_hi) {
-              float4 *ph = reinterpret_cast<float4 *>(epi.C_hi + row * epi.ldc + col0);
-              float4 *pl = reinterpret_cast<float4 *>(epi.C_lo + row * epi.ldc + col0);
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                ph[i] = make_float4(h[4 * i], h[4 * i + 1], h[4 * i + 2], h[4 * i + 3]);
-                pl[i] = make_float4(l[4 * i], l[4 * i + 1], l[4 * i + 2], l[4 * i + 3]);
-              }
-            }
-            if (epi.Ct_hi) {   // transposed: lanes are consecutive rows -> one coalesced 128-byte store per column
-#pragma unroll
-              for (int i = 0; i < 32; ++i) {
-                epi.Ct_hi[(col0 + i) * epi.ldct + row] = h[i];
-                epi.Ct_lo[(col0 + i) * epi.ldct + row] = l[i];
-              }
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(tempty_bar + 8 * acc);
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(C::TMEM_COLS) : "memory");
+
+  // -------------------------------------------------------------------- consumers: 64 rows each
+  const int half = wg - 1;
+  const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const uint32_t a_off = (uint32_t)half * 64 * BK * 4;    // this warpgroup's rows inside the A box
+  int stage = 0;
+  uint32_t phase = 0;
+  float acc[C::ACC];
+  for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+    const TcTile tl = tiles[t];
+#pragma unroll
+    for (int i = 0; i < C::ACC; ++i) acc[i] = 0.0f;
+    int prev = -1;
+    for (int k0 = tl.kbeg; k0 < tl.kend; k0 += BK) {
+      mbar_wait(full_bar + 8 * stage, phase);
+      const uint32_t sb = base + stage * C::STAGE_BYTES;
+      const uint64_t da_hi = make_sw128_desc(sb + a_off);
+      const uint64_t da_lo = make_sw128_desc(sb + C::A_BYTES + a_off);
+      const uint64_t db_hi = make_sw128_desc(sb + 2 * C::A_BYTES);
+      const uint64_t db_lo = make_sw128_desc(sb + 2 * C::A_BYTES + C::B_BYTES);
+      fence_regs(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / UK; ++k) {
+        const uint64_t adv = (uint64_t)((k * UK * 4) >> 4);   // 32 bytes per k-step inside the 128-byte swizzle row
+        mma3<BN>(acc, da_hi + adv, da_lo + adv, db_hi + adv, db_lo + adv);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                                         // the previous k-block's MMAs have retired
+      fence_regs(acc);
+      if (prev >= 0) mbar_arrive(empty_bar + 8 * prev);
+      prev = stage;
+      if (++stage == C::STAGES) {
+        stage = 0;
+        phase ^= 1u;
+      }
+    }
+    wgmma_wait<0>();
+    fence_regs(acc);
+    mbar_arrive(empty_bar + 8 * prev);                         // tables never contain empty k ranges
+
+    // epilogue from registers: thread holds rows rr and rr + 8, columns 8 j + cq, 8 j + cq + 1
+    const int64_t rr = (int64_t)tl.c_row + half * 64 + w * 16 + (lane >> 2);
+    const int cq = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int64_t col = (int64_t)tl.c_col + 8 * j + cq;
+      if (col >= epi.ncols) continue;                          // tile overhangs the matrix edge
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t row = rr + 8 * h;
+        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        if (epi.mode == TC_EPI_RMW_SUB) {
+          if (row >= epi.r0 && col >= epi.r0) {
+            float2 *p = reinterpret_cast<float2 *>(epi.C + row * epi.ldc + col);
+            float2 cv = *p;
+            cv.x -= v0;
+            cv.y -= v1;
+            *p = cv;
+          }
+          continue;
+        }
+        v0 *= epi.sign;
+        v1 *= epi.sign;
+        if (epi.C) *reinterpret_cast<float2 *>(epi.C + row * epi.ldc + col) = make_float2(v0, v1);
+        if (epi.C_hi || epi.Ct_hi) {
+          float h0, l0, h1, l1;
+          split1(v0, h0, l0);
+          split1(v1, h1, l1);
+          if (epi.C_hi) {
+            *reinterpret_cast<float2 *>(epi.C_hi + row * epi.ldc + col) = make_float2(h0, h1);
+            *reinterpret_cast<float2 *>(epi.C_lo + row * epi.ldc + col) = make_float2(l0, l1);
+          }
+          if (epi.Ct_hi) {
+            epi.Ct_hi[col * epi.ldct + row] = h0;
+            epi.Ct_lo[col * epi.ldct + row] = l0;
+            epi.Ct_hi[(col + 1) * epi.ldct + row] = h1;
+            epi.Ct_lo[(col + 1) * epi.ldct + row] = l1;
+          }
+        }
+      }
+    }
   }
 }
 
@@ -277,9 +243,9 @@ int launch_tcgemm(const TcOperand &A, const TcOperand &B, int bn, const TcTile *
   }
   const int grid = ntiles < num_sms ? ntiles : num_sms;
   if (bn == 256)
-    tcgemm_kernel<256><<<grid, 256, Cfg<256>::SMEM_BYTES, st>>>(ma_hi, ma_lo, mb_hi, mb_lo, tiles, ntiles, epi);
+    tcgemm_kernel<256><<<grid, 384, Cfg<256>::SMEM_BYTES, st>>>(ma_hi, ma_lo, mb_hi, mb_lo, tiles, ntiles, epi);
   else
-    tcgemm_kernel<128><<<grid, 256, Cfg<128>::SMEM_BYTES, st>>>(ma_hi, ma_lo, mb_hi, mb_lo, tiles, ntiles, epi);
+    tcgemm_kernel<128><<<grid, 384, Cfg<128>::SMEM_BYTES, st>>>(ma_hi, ma_lo, mb_hi, mb_lo, tiles, ntiles, epi);
   count_launches(1);
   HB_LAUNCH_CHECK("tcgemm");
   return HB_OK;

@@ -8,12 +8,11 @@
 
 namespace hb {
 
-struct TcTile {       // one 128 x BN output tile (tcgemm.cu) or one 256 x 256 PAIR tile (tcgemm2.cu)
+struct TcTile {       // one 128 x BN output tile
   int a_row, a_k0;    // A box: rows [a_row, a_row+128), columns a_k0 + k
   int b_row, b_k0;    // B box: rows [b_row, b_row+BN),  columns b_k0 + k
   int kbeg, kend;     // k range (multiples of 32, kend > kbeg)
   int c_row, c_col;   // output tile origin
-  int valid = 3;      // pair tiles: bit r set = the 128-row half of CTA rank r is written
 };
 
 enum { TC_EPI_STORE = 0, TC_EPI_RMW_SUB = 1 };
@@ -38,8 +37,6 @@ const TcTile *tc_table_lookup(uint64_t key, int *count);
 const TcTile *tc_table_store(uint64_t key, const std::vector<TcTile> &host, int *count);
 int launch_tcgemm(const TcOperand &A, const TcOperand &B, int bn, const TcTile *tiles, int ntiles, const TcEpilogue &epi,
                   cudaStream_t st);
-int launch_tcgemm2(const TcOperand &A, const TcOperand &B, const TcTile *tiles, int ntiles, const TcEpilogue &epi,
-                   cudaStream_t st);
 int launch_split_region(const float *x, int64_t ldx, float *hi, float *lo, int64_t ldo, int64_t rows, int64_t cols,
                         cudaStream_t st);
 

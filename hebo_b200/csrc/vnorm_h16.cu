@@ -1,14 +1,15 @@
-// Posterior variance contraction V = K* Linv^T, row sums of squares, on CTA pairs (cta_group::2).  The operands are
-// two-level fp16 splits (instead of the 3xTF32 hi/lo pairs of the fit GEMMs, tcgemm2.cu),
+// Posterior variance contraction V = K* Linv^T, row sums of squares, on the Hopper tensor cores (wgmma).  The operands are
+// two-level fp16 splits (instead of the 3xTF32 hi/lo pairs of the fit GEMMs, tcgemm.cu),
 //     x * scale = h0 + h1 / 2048,   h0 = rn_fp16(x * scale),  h1 = rn_fp16((x * scale - h0) * 2048)
 // (11 + 11 significant bits, the same 2^-22 as tf32 hi/lo; `scale` a power of two per matrix so that the largest entry
-// sits well inside the fp16 range, and the 2048-fold residual keeps small entries out of the subnormals).  kind::f16
-// MMAs run at TWICE the tf32 rate and an fp16 k-block of 64 elements occupies the same 128-byte swizzle row as 32
-// tf32 elements, so the contraction costs half the tensor time and half the L2 / shared-memory bytes per MAC:
-//     main  = sum h0a h0b            (TMEM accumulator 0)
-//     cross = sum h0a h1b + h1a h0b  (TMEM accumulator 1)         v = (main + cross / 2048) / (scale_a scale_b)
-// The dropped h1a h1b term is 2^-22 relative, as the lo*lo term of 3xTF32.  fp32 accumulation in TMEM as before (half as
-// many accumulate steps per dot product).  Pipeline protocol: tc_common.cuh.
+// sits well inside the fp16 range, and the 2048-fold residual keeps small entries out of the subnormals).  f16 MMAs
+// run at TWICE the tf32 rate and an fp16 k-block of 64 elements occupies the same 128-byte swizzle row as 32 tf32
+// elements, so the contraction costs half the tensor time and half the L2 / shared-memory bytes per MAC:
+//     main  = sum h0a h0b            (accumulator 0)
+//     cross = sum h0a h1b + h1a h0b  (accumulator 1)         v = (main + cross / 2048) / (scale_a scale_b)
+// The dropped h1a h1b term is 2^-22 relative, as the lo*lo term of 3xTF32.  fp32 accumulation in registers (half as
+// many accumulate steps per dot product).  A 128 x 128 tile keeps both accumulators of a consumer thread in 128
+// registers.  Pipeline protocol: tc_common.cuh.
 #include <cuda.h>
 
 #include <cuda_fp16.h>
@@ -25,37 +26,22 @@ namespace hb {
 namespace h16 {
 using namespace hb::tc;
 
-constexpr int BM = 128;            // candidates per tile (UMMA M)
-constexpr int BN = 256;            // Linv rows per tile (UMMA N)
+constexpr int BM = 128;            // candidates per tile (two consumer warpgroups of 64)
+constexpr int BN = 128;            // Linv rows per tile (wgmma N)
 constexpr int BK = 64;             // fp16 elements per k-block = one 128-byte swizzle row
-constexpr int UK = 16;             // UMMA K for kind::f16
+constexpr int UK = 16;             // wgmma K for f16
 constexpr int STAGES = 3;
 constexpr uint32_t A_BYTES = BM * BK * 2;                  // 16 KiB
-constexpr uint32_t B_BYTES = (BN / 2) * BK * 2;            // 16 KiB: each CTA stages half of the B tile
-constexpr uint32_t STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;  // 64 KiB per CTA
+constexpr uint32_t B_BYTES = BN * BK * 2;                  // 16 KiB
+constexpr uint32_t STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;  // 64 KiB
 constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-constexpr uint32_t TMEM_COLS = 512;
 
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// kind::f16 with fp16 A/B (format 0), fp32 accumulate (c_format 1), K-major, M=256 (pair), N=256
-constexpr uint32_t IDESC = (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)((2 * BM) >> 4) << 24);
-
-// Tile schedule: a host-built list per CTA pair (codes rt << 16 | J, terminated by -1).  Tiles are handed out in
-// BAND-MAJOR order -- all column tiles J of one 256-candidate band, heaviest (longest k range) first, before the next
-// band -- to whichever pair is least loaded at that point (a simulation of a dynamic scheduler with the k-block count +
-// an epilogue allowance as the cost; the last bands are dealt heaviest-first ACROSS bands so that the lists end with
-// cheap tiles).  Two effects: (1) the static round-robin it replaces left the pairs 13 % above the mean load at
-// 8192 x 4096; these lists are within 5 % (1.3 % at 32768 rows); (2) the ~16
-// pairs working on one band at the same time read its K* rows once from HBM and then from L2, instead of streaming the
-// whole K* chunk once per column tile (J-major order: 2.9x the algorithmic DRAM traffic, VERDICT r1).
+// Tile schedule: a host-built list per CTA (codes rt << 16 | J, terminated by -1).  Tiles are handed out in BAND-MAJOR
+// order -- all column tiles J of one 128-candidate band, heaviest (longest k range) first, before the next band -- to
+// whichever CTA is least loaded at that point (a simulation of a dynamic scheduler with the k-block count + an epilogue
+// allowance as the cost; the last bands are dealt heaviest-first ACROSS bands so that the lists end with cheap tiles).
+// Two effects: the CTAs finish within a few per cent of each other, and the CTAs working on one band at the same time
+// read its K* rows once from HBM and then from L2, instead of streaming the whole K* chunk once per column tile.
 __device__ __forceinline__ bool next_tile(const int32_t *__restrict__ list, int it, int &rt, int &J) {
   const int code = __ldg(list + it);
   rt = code >> 16;
@@ -63,161 +49,132 @@ __device__ __forceinline__ bool next_tile(const int32_t *__restrict__ list, int 
   return code >= 0;
 }
 
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(256, 1)
+__global__ void __launch_bounds__(384, 1)
 vnorm_h16_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
-                const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo, int np,
-                const int32_t *__restrict__ sched, int sched_len, int64_t mc_pad, float *__restrict__ vpart,
-                const float *__restrict__ hyp, const float *__restrict__ scale_b) {
+                 const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo, int np,
+                 const int32_t *__restrict__ sched, int sched_len, int64_t mc_pad, float *__restrict__ vpart,
+                 const float *__restrict__ hyp, const float *__restrict__ scale_b) {
   extern __shared__ unsigned char smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;            // SWIZZLE_128B tiles need 1024-byte alignment
-  const uint32_t bars = base + STAGES * STAGE_BYTES;       // 8-byte mbarriers after the tiles
-  const uint32_t full_bar = bars;                          // [STAGES]
-  const uint32_t empty_bar = bars + 8 * STAGES;            // [STAGES]
-  const uint32_t tfull_bar = bars + 16 * STAGES;           // [2]
-  const uint32_t tempty_bar = bars + 16 * STAGES + 16;     // [2]
-  const uint32_t tmem_slot = bars + 16 * STAGES + 32;      // u32 written by tcgen05.alloc
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();                 // 0 = leader (issues the MMAs)
-  const int32_t *my_tiles = sched + (int64_t)(blockIdx.x >> 1) * sched_len;   // this pair's list
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // SWIZZLE_128B tiles need 1024-byte alignment
+  const uint32_t full_bar = base + STAGES * STAGE_BYTES;          // [STAGES] 8-byte mbarriers after the tiles
+  const uint32_t empty_bar = full_bar + 8 * STAGES;               // [STAGES]
+  const int wg = threadIdx.x >> 7;
+  const int32_t *my_tiles = sched + (int64_t)blockIdx.x * sched_len;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar + 8 * s, 1);                      // used in the leader only: its producer's arrive + all bytes
-      mbar_init(empty_bar + 8 * s, 1);                     // one multicast commit per use, in both CTAs
+      mbar_init(full_bar + 8 * s, 1);                      // the producer's arrive + all bytes
+      mbar_init(empty_bar + 8 * s, CONSUMER_THREADS);
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar + 8 * a, 1);
-      mbar_init(tempty_bar + 8 * a, 256);                  // used in the leader only: 128 epilogue threads x 2 CTAs
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init_fence();
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  cluster_sync_all();                                      // barriers initialised + TMEM allocated in both CTAs
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
+  __syncthreads();
 
-  if (warp == 0 && lane == 0) {
+  if (wg == 0) {
     // ------------------------------------------------------------------ TMA producer
+    if (threadIdx.x != 0) return;
     int stage = 0;
     uint32_t phase = 0;
     for (int it = 0;; ++it) {
       int rt, J;
       if (!next_tile(my_tiles, it, rt, J)) break;
       const int kend = min((J + 1) * BN, np);
-      const int arow = rt * 2 * BM + (int)rank * BM;         // this CTA's 128 candidate rows of the 256-row tile
-      const int brow = J * BN + (int)rank * (BN / 2);        // this CTA's half of the Linv rows
       for (int k0 = 0; k0 < kend; k0 += BK) {
-        mbar_wait(empty_bar + 8 * stage, phase ^ 1u);        // own stage free (multicast commit of the leader)
+        mbar_wait(empty_bar + 8 * stage, phase ^ 1u);
         const uint32_t sb = base + stage * STAGE_BYTES;
-        const uint32_t fb = (full_bar + 8 * stage) & 0xFEFFFFFFu;   // the LEADER's full barrier (peer bit cleared)
-        if (rank == 0) mbar_expect_tx(full_bar + 8 * stage, 2 * STAGE_BYTES);
-        tma_load_2d_pair(sb, &map_a_hi, fb, k0, arow);
-        tma_load_2d_pair(sb + A_BYTES, &map_a_lo, fb, k0, arow);
-        tma_load_2d_pair(sb + 2 * A_BYTES, &map_b_hi, fb, k0, brow);
-        tma_load_2d_pair(sb + 2 * A_BYTES + B_BYTES, &map_b_lo, fb, k0, brow);
+        const uint32_t fb = full_bar + 8 * stage;
+        mbar_expect_tx(fb, STAGE_BYTES);
+        tma_load_2d(sb, &map_a_hi, fb, k0, rt * BM);
+        tma_load_2d(sb + A_BYTES, &map_a_lo, fb, k0, rt * BM);
+        tma_load_2d(sb + 2 * A_BYTES, &map_b_hi, fb, k0, J * BN);
+        tma_load_2d(sb + 2 * A_BYTES + B_BYTES, &map_b_lo, fb, k0, J * BN);
         if (++stage == STAGES) {
           stage = 0;
           phase ^= 1u;
         }
       }
     }
-  } else if (warp == 1 && lane == 0 && rank == 0) {
-    // ------------------------------------------------------------------ MMA issuer (leader CTA only)
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int it = 0;; ++it) {
-      int rt, J;
-      if (!next_tile(my_tiles, it, rt, J)) break;
-      const int kend = min((J + 1) * BN, np);
-      // two accumulators per tile (single buffered): MAIN takes hi*hi only, CROSS the two small hi*lo terms.  The
-      // tensor core's fp32 accumulation truncates (measured bias ~3e-8 per accumulate step relative to the running
-      // sum); keeping the 2^-11-sized cross terms out of the main sum cuts the truncations on it by 3x.
-      const uint32_t acc_phase = (uint32_t)it & 1u;
-      mbar_wait(tempty_bar, acc_phase ^ 1u);                 // epilogue drained the accumulators
-      tc_fence_after();
-      const uint32_t tmem_main = tmem_base;
-      const uint32_t tmem_cross = tmem_base + (uint32_t)BN;
-      uint32_t accumulate = 0;
-      for (int k0 = 0; k0 < kend; k0 += BK) {
-        mbar_wait(full_bar + 8 * stage, phase);              // TMA bytes have landed
-        tc_fence_after();
-        const uint32_t sb = base + stage * STAGE_BYTES;
-        const uint64_t da_hi = make_sw128_desc(sb);
-        const uint64_t da_lo = make_sw128_desc(sb + A_BYTES);
-        const uint64_t db_hi = make_sw128_desc(sb + 2 * A_BYTES);
-        const uint64_t db_lo = make_sw128_desc(sb + 2 * A_BYTES + B_BYTES);
-#pragma unroll
-        for (int k = 0; k < BK / UK; ++k) {
-          const uint64_t adv = (uint64_t)((k * UK * 2) >> 4);   // 32 bytes per k-step inside the 128-byte swizzle row
-          umma_f16(tmem_main, da_hi + adv, db_hi + adv, IDESC, accumulate);
-          umma_f16(tmem_cross, da_hi + adv, db_lo + adv, IDESC, accumulate);
-          umma_f16(tmem_cross, da_lo + adv, db_hi + adv, IDESC, 1u);
-          accumulate = 1u;
-        }
-        umma_commit_pair(empty_bar + 8 * stage);                  // frees the stage once these MMAs retire
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1u;
-        }
-      }
-      umma_commit_pair(tfull_bar);                                // accumulators complete -> epilogue
-    }
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------------ epilogue (TMEM -> registers -> row norm)
-    const int q = warp & 3;                                  // TMEM lane quarter this warp may access
-    const float inv = 1.0f / (pow2_scale(hyp[2], 1) * scale_b[0]);   // undo the operand scales (exact: powers of two)
-    const float lo_w = inv * (1.0f / 2048.0f);
-    for (int it = 0;; ++it) {
-      int rt, J;
-      if (!next_tile(my_tiles, it, rt, J)) break;
-      const uint32_t acc_phase = (uint32_t)it & 1u;
-      mbar_wait(tfull_bar, acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-      float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-      // software-pipelined drain: the loads of chunk c+1 are in flight while chunk c is reduced (tcgen05.wait::ld waits
-      // for everything outstanding, so the wait sits AFTER the arithmetic of the previous chunk)
-      uint32_t v[2][32], w[2][32];
-      tmem_ld32_nowait(taddr, v[0]);                                 // h0*h0
-      tmem_ld32_nowait(taddr + (uint32_t)BN, w[0]);                  // (h0*h1 + h1*h0), still times 2048
-      tmem_ld_wait();
-#pragma unroll
-      for (int c = 0; c < BN / 32; ++c) {
-        const int cur = c & 1, nxt = cur ^ 1;
-        if (c + 1 < BN / 32) {
-          tmem_ld32_nowait(taddr + (uint32_t)((c + 1) * 32), v[nxt]);
-          tmem_ld32_nowait(taddr + (uint32_t)(BN + (c + 1) * 32), w[nxt]);
-        }
-#pragma unroll
-        for (int i = 0; i < 32; i += 4) {
-          const float x0 = fmaf(__uint_as_float(w[cur][i + 0]), lo_w, __uint_as_float(v[cur][i + 0]) * inv);
-          const float x1 = fmaf(__uint_as_float(w[cur][i + 1]), lo_w, __uint_as_float(v[cur][i + 1]) * inv);
-          const float x2 = fmaf(__uint_as_float(w[cur][i + 2]), lo_w, __uint_as_float(v[cur][i + 2]) * inv);
-          const float x3 = fmaf(__uint_as_float(w[cur][i + 3]), lo_w, __uint_as_float(v[cur][i + 3]) * inv);
-          s0 = fmaf(x0, x0, s0);
-          s1 = fmaf(x1, x1, s1);
-          s2 = fmaf(x2, x2, s2);
-          s3 = fmaf(x3, x3, s3);
-        }
-        if (c + 1 < BN / 32) tmem_ld_wait();
-      }
-      tc_fence_before();
-      mbar_arrive_leader(tempty_bar);              // 256 arrivals (both CTAs) release the accumulator
-      vpart[(int64_t)J * mc_pad + (int64_t)rt * 2 * BM + (int64_t)rank * BM + q * 32 + lane] = (s0 + s1) + (s2 + s3);
-    }
+    return;
   }
-  tc_fence_before();
-  cluster_sync_all();                                      // nobody in the pair touches TMEM / peer barriers any more
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
+
+  // -------------------------------------------------------------------- consumers: 64 candidate rows each
+  const int half = wg - 1;
+  const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const uint32_t a_off = (uint32_t)half * 64 * BK * 2;
+  const float inv = 1.0f / (pow2_scale(hyp[2], 1) * scale_b[0]);   // undo the operand scales (exact: powers of two)
+  const float lo_w = inv * (1.0f / 2048.0f);
+  int stage = 0;
+  uint32_t phase = 0;
+  // two accumulators per tile: MAIN takes hi*hi only, CROSS the two small hi*lo terms.  The tensor core's fp32
+  // accumulation truncates; keeping the 2^-11-sized cross terms out of the main sum cuts the truncations on it by 3x.
+  float acc_main[BN / 2], acc_cross[BN / 2];
+  for (int it = 0;; ++it) {
+    int rt, J;
+    if (!next_tile(my_tiles, it, rt, J)) break;
+    const int kend = min((J + 1) * BN, np);
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) {
+      acc_main[i] = 0.0f;
+      acc_cross[i] = 0.0f;
+    }
+    int prev = -1;
+    for (int k0 = 0; k0 < kend; k0 += BK) {
+      mbar_wait(full_bar + 8 * stage, phase);              // TMA bytes have landed
+      const uint32_t sb = base + stage * STAGE_BYTES;
+      const uint64_t da_hi = make_sw128_desc(sb + a_off);
+      const uint64_t da_lo = make_sw128_desc(sb + A_BYTES + a_off);
+      const uint64_t db_hi = make_sw128_desc(sb + 2 * A_BYTES);
+      const uint64_t db_lo = make_sw128_desc(sb + 2 * A_BYTES + B_BYTES);
+      fence_regs(acc_main);
+      fence_regs(acc_cross);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / UK; ++k) {
+        const uint64_t adv = (uint64_t)((k * UK * 2) >> 4);   // 32 bytes per k-step inside the 128-byte swizzle row
+        wgmma_f16_n128(acc_main, da_hi + adv, db_hi + adv);
+        wgmma_f16_n128(acc_cross, da_hi + adv, db_lo + adv);
+        wgmma_f16_n128(acc_cross, da_lo + adv, db_hi + adv);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                                     // the previous k-block's MMAs have retired
+      fence_regs(acc_main);
+      fence_regs(acc_cross);
+      if (prev >= 0) mbar_arrive(empty_bar + 8 * prev);
+      prev = stage;
+      if (++stage == STAGES) {
+        stage = 0;
+        phase ^= 1u;
+      }
+    }
+    wgmma_wait<0>();
+    fence_regs(acc_main);
+    fence_regs(acc_cross);
+    mbar_arrive(empty_bar + 8 * prev);
+
+    // epilogue: thread holds rows r and r + 8 of its warpgroup's 64, two columns of every 8; the 4 lanes of a quad share
+    // the rows
+    float s0 = 0.f, s1 = 0.f, t0 = 0.f, t1 = 0.f;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const float x0 = fmaf(acc_cross[4 * j + 0], lo_w, acc_main[4 * j + 0] * inv);
+      const float x1 = fmaf(acc_cross[4 * j + 1], lo_w, acc_main[4 * j + 1] * inv);
+      const float x2 = fmaf(acc_cross[4 * j + 2], lo_w, acc_main[4 * j + 2] * inv);
+      const float x3 = fmaf(acc_cross[4 * j + 3], lo_w, acc_main[4 * j + 3] * inv);
+      s0 = fmaf(x0, x0, s0);
+      s1 = fmaf(x1, x1, s1);
+      t0 = fmaf(x2, x2, t0);
+      t1 = fmaf(x3, x3, t1);
+    }
+    float s = s0 + s1, t = t0 + t1;
+    s += __shfl_xor_sync(0xffffffffu, s, 1);
+    t += __shfl_xor_sync(0xffffffffu, t, 1);
+    s += __shfl_xor_sync(0xffffffffu, s, 2);
+    t += __shfl_xor_sync(0xffffffffu, t, 2);
+    if ((lane & 3) == 0) {
+      float *out = vpart + (int64_t)J * mc_pad + (int64_t)rt * BM + half * 64 + w * 16 + (lane >> 2);
+      out[0] = s;
+      out[8] = t;
+    }
   }
 }
 
@@ -243,34 +200,34 @@ namespace h16 {
 
 struct SchedEntry {
   int32_t *dev = nullptr;
-  int len = 0, pairs = 0;
+  int len = 0, ctas = 0;
 };
 struct SchedKey {
-  int dev, np, n_rt2, pairs;
+  int dev, np, n_rt, ctas;
   bool operator<(const SchedKey &o) const {
     if (dev != o.dev) return dev < o.dev;
     if (np != o.np) return np < o.np;
-    if (n_rt2 != o.n_rt2) return n_rt2 < o.n_rt2;
-    return pairs < o.pairs;
+    if (n_rt != o.n_rt) return n_rt < o.n_rt;
+    return ctas < o.ctas;
   }
 };
 
-static const SchedEntry *get_schedule(int dev, int np, int n_rt2, int pairs, cudaStream_t st) {
+static const SchedEntry *get_schedule(int dev, int np, int n_rt, int ctas, cudaStream_t st) {
   static std::map<SchedKey, SchedEntry> cache;
-  const SchedKey key{dev, np, n_rt2, pairs};
+  const SchedKey key{dev, np, n_rt, ctas};
   auto it = cache.find(key);
   if (it != cache.end()) return &it->second;
   const int n_j = (np + BN - 1) / BN;
-  constexpr int EPI_COST = 3;   // epilogue + accumulator hand-over in k-block units (~4.5k of 1.5k cycles per k-block)
-  std::vector<std::vector<int32_t>> lists(pairs);
-  std::vector<long long> load(pairs, 0);
+  constexpr int EPI_COST = 1;   // epilogue in k-block units (a register drain and one shuffle reduction per tile)
+  std::vector<std::vector<int32_t>> lists(ctas);
+  std::vector<long long> load(ctas, 0);
   // band-major body, then the tiles of the last TAIL_BANDS bands heaviest-first across bands (an LPT tail: the list ends
-  // with the cheapest tiles, which levels the pairs to ~1-5 % instead of one heavy tile of overhang)
-  constexpr int TAIL_BANDS = 8;
-  const int body = std::max(0, n_rt2 - TAIL_BANDS);
+  // with the cheapest tiles, which levels the CTAs instead of leaving one heavy tile of overhang)
+  constexpr int TAIL_BANDS = 16;
+  const int body = std::max(0, n_rt - TAIL_BANDS);
   auto give = [&](int rt, int J) {
     int best = 0;
-    for (int p = 1; p < pairs; ++p)
+    for (int p = 1; p < ctas; ++p)
       if (load[p] < load[best]) best = p;
     const int kend = std::min((J + 1) * BN, np);
     load[best] += kend / BK + EPI_COST;
@@ -279,15 +236,15 @@ static const SchedEntry *get_schedule(int dev, int np, int n_rt2, int pairs, cud
   for (int rt = 0; rt < body; ++rt)
     for (int J = n_j - 1; J >= 0; --J) give(rt, J);
   for (int J = n_j - 1; J >= 0; --J)
-    for (int rt = body; rt < n_rt2; ++rt) give(rt, J);
+    for (int rt = body; rt < n_rt; ++rt) give(rt, J);
   size_t len = 0;
   for (auto &l : lists) len = std::max(len, l.size());
   len += 1;
-  std::vector<int32_t> flat((size_t)pairs * len, -1);
-  for (int p = 0; p < pairs; ++p) std::copy(lists[p].begin(), lists[p].end(), flat.begin() + (size_t)p * len);
+  std::vector<int32_t> flat((size_t)ctas * len, -1);
+  for (int p = 0; p < ctas; ++p) std::copy(lists[p].begin(), lists[p].end(), flat.begin() + (size_t)p * len);
   SchedEntry e;
   e.len = (int)len;
-  e.pairs = pairs;
+  e.ctas = ctas;
   if (cudaMalloc(&e.dev, flat.size() * sizeof(int32_t)) != cudaSuccess) return nullptr;
   if (cudaMemcpyAsync(e.dev, flat.data(), flat.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st) != cudaSuccess ||
       cudaStreamSynchronize(st) != cudaSuccess)   // `flat` is pageable and dies with this frame
@@ -298,12 +255,12 @@ static const SchedEntry *get_schedule(int dev, int np, int n_rt2, int pairs, cud
 }  // namespace h16
 
 // ks_h0 / ks_h1 [ks_rows, np] fp16 split of K* (scale 2^k from the outputscale hyp[2]); linv_h0 / linv_h1 [np, np] fp16 split
-// of Linv with the device scalar scale_b; ks_rows and mc_pad multiples of 256
+// of Linv with the device scalar scale_b; ks_rows and mc_pad multiples of 128
 int launch_vnorm_h16(const __half *ks_h0, const __half *ks_h1, int64_t ks_rows, const __half *linv_h0, const __half *linv_h1,
                      const float *scale_b, const float *hyp, int64_t np, int64_t mc_pad, int64_t vpart_stride, float *vpart,
                      cudaStream_t st) {
   using namespace h16;
-  if (np % TILE != 0 || mc_pad % (2 * BM) != 0 || mc_pad > ks_rows || np > 65535 * BN || mc_pad / (2 * BM) > 32767) return HB_ERR_INVALID;
+  if (np % TILE != 0 || mc_pad % BM != 0 || mc_pad > ks_rows || np > 65535 * BN || mc_pad / BM > 32767) return HB_ERR_INVALID;
   static PerDevice once;
   bool fresh = false;
   const int dev = once.slot(&fresh);
@@ -316,23 +273,23 @@ int launch_vnorm_h16(const __half *ks_h0, const __half *ks_h1, int64_t ks_rows, 
   CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
   if (!make_map(&ma_hi, ks_h0, (uint64_t)ks_rows, (uint64_t)np, BM) ||
       !make_map(&ma_lo, ks_h1, (uint64_t)ks_rows, (uint64_t)np, BM) ||
-      !make_map(&mb_hi, linv_h0, (uint64_t)np, (uint64_t)np, BN / 2) ||
-      !make_map(&mb_lo, linv_h1, (uint64_t)np, (uint64_t)np, BN / 2)) {
+      !make_map(&mb_hi, linv_h0, (uint64_t)np, (uint64_t)np, BN) ||
+      !make_map(&mb_lo, linv_h1, (uint64_t)np, (uint64_t)np, BN)) {
     set_error(cudaErrorUnknown, "cuTensorMapEncodeTiled");
     return HB_ERR_CUDA;
   }
-  const int n_rt2 = (int)(mc_pad / (2 * BM));
+  const int n_rt = (int)(mc_pad / BM);
   const int n_j = (int)ceil_div(np, BN);
-  const int total = n_rt2 * n_j;
-  int pairs = once.sms[dev] / 2;
-  if (total < pairs) pairs = total;
-  const SchedEntry *sc = get_schedule(dev, (int)np, n_rt2, pairs, st);
+  const int total = n_rt * n_j;
+  int ctas = once.sms[dev];
+  if (total < ctas) ctas = total;
+  const SchedEntry *sc = get_schedule(dev, (int)np, n_rt, ctas, st);
   if (!sc) {
     set_error(cudaErrorMemoryAllocation, "vnorm_h16 schedule table");
     return HB_ERR_CUDA;
   }
   prof_begin(st);
-  vnorm_h16_kernel<<<2 * pairs, 256, SMEM_BYTES, st>>>(ma_hi, ma_lo, mb_hi, mb_lo, (int)np, sc->dev, sc->len, vpart_stride, vpart,
+  vnorm_h16_kernel<<<ctas, 384, SMEM_BYTES, st>>>(ma_hi, ma_lo, mb_hi, mb_lo, (int)np, sc->dev, sc->len, vpart_stride, vpart,
                                                      hyp, scale_b);
   prof_end(st);
   count_launches(1);
@@ -372,7 +329,7 @@ __global__ void split_h16_kernel(const float *__restrict__ x, int64_t n4, __half
 int launch_split_h16(const float *x, int64_t count, __half *h0, __half *h1, float *scale_slot, cudaStream_t st) {
   if (count % 4 != 0) return HB_ERR_INVALID;
   HB_CUDA(cudaMemsetAsync(scale_slot, 0, 2 * sizeof(float), st));
-  const int blocks = (int)std::min<int64_t>(ceil_div(count / 4, 256), 148 * 8);
+  const int blocks = (int)std::min<int64_t>(ceil_div(count / 4, 256), 1024);
   absmax_kernel<<<blocks, 256, 0, st>>>(x, count / 4, reinterpret_cast<unsigned int *>(scale_slot + 1));
   split_h16_kernel<<<blocks, 256, 0, st>>>(x, count / 4, h0, h1, scale_slot);
   count_launches(2);

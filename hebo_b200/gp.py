@@ -1,9 +1,9 @@
-"""B200-native exact-GP surrogate behind HEBO's ``BaseModel`` plugin surface.
+"""H100-native exact-GP surrogate behind HEBO's ``BaseModel`` plugin surface.
 
 Drop-in for ``hebo.models.gp.gp.GP`` (HEBO/hebo/models/gp/gp.py:35-184): same constructor keys, same
 ``fit / predict / noise / sample_y / sample_f`` contract, CPU tensors in and out, but the arithmetic
 (Gram build, Cholesky, solves, log-det, MLL gradient, pSGLD loop, posterior, MACE) runs in the hand-written
-sm_100a kernels of libhebo_b200.so through the C ABI -- no GPyTorch, no CPU fallback.
+sm_90a kernels of libhebo_b200.so through the C ABI -- no GPyTorch, no CPU fallback.
 
 Extra conf keys (unknown keys are ignored by the reference's ``conf.get``, so they are safe to pass through
 ``HEBO(model_config=...)``):
@@ -70,7 +70,7 @@ class GP(BaseModel):
         self.ard_kernel = conf.get("ard_kernel", True)
         self.xscaler = MinMaxScaler((-1, 1))
         self.yscaler = StandardScaler()
-        # B200 extras
+        # extras of this implementation
         self.kernel = self._resolve_kernel(conf)
         self.kern_id = _lib.KERNEL_IDS[self.kernel]
         self.device = torch.device(conf.get("device", "cuda"))
@@ -80,7 +80,7 @@ class GP(BaseModel):
         self.warp_a = conf.get("warp_a", None)
         self.warp_b = conf.get("warp_b", None)
         self.langevin = conf.get("langevin", True)
-        self.tensor_cores = conf.get("tensor_cores", True)   # posterior contraction on tcgen05 (fp16 two-level split / 3xTF32) vs FP32 SIMT
+        self.tensor_cores = conf.get("tensor_cores", True)   # posterior contraction on the tensor cores (wgmma, fp16 two-level split) vs FP32 SIMT
         # categorical columns: one learned embedding table per column (layers.py:14-34), product kernel (gp_util.py:54-57)
         self.num_uniqs = [int(v) for v in conf.get("num_uniqs", [])] if self.num_enum > 0 else []
         if self.num_enum > 0:

@@ -1,4 +1,4 @@
-"""HEBO.suggest / observe on the B200 path (SURVEY rows a1-a3, a14-a18, f1).
+"""HEBO.suggest / observe on the CUDA path (SURVEY rows a1-a3, a14-a18, f1).
 
 Mirrors the control flow of HEBO/hebo/optimizers/hebo.py:119-229 -- Sobol start-up, y power transform with the raw-y
 refit fallback, GP fit, tau = mu(best_x), kappa schedule, MACE, Pareto set, duplicate check, Sobol top-up, random pick of q

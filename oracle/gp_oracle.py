@@ -6,7 +6,7 @@ only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s ``cpu_baseline``
 
 PARITY UNPINNED at the gpytorch boundary: the arithmetic of this path lives in the
 third-party ``gpytorch`` package (``HEBO/requirements.txt:6`` ``gpytorch>=1.4.0``, unpinned,
-not vendored under /root/reference and not installable here), and no reference test holds a
+not vendored in the reference repository), and no reference test holds a
 numeric golden vector for it (``HEBO/test/util.py:13-19`` checks shape/finite/positive only).
 What *is* pinned: the MACE arithmetic, the scalers and the pSGLD rule are checked against the
 reference's real ``acq.py`` / ``scalers.py`` loaded by path (``oracle/ref_loader.py``,

@@ -1,13 +1,12 @@
-"""Load the reference's real ``acq.py`` / ``scalers.py`` / ``base_model.py`` by path.
+"""Load the reference's real source files (HEBO's ``acq.py`` / ``scalers.py`` / ``base_model.py`` and a few layers) by
+path.
 
-TEST INFRASTRUCTURE ONLY, and only usable in the build container: /root/reference does not exist
-on the GPU box, so nothing that runs there (``-m gpu`` tests, smoke(), bench.py) may call this.
-It is used by ``oracle/make_golden.py`` to generate committed fixtures and by the CPU test
-``tests/test_oracle.py`` (skipped when /root/reference is absent) to pin the oracle's MACE /
-scaler restatements against the reference's own code.
+TEST INFRASTRUCTURE ONLY: used by ``oracle/make_golden.py`` to regenerate the committed fixtures under tests/golden/ from
+a checkout of the HEBO sources, given as ``HEBO_SRC=<directory that contains hebo/>``.  Nothing else (tests, smoke(),
+bench.py) reads the reference; the tests compare against the stored vectors.
 
-``import hebo`` itself fails here (pymoo / gpytorch missing: evolution_optimizer.py:14, gp.py:14);
-the files below import only torch/numpy/sklearn and load unmodified under stub parent packages.
+``import hebo`` itself needs pymoo / gpytorch (evolution_optimizer.py:14, gp.py:14); the files below import only
+torch/numpy/sklearn/pandas and load unmodified under stub parent packages.
 """
 from __future__ import annotations
 
@@ -16,11 +15,35 @@ import os
 import sys
 import types
 
-REF_ROOT = "/root/reference/HEBO/hebo"
+REF_ROOT = os.path.join(os.environ.get("HEBO_SRC", ""), "hebo")
 
 
 def available() -> bool:
-    return os.path.isfile(os.path.join(REF_ROOT, "acquisitions", "acq.py"))
+    return bool(os.environ.get("HEBO_SRC")) and os.path.isfile(os.path.join(REF_ROOT, "acquisitions", "acq.py"))
+
+
+def load_file(modname: str, relpath: str, stubs=()):
+    """Load one reference source file unmodified under stub parents: stubs = [(module name, attribute names)]"""
+    saved = {}
+    for name, attrs in stubs:
+        saved[name] = sys.modules.get(name)
+        m = types.ModuleType(name)
+        m.__path__ = []
+        for k in attrs:
+            setattr(m, k, type(k, (), {}))
+        sys.modules[name] = m
+    try:
+        spec = importlib.util.spec_from_file_location(modname, os.path.join(REF_ROOT, relpath))
+        mod = importlib.util.module_from_spec(spec)
+        sys.modules[modname] = mod
+        spec.loader.exec_module(mod)
+        return mod
+    finally:
+        for name, old in saved.items():
+            if old is None:
+                sys.modules.pop(name, None)
+            else:
+                sys.modules[name] = old
 
 
 def _load(modname: str, relpath: str):
@@ -36,7 +59,7 @@ def _load(modname: str, relpath: str):
 def load_reference():
     """Returns a namespace with the reference's MACE, Mean, Sigma, BaseModel, scalers."""
     if not available():
-        raise RuntimeError("/root/reference is not present")
+        raise RuntimeError("set HEBO_SRC to a checkout of the HEBO sources")
     for pkg in ("_hebo_ref", "_hebo_ref.models", "_hebo_ref.acquisitions"):
         if pkg not in sys.modules:
             m = types.ModuleType(pkg)

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box).  Everything goes through the reference-facing classes,
+"""GPU parity tests (run with -m gpu on an H100).  Everything goes through the reference-facing classes,
 i.e. through the C ABI of libhebo_b200.so; the oracle is only the checker.
 
 Tolerances (BASELINE.md section 5 / north_star):
@@ -412,7 +412,7 @@ def test_cholesky_two_level_blocking_shapes(NP):
 
 
 def test_tensor_path_guard_recomputes_cancelling_rows_on_fp32():
-    """tcgen05 fp16-split path vs the FP32 SIMT path: rows with sigma^2 << s (dense data: heavy cancellation) are
+    """Tensor-core fp16-split path vs the FP32 SIMT path: rows with sigma^2 << s (dense data: heavy cancellation) are
     flagged by the guard and recomputed on the FP32 pipe (fp64 chunk accumulation); the other rows agree to ~1e-5."""
     n, d, m = 700, 3, 3000
     X, y = seeded_problem(n, d, 21)

@@ -97,7 +97,7 @@ def test_langevin_draws_of_a_mixed_model_follow_registration_order_and_shapes():
 
 @pytest.mark.gpu
 def test_generic_mace_path_matches_reference_vectors():
-    """MACE over a non-B200 model pushes model.predict through the CUDA epilogue (acq.py:151-171 arithmetic), drawing the
+    """MACE over a model of another library pushes model.predict through the CUDA epilogue (acq.py:151-171 arithmetic), drawing the
     two N(0,1) tensors from torch's CPU generator in the reference's order."""
     g = load_golden("ref_mace.npz")
 
@@ -179,8 +179,8 @@ SPEC = [{"name": "lr", "type": "pow", "lb": 1e-4, "ub": 1e-1}, {"name": "n", "ty
 
 def test_design_space_types_round_trip_like_the_reference():
     """hebo_b200.space against the semantics of HEBO/hebo/design_space/*.py (transform / inverse_transform / bounds / the
-    pymoo variable kind of evolution_optimizer.py:26-41), incl. a cross-check with the reference's own classes when
-    /root/reference is present."""
+    pymoo variable kind of evolution_optimizer.py:26-41), incl. a cross-check with the reference's own classes (their
+    outputs are stored in ref_live.npz)."""
     import pandas as pd
     from hebo_b200.space import DesignSpace
     sp = DesignSpace().parse(SPEC)
@@ -202,22 +202,13 @@ def test_design_space_types_round_trip_like_the_reference():
     xs, es = sp.transform(smp)
     lo, hi = sp.opt_lb.float(), sp.opt_ub.float()
     assert bool(((torch.cat([xs, es.float()], 1) >= lo - 1e-5) & (torch.cat([xs, es.float()], 1) <= hi + 1e-5)).all())
-    ref_dir = "/root/reference/HEBO/hebo/design_space"
-    import os
-    if os.path.isdir(ref_dir):                       # the reference's own DesignSpace, loaded by path (build container only)
-        import importlib.util, sys, types
-        pkg = types.ModuleType("_ref_ds"); pkg.__path__ = [ref_dir]; sys.modules["_ref_ds"] = pkg
-        for mod in ("param", "numeric_param", "integer_param", "pow_param", "categorical_param", "bool_param", "pow_integer_param",
-                    "int_exponent_param", "step_int", "design_space"):
-            spec = importlib.util.spec_from_file_location(f"_ref_ds.{mod}", os.path.join(ref_dir, mod + ".py"))
-            m = importlib.util.module_from_spec(spec); sys.modules[f"_ref_ds.{mod}"] = m; spec.loader.exec_module(m)
-        ref = sys.modules["_ref_ds.design_space"].DesignSpace().parse(SPEC)
-        rc, re_ = ref.transform(df)
-        assert torch.allclose(rc, xc) and torch.equal(re_, xe) and ref.para_names == sp.para_names
-        assert torch.allclose(ref.opt_lb.double(), sp.opt_lb) and torch.allclose(ref.opt_ub.double(), sp.opt_ub)
-        rb = ref.inverse_transform(xc, xe)
-        for col in sp.para_names:
-            assert [str(v) for v in rb[col].tolist()] == [str(v) for v in back[col].tolist()] or np.allclose(rb[col].values.astype(float), back[col].values.astype(float))
+    ref = load_golden("ref_live.npz")                # the reference's own DesignSpace on the same space and frame
+    assert torch.allclose(torch.from_numpy(ref["ds_xc"]), xc) and torch.equal(torch.from_numpy(ref["ds_xe"]), xe)
+    assert ref["ds_names"].tolist() == sp.para_names
+    assert torch.allclose(torch.from_numpy(ref["ds_lb"]), sp.opt_lb) and torch.allclose(torch.from_numpy(ref["ds_ub"]), sp.opt_ub)
+    for col in sp.para_names:
+        rb = ref[f"ds_back_{col}"].tolist()
+        assert rb == [str(v) for v in back[col].tolist()] or np.allclose(np.array(rb, dtype=float), back[col].values.astype(float))
 
 
 def test_standalone_hebo_host_logic_typed_space():
