@@ -1,7 +1,6 @@
 // extern "C" entry points of libhebo_b200.so (declared in include/hebo_b200.h) and the native fit-loop
 // runtime (the 100-epoch pSGLD loop of HEBO/hebo/models/gp/gp.py:96-135 without Python in the loop).
 #include <stdio.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include <atomic>
@@ -239,20 +238,10 @@ __global__ void __launch_bounds__(256) psgld_guarded_kernel(float *__restrict__ 
   }
 }
 
-// gram -> cholesky at (hyp, jitter); info left on the device
-// FP32 SIMT fallback for the fit's GEMM stages: HEBO_B200_FIT_SIMT=1 (A/B timing, debugging)
-static bool fit_use_tc() {
-  static int v = -1;
-  if (v < 0) {
-    const char *e = getenv("HEBO_B200_FIT_SIMT");
-    v = (e && e[0] == '1') ? 0 : 1;
-  }
-  return v == 1;
-}
-
-// (mixed model: gathers the embedding features at the current tables / lengthscale first)
+// gram -> cholesky at (hyp, jitter); info left on the device.  tc: the Cholesky's outer update on the tensor cores
+// (nullptr: FP32 SIMT).  (mixed model: gathers the embedding features at the current tables / lengthscale first)
 static int factor_once(const float *Xt, int64_t n, int64_t np, const ModelSpec &sp, const float *raw, int kern,
-                       const float *noise_diag, float jitter, FitWs &w, cudaStream_t st, bool allow_tc = true) {
+                       const float *noise_diag, float jitter, FitWs &w, cudaStream_t st, const TcBuffers *tc) {
   HB_CUDA(cudaMemsetAsync(w.info, 0, sizeof(int32_t), st));
   int s = launch_emb_gather(raw + sp.i_tab(), sp, n, np, w.hyp, w.Ets, w.tab_s, st);
   if (s != HB_OK) return s;
@@ -262,7 +251,7 @@ static int factor_once(const float *Xt, int64_t n, int64_t np, const ModelSpec &
   }
   s = launch_gram(sp.warp ? w.Zt : Xt, w.Ets, n, np, sp, w.hyp, kern, noise_diag, jitter, w.L, st);
   if (s != HB_OK) return s;
-  return launch_cholesky(w.L, np, w.cholws, w.info, st, (allow_tc && fit_use_tc()) ? &w.tc : nullptr);
+  return launch_cholesky(w.L, np, w.cholws, w.info, st, tc);
 }
 
 static float next_jitter(float j) { return j == 0.0f ? 1e-6f : j * 10.0f; }   // fp32 ladder of gp.py:104-110
@@ -445,7 +434,7 @@ int32_t hb_factorize_ex(const float *Xt, const int32_t *Xe, const float *y, int6
   for (;;) {   // gp.py:140-157 jitter escalation of predict()
     // the prediction state is built ONCE per fit: keep it on the FP32 SIMT pipe (round-to-nearest accumulation);
     // the 3xTF32 tensor path (the tensor cores' fp32 accumulation is not RN) is used for the 100 gradient epochs only
-    s = factor_once(Xt, n, np, sp, raw, kern, noise_diag, jitter, w, st, /*allow_tc=*/false);
+    s = factor_once(Xt, n, np, sp, raw, kern, noise_diag, jitter, w, st, nullptr);
     if (s != HB_OK) return s;
     HB_CUDA(cudaMemcpyAsync(&hs->info, w.info, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     HB_CUDA(cudaStreamSynchronize(st));
@@ -494,7 +483,7 @@ int32_t hb_mll_fwd_bwd(const float *Xt, const int32_t *Xe, const float *y, int64
   if (s != HB_OK) return s;
   s = launch_transform_hypers(raw, sp, noise_lb, w.hyp, st);
   if (s != HB_OK) return s;
-  s = factor_once(Xt, n, np, sp, raw, kern, noise_diag, jitter, w, st, /*allow_tc=*/false);
+  s = factor_once(Xt, n, np, sp, raw, kern, noise_diag, jitter, w, st, nullptr);
   if (s != HB_OK) return s;
   s = launch_tri_inverse(w.L, np, w.Linv, w.tmp, st);
   if (s != HB_OK) return s;
@@ -538,18 +527,14 @@ int32_t hb_fit_ex(const float *Xt, const int32_t *Xe, const float *y, int64_t n,
   auto enqueue_epoch = [&](float jitter, cudaStream_t s_) -> int {
     int s = launch_transform_hypers(raw, sp, noise_lb, w.hyp, s_);
     if (s != HB_OK) return s;
-    s = factor_once(Xt, n, np, sp, raw, kern, noise_diag, jitter, w, s_);
+    s = factor_once(Xt, n, np, sp, raw, kern, noise_diag, jitter, w, s_, &w.tc);
     if (s != HB_OK) return s;
-    if (fit_use_tc()) {
-      s = launch_tri_inverse_tc(w.L, np, w.Linv, w.tc, !zeroed, s_);
-      zeroed = true;
-    } else {
-      s = launch_tri_inverse(w.L, np, w.Linv, w.tmp, s_);
-    }
+    s = launch_tri_inverse_tc(w.L, np, w.Linv, w.tc, !zeroed, s_);
+    zeroed = true;
     if (s != HB_OK) return s;
     s = launch_solve_logdet(w.L, w.Linv, y, n, np, w.hyp, w.alpha, w.scal, w.solvews, s_);
     if (s != HB_OK) return s;
-    s = fit_use_tc() ? launch_kinv_tc(np, w.tmp, w.tc, s_) : launch_kinv(w.Linv, np, w.tmp, s_);
+    s = launch_kinv_tc(np, w.tmp, w.tc, s_);
     if (s != HB_OK) return s;
     s = launch_mll_grad(sp.warp ? w.Zt : Xt, w.Ets, n, np, sp, raw, w.hyp, kern, w.tmp, w.alpha, w.scal, noise_guess, w.grad, w.loss,
                         w.gradws, s_, w.dZa, w.dZb);
@@ -603,14 +588,10 @@ int32_t hb_fit_ex(const float *Xt, const int32_t *Xe, const float *y, int64_t n,
   // Remaining epochs: capture ONE epoch (jitter 0) into a CUDA graph and replay it FIT_BATCH times per host
   // synchronisation.  A failed factorisation leaves the hypers, the RMS state and the device epoch counter untouched
   // (the pSGLD kernel is guarded), so every later replay of the batch fails the same way; the host then runs that epoch
-  // through the jitter ladder on the plain path and resumes.  HEBO_B200_FIT_GRAPH=0 disables the graph path.
-  static const bool graph_on = [] {
-    const char *e = getenv("HEBO_B200_FIT_GRAPH"), *t = getenv("HEBO_B200_CHOL_TIMING");
-    return !(e && e[0] == '0') && !(t && t[0] == '1');
-  }();
+  // through the jitter ladder on the plain path and resumes.
   cudaGraphExec_t exec = nullptr;
   long long launches_per_epoch = 0;
-  if (graph_on && num_epochs - ep >= 4) {
+  if (num_epochs - ep >= 4) {
     static cudaStream_t gs_dev[MAX_DEVICES] = {};   // one capture stream per device
     int cur_dev = 0;
     cudaGetDevice(&cur_dev);

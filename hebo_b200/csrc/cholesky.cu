@@ -18,10 +18,6 @@
 // This is what gpytorch's psd_safe_cholesky does through LAPACK potrf for HEBO/hebo/models/gp/gp.py:112-113,148.
 // `info` follows LAPACK: j > 0 = leading minor j not positive definite (first failing pivot wins).
 #include <limits.h>
-#include <stdio.h>
-#include <stdlib.h>
-
-#include <vector>
 
 #include "gemm_core.cuh"
 #include "kernels.h"
@@ -32,13 +28,6 @@ constexpr int OUTER = 512;             // outer block width
 constexpr int TS = 64;                 // tile size of the block-column DAG
 constexpr int MAXBC64 = OUTER / TS;    // tile columns per outer block
 constexpr int SP64 = TS + 4;           // shared-tile pitch (16-byte aligned, staggers banks)
-
-// phase clock stamps of the second diagonal task of a block column (debug: HEBO_B200_CHOL_TIMING=1 prints them)
-__device__ long long g_chol_clk[8];
-#define CHOL_STAMP(k)                        \
-  do {                                       \
-    if (stamp_on) g_chol_clk[k] = clock64(); \
-  } while (0)
 
 __device__ __forceinline__ int ld_acquire(const int *p) {
   int v;
@@ -310,8 +299,6 @@ __global__ void __launch_bounds__(GTHREADS, 1) chol_block64_kernel(float *__rest
     const int j = jb0 + jl;
     const int64_t col = (int64_t)j * TS;
     if (t == 0) sm.fail = INT_MAX;
-    const bool stamp_on = (tt == 0 && jl == 1 && t == 0);
-    CHOL_STAMP(0);
     if (tt == 0) {
       // ------------------------------------------------------------------ D(j)
       float S[4][4], S2[4][4];
@@ -330,21 +317,16 @@ __global__ void __launch_bounds__(GTHREADS, 1) chol_block64_kernel(float *__rest
         }
         tile4x4_to_smem(S2, sm.T, ti, tc);
         stage_factor(sm, A, np, j - 1, flags + (j - 1) * MAXBC64 + (jl - 1), token);
-        CHOL_STAMP(1);
         trsm64<true>(sm);
         __syncthreads();
-        CHOL_STAMP(2);
         store_tile(sm, Cs, np);                       // L(j, j-1): its flag is released inside the sweep
         update64(S, sm.At, sm.At, ti, tc);            // the one update on the critical path, straight from smem
       }
-      CHOL_STAMP(3);
       sweep64(S, &sm.Lt[0][0], &sm.fail, j * TS, warp, lane, ti, tc, jl >= 1 ? flags + j * MAXBC64 + (jl - 1) : nullptr, token);
       tile4x4_to_smem(S, sm.T, ti, tc);
       __syncthreads();
       if (t == 0 && sm.fail != INT_MAX) atomicCAS(info, 0, sm.fail + 1);
-      CHOL_STAMP(4);
       publish_tile(sm, Cd, np, flags + j * MAXBC64 + jl, token);
-      CHOL_STAMP(5);
     } else {
       // ------------------------------------------------------------------ R(i, j)
       const int i = j + (jl == nbc - 1 ? 1 : 2) + (tt - 1);
@@ -532,51 +514,6 @@ __global__ void __launch_bounds__(GTHREADS, 2) chol_update_kernel(float *__restr
   }
 }
 
-// HEBO_B200_CHOL_TIMING=1: warm, in-stream CUDA-event timing of every launch class (printed per call)
-struct ChTimer {
-  bool on;
-  std::vector<cudaEvent_t> ev;
-  std::vector<int> cls;
-  ChTimer() {
-    const char *e = getenv("HEBO_B200_CHOL_TIMING");
-    on = e && e[0] == '1';
-  }
-  void mark(int c, cudaStream_t st) {
-    if (!on) return;
-    cudaEvent_t e;
-    cudaEventCreate(&e);
-    cudaEventRecord(e, st);
-    ev.push_back(e);
-    cls.push_back(c);
-  }
-  void report(cudaStream_t st) {
-    if (!on || ev.empty()) return;
-    cudaStreamSynchronize(st);
-    double tot[4] = {0, 0, 0, 0};
-    int cnt[4] = {0, 0, 0, 0};
-    for (size_t i = 0; i + 1 < ev.size(); ++i) {
-      float ms = 0;
-      cudaEventElapsedTime(&ms, ev[i], ev[i + 1]);
-      tot[cls[i]] += ms;
-      cnt[cls[i]]++;
-    }
-    fprintf(stderr, "[chol timing] block column %d x %.1f us = %.3f ms | outer update: split %d x %.1f us = %.3f ms, gemm %d x %.1f us = %.3f ms\n",
-            cnt[0], cnt[0] ? 1e3 * tot[0] / cnt[0] : 0.0, tot[0], cnt[1], cnt[1] ? 1e3 * tot[1] / cnt[1] : 0.0, tot[1], cnt[2],
-            cnt[2] ? 1e3 * tot[2] / cnt[2] : 0.0, tot[2]);
-    long long c[8];
-    if (cudaMemcpyFromSymbol(c, g_chol_clk, sizeof(c)) == cudaSuccess)
-      fprintf(stderr, "[chol phases, cycles, 2nd diagonal task of the last block column] wait+stage factor %lld | trsm %lld | update+publish "
-                      "%lld | potrf %lld | publish %lld\n",
-              c[1] - c[0], c[2] - c[1], c[3] - c[2], c[4] - c[3], c[5] - c[4]);
-    for (auto e : ev) cudaEventDestroy(e);
-    ev.clear();
-    cls.clear();
-  }
-};
-
-static ChTimer timer;
-void chol_timer_mark(int cls, cudaStream_t st) { timer.mark(cls, st); }
-
 int launch_cholesky(float *A, int64_t np, float *ws, int32_t *info, cudaStream_t st, const TcBuffers *tc) {
   if (np <= 0 || np % GT != 0) return HB_ERR_INVALID;
   static PerDevice once;   // aux[dev] = co-resident CTAs of the cooperative block kernel on that device
@@ -612,7 +549,6 @@ int launch_cholesky(float *A, int64_t np, float *ws, int32_t *info, cudaStream_t
       ntasks += 1 + (rest > 0 ? rest : 0);
     }
     ++token;
-    timer.mark(0, st);
     {
       const int grid = ntasks < max_ctas ? ntasks : max_ctas;
       void *args[] = {&A, &np, &jb0, &nbc, &ntasks, &flags, &token, &info};
@@ -620,12 +556,10 @@ int launch_cholesky(float *A, int64_t np, float *ws, int32_t *info, cudaStream_t
       count_launches(1);
     }
     if (ce == np) break;
-    timer.mark(1, st);
     if (tc) {   // outer update on the tensor cores (wgmma 3xTF32, fit_tc.cu)
       const int s = launch_chol_outer_update_tc(A, np, cb, ce, *tc, st);
       if (s != HB_OK) return s;
     } else {    // everything right of the block, K = block width
-      timer.mark(2, st);
       const int J0 = (int)(ce / GT);
       int ntiles = 0;
       for (int J = J0; J < nt; ++J) ntiles += nt - J;
@@ -633,8 +567,6 @@ int launch_cholesky(float *A, int64_t np, float *ws, int32_t *info, cudaStream_t
       count_launches(1);
     }
   }
-  timer.mark(3, st);
-  timer.report(st);
   HB_LAUNCH_CHECK("cholesky");
   return HB_OK;
 }

@@ -9,9 +9,6 @@
 //                                 -> Linv (fp32 + hi/lo) and U = X21^T (hi/lo)
 //   K^-1 = U U^T            lower tiles, k >= row tile        -> Kinv fp32
 // (gpytorch's backward through the Cholesky MLL, HEBO/hebo/models/gp/gp.py:115, as explicit dense algebra.)
-#include <stdio.h>
-#include <stdlib.h>
-
 #include <vector>
 
 #include "gemm_core.cuh"
@@ -33,7 +30,6 @@ int launch_chol_outer_update_tc(float *A, int64_t np, int64_t cb, int64_t ce, co
   // hi/lo copy of the finished panel rows [ce, np) x [cb, ce) -> P[r][c - cb], leading dimension K
   int s = launch_split_region(A + ce * np + cb, np, tc.P_hi + ce * K, tc.P_lo + ce * K, K, np - ce, K, st);
   if (s != HB_OK) return s;
-  chol_timer_mark(2, st);
   int ntiles = 0;
   const uint64_t key = table_key(1, np, cb, ce);
   const TcTile *tiles = tc_table_lookup(key, &ntiles);
@@ -58,72 +54,9 @@ int launch_chol_outer_update_tc(float *A, int64_t np, int64_t cb, int64_t ce, co
 }
 
 // ------------------------------------------------------------------------------------------ triangular inverse
-// base case: one CTA inverts one 128x128 diagonal block (thread i -> row i of the inverse) and writes it as
-// Linv (fp32 + hi/lo) and transposed as U (hi/lo)
-struct TriBaseSmemTc {
-  float Ls[GT][GT + 1];
-  float Xs[GT][GT + 1];
-};
-
-__global__ void __launch_bounds__(GT) triinv_base_tc_kernel(const float *__restrict__ L, int64_t np, float *__restrict__ Linv,
-                                                            float *__restrict__ Linv_hi, float *__restrict__ Linv_lo,
-                                                            float *__restrict__ U_hi, float *__restrict__ U_lo) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  TriBaseSmemTc &sm = *reinterpret_cast<TriBaseSmemTc *>(smem_raw);
-  const int t = threadIdx.x;
-  const int64_t o = (int64_t)blockIdx.x * GT;
-  for (int f = t; f < GT * GT / 4; f += GT) {
-    const int row = f >> 5, c4 = f & 31;
-    const float4 v = *reinterpret_cast<const float4 *>(L + (o + row) * np + o + c4 * 4);
-    sm.Ls[row][c4 * 4 + 0] = v.x;
-    sm.Ls[row][c4 * 4 + 1] = v.y;
-    sm.Ls[row][c4 * 4 + 2] = v.z;
-    sm.Ls[row][c4 * 4 + 3] = v.w;
-  }
-  __syncthreads();
-  const int i = t;
-  for (int j = GT - 1; j > i; --j) sm.Xs[i][j] = 0.0f;
-  for (int j = i; j >= 0; --j) {
-    float s0 = (j == i) ? 1.0f : 0.0f, s1 = 0.0f, s2 = 0.0f, s3 = 0.0f;
-    int kk = j + 1;
-    for (; kk + 3 <= i; kk += 4) {
-      s0 = fmaf(-sm.Xs[i][kk + 0], sm.Ls[kk + 0][j], s0);
-      s1 = fmaf(-sm.Xs[i][kk + 1], sm.Ls[kk + 1][j], s1);
-      s2 = fmaf(-sm.Xs[i][kk + 2], sm.Ls[kk + 2][j], s2);
-      s3 = fmaf(-sm.Xs[i][kk + 3], sm.Ls[kk + 3][j], s3);
-    }
-    for (; kk <= i; ++kk) s0 = fmaf(-sm.Xs[i][kk], sm.Ls[kk][j], s0);
-    sm.Xs[i][j] = ((s0 + s1) + (s2 + s3)) / sm.Ls[j][j];
-  }
-  __syncthreads();
-  for (int f = t; f < GT * GT; f += GT) {
-    const int row = f >> 7, col = f & 127;          // coalesced along col
-    const float x = sm.Xs[row][col];
-    uint32_t hb;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hb) : "f"(x));
-    const float h = __uint_as_float(hb), l = x - h;
-    const int64_t a = (o + row) * np + o + col;
-    Linv[a] = x;
-    Linv_hi[a] = h;
-    Linv_lo[a] = l;
-    const float xt = sm.Xs[col][row];               // U[row][col] = Linv[col][row]
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hb) : "f"(xt));
-    const float ht = __uint_as_float(hb);
-    U_hi[a] = ht;
-    U_lo[a] = xt - ht;
-  }
-}
-
+// base case: triinv_base2_kernel (cholesky.cu) inverts the 128x128 diagonal blocks into Linv (fp32 + hi/lo) and U (hi/lo)
 int launch_tri_inverse_tc(const float *L, int64_t np, float *Linv, const TcBuffers &tc, bool zero_fill, cudaStream_t st) {
   if (np <= 0 || np % GT != 0) return HB_ERR_INVALID;
-  static PerDevice once;
-  bool fresh = false;
-  const int dev = once.slot(&fresh);
-  if (dev < 0) return HB_ERR_CUDA;
-  if (fresh) {
-    HB_CUDA(cudaFuncSetAttribute(triinv_base_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TriBaseSmemTc)));
-    once.done[dev] = true;
-  }
   const size_t bytes = (size_t)np * np * sizeof(float);
   if (zero_fill) {   // the triangular complements are never written afterwards: once per workspace is enough
     HB_CUDA(cudaMemsetAsync(Linv, 0, bytes, st));
@@ -134,17 +67,8 @@ int launch_tri_inverse_tc(const float *L, int64_t np, float *Linv, const TcBuffe
   }
   int s = launch_split_region(L, np, tc.L_hi, tc.L_lo, np, np, np, st);
   if (s != HB_OK) return s;
-  static const bool old_base = [] {
-    const char *e = getenv("HEBO_B200_TRIINV_BASE1");
-    return e && e[0] == '1';
-  }();
-  if (old_base) {
-    triinv_base_tc_kernel<<<(int)(np / GT), GT, sizeof(TriBaseSmemTc), st>>>(L, np, Linv, tc.Linv_hi, tc.Linv_lo, tc.U_hi, tc.U_lo);
-    count_launches(1);
-  } else {
-    s = launch_triinv_base2(L, np, Linv, tc.Linv_hi, tc.Linv_lo, tc.U_hi, tc.U_lo, st);
-    if (s != HB_OK) return s;
-  }
+  s = launch_triinv_base2(L, np, Linv, tc.Linv_hi, tc.Linv_lo, tc.U_hi, tc.U_lo, st);
+  if (s != HB_OK) return s;
   TcOperand opL{tc.L_hi, tc.L_lo, (uint64_t)np, (uint64_t)np, (uint64_t)np};
   TcOperand opU{tc.U_hi, tc.U_lo, (uint64_t)np, (uint64_t)np, (uint64_t)np};
   TcOperand opLinv{tc.Linv_hi, tc.Linv_lo, (uint64_t)np, (uint64_t)np, (uint64_t)np};

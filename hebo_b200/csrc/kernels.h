@@ -46,12 +46,11 @@ struct ModelSpec {
   __host__ __device__ int dtot() const { return d + De; }
 };
 
-// cholesky.cu / linalg.cu   (tc == nullptr -> FP32 SIMT everywhere)
+// cholesky.cu / linalg.cu   (tc: outer update on the tensor cores, the gradient epochs; nullptr -> FP32 SIMT)
 int launch_cholesky(float *A, int64_t np, float *ws, int32_t *info, cudaStream_t st, const TcBuffers *tc = nullptr);
-// fit_tc.cu
 int launch_triinv_base2(const float *L, int64_t np, float *Linv, float *Linv_hi, float *Linv_lo, float *U_hi, float *U_lo,
                         cudaStream_t st);
-void chol_timer_mark(int cls, cudaStream_t st);   // debug timing (HEBO_B200_CHOL_TIMING=1)
+// fit_tc.cu
 int launch_chol_outer_update_tc(float *A, int64_t np, int64_t cb, int64_t ce, const TcBuffers &tc, cudaStream_t st);
 int launch_tri_inverse_tc(const float *L, int64_t np, float *Linv, const TcBuffers &tc, bool zero_fill, cudaStream_t st);
 int launch_kinv_tc(int64_t np, float *Kinv, const TcBuffers &tc, cudaStream_t st);

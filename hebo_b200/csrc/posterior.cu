@@ -8,8 +8,6 @@
 //                  ||v||^2 per row (V itself is never stored)
 //   mace_kernel  : variance floors, un-scaling, MACE arithmetic (fp32, same operation order as the reference)
 // All partial sums go to workspace slots and are combined in a fixed order: results are deterministic.
-#include <stdlib.h>
-
 #include "gemm_core.cuh"
 #include "h16.cuh"
 #include "kernels.h"
@@ -177,17 +175,10 @@ __global__ void __launch_bounds__(GTHREADS, 2) vnorm_kernel(const float *__restr
 // ---- precision guard of the tensor path ------------------------------------------------------------------
 // sigma^2 = s - ||v||^2 cancels when a candidate sits on the data; the tensor cores' fp32 accumulation is
 // not round-to-nearest, which would exceed the 1e-4 sigma criterion once
-// sigma^2 < ~s/40.  Rows whose variance falls below theta * s (default 0.12) are therefore flagged and their ||v||^2 is
+// sigma^2 < ~s/40.  Rows whose variance falls below GUARD_THETA * s are therefore flagged and their ||v||^2 is
 // recomputed on the FP32 SIMT pipe from the same operands (K* = hi + lo); typical BO batches flag few rows, a
 // batch that sits entirely on the data degrades gracefully to the SIMT contraction.
-static float guard_theta() {   // HEBO_B200_GUARD_THETA overrides (0 disables the guard: measurement only)
-  static float v = -1.0f;
-  if (v < 0.0f) {
-    const char *e = getenv("HEBO_B200_GUARD_THETA");
-    v = e ? (float)atof(e) : 0.12f;
-  }
-  return v;
-}
+constexpr float GUARD_THETA = 0.12f;
 
 // measurement hook (bench.py "guard_flagged_frac"): rows seen / rows flagged by the guard since the last reset
 __device__ unsigned long long g_guard_stats[2];
@@ -436,7 +427,6 @@ int launch_posterior_mace(const float *Xs, const int32_t *Xe_s, int64_t m, int64
   const int ncg = (int)ceil_div(np, KS_GROUP);
   const int nt = (int)(np / GT);
   const bool tensor = Linv_hi != nullptr && Linv_lo != nullptr;   // wgmma path (two-level fp16 split), else FP32 SIMT
-  const bool h16 = tensor;
   // workspace: the K* chunk (KS: fp32 rows of the SIMT / guard passes; KS2: the fp16 two-level split h0 | h1 of the
   // tensor path), the mean partials and the per-chunk partial-sum buffers.  (Building chunk i+1 on a side stream under
   // the tensor-core contraction of chunk i was measured and dropped: the contraction draws ~all of the L2 -> SM
@@ -452,20 +442,19 @@ int launch_posterior_mace(const float *Xs, const int32_t *Xe_s, int64_t m, int64
   for (int64_t c0 = 0; c0 < m; c0 += m_chunk) {
     const int64_t mc = min(m_chunk, m - c0);
     const int64_t mc_pad = round_up(mc, GT);
-    const cudaStream_t ks_st = st;
     const dim3 g1((unsigned)ceil_div(mc, KS_ROWS), (unsigned)ncg);
     const float *xs = Xs + c0 * d;
     const int32_t *xe = sp.e > 0 ? Xe_s + c0 * sp.e : nullptr;
 #define HB_KSTAR(K, S)                                                                                                          \
   do {                                                                                                                          \
     if (sp.e > 0)                                                                                                               \
-      kstar_kernel<K, S, true><<<g1, 256, dyn, ks_st>>>(xs, mc, (int)d, x_mul, x_add, Zt, alpha, hyp, n, np, KS, KS2, mupart,   \
-                                                        mc_pad_max, nullptr, nullptr, xe, tab_s, sp);                          \
+      kstar_kernel<K, S, true><<<g1, 256, dyn, st>>>(xs, mc, (int)d, x_mul, x_add, Zt, alpha, hyp, n, np, KS, KS2, mupart,      \
+                                                     mc_pad_max, nullptr, nullptr, xe, tab_s, sp);                             \
     else                                                                                                                        \
-      kstar_kernel<K, S, false><<<g1, 256, dyn, ks_st>>>(xs, mc, (int)d, x_mul, x_add, Zt, alpha, hyp, n, np, KS, KS2, mupart,  \
-                                                         mc_pad_max, nullptr, nullptr, nullptr, nullptr, sp);                  \
+      kstar_kernel<K, S, false><<<g1, 256, dyn, st>>>(xs, mc, (int)d, x_mul, x_add, Zt, alpha, hyp, n, np, KS, KS2, mupart,     \
+                                                      mc_pad_max, nullptr, nullptr, nullptr, nullptr, sp);                     \
   } while (0)
-    if (h16) {
+    if (tensor) {
       if (kern == HB_KERN_MATERN32) HB_KSTAR(0, 2); else if (kern == HB_KERN_MATERN52) HB_KSTAR(1, 2); else HB_KSTAR(2, 2);
     } else {
       if (kern == HB_KERN_MATERN32) HB_KSTAR(0, 0); else if (kern == HB_KERN_MATERN52) HB_KSTAR(1, 0); else HB_KSTAR(2, 0);
@@ -480,7 +469,7 @@ int launch_posterior_mace(const float *Xs, const int32_t *Xe_s, int64_t m, int64
       if (s != HB_OK) return s;
       nslots = (int)ceil_div(np, 128);
       HB_CUDA(cudaMemsetAsync(fixcount, 0, sizeof(int32_t), st));
-      guard_kernel<<<(int)ceil_div(mc, 256), 256, 0, st>>>(vpart, nslots, mc, mc_pad_max, hyp, guard_theta(), fixmap, fixlist, fixcount);
+      guard_kernel<<<(int)ceil_div(mc, 256), 256, 0, st>>>(vpart, nslots, mc, mc_pad_max, hyp, GUARD_THETA, fixmap, fixlist, fixcount);
       const dim3 gf((unsigned)nt, (unsigned)(mc_pad / GT));
       {   // exact fp32 K* rows of the flagged candidates only (compact, row = slot), then their FP32 contraction
 #define HB_KFIX(K)                                                                                                              \

@@ -101,7 +101,6 @@ class GP(BaseModel):
             wa, wb = torch.as_tensor(self.warp_a, dtype=torch.float32), torch.as_tensor(self.warp_b, dtype=torch.float32)
             assert wa.numel() == self.num_cont == wb.numel() and bool(((wa > 0.01) & (wa < 10) & (wb > 0.01) & (wb < 10)).all()), \
                 "fixed warp exponents must lie inside (0.01, 10)"
-        self._general = self.num_enum > 0 or not self.ard_kernel or self.warp_mode > 0     # needs the `_ex` entry points
         self._c_uniqs = (C.c_int32 * max(1, self.num_enum))(*self.num_uniqs)
         self._c_embs = (C.c_int32 * max(1, self.num_enum))(*self.emb_sizes)
         self._spec = _lib.ModelSpec(int(bool(self.ard_kernel)), self.num_enum, self._c_uniqs, self._c_embs, self.warp_mode)
@@ -145,7 +144,7 @@ class GP(BaseModel):
         return Xc_t, Xe_t
 
     def _spec_ptr(self):
-        return C.byref(self._spec) if self._general else None
+        return C.byref(self._spec)
 
     # FIXED warp exponents (warp_a / warp_b) are not hyper-parameters: `raw`, `raw_init`, `init_raw`, `set_hypers` and the
     # Langevin draws use the vector WITHOUT them; the device vector carries them (frozen) between the tables and the mean.
@@ -435,51 +434,22 @@ class GP(BaseModel):
     # ------------------------------------------------------------------ loss / gradient at the current hypers
     def evaluate_loss(self, return_grad: bool = False):
         """-mll/n (and its gradient w.r.t. the raw parameters) at the current hypers; used for verbose printing and the
-        parity tests.  Numeric ARD models go through the individual C-ABI calls (gram, cholesky, ...), mixed / non-ARD
-        models through the fused hb_mll_fwd_bwd on a scratch workspace (the prediction state is left untouched)."""
+        parity tests.  One hb_mll_fwd_bwd on a scratch workspace (the prediction state is left untouched)."""
         lib = _lib.lib()
-        n, d, NP, dev = self.n, self.d, self.NP, self.device
-        st = _lib.stream_ptr()
+        n, d, dev = self.n, self.d, self.device
         P = self._param_layout()["P"]
         info = torch.zeros(1, dtype=torch.int32, device=dev)
         grad = torch.empty(P, dtype=torch.float32, device=dev)
         loss = torch.empty(1, dtype=torch.float32, device=dev)
-        if self._general:
-            scratch = torch.empty(self._ws.numel(), dtype=torch.uint8, device=dev)
-            with torch.cuda.device(dev):
-                _lib.check(lib.hb_mll_fwd_bwd(_lib.ptr(self._XtT) if d > 0 else None, _lib.ptr(self._Xe_dev), _lib.ptr(self._y_dev),
-                                              n, d, self._spec_ptr(), _lib.ptr(self._raw_dev), self.kern_id, _lib.ptr(self._nd_dev),
-                                              float(self.noise_lb), float(self.noise_guess), 0.0, _lib.ptr(grad), _lib.ptr(loss),
-                                              _lib.ptr(info), _lib.ptr(scratch), scratch.numel(), st), "hb_mll_fwd_bwd")
-            if int(info.item()) != 0:
-                raise _lib.NotPositiveDefinite(f"leading minor {int(info.item())} not positive definite")
-            return (float(loss.item()), self._strip_raw(grad.cpu())) if return_grad else float(loss.item())
-        hyp = torch.empty(d + 3, dtype=torch.float32, device=dev)
-        K = torch.empty(NP, NP, dtype=torch.float32, device=dev)
-        Linv = torch.empty_like(K)
-        tmp = torch.empty_like(K)
-        cholws = torch.empty(128 * 128, dtype=torch.float32, device=dev)
-        alpha = torch.empty(NP, dtype=torch.float32, device=dev)
-        scal = torch.empty(2, dtype=torch.float64, device=dev)
-        sws = torch.empty(NP * 8 * (1 + NP // 64) + 256, dtype=torch.uint8, device=dev)
-        gws = torch.empty((NP // 128) * (NP // 128 + 1) // 2 * (d + 3) * 4 + 512, dtype=torch.uint8, device=dev)
+        scratch = torch.empty(self._ws.numel(), dtype=torch.uint8, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(lib.hb_transform_hypers(_lib.ptr(self._raw_dev), d, float(self.noise_lb), _lib.ptr(hyp), st), "transform")
-            _lib.check(lib.hb_gram(_lib.ptr(self._XtT), n, d, _lib.ptr(hyp), self.kern_id, _lib.ptr(self._nd_dev), 0.0,
-                                   _lib.ptr(K), st), "gram")
-            _lib.check(lib.hb_cholesky(_lib.ptr(K), NP, _lib.ptr(cholws), _lib.ptr(info), st), "cholesky")
-            _lib.check(lib.hb_tri_inverse(_lib.ptr(K), NP, _lib.ptr(Linv), _lib.ptr(tmp), st), "tri_inverse")
-            _lib.check(lib.hb_solve_logdet(_lib.ptr(K), _lib.ptr(Linv), _lib.ptr(self._y_dev), n, NP, _lib.ptr(hyp),
-                                           _lib.ptr(alpha), _lib.ptr(scal), _lib.ptr(sws), st), "solve_logdet")
-            _lib.check(lib.hb_kinv(_lib.ptr(Linv), NP, _lib.ptr(tmp), st), "kinv")
-            _lib.check(lib.hb_mll_grad(_lib.ptr(self._XtT), n, d, _lib.ptr(self._raw_dev), _lib.ptr(hyp), self.kern_id,
-                                       _lib.ptr(tmp), _lib.ptr(alpha), _lib.ptr(scal), float(self.noise_guess),
-                                       _lib.ptr(grad), _lib.ptr(loss), _lib.ptr(gws), st), "mll_grad")
+            _lib.check(lib.hb_mll_fwd_bwd(_lib.ptr(self._XtT) if d > 0 else None, _lib.ptr(self._Xe_dev), _lib.ptr(self._y_dev),
+                                          n, d, self._spec_ptr(), _lib.ptr(self._raw_dev), self.kern_id, _lib.ptr(self._nd_dev),
+                                          float(self.noise_lb), float(self.noise_guess), 0.0, _lib.ptr(grad), _lib.ptr(loss),
+                                          _lib.ptr(info), _lib.ptr(scratch), scratch.numel(), _lib.stream_ptr()), "hb_mll_fwd_bwd")
         if int(info.item()) != 0:
             raise _lib.NotPositiveDefinite(f"leading minor {int(info.item())} not positive definite")
-        if return_grad:
-            return float(loss.item()), grad.cpu()
-        return float(loss.item())
+        return (float(loss.item()), self._strip_raw(grad.cpu())) if return_grad else float(loss.item())
 
     # ------------------------------------------------------------------ posterior (gp.py:137-164) + MACE (acq.py:146-171)
     def _copy_stream(self):
@@ -641,7 +611,7 @@ class GP(BaseModel):
         with torch.cuda.device(dev):
             # (a warp stays in torch in front of this call so that autograd chains through it: the kernels get warp = 0)
             st = lib.hb_posterior_grad_ex(_lib.ptr(Xin), _lib.ptr(self._grad_xe), m, self.n, self.d,
-                                          C.byref(self._spec_nowarp) if self._general else None,
+                                          C.byref(self._spec_nowarp),
                                           _lib.ptr(self._emb_meta_dev) if self.num_enum else None,
                                           _lib.ptr(self.tab_s_dev) if self.num_enum else None, _lib.ptr(x_mul), _lib.ptr(x_add),
                                           _lib.ptr(self.Zt_dev), _lib.ptr(self.alpha_dev), _lib.ptr(self.Linv_dev),
@@ -709,8 +679,6 @@ class GP(BaseModel):
         half = self.NP * self.NP // 2
         ts = [self.hyp_dev, self.alpha_dev, self.Zt_dev, self.Linv_dev, self.Linv_hi_dev.view(-1)[:half],
               self.Linv_lo_dev.view(-1)[:half + 2]]
-        if _lib.lib().hb_vnorm_operand_kind() != 0:       # 3xTF32 operands occupy the whole buffers
-            ts[4:] = [self.Linv_hi_dev, self.Linv_lo_dev]
         if self.num_enum > 0:
             ts += [self.tab_s_dev, self._emb_meta_dev]
         return ts

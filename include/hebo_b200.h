@@ -202,7 +202,7 @@ int32_t hb_fit_state_ex(void *ws, int64_t n, int64_t d, const hb_model_spec_t *s
  * acquisitions/acq.py:146-171; Mean/Sigma acq.py:66-82 read mu/var) ----------------------------
  * Xs        [m, d] RAW candidates; x_mul/x_add [d]: MinMax scale_/min_ (models/scalers.py:86-87)
  * Zt, alpha, Linv, hyp: from hb_fit_state.  Linv_hi/Linv_lo: from hb_fit_state -> variance contraction on the
- *           wgmma tensor cores (error-compensated fp16 two-level split, or 3xTF32); both NULL -> FP32 SIMT contraction.
+ *           wgmma tensor cores (error-compensated fp16 two-level split); both NULL -> FP32 SIMT contraction.
  * y_mean,y_std: TorchStandardScaler (models/scalers.py:56-60).  pred_likeli: gp.py:158-159.
  * tau,kappa,eps: MACE(best_y, kappa, eps).  xi1, xi2 [m]: the two torch.randn draws of acq.py:154-155
  *           (NULL -> Philox N(0,1) from `seed`, independent streams per row).

@@ -411,6 +411,52 @@ def test_cholesky_two_level_blocking_shapes(NP):
     assert err < 2e-6, err
 
 
+@pytest.mark.parametrize("hetero", [False, True])
+@pytest.mark.parametrize("kind", ["matern32", "matern52", "rbf"])
+def test_stage_chain_equals_fused_mll_fwd_bwd_bitwise(kind, hetero):
+    """The seven single-stage entry points (transform, gram, cholesky, tri_inverse, solve_logdet, kinv, mll_grad) and the
+    fused hb_mll_fwd_bwd -- with a NULL spec and with the numeric ARD spec the model passes -- run the same FP32 SIMT kernels
+    in the same order: loss and gradient are bit-identical, and GP.evaluate_loss returns exactly those values."""
+    lib = _lib.lib()
+    n, d = 700, 5
+    X, y = seeded_problem(n, d, 17)
+    nd = (1e-2 * (1 + (X.double() ** 2).sum(1) / d)).float() if hetero else None
+    np.random.seed(0)
+    gp = hebo_b200.GP(d, 0, 1, kernel=kind, lr=0.01, num_epochs=3, noise_lb=8e-4, pred_likeli=False, langevin=False,
+                      noise_diag=nd)
+    gp.fit(X, None, y)
+    NP, st, dev = gp.NP, _lib.stream_ptr(), gp.device
+    XtT, yd, raw, ndd = _lib.ptr(gp._XtT), _lib.ptr(gp._y_dev), _lib.ptr(gp._raw_dev), _lib.ptr(gp._nd_dev)
+    f32 = dict(dtype=torch.float32, device=dev)
+    ws_bytes = int(lib.hb_fit_workspace_bytes(n, d))     # holds the solve and gradient workspaces: an upper bound for each
+    hyp, alpha, grad, loss = torch.empty(d + 3, **f32), torch.empty(NP, **f32), torch.empty(d + 3, **f32), torch.empty(1, **f32)
+    K, Linv, tmp = (torch.empty(NP, NP, **f32) for _ in range(3))
+    cholws = torch.empty(128 * 128, **f32)
+    scal = torch.empty(2, dtype=torch.float64, device=dev)
+    sws, gws = (torch.empty(ws_bytes, dtype=torch.uint8, device=dev) for _ in range(2))
+    info = torch.zeros(1, dtype=torch.int32, device=dev)
+    _lib.check(lib.hb_transform_hypers(raw, d, float(gp.noise_lb), _lib.ptr(hyp), st), "transform")
+    _lib.check(lib.hb_gram(XtT, n, d, _lib.ptr(hyp), gp.kern_id, ndd, 0.0, _lib.ptr(K), st), "gram")
+    _lib.check(lib.hb_cholesky(_lib.ptr(K), NP, _lib.ptr(cholws), _lib.ptr(info), st), "cholesky")
+    _lib.check(lib.hb_tri_inverse(_lib.ptr(K), NP, _lib.ptr(Linv), _lib.ptr(tmp), st), "tri_inverse")
+    _lib.check(lib.hb_solve_logdet(_lib.ptr(K), _lib.ptr(Linv), yd, n, NP, _lib.ptr(hyp), _lib.ptr(alpha), _lib.ptr(scal),
+                                   _lib.ptr(sws), st), "solve_logdet")
+    _lib.check(lib.hb_kinv(_lib.ptr(Linv), NP, _lib.ptr(tmp), st), "kinv")
+    _lib.check(lib.hb_mll_grad(XtT, n, d, raw, _lib.ptr(hyp), gp.kern_id, _lib.ptr(tmp), _lib.ptr(alpha), _lib.ptr(scal),
+                               float(gp.noise_guess), _lib.ptr(grad), _lib.ptr(loss), _lib.ptr(gws), st), "mll_grad")
+    assert int(info.item()) == 0 and torch.isfinite(grad).all() and torch.isfinite(loss).all()
+    for spec in (None, C.byref(gp._spec)):
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        grad2, loss2, info2 = torch.empty_like(grad), torch.empty_like(loss), torch.zeros_like(info)
+        _lib.check(lib.hb_mll_fwd_bwd(XtT, None, yd, n, d, spec, raw, gp.kern_id, ndd, float(gp.noise_lb), float(gp.noise_guess),
+                                      0.0, _lib.ptr(grad2), _lib.ptr(loss2), _lib.ptr(info2), _lib.ptr(ws), ws_bytes, st),
+                   "hb_mll_fwd_bwd")
+        assert int(info2.item()) == 0
+        assert torch.equal(loss2, loss) and torch.equal(grad2, grad), (kind, hetero, spec is None)
+    loss_e, grad_e = gp.evaluate_loss(return_grad=True)
+    assert torch.equal(torch.tensor([loss_e], dtype=torch.float32), loss.cpu()) and torch.equal(grad_e, grad.cpu())
+
+
 def test_tensor_path_guard_recomputes_cancelling_rows_on_fp32():
     """Tensor-core fp16-split path vs the FP32 SIMT path: rows with sigma^2 << s (dense data: heavy cancellation) are
     flagged by the guard and recomputed on the FP32 pipe (fp64 chunk accumulation); the other rows agree to ~1e-5."""
