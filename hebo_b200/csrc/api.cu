@@ -218,13 +218,7 @@ __global__ void __launch_bounds__(256) psgld_guarded_kernel(float *__restrict__ 
   if (ok) {
     for (int i = threadIdx.x; i < p; i += blockDim.x) {
       if (i >= frozen_begin && i < frozen_end) continue;   // fixed (not learned) warp exponents are not optimiser parameters
-      const float g = grad[i];
-      const float v = a * sq[i] + (1.0f - a) * g * g;
-      sq[i] = v;
-      const float avg = sqrtf(v) + eps;
-      float x = raw[i] - lr * g / avg;
-      if (xi) x += factor * sqrtf(2.0f * lr / avg) * xi[i];
-      raw[i] = x;
+      psgld_update(raw, grad, sq, i, lr, a, eps, factor, xi);
     }
   }
   __syncthreads();   // every thread has read the counters
@@ -252,6 +246,26 @@ static int factor_once(const float *Xt, int64_t n, int64_t np, const ModelSpec &
   s = launch_gram(sp.warp ? w.Zt : Xt, w.Ets, n, np, sp, w.hyp, kern, noise_diag, jitter, w.L, st);
   if (s != HB_OK) return s;
   return launch_cholesky(w.L, np, w.cholws, w.info, st, tc);
+}
+
+// one MLL forward + backward at `raw`: transform -> [gather] -> Gram -> Cholesky -> L^-1 -> alpha / log-det -> K^-1 ->
+// gradient, into w.grad / w.loss (factorisation status in w.info).  tc: the GEMM stages on the 3xTF32 tensor cores, with
+// zero_fill on the first use of the workspace in a fit (see launch_tri_inverse_tc); nullptr: FP32 SIMT.
+static int enqueue_mll(const float *Xt, const float *y, int64_t n, int64_t np, const ModelSpec &sp, const float *raw, int kern,
+                       const float *noise_diag, float noise_lb, float noise_guess, float jitter, FitWs &w, cudaStream_t st,
+                       const TcBuffers *tc, bool zero_fill) {
+  int s = launch_transform_hypers(raw, sp, noise_lb, w.hyp, st);
+  if (s != HB_OK) return s;
+  s = factor_once(Xt, n, np, sp, raw, kern, noise_diag, jitter, w, st, tc);
+  if (s != HB_OK) return s;
+  s = tc ? launch_tri_inverse_tc(w.L, np, w.Linv, *tc, zero_fill, st) : launch_tri_inverse(w.L, np, w.Linv, w.tmp, st);
+  if (s != HB_OK) return s;
+  s = launch_solve_logdet(w.L, w.Linv, y, n, np, w.hyp, w.alpha, w.scal, w.solvews, st);
+  if (s != HB_OK) return s;
+  s = tc ? launch_kinv_tc(np, w.tmp, *tc, st) : launch_kinv(w.Linv, np, w.tmp, st);
+  if (s != HB_OK) return s;
+  return launch_mll_grad(sp.warp ? w.Zt : Xt, w.Ets, n, np, sp, raw, w.hyp, kern, w.tmp, w.alpha, w.scal, noise_guess, w.grad,
+                         w.loss, w.gradws, st, w.dZa, w.dZb);
 }
 
 static float next_jitter(float j) { return j == 0.0f ? 1e-6f : j * 10.0f; }   // fp32 ladder of gp.py:104-110
@@ -466,8 +480,8 @@ int32_t hb_factorize(const float *Xt, const float *y, int64_t n, int64_t d, cons
   return hb_factorize_ex(Xt, nullptr, y, n, d, nullptr, raw, kern, noise_diag, noise_lb, jitter_used, ws, ws_bytes, stream);
 }
 
-// one MLL forward + backward at `raw` (SURVEY 8b `hb_mll_fwd_bwd`): transform -> [gather] -> Gram -> Cholesky -> L^-1 ->
-// alpha / log-det -> K^-1 -> gradient; FP32 SIMT GEMM stages.  Results stay on the device (fit-state grad / loss, `info`).
+// one MLL forward + backward at `raw` (SURVEY 8b `hb_mll_fwd_bwd`) with FP32 SIMT GEMM stages.  Results stay on the device
+// (fit-state grad / loss, `info`).
 int32_t hb_mll_fwd_bwd(const float *Xt, const int32_t *Xe, const float *y, int64_t n, int64_t d, const hb_model_spec_t *spec,
                        const float *raw, int32_t kern, const float *noise_diag, float noise_lb, float noise_guess, float jitter,
                        float *grad, float *loss, int32_t *info, void *ws, int64_t ws_bytes, void *stream) {
@@ -481,18 +495,7 @@ int32_t hb_mll_fwd_bwd(const float *Xt, const int32_t *Xe, const float *y, int64
   const int64_t np = round_up(n, TILE);
   int s = bind_spec_ws(spec, sp, w, Xe, n, st);
   if (s != HB_OK) return s;
-  s = launch_transform_hypers(raw, sp, noise_lb, w.hyp, st);
-  if (s != HB_OK) return s;
-  s = factor_once(Xt, n, np, sp, raw, kern, noise_diag, jitter, w, st, nullptr);
-  if (s != HB_OK) return s;
-  s = launch_tri_inverse(w.L, np, w.Linv, w.tmp, st);
-  if (s != HB_OK) return s;
-  s = launch_solve_logdet(w.L, w.Linv, y, n, np, w.hyp, w.alpha, w.scal, w.solvews, st);
-  if (s != HB_OK) return s;
-  s = launch_kinv(w.Linv, np, w.tmp, st);
-  if (s != HB_OK) return s;
-  s = launch_mll_grad(sp.warp ? w.Zt : Xt, w.Ets, n, np, sp, raw, w.hyp, kern, w.tmp, w.alpha, w.scal, noise_guess, w.grad, w.loss,
-                      w.gradws, st, w.dZa, w.dZb);
+  s = enqueue_mll(Xt, y, n, np, sp, raw, kern, noise_diag, noise_lb, noise_guess, jitter, w, st, nullptr, false);
   if (s != HB_OK) return s;
   HB_CUDA(cudaMemcpyAsync(grad, w.grad, sp.P() * sizeof(float), cudaMemcpyDeviceToDevice, st));
   HB_CUDA(cudaMemcpyAsync(loss, w.loss, sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -523,21 +526,10 @@ int32_t hb_fit_ex(const float *Xt, const int32_t *Xe, const float *y, int64_t n,
   const int pretrain = num_epochs / 10;          // gp.py:99 pretrain_step = num_epochs // 10
   const float factor = 1.0f / (float)n;          // gp.py:99 factor = 1 / y.shape[0]
 
-  // one epoch = transform -> [gather] -> Gram -> Cholesky -> L^-1 -> alpha / log-det -> K^-1 -> gradient -> guarded pSGLD step
+  // one epoch = MLL forward + backward on the tensor cores -> guarded pSGLD step
   auto enqueue_epoch = [&](float jitter, cudaStream_t s_) -> int {
-    int s = launch_transform_hypers(raw, sp, noise_lb, w.hyp, s_);
-    if (s != HB_OK) return s;
-    s = factor_once(Xt, n, np, sp, raw, kern, noise_diag, jitter, w, s_, &w.tc);
-    if (s != HB_OK) return s;
-    s = launch_tri_inverse_tc(w.L, np, w.Linv, w.tc, !zeroed, s_);
+    const int s = enqueue_mll(Xt, y, n, np, sp, raw, kern, noise_diag, noise_lb, noise_guess, jitter, w, s_, &w.tc, !zeroed);
     zeroed = true;
-    if (s != HB_OK) return s;
-    s = launch_solve_logdet(w.L, w.Linv, y, n, np, w.hyp, w.alpha, w.scal, w.solvews, s_);
-    if (s != HB_OK) return s;
-    s = launch_kinv_tc(np, w.tmp, w.tc, s_);
-    if (s != HB_OK) return s;
-    s = launch_mll_grad(sp.warp ? w.Zt : Xt, w.Ets, n, np, sp, raw, w.hyp, kern, w.tmp, w.alpha, w.scal, noise_guess, w.grad, w.loss,
-                        w.gradws, s_, w.dZa, w.dZb);
     if (s != HB_OK) return s;
     psgld_guarded_kernel<<<1, 256, 0, s_>>>(raw, w.grad, w.sq, (int)P, lr, 0.99f, 1e-8f, factor, langevin, pretrain, w.info,
                                            w.loss, w.status, w.hyp, sp.H(), sp.warp == 2 ? sp.i_wa() : 0,

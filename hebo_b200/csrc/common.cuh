@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <math.h>
+#include <type_traits>
 #include "../../include/hebo_b200.h"
 
 namespace hb {
@@ -49,6 +50,24 @@ void prof_end(cudaStream_t st);
     int _s = hb::check_launch(name);                    \
     if (_s != HB_OK) return _s;                         \
   } while (0)
+
+// Kernel-template dispatch: calls f(kk) with kk = std::integral_constant<int, KERN> for the runtime kernel id, so a launch
+// site names its instance as decltype(kk)::value.  An unknown id launches nothing and gives HB_ERR_INVALID.
+template <class F> int with_kernel(int kern, F &&f) {
+  switch (kern) {
+    case HB_KERN_MATERN32: f(std::integral_constant<int, HB_KERN_MATERN32>{}); return HB_OK;
+    case HB_KERN_MATERN52: f(std::integral_constant<int, HB_KERN_MATERN52>{}); return HB_OK;
+    case HB_KERN_RBF:      f(std::integral_constant<int, HB_KERN_RBF>{}); return HB_OK;
+    default: return HB_ERR_INVALID;
+  }
+}
+// ... and f(kk, ee) for kernels templated on <KERN, EMB> as well, ee = std::bool_constant<emb>
+template <class F> int with_kernel(int kern, bool emb, F &&f) {
+  return with_kernel(kern, [&](auto kk) {
+    if (emb) f(kk, std::true_type{});
+    else f(kk, std::false_type{});
+  });
+}
 
 // ---------------------------------------------------------------- stationary kernels
 // k(r2) with unit outputscale.  KERN: 0 Matern-3/2, 1 Matern-5/2, 2 RBF (gpytorch MaternKernel/RBFKernel).
@@ -131,6 +150,19 @@ __device__ __forceinline__ float softplus_f(float u) {
   return u > 20.0f ? u : log1pf(expf(u));
 }
 __device__ __forceinline__ float sigmoid_f(float u) { return 1.0f / (1.0f + expf(-u)); }
+
+// pSGLD update of parameter i: torch.optim.RMSprop step followed by the Langevin term of HEBO/hebo/models/nn/sgld.py:57-70
+// (xi == nullptr: no Langevin term)
+__device__ __forceinline__ void psgld_update(float *raw, const float *grad, float *sq, int i, float lr, float a, float eps,
+                                             float factor, const float *xi) {
+  const float g = grad[i];
+  const float v = a * sq[i] + (1.0f - a) * g * g;
+  sq[i] = v;
+  const float avg = sqrtf(v) + eps;
+  float x = raw[i] - lr * g / avg;
+  if (xi) x += factor * sqrtf(2.0f * lr / avg) * xi[i];
+  raw[i] = x;
+}
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

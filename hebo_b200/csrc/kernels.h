@@ -46,6 +46,25 @@ struct ModelSpec {
   __host__ __device__ int dtot() const { return d + De; }
 };
 
+// ---- candidate feature map (DESIGN §5).  Every kernel that scales candidate rows goes through these two functions, and
+// the training rows take the same operations in the same order (scale_zt_kernel, emb_gather_kernel), so that a candidate
+// duplicating a training row has r = 0 exactly.
+// Index into the embedding tables of embedding coordinate q of row `row` of the categories Xe [rows, e]
+// (EmbTransform.forward, layers.py:33-34).
+__device__ __forceinline__ int emb_entry(const ModelSpec &sp, const int32_t *Xe, int64_t row, int q) {
+  const int c = sp.q_col[q];
+  return sp.tab_off[c] + Xe[row * sp.e + c] * sp.emb_size[c] + sp.q_loc[q];
+}
+// Numeric coordinate k of a candidate x_k: MinMax scale (TorchMinMaxScaler.transform, scalers.py:86-87), the Kumaraswamy
+// warp when `warp`, then the reciprocal of the lengthscale times the result.
+__device__ __forceinline__ float cand_feature(const ModelSpec &sp, bool warp, float x, int k, const float *x_mul,
+                                              const float *x_add, const float *hyp) {
+  float xt = __fadd_rn(__fmul_rn(x_mul[k], x), x_add[k]);
+  if (warp) xt = kumar_warp(xt, hyp[sp.h_wa() + k], hyp[sp.h_wb() + k]);
+  const float *ls = hyp + 3;
+  return xt * (1.0f / ls[k]);
+}
+
 // cholesky.cu / linalg.cu   (tc: outer update on the tensor cores, the gradient epochs; nullptr -> FP32 SIMT)
 int launch_cholesky(float *A, int64_t np, float *ws, int32_t *info, cudaStream_t st, const TcBuffers *tc = nullptr);
 int launch_triinv_base2(const float *L, int64_t np, float *Linv, float *Linv_hi, float *Linv_lo, float *U_hi, float *U_lo,
@@ -91,18 +110,20 @@ size_t posterior_ws_bytes(int64_t np, int64_t d, int64_t m_chunk);
 int guard_stats(unsigned long long *out, int reset);
 int launch_mace_only(const float *mu, const float *var, int64_t m, float noise_var, float tau, float kappa, float eps,
                      const float *xi1, const float *xi2, uint64_t seed, float *F, cudaStream_t st);
-
-// fp16 two-level split tensor path of the posterior (vnorm_h16.cu: wgmma / TMA / mbarrier)
 int kstar_groups(int64_t np);
-int launch_kstar_plain(const float *xs, const int32_t *xe, int64_t mc, const ModelSpec &sp, const float *tab_s,
-                       const float *x_mul, const float *x_add, const float *Zt,
-                       const float *alpha, const float *hyp, int64_t n, int64_t np, int kern, float *KS, float *mupart,
-                       int64_t mc_pad, cudaStream_t st);
+int launch_kstar(const float *xs, const int32_t *xe, int64_t mc, const ModelSpec &sp, const float *tab_s, const float *x_mul,
+                 const float *x_add, const float *Zt, const float *alpha, const float *hyp, int64_t n, int64_t np, int kern,
+                 float *KS, float *KS_h16, float *mupart, int64_t mc_pad, const int32_t *fixlist, const int32_t *fixcount,
+                 cudaStream_t st);
+
+// posterior_grad.cu
 int launch_posterior_grad(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, int64_t np, const ModelSpec &sp,
                           const float *tab_s, const float *x_mul, const float *x_add,
                           const float *Zt, const float *alpha, const float *Linv, const float *hyp, int kern, float y_mean,
                           float y_std, int pred_likeli, float *mu, float *var, float *dmu, float *dvar, void *ws,
                           int64_t ws_bytes, int64_t m_chunk, cudaStream_t st);
+
+// fp16 two-level split tensor path of the posterior (vnorm_h16.cu: wgmma / TMA / mbarrier)
 int launch_split_h16(const float *x, int64_t count, __half *h0, __half *h1, float *scale_slot, cudaStream_t st);
 int launch_vnorm_h16(const __half *ks_h0, const __half *ks_h1, int64_t ks_rows, const __half *linv_h0, const __half *linv_h1,
                      const float *scale_b, const float *hyp, int64_t np, int64_t mc_pad, int64_t vpart_stride, float *vpart,

@@ -130,18 +130,11 @@ int launch_gram(const float *Xt, const float *Ets, int64_t n, int64_t np, const 
   const int nt = (int)(np / PT);
   const int grid = nt * (nt + 1) / 2;
   const int pre = sp.warp ? 1 : 0;   // warped models: the caller passes Zt = warp(Xt) / lengthscale in place of Xt
-#define HB_GRAM(K_)                                                                                                     \
-  do {                                                                                                                  \
-    if (sp.e > 0) gram_kernel<K_, true><<<grid, 256, 0, st>>>(Xt, Ets, n, np, sp.d, sp.De, hyp, noise_diag, jitter, K, pre); \
-    else gram_kernel<K_, false><<<grid, 256, 0, st>>>(Xt, nullptr, n, np, sp.d, 0, hyp, noise_diag, jitter, K, pre);         \
-  } while (0)
-  switch (kern) {
-    case HB_KERN_MATERN32: HB_GRAM(0); break;
-    case HB_KERN_MATERN52: HB_GRAM(1); break;
-    case HB_KERN_RBF:      HB_GRAM(2); break;
-    default: return HB_ERR_INVALID;
-  }
-#undef HB_GRAM
+  const int s = with_kernel(kern, sp.e > 0, [&](auto kk, auto ee) {
+    gram_kernel<decltype(kk)::value, decltype(ee)::value><<<grid, 256, 0, st>>>(Xt, Ets, n, np, sp.d, sp.De, hyp, noise_diag,
+                                                                                 jitter, K, pre);
+  });
+  if (s != HB_OK) return s;
   count_launches(1);
   HB_LAUNCH_CHECK("gram");
   return HB_OK;
@@ -525,18 +518,11 @@ int launch_mll_grad(const float *Xt, const float *Ets, int64_t n, int64_t np, co
   const size_t dyn = (size_t)8 * (3 * d + 3) * sizeof(float);
   if (dyn > 12 * 1024) return HB_ERR_INVALID;  // static 32 KB + dynamic must stay under 48 KB (d <= 381; d <= 127 with a warp)
   float *part = reinterpret_cast<float *>(ws);
-#define HB_MG(K_)                                                                                                  \
-  do {                                                                                                             \
-    if (sp.e > 0) mll_grad_kernel<K_, true><<<grid, 256, dyn, st>>>(Xt, Ets, n, np, d, sp.De, hyp, Kinv, alpha, part, dZa, dZb); \
-    else mll_grad_kernel<K_, false><<<grid, 256, dyn, st>>>(Xt, nullptr, n, np, d, 0, hyp, Kinv, alpha, part, dZa, dZb);     \
-  } while (0)
-  switch (kern) {
-    case HB_KERN_MATERN32: HB_MG(0); break;
-    case HB_KERN_MATERN52: HB_MG(1); break;
-    case HB_KERN_RBF:      HB_MG(2); break;
-    default: return HB_ERR_INVALID;
-  }
-#undef HB_MG
+  int s = with_kernel(kern, sp.e > 0, [&](auto kk, auto ee) {
+    mll_grad_kernel<decltype(kk)::value, decltype(ee)::value><<<grid, 256, dyn, st>>>(Xt, Ets, n, np, d, sp.De, hyp, Kinv, alpha,
+                                                                                       part, dZa, dZb);
+  });
+  if (s != HB_OK) return s;
   mll_finish_kernel<<<1, 256, 0, st>>>(part, grid, n, sp, raw, hyp, alpha, scal, noise_guess, grad, loss);
   count_launches(2);
   if (sp.e > 0) {
@@ -544,11 +530,10 @@ int launch_mll_grad(const float *Xt, const float *Ets, int64_t n, int64_t np, co
     off = (off + 255) / 256 * 256;
     float *gE = reinterpret_cast<float *>(reinterpret_cast<unsigned char *>(ws) + off);
     const dim3 g2((unsigned)nt, (unsigned)nt);
-    switch (kern) {
-      case HB_KERN_MATERN32: emb_rowgrad_kernel<0><<<g2, 256, 0, st>>>(Xt, Ets, n, np, d, sp.De, hyp, Kinv, alpha, gE, sp.warp ? 1 : 0); break;
-      case HB_KERN_MATERN52: emb_rowgrad_kernel<1><<<g2, 256, 0, st>>>(Xt, Ets, n, np, d, sp.De, hyp, Kinv, alpha, gE, sp.warp ? 1 : 0); break;
-      default:               emb_rowgrad_kernel<2><<<g2, 256, 0, st>>>(Xt, Ets, n, np, d, sp.De, hyp, Kinv, alpha, gE, sp.warp ? 1 : 0); break;
-    }
+    s = with_kernel(kern, [&](auto kk) {
+      emb_rowgrad_kernel<decltype(kk)::value><<<g2, 256, 0, st>>>(Xt, Ets, n, np, d, sp.De, hyp, Kinv, alpha, gE, sp.warp ? 1 : 0);
+    });
+    if (s != HB_OK) return s;
     emb_scatter_kernel<<<sp.T, 256, 0, st>>>(gE, nt, n, np, sp, hyp, grad);
     count_launches(2);
   }
@@ -579,18 +564,11 @@ int launch_transform_hypers(const float *raw, const ModelSpec &sp, float noise_l
   return HB_OK;
 }
 
-// torch.optim.RMSprop step followed by the Langevin term of HEBO/hebo/models/nn/sgld.py:57-70
 __global__ void psgld_kernel(float *__restrict__ raw, const float *__restrict__ grad, float *__restrict__ sq, int p,
                              float lr, float a, float eps, float factor, const float *__restrict__ xi) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= p) return;
-  const float g = grad[i];
-  const float v = a * sq[i] + (1.0f - a) * g * g;
-  sq[i] = v;
-  const float avg = sqrtf(v) + eps;
-  float x = raw[i] - lr * g / avg;
-  if (xi) x += factor * sqrtf(2.0f * lr / avg) * xi[i];
-  raw[i] = x;
+  psgld_update(raw, grad, sq, i, lr, a, eps, factor, xi);
 }
 
 int launch_psgld(float *raw, const float *grad, float *sq, int64_t p, float lr, float a, float eps, float factor,
@@ -643,10 +621,7 @@ __global__ void emb_gather_kernel(const float *__restrict__ tables, ModelSpec sp
   const int q = (int)(idx / np);
   const int64_t i = idx - (int64_t)q * np;
   float v = 0.0f;
-  if (i < n) {
-    const int c = sp.q_col[q];
-    v = tables[sp.tab_off[c] + sp.Xe[i * sp.e + c] * sp.emb_size[c] + sp.q_loc[q]] * inv;
-  }
+  if (i < n) v = tables[emb_entry(sp, sp.Xe, i, q)] * inv;
   Ets[idx] = v;
 }
 

@@ -43,16 +43,12 @@ __global__ void __launch_bounds__(256) kstar_kernel(const float *__restrict__ Xs
   const int64_t r0 = (int64_t)blockIdx.x * KS_ROWS;
   const int64_t nrows = fixlist ? (int64_t)*fixcount : mc;
   if (r0 >= nrows) return;   // (block-uniform; only the guard pass launches more blocks than it needs)
-  const float *ls = hyp + 3;
   for (int f = t; f < KS_ROWS * d; f += 256) {
     const int row = f / d, k = f - row * d;
     float z = 0.0f;
     if (r0 + row < nrows) {
       const int64_t src = fixlist ? (int64_t)fixlist[r0 + row] : r0 + row;
-      const float x = Xs[src * d + k];
-      float xt = __fadd_rn(__fmul_rn(x_mul[k], x), x_add[k]);   // TorchMinMaxScaler.transform, scalers.py:86-87
-      if (sp.warp) xt = kumar_warp(xt, hyp[sp.h_wa() + k], hyp[sp.h_wb() + k]);   // input warp fused into the load stage
-      z = xt * (1.0f / ls[k]);
+      z = cand_feature(sp, sp.warp, Xs[src * d + k], k, x_mul, x_add, hyp);   // input warp fused into the load stage
     }
     zs[k * (KS_ROWS + 1) + row] = z;
   }
@@ -63,8 +59,7 @@ __global__ void __launch_bounds__(256) kstar_kernel(const float *__restrict__ Xs
       float z = 0.0f;
       if (r0 + row < nrows) {
         const int64_t src = fixlist ? (int64_t)fixlist[r0 + row] : r0 + row;
-        const int c = sp.q_col[q];
-        z = tab_s[sp.tab_off[c] + Xe_s[src * sp.e + c] * sp.emb_size[c] + sp.q_loc[q]];   // EmbTransform.forward, layers.py:33-34
+        z = tab_s[emb_entry(sp, Xe_s, src, q)];
       }
       zs[(d + q) * (KS_ROWS + 1) + row] = z;
     }
@@ -380,26 +375,29 @@ __global__ void __launch_bounds__(256) mace_kernel(const float *__restrict__ mup
 
 int kstar_groups(int64_t np) { return (int)ceil_div(np, KS_GROUP); }
 
-// plain fp32 K* rows + mean partials (posterior_grad.cu)
-int launch_kstar_plain(const float *xs, const int32_t *xe, int64_t mc, const ModelSpec &sp, const float *tab_s,
-                       const float *x_mul, const float *x_add, const float *Zt,
-                       const float *alpha, const float *hyp, int64_t n, int64_t np, int kern, float *KS, float *mupart,
-                       int64_t mc_pad, cudaStream_t st) {
-  const int d = sp.d;
+// K* rows of the mc candidates xs [mc, d] (categories xe [mc, e]), in one of three output forms:
+//   KS_h16 != nullptr:  the two-level fp16 split into KS_h16 (tensor path), mean partials into mupart;
+//   fixlist != nullptr: the guard pass: KS row `slot` is the exact fp32 row of candidate fixlist[slot], slot < *fixcount
+//                       (mupart nullptr);
+//   otherwise:          fp32 rows into KS, mean partials into mupart.
+int launch_kstar(const float *xs, const int32_t *xe, int64_t mc, const ModelSpec &sp, const float *tab_s, const float *x_mul,
+                 const float *x_add, const float *Zt, const float *alpha, const float *hyp, int64_t n, int64_t np, int kern,
+                 float *KS, float *KS_h16, float *mupart, int64_t mc_pad, const int32_t *fixlist, const int32_t *fixcount,
+                 cudaStream_t st) {
   const size_t dyn = (size_t)sp.dtot() * (KS_ROWS + 1) * sizeof(float);
-  if (dyn > 30 * 1024) return HB_ERR_INVALID;
-  const dim3 g1((unsigned)ceil_div(mc, KS_ROWS), (unsigned)kstar_groups(np));
-#define HB_KP(K)                                                                                                              \
-  do {                                                                                                                        \
-    if (sp.e > 0)                                                                                                             \
-      kstar_kernel<K, 0, true><<<g1, 256, dyn, st>>>(xs, mc, d, x_mul, x_add, Zt, alpha, hyp, n, np, KS, nullptr, mupart,     \
-                                                     mc_pad, nullptr, nullptr, xe, tab_s, sp);                               \
-    else                                                                                                                      \
-      kstar_kernel<K, 0, false><<<g1, 256, dyn, st>>>(xs, mc, d, x_mul, x_add, Zt, alpha, hyp, n, np, KS, nullptr, mupart,    \
-                                                      mc_pad, nullptr, nullptr, nullptr, nullptr, sp);                       \
-  } while (0)
-  if (kern == HB_KERN_MATERN32) HB_KP(0); else if (kern == HB_KERN_MATERN52) HB_KP(1); else HB_KP(2);
-#undef HB_KP
+  if (dyn > 30 * 1024) return HB_ERR_INVALID;   // d + De <= 232 with the static 16 KB tile
+  const dim3 grid((unsigned)ceil_div(mc, KS_ROWS), (unsigned)kstar_groups(np));
+  const int s = with_kernel(kern, sp.e > 0, [&](auto kk, auto ee) {
+    constexpr int KERN = decltype(kk)::value;
+    constexpr bool EMB = decltype(ee)::value;
+    if (KS_h16)
+      kstar_kernel<KERN, 2, EMB><<<grid, 256, dyn, st>>>(xs, mc, sp.d, x_mul, x_add, Zt, alpha, hyp, n, np, KS, KS_h16, mupart,
+                                                         mc_pad, fixlist, fixcount, xe, tab_s, sp);
+    else
+      kstar_kernel<KERN, 0, EMB><<<grid, 256, dyn, st>>>(xs, mc, sp.d, x_mul, x_add, Zt, alpha, hyp, n, np, KS, KS_h16, mupart,
+                                                         mc_pad, fixlist, fixcount, xe, tab_s, sp);
+  });
+  if (s != HB_OK) return s;
   count_launches(1);
   return HB_OK;
 }
@@ -421,8 +419,6 @@ int launch_posterior_mace(const float *Xs, const int32_t *Xe_s, int64_t m, int64
   if (m <= 0 || n <= 0 || sp.dtot() <= 0 || np % GT != 0 || n > np || m_chunk <= 0) return HB_ERR_INVALID;
   if (kern < 0 || kern > 2 || (sp.e > 0 && (!Xe_s || !tab_s))) return HB_ERR_INVALID;
   if ((size_t)ws_bytes < posterior_ws_bytes(np, d, m_chunk)) return HB_ERR_INVALID;
-  const size_t dyn = (size_t)sp.dtot() * (KS_ROWS + 1) * sizeof(float);
-  if (dyn > 30 * 1024) return HB_ERR_INVALID;   // d + De <= 232 with the static 16 KB tile
   const int64_t mc_pad_max = round_up(m_chunk, 2 * GT);
   const int ncg = (int)ceil_div(np, KS_GROUP);
   const int nt = (int)(np / GT);
@@ -442,57 +438,33 @@ int launch_posterior_mace(const float *Xs, const int32_t *Xe_s, int64_t m, int64
   for (int64_t c0 = 0; c0 < m; c0 += m_chunk) {
     const int64_t mc = min(m_chunk, m - c0);
     const int64_t mc_pad = round_up(mc, GT);
-    const dim3 g1((unsigned)ceil_div(mc, KS_ROWS), (unsigned)ncg);
     const float *xs = Xs + c0 * d;
     const int32_t *xe = sp.e > 0 ? Xe_s + c0 * sp.e : nullptr;
-#define HB_KSTAR(K, S)                                                                                                          \
-  do {                                                                                                                          \
-    if (sp.e > 0)                                                                                                               \
-      kstar_kernel<K, S, true><<<g1, 256, dyn, st>>>(xs, mc, (int)d, x_mul, x_add, Zt, alpha, hyp, n, np, KS, KS2, mupart,      \
-                                                     mc_pad_max, nullptr, nullptr, xe, tab_s, sp);                             \
-    else                                                                                                                        \
-      kstar_kernel<K, S, false><<<g1, 256, dyn, st>>>(xs, mc, (int)d, x_mul, x_add, Zt, alpha, hyp, n, np, KS, KS2, mupart,     \
-                                                      mc_pad_max, nullptr, nullptr, nullptr, nullptr, sp);                     \
-  } while (0)
-    if (tensor) {
-      if (kern == HB_KERN_MATERN32) HB_KSTAR(0, 2); else if (kern == HB_KERN_MATERN52) HB_KSTAR(1, 2); else HB_KSTAR(2, 2);
-    } else {
-      if (kern == HB_KERN_MATERN32) HB_KSTAR(0, 0); else if (kern == HB_KERN_MATERN52) HB_KSTAR(1, 0); else HB_KSTAR(2, 0);
-    }
-#undef HB_KSTAR
+    int s = launch_kstar(xs, xe, mc, sp, tab_s, x_mul, x_add, Zt, alpha, hyp, n, np, kern, KS, tensor ? KS2 : nullptr, mupart,
+                         mc_pad_max, nullptr, nullptr, st);
+    if (s != HB_OK) return s;
     int nslots = nt;
     if (tensor) {
       const __half *kh0 = reinterpret_cast<const __half *>(KS2), *kh1 = kh0 + mc_pad_max * np;
-      const int s = launch_vnorm_h16(kh0, kh1, mc_pad_max, reinterpret_cast<const __half *>(Linv_hi),
-                                     reinterpret_cast<const __half *>(Linv_lo), Linv_lo + np * np / 2, hyp, np, mc_pad,
-                                     mc_pad_max, vpart, st);
+      s = launch_vnorm_h16(kh0, kh1, mc_pad_max, reinterpret_cast<const __half *>(Linv_hi),
+                           reinterpret_cast<const __half *>(Linv_lo), Linv_lo + np * np / 2, hyp, np, mc_pad, mc_pad_max, vpart, st);
       if (s != HB_OK) return s;
       nslots = (int)ceil_div(np, 128);
       HB_CUDA(cudaMemsetAsync(fixcount, 0, sizeof(int32_t), st));
       guard_kernel<<<(int)ceil_div(mc, 256), 256, 0, st>>>(vpart, nslots, mc, mc_pad_max, hyp, GUARD_THETA, fixmap, fixlist, fixcount);
+      // exact fp32 K* rows of the flagged candidates only (compact, row = slot), then their FP32 contraction
+      s = launch_kstar(xs, xe, mc, sp, tab_s, x_mul, x_add, Zt, alpha, hyp, n, np, kern, KS, nullptr, nullptr, mc_pad_max, fixlist,
+                       fixcount, st);
+      if (s != HB_OK) return s;
       const dim3 gf((unsigned)nt, (unsigned)(mc_pad / GT));
-      {   // exact fp32 K* rows of the flagged candidates only (compact, row = slot), then their FP32 contraction
-#define HB_KFIX(K)                                                                                                              \
-  do {                                                                                                                          \
-    if (sp.e > 0)                                                                                                               \
-      kstar_kernel<K, 0, true><<<g1, 256, dyn, st>>>(xs, mc, (int)d, x_mul, x_add, Zt, alpha, hyp, n, np, KS, nullptr, nullptr, \
-                                                     mc_pad_max, fixlist, fixcount, xe, tab_s, sp);                            \
-    else                                                                                                                        \
-      kstar_kernel<K, 0, false><<<g1, 256, dyn, st>>>(xs, mc, (int)d, x_mul, x_add, Zt, alpha, hyp, n, np, KS, nullptr, nullptr,\
-                                                      mc_pad_max, fixlist, fixcount, nullptr, nullptr, sp);                    \
-  } while (0)
-        if (kern == HB_KERN_MATERN32) HB_KFIX(0); else if (kern == HB_KERN_MATERN52) HB_KFIX(1); else HB_KFIX(2);
-#undef HB_KFIX
-        count_launches(1);
-      }
       vnorm_fix_kernel<<<gf, GTHREADS, 0, st>>>(KS, nullptr, Linv, np, mc_pad_max, fixlist, fixcount, vfix, 1);
-      count_launches(4);
+      count_launches(3);
     } else {
       const dim3 g2((unsigned)nt, (unsigned)(mc_pad / GT));
       prof_begin(st);
       vnorm_kernel<<<g2, GTHREADS, 0, st>>>(KS, Linv, np, mc_pad_max, vpart);
       prof_end(st);
-      count_launches(3);
+      count_launches(2);
     }
     mace_kernel<<<(int)ceil_div(mc, 256), 256, 0, st>>>(mupart, ncg, vpart, nslots, tensor ? fixmap : nullptr, vfix, nt, mc,
                                                         mc_pad_max, c0, rng_offset, hyp, y_mean, y_std,

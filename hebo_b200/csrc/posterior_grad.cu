@@ -61,19 +61,15 @@ __global__ void __launch_bounds__(256) post_grad_kernel(const float *__restrict_
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
   const int64_t r = blockIdx.x;                 // row inside the chunk
   const int64_t gr = row_offset + r;            // global candidate index
+  // no warp here: the caller applies it in front of this kernel, so that the Jacobian row is x_mul / l
   const float *ls = hyp + 3;
   for (int k = t; k < d; k += 256) {
-    const float xt = __fadd_rn(__fmul_rn(x_mul[k], Xs[gr * d + k]), x_add[k]);
-    const float il = 1.0f / ls[k];
-    zs[k] = xt * il;
-    zs[d + k] = x_mul[k] * il;
+    zs[k] = cand_feature(sp, false, Xs[gr * d + k], k, x_mul, x_add, hyp);
+    zs[d + k] = x_mul[k] * (1.0f / ls[k]);
   }
   const int De = EMB ? sp.De : 0;
   if (EMB) {
-    for (int q = t; q < De; q += 256) {
-      const int c = sp.q_col[q];
-      zs[2 * d + q] = tab_s[sp.tab_off[c] + Xe_s[gr * sp.e + c] * sp.emb_size[c] + sp.q_loc[q]];
-    }
+    for (int q = t; q < De; q += 256) zs[2 * d + q] = tab_s[emb_entry(sp, Xe_s, gr, q)];
   }
   float *v = V + r * np, *w = W + r * np;
   // |v|^2
@@ -169,25 +165,18 @@ int launch_posterior_grad(const float *Xs, const int32_t *Xe_s, int64_t m, int64
   for (int64_t c0 = 0; c0 < m; c0 += m_chunk) {
     const int64_t mc = min(m_chunk, m - c0);
     const int64_t mc_pad = round_up(mc, GT);
-    int s = launch_kstar_plain(Xs + c0 * d, sp.e > 0 ? Xe_s + c0 * sp.e : nullptr, mc, sp, tab_s, x_mul, x_add, Zt, alpha, hyp, n, np,
-                               kern, KS, mupart, mc_pad_max, st);
+    int s = launch_kstar(Xs + c0 * d, sp.e > 0 ? Xe_s + c0 * sp.e : nullptr, mc, sp, tab_s, x_mul, x_add, Zt, alpha, hyp, n, np,
+                         kern, KS, nullptr, mupart, mc_pad_max, nullptr, nullptr, st);
     if (s != HB_OK) return s;
     const dim3 g((unsigned)nt, (unsigned)(mc_pad / GT));
     rows_gemm_kernel<0><<<g, GTHREADS, 0, st>>>(KS, Linv, np, Vb);
     rows_gemm_kernel<1><<<g, GTHREADS, 0, st>>>(Vb, Linv, np, KS);
-#define HB_PG(K)                                                                                                              \
-  do {                                                                                                                        \
-    if (sp.e > 0)                                                                                                             \
-      post_grad_kernel<K, true><<<(unsigned)mc, 256, dyn, st>>>(Xs, (int)d, x_mul, x_add, Zt, alpha, hyp, n, np, Vb, KS,      \
-                                                                mupart, ncg, mc_pad_max, c0, y_mean, y_std, pred_likeli, mu,  \
-                                                                var, dmu, dvar, Xe_s, tab_s, sp);                             \
-    else                                                                                                                      \
-      post_grad_kernel<K, false><<<(unsigned)mc, 256, dyn, st>>>(Xs, (int)d, x_mul, x_add, Zt, alpha, hyp, n, np, Vb, KS,     \
-                                                                 mupart, ncg, mc_pad_max, c0, y_mean, y_std, pred_likeli, mu, \
-                                                                 var, dmu, dvar, nullptr, nullptr, sp);                       \
-  } while (0)
-    if (kern == HB_KERN_MATERN32) HB_PG(0); else if (kern == HB_KERN_MATERN52) HB_PG(1); else HB_PG(2);
-#undef HB_PG
+    s = with_kernel(kern, sp.e > 0, [&](auto kk, auto ee) {
+      post_grad_kernel<decltype(kk)::value, decltype(ee)::value><<<(unsigned)mc, 256, dyn, st>>>(
+          Xs, (int)d, x_mul, x_add, Zt, alpha, hyp, n, np, Vb, KS, mupart, ncg, mc_pad_max, c0, y_mean, y_std, pred_likeli, mu,
+          var, dmu, dvar, Xe_s, tab_s, sp);
+    });
+    if (s != HB_OK) return s;
     count_launches(3);
   }
   HB_LAUNCH_CHECK("posterior_grad");
@@ -216,14 +205,8 @@ __global__ void cand_features_kernel(const float *__restrict__ Xs, const int32_t
   const int64_t i = idx - (int64_t)k * mp;
   float z = 0.0f;
   if (i < m) {
-    if (k < sp.d) {     // same arithmetic as the K* load stage (posterior.cu)
-      float xt = __fadd_rn(__fmul_rn(x_mul[k], Xs[i * sp.d + k]), x_add[k]);
-      if (sp.warp) xt = kumar_warp(xt, hyp[sp.h_wa() + k], hyp[sp.h_wb() + k]);
-      z = xt * (1.0f / hyp[3 + k]);
-    } else {
-      const int q = k - sp.d, c = sp.q_col[q];
-      z = tab_s[sp.tab_off[c] + Xe_s[i * sp.e + c] * sp.emb_size[c] + sp.q_loc[q]];
-    }
+    if (k < sp.d) z = cand_feature(sp, sp.warp, Xs[i * sp.d + k], k, x_mul, x_add, hyp);
+    else z = tab_s[emb_entry(sp, Xe_s, i, k - sp.d)];
   }
   ZsT[idx] = z;
 }
@@ -296,7 +279,7 @@ int launch_sample_y(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, 
   float *cholws = ZsT + (int64_t)sp.dtot() * mp;
   int32_t *info = reinterpret_cast<int32_t *>(cholws + GT * GT);
   HB_CUDA(cudaMemsetAsync(KS, 0, (size_t)mp * np * sizeof(float), st));     // rows m..mp of K* must be zero for the GEMMs
-  int s = launch_kstar_plain(Xs, Xe_s, m, sp, tab_s, x_mul, x_add, Zt, alpha, hyp, n, np, kern, KS, mupart, mp, st);
+  int s = launch_kstar(Xs, Xe_s, m, sp, tab_s, x_mul, x_add, Zt, alpha, hyp, n, np, kern, KS, nullptr, mupart, mp, nullptr, nullptr, st);
   if (s != HB_OK) return s;
   const dim3 g((unsigned)(np / GT), (unsigned)(mp / GT));
   rows_gemm_kernel<0><<<g, GTHREADS, 0, st>>>(KS, Linv, np, Vb);
