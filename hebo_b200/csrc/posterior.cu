@@ -11,6 +11,7 @@
 #include "gemm_core.cuh"
 #include "h16.cuh"
 #include "kernels.h"
+#include "vnorm_sched.h"
 
 namespace hb {
 
@@ -18,6 +19,10 @@ constexpr int KS_ROWS = 32;     // candidates per CTA in kstar_kernel
 constexpr int KS_COLS = 128;    // training points per sub-tile
 constexpr int KS_GROUP = 512;   // training points per CTA (4 sub-tiles)
 constexpr int KS_DC = 32;
+// chunk rows of the workspace are rounded to whole clusters of 128-row bands: the tensor contraction pads the band count
+// of a chunk to a multiple of the cluster size
+constexpr int64_t CHUNK_ROWS = h16::CLUSTER * h16::BM;
+static_assert(CHUNK_ROWS % (2 * GT) == 0, "chunk rows: a multiple of 2 GT");
 
 // SPLIT: 0 = plain fp32 K* in KS (SIMT contraction / guard pass); 2 = the two-level fp16 split in the KS_lo buffer
 // (h0 [mc_pad, np] halfs, then h1) and nothing else.
@@ -403,7 +408,7 @@ int launch_kstar(const float *xs, const int32_t *xe, int64_t mc, const ModelSpec
 }
 
 size_t posterior_ws_bytes(int64_t np, int64_t d, int64_t m_chunk) {
-  const int64_t mc_pad = round_up(m_chunk, 2 * GT);
+  const int64_t mc_pad = round_up(m_chunk, CHUNK_ROWS);
   const int64_t ncg = ceil_div(np, KS_GROUP);
   const int64_t nt = np / GT;
   return (size_t)(2 * mc_pad * np + ncg * mc_pad + 2 * nt * mc_pad + 2 * mc_pad) * sizeof(float) + 512;
@@ -419,14 +424,15 @@ int launch_posterior_mace(const float *Xs, const int32_t *Xe_s, int64_t m, int64
   if (m <= 0 || n <= 0 || sp.dtot() <= 0 || np % GT != 0 || n > np || m_chunk <= 0) return HB_ERR_INVALID;
   if (kern < 0 || kern > 2 || (sp.e > 0 && (!Xe_s || !tab_s))) return HB_ERR_INVALID;
   if ((size_t)ws_bytes < posterior_ws_bytes(np, d, m_chunk)) return HB_ERR_INVALID;
-  const int64_t mc_pad_max = round_up(m_chunk, 2 * GT);
+  const int64_t mc_pad_max = round_up(m_chunk, CHUNK_ROWS);
   const int ncg = (int)ceil_div(np, KS_GROUP);
   const int nt = (int)(np / GT);
   const bool tensor = Linv_hi != nullptr && Linv_lo != nullptr;   // wgmma path (two-level fp16 split), else FP32 SIMT
   // workspace: the K* chunk (KS: fp32 rows of the SIMT / guard passes; KS2: the fp16 two-level split h0 | h1 of the
   // tensor path), the mean partials and the per-chunk partial-sum buffers.  (Building chunk i+1 on a side stream under
-  // the tensor-core contraction of chunk i was measured and dropped: the contraction draws ~all of the L2 -> SM
-  // bandwidth, the co-running CUDA-core kernel slowed it by 30 %.)
+  // the tensor-core contraction of chunk i was measured and dropped: the contraction then drew ~all of the L2 -> SM
+  // bandwidth, the co-running CUDA-core kernel slowed it by 30 %.  Since the Linv multicast it draws 5/8 of those bytes
+  // per k-block; the overlap has not been measured again.)
   float *KS = reinterpret_cast<float *>(ws);
   float *KS2 = KS + mc_pad_max * np;
   float *mupart = KS2 + mc_pad_max * np;

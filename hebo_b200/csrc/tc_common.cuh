@@ -12,6 +12,9 @@
 //                                         wait for all groups, release the last stage and run the epilogue from registers
 //                                         while the producer already fills the ring for the next tile
 // Stage barriers carry one phase bit per ring wrap; every wait is bounded (mbar_wait traps instead of hanging the GPU).
+// vnorm_h16.cu runs the same ring in clusters of CTAs that multicast the shared operand: there a stage is released by one
+// lane per consumer warp on the empty[stage] barrier of EVERY CTA of the cluster (each producer writes into its peers'
+// stages), and a cluster barrier follows the barrier init and precedes exit.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -21,7 +24,7 @@ namespace hb {
 namespace tc {
 
 constexpr uint32_t SPIN_LIMIT = 1u << 26;
-constexpr int CONSUMER_THREADS = 256;   // two consumer warpgroups: the arrival count of every empty[stage] barrier
+constexpr int CONSUMER_THREADS = 256;   // two consumer warpgroups: the arrival count of tcgemm.cu's empty[stage] barriers
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -54,10 +57,46 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 }
 __device__ __forceinline__ void mbar_init_fence() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 
+// ---- thread-block clusters (vnorm_h16.cu)
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t cluster_id_x() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster; orders the shared-memory writes and barrier inits before it (release) against
+// the accesses after it (acquire).  Not .aligned: the threads of a warp may reach it at different points.
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// arrive on the mbarrier at shared address `bar` of CTA `cta` of the cluster (this CTA included).  Default (.release.cta)
+// semantics, as a consumer release needs: it orders this thread's completed shared-memory reads before the arrive without
+// the GPU-scope fence that .release.cluster costs on every k-block.
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 remote;\n\t"
+      "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [remote];\n\t}" ::"r"(bar), "r"(cta)
+      : "memory");
+}
+
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c_inner, int c_outer) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
       "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c_inner), "r"(c_outer)
+      : "memory");
+}
+// the same box written to the same shared offset `dst` of every CTA in `cta_mask`, each signalling its own mbarrier at `bar`
+__device__ __forceinline__ void tma_load_2d_multicast(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c_inner,
+                                                      int c_outer, uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], "
+      "[%2], %5;" ::"r"(dst),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c_inner), "r"(c_outer), "h"(cta_mask)
       : "memory");
 }
 

@@ -21,34 +21,33 @@
 #include "h16.cuh"
 #include "kernels.h"
 #include "tc_common.cuh"
+#include "vnorm_sched.h"
 
 namespace hb {
 namespace h16 {
 using namespace hb::tc;
 
-constexpr int BM = 128;            // candidates per tile (two consumer warpgroups of 64)
-constexpr int BN = 128;            // Linv rows per tile (wgmma N)
-constexpr int BK = 64;             // fp16 elements per k-block = one 128-byte swizzle row
 constexpr int UK = 16;             // wgmma K for f16
 constexpr int STAGES = 3;
 constexpr uint32_t A_BYTES = BM * BK * 2;                  // 16 KiB
 constexpr uint32_t B_BYTES = BN * BK * 2;                  // 16 KiB
+constexpr uint32_t B_SLICE = B_BYTES / CLUSTER;            // the Linv rows of a box that one CTA loads for the cluster
 constexpr uint32_t STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;  // 64 KiB
 constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+static_assert(B_SLICE % 1024 == 0, "a multicast Linv slice must start on a SWIZZLE_128B atom (8 rows x 128 B)");
 
-// Tile schedule: a host-built list per CTA (codes rt << 16 | J, terminated by -1).  Tiles are handed out in BAND-MAJOR
-// order -- all column tiles J of one 128-candidate band, heaviest (longest k range) first, before the next band -- to
-// whichever CTA is least loaded at that point (a simulation of a dynamic scheduler with the k-block count + an epilogue
-// allowance as the cost; the last bands are dealt heaviest-first ACROSS bands so that the lists end with cheap tiles).
-// Two effects: the CTAs finish within a few per cent of each other, and the CTAs working on one band at the same time
-// read its K* rows once from HBM and then from L2, instead of streaming the whole K* chunk once per column tile.
-__device__ __forceinline__ bool next_tile(const int32_t *__restrict__ list, int it, int &rt, int &J) {
+__device__ __forceinline__ bool next_tile(const int32_t *__restrict__ list, int it, int &p, int &J) {
   const int code = __ldg(list + it);
-  rt = code >> 16;
+  p = code >> 16;
   J = code & 0xffff;
   return code >= 0;
 }
 
+// Clusters of CLUSTER CTAs (schedule: vnorm_sched.h).  The CTAs of a cluster run the same column tile J on neighbouring
+// bands, so they need the same Linv boxes: each producer loads 1 / CLUSTER of the rows of every Linv box and multicasts it
+// to the same stage offset in every CTA of the cluster, signalling each CTA's own full[stage].  The K* boxes stay per CTA.
+// Because a producer writes into its peers' stages, a stage is free only when the consumers of ALL CTAs of the cluster
+// have released it: one lane per consumer warp arrives on empty[stage] of every CTA.
 __global__ void __launch_bounds__(384, 1)
 vnorm_h16_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                  const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo, int np,
@@ -59,123 +58,135 @@ vnorm_h16_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_cons
   const uint32_t full_bar = base + STAGES * STAGE_BYTES;          // [STAGES] 8-byte mbarriers after the tiles
   const uint32_t empty_bar = full_bar + 8 * STAGES;               // [STAGES]
   const int wg = threadIdx.x >> 7;
-  const int32_t *my_tiles = sched + (int64_t)blockIdx.x * sched_len;
+  const int rank = (int)cluster_ctarank();
+  const int32_t *my_tiles = sched + (int64_t)cluster_id_x() * sched_len;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar + 8 * s, 1);                      // the producer's arrive + all bytes
-      mbar_init(empty_bar + 8 * s, CONSUMER_THREADS);
+      mbar_init(full_bar + 8 * s, 1);                             // the local producer's arrive + all bytes
+      mbar_init(empty_bar + 8 * s, CLUSTER * CONSUMER_THREADS / 32);   // one lane per consumer warp of the cluster
     }
     mbar_init_fence();
   }
-  __syncthreads();
+  cluster_sync();   // the peers' barriers are initialised before any multicast or remote arrive reaches them
 
-  if (wg == 0) {
+  if (threadIdx.x == 0) {
     // ------------------------------------------------------------------ TMA producer
-    if (threadIdx.x != 0) return;
     int stage = 0;
     uint32_t phase = 0;
     for (int it = 0;; ++it) {
-      int rt, J;
-      if (!next_tile(my_tiles, it, rt, J)) break;
+      int p, J;
+      if (!next_tile(my_tiles, it, p, J)) break;
+      const int rt = p * CLUSTER + rank;
       const int kend = min((J + 1) * BN, np);
       for (int k0 = 0; k0 < kend; k0 += BK) {
         mbar_wait(empty_bar + 8 * stage, phase ^ 1u);
         const uint32_t sb = base + stage * STAGE_BYTES;
         const uint32_t fb = full_bar + 8 * stage;
+        // the whole stage, the peers' multicast slices included (their complete_tx may land before this expect_tx; the
+        // phase cannot complete before this arrive)
         mbar_expect_tx(fb, STAGE_BYTES);
         tma_load_2d(sb, &map_a_hi, fb, k0, rt * BM);
         tma_load_2d(sb + A_BYTES, &map_a_lo, fb, k0, rt * BM);
-        tma_load_2d(sb + 2 * A_BYTES, &map_b_hi, fb, k0, J * BN);
-        tma_load_2d(sb + 2 * A_BYTES + B_BYTES, &map_b_lo, fb, k0, J * BN);
+        const uint32_t slice = rank * B_SLICE;
+        const int brow = J * BN + rank * (BN / CLUSTER);
+        tma_load_2d_multicast(sb + 2 * A_BYTES + slice, &map_b_hi, fb, k0, brow, (1u << CLUSTER) - 1);
+        tma_load_2d_multicast(sb + 2 * A_BYTES + B_BYTES + slice, &map_b_lo, fb, k0, brow, (1u << CLUSTER) - 1);
         if (++stage == STAGES) {
           stage = 0;
           phase ^= 1u;
         }
       }
     }
-    return;
-  }
-
-  // -------------------------------------------------------------------- consumers: 64 candidate rows each
-  const int half = wg - 1;
-  const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
-  const uint32_t a_off = (uint32_t)half * 64 * BK * 2;
-  const float inv = 1.0f / (pow2_scale(hyp[2], 1) * scale_b[0]);   // undo the operand scales (exact: powers of two)
-  const float lo_w = inv * (1.0f / 2048.0f);
-  int stage = 0;
-  uint32_t phase = 0;
-  // two accumulators per tile: MAIN takes hi*hi only, CROSS the two small hi*lo terms.  The tensor core's fp32
-  // accumulation truncates; keeping the 2^-11-sized cross terms out of the main sum cuts the truncations on it by 3x.
-  float acc_main[BN / 2], acc_cross[BN / 2];
-  for (int it = 0;; ++it) {
-    int rt, J;
-    if (!next_tile(my_tiles, it, rt, J)) break;
-    const int kend = min((J + 1) * BN, np);
+  } else if (wg > 0) {
+    // ------------------------------------------------------------------ consumers: 64 candidate rows each
+    const int half = wg - 1;
+    const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+    const uint32_t a_off = (uint32_t)half * 64 * BK * 2;
+    const float inv = 1.0f / (pow2_scale(hyp[2], 1) * scale_b[0]);   // undo the operand scales (exact: powers of two)
+    const float lo_w = inv * (1.0f / 2048.0f);
+    // after the warp's wgmma.wait_group: the MMAs that read the stage have retired for the whole warp
+    auto release = [&](int s) {
+      if (lane == 0)
+        for (int c = 0; c < CLUSTER; ++c) mbar_arrive_cluster(empty_bar + 8 * s, (uint32_t)c);
+    };
+    int stage = 0;
+    uint32_t phase = 0;
+    // two accumulators per tile: MAIN takes hi*hi only, CROSS the two small hi*lo terms.  The tensor core's fp32
+    // accumulation truncates; keeping the 2^-11-sized cross terms out of the main sum cuts the truncations on it by 3x.
+    float acc_main[BN / 2], acc_cross[BN / 2];
+    for (int it = 0;; ++it) {
+      int p, J;
+      if (!next_tile(my_tiles, it, p, J)) break;
+      const int rt = p * CLUSTER + rank;
+      const int kend = min((J + 1) * BN, np);
 #pragma unroll
-    for (int i = 0; i < BN / 2; ++i) {
-      acc_main[i] = 0.0f;
-      acc_cross[i] = 0.0f;
-    }
-    int prev = -1;
-    for (int k0 = 0; k0 < kend; k0 += BK) {
-      mbar_wait(full_bar + 8 * stage, phase);              // TMA bytes have landed
-      const uint32_t sb = base + stage * STAGE_BYTES;
-      const uint64_t da_hi = make_sw128_desc(sb + a_off);
-      const uint64_t da_lo = make_sw128_desc(sb + A_BYTES + a_off);
-      const uint64_t db_hi = make_sw128_desc(sb + 2 * A_BYTES);
-      const uint64_t db_lo = make_sw128_desc(sb + 2 * A_BYTES + B_BYTES);
+      for (int i = 0; i < BN / 2; ++i) {
+        acc_main[i] = 0.0f;
+        acc_cross[i] = 0.0f;
+      }
+      int prev = -1;
+      for (int k0 = 0; k0 < kend; k0 += BK) {
+        mbar_wait(full_bar + 8 * stage, phase);              // TMA bytes have landed
+        const uint32_t sb = base + stage * STAGE_BYTES;
+        const uint64_t da_hi = make_sw128_desc(sb + a_off);
+        const uint64_t da_lo = make_sw128_desc(sb + A_BYTES + a_off);
+        const uint64_t db_hi = make_sw128_desc(sb + 2 * A_BYTES);
+        const uint64_t db_lo = make_sw128_desc(sb + 2 * A_BYTES + B_BYTES);
+        fence_regs(acc_main);
+        fence_regs(acc_cross);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / UK; ++k) {
+          const uint64_t adv = (uint64_t)((k * UK * 2) >> 4);   // 32 bytes per k-step inside the 128-byte swizzle row
+          wgmma_f16_n128(acc_main, da_hi + adv, db_hi + adv);
+          wgmma_f16_n128(acc_cross, da_hi + adv, db_lo + adv);
+          wgmma_f16_n128(acc_cross, da_lo + adv, db_hi + adv);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                                     // the previous k-block's MMAs have retired
+        fence_regs(acc_main);
+        fence_regs(acc_cross);
+        if (prev >= 0) release(prev);
+        prev = stage;
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1u;
+        }
+      }
+      wgmma_wait<0>();
       fence_regs(acc_main);
       fence_regs(acc_cross);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < BK / UK; ++k) {
-        const uint64_t adv = (uint64_t)((k * UK * 2) >> 4);   // 32 bytes per k-step inside the 128-byte swizzle row
-        wgmma_f16_n128(acc_main, da_hi + adv, db_hi + adv);
-        wgmma_f16_n128(acc_cross, da_hi + adv, db_lo + adv);
-        wgmma_f16_n128(acc_cross, da_lo + adv, db_hi + adv);
-      }
-      wgmma_commit();
-      wgmma_wait<1>();                                     // the previous k-block's MMAs have retired
-      fence_regs(acc_main);
-      fence_regs(acc_cross);
-      if (prev >= 0) mbar_arrive(empty_bar + 8 * prev);
-      prev = stage;
-      if (++stage == STAGES) {
-        stage = 0;
-        phase ^= 1u;
-      }
-    }
-    wgmma_wait<0>();
-    fence_regs(acc_main);
-    fence_regs(acc_cross);
-    mbar_arrive(empty_bar + 8 * prev);
+      release(prev);
 
-    // epilogue: thread holds rows r and r + 8 of its warpgroup's 64, two columns of every 8; the 4 lanes of a quad share
-    // the rows
-    float s0 = 0.f, s1 = 0.f, t0 = 0.f, t1 = 0.f;
+      // epilogue: thread holds rows r and r + 8 of its warpgroup's 64, two columns of every 8; the 4 lanes of a quad share
+      // the rows
+      float s0 = 0.f, s1 = 0.f, t0 = 0.f, t1 = 0.f;
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const float x0 = fmaf(acc_cross[4 * j + 0], lo_w, acc_main[4 * j + 0] * inv);
-      const float x1 = fmaf(acc_cross[4 * j + 1], lo_w, acc_main[4 * j + 1] * inv);
-      const float x2 = fmaf(acc_cross[4 * j + 2], lo_w, acc_main[4 * j + 2] * inv);
-      const float x3 = fmaf(acc_cross[4 * j + 3], lo_w, acc_main[4 * j + 3] * inv);
-      s0 = fmaf(x0, x0, s0);
-      s1 = fmaf(x1, x1, s1);
-      t0 = fmaf(x2, x2, t0);
-      t1 = fmaf(x3, x3, t1);
-    }
-    float s = s0 + s1, t = t0 + t1;
-    s += __shfl_xor_sync(0xffffffffu, s, 1);
-    t += __shfl_xor_sync(0xffffffffu, t, 1);
-    s += __shfl_xor_sync(0xffffffffu, s, 2);
-    t += __shfl_xor_sync(0xffffffffu, t, 2);
-    if ((lane & 3) == 0) {
-      float *out = vpart + (int64_t)J * mc_pad + (int64_t)rt * BM + half * 64 + w * 16 + (lane >> 2);
-      out[0] = s;
-      out[8] = t;
+      for (int j = 0; j < BN / 8; ++j) {
+        const float x0 = fmaf(acc_cross[4 * j + 0], lo_w, acc_main[4 * j + 0] * inv);
+        const float x1 = fmaf(acc_cross[4 * j + 1], lo_w, acc_main[4 * j + 1] * inv);
+        const float x2 = fmaf(acc_cross[4 * j + 2], lo_w, acc_main[4 * j + 2] * inv);
+        const float x3 = fmaf(acc_cross[4 * j + 3], lo_w, acc_main[4 * j + 3] * inv);
+        s0 = fmaf(x0, x0, s0);
+        s1 = fmaf(x1, x1, s1);
+        t0 = fmaf(x2, x2, t0);
+        t1 = fmaf(x3, x3, t1);
+      }
+      float s = s0 + s1, t = t0 + t1;
+      s += __shfl_xor_sync(0xffffffffu, s, 1);
+      t += __shfl_xor_sync(0xffffffffu, t, 1);
+      s += __shfl_xor_sync(0xffffffffu, s, 2);
+      t += __shfl_xor_sync(0xffffffffu, t, 2);
+      if ((lane & 3) == 0) {
+        float *out = vpart + (int64_t)J * mc_pad + (int64_t)rt * BM + half * 64 + w * 16 + (lane >> 2);
+        out[0] = s;
+        out[8] = t;
+      }
     }
   }
+  // no CTA leaves while a peer may still multicast into its shared memory or arrive on its barriers
+  cluster_sync();
 }
 
 
@@ -200,51 +211,26 @@ namespace h16 {
 
 struct SchedEntry {
   int32_t *dev = nullptr;
-  int len = 0, ctas = 0;
+  int len = 0;
 };
 struct SchedKey {
-  int dev, np, n_rt, ctas;
+  int dev, np, n_rt, clusters, cluster;
   bool operator<(const SchedKey &o) const {
     if (dev != o.dev) return dev < o.dev;
     if (np != o.np) return np < o.np;
     if (n_rt != o.n_rt) return n_rt < o.n_rt;
-    return ctas < o.ctas;
+    if (clusters != o.clusters) return clusters < o.clusters;
+    return cluster < o.cluster;
   }
 };
 
-static const SchedEntry *get_schedule(int dev, int np, int n_rt, int ctas, cudaStream_t st) {
+static const SchedEntry *get_schedule(int dev, int np, int n_rt, int clusters, cudaStream_t st) {
   static std::map<SchedKey, SchedEntry> cache;
-  const SchedKey key{dev, np, n_rt, ctas};
+  const SchedKey key{dev, np, n_rt, clusters, CLUSTER};
   auto it = cache.find(key);
   if (it != cache.end()) return &it->second;
-  const int n_j = (np + BN - 1) / BN;
-  constexpr int EPI_COST = 1;   // epilogue in k-block units (a register drain and one shuffle reduction per tile)
-  std::vector<std::vector<int32_t>> lists(ctas);
-  std::vector<long long> load(ctas, 0);
-  // band-major body, then the tiles of the last TAIL_BANDS bands heaviest-first across bands (an LPT tail: the list ends
-  // with the cheapest tiles, which levels the CTAs instead of leaving one heavy tile of overhang)
-  constexpr int TAIL_BANDS = 16;
-  const int body = std::max(0, n_rt - TAIL_BANDS);
-  auto give = [&](int rt, int J) {
-    int best = 0;
-    for (int p = 1; p < ctas; ++p)
-      if (load[p] < load[best]) best = p;
-    const int kend = std::min((J + 1) * BN, np);
-    load[best] += kend / BK + EPI_COST;
-    lists[best].push_back((rt << 16) | J);
-  };
-  for (int rt = 0; rt < body; ++rt)
-    for (int J = n_j - 1; J >= 0; --J) give(rt, J);
-  for (int J = n_j - 1; J >= 0; --J)
-    for (int rt = body; rt < n_rt; ++rt) give(rt, J);
-  size_t len = 0;
-  for (auto &l : lists) len = std::max(len, l.size());
-  len += 1;
-  std::vector<int32_t> flat((size_t)ctas * len, -1);
-  for (int p = 0; p < ctas; ++p) std::copy(lists[p].begin(), lists[p].end(), flat.begin() + (size_t)p * len);
   SchedEntry e;
-  e.len = (int)len;
-  e.ctas = ctas;
+  const std::vector<int32_t> flat = build_schedule(np, n_rt, clusters, &e.len);
   if (cudaMalloc(&e.dev, flat.size() * sizeof(int32_t)) != cudaSuccess) return nullptr;
   if (cudaMemcpyAsync(e.dev, flat.data(), flat.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st) != cudaSuccess ||
       cudaStreamSynchronize(st) != cudaSuccess)   // `flat` is pageable and dies with this frame
@@ -255,43 +241,67 @@ static const SchedEntry *get_schedule(int dev, int np, int n_rt, int ctas, cudaS
 }  // namespace h16
 
 // ks_h0 / ks_h1 [ks_rows, np] fp16 split of K* (scale 2^k from the outputscale hyp[2]); linv_h0 / linv_h1 [np, np] fp16 split
-// of Linv with the device scalar scale_b; ks_rows and mc_pad multiples of 128
+// of Linv with the device scalar scale_b; ks_rows and mc_pad multiples of 128.  The rows of K* and vpart up to
+// round_up(mc_pad, CLUSTER * BM) must exist: the last cluster runs padding bands there when the band count is not a
+// multiple of CLUSTER.
 int launch_vnorm_h16(const __half *ks_h0, const __half *ks_h1, int64_t ks_rows, const __half *linv_h0, const __half *linv_h1,
                      const float *scale_b, const float *hyp, int64_t np, int64_t mc_pad, int64_t vpart_stride, float *vpart,
                      cudaStream_t st) {
   using namespace h16;
-  if (np % TILE != 0 || mc_pad % BM != 0 || mc_pad > ks_rows || np > 65535 * BN || mc_pad / BM > 32767) return HB_ERR_INVALID;
-  static PerDevice once;
+  const int64_t rows = round_up(mc_pad, (int64_t)CLUSTER * BM);   // bands rounded up to whole clusters
+  if (np % TILE != 0 || mc_pad % BM != 0 || rows > ks_rows || rows > vpart_stride || np > 65535 * BN || mc_pad / BM > 32767)
+    return HB_ERR_INVALID;
+  static PerDevice once;   // aux: the most clusters of this kernel that fit on the device at once
   bool fresh = false;
   const int dev = once.slot(&fresh);
   if (dev < 0) return HB_ERR_CUDA;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = CLUSTER;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(CLUSTER);
+  cfg.blockDim = dim3(384);
+  cfg.dynamicSmemBytes = SMEM_BYTES;
+  cfg.stream = st;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
   if (fresh) {   // per DEVICE: cudaFuncSetAttribute applies to the current device only
-    HB_CUDA(cudaDeviceGetAttribute(&once.sms[dev], cudaDevAttrMultiProcessorCount, dev));
     HB_CUDA(cudaFuncSetAttribute(vnorm_h16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+    HB_CUDA(cudaOccupancyMaxActiveClusters(&once.aux[dev], vnorm_h16_kernel, &cfg));
+    if (once.aux[dev] < 1) {
+      set_error(cudaErrorInvalidConfiguration, "vnorm_h16: no cluster fits on the device");
+      return HB_ERR_CUDA;
+    }
     once.done[dev] = true;
   }
   CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
   if (!make_map(&ma_hi, ks_h0, (uint64_t)ks_rows, (uint64_t)np, BM) ||
       !make_map(&ma_lo, ks_h1, (uint64_t)ks_rows, (uint64_t)np, BM) ||
-      !make_map(&mb_hi, linv_h0, (uint64_t)np, (uint64_t)np, BN) ||
-      !make_map(&mb_lo, linv_h1, (uint64_t)np, (uint64_t)np, BN)) {
+      !make_map(&mb_hi, linv_h0, (uint64_t)np, (uint64_t)np, BN / CLUSTER) ||
+      !make_map(&mb_lo, linv_h1, (uint64_t)np, (uint64_t)np, BN / CLUSTER)) {
     set_error(cudaErrorUnknown, "cuTensorMapEncodeTiled");
     return HB_ERR_CUDA;
   }
   const int n_rt = (int)(mc_pad / BM);
   const int n_j = (int)ceil_div(np, BN);
-  const int total = n_rt * n_j;
-  int ctas = once.sms[dev];
-  if (total < ctas) ctas = total;
-  const SchedEntry *sc = get_schedule(dev, (int)np, n_rt, ctas, st);
+  const int units = (int)(rows / BM / CLUSTER) * n_j;
+  const int clusters = std::min(once.aux[dev], units);
+  const SchedEntry *sc = get_schedule(dev, (int)np, n_rt, clusters, st);
   if (!sc) {
     set_error(cudaErrorMemoryAllocation, "vnorm_h16 schedule table");
     return HB_ERR_CUDA;
   }
+  cfg.gridDim = dim3((unsigned)(clusters * CLUSTER));
   prof_begin(st);
-  vnorm_h16_kernel<<<ctas, 384, SMEM_BYTES, st>>>(ma_hi, ma_lo, mb_hi, mb_lo, (int)np, sc->dev, sc->len, vpart_stride, vpart,
-                                                     hyp, scale_b);
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, vnorm_h16_kernel, ma_hi, ma_lo, mb_hi, mb_lo, (int)np, (const int32_t *)sc->dev,
+                                           sc->len, vpart_stride, vpart, hyp, scale_b);
   prof_end(st);
+  if (e != cudaSuccess) {
+    set_error(e, "vnorm_h16 cluster launch");
+    return HB_ERR_CUDA;
+  }
   count_launches(1);
   HB_LAUNCH_CHECK("vnorm_h16");
   return HB_OK;
