@@ -86,6 +86,8 @@ SIGNATURES = {
     "hb_nsga2_init": (_i32, [_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _u64, _vp, _vp, _vp]),
     "hb_nsga2_mate": (_i32, [_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _u64, _i32, _vp, _vp, _vp, _vp]),
     "hb_nsga2_survive": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "hb_nsga2_workspace_bytes": (_i64, [_i64, _i64]),
+    "hb_nsga2_survive_ex": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
     "hb_front_merge_workspace_bytes": (_i64, [_i64, _i64]),
     "hb_front_pack": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp]),
     "hb_front_merge": (_i32, [_vp, _i64, _i64, _vp, _vp, _i64, _vp]),

@@ -768,7 +768,17 @@ int32_t hb_nsga2_mate(const float *X, int64_t pop, int64_t D, int64_t d, const i
 int32_t hb_nsga2_survive(const float *X, const float *F, const float *C, const float *FC, int64_t pop, int64_t D, int64_t d,
                          float *X_next, float *F_next, float *Xc_next, int32_t *Xe_next, void *stream) {
   if (!X || !F || !C || !FC || !X_next || !F_next || (d > 0 && !Xc_next) || (D > d && !Xe_next)) return HB_ERR_INVALID;
-  return launch_nsga_survive(X, F, C, FC, pop, D, d, X_next, F_next, Xc_next, Xe_next, (cudaStream_t)stream);
+  if (pop > 256) return HB_ERR_INVALID;   // the workspace-free entry keeps the single-CTA limit
+  return launch_nsga_survive(X, F, C, FC, pop, D, d, X_next, F_next, Xc_next, Xe_next, nullptr, 0, (cudaStream_t)stream);
+}
+
+int64_t hb_nsga2_workspace_bytes(int64_t pop, int64_t D) { return nsga_survive_ws_query(pop, D); }
+
+int32_t hb_nsga2_survive_ex(const float *X, const float *F, const float *C, const float *FC, int64_t pop, int64_t D,
+                            int64_t d, float *X_next, float *F_next, float *Xc_next, int32_t *Xe_next, void *ws,
+                            int64_t ws_bytes, void *stream) {
+  if (!X || !F || !C || !FC || !X_next || !F_next || (d > 0 && !Xc_next) || (D > d && !Xe_next)) return HB_ERR_INVALID;
+  return launch_nsga_survive(X, F, C, FC, pop, D, d, X_next, F_next, Xc_next, Xe_next, ws, ws_bytes, (cudaStream_t)stream);
 }
 
 }  // extern "C"

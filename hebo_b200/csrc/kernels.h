@@ -149,7 +149,10 @@ int launch_nsga_init(float *X, int64_t P, int64_t D, int64_t d, const int32_t *k
                      const float *fixed, const float *init, int64_t n_init, uint64_t seed, float *Xc, int32_t *Xe, cudaStream_t st);
 int launch_nsga_mate(const float *X, int64_t P, int64_t D, int64_t d, const int32_t *kind, const float *lb, const float *ub,
                      const float *fixed, uint64_t seed, int gen, float *C, float *Cc, int32_t *Ce, cudaStream_t st);
+// survival of the 2P merged rows: one CTA for 2P <= 512 (ws may be NULL), the cooperative multi-CTA kernel up to
+// P = 16384 (ws_bytes >= nsga_survive_ws_query(P, D))
+int64_t nsga_survive_ws_query(int64_t P, int64_t D);
 int launch_nsga_survive(const float *X, const float *F, const float *C, const float *FC, int64_t P, int64_t D, int64_t d,
-                        float *Xn, float *Fn, float *Xcn, int32_t *Xen, cudaStream_t st);
+                        float *Xn, float *Fn, float *Xcn, int32_t *Xen, void *ws, int64_t ws_bytes, cudaStream_t st);
 
 }  // namespace hb

@@ -9,6 +9,10 @@
 //
 // Layout: X [P, D] fp32 in the optimisation space (numeric columns first, then the categorical indices as floats);
 // kind[D]: 0 real, 1 integer, 2 choice; lb / ub [D]; fixed[D] (NaN = free, else the value of a `fix_input` column).
+#include <cooperative_groups.h>
+
+#include <algorithm>
+
 #include "kernels.h"
 
 namespace hb {
@@ -127,7 +131,47 @@ __global__ void nsga_mate_kernel(const float *__restrict__ X, int P, int D, int 
   if (second) split_row(c2, d, D - d, Cc + (int64_t)(2 * t + 1) * d, Ce + (int64_t)(2 * t + 1) * (D - d));
 }
 
-// ---- rank-and-crowding survival of the merged population (pop rows 0..P-1, offspring rows P..2P-1), one CTA.
+// ---- rank-and-crowding survival of the merged population (pop rows 0..P-1, offspring rows P..2P-1).
+// Both survival kernels below (one CTA for 2P <= 512, the cooperative multi-CTA one for 512 < 2P <= 32768) give the
+// same result, bit for bit:
+//  * sanitising: every objective component that is not finite becomes +inf, one component at a time;
+//  * duplicates (pymoo MixedVariableDuplicateElimination): child i is a duplicate when |o[k] - me[k]| <= 1e-16f for every
+//    k against ANY earlier merged row j < i (population rows first, then earlier children, duplicates included); its three
+//    objectives become +inf;
+//  * ranks: fast non-dominated sort (j dominates i: all <=, one <), fronts peeled until the cumulative count reaches P;
+//    whole fronts below the cut front survive;
+//  * cut front: fp32 crowding distance, objective k = 0, 1, 2 in that order: members ordered by f_k with ties by merged
+//    index, the two end positions become +inf, an interior member adds (f[next] - f[prev]) / (fmax - fmin) when
+//    fmax > fmin and fmax - fmin is finite; the `need` members with the largest crowding survive, ties by lower index;
+//  * output: survivors in ascending merged-row order, F_next holds the sanitised (duplicate -> +inf) objectives.
+__device__ __forceinline__ float sanitize_obj(float v) { return isfinite(v) ? v : INFINITY; }
+
+// a dominates b (minimisation): all <=, at least one <
+__device__ __forceinline__ bool dominates3(float a0, float a1, float a2, float b0, float b1, float b2) {
+  const bool le = a0 <= b0 && a1 <= b1 && a2 <= b2;
+  const bool lt = a0 < b0 || a1 < b1 || a2 < b2;
+  return le && lt;
+}
+
+__device__ __forceinline__ bool same_row(const float *o, const float *me, int D) {
+  bool same = true;
+  for (int k = 0; k < D && same; ++k) same = fabsf(o[k] - me[k]) <= 1e-16f;
+  return same;
+}
+
+// (fj, j) before (fi, i) in ascending f order, ties by index; in descending crowding order, ties by index
+__device__ __forceinline__ bool before_asc(float fj, int j, float fi, int i) { return fj < fi || (fj == fi && j < i); }
+__device__ __forceinline__ bool before_desc(float cj, int j, float ci, int i) { return cj > ci || (cj == ci && j < i); }
+
+// the crowding term of an interior member of the cut front along one objective
+__device__ __forceinline__ float crowd_interior(float acc, float fprev, float fnext, float fmin, float fmax) {
+  return (fmax > fmin && isfinite(fmax - fmin)) ? acc + (fnext - fprev) / (fmax - fmin) : acc;
+}
+
+__device__ __forceinline__ const float *merged_row(const float *X, const float *C, int P, int D, int j) {
+  return j < P ? X + (int64_t)j * D : C + (int64_t)(j - P) * D;
+}
+
 constexpr int NSGA_MAX = 512;
 __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__restrict__ X, const float *__restrict__ F,
                                                                 const float *__restrict__ C, const float *__restrict__ FC,
@@ -143,36 +187,23 @@ __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__r
   const bool on = i < N;
   if (on) {
     const float *src = i < P ? F + (int64_t)i * 3 : FC + (int64_t)(i - P) * 3;
-    for (int k = 0; k < 3; ++k) {
-      const float v = src[k];
-      f[i][k] = isfinite(v) ? v : INFINITY;                // NaN / inf objectives never survive (evolution_optimizer.py:104 F)
-    }
+    for (int k = 0; k < 3; ++k) f[i][k] = sanitize_obj(src[k]);   // NaN / inf objectives never survive (evolution_optimizer.py:104 F)
     rank[i] = -1;
     keep[i] = 0;
     infront[i] = 0;
   }
   __syncthreads();
   if (on && i >= P) {
-    // duplicate elimination (pymoo MixedVariableDuplicateElimination): a child equal to a population member or to an
-    // earlier child is discarded
+    // duplicate elimination: a child equal to a population member or to an earlier child is discarded
     const float *me = C + (int64_t)(i - P) * D;
     bool dup = false;
-    for (int j = 0; j < i && !dup; ++j) {
-      const float *o = j < P ? X + (int64_t)j * D : C + (int64_t)(j - P) * D;
-      bool same = true;
-      for (int k = 0; k < D && same; ++k) same = fabsf(o[k] - me[k]) <= 1e-16f;
-      dup = same;
-    }
+    for (int j = 0; j < i && !dup; ++j) dup = same_row(merged_row(X, C, P, D, j), me, D);
     if (dup) f[i][0] = f[i][1] = f[i][2] = INFINITY;
   }
   __syncthreads();
   if (on) {
     int c = 0;
-    for (int j = 0; j < N; ++j) {
-      const bool le = f[j][0] <= f[i][0] && f[j][1] <= f[i][1] && f[j][2] <= f[i][2];
-      const bool lt = f[j][0] < f[i][0] || f[j][1] < f[i][1] || f[j][2] < f[i][2];
-      c += (le && lt) ? 1 : 0;
-    }
+    for (int j = 0; j < N; ++j) c += dominates3(f[j][0], f[j][1], f[j][2], f[i][0], f[i][1], f[i][2]) ? 1 : 0;
     ndom[i] = c;
   }
   if (i == 0) { cum = 0; r_cut = -1; need = 0; }
@@ -198,11 +229,7 @@ __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__r
     if (on && rank[i] < 0) {
       int sub = 0;
       for (int j = 0; j < N; ++j)
-        if (infront[j]) {
-          const bool le = f[j][0] <= f[i][0] && f[j][1] <= f[i][1] && f[j][2] <= f[i][2];
-          const bool lt = f[j][0] < f[i][0] || f[j][1] < f[i][1] || f[j][2] < f[i][2];
-          sub += (le && lt) ? 1 : 0;
-        }
+        if (infront[j]) sub += dominates3(f[j][0], f[j][1], f[j][2], f[i][0], f[i][1], f[i][2]) ? 1 : 0;
       ndom[i] -= sub;
     }
     __syncthreads();
@@ -225,7 +252,7 @@ __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__r
       for (int j = 0; j < N; ++j)
         if (rank[j] == rc) {
           ++m;
-          pos += (f[j][k] < f[i][k] || (f[j][k] == f[i][k] && j < i)) ? 1 : 0;
+          pos += before_asc(f[j][k], j, f[i][k], i) ? 1 : 0;
           fmin = fminf(fmin, f[j][k]);
           fmax = fmaxf(fmax, f[j][k]);
         }
@@ -234,14 +261,14 @@ __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__r
     __syncthreads();
     if (mine) {
       if (pos == 0 || pos == m - 1) crowd[i] = INFINITY;
-      else if (fmax > fmin && isfinite(fmax - fmin)) crowd[i] += (f[order[pos + 1]][k] - f[order[pos - 1]][k]) / (fmax - fmin);
+      else crowd[i] = crowd_interior(crowd[i], f[order[pos - 1]][k], f[order[pos + 1]][k], fmin, fmax);
     }
     __syncthreads();
   }
   if (mine) {
     int better = 0;
     for (int j = 0; j < N; ++j)
-      if (rank[j] == rc) better += (crowd[j] > crowd[i] || (crowd[j] == crowd[i] && j < i)) ? 1 : 0;
+      if (rank[j] == rc) better += before_desc(crowd[j], j, crowd[i], i) ? 1 : 0;
     if (better < need) keep[i] = 1;
   }
   __syncthreads();
@@ -249,7 +276,7 @@ __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__r
   if (on && keep[i]) {
     int dst = 0;
     for (int j = 0; j < i; ++j) dst += keep[j];
-    const float *src = i < P ? X + (int64_t)i * D : C + (int64_t)(i - P) * D;
+    const float *src = merged_row(X, C, P, D, i);
     float *row = Xn + (int64_t)dst * D;
     for (int k = 0; k < D; ++k) row[k] = src[k];
     for (int k = 0; k < 3; ++k) Fn[(int64_t)dst * 3 + k] = f[i][k];
@@ -257,6 +284,328 @@ __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__r
   }
 }
 
+// ---- multi-CTA survival for 512 < 2P <= 32768 merged rows: one persistent cooperative kernel (grid sized by occupancy,
+// every phase separated by a grid barrier), so a call is one launch and never reads anything back to the host whatever
+// the number of fronts.  Same rules and results as nsga_survive_kernel (see above); how it gets there:
+//  * duplicates: rows are hashed into a bucket table.  The key of a coordinate is 0 for |v| < 2^-20 and its bit pattern
+//    otherwise; the fp32 spacing above 2^-20 exceeds 1e-16, so two rows the predicate calls equal always share a bucket.
+//    A child then tests the exact predicate against the lower merged indices of its bucket only.  Bucket chains are
+//    built with atomicExch, so their order varies from run to run; the answer (does an equal earlier row exist) does not;
+//  * ranks: the N^2 dominance counts are tiled through shared memory, one 8-lane team per row.  Fronts are appended to
+//    one list in peeling order (front r at [start_r, start_r + cnt_r)); a round subtracts front r's dominance from every
+//    unranked row and appends the rows whose count reaches zero to front r + 1.  One grid barrier per front: the cost
+//    grows linearly with the number of fronts peeled (P of them when the objectives are totally ordered);
+//  * cut front: each member's position along f_k (counting, ties by index) gives the sorted order, the members then add
+//    their crowding terms for k = 0, 1, 2 in that order, and a second count against the cut front ranks the crowding;
+//  * output: a per-CTA count + exclusive scan maps survivors to ascending rows, then a coalesced copy.
+// Only integer atomics are used and every float is computed by one thread in a fixed order: outputs are bit-identical
+// from run to run.
+constexpr int NSGA_LARGE_MAX_POP = 16384;
+constexpr int NSGA_LT = 512;                       // threads per CTA
+constexpr int NSGA_TEAM = 8;                       // lanes per row in the tiled sweeps
+constexpr int NSGA_ROWS = NSGA_LT / NSGA_TEAM;     // rows per CTA pass
+constexpr int NSGA_TJ = 1024;                      // shared-memory tile of the swept set
+constexpr int NSGA_GRID_MAX = 1024;
+
+struct SweepEntry {
+  float v[3];
+  int id;
+};
+
+struct SurviveWs {
+  float *f;       // [3][N] sanitised objectives (duplicates -> +inf)
+  int *ndom;      // [N] dominator count; phase 1 parks the bucket index here
+  int *rank;      // [N] front index, -1 = not yet ranked
+  int *list;      // [N] the fronts in peeling order
+  int *cnt;       // [N + 2] size of front r
+  int *head;      // [H] bucket -> last inserted merged row
+  int *next;      // [N] bucket chains
+  int *pos;       // [3][N] position of cut-front member a along f_k
+  int *order;     // [3][N] cut-front members sorted along f_k
+  float *crowd;   // [N] crowding of cut-front member a
+  int *keep;      // [N]
+  int *sel;       // [P] survivor r -> merged row
+  int *bsum;      // [NSGA_GRID_MAX] survivors per CTA
+  int H;          // bucket count (power of two)
+};
+
+static int64_t nsga_buckets(int64_t P) {
+  int64_t H = 1;
+  while (H < 4 * P) H <<= 1;
+  return H;
+}
+
+size_t nsga_survive_ws_bytes(int64_t P) {
+  const int64_t N = 2 * P;
+  const int64_t words[] = {3 * N, N, N, N, N + 2, nsga_buckets(P), N, 3 * N, 3 * N, N, N, P, NSGA_GRID_MAX};
+  size_t total = 0;
+  for (int64_t w : words) total += (size_t)round_up(w * 4, 256);
+  return total;
+}
+
+static SurviveWs nsga_carve(void *ws, int64_t P) {
+  const int64_t N = 2 * P, H = nsga_buckets(P);
+  char *p = (char *)ws;
+  auto take = [&](int64_t words) {
+    char *q = p;
+    p += round_up(words * 4, 256);
+    return q;
+  };
+  SurviveWs w;
+  w.f = (float *)take(3 * N);
+  w.ndom = (int *)take(N);
+  w.rank = (int *)take(N);
+  w.list = (int *)take(N);
+  w.cnt = (int *)take(N + 2);
+  w.head = (int *)take(H);
+  w.next = (int *)take(N);
+  w.pos = (int *)take(3 * N);
+  w.order = (int *)take(3 * N);
+  w.crowd = (float *)take(N);
+  w.keep = (int *)take(N);
+  w.sel = (int *)take(P);
+  w.bsum = (int *)take(NSGA_GRID_MAX);
+  w.H = (int)H;
+  return w;
+}
+
+__device__ __forceinline__ uint32_t row_bucket(const float *row, int D, int H) {
+  uint32_t h = 0x811C9DC5u;
+  for (int k = 0; k < D; ++k) {
+    const float v = row[k];
+    const uint32_t key = fabsf(v) < 0x1p-20f ? 0u : __float_as_uint(v);   // -0, +0 and everything within 2^-20 of 0 agree
+    h = (h ^ key) * 0x01000193u;
+    h ^= h >> 15;
+  }
+  h ^= h >> 16;
+  h *= 0x85EBCA6Bu;
+  h ^= h >> 13;
+  h *= 0xC2B2AE35u;
+  h ^= h >> 16;
+  return h & (uint32_t)(H - 1);
+}
+
+// Tiled count: for every row r < nr (one 8-lane team each), acc[0..2] = sums of test(me, entry) over the nc entries of
+// the swept set, staged NSGA_TJ at a time in shared memory; out(r, me, acc) runs on the team's lane 0.  Every thread of
+// the CTA must call it (it holds __syncthreads and warp shuffles).
+template <class Row, class Col, class Test, class Out>
+__device__ __forceinline__ void team_sweep(SweepEntry *tile, int nr, int nc, Row row, Col col, Test test, Out out) {
+  const int team = threadIdx.x / NSGA_TEAM, lane = threadIdx.x % NSGA_TEAM;
+  for (int base = blockIdx.x * NSGA_ROWS; base < nr; base += gridDim.x * NSGA_ROWS) {
+    const int r = base + team;
+    SweepEntry me;
+    const bool act = r < nr && row(r, me);
+    int acc[3] = {0, 0, 0};
+    for (int c0 = 0; c0 < nc; c0 += NSGA_TJ) {
+      const int ce = min(NSGA_TJ, nc - c0);
+      __syncthreads();
+      for (int t = threadIdx.x; t < ce; t += blockDim.x) tile[t] = col(c0 + t);
+      __syncthreads();
+      if (act)
+        for (int t = lane; t < ce; t += NSGA_TEAM) test(me, tile[t], acc);
+    }
+#pragma unroll
+    for (int o = NSGA_TEAM / 2; o > 0; o >>= 1)
+#pragma unroll
+      for (int k = 0; k < 3; ++k) acc[k] += __shfl_xor_sync(0xFFFFFFFFu, acc[k], o);
+    if (act && lane == 0) out(r, me, acc);
+  }
+}
+
+__global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const float *__restrict__ X, const float *__restrict__ F,
+                                                                        const float *__restrict__ C, const float *__restrict__ FC,
+                                                                        int P, int D, int d, float *__restrict__ Xn,
+                                                                        float *__restrict__ Fn, float *__restrict__ Xcn,
+                                                                        int32_t *__restrict__ Xen, const SurviveWs w_arg) {
+  namespace cg = cooperative_groups;
+  SurviveWs w = w_arg;
+  cg::grid_group grid = cg::this_grid();
+  __shared__ SweepEntry tile[NSGA_TJ];
+  __shared__ int s_warp[NSGA_LT / 32], s_base;
+  const int N = 2 * P;
+  const int gtid = blockIdx.x * blockDim.x + threadIdx.x, gsz = gridDim.x * blockDim.x;
+  float *f0 = w.f, *f1 = w.f + N, *f2 = w.f + 2 * N;
+  auto obj = [&](int j) {   // written in this kernel: read through L2 after a grid barrier
+    SweepEntry e;
+    e.v[0] = __ldcg(f0 + j);
+    e.v[1] = __ldcg(f1 + j);
+    e.v[2] = __ldcg(f2 + j);
+    e.id = j;
+    return e;
+  };
+
+  // ---- 0: sanitise, clear the bucket table and the front sizes
+  for (int i = gtid; i < N; i += gsz) {
+    const float *src = i < P ? F + (int64_t)i * 3 : FC + (int64_t)(i - P) * 3;
+    f0[i] = sanitize_obj(src[0]);
+    f1[i] = sanitize_obj(src[1]);
+    f2[i] = sanitize_obj(src[2]);
+  }
+  for (int h = gtid; h < w.H; h += gsz) w.head[h] = -1;
+  for (int r = gtid; r < N + 2; r += gsz) w.cnt[r] = 0;
+  grid.sync();
+  // ---- 1: bucket every merged row
+  for (int i = gtid; i < N; i += gsz) {
+    const int b = (int)row_bucket(merged_row(X, C, P, D, i), D, w.H);
+    w.ndom[i] = b;
+    w.next[i] = atomicExch(&w.head[b], i);
+  }
+  grid.sync();
+  // ---- 2: duplicate children
+  for (int i = P + gtid; i < N; i += gsz) {
+    const float *me = C + (int64_t)(i - P) * D;
+    bool dup = false;
+    for (int j = __ldcg(&w.head[__ldcg(&w.ndom[i])]); j >= 0 && !dup; j = __ldcg(&w.next[j]))
+      dup = j < i && same_row(merged_row(X, C, P, D, j), me, D);
+    if (dup) f0[i] = f1[i] = f2[i] = INFINITY;
+  }
+  grid.sync();
+  // ---- 3: dominator counts; front 0
+  team_sweep(
+      tile, N, N, [&](int r, SweepEntry &me) { me = obj(r); return true; }, obj,
+      [](const SweepEntry &me, const SweepEntry &o, int *acc) {
+        acc[0] += dominates3(o.v[0], o.v[1], o.v[2], me.v[0], me.v[1], me.v[2]) ? 1 : 0;
+      },
+      [&](int r, const SweepEntry &, const int *acc) {
+        w.ndom[r] = acc[0];
+        w.rank[r] = acc[0] == 0 ? 0 : -1;
+        if (acc[0] == 0) w.list[atomicAdd(&w.cnt[0], 1)] = r;
+      });
+  grid.sync();
+  // ---- 4: peel fronts until P rows are covered (every CTA reads the same counts, so all leave at the same round)
+  int start = 0, rc = -1, need = 0;
+  for (int r = 0; r < N; ++r) {
+    const int c = __ldcg(&w.cnt[r]);
+    if (c == 0) break;
+    if (start + c >= P) { rc = r; need = P - start; break; }
+    const int nxt = start + c;
+    team_sweep(
+        tile, N, c,
+        [&](int i, SweepEntry &me) {
+          if (__ldcg(&w.rank[i]) >= 0) return false;
+          me = obj(i);
+          return true;
+        },
+        [&](int t) { return obj(__ldcg(&w.list[start + t])); },
+        [](const SweepEntry &me, const SweepEntry &o, int *acc) {
+          acc[0] += dominates3(o.v[0], o.v[1], o.v[2], me.v[0], me.v[1], me.v[2]) ? 1 : 0;
+        },
+        [&](int i, const SweepEntry &, const int *acc) {
+          if (acc[0] == 0) return;
+          const int nd = __ldcg(&w.ndom[i]) - acc[0];
+          w.ndom[i] = nd;
+          if (nd == 0) {
+            w.rank[i] = r + 1;
+            w.list[nxt + atomicAdd(&w.cnt[r + 1], 1)] = i;
+          }
+        });
+    start = nxt;
+    grid.sync();
+  }
+  const int m = rc >= 0 ? __ldcg(&w.cnt[rc]) : 0;
+  const int *front = w.list + start;
+  // ---- 5: cut front: positions along f_0, f_1, f_2; whole fronts below the cut survive
+  for (int i = gtid; i < N; i += gsz) {
+    const int rk = __ldcg(&w.rank[i]);
+    w.keep[i] = (rc >= 0 && rk >= 0 && rk < rc) ? 1 : 0;
+  }
+  team_sweep(
+      tile, m, m, [&](int a, SweepEntry &me) { me = obj(__ldcg(front + a)); return true; },
+      [&](int t) { return obj(__ldcg(front + t)); },
+      [](const SweepEntry &me, const SweepEntry &o, int *acc) {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) acc[k] += before_asc(o.v[k], o.id, me.v[k], me.id) ? 1 : 0;
+      },
+      [&](int a, const SweepEntry &me, const int *acc) {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+          w.pos[k * N + a] = acc[k];
+          w.order[k * N + acc[k]] = me.id;
+        }
+      });
+  grid.sync();
+  // ---- 6: crowding, k = 0, 1, 2 in order, by the member itself
+  for (int a = gtid; a < m; a += gsz) {
+    float cr = 0.0f;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const float *fk = w.f + k * N;
+      const int *ok = w.order + k * N;
+      const int p = __ldcg(w.pos + k * N + a);
+      if (p == 0 || p == m - 1) cr = INFINITY;
+      else cr = crowd_interior(cr, __ldcg(fk + __ldcg(ok + p - 1)), __ldcg(fk + __ldcg(ok + p + 1)), __ldcg(fk + __ldcg(ok)),
+                               __ldcg(fk + __ldcg(ok + m - 1)));
+    }
+    w.crowd[a] = cr;
+  }
+  grid.sync();
+  // ---- 7: the `need` members with the largest crowding survive
+  auto crowd_entry = [&](int a) {
+    SweepEntry e;
+    e.v[0] = __ldcg(w.crowd + a);
+    e.v[1] = e.v[2] = 0.0f;
+    e.id = __ldcg(front + a);
+    return e;
+  };
+  team_sweep(
+      tile, m, m, [&](int a, SweepEntry &me) { me = crowd_entry(a); return true; }, crowd_entry,
+      [](const SweepEntry &me, const SweepEntry &o, int *acc) { acc[0] += before_desc(o.v[0], o.id, me.v[0], me.id) ? 1 : 0; },
+      [&](int, const SweepEntry &me, const int *acc) {
+        if (acc[0] < need) w.keep[me.id] = 1;
+      });
+  grid.sync();
+  // ---- 8: survivors -> ascending output rows (CTA b owns merged rows [b * chunk, (b + 1) * chunk))
+  const int chunk = (int)ceil_div(N, gridDim.x);
+  const int r0 = blockIdx.x * chunk, r1 = min(N, r0 + chunk);
+  int kept = 0;
+  for (int t0 = r0; t0 < r1; t0 += blockDim.x) {
+    const int i = t0 + threadIdx.x;
+    kept += __syncthreads_count(i < r1 && __ldcg(w.keep + i));
+  }
+  if (threadIdx.x == 0) w.bsum[blockIdx.x] = kept;
+  grid.sync();
+  if (threadIdx.x == 0) {
+    int b0 = 0;
+    for (int b = 0; b < (int)blockIdx.x; ++b) b0 += __ldcg(w.bsum + b);
+    s_base = b0;
+  }
+  __syncthreads();
+  int base = s_base;
+  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  for (int t0 = r0; t0 < r1; t0 += blockDim.x) {
+    const int i = t0 + threadIdx.x;
+    const bool k = i < r1 && __ldcg(w.keep + i);
+    const unsigned bal = __ballot_sync(0xFFFFFFFFu, k);
+    if (lane == 0) s_warp[warp] = __popc(bal);
+    __syncthreads();
+    int off = base;
+    for (int q = 0; q < warp; ++q) off += s_warp[q];
+    if (k) w.sel[off + __popc(bal & ((1u << lane) - 1u))] = i;
+    for (int q = 0; q < NSGA_LT / 32; ++q) base += s_warp[q];
+    __syncthreads();
+  }
+  grid.sync();
+  int total = 0;
+  for (int b = 0; b < (int)gridDim.x; ++b) total += __ldcg(w.bsum + b);
+  // ---- 9: coalesced copy of the survivors
+  const int e = D - d;
+  for (int64_t q = gtid; q < (int64_t)total * D; q += gsz) {
+    const int r = (int)(q / D), k = (int)(q % D);
+    Xn[q] = merged_row(X, C, P, D, __ldcg(w.sel + r))[k];
+  }
+  for (int64_t q = gtid; q < (int64_t)total * 3; q += gsz) {
+    const int r = (int)(q / 3), k = (int)(q % 3);
+    Fn[q] = __ldcg(w.f + k * N + __ldcg(w.sel + r));
+  }
+  for (int64_t q = gtid; q < (int64_t)total * d; q += gsz) {
+    const int r = (int)(q / d), k = (int)(q % d);
+    Xcn[q] = merged_row(X, C, P, D, __ldcg(w.sel + r))[k];
+  }
+  for (int64_t q = gtid; q < (int64_t)total * e; q += gsz) {
+    const int r = (int)(q / e), k = (int)(q % e);
+    Xen[q] = (int32_t)rintf(merged_row(X, C, P, D, __ldcg(w.sel + r))[d + k]);
+  }
+}
 int launch_nsga_init(float *X, int64_t P, int64_t D, int64_t d, const int32_t *kind, const float *lb, const float *ub,
                      const float *fixed, const float *init, int64_t n_init, uint64_t seed, float *Xc, int32_t *Xe, cudaStream_t st) {
   if (P <= 0 || D <= 0 || d < 0 || d > D || n_init < 0 || n_init > P) return HB_ERR_INVALID;
@@ -276,12 +625,45 @@ int launch_nsga_mate(const float *X, int64_t P, int64_t D, int64_t d, const int3
   return HB_OK;
 }
 
+int64_t nsga_survive_ws_query(int64_t P, int64_t D) {
+  if (P < 1 || P > NSGA_LARGE_MAX_POP || D < 1) return -1;
+  return (int64_t)nsga_survive_ws_bytes(P);
+}
+
 int launch_nsga_survive(const float *X, const float *F, const float *C, const float *FC, int64_t P, int64_t D, int64_t d,
-                        float *Xn, float *Fn, float *Xcn, int32_t *Xen, cudaStream_t st) {
-  if (P <= 0 || 2 * P > NSGA_MAX || D <= 0 || d < 0 || d > D) return HB_ERR_INVALID;
-  nsga_survive_kernel<<<1, NSGA_MAX, 0, st>>>(X, F, C, FC, (int)P, (int)D, (int)d, Xn, Fn, Xcn, Xen);
+                        float *Xn, float *Fn, float *Xcn, int32_t *Xen, void *ws, int64_t ws_bytes, cudaStream_t st) {
+  if (P <= 0 || P > NSGA_LARGE_MAX_POP || D <= 0 || d < 0 || d > D) return HB_ERR_INVALID;
+  if (2 * P <= NSGA_MAX) {
+    nsga_survive_kernel<<<1, NSGA_MAX, 0, st>>>(X, F, C, FC, (int)P, (int)D, (int)d, Xn, Fn, Xcn, Xen);
+    count_launches(1);
+    HB_LAUNCH_CHECK("nsga_survive");
+    return HB_OK;
+  }
+  if (!ws || ws_bytes < (int64_t)nsga_survive_ws_bytes(P)) return HB_ERR_INVALID;
+  static PerDevice once;   // aux[dev] = co-resident CTAs of the cooperative survival kernel on that device
+  bool fresh = false;
+  const int dev = once.slot(&fresh);
+  if (dev < 0) return HB_ERR_CUDA;
+  if (fresh) {
+    int sms = 0, per_sm = 0, coop = 0;
+    HB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    HB_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
+    HB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nsga_survive_large_kernel, NSGA_LT, 0));
+    if (!coop || per_sm < 1) {
+      set_error(cudaErrorNotSupported, "nsga_survive: cooperative launch unavailable");
+      return HB_ERR_CUDA;
+    }
+    once.aux[dev] = sms * min(per_sm, 2);
+    once.done[dev] = true;
+  }
+  // no more CTAs than row passes of the N-row sweeps, and no more than the per-CTA survivor counts the workspace holds
+  const int grid = (int)std::min<int64_t>({(int64_t)once.aux[dev], ceil_div(2 * P, NSGA_ROWS), (int64_t)NSGA_GRID_MAX});
+  SurviveWs w = nsga_carve(ws, P);
+  int Pi = (int)P, Di = (int)D, di = (int)d;
+  void *args[] = {&X, &F, &C, &FC, &Pi, &Di, &di, &Xn, &Fn, &Xcn, &Xen, &w};
+  HB_CUDA(cudaLaunchCooperativeKernel((const void *)nsga_survive_large_kernel, dim3(grid), dim3(NSGA_LT), args, 0, st));
   count_launches(1);
-  HB_LAUNCH_CHECK("nsga_survive");
+  HB_LAUNCH_CHECK("nsga_survive_large");
   return HB_OK;
 }
 

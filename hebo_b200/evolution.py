@@ -189,16 +189,19 @@ class DeviceNSGA2:
 
     kinds [D]: 'real' | 'int' | 'choice' per optimisation column (numeric columns first, then the categorical ones:
     evolution_optimizer.py:26-41); lb / ub [D]; fixed: {column index: value} (fix_input, :97-101).  `score(Xc, Xe, gen)`
-    returns the objectives F [pop, 3] of a batch as a device tensor (the fused posterior + MACE call)."""
+    returns the objectives F [pop, 3] of a batch as a device tensor (the fused posterior + MACE call).  2 <= pop <= 16384:
+    survival runs in one CTA up to pop 256 and in a cooperative multi-CTA kernel above, with the same results."""
 
     KIND = {"real": 0, "int": 1, "choice": 2}
+    MAX_POP = 16384                                 # hb_nsga2_survive_ex: single CTA up to 256, cooperative multi-CTA above
 
     def __init__(self, kinds, lb, ub, num_numeric: int, score: Callable, pop: int = 100, iters: int = 100,
                  seed: Optional[int] = None, fixed: Optional[dict] = None, device="cuda"):
         import torch
         self.torch = torch
         self.D, self.d, self.pop, self.iters = len(kinds), int(num_numeric), int(pop), int(iters)
-        assert 2 * self.pop <= 512 and self.pop >= 2
+        if not 2 <= self.pop <= self.MAX_POP:
+            raise ValueError(f"DeviceNSGA2: pop must lie in [2, {self.MAX_POP}], got {self.pop}")
         dev = torch.device(device)
         self.dev = dev
         self.kind = torch.tensor([self.KIND[k] for k in kinds], dtype=torch.int32, device=dev)
@@ -230,6 +233,10 @@ class DeviceNSGA2:
         init = None if initial_suggest is None else t.as_tensor(np.asarray(initial_suggest, dtype=np.float32).reshape(-1, D)).to(self.dev)
         n_init = 0 if init is None else min(init.shape[0], P)
         pc = lambda x: _lib.ptr(x) if x.numel() else None
+        ws_bytes = int(lib.hb_nsga2_workspace_bytes(P, D))
+        if ws_bytes < 0:
+            raise _lib.HeboB200Error(f"hb_nsga2_workspace_bytes: invalid size (pop {P}, D {D})")
+        ws = t.empty(ws_bytes, dtype=t.uint8, device=self.dev)       # survival workspace, reused by every generation
         with t.cuda.device(self.dev):
             _lib.check(lib.hb_nsga2_init(_lib.ptr(X), P, D, d, _lib.ptr(self.kind), _lib.ptr(self.lb), _lib.ptr(self.ub), _lib.ptr(self.fixed),
                                          _lib.ptr(init), n_init, self.seed, pc(Xc), pc(Xe), st()), "hb_nsga2_init")
@@ -240,8 +247,8 @@ class DeviceNSGA2:
                 _lib.check(lib.hb_nsga2_mate(_lib.ptr(X), P, D, d, _lib.ptr(self.kind), _lib.ptr(self.lb), _lib.ptr(self.ub),
                                              _lib.ptr(self.fixed), self.seed, gen, _lib.ptr(C), pc(Cc), pc(Ce), st()), "hb_nsga2_mate")
                 FC = self.score(Cc, Ce, gen).contiguous()
-                _lib.check(lib.hb_nsga2_survive(_lib.ptr(X), _lib.ptr(F), _lib.ptr(C), _lib.ptr(FC), P, D, d, _lib.ptr(Xn), _lib.ptr(Fn),
-                                                pc(Xcn), pc(Xen), st()), "hb_nsga2_survive")
+                _lib.check(lib.hb_nsga2_survive_ex(_lib.ptr(X), _lib.ptr(F), _lib.ptr(C), _lib.ptr(FC), P, D, d, _lib.ptr(Xn), _lib.ptr(Fn),
+                                                   pc(Xcn), pc(Xen), _lib.ptr(ws), ws_bytes, st()), "hb_nsga2_survive_ex")
                 X, Xn, Xc, Xcn, Xe, Xen, F, Fn = Xn, X, Xcn, Xc, Xen, Xe, Fn, F
                 self.n_evals += P
         self.pop_X, self.pop_F = X, F

@@ -279,14 +279,23 @@ int32_t hb_pareto_front3(const float *F, int64_t m, int32_t *idx_out, int32_t *c
  * (d numeric columns, then D - d categorical indices), kind [D] (0 Real, 1 Integer, 2 Choice), lb / ub [D],
  * fixed [D] (NaN = free; otherwise the value of a fix_input column, :97-101).  Every call also emits the rows split into
  * the model's inputs Xc [pop, d] fp32 / Xe [pop, D - d] int32.  One generation = hb_nsga2_mate -> hb_posterior_mace_ex on
- * the offspring -> hb_nsga2_survive (rank + crowding of the 2 pop merged rows, duplicates and non-finite objectives never
- * survive; pop <= 256); nothing synchronises with the host.  Philox streams keyed by (seed, generation). */
+ * the offspring -> hb_nsga2_survive_ex (rank + crowding of the 2 pop merged rows, duplicates and non-finite objectives
+ * never survive); nothing synchronises with the host.  Philox streams keyed by (seed, generation).
+ * hb_nsga2_survive_ex: 1 <= pop <= 16384, one launch per call.  pop <= 256 runs the single-CTA kernel (ws may be NULL);
+ *   larger populations run a cooperative multi-CTA kernel and need ws_bytes >= hb_nsga2_workspace_bytes(pop, D).
+ *   Both give the same survivors, bit for bit, and are deterministic.
+ * hb_nsga2_workspace_bytes: host only; < 0 if pop < 1, pop > 16384 or D < 1.
+ * hb_nsga2_survive: the workspace-free entry, pop <= 256. */
 int32_t hb_nsga2_init(float *X, int64_t pop, int64_t D, int64_t d, const int32_t *kind, const float *lb, const float *ub,
                       const float *fixed, const float *init, int64_t n_init, uint64_t seed, float *Xc, int32_t *Xe, void *stream);
 int32_t hb_nsga2_mate(const float *X, int64_t pop, int64_t D, int64_t d, const int32_t *kind, const float *lb, const float *ub,
                       const float *fixed, uint64_t seed, int32_t generation, float *C, float *Cc, int32_t *Ce, void *stream);
 int32_t hb_nsga2_survive(const float *X, const float *F, const float *C, const float *FC, int64_t pop, int64_t D, int64_t d,
                          float *X_next, float *F_next, float *Xc_next, int32_t *Xe_next, void *stream);
+int64_t hb_nsga2_workspace_bytes(int64_t pop, int64_t D);
+int32_t hb_nsga2_survive_ex(const float *X, const float *F, const float *C, const float *FC, int64_t pop, int64_t D,
+                            int64_t d, float *X_next, float *F_next, float *Xc_next, int32_t *Xe_next,
+                            void *ws, int64_t ws_bytes, void *stream);
 
 /* ---- multi-GPU front exchange  (candidate-sharded scoring, BASELINE config 5: every rank filters its shard, ONE
  * all-gather of fixed-capacity front buffers, every rank merges; no reference counterpart -- the reference is one process,
