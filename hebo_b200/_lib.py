@@ -13,6 +13,7 @@ LIB_PATH = os.path.join(HERE, "lib", "libhebo_b200.so")
 
 HB_OK, HB_ERR_INVALID, HB_ERR_NOT_PD, HB_ERR_CUDA = 0, 1, 2, 3
 KERNEL_IDS = {"matern32": 0, "matern52": 1, "rbf": 2}
+HB_MAX_FEATURES = 4096   # d + sum(emb_sizes) a model may have (include/hebo_b200.h)
 
 
 class HeboB200Error(RuntimeError):

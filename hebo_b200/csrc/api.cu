@@ -90,7 +90,7 @@ static bool build_spec(int64_t d, const hb_model_spec_t *c, ModelSpec &sp) {
       sp.T += c->num_uniqs[k] * c->emb_sizes[k];
     }
   }
-  return sp.dtot() > 0;
+  return sp.dtot() > 0 && sp.dtot() <= HB_MAX_FEATURES;
 }
 static size_t meta_ints(const ModelSpec &sp) { return (size_t)2 * sp.De + 2 * sp.e + 3 * sp.T; }
 static void bind_meta(ModelSpec &sp, const int32_t *meta, const int32_t *Xe) {

@@ -158,12 +158,22 @@ __global__ void __launch_bounds__(256, EMB ? 1 : 2) mll_grad_kernel(const float 
                                                                     float *__restrict__ part, const float *__restrict__ dZa,
                                                                     const float *__restrict__ dZb) {
   __shared__ PairSmem sm;
-  extern __shared__ float wacc[];  // [8 warps][stride]
+  __shared__ float wpart[8][DC];   // per-warp partials of the current feature chunk, summed in warp order into `part`
   int I, J;
   tri_decode((int)blockIdx.x, I, J);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int stride = d + 2 + (EMB ? 1 : 0) + (dZa ? 2 * d : 0);   // dZa != nullptr: warped model, Xt = Zt is prescaled
-  for (int f = threadIdx.x; f < 8 * stride; f += blockDim.x) wacc[f] = 0.0f;
+  float *bpart = part + (int64_t)blockIdx.x * stride;
+  // after a feature chunk: part slots [slot, slot + kc) of this block = sum over the warps, in warp order 0..7
+  auto flush = [&](int slot, int kc) {
+    __syncthreads();
+    if ((int)threadIdx.x < kc) {
+      float v = 0.0f;
+#pragma unroll
+      for (int wv = 0; wv < 8; ++wv) v += wpart[wv][threadIdx.x];
+      bpart[slot + threadIdx.x] = v;
+    }
+  };
 
   float g[8][8];
 #pragma unroll
@@ -253,8 +263,9 @@ __global__ void __launch_bounds__(256, EMB ? 1 : 2) mll_grad_kernel(const float 
           p = fmaf(g[i][j] * df, df, p);
         }
       p = warp_sum(p);
-      if (lane == 0) wacc[warp * stride + k0 + kk] += p;
+      if (lane == 0) wpart[warp][kk] = p;
     }
+    flush(k0, kc);
   }
   // warped model: d K / d a_k = -s h dz_k dz'_k with z' = d z / d a_k (same for b): two more sweeps, 16 features at a time
   // (the z rows in the lower half of the staging buffers, the derivative rows in the upper half)
@@ -292,26 +303,22 @@ __global__ void __launch_bounds__(256, EMB ? 1 : 2) mll_grad_kernel(const float 
 #pragma unroll
             for (int j = 0; j < 8; ++j) p = fmaf(g[i][j] * (a[i] - b[j]), da[i] - db[j], p);
           p = warp_sum(p);
-          if (lane == 0) wacc[warp * stride + slot0 + k0 + kk] += p;
+          if (lane == 0) wpart[warp][kk] = p;
         }
+        flush(slot0 + k0, kc);
       }
     }
   }
   sum_wk = warp_sum(sum_wk);
   tr_w = warp_sum(tr_w);
   if (EMB) sum_le = warp_sum(sum_le);
+  __syncthreads();   // the last chunk's partials have been read
   if (lane == 0) {
-    wacc[warp * stride + d] = sum_wk;
-    wacc[warp * stride + d + 1] = tr_w;
-    if (EMB) wacc[warp * stride + d + 2] = sum_le;
+    wpart[warp][0] = sum_wk;
+    wpart[warp][1] = tr_w;
+    if (EMB) wpart[warp][2] = sum_le;
   }
-  __syncthreads();
-  for (int f = threadIdx.x; f < stride; f += blockDim.x) {
-    float v = 0.0f;
-#pragma unroll
-    for (int wv = 0; wv < 8; ++wv) v += wacc[wv * stride + f];
-    part[(int64_t)blockIdx.x * stride + f] = v;
-  }
+  flush(d, EMB ? 3 : 2);
 }
 
 // ---- gradient w.r.t. the embedding rows (mixed model):  d data / d e_i = -(1/le) sum_j G2_ij (E_i - E_j),
@@ -515,11 +522,9 @@ int launch_mll_grad(const float *Xt, const float *Ets, int64_t n, int64_t np, co
   const int nt = (int)(np / PT);
   const int grid = nt * (nt + 1) / 2;
   const int d = sp.d;
-  const size_t dyn = (size_t)8 * (3 * d + 3) * sizeof(float);
-  if (dyn > 12 * 1024) return HB_ERR_INVALID;  // static 32 KB + dynamic must stay under 48 KB (d <= 381; d <= 127 with a warp)
   float *part = reinterpret_cast<float *>(ws);
   int s = with_kernel(kern, sp.e > 0, [&](auto kk, auto ee) {
-    mll_grad_kernel<decltype(kk)::value, decltype(ee)::value><<<grid, 256, dyn, st>>>(Xt, Ets, n, np, d, sp.De, hyp, Kinv, alpha,
+    mll_grad_kernel<decltype(kk)::value, decltype(ee)::value><<<grid, 256, 0, st>>>(Xt, Ets, n, np, d, sp.De, hyp, Kinv, alpha,
                                                                                        part, dZa, dZb);
   });
   if (s != HB_OK) return s;

@@ -31,6 +31,8 @@ static_assert(CHUNK_ROWS % (2 * GT) == 0, "chunk rows: a multiple of 2 GT");
 // EMB: mixed model (gp_util.py:54-57): Zt holds d numeric rows followed by De embedding rows (both already divided by
 // their lengthscales); the candidate's embedding features are gathered from tab_s (tables / le) by its categories
 // Xe_s [m, e]; k* = s k_KERN(r over the numeric rows) Matern32(r over the embedding rows).
+// The candidates' features are staged one KS_DC chunk at a time next to the matching chunk of Zt, so shared memory is
+// fixed whatever d + De is; each 128-column sub-tile recomputes them (KS_DC features x KS_ROWS candidates per chunk).
 template <int KERN, int SPLIT, bool EMB>
 __global__ void __launch_bounds__(256) kstar_kernel(const float *__restrict__ Xs, int64_t mc, int d,
                                                     const float *__restrict__ x_mul, const float *__restrict__ x_add,
@@ -41,34 +43,14 @@ __global__ void __launch_bounds__(256) kstar_kernel(const float *__restrict__ Xs
                                                     const int32_t *__restrict__ fixlist, const int32_t *__restrict__ fixcount,
                                                     const int32_t *__restrict__ Xe_s, const float *__restrict__ tab_s,
                                                     ModelSpec sp) {
-  extern __shared__ float zs[];                 // [d + De][KS_ROWS + 1] scaled candidates, transposed
+  __shared__ float zs[KS_DC][KS_ROWS + 1];      // scaled candidate features of the chunk, transposed
   __shared__ __align__(16) float zt[KS_DC][KS_COLS];
   const int t = threadIdx.x;
   const int tx = t & 31, ty = t >> 5;           // warp ty owns rows ty*4..+3, lane tx owns cols tx*4..+3
   const int64_t r0 = (int64_t)blockIdx.x * KS_ROWS;
   const int64_t nrows = fixlist ? (int64_t)*fixcount : mc;
   if (r0 >= nrows) return;   // (block-uniform; only the guard pass launches more blocks than it needs)
-  for (int f = t; f < KS_ROWS * d; f += 256) {
-    const int row = f / d, k = f - row * d;
-    float z = 0.0f;
-    if (r0 + row < nrows) {
-      const int64_t src = fixlist ? (int64_t)fixlist[r0 + row] : r0 + row;
-      z = cand_feature(sp, sp.warp, Xs[src * d + k], k, x_mul, x_add, hyp);   // input warp fused into the load stage
-    }
-    zs[k * (KS_ROWS + 1) + row] = z;
-  }
   const int De = EMB ? sp.De : 0;
-  if (EMB) {
-    for (int f = t; f < KS_ROWS * De; f += 256) {
-      const int row = f / De, q = f - row * De;
-      float z = 0.0f;
-      if (r0 + row < nrows) {
-        const int64_t src = fixlist ? (int64_t)fixlist[r0 + row] : r0 + row;
-        z = tab_s[emb_entry(sp, Xe_s, src, q)];
-      }
-      zs[(d + q) * (KS_ROWS + 1) + row] = z;
-    }
-  }
   const float s = hyp[2];
   const float sa = pow2_scale(s, 1);   // fp16 operand scale: K* <= s lands in [0, 2)
   __half *KS_h0 = reinterpret_cast<__half *>(KS_lo), *KS_h1 = KS_h0 + mc_pad * np;
@@ -94,12 +76,23 @@ __global__ void __launch_bounds__(256) kstar_kernel(const float *__restrict__ Xs
           *reinterpret_cast<float4 *>(&zt[kk][c4 * 4]) =
               __ldg(reinterpret_cast<const float4 *>(Zt + (int64_t)(k0 + kk) * np + c0 + c4 * 4));
         }
+        for (int f = t; f < KS_ROWS * KS_DC; f += 256) {
+          const int row = f / KS_DC, kk = f % KS_DC;
+          if (kk >= kc) continue;
+          float z = 0.0f;
+          if (r0 + row < nrows) {
+            const int64_t src = fixlist ? (int64_t)fixlist[r0 + row] : r0 + row;
+            z = phase ? tab_s[emb_entry(sp, Xe_s, src, k0 + kk - d)]
+                      : cand_feature(sp, sp.warp, Xs[src * d + k0 + kk], k0 + kk, x_mul, x_add, hyp);   // input warp fused here
+          }
+          zs[kk][row] = z;
+        }
         __syncthreads();
 #pragma unroll 4
         for (int kk = 0; kk < kc; ++kk) {
           const float4 b4 = *reinterpret_cast<const float4 *>(&zt[kk][tx * 4]);
           const float b[4] = {b4.x, b4.y, b4.z, b4.w};
-          const float *zr = zs + (k0 + kk) * (KS_ROWS + 1) + ty * 4;
+          const float *zr = &zs[kk][ty * 4];
           const float a[4] = {zr[0], zr[1], zr[2], zr[3]};
 #pragma unroll
           for (int i = 0; i < 4; ++i)
@@ -389,17 +382,15 @@ int launch_kstar(const float *xs, const int32_t *xe, int64_t mc, const ModelSpec
                  const float *x_add, const float *Zt, const float *alpha, const float *hyp, int64_t n, int64_t np, int kern,
                  float *KS, float *KS_h16, float *mupart, int64_t mc_pad, const int32_t *fixlist, const int32_t *fixcount,
                  cudaStream_t st) {
-  const size_t dyn = (size_t)sp.dtot() * (KS_ROWS + 1) * sizeof(float);
-  if (dyn > 30 * 1024) return HB_ERR_INVALID;   // d + De <= 232 with the static 16 KB tile
   const dim3 grid((unsigned)ceil_div(mc, KS_ROWS), (unsigned)kstar_groups(np));
   const int s = with_kernel(kern, sp.e > 0, [&](auto kk, auto ee) {
     constexpr int KERN = decltype(kk)::value;
     constexpr bool EMB = decltype(ee)::value;
     if (KS_h16)
-      kstar_kernel<KERN, 2, EMB><<<grid, 256, dyn, st>>>(xs, mc, sp.d, x_mul, x_add, Zt, alpha, hyp, n, np, KS, KS_h16, mupart,
+      kstar_kernel<KERN, 2, EMB><<<grid, 256, 0, st>>>(xs, mc, sp.d, x_mul, x_add, Zt, alpha, hyp, n, np, KS, KS_h16, mupart,
                                                          mc_pad, fixlist, fixcount, xe, tab_s, sp);
     else
-      kstar_kernel<KERN, 0, EMB><<<grid, 256, dyn, st>>>(xs, mc, sp.d, x_mul, x_add, Zt, alpha, hyp, n, np, KS, KS_h16, mupart,
+      kstar_kernel<KERN, 0, EMB><<<grid, 256, 0, st>>>(xs, mc, sp.d, x_mul, x_add, Zt, alpha, hyp, n, np, KS, KS_h16, mupart,
                                                          mc_pad, fixlist, fixcount, xe, tab_s, sp);
   });
   if (s != HB_OK) return s;

@@ -93,8 +93,10 @@ class GP(BaseModel):
             self.emb_sizes = []
         self.De = int(sum(self.emb_sizes))
         self.T = int(sum(u * e for u, e in zip(self.num_uniqs, self.emb_sizes)))
-        if self.num_cont + self.De > 232:
-            raise NotImplementedError("more than 232 feature dimensions exceed the shared-memory tiling of the kernels")
+        if self.num_cont + self.De > _lib.HB_MAX_FEATURES:
+            raise NotImplementedError(
+                f"num_cont + sum(emb_sizes) = {self.num_cont} + {self.De} = {self.num_cont + self.De} feature dimensions "
+                f"exceed the limit of {_lib.HB_MAX_FEATURES}")
         # input warp: 0 none, 1 learned exponents, 2 fixed exponents (include/hebo_b200.h hb_model_spec_t.warp)
         self.warp_mode = 2 if self.warp_a is not None else (1 if conf.get("warp", False) and self.num_cont > 0 else 0)
         if self.warp_mode == 2:

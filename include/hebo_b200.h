@@ -62,6 +62,11 @@ extern "C" {
 #define HB_KERN_MATERN52   1   /* conf['kern'] injection, models/gp/gp.py:201            */
 #define HB_KERN_RBF        2
 
+/* Largest feature count d + De (numeric dims plus the summed embedding widths of the categorical columns) a model may
+ * have.  Every entry point that takes a model description returns HB_ERR_INVALID above it (hb_num_params and the
+ * workspace queries return -1).  The kernels stream features in 32-wide chunks, so shared memory does not grow with it. */
+#define HB_MAX_FEATURES    4096
+
 /* Model description beyond the numeric ARD default (HOST struct; NULL = numeric-only, ard_kernel=True). */
 typedef struct {
   int32_t        ard_kernel;  /* conf['ard_kernel'] (models/gp/gp.py:47, gp_util.py:45): 0 = one shared numeric lengthscale */
