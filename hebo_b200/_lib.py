@@ -14,6 +14,7 @@ LIB_PATH = os.path.join(HERE, "lib", "libhebo_b200.so")
 HB_OK, HB_ERR_INVALID, HB_ERR_NOT_PD, HB_ERR_CUDA = 0, 1, 2, 3
 KERNEL_IDS = {"matern32": 0, "matern52": 1, "rbf": 2}
 HB_MAX_FEATURES = 4096   # d + sum(emb_sizes) a model may have (include/hebo_b200.h)
+HB_MAX_OUTPUTS = 32      # outputs one batched fit trains together (hb_fit_multi_ex)
 
 
 class HeboB200Error(RuntimeError):
@@ -69,6 +70,9 @@ SIGNATURES = {
     "hb_fit_state_ex": (_i32, [_vp, _i64, _i64, _sp, C.POINTER(FitState)]),
     "hb_fit_ex": (_i32, [_vp, _vp, _vp, _i64, _i64, _sp, _vp, _i32, _vp, _f32, _f32, _f32, _i32, _vp,
                          C.POINTER(C.c_float), _vp, _i64, _vp]),
+    "hb_fit_multi_workspace_bytes": (_i64, [_i64, _i64, _sp, _i64]),
+    "hb_fit_multi_ex": (_i32, [_vp, _vp, _vp, _i64, _i64, _sp, _i64, _vp, _i32, _vp, _f32, _f32, _f32, _i32, _vp,
+                               C.POINTER(C.c_float), C.POINTER(C.c_int32), _vp, _i64, _vp]),
     "hb_factorize_ex": (_i32, [_vp, _vp, _vp, _i64, _i64, _sp, _vp, _i32, _vp, _f32, C.POINTER(C.c_float), _vp, _i64, _vp]),
     "hb_mll_fwd_bwd": (_i32, [_vp, _vp, _vp, _i64, _i64, _sp, _vp, _i32, _vp, _f32, _f32, _f32, _vp, _vp, _vp, _vp, _i64, _vp]),
     "hb_posterior_mace_ex": (_i32, [_vp, _vp, _i64, _i64, _i64, _i64, _sp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32,

@@ -58,7 +58,7 @@ constexpr int FIT_BATCH = 16;   // epochs replayed per host synchronisation (CUD
 
 struct FitWs {
   float *hyp, *grad, *sq, *loss;
-  int32_t *info;          // [0] factorisation status, [1] epoch counter, [2] replay slot of the current batch
+  int32_t *info;          // [0] factorisation status, [1] epoch counter, [2] replay slot of the current batch (per output)
   double *scal;
   float *status;          // [FIT_BATCH][2]: (info, loss) of every epoch of a batch
   float *L, *Linv, *tmp, *alpha, *Zt, *cholws, *Linv_hi, *Linv_lo;
@@ -178,7 +178,7 @@ struct HostStatus {
   float loss;
   int32_t set_epoch;
   int32_t pad;
-  float batch[FIT_BATCH * 2];   // (info as float bits, loss) per replay slot
+  float batch[HB_MAX_OUTPUTS][FIT_BATCH * 2];   // per output: (info as float bits, loss) per replay slot
 };
 // one pinned status block per DEVICE (the header allows one in-flight call per process and device)
 static HostStatus *pinned_status() {
@@ -191,16 +191,30 @@ static HostStatus *pinned_status() {
   return p[dev];
 }
 
-// conditional pSGLD (sgld.py:57-70): skipped on the device when the epoch's factorisation failed.  One block.  The epoch
+// conditional pSGLD (sgld.py:57-70): skipped on the device when the epoch's factorisation failed.  One block per output
+// (Batch: raw rows P apart, Langevin draws num_epochs * P apart, the rest in the output's workspace slice).  The epoch
 // index lives on the device (info[1], advanced on success only), so the same launch -- and a CUDA graph replay of it -- works
 // for every epoch: the Langevin row is langevin[epoch] once epoch + 1 > pretrain (n_step is incremented first in the
-// reference).  (info, loss) of the attempt go to status[slot], slot = info[2]++.
+// reference).  An output whose counter has reached num_epochs is done and never stepped again (the outputs of a batch
+// advance independently).  (info, loss) of the attempt go to status[slot], slot = info[2]++.
 __global__ void __launch_bounds__(256) psgld_guarded_kernel(float *__restrict__ raw, const float *__restrict__ grad,
                                                             float *__restrict__ sq, int p, float lr, float a, float eps,
                                                             float factor, const float *__restrict__ langevin, int pretrain,
-                                                            int32_t *__restrict__ info, const float *__restrict__ loss,
-                                                            float *__restrict__ status, const float *__restrict__ hyp,
-                                                            int nhyp, int frozen_begin, int frozen_end) {
+                                                            int num_epochs, int32_t *__restrict__ info,
+                                                            const float *__restrict__ loss, float *__restrict__ status,
+                                                            const float *__restrict__ hyp, int nhyp, int frozen_begin,
+                                                            int frozen_end, int64_t wss) {
+  {
+    const int b = blockIdx.x;
+    raw += (int64_t)b * p;
+    if (langevin) langevin += (int64_t)b * num_epochs * p;
+    grad = slice(grad, wss, b);
+    sq = slice(sq, wss, b);
+    info = slice(info, wss, b);
+    loss = slice(loss, wss, b);
+    status = slice(status, wss, b);
+    hyp = slice(hyp, wss, b);
+  }
   // hopeless epoch: a constrained hyper-parameter is not finite or a lengthscale / outputscale has underflowed to zero
   // (pSGLD's Langevin step divides by sqrt(sqrt(v) + 1e-8): a parameter with a vanishing gradient random-walks in steps of
   // ~5 raw units, sgld.py:64-70).  K is then NaN, no jitter can repair it, and -- as in the reference, where the closure
@@ -213,7 +227,7 @@ __global__ void __launch_bounds__(256) psgld_guarded_kernel(float *__restrict__ 
     if (!isfinite(h) || (i != 1 && !(h > 0.0f))) bad = 1;
   }
   __syncthreads();
-  const int ok = info[0] == 0 && !bad, ep = info[1], slot = info[2];
+  const int ep = info[1], slot = info[2], ok = info[0] == 0 && !bad && ep < num_epochs;
   const float *xi = (langevin && (ep + 1) > pretrain) ? langevin + (int64_t)ep * p : nullptr;
   if (ok) {
     for (int i = threadIdx.x; i < p; i += blockDim.x) {
@@ -234,38 +248,42 @@ __global__ void __launch_bounds__(256) psgld_guarded_kernel(float *__restrict__ 
 
 // gram -> cholesky at (hyp, jitter); info left on the device.  tc: the Cholesky's outer update on the tensor cores
 // (nullptr: FP32 SIMT).  (mixed model: gathers the embedding features at the current tables / lengthscale first)
+// bt: the outputs of a batch, w = the workspace of output 0, raw = its raw row.
 static int factor_once(const float *Xt, int64_t n, int64_t np, const ModelSpec &sp, const float *raw, int kern,
-                       const float *noise_diag, float jitter, FitWs &w, cudaStream_t st, const TcBuffers *tc) {
-  HB_CUDA(cudaMemsetAsync(w.info, 0, sizeof(int32_t), st));
-  int s = launch_emb_gather(raw + sp.i_tab(), sp, n, np, w.hyp, w.Ets, w.tab_s, st);
+                       const float *noise_diag, float jitter, FitWs &w, cudaStream_t st, const TcBuffers *tc,
+                       const Batch &bt = Batch()) {
+  HB_CUDA(memset_slices(w.info, 0, sizeof(int32_t), bt, st));
+  int s = launch_emb_gather(raw + sp.i_tab(), sp, n, np, w.hyp, w.Ets, w.tab_s, st, bt);
   if (s != HB_OK) return s;
   if (sp.warp) {   // warped features (and their exponent derivatives) at the current a, b, lengthscales
-    s = launch_scale_zt(Xt, np, sp, w.hyp, w.Zt, w.dZa, w.dZb, st);
+    s = launch_scale_zt(Xt, np, sp, w.hyp, w.Zt, w.dZa, w.dZb, st, bt);
     if (s != HB_OK) return s;
   }
-  s = launch_gram(sp.warp ? w.Zt : Xt, w.Ets, n, np, sp, w.hyp, kern, noise_diag, jitter, w.L, st);
+  s = launch_gram(sp.warp ? w.Zt : Xt, w.Ets, n, np, sp, w.hyp, kern, noise_diag, jitter, w.L, st, bt);
   if (s != HB_OK) return s;
-  return launch_cholesky(w.L, np, w.cholws, w.info, st, tc);
+  return launch_cholesky(w.L, np, w.cholws, w.info, st, tc, bt);
 }
 
 // one MLL forward + backward at `raw`: transform -> [gather] -> Gram -> Cholesky -> L^-1 -> alpha / log-det -> K^-1 ->
 // gradient, into w.grad / w.loss (factorisation status in w.info).  tc: the GEMM stages on the 3xTF32 tensor cores, with
 // zero_fill on the first use of the workspace in a fit (see launch_tri_inverse_tc); nullptr: FP32 SIMT.
+// bt: all outputs of a batch (tensor-core path only), w / raw / y those of output 0.
 static int enqueue_mll(const float *Xt, const float *y, int64_t n, int64_t np, const ModelSpec &sp, const float *raw, int kern,
                        const float *noise_diag, float noise_lb, float noise_guess, float jitter, FitWs &w, cudaStream_t st,
-                       const TcBuffers *tc, bool zero_fill) {
-  int s = launch_transform_hypers(raw, sp, noise_lb, w.hyp, st);
+                       const TcBuffers *tc, bool zero_fill, const Batch &bt = Batch()) {
+  if (!tc && bt.nout != 1) return HB_ERR_INVALID;
+  int s = launch_transform_hypers(raw, sp, noise_lb, w.hyp, st, bt);
   if (s != HB_OK) return s;
-  s = factor_once(Xt, n, np, sp, raw, kern, noise_diag, jitter, w, st, tc);
+  s = factor_once(Xt, n, np, sp, raw, kern, noise_diag, jitter, w, st, tc, bt);
   if (s != HB_OK) return s;
-  s = tc ? launch_tri_inverse_tc(w.L, np, w.Linv, *tc, zero_fill, st) : launch_tri_inverse(w.L, np, w.Linv, w.tmp, st);
+  s = tc ? launch_tri_inverse_tc(w.L, np, w.Linv, *tc, zero_fill, st, bt) : launch_tri_inverse(w.L, np, w.Linv, w.tmp, st);
   if (s != HB_OK) return s;
-  s = launch_solve_logdet(w.L, w.Linv, y, n, np, w.hyp, w.alpha, w.scal, w.solvews, st);
+  s = launch_solve_logdet(w.L, w.Linv, y, n, np, w.hyp, w.alpha, w.scal, w.solvews, st, bt);
   if (s != HB_OK) return s;
-  s = tc ? launch_kinv_tc(np, w.tmp, *tc, st) : launch_kinv(w.Linv, np, w.tmp, st);
+  s = tc ? launch_kinv_tc(np, w.tmp, *tc, st, bt) : launch_kinv(w.Linv, np, w.tmp, st);
   if (s != HB_OK) return s;
   return launch_mll_grad(sp.warp ? w.Zt : Xt, w.Ets, n, np, sp, raw, w.hyp, kern, w.tmp, w.alpha, w.scal, noise_guess, w.grad,
-                         w.loss, w.gradws, st, w.dZa, w.dZb);
+                         w.loss, w.gradws, st, w.dZa, w.dZb, bt);
 }
 
 static float next_jitter(float j) { return j == 0.0f ? 1e-6f : j * 10.0f; }   // fp32 ladder of gp.py:104-110
@@ -503,87 +521,141 @@ int32_t hb_mll_fwd_bwd(const float *Xt, const int32_t *Xe, const float *y, int64
   return HB_OK;
 }
 
-int32_t hb_fit_ex(const float *Xt, const int32_t *Xe, const float *y, int64_t n, int64_t d, const hb_model_spec_t *spec,
-                  float *raw, int32_t kern, const float *noise_diag, float noise_lb, float noise_guess, float lr,
-                  int32_t num_epochs, const float *langevin, float *losses, void *ws, int64_t ws_bytes, void *stream) {
+int64_t hb_fit_multi_workspace_bytes(int64_t n, int64_t d, const hb_model_spec_t *spec, int64_t num_out) {
+  if (num_out < 1 || num_out > HB_MAX_OUTPUTS) return -1;
+  const int64_t one = hb_fit_workspace_bytes_ex(n, d, spec);
+  return one < 0 ? -1 : one * num_out;
+}
+
+int32_t hb_fit_multi_ex(const float *Xt, const int32_t *Xe, const float *Y, int64_t n, int64_t d, const hb_model_spec_t *spec,
+                        int64_t num_out, float *raw, int32_t kern, const float *noise_diag, float noise_lb, float noise_guess,
+                        float lr, int32_t num_epochs, const float *langevin, float *losses, int32_t *status, void *ws,
+                        int64_t ws_bytes, void *stream) {
   ModelSpec sp;
-  if (!y || !raw || !ws || n <= 0 || kern < 0 || kern > 2 || num_epochs < 0 || !build_spec(d, spec, sp) || (sp.d > 0 && !Xt))
+  if (!Y || !raw || !ws || !status || n <= 0 || kern < 0 || kern > 2 || num_epochs < 0 || num_out < 1 ||
+      num_out > HB_MAX_OUTPUTS || !build_spec(d, spec, sp) || (sp.d > 0 && !Xt))
     return HB_ERR_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
-  FitWs w = carve_fit(ws, n, sp);
-  if ((size_t)ws_bytes < w.total) return HB_ERR_INVALID;
+  const int B = (int)num_out;
+  FitWs w = carve_fit(ws, n, sp);          // output 0; output b's workspace starts b * stride bytes later
+  const int64_t stride = (int64_t)w.total;
+  if (ws_bytes / B < stride) return HB_ERR_INVALID;
+  const Batch all{B, stride};
   const int64_t np = round_up(n, TILE);
   const int64_t P = sp.P();
   HostStatus *hs = pinned_status();
   if (!hs) return HB_ERR_CUDA;
-  {
-    const int s = bind_spec_ws(spec, sp, w, Xe, n, st);
+  for (int b = B - 1; b >= 0; --b) {        // every slice is a complete workspace; sp ends up bound to slice 0's arrays
+    FitWs wb = carve_fit(slice(ws, stride, b), n, sp);
+    const int s = bind_spec_ws(spec, sp, wb, Xe, n, st);
     if (s != HB_OK) return s;
   }
-  HB_CUDA(cudaMemsetAsync(w.sq, 0, P * sizeof(float), st));
-  HB_CUDA(cudaMemsetAsync(w.info, 0, 4 * sizeof(int32_t), st));   // status, epoch counter, replay slot
+  HB_CUDA(memset_slices(w.sq, 0, P * sizeof(float), all, st));
+  HB_CUDA(memset_slices(w.info, 0, 4 * sizeof(int32_t), all, st));   // status, epoch counter, replay slot
   bool zeroed = false;                           // triangular complements of Linv / U zero-filled once per fit
   const int pretrain = num_epochs / 10;          // gp.py:99 pretrain_step = num_epochs // 10
   const float factor = 1.0f / (float)n;          // gp.py:99 factor = 1 / y.shape[0]
 
-  // one epoch = MLL forward + backward on the tensor cores -> guarded pSGLD step
-  auto enqueue_epoch = [&](float jitter, cudaStream_t s_) -> int {
-    const int s = enqueue_mll(Xt, y, n, np, sp, raw, kern, noise_diag, noise_lb, noise_guess, jitter, w, s_, &w.tc, !zeroed);
+  // one epoch of outputs [b0, b0 + bt.nout) = MLL forward + backward on the tensor cores -> guarded pSGLD step
+  auto enqueue_epoch = [&](float jitter, cudaStream_t s_, int b0, const Batch &bt) -> int {
+    FitWs wb = carve_fit(slice(ws, stride, b0), n, sp);
+    const int s = enqueue_mll(Xt, Y + b0 * n, n, np, sp, raw + b0 * P, kern, noise_diag, noise_lb, noise_guess, jitter, wb, s_,
+                              &wb.tc, !zeroed, bt);
     zeroed = true;
     if (s != HB_OK) return s;
-    psgld_guarded_kernel<<<1, 256, 0, s_>>>(raw, w.grad, w.sq, (int)P, lr, 0.99f, 1e-8f, factor, langevin, pretrain, w.info,
-                                           w.loss, w.status, w.hyp, sp.H(), sp.warp == 2 ? sp.i_wa() : 0,
-                                           sp.warp == 2 ? sp.i_wa() + sp.n_w() : 0);
+    psgld_guarded_kernel<<<bt.nout, 256, 0, s_>>>(raw + b0 * P, wb.grad, wb.sq, (int)P, lr, 0.99f, 1e-8f, factor,
+                                                 langevin ? langevin + (int64_t)b0 * num_epochs * P : nullptr, pretrain,
+                                                 num_epochs, wb.info, wb.loss, wb.status, wb.hyp, sp.H(),
+                                                 sp.warp == 2 ? sp.i_wa() : 0, sp.warp == 2 ? sp.i_wa() + sp.n_w() : 0, stride);
     count_launches(1);
     HB_LAUNCH_CHECK("psgld_guarded");
     return HB_OK;
   };
-  // epoch `ep` with the jitter ladder of gp.py:104-126, one host synchronisation per attempt
-  bool hopeless = false;
-  int hopeless_from = 0;
-  auto slow_epoch = [&](int ep) -> int {
+  // per-output host state: next epoch, and whether the output stopped on a hopeless epoch (from which epoch)
+  std::vector<int> ep(B, 0), hopeless_from(B, -1);
+  auto active = [&](int b) { return hopeless_from[b] < 0 && ep[b] < num_epochs; };
+  auto loss_out = [&](int b, int e, float v) {
+    if (losses) losses[(int64_t)b * num_epochs + e] = v;
+  };
+  // epoch ep[b] of output b with the jitter ladder of gp.py:104-126 on its own slice, one host synchronisation per attempt;
+  // the other outputs are not touched
+  const Batch one{1, stride};
+  auto slow_epoch = [&](int b) -> int {
+    FitWs wb = carve_fit(slice(ws, stride, b), n, sp);
     float jitter = 0.0f;
     for (;;) {
-      HB_CUDA(cudaMemsetAsync(w.info + 2, 0, sizeof(int32_t), st));           // replay slot 0
-      const int s = enqueue_epoch(jitter, st);
+      HB_CUDA(cudaMemsetAsync(wb.info + 2, 0, sizeof(int32_t), st));          // replay slot 0
+      const int s = enqueue_epoch(jitter, st, b, one);
       if (s != HB_OK) return s;
-      HB_CUDA(cudaMemcpyAsync(hs->batch, w.status, 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
+      HB_CUDA(cudaMemcpyAsync(hs->batch[b], wb.status, 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
       HB_CUDA(cudaStreamSynchronize(st));
       int32_t info;
-      memcpy(&info, &hs->batch[0], sizeof(info));
+      memcpy(&info, &hs->batch[b][0], sizeof(info));
       if (info == 0) {
-        if (losses) losses[ep] = hs->batch[1];
+        loss_out(b, ep[b], hs->batch[b][1]);
+        ++ep[b];
         return HB_OK;
       }
       if (info == -1) {            // hopeless (see psgld_guarded_kernel): this and every later epoch is given up
-        hopeless = true;
-        hopeless_from = ep;
+        hopeless_from[b] = ep[b];
         return HB_OK;
       }
       jitter = next_jitter(jitter);
       if (jitter > JITTER_MAX) {   // "jitter is too large, give up fitting GP": epoch skipped, gp.py:121-122
-        if (losses) losses[ep] = INFINITY;
-        hs->set_epoch = ep + 1;     // the device counter only advances on success
-        HB_CUDA(cudaMemcpyAsync(w.info + 1, &hs->set_epoch, sizeof(int32_t), cudaMemcpyHostToDevice, st));
+        loss_out(b, ep[b], INFINITY);
+        hs->set_epoch = ++ep[b];    // the device counter only advances on success
+        HB_CUDA(cudaMemcpyAsync(wb.info + 1, &hs->set_epoch, sizeof(int32_t), cudaMemcpyHostToDevice, st));
         HB_CUDA(cudaStreamSynchronize(st));
         return HB_OK;
       }
     }
   };
+  // (info, loss) of the first `slots` replays of every output -> hs->batch
+  auto read_status = [&](int slots) -> int {
+    HB_CUDA(cudaMemcpy2DAsync(hs->batch, sizeof(hs->batch[0]), w.status, (size_t)stride, (size_t)slots * 2 * sizeof(float), B,
+                              cudaMemcpyDeviceToHost, st));
+    HB_CUDA(cudaStreamSynchronize(st));
+    return HB_OK;
+  };
+  // outputs whose slot `slot` holds a failed attempt go through the ladder; returns whether any did
+  auto consume = [&](int slots, int &failed) -> int {
+    failed = 0;
+    for (int b = 0; b < B; ++b) {
+      if (!active(b)) continue;
+      const int need = slots < num_epochs - ep[b] ? slots : num_epochs - ep[b];
+      int done = 0;
+      for (; done < need; ++done) {
+        int32_t info;
+        memcpy(&info, &hs->batch[b][2 * done], sizeof(info));
+        if (info != 0) break;
+        loss_out(b, ep[b] + done, hs->batch[b][2 * done + 1]);
+      }
+      ep[b] += done;
+      if (done < need) {   // epoch ep[b] needs jitter: the plain path with the ladder, then back to the batch
+        failed = 1;
+        const int s = slow_epoch(b);
+        if (s != HB_OK) return s;
+      }
+    }
+    return HB_OK;
+  };
 
-  int ep = 0;
-  if (num_epochs > 0) {   // first epoch on the plain path: it also builds every lazily created table / attribute
-    const int s = slow_epoch(0);
+  if (num_epochs > 0) {   // first epoch of every output on the plain path: it also builds every lazily created table / attribute
+    HB_CUDA(memset_slices(w.info + 2, 0, sizeof(int32_t), all, st));
+    int s = enqueue_epoch(0.0f, st, 0, all);
+    if (s == HB_OK) s = read_status(1);
+    int failed = 0;
+    if (s == HB_OK) s = consume(1, failed);
     if (s != HB_OK) return s;
-    ep = 1;
   }
-  // Remaining epochs: capture ONE epoch (jitter 0) into a CUDA graph and replay it FIT_BATCH times per host
-  // synchronisation.  A failed factorisation leaves the hypers, the RMS state and the device epoch counter untouched
-  // (the pSGLD kernel is guarded), so every later replay of the batch fails the same way; the host then runs that epoch
-  // through the jitter ladder on the plain path and resumes.
+  // Remaining epochs: capture ONE epoch of all outputs (jitter 0) into a CUDA graph and replay it FIT_BATCH times per host
+  // synchronisation.  A failed factorisation leaves that output's hypers, RMS state and device epoch counter untouched
+  // (the pSGLD kernel is guarded), so every later replay of the batch fails the same way for it; the host then runs that
+  // output's epoch through the jitter ladder on the plain path, on its own slice, and resumes.  The other outputs are
+  // unaffected: each has its own counter and replay slots.
   cudaGraphExec_t exec = nullptr;
   long long launches_per_epoch = 0;
-  if (num_epochs - ep >= 4) {
+  if (num_epochs - 1 >= 4) {
     static cudaStream_t gs_dev[MAX_DEVICES] = {};   // one capture stream per device
     int cur_dev = 0;
     cudaGetDevice(&cur_dev);
@@ -594,7 +666,7 @@ int32_t hb_fit_ex(const float *Xt, const int32_t *Xe, const float *y, int64_t n,
       cudaGraph_t graph = nullptr;
       const long long before = g_launches.load();
       if (cudaStreamBeginCapture(gs, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
-        const int s = enqueue_epoch(0.0f, gs);
+        const int s = enqueue_epoch(0.0f, gs, 0, all);
         const cudaError_t e = cudaStreamEndCapture(gs, &graph);
         if (s == HB_OK && e == cudaSuccess && graph && cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess) {
           launches_per_epoch = g_launches.load() - before;
@@ -608,43 +680,53 @@ int32_t hb_fit_ex(const float *Xt, const int32_t *Xe, const float *y, int64_t n,
     }
   }
   int batch = FIT_BATCH;
-  while (ep < num_epochs) {
-    if (hopeless) break;
+  for (;;) {
+    int left = 0;   // epochs the furthest-behind active output still needs
+    for (int b = 0; b < B; ++b)
+      if (active(b) && num_epochs - ep[b] > left) left = num_epochs - ep[b];
+    if (left == 0) break;
     if (!exec) {
-      const int s = slow_epoch(ep);
-      if (s != HB_OK) return s;
-      ++ep;
+      for (int b = 0; b < B; ++b) {
+        if (!active(b)) continue;
+        const int s = slow_epoch(b);
+        if (s != HB_OK) return s;
+      }
       continue;
     }
-    int B = batch < FIT_BATCH ? batch : FIT_BATCH;   // ramps 1, 2, 4, .. after a failure: a failing epoch wastes the rest
-    if (B > num_epochs - ep) B = num_epochs - ep;    // of its batch, and failures come in runs (gp.py:117-126 territory)
-    HB_CUDA(cudaMemsetAsync(w.info + 2, 0, sizeof(int32_t), st));
-    for (int b = 0; b < B; ++b) HB_CUDA(cudaGraphLaunch(exec, st));
-    count_launches(launches_per_epoch * B);
-    HB_CUDA(cudaMemcpyAsync(hs->batch, w.status, (size_t)B * 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
-    HB_CUDA(cudaStreamSynchronize(st));
-    int done = 0;
-    for (; done < B; ++done) {
-      int32_t info;
-      memcpy(&info, &hs->batch[2 * done], sizeof(info));
-      if (info != 0) break;
-      if (losses) losses[ep + done] = hs->batch[2 * done + 1];
+    int R = batch < FIT_BATCH ? batch : FIT_BATCH;   // ramps 1, 2, 4, .. after a failure: a failing epoch wastes the rest
+    if (R > left) R = left;                         // of its batch, and failures come in runs (gp.py:117-126 territory)
+    HB_CUDA(memset_slices(w.info + 2, 0, sizeof(int32_t), all, st));
+    for (int r = 0; r < R; ++r) HB_CUDA(cudaGraphLaunch(exec, st));
+    count_launches(launches_per_epoch * R);
+    int failed = 0;
+    int s = read_status(R);
+    if (s == HB_OK) s = consume(R, failed);
+    if (s != HB_OK) {
+      cudaGraphExecDestroy(exec);
+      return s;
     }
-    ep += done;
-    batch = (done < B) ? 1 : (2 * batch > FIT_BATCH ? FIT_BATCH : 2 * batch);
-    if (done < B) {   // epoch `ep` needs jitter: plain path with the ladder, then back to the graph
-      const int s = slow_epoch(ep);
-      if (s != HB_OK) {
-        cudaGraphExecDestroy(exec);
-        return s;
-      }
-      ++ep;
-    }
+    batch = failed ? 1 : (2 * batch > FIT_BATCH ? FIT_BATCH : 2 * batch);
   }
   if (exec) cudaGraphExecDestroy(exec);
-  if (hopeless && losses)          // "jitter is too large, give up fitting GP" for that and every remaining epoch
-    for (int e = hopeless_from; e < num_epochs; ++e) losses[e] = INFINITY;
-  return hb_factorize_ex(Xt, w.Xe, y, n, d, spec, raw, kern, noise_diag, noise_lb, nullptr, ws, ws_bytes, stream);
+  // final prediction state of every output, once per fit
+  for (int b = 0; b < B; ++b) {
+    if (hopeless_from[b] >= 0)   // "jitter is too large, give up fitting GP" for that and every remaining epoch
+      for (int e = hopeless_from[b]; e < num_epochs; ++e) loss_out(b, e, INFINITY);
+    const int s = hb_factorize_ex(Xt, w.Xe, Y + b * n, n, d, spec, raw + b * P, kern, noise_diag, noise_lb, nullptr,
+                                  slice(ws, stride, b), stride, stream);
+    if (s != HB_OK && s != HB_ERR_NOT_PD) return s;
+    status[b] = s;
+  }
+  return HB_OK;
+}
+
+int32_t hb_fit_ex(const float *Xt, const int32_t *Xe, const float *y, int64_t n, int64_t d, const hb_model_spec_t *spec,
+                  float *raw, int32_t kern, const float *noise_diag, float noise_lb, float noise_guess, float lr,
+                  int32_t num_epochs, const float *langevin, float *losses, void *ws, int64_t ws_bytes, void *stream) {
+  int32_t status = HB_OK;
+  const int32_t s = hb_fit_multi_ex(Xt, Xe, y, n, d, spec, 1, raw, kern, noise_diag, noise_lb, noise_guess, lr, num_epochs,
+                                    langevin, losses, &status, ws, ws_bytes, stream);
+  return s != HB_OK ? s : status;
 }
 int32_t hb_fit(const float *Xt, const float *y, int64_t n, int64_t d, float *raw, int32_t kern,
                const float *noise_diag, float noise_lb, float noise_guess, float lr, int32_t num_epochs,

@@ -278,16 +278,23 @@ __device__ __forceinline__ void stage_factor(Block64Smem &sm, const float *__res
 //   D(j)            : composite = sub-diagonal tile (j, j-1) [jl >= 1] followed by the diagonal tile (j, j), both
 //                     finished by ONE CTA so that the trsm result feeds the diagonal update straight from shared memory
 //   R(i, j), i >= j+2 (i >= j+1 in the last column of the block): the other tiles of column j
-__global__ void __launch_bounds__(GTHREADS, 1) chol_block64_kernel(float *__restrict__ A, int64_t np, int jb0, int nbc,
-                                                                   int ntasks, int *__restrict__ flags, int token,
-                                                                   int32_t *info) {
+//   Batch: the tasks of the `nout` outputs are interleaved, global task = task * nout + output, so the pivot chains of all
+//   outputs advance together.  A task only depends on smaller tasks of its own output, which have smaller global numbers:
+//   the argument above still holds.  A, the flags and info of output b live in its workspace slice (wss bytes apart).
+__global__ void __launch_bounds__(GTHREADS, 1) chol_block64_kernel(float *__restrict__ A0, int64_t np, int jb0, int nbc,
+                                                                   int ntasks, int *__restrict__ flags0, int token,
+                                                                   int32_t *info0, int nout, int64_t wss) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   Block64Smem &sm = *reinterpret_cast<Block64Smem *>(smem_raw);
   const int t = threadIdx.x;
   const int warp = t >> 5, lane = t & 31;
   const int tc = 2 * warp + (lane >> 4), ti = lane & 15;   // 4x4 micro-tile: rows 4 ti.., cols 4 tc..
   const int nt = (int)(np / TS);
-  for (int task = blockIdx.x; task < ntasks; task += gridDim.x) {
+  for (int gtask = blockIdx.x; gtask < ntasks * nout; gtask += gridDim.x) {
+    const int task = gtask / nout, ob = gtask - task * nout;
+    float *__restrict__ A = slice(A0, wss, ob);
+    int *__restrict__ flags = slice(flags0, wss, ob);
+    int32_t *info = slice(info0, wss, ob);
     int jl = 0, tt = task;
     for (;;) {
       const int j_ = jb0 + jl;
@@ -385,7 +392,13 @@ __device__ __forceinline__ void split_store4(float *__restrict__ f32, float *__r
 __global__ void __launch_bounds__(GTHREADS, 1) triinv_base2_kernel(const float *__restrict__ L, int64_t np,
                                                                    float *__restrict__ Linv, float *__restrict__ Linv_hi,
                                                                    float *__restrict__ Linv_lo, float *__restrict__ U_hi,
-                                                                   float *__restrict__ U_lo) {
+                                                                   float *__restrict__ U_lo, int64_t wss) {
+  L = slice(L, wss, blockIdx.z);   // output (Batch)
+  Linv = slice(Linv, wss, blockIdx.z);
+  Linv_hi = slice(Linv_hi, wss, blockIdx.z);
+  Linv_lo = slice(Linv_lo, wss, blockIdx.z);
+  U_hi = slice(U_hi, wss, blockIdx.z);
+  U_lo = slice(U_lo, wss, blockIdx.z);
   extern __shared__ __align__(16) unsigned char smem_raw[];
   TriBase2Smem &sm = *reinterpret_cast<TriBase2Smem *>(smem_raw);
   const int t = threadIdx.x;
@@ -462,7 +475,7 @@ __global__ void __launch_bounds__(GTHREADS, 1) triinv_base2_kernel(const float *
 }
 
 int launch_triinv_base2(const float *L, int64_t np, float *Linv, float *Linv_hi, float *Linv_lo, float *U_hi, float *U_lo,
-                        cudaStream_t st) {
+                        cudaStream_t st, const Batch &bt) {
   static PerDevice once;
   bool fresh = false;
   const int dev = once.slot(&fresh);
@@ -471,7 +484,8 @@ int launch_triinv_base2(const float *L, int64_t np, float *Linv, float *Linv_hi,
     HB_CUDA(cudaFuncSetAttribute(triinv_base2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TriBase2Smem)));
     once.done[dev] = true;
   }
-  triinv_base2_kernel<<<(int)(np / GT), GTHREADS, sizeof(TriBase2Smem), st>>>(L, np, Linv, Linv_hi, Linv_lo, U_hi, U_lo);
+  triinv_base2_kernel<<<dim3((unsigned)(np / GT), 1, (unsigned)bt.nout), GTHREADS, sizeof(TriBase2Smem), st>>>(
+      L, np, Linv, Linv_hi, Linv_lo, U_hi, U_lo, bt.ws);
   count_launches(1);
   HB_LAUNCH_CHECK("triinv_base2");
   return HB_OK;
@@ -514,8 +528,9 @@ __global__ void __launch_bounds__(GTHREADS, 2) chol_update_kernel(float *__restr
   }
 }
 
-int launch_cholesky(float *A, int64_t np, float *ws, int32_t *info, cudaStream_t st, const TcBuffers *tc) {
+int launch_cholesky(float *A, int64_t np, float *ws, int32_t *info, cudaStream_t st, const TcBuffers *tc, const Batch &bt) {
   if (np <= 0 || np % GT != 0) return HB_ERR_INVALID;
+  if (!tc && bt.nout != 1) return HB_ERR_INVALID;   // the FP32 SIMT outer update serves single factorisations only
   static PerDevice once;   // aux[dev] = co-resident CTAs of the cooperative block kernel on that device
   bool fresh = false;
   const int dev = once.slot(&fresh);
@@ -538,7 +553,7 @@ int launch_cholesky(float *A, int64_t np, float *ws, int32_t *info, cudaStream_t
   const int nt = (int)(np / GT), nt64 = (int)(np / TS);
   int *flags = reinterpret_cast<int *>(ws);   // [nt64][MAXBC64] tile flags (ws holds >= 64 KiB)
   if ((size_t)nt64 * MAXBC64 * sizeof(int) > (size_t)GT * GT * sizeof(float)) return HB_ERR_INVALID;
-  HB_CUDA(cudaMemsetAsync(flags, 0, (size_t)nt64 * MAXBC64 * sizeof(int), st));
+  HB_CUDA(memset_slices(flags, 0, (size_t)nt64 * MAXBC64 * sizeof(int), bt, st));
   int token = 0;
   for (int64_t cb = 0; cb < np; cb += OUTER) {
     const int64_t ce = cb + OUTER < np ? cb + OUTER : np;
@@ -550,14 +565,16 @@ int launch_cholesky(float *A, int64_t np, float *ws, int32_t *info, cudaStream_t
     }
     ++token;
     {
-      const int grid = ntasks < max_ctas ? ntasks : max_ctas;
-      void *args[] = {&A, &np, &jb0, &nbc, &ntasks, &flags, &token, &info};
+      int nout = bt.nout;
+      int64_t wss = bt.ws;
+      const int grid = ntasks * nout < max_ctas ? ntasks * nout : max_ctas;
+      void *args[] = {&A, &np, &jb0, &nbc, &ntasks, &flags, &token, &info, &nout, &wss};
       HB_CUDA(cudaLaunchCooperativeKernel((const void *)chol_block64_kernel, dim3(grid), dim3(GTHREADS), args, BLOCK64_SMEM, st));
       count_launches(1);
     }
     if (ce == np) break;
     if (tc) {   // outer update on the tensor cores (wgmma 3xTF32, fit_tc.cu)
-      const int s = launch_chol_outer_update_tc(A, np, cb, ce, *tc, st);
+      const int s = launch_chol_outer_update_tc(A, np, cb, ce, *tc, st, bt);
       if (s != HB_OK) return s;
     } else {    // everything right of the block, K = block width
       const int J0 = (int)(ce / GT);

@@ -18,20 +18,21 @@
 namespace hb {
 
 // tables live in device memory: the current device is part of the key (a process may drive more than one GPU)
-static inline uint64_t table_key(int op, int64_t np, int64_t p1, int64_t p2) {
+static inline TcTableKey table_key(int op, int64_t np, int64_t p1, int64_t p2, const Batch &bt) {
   int dev = 0;
   cudaGetDevice(&dev);
-  return ((uint64_t)(dev & 15) << 60) ^ ((uint64_t)op << 54) ^ ((uint64_t)np << 36) ^ ((uint64_t)p1 << 18) ^ (uint64_t)p2;
+  return TcTableKey{dev, op, np, p1, p2, bt.nout};
 }
 
 // ------------------------------------------------------------------------------------------ Cholesky outer update
-int launch_chol_outer_update_tc(float *A, int64_t np, int64_t cb, int64_t ce, const TcBuffers &tc, cudaStream_t st) {
+int launch_chol_outer_update_tc(float *A, int64_t np, int64_t cb, int64_t ce, const TcBuffers &tc, cudaStream_t st,
+                                const Batch &bt) {
   const int64_t K = ce - cb;
   // hi/lo copy of the finished panel rows [ce, np) x [cb, ce) -> P[r][c - cb], leading dimension K
-  int s = launch_split_region(A + ce * np + cb, np, tc.P_hi + ce * K, tc.P_lo + ce * K, K, np - ce, K, st);
+  int s = launch_split_region(A + ce * np + cb, np, tc.P_hi + ce * K, tc.P_lo + ce * K, K, np - ce, K, st, bt);
   if (s != HB_OK) return s;
   int ntiles = 0;
-  const uint64_t key = table_key(1, np, cb, ce);
+  const TcTableKey key = table_key(1, np, cb, ce, bt);
   const TcTile *tiles = tc_table_lookup(key, &ntiles);
   if (!tiles) {
     std::vector<TcTile> host;
@@ -50,24 +51,25 @@ int launch_chol_outer_update_tc(float *A, int64_t np, int64_t cb, int64_t ce, co
   epi.ldc = np;
   epi.r0 = (int)ce;
   epi.ncols = (int)np;
-  return launch_tcgemm(P, P, 256, tiles, ntiles, epi, st);
+  return launch_tcgemm(P, P, 256, tiles, ntiles, epi, st, bt);
 }
 
 // ------------------------------------------------------------------------------------------ triangular inverse
 // base case: triinv_base2_kernel (cholesky.cu) inverts the 128x128 diagonal blocks into Linv (fp32 + hi/lo) and U (hi/lo)
-int launch_tri_inverse_tc(const float *L, int64_t np, float *Linv, const TcBuffers &tc, bool zero_fill, cudaStream_t st) {
+int launch_tri_inverse_tc(const float *L, int64_t np, float *Linv, const TcBuffers &tc, bool zero_fill, cudaStream_t st,
+                          const Batch &bt) {
   if (np <= 0 || np % GT != 0) return HB_ERR_INVALID;
   const size_t bytes = (size_t)np * np * sizeof(float);
   if (zero_fill) {   // the triangular complements are never written afterwards: once per workspace is enough
-    HB_CUDA(cudaMemsetAsync(Linv, 0, bytes, st));
-    HB_CUDA(cudaMemsetAsync(tc.Linv_hi, 0, bytes, st));
-    HB_CUDA(cudaMemsetAsync(tc.Linv_lo, 0, bytes, st));
-    HB_CUDA(cudaMemsetAsync(tc.U_hi, 0, bytes, st));
-    HB_CUDA(cudaMemsetAsync(tc.U_lo, 0, bytes, st));
+    HB_CUDA(memset_slices(Linv, 0, bytes, bt, st));
+    HB_CUDA(memset_slices(tc.Linv_hi, 0, bytes, bt, st));
+    HB_CUDA(memset_slices(tc.Linv_lo, 0, bytes, bt, st));
+    HB_CUDA(memset_slices(tc.U_hi, 0, bytes, bt, st));
+    HB_CUDA(memset_slices(tc.U_lo, 0, bytes, bt, st));
   }
-  int s = launch_split_region(L, np, tc.L_hi, tc.L_lo, np, np, np, st);
+  int s = launch_split_region(L, np, tc.L_hi, tc.L_lo, np, np, np, st, bt);
   if (s != HB_OK) return s;
-  s = launch_triinv_base2(L, np, Linv, tc.Linv_hi, tc.Linv_lo, tc.U_hi, tc.U_lo, st);
+  s = launch_triinv_base2(L, np, Linv, tc.Linv_hi, tc.Linv_lo, tc.U_hi, tc.U_lo, st, bt);
   if (s != HB_OK) return s;
   TcOperand opL{tc.L_hi, tc.L_lo, (uint64_t)np, (uint64_t)np, (uint64_t)np};
   TcOperand opU{tc.U_hi, tc.U_lo, (uint64_t)np, (uint64_t)np, (uint64_t)np};
@@ -77,7 +79,7 @@ int launch_tri_inverse_tc(const float *L, int64_t np, float *Linv, const TcBuffe
     const int bn = b >= 256 ? 256 : 128;
     for (int phase = 0; phase < 2; ++phase) {
       int ntiles = 0;
-      const uint64_t key = table_key(2 + phase, np, b, 0);
+      const TcTableKey key = table_key(2 + phase, np, b, 0, bt);
       const TcTile *tiles = tc_table_lookup(key, &ntiles);
       if (!tiles) {
         std::vector<TcTile> host;
@@ -111,7 +113,7 @@ int launch_tri_inverse_tc(const float *L, int64_t np, float *Linv, const TcBuffe
         epi.sign = 1.0f;
         epi.C_hi = tc.T_hi;
         epi.C_lo = tc.T_lo;
-        s = launch_tcgemm(opU, opL, bn, tiles, ntiles, epi, st);
+        s = launch_tcgemm(opU, opL, bn, tiles, ntiles, epi, st, bt);
       } else {
         epi.sign = -1.0f;
         epi.C = Linv;
@@ -119,7 +121,7 @@ int launch_tri_inverse_tc(const float *L, int64_t np, float *Linv, const TcBuffe
         epi.C_lo = tc.Linv_lo;
         epi.Ct_hi = tc.U_hi;
         epi.Ct_lo = tc.U_lo;
-        s = launch_tcgemm(opLinv, opT, bn, tiles, ntiles, epi, st);
+        s = launch_tcgemm(opLinv, opT, bn, tiles, ntiles, epi, st, bt);
       }
       if (s != HB_OK) return s;
     }
@@ -128,10 +130,10 @@ int launch_tri_inverse_tc(const float *L, int64_t np, float *Linv, const TcBuffe
 }
 
 // ------------------------------------------------------------------------------------------ K^-1 = U U^T
-int launch_kinv_tc(int64_t np, float *Kinv, const TcBuffers &tc, cudaStream_t st) {
+int launch_kinv_tc(int64_t np, float *Kinv, const TcBuffers &tc, cudaStream_t st, const Batch &bt) {
   if (np <= 0 || np % GT != 0) return HB_ERR_INVALID;
   int ntiles = 0;
-  const uint64_t key = table_key(4, np, 0, 0);
+  const TcTableKey key = table_key(4, np, 0, 0, bt);
   const TcTile *tiles = tc_table_lookup(key, &ntiles);
   if (!tiles) {
     std::vector<TcTile> host;
@@ -148,7 +150,7 @@ int launch_kinv_tc(int64_t np, float *Kinv, const TcBuffers &tc, cudaStream_t st
   epi.C = Kinv;
   epi.ldc = np;
   epi.ncols = (int)np;
-  return launch_tcgemm(opU, opU, 256, tiles, ntiles, epi, st);
+  return launch_tcgemm(opU, opU, 256, tiles, ntiles, epi, st, bt);
 }
 
 }  // namespace hb

@@ -46,6 +46,24 @@ struct ModelSpec {
   __host__ __device__ int dtot() const { return d + De; }
 };
 
+// ---- output dimension of the fit-loop kernels (DESIGN §3).  A batch of `nout` outputs that share one training set is
+// `nout` consecutive single-output workspaces `ws` bytes apart; output b reads its raw row at raw + b * P and its targets at
+// y + b * n, and shares the training inputs Xt / Xe.  Element-wise and tile kernels take b from blockIdx.z, the persistent
+// and cooperative ones from their work item.  nout = 1 is the single-output fit.
+struct Batch {
+  int nout = 1;
+  int64_t ws = 0;   // workspace slice stride in bytes (256-byte aligned)
+};
+template <class T>
+__host__ __device__ __forceinline__ T *slice(T *p, int64_t stride_bytes, int b) {
+  return p ? reinterpret_cast<T *>(reinterpret_cast<uintptr_t>(p) + (uintptr_t)(stride_bytes * b)) : p;
+}
+// memset of `bytes` at p in every slice of the batch
+inline cudaError_t memset_slices(void *p, int value, size_t bytes, const Batch &bt, cudaStream_t st) {
+  if (bt.nout == 1) return cudaMemsetAsync(p, value, bytes, st);
+  return cudaMemset2DAsync(p, (size_t)bt.ws, value, bytes, (size_t)bt.nout, st);
+}
+
 // ---- candidate feature map (DESIGN §5).  Every kernel that scales candidate rows goes through these two functions, and
 // the training rows take the same operations in the same order (scale_zt_kernel, emb_gather_kernel), so that a candidate
 // duplicating a training row has r = 0 exactly.
@@ -66,34 +84,39 @@ __device__ __forceinline__ float cand_feature(const ModelSpec &sp, bool warp, fl
 }
 
 // cholesky.cu / linalg.cu   (tc: outer update on the tensor cores, the gradient epochs; nullptr -> FP32 SIMT)
-int launch_cholesky(float *A, int64_t np, float *ws, int32_t *info, cudaStream_t st, const TcBuffers *tc = nullptr);
+int launch_cholesky(float *A, int64_t np, float *ws, int32_t *info, cudaStream_t st, const TcBuffers *tc = nullptr,
+                    const Batch &bt = Batch());
 int launch_triinv_base2(const float *L, int64_t np, float *Linv, float *Linv_hi, float *Linv_lo, float *U_hi, float *U_lo,
-                        cudaStream_t st);
+                        cudaStream_t st, const Batch &bt = Batch());
 // fit_tc.cu
-int launch_chol_outer_update_tc(float *A, int64_t np, int64_t cb, int64_t ce, const TcBuffers &tc, cudaStream_t st);
-int launch_tri_inverse_tc(const float *L, int64_t np, float *Linv, const TcBuffers &tc, bool zero_fill, cudaStream_t st);
-int launch_kinv_tc(int64_t np, float *Kinv, const TcBuffers &tc, cudaStream_t st);
+int launch_chol_outer_update_tc(float *A, int64_t np, int64_t cb, int64_t ce, const TcBuffers &tc, cudaStream_t st,
+                                const Batch &bt);
+int launch_tri_inverse_tc(const float *L, int64_t np, float *Linv, const TcBuffers &tc, bool zero_fill, cudaStream_t st,
+                          const Batch &bt);
+int launch_kinv_tc(int64_t np, float *Kinv, const TcBuffers &tc, cudaStream_t st, const Batch &bt);
 int launch_tri_inverse(const float *L, int64_t np, float *Linv, float *tmp, cudaStream_t st);
 int launch_kinv(const float *Linv, int64_t np, float *Kinv, cudaStream_t st);
 int launch_linv_refine(float *L, float *Linv, int64_t np, float *R, float *out, cudaStream_t st);
 int launch_solve_logdet(const float *L, const float *Linv, const float *y, int64_t n, int64_t np,
-                        const float *hyp, float *alpha, double *scal, void *ws, cudaStream_t st);
+                        const float *hyp, float *alpha, double *scal, void *ws, cudaStream_t st, const Batch &bt = Batch());
 size_t solve_ws_bytes(int64_t np);
 
 // pairwise.cu
-int launch_transform_hypers(const float *raw, const ModelSpec &sp, float noise_lb, float *hyp, cudaStream_t st);
+int launch_transform_hypers(const float *raw, const ModelSpec &sp, float noise_lb, float *hyp, cudaStream_t st,
+                            const Batch &bt = Batch());
 int launch_gram(const float *Xt, const float *Ets, int64_t n, int64_t np, const ModelSpec &sp, const float *hyp, int kern,
-                const float *noise_diag, float jitter, float *K, cudaStream_t st);
+                const float *noise_diag, float jitter, float *K, cudaStream_t st, const Batch &bt = Batch());
 int launch_mll_grad(const float *Xt, const float *Ets, int64_t n, int64_t np, const ModelSpec &sp, const float *raw,
                     const float *hyp, int kern, const float *Kinv, const float *alpha, const double *scal, float noise_guess,
-                    float *grad, float *loss, void *ws, cudaStream_t st, const float *dZa = nullptr, const float *dZb = nullptr);
+                    float *grad, float *loss, void *ws, cudaStream_t st, const float *dZa = nullptr, const float *dZb = nullptr,
+                    const Batch &bt = Batch());
 size_t grad_ws_bytes(int64_t np, const ModelSpec &sp);
 int launch_emb_gather(const float *tables, const ModelSpec &sp, int64_t n, int64_t np, const float *hyp, float *Ets, float *tab_s,
-                      cudaStream_t st);
+                      cudaStream_t st, const Batch &bt = Batch());
 int launch_psgld(float *raw, const float *grad, float *sq, int64_t p, float lr, float a, float eps,
                  float factor, const float *xi, cudaStream_t st);
 int launch_scale_zt(const float *Xt, int64_t np, const ModelSpec &sp, const float *hyp, float *Zt, float *dZa, float *dZb,
-                    cudaStream_t st);
+                    cudaStream_t st, const Batch &bt = Batch());
 
 // init.cu
 int launch_median_pdist(const float *Xt, int64_t np, int64_t d, const int32_t *idx, int64_t k, float clamp_min,

@@ -249,7 +249,11 @@ int launch_kinv(const float *Linv, int64_t np, float *Kinv, cudaStream_t st) {
 // v = Linv r  (warp per row, fp64 accumulate; r = y - c on the first n entries, 0 on the pad)
 __global__ void __launch_bounds__(256) gemv_rows_kernel(const float *__restrict__ Linv, const float *__restrict__ y,
                                                         const float *__restrict__ hyp, int64_t n, int64_t np,
-                                                        double *__restrict__ v) {
+                                                        double *__restrict__ v, int64_t wss) {
+  Linv = slice(Linv, wss, blockIdx.z);   // output (Batch): targets are n apart
+  y += (int64_t)blockIdx.z * n;
+  hyp = slice(hyp, wss, blockIdx.z);
+  v = slice(v, wss, blockIdx.z);
   const int warp = (int)((blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5);
   const int lane = threadIdx.x & 31;
   if (warp >= np) return;
@@ -273,7 +277,10 @@ __global__ void __launch_bounds__(256) gemv_rows_kernel(const float *__restrict_
 // partial[rs][j] = sum_{i in row slab rs, i >= j} Linv[i][j] v[i]
 constexpr int GEMVT_ROWS = 64;  // rows per slab
 __global__ void __launch_bounds__(128) gemv_cols_kernel(const float *__restrict__ Linv, const double *__restrict__ v,
-                                                        int64_t np, double *__restrict__ partial) {
+                                                        int64_t np, double *__restrict__ partial, int64_t wss) {
+  Linv = slice(Linv, wss, blockIdx.z);
+  v = slice(v, wss, blockIdx.z);
+  partial = slice(partial, wss, blockIdx.z);
   const int j = blockIdx.x * 128 + threadIdx.x;
   const int64_t i0 = (int64_t)blockIdx.y * GEMVT_ROWS;
   double s = 0.0;
@@ -297,7 +304,12 @@ __global__ void __launch_bounds__(128) gemv_cols_kernel(const float *__restrict_
 __global__ void __launch_bounds__(256) solve_finish_kernel(const float *__restrict__ L, const double *__restrict__ v,
                                                            const double *__restrict__ partial, int64_t n,
                                                            int64_t np, int nslab, float *__restrict__ alpha,
-                                                           double *__restrict__ scal) {
+                                                           double *__restrict__ scal, int64_t wss) {
+  L = slice(L, wss, blockIdx.z);
+  v = slice(v, wss, blockIdx.z);
+  partial = slice(partial, wss, blockIdx.z);
+  alpha = slice(alpha, wss, blockIdx.z);
+  scal = slice(scal, wss, blockIdx.z);
   // alpha (every block handles a strip), block 0 additionally reduces quad and logdet
   const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j < np) {
@@ -332,14 +344,15 @@ __global__ void __launch_bounds__(256) solve_finish_kernel(const float *__restri
 size_t solve_ws_bytes(int64_t np) { return (size_t)np * sizeof(double) * (1 + (size_t)(np / GEMVT_ROWS)); }
 
 int launch_solve_logdet(const float *L, const float *Linv, const float *y, int64_t n, int64_t np, const float *hyp,
-                        float *alpha, double *scal, void *ws, cudaStream_t st) {
+                        float *alpha, double *scal, void *ws, cudaStream_t st, const Batch &bt) {
   if (np <= 0 || np % GT != 0 || n > np) return HB_ERR_INVALID;
   double *v = reinterpret_cast<double *>(ws);
   double *partial = v + np;
   const int nslab = (int)(np / GEMVT_ROWS);
-  gemv_rows_kernel<<<(int)ceil_div(np * 32, 256), 256, 0, st>>>(Linv, y, hyp, n, np, v);
-  gemv_cols_kernel<<<dim3((unsigned)(np / 128), (unsigned)nslab), 128, 0, st>>>(Linv, v, np, partial);
-  solve_finish_kernel<<<(int)ceil_div(np, 256), 256, 0, st>>>(L, v, partial, n, np, nslab, alpha, scal);
+  const unsigned nz = (unsigned)bt.nout;
+  gemv_rows_kernel<<<dim3((unsigned)ceil_div(np * 32, 256), 1, nz), 256, 0, st>>>(Linv, y, hyp, n, np, v, bt.ws);
+  gemv_cols_kernel<<<dim3((unsigned)(np / 128), (unsigned)nslab, nz), 128, 0, st>>>(Linv, v, np, partial, bt.ws);
+  solve_finish_kernel<<<dim3((unsigned)ceil_div(np, 256), 1, nz), 256, 0, st>>>(L, v, partial, n, np, nslab, alpha, scal, bt.ws);
   count_launches(3);
   HB_LAUNCH_CHECK("solve_logdet");
   return HB_OK;

@@ -68,8 +68,13 @@ __global__ void __launch_bounds__(256, EMB ? 1 : 2) gram_kernel(const float *__r
                                                                 int64_t n, int64_t np, int d, int De,
                                                                 const float *__restrict__ hyp,
                                                                 const float *__restrict__ noise_diag, float jitter,
-                                                                float *__restrict__ K, int prescaled) {
+                                                                float *__restrict__ K, int prescaled, int64_t xs, int64_t wss) {
   __shared__ PairSmem sm;
+  const int b = blockIdx.z;   // output (Batch): Xt is per output only when it is the warped Zt
+  Xt = slice(Xt, xs, b);
+  Ets = slice(Ets, wss, b);
+  hyp = slice(hyp, wss, b);
+  K = slice(K, wss, b);
   int I, J;
   tri_decode((int)blockIdx.x, I, J);
   float r2[8][8];
@@ -125,14 +130,15 @@ __global__ void __launch_bounds__(256, EMB ? 1 : 2) gram_kernel(const float *__r
 }
 
 int launch_gram(const float *Xt, const float *Ets, int64_t n, int64_t np, const ModelSpec &sp, const float *hyp, int kern,
-                const float *noise_diag, float jitter, float *K, cudaStream_t st) {
+                const float *noise_diag, float jitter, float *K, cudaStream_t st, const Batch &bt) {
   if (n <= 0 || sp.dtot() <= 0 || np % PT != 0 || n > np || (sp.e > 0 && !Ets)) return HB_ERR_INVALID;
   const int nt = (int)(np / PT);
-  const int grid = nt * (nt + 1) / 2;
+  const dim3 grid((unsigned)(nt * (nt + 1) / 2), 1, (unsigned)bt.nout);
   const int pre = sp.warp ? 1 : 0;   // warped models: the caller passes Zt = warp(Xt) / lengthscale in place of Xt
+  const int64_t xs = sp.warp ? bt.ws : 0;
   const int s = with_kernel(kern, sp.e > 0, [&](auto kk, auto ee) {
     gram_kernel<decltype(kk)::value, decltype(ee)::value><<<grid, 256, 0, st>>>(Xt, Ets, n, np, sp.d, sp.De, hyp, noise_diag,
-                                                                                 jitter, K, pre);
+                                                                                 jitter, K, pre, xs, bt.ws);
   });
   if (s != HB_OK) return s;
   count_launches(1);
@@ -156,14 +162,16 @@ __global__ void __launch_bounds__(256, EMB ? 1 : 2) mll_grad_kernel(const float 
                                                                     const float *__restrict__ Kinv,
                                                                     const float *__restrict__ alpha,
                                                                     float *__restrict__ part, const float *__restrict__ dZa,
-                                                                    const float *__restrict__ dZb) {
+                                                                    const float *__restrict__ dZb, int64_t xs, int64_t wss) {
   __shared__ PairSmem sm;
+  // output (Batch): the per-output pointers are formed where they are used, so the parameters stay in the constant bank
+#define OUT(p, st) slice(p, st, blockIdx.z)
   __shared__ float wpart[8][DC];   // per-warp partials of the current feature chunk, summed in warp order into `part`
   int I, J;
   tri_decode((int)blockIdx.x, I, J);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int stride = d + 2 + (EMB ? 1 : 0) + (dZa ? 2 * d : 0);   // dZa != nullptr: warped model, Xt = Zt is prescaled
-  float *bpart = part + (int64_t)blockIdx.x * stride;
+  float *bpart = OUT(part, wss) + (int64_t)blockIdx.x * stride;
   // after a feature chunk: part slots [slot, slot + kc) of this block = sum over the warps, in warp order 0..7
   auto flush = [&](int slot, int kc) {
     __syncthreads();
@@ -180,11 +188,11 @@ __global__ void __launch_bounds__(256, EMB ? 1 : 2) mll_grad_kernel(const float 
   for (int i = 0; i < 8; ++i)
 #pragma unroll
     for (int j = 0; j < 8; ++j) g[i][j] = 0.0f;
-  const float *ls = dZa ? nullptr : hyp + 3;
+  const float *ls = dZa ? nullptr : OUT(hyp, wss) + 3;
   for (int k0 = 0; k0 < d; k0 += DC) {
     const int kc = min(DC, d - k0);
     __syncthreads();
-    stage_chunk(sm, Xt, np, I, J, k0, kc, ls);
+    stage_chunk(sm, OUT(Xt, xs), np, I, J, k0, kc, ls);
     __syncthreads();
     accum_sqdist(sm, kc, g);
   }
@@ -197,27 +205,27 @@ __global__ void __launch_bounds__(256, EMB ? 1 : 2) mll_grad_kernel(const float 
     for (int k0 = 0; k0 < De; k0 += DC) {
       const int kc = min(DC, De - k0);
       __syncthreads();
-      stage_chunk(sm, Ets, np, I, J, k0, kc, nullptr);
+      stage_chunk(sm, OUT(Ets, wss), np, I, J, k0, kc, nullptr);
       __syncthreads();
       accum_sqdist(sm, kc, r2e);
     }
   }
   // g currently holds r2; turn it into G and collect the scalar sums
-  const float s = hyp[2];
+  const float s = OUT(hyp, wss)[2];
   const float w = (I > J) ? 2.0f : 1.0f;
   float sum_wk = 0.0f, tr_w = 0.0f, sum_le = 0.0f;
   float ai[8], aj[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
-    ai[i] = alpha[(int64_t)I * PT + pr_row(i)];
-    aj[i] = alpha[(int64_t)J * PT + pr_col(i)];
+    ai[i] = OUT(alpha, wss)[(int64_t)I * PT + pr_row(i)];
+    aj[i] = OUT(alpha, wss)[(int64_t)J * PT + pr_col(i)];
   }
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     const int64_t gi = (int64_t)I * PT + pr_row(i);
 #pragma unroll
     for (int jh = 0; jh < 2; ++jh) {
-      const float4 kv = __ldg(reinterpret_cast<const float4 *>(Kinv + gi * np + (int64_t)J * PT + pr_col(jh * 4)));
+      const float4 kv = __ldg(reinterpret_cast<const float4 *>(OUT(Kinv, wss) + gi * np + (int64_t)J * PT + pr_col(jh * 4)));
       const float kvv[4] = {kv.x, kv.y, kv.z, kv.w};
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
@@ -245,7 +253,7 @@ __global__ void __launch_bounds__(256, EMB ? 1 : 2) mll_grad_kernel(const float 
   for (int k0 = 0; k0 < d; k0 += DC) {
     const int kc = min(DC, d - k0);
     __syncthreads();
-    stage_chunk(sm, Xt, np, I, J, k0, kc, ls);
+    stage_chunk(sm, OUT(Xt, xs), np, I, J, k0, kc, ls);
     __syncthreads();
     for (int kk = 0; kk < kc; ++kk) {
       const float4 a0 = *reinterpret_cast<const float4 *>(&sm.xi[kk][ty * 4]);
@@ -271,14 +279,14 @@ __global__ void __launch_bounds__(256, EMB ? 1 : 2) mll_grad_kernel(const float 
   // (the z rows in the lower half of the staging buffers, the derivative rows in the upper half)
   if (dZa) {
     for (int which = 0; which < 2; ++which) {
-      const float *dZ = which ? dZb : dZa;
+      const float *dZ = which ? OUT(dZb, wss) : OUT(dZa, wss);
       const int slot0 = d + 2 + (EMB ? 1 : 0) + which * d;
       for (int k0 = 0; k0 < d; k0 += DC / 2) {
         const int kc = min(DC / 2, d - k0);
         __syncthreads();
         for (int f = threadIdx.x; f < 2 * kc * (PT / 4); f += blockDim.x) {
           const int kk = f >> 5, c4 = f & 31;
-          const float *src = (kk < kc) ? Xt + (int64_t)(k0 + kk) * np : dZ + (int64_t)(k0 + kk - kc) * np;
+          const float *src = (kk < kc) ? OUT(Xt, xs) + (int64_t)(k0 + kk) * np : dZ + (int64_t)(k0 + kk - kc) * np;
           const int row = (kk < kc) ? kk : DC / 2 + (kk - kc);
           *reinterpret_cast<float4 *>(&sm.xi[row][c4 * 4]) = __ldg(reinterpret_cast<const float4 *>(src + (int64_t)I * PT + c4 * 4));
           *reinterpret_cast<float4 *>(&sm.xj[row][c4 * 4]) = __ldg(reinterpret_cast<const float4 *>(src + (int64_t)J * PT + c4 * 4));
@@ -320,6 +328,7 @@ __global__ void __launch_bounds__(256, EMB ? 1 : 2) mll_grad_kernel(const float 
   }
   flush(d, EMB ? 3 : 2);
 }
+#undef OUT
 
 // ---- gradient w.r.t. the embedding rows (mixed model):  d data / d e_i = -(1/le) sum_j G2_ij (E_i - E_j),
 // G2 = W s phi1 h2 over the FULL pair matrix (both (i,j) and (j,i) contribute, which cancels the 1/2), E = e / le.
@@ -330,8 +339,18 @@ template <int KERN>
 __global__ void __launch_bounds__(256, 1) emb_rowgrad_kernel(const float *__restrict__ Xt, const float *__restrict__ Ets,
                                                              int64_t n, int64_t np, int d, int De,
                                                              const float *__restrict__ hyp, const float *__restrict__ Kinv,
-                                                             const float *__restrict__ alpha, float *__restrict__ gE, int prescaled) {
+                                                             const float *__restrict__ alpha, float *__restrict__ gE, int prescaled,
+                                                             int64_t xs, int64_t wss) {
   __shared__ PairSmem sm;
+  {
+    const int b = blockIdx.z;   // output (Batch)
+    Xt = slice(Xt, xs, b);
+    Ets = slice(Ets, wss, b);
+    hyp = slice(hyp, wss, b);
+    Kinv = slice(Kinv, wss, b);
+    alpha = slice(alpha, wss, b);
+    gE = slice(gE, wss, b);
+  }
   const int J = blockIdx.x, I = blockIdx.y;
   float g[8][8], r2e[8][8];
 #pragma unroll
@@ -397,9 +416,9 @@ __global__ void __launch_bounds__(256, 1) emb_rowgrad_kernel(const float *__rest
 
 // one block per table entry t = (column c, category u, coordinate q):  grad[1 + t] = (1 / (n le)) sum_{i: Xe[i,c] == u} sum_J gE[J][q][i]
 __global__ void __launch_bounds__(256) emb_scatter_kernel(const float *__restrict__ gE, int nt, int64_t n, int64_t np, ModelSpec sp,
-                                                          const float *__restrict__ hyp, float *__restrict__ grad) {
+                                                          const float *__restrict__ hyp, float *__restrict__ grad, int64_t wss) {
   __shared__ double red[256];
-  const int t = blockIdx.x;
+  const int t = blockIdx.x;   // (output: blockIdx.z, Batch)
   const int c = sp.ent_col[t], u = sp.ent_u[t];
   int qg = sp.ent_q[t];   // global embedding coordinate = (#coordinates of earlier columns) + coordinate inside column c
   for (int cc = 0; cc < c; ++cc) qg += sp.emb_size[cc];
@@ -407,7 +426,7 @@ __global__ void __launch_bounds__(256) emb_scatter_kernel(const float *__restric
   for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
     if (sp.Xe[i * sp.e + c] != u) continue;
     float a = 0.0f;
-    for (int Jt = 0; Jt < nt; ++Jt) a += gE[((int64_t)Jt * sp.De + qg) * np + i];
+    for (int Jt = 0; Jt < nt; ++Jt) a += slice(gE, wss, blockIdx.z)[((int64_t)Jt * sp.De + qg) * np + i];
     acc += (double)a;
   }
   red[threadIdx.x] = acc;
@@ -416,7 +435,8 @@ __global__ void __launch_bounds__(256) emb_scatter_kernel(const float *__restric
     if ((int)threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
     __syncthreads();
   }
-  if (threadIdx.x == 0) grad[sp.i_tab() + t] = (float)(red[0] / ((double)n * (double)hyp[3 + sp.d]));
+  if (threadIdx.x == 0)
+    slice(grad, wss, blockIdx.z)[sp.i_tab() + t] = (float)(red[0] / ((double)n * (double)slice(hyp, wss, blockIdx.z)[3 + sp.d]));
 }
 
 // One block: reduce the per-tile partials in fp64, add the priors, chain through softplus, scale by -1/n.
@@ -425,7 +445,17 @@ __global__ void __launch_bounds__(256) mll_finish_kernel(const float *__restrict
                                                          const float *__restrict__ raw, const float *__restrict__ hyp,
                                                          const float *__restrict__ alpha,
                                                          const double *__restrict__ scal, float noise_guess,
-                                                         float *__restrict__ grad, float *__restrict__ loss) {
+                                                         float *__restrict__ grad, float *__restrict__ loss, int64_t wss) {
+  {
+    const int b = blockIdx.z;   // output (Batch): raw rows are P apart
+    part = slice(part, wss, b);
+    raw += (int64_t)b * sp.P();
+    hyp = slice(hyp, wss, b);
+    alpha = slice(alpha, wss, b);
+    scal = slice(scal, wss, b);
+    grad = slice(grad, wss, b);
+    loss = slice(loss, wss, b);
+  }
   const int d = sp.d;
   const int stride = d + 2 + (sp.e > 0 ? 1 : 0) + sp.n_w();
   __shared__ double red[256];
@@ -515,31 +545,34 @@ size_t grad_ws_bytes(int64_t np, const ModelSpec &sp) {
 
 int launch_mll_grad(const float *Xt, const float *Ets, int64_t n, int64_t np, const ModelSpec &sp, const float *raw,
                     const float *hyp, int kern, const float *Kinv, const float *alpha, const double *scal, float noise_guess,
-                    float *grad, float *loss, void *ws, cudaStream_t st, const float *dZa, const float *dZb) {
+                    float *grad, float *loss, void *ws, cudaStream_t st, const float *dZa, const float *dZb, const Batch &bt) {
   if (sp.warp && (!dZa || !dZb)) return HB_ERR_INVALID;   // warped model: Xt must be Zt = warp(x) / l, with its derivative rows
   if (!sp.warp) dZa = dZb = nullptr;
   if (n <= 0 || sp.dtot() <= 0 || np % PT != 0 || n > np || (sp.e > 0 && !Ets)) return HB_ERR_INVALID;
   const int nt = (int)(np / PT);
   const int grid = nt * (nt + 1) / 2;
   const int d = sp.d;
+  const unsigned nz = (unsigned)bt.nout;
+  const int64_t xs = sp.warp ? bt.ws : 0;   // Xt is the per-output Zt of a warped model
   float *part = reinterpret_cast<float *>(ws);
   int s = with_kernel(kern, sp.e > 0, [&](auto kk, auto ee) {
-    mll_grad_kernel<decltype(kk)::value, decltype(ee)::value><<<grid, 256, 0, st>>>(Xt, Ets, n, np, d, sp.De, hyp, Kinv, alpha,
-                                                                                       part, dZa, dZb);
+    mll_grad_kernel<decltype(kk)::value, decltype(ee)::value><<<dim3((unsigned)grid, 1, nz), 256, 0, st>>>(
+        Xt, Ets, n, np, d, sp.De, hyp, Kinv, alpha, part, dZa, dZb, xs, bt.ws);
   });
   if (s != HB_OK) return s;
-  mll_finish_kernel<<<1, 256, 0, st>>>(part, grid, n, sp, raw, hyp, alpha, scal, noise_guess, grad, loss);
+  mll_finish_kernel<<<dim3(1, 1, nz), 256, 0, st>>>(part, grid, n, sp, raw, hyp, alpha, scal, noise_guess, grad, loss, bt.ws);
   count_launches(2);
   if (sp.e > 0) {
     size_t off = (size_t)grid * (size_t)(3 * d + 3) * sizeof(float);
     off = (off + 255) / 256 * 256;
     float *gE = reinterpret_cast<float *>(reinterpret_cast<unsigned char *>(ws) + off);
-    const dim3 g2((unsigned)nt, (unsigned)nt);
+    const dim3 g2((unsigned)nt, (unsigned)nt, nz);
     s = with_kernel(kern, [&](auto kk) {
-      emb_rowgrad_kernel<decltype(kk)::value><<<g2, 256, 0, st>>>(Xt, Ets, n, np, d, sp.De, hyp, Kinv, alpha, gE, sp.warp ? 1 : 0);
+      emb_rowgrad_kernel<decltype(kk)::value><<<g2, 256, 0, st>>>(Xt, Ets, n, np, d, sp.De, hyp, Kinv, alpha, gE, sp.warp ? 1 : 0,
+                                                                  xs, bt.ws);
     });
     if (s != HB_OK) return s;
-    emb_scatter_kernel<<<sp.T, 256, 0, st>>>(gE, nt, n, np, sp, hyp, grad);
+    emb_scatter_kernel<<<dim3((unsigned)sp.T, 1, nz), 256, 0, st>>>(gE, nt, n, np, sp, hyp, grad, bt.ws);
     count_launches(2);
   }
   HB_LAUNCH_CHECK("mll_grad");
@@ -548,7 +581,10 @@ int launch_mll_grad(const float *Xt, const float *Ets, int64_t n, int64_t np, co
 
 // =============================================================================== small kernels
 // gpytorch Positive() / GreaterThan() constraints (gp.py:86, gp_util.py:46,55,57): raw (ModelSpec layout) -> hyp
-__global__ void transform_hypers_kernel(const float *__restrict__ raw, ModelSpec sp, float noise_lb, float *__restrict__ hyp) {
+__global__ void transform_hypers_kernel(const float *__restrict__ raw, ModelSpec sp, float noise_lb, float *__restrict__ hyp,
+                                        int64_t wss) {
+  raw += (int64_t)blockIdx.z * sp.P();
+  hyp = slice(hyp, wss, blockIdx.z);
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= sp.H()) return;
   float v;
@@ -561,9 +597,11 @@ __global__ void transform_hypers_kernel(const float *__restrict__ raw, ModelSpec
   hyp[i] = v;
 }
 
-int launch_transform_hypers(const float *raw, const ModelSpec &sp, float noise_lb, float *hyp, cudaStream_t st) {
+int launch_transform_hypers(const float *raw, const ModelSpec &sp, float noise_lb, float *hyp, cudaStream_t st,
+                            const Batch &bt) {
   if (sp.dtot() <= 0) return HB_ERR_INVALID;
-  transform_hypers_kernel<<<(int)ceil_div(sp.H(), 128), 128, 0, st>>>(raw, sp, noise_lb, hyp);
+  transform_hypers_kernel<<<dim3((unsigned)ceil_div(sp.H(), 128), 1, (unsigned)bt.nout), 128, 0, st>>>(raw, sp, noise_lb, hyp,
+                                                                                                        bt.ws);
   count_launches(1);
   HB_LAUNCH_CHECK("transform_hypers");
   return HB_OK;
@@ -589,7 +627,11 @@ int launch_psgld(float *raw, const float *grad, float *sq, int64_t p, float lr, 
 // rows dZa = d z / d a_k, dZb = d z / d b_k the gradient contraction needs (O(n d): a prologue of the epoch, the n^2 kernels
 // read Zt; the CANDIDATE side is warped inside the K* load stage, posterior.cu).
 __global__ void scale_zt_kernel(const float *__restrict__ Xt, int64_t np, ModelSpec sp, const float *__restrict__ hyp,
-                                float *__restrict__ Zt, float *__restrict__ dZa, float *__restrict__ dZb) {
+                                float *__restrict__ Zt, float *__restrict__ dZa, float *__restrict__ dZb, int64_t wss) {
+  hyp = slice(hyp, wss, blockIdx.z);   // (Xt is shared by the outputs of a batch)
+  Zt = slice(Zt, wss, blockIdx.z);
+  dZa = slice(dZa, wss, blockIdx.z);
+  dZb = slice(dZb, wss, blockIdx.z);
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (int64_t)sp.d * np) return;
   const int k = (int)(idx / np);
@@ -606,9 +648,10 @@ __global__ void scale_zt_kernel(const float *__restrict__ Xt, int64_t np, ModelS
 }
 
 int launch_scale_zt(const float *Xt, int64_t np, const ModelSpec &sp, const float *hyp, float *Zt, float *dZa, float *dZb,
-                    cudaStream_t st) {
+                    cudaStream_t st, const Batch &bt) {
   if (sp.d <= 0) return HB_OK;
-  scale_zt_kernel<<<(int)ceil_div((int64_t)sp.d * np, 256), 256, 0, st>>>(Xt, np, sp, hyp, Zt, dZa, dZb);
+  scale_zt_kernel<<<dim3((unsigned)ceil_div((int64_t)sp.d * np, 256), 1, (unsigned)bt.nout), 256, 0, st>>>(Xt, np, sp, hyp, Zt, dZa,
+                                                                                                          dZb, bt.ws);
   count_launches(1);
   HB_LAUNCH_CHECK("scale_zt");
   return HB_OK;
@@ -618,7 +661,11 @@ int launch_scale_zt(const float *Xt, int64_t np, const ModelSpec &sp, const floa
 //   Ets [De, NP]: Ets[q][i] = table_{c(q)}[Xe[i, c(q)]][q_loc(q)] / le   (pad columns zero)
 //   tab_s [T]   : tables / le   (the candidate side of the posterior gathers from it)
 __global__ void emb_gather_kernel(const float *__restrict__ tables, ModelSpec sp, int64_t n, int64_t np,
-                                  const float *__restrict__ hyp, float *__restrict__ Ets, float *__restrict__ tab_s) {
+                                  const float *__restrict__ hyp, float *__restrict__ Ets, float *__restrict__ tab_s, int64_t wss) {
+  tables += (int64_t)blockIdx.z * sp.P();   // raw rows are P apart; the categories sp.Xe are shared
+  hyp = slice(hyp, wss, blockIdx.z);
+  Ets = slice(Ets, wss, blockIdx.z);
+  tab_s = slice(tab_s, wss, blockIdx.z);
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const float inv = 1.0f / hyp[3 + sp.d];
   if (tab_s && idx < sp.T) tab_s[idx] = tables[idx] * inv;
@@ -631,10 +678,11 @@ __global__ void emb_gather_kernel(const float *__restrict__ tables, ModelSpec sp
 }
 
 int launch_emb_gather(const float *tables, const ModelSpec &sp, int64_t n, int64_t np, const float *hyp, float *Ets, float *tab_s,
-                      cudaStream_t st) {
+                      cudaStream_t st, const Batch &bt) {
   if (sp.e <= 0) return HB_OK;
   const int64_t work = sp.De * np > sp.T ? sp.De * np : sp.T;
-  emb_gather_kernel<<<(int)ceil_div(work, 256), 256, 0, st>>>(tables, sp, n, np, hyp, Ets, tab_s);
+  emb_gather_kernel<<<dim3((unsigned)ceil_div(work, 256), 1, (unsigned)bt.nout), 256, 0, st>>>(tables, sp, n, np, hyp, Ets, tab_s,
+                                                                                             bt.ws);
   count_launches(1);
   HB_LAUNCH_CHECK("emb_gather");
   return HB_OK;

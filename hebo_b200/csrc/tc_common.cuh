@@ -90,6 +90,12 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map
       "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c_inner), "r"(c_outer)
       : "memory");
 }
+__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c0, int c1, int c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
 // the same box written to the same shared offset `dst` of every CTA in `cta_mask`, each signalling its own mbarrier at `bar`
 __device__ __forceinline__ void tma_load_2d_multicast(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c_inner,
                                                       int c_outer, uint16_t cta_mask) {

@@ -54,7 +54,7 @@ template <int BN>
 __global__ void __launch_bounds__(384, 1)
 tcgemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
               const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
-              const TcTile *__restrict__ tiles, int ntiles, TcEpilogue epi) {
+              const TcTile *__restrict__ tiles, int ntiles, TcEpilogue epi, int64_t wss) {
   using C = Cfg<BN>;
   extern __shared__ unsigned char smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // SWIZZLE_128B tiles need 1024-byte alignment
@@ -83,10 +83,10 @@ tcgemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constan
         const uint32_t sb = base + stage * C::STAGE_BYTES;
         const uint32_t fb = full_bar + 8 * stage;
         mbar_expect_tx(fb, C::STAGE_BYTES);
-        tma_load_2d(sb, &map_a_hi, fb, tl.a_k0 + k0, tl.a_row);
-        tma_load_2d(sb + C::A_BYTES, &map_a_lo, fb, tl.a_k0 + k0, tl.a_row);
-        tma_load_2d(sb + 2 * C::A_BYTES, &map_b_hi, fb, tl.b_k0 + k0, tl.b_row);
-        tma_load_2d(sb + 2 * C::A_BYTES + C::B_BYTES, &map_b_lo, fb, tl.b_k0 + k0, tl.b_row);
+        tma_load_3d(sb, &map_a_hi, fb, tl.a_k0 + k0, tl.a_row, tl.out);
+        tma_load_3d(sb + C::A_BYTES, &map_a_lo, fb, tl.a_k0 + k0, tl.a_row, tl.out);
+        tma_load_3d(sb + 2 * C::A_BYTES, &map_b_hi, fb, tl.b_k0 + k0, tl.b_row, tl.out);
+        tma_load_3d(sb + 2 * C::A_BYTES + C::B_BYTES, &map_b_lo, fb, tl.b_k0 + k0, tl.b_row, tl.out);
         if (++stage == C::STAGES) {
           stage = 0;
           phase ^= 1u;
@@ -137,6 +137,9 @@ tcgemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constan
     mbar_arrive(empty_bar + 8 * prev);                         // tables never contain empty k ranges
 
     // epilogue from registers: thread holds rows rr and rr + 8, columns 8 j + cq, 8 j + cq + 1
+    float *const Cb = slice(epi.C, wss, tl.out);
+    float *const Cb_hi = slice(epi.C_hi, wss, tl.out), *const Cb_lo = slice(epi.C_lo, wss, tl.out);
+    float *const Ctb_hi = slice(epi.Ct_hi, wss, tl.out), *const Ctb_lo = slice(epi.Ct_lo, wss, tl.out);
     const int64_t rr = (int64_t)tl.c_row + half * 64 + w * 16 + (lane >> 2);
     const int cq = 2 * (lane & 3);
 #pragma unroll
@@ -149,7 +152,7 @@ tcgemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constan
         float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
         if (epi.mode == TC_EPI_RMW_SUB) {
           if (row >= epi.r0 && col >= epi.r0) {
-            float2 *p = reinterpret_cast<float2 *>(epi.C + row * epi.ldc + col);
+            float2 *p = reinterpret_cast<float2 *>(Cb + row * epi.ldc + col);
             float2 cv = *p;
             cv.x -= v0;
             cv.y -= v1;
@@ -159,20 +162,20 @@ tcgemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constan
         }
         v0 *= epi.sign;
         v1 *= epi.sign;
-        if (epi.C) *reinterpret_cast<float2 *>(epi.C + row * epi.ldc + col) = make_float2(v0, v1);
-        if (epi.C_hi || epi.Ct_hi) {
+        if (Cb) *reinterpret_cast<float2 *>(Cb + row * epi.ldc + col) = make_float2(v0, v1);
+        if (Cb_hi || Ctb_hi) {
           float h0, l0, h1, l1;
           split1(v0, h0, l0);
           split1(v1, h1, l1);
-          if (epi.C_hi) {
-            *reinterpret_cast<float2 *>(epi.C_hi + row * epi.ldc + col) = make_float2(h0, h1);
-            *reinterpret_cast<float2 *>(epi.C_lo + row * epi.ldc + col) = make_float2(l0, l1);
+          if (Cb_hi) {
+            *reinterpret_cast<float2 *>(Cb_hi + row * epi.ldc + col) = make_float2(h0, h1);
+            *reinterpret_cast<float2 *>(Cb_lo + row * epi.ldc + col) = make_float2(l0, l1);
           }
-          if (epi.Ct_hi) {
-            epi.Ct_hi[col * epi.ldct + row] = h0;
-            epi.Ct_lo[col * epi.ldct + row] = l0;
-            epi.Ct_hi[(col + 1) * epi.ldct + row] = h1;
-            epi.Ct_lo[(col + 1) * epi.ldct + row] = l1;
+          if (Ctb_hi) {
+            Ctb_hi[col * epi.ldct + row] = h0;
+            Ctb_lo[col * epi.ldct + row] = l0;
+            Ctb_hi[(col + 1) * epi.ldct + row] = h1;
+            Ctb_lo[(col + 1) * epi.ldct + row] = l1;
           }
         }
       }
@@ -180,14 +183,16 @@ tcgemm_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constan
   }
 }
 
-static bool make_map(CUtensorMap *m, const float *ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
+// [nout][rows][cols] with the outputs `slice` bytes apart; the box covers one output
+static bool make_map(CUtensorMap *m, const float *ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows, int nout,
+                     uint64_t slice) {
   EncodeTiledFn enc = encode_fn();
   if (!enc) return false;
-  cuuint64_t gdim[2] = {cols, rows};
-  cuuint64_t gstride[1] = {ld * sizeof(float)};
-  cuuint32_t box[2] = {(cuuint32_t)BK, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(ptr), gdim, gstride, box, estr,
+  cuuint64_t gdim[3] = {cols, rows, (cuuint64_t)nout};
+  cuuint64_t gstride[2] = {ld * sizeof(float), slice};
+  cuuint32_t box[3] = {(cuuint32_t)BK, box_rows, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float *>(ptr), gdim, gstride, box, estr,
              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
@@ -197,30 +202,37 @@ struct TableEntry {
   TcTile *dev = nullptr;
   int n = 0;
 };
-static std::map<uint64_t, TableEntry> g_tables;
+static std::map<TcTableKey, TableEntry> g_tables;
 
 }  // namespace tcg
 
-const TcTile *tc_table_lookup(uint64_t key, int *count) {
+const TcTile *tc_table_lookup(const TcTableKey &key, int *count) {
   auto it = tcg::g_tables.find(key);
   if (it == tcg::g_tables.end()) return nullptr;
   *count = it->second.n;
   return it->second.dev;
 }
 
-const TcTile *tc_table_store(uint64_t key, const std::vector<TcTile> &host, int *count) {
+const TcTile *tc_table_store(const TcTableKey &key, const std::vector<TcTile> &host, int *count) {
+  std::vector<TcTile> all;
+  all.reserve(host.size() * key.nout);
+  for (const TcTile &t : host)
+    for (int b = 0; b < key.nout; ++b) {
+      all.push_back(t);
+      all.back().out = b;
+    }
   tcg::TableEntry e;
-  e.n = (int)host.size();
+  e.n = (int)all.size();
   if (e.n == 0) return nullptr;
-  if (cudaMalloc(&e.dev, sizeof(TcTile) * host.size()) != cudaSuccess) return nullptr;
-  if (cudaMemcpy(e.dev, host.data(), sizeof(TcTile) * host.size(), cudaMemcpyHostToDevice) != cudaSuccess) return nullptr;
+  if (cudaMalloc(&e.dev, sizeof(TcTile) * all.size()) != cudaSuccess) return nullptr;
+  if (cudaMemcpy(e.dev, all.data(), sizeof(TcTile) * all.size(), cudaMemcpyHostToDevice) != cudaSuccess) return nullptr;
   tcg::g_tables[key] = e;
   *count = e.n;
   return e.dev;
 }
 
 int launch_tcgemm(const TcOperand &A, const TcOperand &B, int bn, const TcTile *tiles, int ntiles, const TcEpilogue &epi,
-                  cudaStream_t st) {
+                  cudaStream_t st, const Batch &bt) {
   using namespace tcg;
   if (ntiles <= 0) return HB_OK;
   if (bn != 128 && bn != 256) return HB_ERR_INVALID;
@@ -235,17 +247,22 @@ int launch_tcgemm(const TcOperand &A, const TcOperand &B, int bn, const TcTile *
     once.done[dev] = true;
   }
   const int num_sms = once.sms[dev];
+  if (bt.nout > 1 && (bt.ws <= 0 || bt.ws % 16 != 0)) return HB_ERR_INVALID;
+  // (one output: the outermost dimension has extent 1 and its stride is never applied; any legal value will do)
+  const uint64_t sl = bt.nout > 1 ? (uint64_t)bt.ws : (A.rows > B.rows ? A.rows : B.rows) * (A.ld > B.ld ? A.ld : B.ld) * 4;
+  const int no = bt.nout;
   CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
-  if (!make_map(&ma_hi, A.hi, A.rows, A.cols, A.ld, BM) || !make_map(&ma_lo, A.lo, A.rows, A.cols, A.ld, BM) ||
-      !make_map(&mb_hi, B.hi, B.rows, B.cols, B.ld, (uint32_t)bn) || !make_map(&mb_lo, B.lo, B.rows, B.cols, B.ld, (uint32_t)bn)) {
+  if (!make_map(&ma_hi, A.hi, A.rows, A.cols, A.ld, BM, no, sl) || !make_map(&ma_lo, A.lo, A.rows, A.cols, A.ld, BM, no, sl) ||
+      !make_map(&mb_hi, B.hi, B.rows, B.cols, B.ld, (uint32_t)bn, no, sl) ||
+      !make_map(&mb_lo, B.lo, B.rows, B.cols, B.ld, (uint32_t)bn, no, sl)) {
     set_error(cudaErrorUnknown, "cuTensorMapEncodeTiled");
     return HB_ERR_CUDA;
   }
   const int grid = ntiles < num_sms ? ntiles : num_sms;
   if (bn == 256)
-    tcgemm_kernel<256><<<grid, 384, Cfg<256>::SMEM_BYTES, st>>>(ma_hi, ma_lo, mb_hi, mb_lo, tiles, ntiles, epi);
+    tcgemm_kernel<256><<<grid, 384, Cfg<256>::SMEM_BYTES, st>>>(ma_hi, ma_lo, mb_hi, mb_lo, tiles, ntiles, epi, bt.ws);
   else
-    tcgemm_kernel<128><<<grid, 384, Cfg<128>::SMEM_BYTES, st>>>(ma_hi, ma_lo, mb_hi, mb_lo, tiles, ntiles, epi);
+    tcgemm_kernel<128><<<grid, 384, Cfg<128>::SMEM_BYTES, st>>>(ma_hi, ma_lo, mb_hi, mb_lo, tiles, ntiles, epi, bt.ws);
   count_launches(1);
   HB_LAUNCH_CHECK("tcgemm");
   return HB_OK;
@@ -253,7 +270,10 @@ int launch_tcgemm(const TcOperand &A, const TcOperand &B, int bn, const TcTile *
 
 // element-wise split of a sub-matrix: src/hi/lo may have different leading dimensions
 __global__ void split_region_kernel(const float *__restrict__ x, int64_t ldx, float *__restrict__ hi, float *__restrict__ lo,
-                                    int64_t ldo, int64_t rows, int64_t cols4) {
+                                    int64_t ldo, int64_t rows, int64_t cols4, int64_t wss) {
+  x = slice(x, wss, blockIdx.z);   // output (Batch)
+  hi = slice(hi, wss, blockIdx.z);
+  lo = slice(lo, wss, blockIdx.z);
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= rows * cols4) return;
   const int64_t r = i / cols4, c4 = i - r * cols4;
@@ -268,11 +288,12 @@ __global__ void split_region_kernel(const float *__restrict__ x, int64_t ldx, fl
 }
 
 int launch_split_region(const float *x, int64_t ldx, float *hi, float *lo, int64_t ldo, int64_t rows, int64_t cols,
-                        cudaStream_t st) {
+                        cudaStream_t st, const Batch &bt) {
   if (rows <= 0 || cols <= 0) return HB_OK;
   if (cols % 4 != 0) return HB_ERR_INVALID;
   const int64_t tot = rows * (cols / 4);
-  split_region_kernel<<<(unsigned)ceil_div(tot, 256), 256, 0, st>>>(x, ldx, hi, lo, ldo, rows, cols / 4);
+  split_region_kernel<<<dim3((unsigned)ceil_div(tot, 256), 1, (unsigned)bt.nout), 256, 0, st>>>(x, ldx, hi, lo, ldo, rows,
+                                                                                                cols / 4, bt.ws);
   count_launches(1);
   HB_LAUNCH_CHECK("split_region");
   return HB_OK;

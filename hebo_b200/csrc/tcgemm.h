@@ -4,7 +4,7 @@
 
 #include <vector>
 
-#include "common.cuh"
+#include "kernels.h"
 
 namespace hb {
 
@@ -13,6 +13,7 @@ struct TcTile {       // one 128 x BN output tile
   int b_row, b_k0;    // B box: rows [b_row, b_row+BN),  columns b_k0 + k
   int kbeg, kend;     // k range (multiples of 32, kend > kbeg)
   int c_row, c_col;   // output tile origin
+  int out;            // output of the batch (kernels.h Batch): every operand and C are read / written in its slice
 };
 
 enum { TC_EPI_STORE = 0, TC_EPI_RMW_SUB = 1 };
@@ -33,11 +34,29 @@ struct TcOperand {          // K-major fp32 matrix given as a hi/lo pair
   uint64_t rows, cols, ld;
 };
 
-const TcTile *tc_table_lookup(uint64_t key, int *count);
-const TcTile *tc_table_store(uint64_t key, const std::vector<TcTile> &host, int *count);
+// Tile tables are built once per (device, operation, padded size, operation parameters, outputs) and cached on the device.
+struct TcTableKey {
+  int dev, op;
+  int64_t np, p1, p2;
+  int nout;
+  bool operator<(const TcTableKey &o) const {
+    if (dev != o.dev) return dev < o.dev;
+    if (op != o.op) return op < o.op;
+    if (np != o.np) return np < o.np;
+    if (p1 != o.p1) return p1 < o.p1;
+    if (p2 != o.p2) return p2 < o.p2;
+    return nout < o.nout;
+  }
+};
+const TcTile *tc_table_lookup(const TcTableKey &key, int *count);
+// `host` lists the tiles of one output; the stored table repeats each of them for outputs 0 .. nout-1 in turn, so the
+// outputs' tiles are interleaved and the table keeps its longest-first order
+const TcTile *tc_table_store(const TcTableKey &key, const std::vector<TcTile> &host, int *count);
+// one persistent launch over the tiles of every output; the operands' TMA maps are 3-D with the output outermost (stride
+// bt.ws bytes), the epilogue offsets C by the tile's output times bt.ws
 int launch_tcgemm(const TcOperand &A, const TcOperand &B, int bn, const TcTile *tiles, int ntiles, const TcEpilogue &epi,
-                  cudaStream_t st);
+                  cudaStream_t st, const Batch &bt);
 int launch_split_region(const float *x, int64_t ldx, float *hi, float *lo, int64_t ldo, int64_t rows, int64_t cols,
-                        cudaStream_t st);
+                        cudaStream_t st, const Batch &bt);
 
 }  // namespace hb

@@ -267,6 +267,23 @@ class GP(BaseModel):
 
     def fit(self, Xc, Xe, y):
         lib = _lib.lib()
+        raw_dev, lang_dev = self._prepare_fit(Xc, Xe, y)
+        if raw_dev is None:
+            return
+        n, d, ws_bytes = self.n, self.d, self._ws.numel()
+        losses = (C.c_float * max(1, self.num_epochs))()
+        with torch.cuda.device(self.device):
+            st = lib.hb_fit_ex(_lib.ptr(self._XtT) if d > 0 else None, _lib.ptr(self._Xe_dev), _lib.ptr(self._y_dev), n, d,
+                               self._spec_ptr(), _lib.ptr(raw_dev), self.kern_id, _lib.ptr(self._nd_dev), float(self.noise_lb),
+                               float(self.noise_guess), float(self.lr), int(self.num_epochs), _lib.ptr(lang_dev), losses,
+                               _lib.ptr(self._ws), ws_bytes, _lib.stream_ptr())
+        self._finish_fit(raw_dev, np.array(losses[:self.num_epochs], dtype=np.float32), st)
+
+    def _prepare_fit(self, Xc, Xe, y, workspace: bool = True):
+        """Host side of fit() up to the device loop, in the reference's order of random draws (scalers, initial hypers,
+        Langevin draws).  Returns (raw_dev, lang_dev), or (None, None) when a torch optimizer has already fitted the model.
+        workspace=False: the caller binds the model to a slice of a batched workspace (MultiTaskModel)."""
+        lib = _lib.lib()
         Xc, Xe, y = filter_nan(Xc, Xe, y, "all")
         self.fit_scaler(Xc, Xe, y)
         Xt, Xe_t, yt = self.xtrans(Xc, Xe, y)
@@ -293,22 +310,21 @@ class GP(BaseModel):
         if self.noise_diag is not None:
             nd_dev = torch.as_tensor(self.noise_diag, dtype=torch.float32).to(dev).contiguous()
             assert nd_dev.numel() == n
-        ws_bytes = int(lib.hb_fit_workspace_bytes_ex(n, d, self._spec_ptr()))
-        self._ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        if workspace:
+            ws_bytes = int(lib.hb_fit_workspace_bytes_ex(n, d, self._spec_ptr()))
+            self._ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
         self._XtT, self._Xe_dev, self._y_dev, self._nd_dev = XtT, Xe_dev, y_dev, nd_dev
         if self.optimizer != "psgld":
             self._fit_torch_optimizer(raw_dev)
             self._fitted = True
-            return
+            return None, None
         lang = self._draw_langevin(P - (2 * d if self.warp_mode == 2 else 0), d)
         lang_dev = None if lang is None else self._expand_raw(lang).to(dev).contiguous()
-        losses = (C.c_float * max(1, self.num_epochs))()
-        with torch.cuda.device(dev):
-            st = lib.hb_fit_ex(_lib.ptr(XtT) if d > 0 else None, _lib.ptr(Xe_dev), _lib.ptr(y_dev), n, d, self._spec_ptr(),
-                               _lib.ptr(raw_dev), self.kern_id, _lib.ptr(nd_dev), float(self.noise_lb), float(self.noise_guess),
-                               float(self.lr), int(self.num_epochs), _lib.ptr(lang_dev), losses, _lib.ptr(self._ws), ws_bytes,
-                               _lib.stream_ptr())
-        self.losses = np.array(losses[:self.num_epochs], dtype=np.float32)
+        return raw_dev, lang_dev
+
+    def _finish_fit(self, raw_dev: torch.Tensor, losses: np.ndarray, st: int) -> None:
+        """After the device loop: losses, fit status, final hypers and the prediction state bound from the workspace."""
+        self.losses = losses
         for ep in range(self.num_epochs):
             if not np.isfinite(self.losses[ep]):
                 print("jitter is too large, give up fitting GP")
@@ -724,8 +740,44 @@ class MultiTaskModel(BaseModel):
         self.models = [GP(num_cont, num_enum, 1, **self.model_conf) for _ in range(num_out)]
 
     def fit(self, Xc, Xe, y):
+        if self._batched(y):
+            self._fit_batched(Xc, Xe, y)
+            return
         for i in range(self.num_out):
             self.models[i].fit(Xc, Xe, y[:, [i]])
+
+    def _batched(self, y) -> bool:
+        """One batched device fit (hb_fit_multi_ex) for all outputs: the pSGLD loop, at least two outputs, and the same
+        training rows for every output (the reference drops the non-finite rows of each output on its own, gp.py:75)."""
+        if self.num_out < 2 or self.num_out > _lib.HB_MAX_OUTPUTS or self.models[0].optimizer != "psgld":
+            return False
+        fin = torch.isfinite(torch.as_tensor(y))
+        return bool((fin == fin[:, :1]).all())
+
+    def _fit_batched(self, Xc, Xe, y):
+        """Host preparation of every output in output order (scalers, initial hypers, Langevin draws: the random streams of
+        the per-output loop), one device call that trains all outputs, then each model bound to its workspace slice."""
+        lib = _lib.lib()
+        models, B = self.models, self.num_out
+        prep = [m._prepare_fit(Xc, Xe, y[:, [i]], workspace=False) for i, m in enumerate(models)]
+        m0 = models[0]
+        n, d, E, dev = m0.n, m0.d, m0.num_epochs, m0.device
+        stride = int(lib.hb_fit_workspace_bytes_ex(n, d, m0._spec_ptr()))
+        ws = torch.empty(int(lib.hb_fit_multi_workspace_bytes(n, d, m0._spec_ptr(), B)), dtype=torch.uint8, device=dev)
+        Y = torch.stack([m._y_dev for m in models]).contiguous()
+        raw = torch.stack([r for r, _ in prep]).contiguous()
+        lang = None if prep[0][1] is None else torch.stack([l for _, l in prep]).contiguous()
+        losses = (C.c_float * (B * max(1, E)))()
+        status = (C.c_int32 * B)()
+        with torch.cuda.device(dev):
+            _lib.check(lib.hb_fit_multi_ex(_lib.ptr(m0._XtT) if d > 0 else None, _lib.ptr(m0._Xe_dev), _lib.ptr(Y), n, d,
+                                           m0._spec_ptr(), B, _lib.ptr(raw), m0.kern_id, _lib.ptr(m0._nd_dev),
+                                           float(m0.noise_lb), float(m0.noise_guess), float(m0.lr), int(E), _lib.ptr(lang),
+                                           losses, status, _lib.ptr(ws), ws.numel(), _lib.stream_ptr()), "hb_fit_multi")
+        L = np.array(losses[:B * E], dtype=np.float32).reshape(B, E)
+        for i, m in enumerate(models):
+            m._ws = ws[i * stride:(i + 1) * stride]
+            m._finish_fit(raw[i], L[i].copy(), int(status[i]))
 
     def predict(self, Xc, Xe=None):
         out = [m.predict(Xc, Xe) for m in self.models]

@@ -67,6 +67,9 @@ extern "C" {
  * workspace queries return -1).  The kernels stream features in 32-wide chunks, so shared memory does not grow with it. */
 #define HB_MAX_FEATURES    4096
 
+/* Most outputs one batched fit (hb_fit_multi_ex) trains together. */
+#define HB_MAX_OUTPUTS     32
+
 /* Model description beyond the numeric ARD default (HOST struct; NULL = numeric-only, ard_kernel=True). */
 typedef struct {
   int32_t        ard_kernel;  /* conf['ard_kernel'] (models/gp/gp.py:47, gp_util.py:45): 0 = one shared numeric lengthscale */
@@ -179,6 +182,21 @@ int32_t hb_fit_ex(const float *Xt, const int32_t *Xe, const float *y, int64_t n,
 int32_t hb_factorize_ex(const float *Xt, const int32_t *Xe, const float *y, int64_t n, int64_t d, const hb_model_spec_t *spec,
                         const float *raw, int32_t kern, const float *noise_diag, float noise_lb, float *jitter_used,
                         void *ws, int64_t ws_bytes, void *stream);
+/* ---- batched fit of several outputs that share one training set (MultiTaskModel) -----------------------------------
+ * Trains num_out (1 .. HB_MAX_OUTPUTS) independent single-output GPs on the same inputs Xt / Xe in one launch chain per
+ * epoch.  The workspace is num_out consecutive single-output workspaces: slice b starts at ws + b * stride with
+ * stride = hb_fit_workspace_bytes_ex(n, d, spec) and is, after the call, exactly what hb_fit_ex leaves in a workspace of
+ * its own -- hb_fit_state_ex, the posterior / sample / gradient calls and hb_factorize_ex work on it unchanged.
+ * Y [num_out, n] DEVICE targets; raw [num_out, P] DEVICE in/out; langevin [num_out, num_epochs, P] or NULL;
+ * losses HOST [num_out, num_epochs] out (may be NULL); status HOST [num_out] out: HB_OK or HB_ERR_NOT_PD (final
+ * factorisation of that output failed).  Each output runs the loop of hb_fit_ex on its own -- own epoch counter, own
+ * jitter ladder, own give-up -- and its results equal those of hb_fit_ex on its slice bit for bit.  noise_diag [n] is
+ * shared.  Returns HB_OK unless an argument is invalid or CUDA fails.  hb_fit_ex is the num_out = 1 case. */
+int64_t hb_fit_multi_workspace_bytes(int64_t n, int64_t d, const hb_model_spec_t *spec, int64_t num_out);
+int32_t hb_fit_multi_ex(const float *Xt, const int32_t *Xe, const float *Y, int64_t n, int64_t d, const hb_model_spec_t *spec,
+                        int64_t num_out, float *raw, int32_t kern, const float *noise_diag, float noise_lb, float noise_guess,
+                        float lr, int32_t num_epochs, const float *langevin, float *losses, int32_t *status, void *ws,
+                        int64_t ws_bytes, void *stream);
 /* One MLL forward + backward at `raw` (closure of models/gp/gp.py:111-116: loss = -mll(gp(X)) ; loss.backward()):
  * grad [P], loss [1], info [1] (Cholesky status, LAPACK style) are DEVICE outputs; jitter is added to the diagonal. */
 int32_t hb_mll_fwd_bwd(const float *Xt, const int32_t *Xe, const float *y, int64_t n, int64_t d, const hb_model_spec_t *spec,
