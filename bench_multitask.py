@@ -6,7 +6,7 @@ For every (num_out, n): d = 32, Matern-3/2, 100 pSGLD epochs on bench.py's synth
 per output, shifted so that the outputs differ).  The Langevin term is off so that every output runs all 100 epochs (with
 most lengthscale gradients vanishing, pSGLD's noise can random-walk a fit into an early give-up, sgld.py:64-70, which would
 time fewer epochs).  Per shape, after one warm-up fit of each path, the batched fit (one hb_fit_multi_ex call) and the
-loop (one hb_fit_ex per output) are timed alternately, --reps times each, with a host clock around calls that end in a
+loop (one single-output GP.fit per output) are timed alternately, --reps times each, with a host clock around calls that end in a
 device synchronisation; the JSON reports median, min and max.  Every timed pair is checked bit for bit: the raw hypers and
 losses of the batched fit equal those of the loop.  launches_per_epoch = kernel launches of a fit / 100 (hb_launch_count;
 the final per-output factorisation included).  Writes DIR/bench_multitask.json with the card name and power limit read in

@@ -180,15 +180,25 @@ struct HostStatus {
   int32_t pad;
   float batch[HB_MAX_OUTPUTS][FIT_BATCH * 2];   // per output: (info as float bits, loss) per replay slot
 };
-// one pinned status block per DEVICE (the header allows one in-flight call per process and device)
-static HostStatus *pinned_status() {
-  static HostStatus *p[MAX_DEVICES] = {};
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= MAX_DEVICES) return nullptr;
-  if (!p[dev]) {
-    if (cudaMallocHost(&p[dev], sizeof(HostStatus)) != cudaSuccess) p[dev] = nullptr;
+// host state of the fit on one DEVICE (the header allows one in-flight call per process and device): the pinned block the
+// status words are read back into, and the stream an epoch is captured on
+struct FitHost {
+  HostStatus *status = nullptr;
+  cudaStream_t capture = nullptr;
+};
+static int fit_host(FitHost *&h) {
+  static PerDevice once;
+  static FitHost per_dev[MAX_DEVICES];
+  bool fresh = false;
+  const int dev = once.slot(&fresh);
+  if (dev < 0) return HB_ERR_CUDA;
+  h = &per_dev[dev];
+  if (fresh) {
+    if (!h->status) HB_CUDA(cudaMallocHost(&h->status, sizeof(HostStatus)));
+    HB_CUDA(cudaStreamCreateWithFlags(&h->capture, cudaStreamNonBlocking));
+    once.done[dev] = true;
   }
-  return p[dev];
+  return HB_OK;
 }
 
 // conditional pSGLD (sgld.py:57-70): skipped on the device when the epoch's factorisation failed.  One block per output
@@ -288,6 +298,74 @@ static int enqueue_mll(const float *Xt, const float *y, int64_t n, int64_t np, c
 
 static float next_jitter(float j) { return j == 0.0f ? 1e-6f : j * 10.0f; }   // fp32 ladder of gp.py:104-110
 constexpr float JITTER_MAX = 1e3f;                                             // 100 * (jitter <= 10), gp.py:121
+
+// jitter ladder of gp.py:104-126: attempt(jitter, info) at jitter 0, 1e-6, 1e-5, .. until info is 0 (success) or -1 (hopeless,
+// see psgld_guarded_kernel: no jitter can help).  HB_ERR_NOT_PD once the next jitter exceeds JITTER_MAX (`jitter` = that one).
+template <class Attempt> static int jitter_ladder(Attempt &&attempt, float &jitter, int32_t &info) {
+  for (jitter = 0.0f; jitter <= JITTER_MAX; jitter = next_jitter(jitter)) {
+    const int s = attempt(jitter, info);
+    if (s != HB_OK || info == 0 || info == -1) return s;
+  }
+  return HB_ERR_NOT_PD;
+}
+
+// start of every entry point that trains or factorises in a fit workspace of num_out slices: checks the shared arguments,
+// builds the model description, carves slice 0 into w and uploads the categorical layout arrays + training categories into
+// every slice (each slice is a complete workspace); sp is bound to slice 0's copy
+static int open_fit_ws(const float *Xt, const int32_t *Xe, const float *y, int64_t n, int64_t d, const hb_model_spec_t *spec,
+                       const float *raw, int32_t kern, void *ws, int64_t ws_bytes, int64_t num_out, cudaStream_t st,
+                       ModelSpec &sp, FitWs &w) {
+  if (!y || !raw || !ws || n <= 0 || kern < 0 || kern > 2 || !build_spec(d, spec, sp) || (sp.d > 0 && !Xt)) return HB_ERR_INVALID;
+  w = carve_fit(ws, n, sp);
+  if (ws_bytes / num_out < (int64_t)w.total) return HB_ERR_INVALID;
+  if (sp.e <= 0) return HB_OK;
+  if (!Xe) return HB_ERR_INVALID;
+  std::vector<int32_t> m;
+  fill_meta_host(spec, sp, m);
+  for (int b = 0; b < num_out; ++b) {
+    FitWs wb = carve_fit(slice(ws, (int64_t)w.total, b), n, sp);
+    HB_CUDA(cudaMemcpyAsync(wb.meta, m.data(), m.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    HB_CUDA(cudaMemcpyAsync(wb.Xe, Xe, (size_t)n * sp.e * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  }
+  HB_CUDA(cudaStreamSynchronize(st));   // `m` is pageable host memory and dies with this frame
+  bind_meta(sp, w.meta, w.Xe);
+  return HB_OK;
+}
+
+// prediction state at `raw` in a carved and bound workspace: Gram + Cholesky through the jitter ladder (gp.py:140-157),
+// L^-1 with one Newton refinement, its fp16 split, alpha / log-det, the scaled features.  Built ONCE per fit, so it stays on
+// the FP32 SIMT pipe (round-to-nearest accumulation); the 3xTF32 tensor path (the tensor cores' fp32 accumulation is not
+// RN) serves the gradient epochs only.  HB_ERR_NOT_PD: the ladder gave up.
+static int factorize(const float *Xt, const float *y, int64_t n, const ModelSpec &sp, const float *raw, int kern,
+                     const float *noise_diag, float noise_lb, FitWs &w, HostStatus *hs, float *jitter_used, cudaStream_t st) {
+  const int64_t np = round_up(n, TILE);
+  int s = launch_transform_hypers(raw, sp, noise_lb, w.hyp, st);
+  if (s != HB_OK) return s;
+  float jitter = 0.0f;
+  s = jitter_ladder(
+      [&](float j, int32_t &info) -> int {   // info: hs->info (pinned)
+        const int r = factor_once(Xt, n, np, sp, raw, kern, noise_diag, j, w, st, nullptr);
+        if (r != HB_OK) return r;
+        HB_CUDA(cudaMemcpyAsync(&info, w.info, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        HB_CUDA(cudaStreamSynchronize(st));
+        return HB_OK;
+      },
+      jitter, hs->info);
+  if (jitter_used) *jitter_used = jitter;
+  if (s != HB_OK) return s;
+  s = launch_tri_inverse(w.L, np, w.Linv, w.tmp, st);
+  if (s != HB_OK) return s;
+  s = launch_linv_refine(w.L, w.Linv, np, w.tmp, w.tc.T_hi, st);   // Newton step, fp64 residual (scratch: tmp, T_hi)
+  if (s != HB_OK) return s;
+  // operands of the posterior's tensor-core contraction: two-level fp16 split (h0 in the Linv_hi buffer, h1 in the first
+  // half of the Linv_lo buffer, the power-of-two scale right after it)
+  s = launch_split_h16(w.Linv, np * np, reinterpret_cast<__half *>(w.Linv_hi), reinterpret_cast<__half *>(w.Linv_lo),
+                       w.Linv_lo + np * np / 2, st);
+  if (s != HB_OK) return s;
+  s = launch_solve_logdet(w.L, w.Linv, y, n, np, w.hyp, w.alpha, w.scal, w.solvews, st);
+  if (s != HB_OK) return s;
+  return launch_scale_zt(Xt, np, sp, w.hyp, w.Zt, w.dZa, w.dZb, st);   // (embedding rows of Zt: filled by factor_once's gather)
+}
 
 }  // namespace hb
 
@@ -434,62 +512,17 @@ int32_t hb_fit_state(void *ws, int64_t n, int64_t d, hb_fit_state_t *out) {
   return d <= 0 ? HB_ERR_INVALID : hb_fit_state_ex(ws, n, d, nullptr, out);
 }
 
-// uploads the categorical layout arrays + training categories into the workspace and binds the device pointers
-static int bind_spec_ws(const hb_model_spec_t *spec, ModelSpec &sp, FitWs &w, const int32_t *Xe, int64_t n, cudaStream_t st) {
-  if (sp.e <= 0) return HB_OK;
-  if (!Xe) return HB_ERR_INVALID;
-  std::vector<int32_t> m;
-  fill_meta_host(spec, sp, m);
-  HB_CUDA(cudaMemcpyAsync(w.meta, m.data(), m.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  HB_CUDA(cudaStreamSynchronize(st));   // `m` is pageable host memory and dies with this frame
-  if (Xe != w.Xe) HB_CUDA(cudaMemcpyAsync(w.Xe, Xe, (size_t)n * sp.e * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
-  bind_meta(sp, w.meta, w.Xe);
-  return HB_OK;
-}
-
 int32_t hb_factorize_ex(const float *Xt, const int32_t *Xe, const float *y, int64_t n, int64_t d, const hb_model_spec_t *spec,
                         const float *raw, int32_t kern, const float *noise_diag, float noise_lb, float *jitter_used, void *ws,
                         int64_t ws_bytes, void *stream) {
   ModelSpec sp;
-  if (!y || !raw || !ws || n <= 0 || kern < 0 || kern > 2 || !build_spec(d, spec, sp) || (sp.d > 0 && !Xt)) return HB_ERR_INVALID;
-  cudaStream_t st = (cudaStream_t)stream;
-  FitWs w = carve_fit(ws, n, sp);
-  if ((size_t)ws_bytes < w.total) return HB_ERR_INVALID;
-  const int64_t np = round_up(n, TILE);
-  HostStatus *hs = pinned_status();
-  if (!hs) return HB_ERR_CUDA;
-  int s = bind_spec_ws(spec, sp, w, Xe, n, st);
+  FitWs w;
+  int s = open_fit_ws(Xt, Xe, y, n, d, spec, raw, kern, ws, ws_bytes, 1, (cudaStream_t)stream, sp, w);
   if (s != HB_OK) return s;
-  s = launch_transform_hypers(raw, sp, noise_lb, w.hyp, st);
+  FitHost *fh = nullptr;
+  s = fit_host(fh);
   if (s != HB_OK) return s;
-  float jitter = 0.0f;
-  for (;;) {   // gp.py:140-157 jitter escalation of predict()
-    // the prediction state is built ONCE per fit: keep it on the FP32 SIMT pipe (round-to-nearest accumulation);
-    // the 3xTF32 tensor path (the tensor cores' fp32 accumulation is not RN) is used for the 100 gradient epochs only
-    s = factor_once(Xt, n, np, sp, raw, kern, noise_diag, jitter, w, st, nullptr);
-    if (s != HB_OK) return s;
-    HB_CUDA(cudaMemcpyAsync(&hs->info, w.info, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    HB_CUDA(cudaStreamSynchronize(st));
-    if (hs->info == 0) break;
-    jitter = next_jitter(jitter);
-    if (jitter > JITTER_MAX) {
-      if (jitter_used) *jitter_used = jitter;
-      return HB_ERR_NOT_PD;
-    }
-  }
-  if (jitter_used) *jitter_used = jitter;
-  s = launch_tri_inverse(w.L, np, w.Linv, w.tmp, st);
-  if (s != HB_OK) return s;
-  s = launch_linv_refine(w.L, w.Linv, np, w.tmp, w.tc.T_hi, st);   // Newton step, fp64 residual (scratch: tmp, T_hi)
-  if (s != HB_OK) return s;
-  // operands of the posterior's tensor-core contraction: two-level fp16 split (h0 in the Linv_hi buffer, h1 in the first
-  // half of the Linv_lo buffer, the power-of-two scale right after it)
-  s = launch_split_h16(w.Linv, np * np, reinterpret_cast<__half *>(w.Linv_hi), reinterpret_cast<__half *>(w.Linv_lo),
-                       w.Linv_lo + np * np / 2, st);
-  if (s != HB_OK) return s;
-  s = launch_solve_logdet(w.L, w.Linv, y, n, np, w.hyp, w.alpha, w.scal, w.solvews, st);
-  if (s != HB_OK) return s;
-  return launch_scale_zt(Xt, np, sp, w.hyp, w.Zt, w.dZa, w.dZb, st);   // (embedding rows of Zt: filled by factor_once's gather)
+  return factorize(Xt, y, n, sp, raw, kern, noise_diag, noise_lb, w, fh->status, jitter_used, (cudaStream_t)stream);
 }
 int32_t hb_factorize(const float *Xt, const float *y, int64_t n, int64_t d, const float *raw, int32_t kern,
                      const float *noise_diag, float noise_lb, float *jitter_used, void *ws, int64_t ws_bytes,
@@ -503,17 +536,13 @@ int32_t hb_factorize(const float *Xt, const float *y, int64_t n, int64_t d, cons
 int32_t hb_mll_fwd_bwd(const float *Xt, const int32_t *Xe, const float *y, int64_t n, int64_t d, const hb_model_spec_t *spec,
                        const float *raw, int32_t kern, const float *noise_diag, float noise_lb, float noise_guess, float jitter,
                        float *grad, float *loss, int32_t *info, void *ws, int64_t ws_bytes, void *stream) {
-  ModelSpec sp;
-  if (!y || !raw || !ws || !grad || !loss || !info || n <= 0 || kern < 0 || kern > 2 || !build_spec(d, spec, sp) ||
-      (sp.d > 0 && !Xt))
-    return HB_ERR_INVALID;
+  if (!grad || !loss || !info) return HB_ERR_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
-  FitWs w = carve_fit(ws, n, sp);
-  if ((size_t)ws_bytes < w.total) return HB_ERR_INVALID;
-  const int64_t np = round_up(n, TILE);
-  int s = bind_spec_ws(spec, sp, w, Xe, n, st);
+  ModelSpec sp;
+  FitWs w;
+  int s = open_fit_ws(Xt, Xe, y, n, d, spec, raw, kern, ws, ws_bytes, 1, st, sp, w);
   if (s != HB_OK) return s;
-  s = enqueue_mll(Xt, y, n, np, sp, raw, kern, noise_diag, noise_lb, noise_guess, jitter, w, st, nullptr, false);
+  s = enqueue_mll(Xt, y, n, round_up(n, TILE), sp, raw, kern, noise_diag, noise_lb, noise_guess, jitter, w, st, nullptr, false);
   if (s != HB_OK) return s;
   HB_CUDA(cudaMemcpyAsync(grad, w.grad, sp.P() * sizeof(float), cudaMemcpyDeviceToDevice, st));
   HB_CUDA(cudaMemcpyAsync(loss, w.loss, sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -531,25 +560,21 @@ int32_t hb_fit_multi_ex(const float *Xt, const int32_t *Xe, const float *Y, int6
                         int64_t num_out, float *raw, int32_t kern, const float *noise_diag, float noise_lb, float noise_guess,
                         float lr, int32_t num_epochs, const float *langevin, float *losses, int32_t *status, void *ws,
                         int64_t ws_bytes, void *stream) {
-  ModelSpec sp;
-  if (!Y || !raw || !ws || !status || n <= 0 || kern < 0 || kern > 2 || num_epochs < 0 || num_out < 1 ||
-      num_out > HB_MAX_OUTPUTS || !build_spec(d, spec, sp) || (sp.d > 0 && !Xt))
-    return HB_ERR_INVALID;
+  if (!status || num_epochs < 0 || num_out < 1 || num_out > HB_MAX_OUTPUTS) return HB_ERR_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
+  ModelSpec sp;
+  FitWs w;                                  // output 0; output b's workspace starts b * stride bytes later
+  int s = open_fit_ws(Xt, Xe, Y, n, d, spec, raw, kern, ws, ws_bytes, num_out, st, sp, w);
+  if (s != HB_OK) return s;
+  FitHost *fh = nullptr;
+  s = fit_host(fh);
+  if (s != HB_OK) return s;
+  HostStatus *hs = fh->status;
   const int B = (int)num_out;
-  FitWs w = carve_fit(ws, n, sp);          // output 0; output b's workspace starts b * stride bytes later
   const int64_t stride = (int64_t)w.total;
-  if (ws_bytes / B < stride) return HB_ERR_INVALID;
   const Batch all{B, stride};
   const int64_t np = round_up(n, TILE);
   const int64_t P = sp.P();
-  HostStatus *hs = pinned_status();
-  if (!hs) return HB_ERR_CUDA;
-  for (int b = B - 1; b >= 0; --b) {        // every slice is a complete workspace; sp ends up bound to slice 0's arrays
-    FitWs wb = carve_fit(slice(ws, stride, b), n, sp);
-    const int s = bind_spec_ws(spec, sp, wb, Xe, n, st);
-    if (s != HB_OK) return s;
-  }
   HB_CUDA(memset_slices(w.sq, 0, P * sizeof(float), all, st));
   HB_CUDA(memset_slices(w.info, 0, 4 * sizeof(int32_t), all, st));   // status, epoch counter, replay slot
   bool zeroed = false;                           // triangular complements of Linv / U zero-filled once per fit
@@ -577,52 +602,57 @@ int32_t hb_fit_multi_ex(const float *Xt, const int32_t *Xe, const float *Y, int6
   auto loss_out = [&](int b, int e, float v) {
     if (losses) losses[(int64_t)b * num_epochs + e] = v;
   };
-  // epoch ep[b] of output b with the jitter ladder of gp.py:104-126 on its own slice, one host synchronisation per attempt;
-  // the other outputs are not touched
+  // epoch ep[b] of output b through the jitter ladder on its own slice, one host synchronisation per attempt; the other
+  // outputs are not touched
   const Batch one{1, stride};
   auto slow_epoch = [&](int b) -> int {
     FitWs wb = carve_fit(slice(ws, stride, b), n, sp);
     float jitter = 0.0f;
-    for (;;) {
-      HB_CUDA(cudaMemsetAsync(wb.info + 2, 0, sizeof(int32_t), st));          // replay slot 0
-      const int s = enqueue_epoch(jitter, st, b, one);
-      if (s != HB_OK) return s;
-      HB_CUDA(cudaMemcpyAsync(hs->batch[b], wb.status, 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
-      HB_CUDA(cudaStreamSynchronize(st));
-      int32_t info;
-      memcpy(&info, &hs->batch[b][0], sizeof(info));
-      if (info == 0) {
-        loss_out(b, ep[b], hs->batch[b][1]);
-        ++ep[b];
-        return HB_OK;
-      }
-      if (info == -1) {            // hopeless (see psgld_guarded_kernel): this and every later epoch is given up
-        hopeless_from[b] = ep[b];
-        return HB_OK;
-      }
-      jitter = next_jitter(jitter);
-      if (jitter > JITTER_MAX) {   // "jitter is too large, give up fitting GP": epoch skipped, gp.py:121-122
-        loss_out(b, ep[b], INFINITY);
-        hs->set_epoch = ++ep[b];    // the device counter only advances on success
-        HB_CUDA(cudaMemcpyAsync(wb.info + 1, &hs->set_epoch, sizeof(int32_t), cudaMemcpyHostToDevice, st));
-        HB_CUDA(cudaStreamSynchronize(st));
-        return HB_OK;
-      }
+    int32_t info = 0;
+    const int s = jitter_ladder(
+        [&](float j, int32_t &inf) -> int {
+          HB_CUDA(cudaMemsetAsync(wb.info + 2, 0, sizeof(int32_t), st));   // replay slot 0
+          const int r = enqueue_epoch(j, st, b, one);
+          if (r != HB_OK) return r;
+          HB_CUDA(cudaMemcpyAsync(hs->batch[b], wb.status, 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
+          HB_CUDA(cudaStreamSynchronize(st));
+          memcpy(&inf, &hs->batch[b][0], sizeof(inf));
+          return HB_OK;
+        },
+        jitter, info);
+    if (s != HB_OK && s != HB_ERR_NOT_PD) return s;
+    if (s == HB_OK && info == -1) {   // hopeless (see psgld_guarded_kernel): this and every later epoch is given up
+      hopeless_from[b] = ep[b];
+      return HB_OK;
     }
-  };
-  // (info, loss) of the first `slots` replays of every output -> hs->batch
-  auto read_status = [&](int slots) -> int {
-    HB_CUDA(cudaMemcpy2DAsync(hs->batch, sizeof(hs->batch[0]), w.status, (size_t)stride, (size_t)slots * 2 * sizeof(float), B,
-                              cudaMemcpyDeviceToHost, st));
+    // trained, or "jitter is too large, give up fitting GP": epoch skipped, gp.py:121-122
+    loss_out(b, ep[b]++, s == HB_OK ? hs->batch[b][1] : INFINITY);
+    if (s == HB_OK) return HB_OK;
+    hs->set_epoch = ep[b];   // the device counter only advances on success
+    HB_CUDA(cudaMemcpyAsync(wb.info + 1, &hs->set_epoch, sizeof(int32_t), cudaMemcpyHostToDevice, st));
     HB_CUDA(cudaStreamSynchronize(st));
     return HB_OK;
   };
-  // outputs whose slot `slot` holds a failed attempt go through the ladder; returns whether any did
-  auto consume = [&](int slots, int &failed) -> int {
+  // R epochs of every active output at jitter 0 -- replays of the captured graph, or enqueued directly when there is none
+  // -- then one status read-back.  A failed factorisation leaves that output's hypers, RMS state and device epoch counter
+  // untouched (the pSGLD kernel is guarded), so the rest of the batch fails the same way for it; the host then runs that
+  // epoch through the output's ladder.  The other outputs are unaffected: each has its own counter and replay slots.
+  cudaGraphExec_t exec = nullptr;
+  long long launches_per_epoch = 0;
+  auto run_epochs = [&](int R, int &failed) -> int {
+    HB_CUDA(memset_slices(w.info + 2, 0, sizeof(int32_t), all, st));
+    for (int r = 0; r < R; ++r) {
+      if (exec) HB_CUDA(cudaGraphLaunch(exec, st));
+      else if (const int s = enqueue_epoch(0.0f, st, 0, all); s != HB_OK) return s;
+    }
+    if (exec) count_launches(launches_per_epoch * R);
+    HB_CUDA(cudaMemcpy2DAsync(hs->batch, sizeof(hs->batch[0]), w.status, (size_t)stride, (size_t)R * 2 * sizeof(float), B,
+                              cudaMemcpyDeviceToHost, st));
+    HB_CUDA(cudaStreamSynchronize(st));
     failed = 0;
     for (int b = 0; b < B; ++b) {
       if (!active(b)) continue;
-      const int need = slots < num_epochs - ep[b] ? slots : num_epochs - ep[b];
+      const int need = R < num_epochs - ep[b] ? R : num_epochs - ep[b];
       int done = 0;
       for (; done < need; ++done) {
         int32_t info;
@@ -631,7 +661,7 @@ int32_t hb_fit_multi_ex(const float *Xt, const int32_t *Xe, const float *Y, int6
         loss_out(b, ep[b] + done, hs->batch[b][2 * done + 1]);
       }
       ep[b] += done;
-      if (done < need) {   // epoch ep[b] needs jitter: the plain path with the ladder, then back to the batch
+      if (done < need) {
         failed = 1;
         const int s = slow_epoch(b);
         if (s != HB_OK) return s;
@@ -640,44 +670,27 @@ int32_t hb_fit_multi_ex(const float *Xt, const int32_t *Xe, const float *Y, int6
     return HB_OK;
   };
 
-  if (num_epochs > 0) {   // first epoch of every output on the plain path: it also builds every lazily created table / attribute
-    HB_CUDA(memset_slices(w.info + 2, 0, sizeof(int32_t), all, st));
-    int s = enqueue_epoch(0.0f, st, 0, all);
-    if (s == HB_OK) s = read_status(1);
-    int failed = 0;
-    if (s == HB_OK) s = consume(1, failed);
+  int failed = 0;
+  if (num_epochs > 0) {   // enqueued directly: the first epoch also builds every lazily created table / attribute
+    s = run_epochs(1, failed);
     if (s != HB_OK) return s;
   }
-  // Remaining epochs: capture ONE epoch of all outputs (jitter 0) into a CUDA graph and replay it FIT_BATCH times per host
-  // synchronisation.  A failed factorisation leaves that output's hypers, RMS state and device epoch counter untouched
-  // (the pSGLD kernel is guarded), so every later replay of the batch fails the same way for it; the host then runs that
-  // output's epoch through the jitter ladder on the plain path, on its own slice, and resumes.  The other outputs are
-  // unaffected: each has its own counter and replay slots.
-  cudaGraphExec_t exec = nullptr;
-  long long launches_per_epoch = 0;
-  if (num_epochs - 1 >= 4) {
-    static cudaStream_t gs_dev[MAX_DEVICES] = {};   // one capture stream per device
-    int cur_dev = 0;
-    cudaGetDevice(&cur_dev);
-    cudaStream_t &gs = gs_dev[(cur_dev >= 0 && cur_dev < MAX_DEVICES) ? cur_dev : 0];
-    if (!gs && cudaStreamCreateWithFlags(&gs, cudaStreamNonBlocking) != cudaSuccess) gs = nullptr;
-    if (gs) {
-      HB_CUDA(cudaStreamSynchronize(st));
-      cudaGraph_t graph = nullptr;
-      const long long before = g_launches.load();
-      if (cudaStreamBeginCapture(gs, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
-        const int s = enqueue_epoch(0.0f, gs, 0, all);
-        const cudaError_t e = cudaStreamEndCapture(gs, &graph);
-        if (s == HB_OK && e == cudaSuccess && graph && cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess) {
-          launches_per_epoch = g_launches.load() - before;
-        } else {
-          exec = nullptr;
-        }
-        if (graph) cudaGraphDestroy(graph);
+  if (num_epochs - 1 >= 4) {   // capture ONE epoch of all outputs into a CUDA graph for the remaining epochs
+    HB_CUDA(cudaStreamSynchronize(st));
+    cudaGraph_t graph = nullptr;
+    const long long before = g_launches.load();
+    if (cudaStreamBeginCapture(fh->capture, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
+      const int r = enqueue_epoch(0.0f, fh->capture, 0, all);
+      const cudaError_t e = cudaStreamEndCapture(fh->capture, &graph);
+      if (r == HB_OK && e == cudaSuccess && graph && cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess) {
+        launches_per_epoch = g_launches.load() - before;
+      } else {
+        exec = nullptr;
       }
-      g_launches = before;       // nothing was launched by the capture itself
-      (void)cudaGetLastError();  // a failed capture must not poison the plain path
+      if (graph) cudaGraphDestroy(graph);
     }
+    g_launches = before;       // nothing was launched by the capture itself
+    (void)cudaGetLastError();  // a failed capture leaves the direct enqueues to run the epochs
   }
   int batch = FIT_BATCH;
   for (;;) {
@@ -685,35 +698,20 @@ int32_t hb_fit_multi_ex(const float *Xt, const int32_t *Xe, const float *Y, int6
     for (int b = 0; b < B; ++b)
       if (active(b) && num_epochs - ep[b] > left) left = num_epochs - ep[b];
     if (left == 0) break;
-    if (!exec) {
-      for (int b = 0; b < B; ++b) {
-        if (!active(b)) continue;
-        const int s = slow_epoch(b);
-        if (s != HB_OK) return s;
-      }
-      continue;
-    }
     int R = batch < FIT_BATCH ? batch : FIT_BATCH;   // ramps 1, 2, 4, .. after a failure: a failing epoch wastes the rest
     if (R > left) R = left;                         // of its batch, and failures come in runs (gp.py:117-126 territory)
-    HB_CUDA(memset_slices(w.info + 2, 0, sizeof(int32_t), all, st));
-    for (int r = 0; r < R; ++r) HB_CUDA(cudaGraphLaunch(exec, st));
-    count_launches(launches_per_epoch * R);
-    int failed = 0;
-    int s = read_status(R);
-    if (s == HB_OK) s = consume(R, failed);
-    if (s != HB_OK) {
-      cudaGraphExecDestroy(exec);
-      return s;
-    }
+    s = run_epochs(R, failed);
+    if (s != HB_OK) break;
     batch = failed ? 1 : (2 * batch > FIT_BATCH ? FIT_BATCH : 2 * batch);
   }
   if (exec) cudaGraphExecDestroy(exec);
+  if (s != HB_OK) return s;
   // final prediction state of every output, once per fit
   for (int b = 0; b < B; ++b) {
     if (hopeless_from[b] >= 0)   // "jitter is too large, give up fitting GP" for that and every remaining epoch
       for (int e = hopeless_from[b]; e < num_epochs; ++e) loss_out(b, e, INFINITY);
-    const int s = hb_factorize_ex(Xt, w.Xe, Y + b * n, n, d, spec, raw + b * P, kern, noise_diag, noise_lb, nullptr,
-                                  slice(ws, stride, b), stride, stream);
+    FitWs wb = carve_fit(slice(ws, stride, b), n, sp);
+    s = factorize(Xt, Y + b * n, n, sp, raw + b * P, kern, noise_diag, noise_lb, wb, hs, nullptr, st);
     if (s != HB_OK && s != HB_ERR_NOT_PD) return s;
     status[b] = s;
   }

@@ -266,23 +266,14 @@ class GP(BaseModel):
         return Xe.to(self.device, torch.int32, non_blocking=True).contiguous()
 
     def fit(self, Xc, Xe, y):
-        lib = _lib.lib()
-        raw_dev, lang_dev = self._prepare_fit(Xc, Xe, y)
-        if raw_dev is None:
-            return
-        n, d, ws_bytes = self.n, self.d, self._ws.numel()
-        losses = (C.c_float * max(1, self.num_epochs))()
-        with torch.cuda.device(self.device):
-            st = lib.hb_fit_ex(_lib.ptr(self._XtT) if d > 0 else None, _lib.ptr(self._Xe_dev), _lib.ptr(self._y_dev), n, d,
-                               self._spec_ptr(), _lib.ptr(raw_dev), self.kern_id, _lib.ptr(self._nd_dev), float(self.noise_lb),
-                               float(self.noise_guess), float(self.lr), int(self.num_epochs), _lib.ptr(lang_dev), losses,
-                               _lib.ptr(self._ws), ws_bytes, _lib.stream_ptr())
-        self._finish_fit(raw_dev, np.array(losses[:self.num_epochs], dtype=np.float32), st)
+        if self.optimizer == "psgld":
+            _fit_psgld([self], Xc, Xe, y)
+        else:
+            self._fit_torch_optimizer(self._prepare_fit(Xc, Xe, y)[0])
 
-    def _prepare_fit(self, Xc, Xe, y, workspace: bool = True):
+    def _prepare_fit(self, Xc, Xe, y):
         """Host side of fit() up to the device loop, in the reference's order of random draws (scalers, initial hypers,
-        Langevin draws).  Returns (raw_dev, lang_dev), or (None, None) when a torch optimizer has already fitted the model.
-        workspace=False: the caller binds the model to a slice of a batched workspace (MultiTaskModel)."""
+        Langevin draws).  Returns (raw_dev, lang_dev); lang_dev is None without Langevin draws or for a torch optimizer."""
         lib = _lib.lib()
         Xc, Xe, y = filter_nan(Xc, Xe, y, "all")
         self.fit_scaler(Xc, Xe, y)
@@ -310,14 +301,9 @@ class GP(BaseModel):
         if self.noise_diag is not None:
             nd_dev = torch.as_tensor(self.noise_diag, dtype=torch.float32).to(dev).contiguous()
             assert nd_dev.numel() == n
-        if workspace:
-            ws_bytes = int(lib.hb_fit_workspace_bytes_ex(n, d, self._spec_ptr()))
-            self._ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
         self._XtT, self._Xe_dev, self._y_dev, self._nd_dev = XtT, Xe_dev, y_dev, nd_dev
         if self.optimizer != "psgld":
-            self._fit_torch_optimizer(raw_dev)
-            self._fitted = True
-            return None, None
+            return raw_dev, None
         lang = self._draw_langevin(P - (2 * d if self.warp_mode == 2 else 0), d)
         lang_dev = None if lang is None else self._expand_raw(lang).to(dev).contiguous()
         return raw_dev, lang_dev
@@ -351,6 +337,7 @@ class GP(BaseModel):
         Jitter ladder of gp.py:104-126: a step whose closure hits a non-PD matrix is retried with 10x the jitter."""
         lib = _lib.lib()
         n, d, dev = self.n, self.d, self.device
+        self._ws = torch.empty(int(lib.hb_fit_workspace_bytes_ex(n, d, self._spec_ptr())), dtype=torch.uint8, device=dev)
         lay = self._param_layout()
         p = torch.nn.Parameter(raw_dev, requires_grad=True)
         if str(self.optimizer).lower() == "lbfgs":
@@ -400,6 +387,7 @@ class GP(BaseModel):
             if self.verbose and ((ep + 1) % self.print_every == 0 or ep == 0):
                 print("After %d epochs, loss = %g" % (ep + 1, self.losses[ep]), flush=True)
         self.set_hypers(self._strip_raw(p.data.detach().cpu()))
+        self._fitted = True
 
     def set_hypers(self, raw: torch.Tensor):
         """Factorise at given raw hypers (parity tests / warm state); requires a previous fit() for the data."""
@@ -729,6 +717,33 @@ def register(name: str = "gp_b200", override_gp: bool = False) -> bool:
     return True
 
 
+def _fit_psgld(models, Xc, Xe, y) -> None:
+    """The pSGLD fit of models that share the training rows, model i on column i of y, in one device call (hb_fit_multi_ex).
+    Host preparation runs model by model (scalers, initial hypers, Langevin draws: the random streams of one fit per
+    output); each model is then bound to its slice of the workspace."""
+    lib = _lib.lib()
+    B = len(models)
+    prep = [m._prepare_fit(Xc, Xe, y[:, [i]]) for i, m in enumerate(models)]
+    m0 = models[0]
+    n, d, E, dev = m0.n, m0.d, m0.num_epochs, m0.device
+    stride = int(lib.hb_fit_workspace_bytes_ex(n, d, m0._spec_ptr()))
+    ws = torch.empty(int(lib.hb_fit_multi_workspace_bytes(n, d, m0._spec_ptr(), B)), dtype=torch.uint8, device=dev)
+    Y = torch.stack([m._y_dev for m in models]).contiguous()
+    raw = torch.stack([r for r, _ in prep]).contiguous()
+    lang = None if prep[0][1] is None else torch.stack([l for _, l in prep]).contiguous()
+    losses = (C.c_float * (B * max(1, E)))()
+    status = (C.c_int32 * B)()
+    with torch.cuda.device(dev):
+        _lib.check(lib.hb_fit_multi_ex(_lib.ptr(m0._XtT) if d > 0 else None, _lib.ptr(m0._Xe_dev), _lib.ptr(Y), n, d,
+                                       m0._spec_ptr(), B, _lib.ptr(raw), m0.kern_id, _lib.ptr(m0._nd_dev),
+                                       float(m0.noise_lb), float(m0.noise_guess), float(m0.lr), int(E), _lib.ptr(lang),
+                                       losses, status, _lib.ptr(ws), ws.numel(), _lib.stream_ptr()), "hb_fit_multi")
+    L = np.array(losses[:B * E], dtype=np.float32).reshape(B, E)
+    for i, m in enumerate(models):
+        m._ws = ws[i * stride:(i + 1) * stride]
+        m._finish_fit(raw[i], L[i].copy(), int(status[i]))
+
+
 class MultiTaskModel(BaseModel):
     """Multi-output wrapper: one single-output model per column of y (HEBO/hebo/models/model_factory.py:60-92), the
     building block of the reference's multi-objective / constrained optimisers (GeneralBO)."""
@@ -755,29 +770,7 @@ class MultiTaskModel(BaseModel):
         return bool((fin == fin[:, :1]).all())
 
     def _fit_batched(self, Xc, Xe, y):
-        """Host preparation of every output in output order (scalers, initial hypers, Langevin draws: the random streams of
-        the per-output loop), one device call that trains all outputs, then each model bound to its workspace slice."""
-        lib = _lib.lib()
-        models, B = self.models, self.num_out
-        prep = [m._prepare_fit(Xc, Xe, y[:, [i]], workspace=False) for i, m in enumerate(models)]
-        m0 = models[0]
-        n, d, E, dev = m0.n, m0.d, m0.num_epochs, m0.device
-        stride = int(lib.hb_fit_workspace_bytes_ex(n, d, m0._spec_ptr()))
-        ws = torch.empty(int(lib.hb_fit_multi_workspace_bytes(n, d, m0._spec_ptr(), B)), dtype=torch.uint8, device=dev)
-        Y = torch.stack([m._y_dev for m in models]).contiguous()
-        raw = torch.stack([r for r, _ in prep]).contiguous()
-        lang = None if prep[0][1] is None else torch.stack([l for _, l in prep]).contiguous()
-        losses = (C.c_float * (B * max(1, E)))()
-        status = (C.c_int32 * B)()
-        with torch.cuda.device(dev):
-            _lib.check(lib.hb_fit_multi_ex(_lib.ptr(m0._XtT) if d > 0 else None, _lib.ptr(m0._Xe_dev), _lib.ptr(Y), n, d,
-                                           m0._spec_ptr(), B, _lib.ptr(raw), m0.kern_id, _lib.ptr(m0._nd_dev),
-                                           float(m0.noise_lb), float(m0.noise_guess), float(m0.lr), int(E), _lib.ptr(lang),
-                                           losses, status, _lib.ptr(ws), ws.numel(), _lib.stream_ptr()), "hb_fit_multi")
-        L = np.array(losses[:B * E], dtype=np.float32).reshape(B, E)
-        for i, m in enumerate(models):
-            m._ws = ws[i * stride:(i + 1) * stride]
-            m._finish_fit(raw[i], L[i].copy(), int(status[i]))
+        _fit_psgld(self.models, Xc, Xe, y)
 
     def predict(self, Xc, Xe=None):
         out = [m.predict(Xc, Xe) for m in self.models]

@@ -41,10 +41,10 @@ def _problem(n, d, e, B, seed):
     return X, Xe, torch.stack(cols, 1)
 
 
-def _fit_both(d, e, n, B, conf, seed=0, Y=None):
+def _fit_both(d, e, n, B, conf, epochs, seed=0, Y=None):
     X, Xe, Yp = _problem(n, d, e, B, 100 + seed)
     Y = Yp if Y is None else Y
-    cf = dict(conf, num_epochs=30, noise_lb=8e-4)
+    cf = dict(conf, num_epochs=epochs, noise_lb=8e-4)
     np.random.seed(seed)
     torch.manual_seed(seed)
     mt = MultiTaskModel(d, len(e), B, **cf)
@@ -99,11 +99,13 @@ def _assert_equal_models(mt, singles, X, Xe):
     assert mu.shape == (m, mt.num_out) and var.shape == (m, mt.num_out)
 
 
-@pytest.mark.parametrize("family", list(FAMILIES))
-def test_batched_fit_equals_per_output_fits(family):
+# 30 epochs: replays of a captured epoch; 3 epochs: too short to capture, every epoch enqueued directly
+@pytest.mark.parametrize("family,epochs", [pytest.param(f, 30, id=f) for f in FAMILIES]
+                         + [pytest.param(f, 3, id=f"{f}-3epochs") for f in ("matern32", "mixed")])
+def test_batched_fit_equals_per_output_fits(family, epochs):
     d, n, B, conf = FAMILIES[family]
     e = conf.get("num_uniqs", [])
-    mt, singles, X, Xe, batched = _fit_both(d, e, n, B, conf)
+    mt, singles, X, Xe, batched = _fit_both(d, e, n, B, conf, epochs)
     assert batched
     _assert_equal_models(mt, singles, X, Xe)
 
@@ -113,12 +115,12 @@ def test_nan_rows_select_the_path_and_match_per_output_fits():
     X, _, Y = _problem(n, d, [], B, 7)
     same = Y.clone()
     same[[3, 50, 120]] = float("nan")              # the same rows in every column: one batched fit on the 197 others
-    mt, singles, X, _, batched = _fit_both(d, [], n, B, {}, seed=1, Y=same)
+    mt, singles, X, _, batched = _fit_both(d, [], n, B, {}, 30, seed=1, Y=same)
     assert batched and mt.models[0].n == n - 3
     _assert_equal_models(mt, singles, X, None)
     diff = Y.clone()
     diff[3, 0] = float("nan")                      # differing rows: each output keeps its own n, the per-output loop
-    mt, singles, X, _, batched = _fit_both(d, [], n, B, {}, seed=2, Y=diff)
+    mt, singles, X, _, batched = _fit_both(d, [], n, B, {}, 30, seed=2, Y=diff)
     assert not batched and mt.models[0].n == n - 1 and mt.models[1].n == n
     _assert_equal_models(mt, singles, X, None)
 
@@ -168,10 +170,12 @@ def _fit_multi(XtT, Y, raw, n, d, E, lang=None):
 
 
 # (0, -40): ~0 noise on the duplicated rows, the jitter ladder for output 1 only;
-# (3, -200): a lengthscale that underflows to 0, a hopeless output (every epoch given up) next to healthy ones
-@pytest.mark.parametrize("slot,value", [(0, -40.0), (3, -200.0)])
-def test_jitter_ladder_of_one_output_leaves_the_others_alone(slot, value):
-    B, E = 3, 12
+# (3, -200): a lengthscale that underflows to 0, a hopeless output (every epoch given up) next to healthy ones;
+# E = 12 replays a captured epoch, E = 3 is too short to capture and enqueues every epoch directly
+@pytest.mark.parametrize("slot,value,E", [pytest.param(s, v, E, id=f"{s}-{v}" + ("" if E == 12 else f"-E{E}"))
+                                          for E in (12, 3) for s, v in [(0, -40.0), (3, -200.0)]])
+def test_jitter_ladder_of_one_output_leaves_the_others_alone(slot, value, E):
+    B = 3
     XtT, Y, raw, n, d = _abi_inputs(B)
     raw[1, slot] = value
     g = torch.Generator().manual_seed(9)
