@@ -24,19 +24,26 @@ struct PairSmem {
 __device__ __forceinline__ int pr_row(int i) { return (i < 4 ? 0 : 60) + (threadIdx.x >> 4) * 4 + i; }
 __device__ __forceinline__ int pr_col(int j) { return (j < 4 ? 0 : 60) + (threadIdx.x & 15) * 4 + j; }
 
+// four consecutive feature values starting at column c, times inv; columns >= n are pad and staged as 0.  The pad columns
+// of Xt are whatever the caller left there (include/hebo_b200.h): NaN, Inf or a huge value would turn the zero weight of a
+// pad pair into NaN (0 * Inf) in the gradient contractions, so they must never reach the arithmetic.
+__device__ __forceinline__ float4 stage4(float4 v, int64_t c, int64_t n, float inv) {
+  return make_float4(c < n ? v.x * inv : 0.0f, c + 1 < n ? v.y * inv : 0.0f, c + 2 < n ? v.z * inv : 0.0f,
+                     c + 3 < n ? v.w * inv : 0.0f);
+}
+
 // stage rows [k0, k0+kc) of Xt for the two tiles, scaled by 1/lengthscale (ls == nullptr: rows are already scaled --
 // the embedding features Ets, gathered and divided by their lengthscale once per epoch)
-__device__ __forceinline__ void stage_chunk(PairSmem &sm, const float *__restrict__ Xt, int64_t np, int I, int J,
+__device__ __forceinline__ void stage_chunk(PairSmem &sm, const float *__restrict__ Xt, int64_t n, int64_t np, int I, int J,
                                             int k0, int kc, const float *__restrict__ ls) {
   for (int f = threadIdx.x; f < kc * (PT / 4); f += blockDim.x) {
     const int kk = f >> 5, c4 = f & 31;
     const float inv = ls ? 1.0f / ls[k0 + kk] : 1.0f;
-    float4 a = __ldg(reinterpret_cast<const float4 *>(Xt + (int64_t)(k0 + kk) * np + (int64_t)I * PT + c4 * 4));
-    float4 b = __ldg(reinterpret_cast<const float4 *>(Xt + (int64_t)(k0 + kk) * np + (int64_t)J * PT + c4 * 4));
-    a.x *= inv; a.y *= inv; a.z *= inv; a.w *= inv;
-    b.x *= inv; b.y *= inv; b.z *= inv; b.w *= inv;
-    *reinterpret_cast<float4 *>(&sm.xi[kk][c4 * 4]) = a;
-    *reinterpret_cast<float4 *>(&sm.xj[kk][c4 * 4]) = b;
+    const int64_t ci = (int64_t)I * PT + c4 * 4, cj = (int64_t)J * PT + c4 * 4;
+    const float4 a = __ldg(reinterpret_cast<const float4 *>(Xt + (int64_t)(k0 + kk) * np + ci));
+    const float4 b = __ldg(reinterpret_cast<const float4 *>(Xt + (int64_t)(k0 + kk) * np + cj));
+    *reinterpret_cast<float4 *>(&sm.xi[kk][c4 * 4]) = stage4(a, ci, n, inv);
+    *reinterpret_cast<float4 *>(&sm.xj[kk][c4 * 4]) = stage4(b, cj, n, inv);
   }
 }
 
@@ -86,7 +93,7 @@ __global__ void __launch_bounds__(256, EMB ? 1 : 2) gram_kernel(const float *__r
   for (int k0 = 0; k0 < d; k0 += DC) {
     const int kc = min(DC, d - k0);
     __syncthreads();
-    stage_chunk(sm, Xt, np, I, J, k0, kc, ls);
+    stage_chunk(sm, Xt, n, np, I, J, k0, kc, ls);
     __syncthreads();
     accum_sqdist(sm, kc, r2);
   }
@@ -99,7 +106,7 @@ __global__ void __launch_bounds__(256, EMB ? 1 : 2) gram_kernel(const float *__r
     for (int k0 = 0; k0 < De; k0 += DC) {
       const int kc = min(DC, De - k0);
       __syncthreads();
-      stage_chunk(sm, Ets, np, I, J, k0, kc, nullptr);
+      stage_chunk(sm, Ets, n, np, I, J, k0, kc, nullptr);
       __syncthreads();
       accum_sqdist(sm, kc, r2e);
     }
@@ -192,7 +199,7 @@ __global__ void __launch_bounds__(256, EMB ? 1 : 2) mll_grad_kernel(const float 
   for (int k0 = 0; k0 < d; k0 += DC) {
     const int kc = min(DC, d - k0);
     __syncthreads();
-    stage_chunk(sm, OUT(Xt, xs), np, I, J, k0, kc, ls);
+    stage_chunk(sm, OUT(Xt, xs), n, np, I, J, k0, kc, ls);
     __syncthreads();
     accum_sqdist(sm, kc, g);
   }
@@ -205,7 +212,7 @@ __global__ void __launch_bounds__(256, EMB ? 1 : 2) mll_grad_kernel(const float 
     for (int k0 = 0; k0 < De; k0 += DC) {
       const int kc = min(DC, De - k0);
       __syncthreads();
-      stage_chunk(sm, OUT(Ets, wss), np, I, J, k0, kc, nullptr);
+      stage_chunk(sm, OUT(Ets, wss), n, np, I, J, k0, kc, nullptr);
       __syncthreads();
       accum_sqdist(sm, kc, r2e);
     }
@@ -253,7 +260,7 @@ __global__ void __launch_bounds__(256, EMB ? 1 : 2) mll_grad_kernel(const float 
   for (int k0 = 0; k0 < d; k0 += DC) {
     const int kc = min(DC, d - k0);
     __syncthreads();
-    stage_chunk(sm, OUT(Xt, xs), np, I, J, k0, kc, ls);
+    stage_chunk(sm, OUT(Xt, xs), n, np, I, J, k0, kc, ls);
     __syncthreads();
     for (int kk = 0; kk < kc; ++kk) {
       const float4 a0 = *reinterpret_cast<const float4 *>(&sm.xi[kk][ty * 4]);
@@ -288,8 +295,9 @@ __global__ void __launch_bounds__(256, EMB ? 1 : 2) mll_grad_kernel(const float 
           const int kk = f >> 5, c4 = f & 31;
           const float *src = (kk < kc) ? OUT(Xt, xs) + (int64_t)(k0 + kk) * np : dZ + (int64_t)(k0 + kk - kc) * np;
           const int row = (kk < kc) ? kk : DC / 2 + (kk - kc);
-          *reinterpret_cast<float4 *>(&sm.xi[row][c4 * 4]) = __ldg(reinterpret_cast<const float4 *>(src + (int64_t)I * PT + c4 * 4));
-          *reinterpret_cast<float4 *>(&sm.xj[row][c4 * 4]) = __ldg(reinterpret_cast<const float4 *>(src + (int64_t)J * PT + c4 * 4));
+          const int64_t ci = (int64_t)I * PT + c4 * 4, cj = (int64_t)J * PT + c4 * 4;
+          *reinterpret_cast<float4 *>(&sm.xi[row][c4 * 4]) = stage4(__ldg(reinterpret_cast<const float4 *>(src + ci)), ci, n, 1.0f);
+          *reinterpret_cast<float4 *>(&sm.xj[row][c4 * 4]) = stage4(__ldg(reinterpret_cast<const float4 *>(src + cj)), cj, n, 1.0f);
         }
         __syncthreads();
         for (int kk = 0; kk < kc; ++kk) {
@@ -361,14 +369,14 @@ __global__ void __launch_bounds__(256, 1) emb_rowgrad_kernel(const float *__rest
   for (int k0 = 0; k0 < d; k0 += DC) {
     const int kc = min(DC, d - k0);
     __syncthreads();
-    stage_chunk(sm, Xt, np, I, J, k0, kc, ls);
+    stage_chunk(sm, Xt, n, np, I, J, k0, kc, ls);
     __syncthreads();
     accum_sqdist(sm, kc, g);
   }
   for (int k0 = 0; k0 < De; k0 += DC) {
     const int kc = min(DC, De - k0);
     __syncthreads();
-    stage_chunk(sm, Ets, np, I, J, k0, kc, nullptr);
+    stage_chunk(sm, Ets, n, np, I, J, k0, kc, nullptr);
     __syncthreads();
     accum_sqdist(sm, kc, r2e);
   }
@@ -392,7 +400,7 @@ __global__ void __launch_bounds__(256, 1) emb_rowgrad_kernel(const float *__rest
   for (int k0 = 0; k0 < De; k0 += DC) {
     const int kc = min(DC, De - k0);
     __syncthreads();
-    stage_chunk(sm, Ets, np, I, J, k0, kc, nullptr);
+    stage_chunk(sm, Ets, n, np, I, J, k0, kc, nullptr);
     __syncthreads();
     for (int kk = 0; kk < kc; ++kk) {
       const float4 a0 = *reinterpret_cast<const float4 *>(&sm.xi[kk][ty * 4]);

@@ -115,7 +115,10 @@ int32_t hb_median_pdist(const float *Xt, int64_t n, int64_t d, const int32_t *id
 
 /* ---- Gram matrix  (replaces GPyTorchModel.forward -> self.cov(x_all), models/gp/gp.py:203-207,
  * kernel built at models/gp/gp_util.py:39-59) -----------------------------------------------
- * Xt       [d, NP] TRANSPOSED MinMax-scaled training inputs (column i = point i; pad columns ignored)
+ * Xt       [d, NP] TRANSPOSED MinMax-scaled training inputs (column i = point i; pad columns ignored).  The same holds
+ *          for the Xt of hb_mll_grad, hb_fit, hb_fit_ex, hb_fit_multi_ex, hb_mll_fwd_bwd, hb_factorize and
+ *          hb_factorize_ex: the pad columns may hold anything, NaN and Inf included, and no result depends on them or on
+ *          what the workspace held before the call.
  * K        [NP, NP] out: lower triangle (incl. diagonal) of s*k(X,X) + (sigma_n^2 + jitter [+ noise_diag_i]) I;
  *          pad block = identity.  The strict upper triangle of off-diagonal tiles is not written.
  * noise_diag  [n] or NULL: per-row extra noise (BASELINE config 4 "heteroscedastic"; no reference). */

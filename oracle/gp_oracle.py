@@ -245,15 +245,20 @@ def neg_mll_autograd(Xt, yt, hp: Hypers, kind="matern32", noise_guess=0.01, nois
     return loss.detach(), g
 
 
-def neg_mll_closed_form(Xt, yt, hp: Hypers, kind="matern32", noise_guess=0.01, noise_diag=None
+def neg_mll_closed_form(Xt, yt, hp: Hypers, kind="matern32", noise_guess=0.01, noise_diag=None, block: int = 128
                         ) -> Tuple[torch.Tensor, torch.Tensor, dict]:
     """Same loss, gradient by the closed forms of SURVEY Appendix A (what the CUDA path implements):
-    alpha = Khat^-1 r ; W = alpha alpha^T - Khat^-1 ; d(data)/dtheta = 1/2 tr(W dKhat/dtheta)."""
+    alpha = Khat^-1 r ; W = alpha alpha^T - Khat^-1 ; d(data)/dtheta = 1/2 tr(W dKhat/dtheta).
+
+    The pairwise differences are formed ``block`` rows at a time, so memory stays O(n^2 + block n d): the full
+    [n, n, d] difference tensor would be 4.6 GB in fp64 at n = 4224, d = 32."""
     n, d = Xt.shape
     dt = Xt.dtype
     s, sn2, ls, c = hp.outputscale, hp.noise, hp.lengthscale, hp.mean
     Z = Xt / ls
-    r2 = scaled_sqdist(Z, Z)
+    r2 = torch.empty(n, n, dtype=dt)
+    for i0 in range(0, n, block):
+        r2[i0:i0 + block] = scaled_sqdist(Z[i0:i0 + block], Z)
     k = kernel_from_sqdist(r2, kind)
     Khat = s * k + torch.eye(n, dtype=dt) * sn2
     if noise_diag is not None:
@@ -277,8 +282,11 @@ def neg_mll_closed_form(Xt, yt, hp: Hypers, kind="matern32", noise_guess=0.01, n
     else:
         h = k
     G = W * h * s                                            # [n,n]
-    dZ2 = (Z[:, None, :] - Z[None, :, :]) ** 2               # [n,n,d] (small n only)
-    g_ls = 0.5 * torch.einsum("ij,ijk->k", G, dZ2) / ls
+    g_ls = torch.zeros(d, dtype=dt)
+    for i0 in range(0, n, block):
+        dZ2 = (Z[i0:i0 + block, None, :] - Z[None, :, :]) ** 2   # [block,n,d]
+        g_ls = g_ls + torch.einsum("ij,ijk->k", G[i0:i0 + block], dZ2)
+    g_ls = 0.5 * g_ls / ls
     g_s = 0.5 * (W * k).sum()
     g_n = 0.5 * torch.diagonal(W).sum()
     g_c = alpha.sum()

@@ -66,6 +66,12 @@ def test_closed_form_gradient_matches_autograd(kind):
         l2, g2, _ = O.neg_mll_closed_form(f.Xt, f._yt, hp, kind, noise_diag=noise_diag)
         assert abs(float(l1 - l2)) < 1e-12
         assert float((g1 - g2).abs().max()) < 1e-11
+        # the row-blocked contraction (7 rows per block, last block short) against one block over all rows
+        l3, g3, _ = O.neg_mll_closed_form(f.Xt, f._yt, hp, kind, noise_diag=noise_diag, block=7)
+        l4, g4, _ = O.neg_mll_closed_form(f.Xt, f._yt, hp, kind, noise_diag=noise_diag, block=f.Xt.shape[0])
+        assert abs(float(l3 - l1)) < 1e-12 and abs(float(l3 - l4)) < 1e-12
+        assert float((g3 - g1).abs().max()) < 1e-11
+        assert float((g3 - g4).abs().max()) < 1e-12
 
 
 def test_psgld_matches_torch_rmsprop_plus_langevin():
