@@ -2,5 +2,6 @@
 from . import _lib  # noqa: F401
 from .gp import GP, B200GP, MultiTaskModel, register  # noqa: F401
 from .acq import MACE, FusedMACE, Mean, Sigma, LCB  # noqa: F401
+from .embedding import HEBO_Embedding, MACE_Embedding  # noqa: F401
 
-__all__ = ["GP", "B200GP", "MultiTaskModel", "MACE", "FusedMACE", "Mean", "Sigma", "LCB", "register"]
+__all__ = ["GP", "B200GP", "MultiTaskModel", "MACE", "FusedMACE", "Mean", "Sigma", "LCB", "register", "HEBO_Embedding", "MACE_Embedding"]

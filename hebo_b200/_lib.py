@@ -93,6 +93,9 @@ SIGNATURES = {
     "hb_nsga2_survive": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp]),
     "hb_nsga2_workspace_bytes": (_i64, [_i64, _i64]),
     "hb_nsga2_survive_ex": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
+    "hb_nsga2_survive_cv": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
+    "hb_embed_violation_workspace_bytes": (_i64, [_i64, _i64, _i64]),
+    "hb_embed_violation": (_i32, [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _vp]),
     "hb_front_merge_workspace_bytes": (_i64, [_i64, _i64]),
     "hb_front_pack": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp]),
     "hb_front_merge": (_i32, [_vp, _i64, _i64, _vp, _vp, _i64, _vp]),

@@ -849,7 +849,8 @@ int32_t hb_nsga2_survive(const float *X, const float *F, const float *C, const f
                          float *X_next, float *F_next, float *Xc_next, int32_t *Xe_next, void *stream) {
   if (!X || !F || !C || !FC || !X_next || !F_next || (d > 0 && !Xc_next) || (D > d && !Xe_next)) return HB_ERR_INVALID;
   if (pop > 256) return HB_ERR_INVALID;   // the workspace-free entry keeps the single-CTA limit
-  return launch_nsga_survive(X, F, C, FC, pop, D, d, X_next, F_next, Xc_next, Xe_next, nullptr, 0, (cudaStream_t)stream);
+  return launch_nsga_survive(X, F, nullptr, C, FC, nullptr, pop, D, d, X_next, F_next, nullptr, Xc_next, Xe_next, nullptr, 0,
+                             (cudaStream_t)stream);
 }
 
 int64_t hb_nsga2_workspace_bytes(int64_t pop, int64_t D) { return nsga_survive_ws_query(pop, D); }
@@ -858,7 +859,25 @@ int32_t hb_nsga2_survive_ex(const float *X, const float *F, const float *C, cons
                             int64_t d, float *X_next, float *F_next, float *Xc_next, int32_t *Xe_next, void *ws,
                             int64_t ws_bytes, void *stream) {
   if (!X || !F || !C || !FC || !X_next || !F_next || (d > 0 && !Xc_next) || (D > d && !Xe_next)) return HB_ERR_INVALID;
-  return launch_nsga_survive(X, F, C, FC, pop, D, d, X_next, F_next, Xc_next, Xe_next, ws, ws_bytes, (cudaStream_t)stream);
+  return launch_nsga_survive(X, F, nullptr, C, FC, nullptr, pop, D, d, X_next, F_next, nullptr, Xc_next, Xe_next, ws, ws_bytes,
+                             (cudaStream_t)stream);
+}
+
+int32_t hb_nsga2_survive_cv(const float *X, const float *F, const float *G, const float *C, const float *FC, const float *GC,
+                            int64_t pop, int64_t D, int64_t d, float *X_next, float *F_next, float *G_next, float *Xc_next,
+                            int32_t *Xe_next, void *ws, int64_t ws_bytes, void *stream) {
+  if (!X || !F || !G || !C || !FC || !GC || !X_next || !F_next || !G_next || (d > 0 && !Xc_next) || (D > d && !Xe_next))
+    return HB_ERR_INVALID;
+  return launch_nsga_survive(X, F, G, C, FC, GC, pop, D, d, X_next, F_next, G_next, Xc_next, Xe_next, ws, ws_bytes,
+                             (cudaStream_t)stream);
+}
+
+int64_t hb_embed_violation_workspace_bytes(int64_t m, int64_t e, int64_t D) { return embed_violation_ws_query(m, e, D); }
+
+int32_t hb_embed_violation(const float *Y, int64_t m, int64_t e, const float *B, int64_t D, float *G, void *ws, int64_t ws_bytes,
+                           void *stream) {
+  if (!Y || !B || !G || !ws) return HB_ERR_INVALID;
+  return launch_embed_violation(Y, m, e, B, D, G, ws, ws_bytes, (cudaStream_t)stream);
 }
 
 }  // extern "C"

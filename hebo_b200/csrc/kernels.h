@@ -173,9 +173,15 @@ int launch_nsga_init(float *X, int64_t P, int64_t D, int64_t d, const int32_t *k
 int launch_nsga_mate(const float *X, int64_t P, int64_t D, int64_t d, const int32_t *kind, const float *lb, const float *ub,
                      const float *fixed, uint64_t seed, int gen, float *C, float *Cc, int32_t *Ce, cudaStream_t st);
 // survival of the 2P merged rows: one CTA for 2P <= 512 (ws may be NULL), the cooperative multi-CTA kernel up to
-// P = 16384 (ws_bytes >= nsga_survive_ws_query(P, D))
+// P = 16384 (ws_bytes >= nsga_survive_ws_query(P, D)).  G / GC: constraint of the population / offspring (both NULL:
+// unconstrained); Gn (may be NULL): the survivors' constraint.
 int64_t nsga_survive_ws_query(int64_t P, int64_t D);
-int launch_nsga_survive(const float *X, const float *F, const float *C, const float *FC, int64_t P, int64_t D, int64_t d,
-                        float *Xn, float *Fn, float *Xcn, int32_t *Xen, void *ws, int64_t ws_bytes, cudaStream_t st);
+int launch_nsga_survive(const float *X, const float *F, const float *G, const float *C, const float *FC, const float *GC,
+                        int64_t P, int64_t D, int64_t d, float *Xn, float *Fn, float *Gn, float *Xcn, int32_t *Xen, void *ws,
+                        int64_t ws_bytes, cudaStream_t st);
+// embed.cu: G[i] = sum_j max(|sum_k Y[i,k] B[k,j]| - 1, 0)
+int64_t embed_violation_ws_query(int64_t m, int64_t e, int64_t D);
+int launch_embed_violation(const float *Y, int64_t m, int64_t e, const float *B, int64_t D, float *G, void *ws, int64_t ws_bytes,
+                           cudaStream_t st);
 
 }  // namespace hb

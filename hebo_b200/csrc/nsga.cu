@@ -144,6 +144,16 @@ __global__ void nsga_mate_kernel(const float *__restrict__ X, int P, int D, int 
 //    index, the two end positions become +inf, an interior member adds (f[next] - f[prev]) / (fmax - fmin) when
 //    fmax > fmin and fmax - fmin is finite; the `need` members with the largest crowding survive, ties by lower index;
 //  * output: survivors in ascending merged-row order, F_next holds the sanitised (duplicate -> +inf) objectives.
+// With a constraint column G (hb_nsga2_survive_cv; pymoo's survival with infeasible filtering as EvolutionOpt runs it
+// with n_constr = 1, evolution_optimizer.py:82,105,135-140 -- recalled, not checked against pymoo):
+//  * a merged row is feasible iff G <= 0; a non-finite G becomes +inf; a duplicate child gets G = +inf as well;
+//  * nf >= P feasible rows: only the feasible rows enter the rank-and-crowding survival above, unchanged;
+//  * nf < P: every feasible row survives, the other P - nf slots go to infeasible rows in ascending G, ties by the lower
+//    merged index;
+//  * output order as above; G_next holds the survivors' sanitised G.
+// Without G (hb_nsga2_survive_ex) every row is feasible with G = 0, duplicates included, which is the rule above.  G = 0
+// everywhere gives the same survivors unless the cut reaches the front of all-+inf rows that holds a duplicate child:
+// with G the duplicate is infeasible and leaves that front.
 __device__ __forceinline__ float sanitize_obj(float v) { return isfinite(v) ? v : INFINITY; }
 
 // a dominates b (minimisation): all <=, at least one <
@@ -174,11 +184,12 @@ __device__ __forceinline__ const float *merged_row(const float *X, const float *
 
 constexpr int NSGA_MAX = 512;
 __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__restrict__ X, const float *__restrict__ F,
-                                                                const float *__restrict__ C, const float *__restrict__ FC,
+                                                                const float *__restrict__ G, const float *__restrict__ C,
+                                                                const float *__restrict__ FC, const float *__restrict__ GC,
                                                                 int P, int D, int d, float *__restrict__ Xn,
-                                                                float *__restrict__ Fn, float *__restrict__ Xcn,
-                                                                int32_t *__restrict__ Xen) {
-  __shared__ float f[NSGA_MAX][3];
+                                                                float *__restrict__ Fn, float *__restrict__ Gn,
+                                                                float *__restrict__ Xcn, int32_t *__restrict__ Xen) {
+  __shared__ float f[NSGA_MAX][3], g[NSGA_MAX];
   __shared__ int ndom[NSGA_MAX], rank[NSGA_MAX], order[NSGA_MAX];
   __shared__ float crowd[NSGA_MAX];
   __shared__ unsigned char infront[NSGA_MAX], keep[NSGA_MAX];
@@ -188,6 +199,7 @@ __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__r
   if (on) {
     const float *src = i < P ? F + (int64_t)i * 3 : FC + (int64_t)(i - P) * 3;
     for (int k = 0; k < 3; ++k) f[i][k] = sanitize_obj(src[k]);   // NaN / inf objectives never survive (evolution_optimizer.py:104 F)
+    g[i] = G ? sanitize_obj(i < P ? G[i] : GC[i - P]) : 0.0f;      // evolution_optimizer.py:105 G
     rank[i] = -1;
     keep[i] = 0;
     infront[i] = 0;
@@ -198,21 +210,50 @@ __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__r
     const float *me = C + (int64_t)(i - P) * D;
     bool dup = false;
     for (int j = 0; j < i && !dup; ++j) dup = same_row(merged_row(X, C, P, D, j), me, D);
-    if (dup) f[i][0] = f[i][1] = f[i][2] = INFINITY;
+    if (dup) {
+      f[i][0] = f[i][1] = f[i][2] = INFINITY;
+      if (G) g[i] = INFINITY;
+    }
   }
-  __syncthreads();
-  if (on) {
+  // ---- stable compaction of the kept rows into the next population
+  auto compact = [&]() {
+    if (on && keep[i]) {
+      int dst = 0;
+      for (int j = 0; j < i; ++j) dst += keep[j];
+      const float *src = merged_row(X, C, P, D, i);
+      float *row = Xn + (int64_t)dst * D;
+      for (int k = 0; k < D; ++k) row[k] = src[k];
+      for (int k = 0; k < 3; ++k) Fn[(int64_t)dst * 3 + k] = f[i][k];
+      if (Gn) Gn[dst] = g[i];
+      split_row(src, d, D - d, Xcn + (int64_t)dst * d, Xen + (int64_t)dst * (D - d));
+    }
+  };
+  const bool live = on && g[i] <= 0.0f;   // feasible
+  const int nf = __syncthreads_count(live);
+  if (nf < P) {
+    // ---- too few feasible rows: all of them survive, then the least infeasible ones (ascending G, ties by index)
+    if (on) {
+      int better = 0;
+      if (!live)
+        for (int j = 0; j < N; ++j) better += (!(g[j] <= 0.0f) && before_asc(g[j], j, g[i], i)) ? 1 : 0;
+      keep[i] = (live || better < P - nf) ? 1 : 0;
+    }
+    __syncthreads();
+    compact();
+    return;
+  }
+  if (live) {
     int c = 0;
-    for (int j = 0; j < N; ++j) c += dominates3(f[j][0], f[j][1], f[j][2], f[i][0], f[i][1], f[i][2]) ? 1 : 0;
+    for (int j = 0; j < N; ++j) c += (g[j] <= 0.0f && dominates3(f[j][0], f[j][1], f[j][2], f[i][0], f[i][1], f[i][2])) ? 1 : 0;
     ndom[i] = c;
   }
   if (i == 0) { cum = 0; r_cut = -1; need = 0; }
   __syncthreads();
-  // ---- front peeling until P survivors are covered
+  // ---- front peeling of the feasible rows until P survivors are covered
   for (int r = 0; r < N; ++r) {
     if (i == 0) cnt = 0;
     __syncthreads();
-    if (on && rank[i] < 0 && ndom[i] == 0) {
+    if (live && rank[i] < 0 && ndom[i] == 0) {
       infront[i] = 1;
       atomicAdd(&cnt, 1);
     }
@@ -226,7 +267,7 @@ __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__r
     }
     __syncthreads();
     if (r_cut >= 0) break;
-    if (on && rank[i] < 0) {
+    if (live && rank[i] < 0) {
       int sub = 0;
       for (int j = 0; j < N; ++j)
         if (infront[j]) sub += dominates3(f[j][0], f[j][1], f[j][2], f[i][0], f[i][1], f[i][2]) ? 1 : 0;
@@ -272,16 +313,7 @@ __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__r
     if (better < need) keep[i] = 1;
   }
   __syncthreads();
-  // ---- stable compaction into the next population
-  if (on && keep[i]) {
-    int dst = 0;
-    for (int j = 0; j < i; ++j) dst += keep[j];
-    const float *src = merged_row(X, C, P, D, i);
-    float *row = Xn + (int64_t)dst * D;
-    for (int k = 0; k < D; ++k) row[k] = src[k];
-    for (int k = 0; k < 3; ++k) Fn[(int64_t)dst * 3 + k] = f[i][k];
-    split_row(src, d, D - d, Xcn + (int64_t)dst * d, Xen + (int64_t)dst * (D - d));
-  }
+  compact();
 }
 
 // ---- multi-CTA survival for 512 < 2P <= 32768 merged rows: one persistent cooperative kernel (grid sized by occupancy,
@@ -297,7 +329,11 @@ __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__r
 //    grows linearly with the number of fronts peeled (P of them when the objectives are totally ordered);
 //  * cut front: each member's position along f_k (counting, ties by index) gives the sorted order, the members then add
 //    their crowding terms for k = 0, 1, 2 in that order, and a second count against the cut front ranks the crowding;
-//  * output: a per-CTA count + exclusive scan maps survivors to ascending rows, then a coalesced copy.
+//  * output: a per-CTA count + exclusive scan maps survivors to ascending rows, then a coalesced copy;
+//  * constraints: every CTA counts the feasible rows it sanitised (population) or de-duplicated (children), and after
+//    the barrier every CTA adds the per-CTA counts in CTA order, so all of them take the same branch.  Infeasible rows get
+//    rank -2 and NaN objectives as sweep columns (NaN never dominates); with fewer than P feasible rows one tiled count
+//    of (G, index) among the infeasible rows replaces phases 3-7.
 // Only integer atomics are used and every float is computed by one thread in a fixed order: outputs are bit-identical
 // from run to run.
 constexpr int NSGA_LARGE_MAX_POP = 16384;
@@ -314,6 +350,7 @@ struct SweepEntry {
 
 struct SurviveWs {
   float *f;       // [3][N] sanitised objectives (duplicates -> +inf)
+  float *g;       // [N] sanitised constraint (0 without one; duplicates -> +inf with one)
   int *ndom;      // [N] dominator count; phase 1 parks the bucket index here
   int *rank;      // [N] front index, -1 = not yet ranked
   int *list;      // [N] the fronts in peeling order
@@ -326,6 +363,7 @@ struct SurviveWs {
   int *keep;      // [N]
   int *sel;       // [P] survivor r -> merged row
   int *bsum;      // [NSGA_GRID_MAX] survivors per CTA
+  int *fsum;      // [NSGA_GRID_MAX] feasible rows per CTA
   int H;          // bucket count (power of two)
 };
 
@@ -337,7 +375,7 @@ static int64_t nsga_buckets(int64_t P) {
 
 size_t nsga_survive_ws_bytes(int64_t P) {
   const int64_t N = 2 * P;
-  const int64_t words[] = {3 * N, N, N, N, N + 2, nsga_buckets(P), N, 3 * N, 3 * N, N, N, P, NSGA_GRID_MAX};
+  const int64_t words[] = {3 * N, N, N, N, N, N + 2, nsga_buckets(P), N, 3 * N, 3 * N, N, N, P, NSGA_GRID_MAX, NSGA_GRID_MAX};
   size_t total = 0;
   for (int64_t w : words) total += (size_t)round_up(w * 4, 256);
   return total;
@@ -353,6 +391,7 @@ static SurviveWs nsga_carve(void *ws, int64_t P) {
   };
   SurviveWs w;
   w.f = (float *)take(3 * N);
+  w.g = (float *)take(N);
   w.ndom = (int *)take(N);
   w.rank = (int *)take(N);
   w.list = (int *)take(N);
@@ -365,6 +404,7 @@ static SurviveWs nsga_carve(void *ws, int64_t P) {
   w.keep = (int *)take(N);
   w.sel = (int *)take(P);
   w.bsum = (int *)take(NSGA_GRID_MAX);
+  w.fsum = (int *)take(NSGA_GRID_MAX);
   w.H = (int)H;
   return w;
 }
@@ -413,15 +453,17 @@ __device__ __forceinline__ void team_sweep(SweepEntry *tile, int nr, int nc, Row
 }
 
 __global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const float *__restrict__ X, const float *__restrict__ F,
-                                                                        const float *__restrict__ C, const float *__restrict__ FC,
+                                                                        const float *__restrict__ G, const float *__restrict__ C,
+                                                                        const float *__restrict__ FC, const float *__restrict__ GC,
                                                                         int P, int D, int d, float *__restrict__ Xn,
-                                                                        float *__restrict__ Fn, float *__restrict__ Xcn,
-                                                                        int32_t *__restrict__ Xen, const SurviveWs w_arg) {
+                                                                        float *__restrict__ Fn, float *__restrict__ Gn,
+                                                                        float *__restrict__ Xcn, int32_t *__restrict__ Xen,
+                                                                        const SurviveWs w_arg) {
   namespace cg = cooperative_groups;
   SurviveWs w = w_arg;
   cg::grid_group grid = cg::this_grid();
   __shared__ SweepEntry tile[NSGA_TJ];
-  __shared__ int s_warp[NSGA_LT / 32], s_base;
+  __shared__ int s_warp[NSGA_LT / 32], s_base, s_feas;
   const int N = 2 * P;
   const int gtid = blockIdx.x * blockDim.x + threadIdx.x, gsz = gridDim.x * blockDim.x;
   float *f0 = w.f, *f1 = w.f + N, *f2 = w.f + 2 * N;
@@ -433,6 +475,10 @@ __global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const fl
     e.id = j;
     return e;
   };
+  auto feasible = [&](int j) { return __ldcg(w.g + j) <= 0.0f; };
+  if (threadIdx.x == 0) s_feas = 0;
+  __syncthreads();
+  int nfeas = 0;   // feasible rows this thread sanitised (population) or de-duplicated (children)
 
   // ---- 0: sanitise, clear the bucket table and the front sizes
   for (int i = gtid; i < N; i += gsz) {
@@ -440,6 +486,9 @@ __global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const fl
     f0[i] = sanitize_obj(src[0]);
     f1[i] = sanitize_obj(src[1]);
     f2[i] = sanitize_obj(src[2]);
+    const float gi = G ? sanitize_obj(i < P ? G[i] : GC[i - P]) : 0.0f;
+    w.g[i] = gi;
+    nfeas += (i < P && gi <= 0.0f) ? 1 : 0;
   }
   for (int h = gtid; h < w.H; h += gsz) w.head[h] = -1;
   for (int r = gtid; r < N + 2; r += gsz) w.cnt[r] = 0;
@@ -457,103 +506,157 @@ __global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const fl
     bool dup = false;
     for (int j = __ldcg(&w.head[__ldcg(&w.ndom[i])]); j >= 0 && !dup; j = __ldcg(&w.next[j]))
       dup = j < i && same_row(merged_row(X, C, P, D, j), me, D);
-    if (dup) f0[i] = f1[i] = f2[i] = INFINITY;
+    float gi = __ldcg(w.g + i);
+    if (dup) {
+      f0[i] = f1[i] = f2[i] = INFINITY;
+      if (G) w.g[i] = gi = INFINITY;
+    }
+    nfeas += gi <= 0.0f ? 1 : 0;
   }
+  atomicAdd(&s_feas, nfeas);
+  __syncthreads();
+  if (threadIdx.x == 0) w.fsum[blockIdx.x] = s_feas;
   grid.sync();
-  // ---- 3: dominator counts; front 0
-  team_sweep(
-      tile, N, N, [&](int r, SweepEntry &me) { me = obj(r); return true; }, obj,
-      [](const SweepEntry &me, const SweepEntry &o, int *acc) {
-        acc[0] += dominates3(o.v[0], o.v[1], o.v[2], me.v[0], me.v[1], me.v[2]) ? 1 : 0;
-      },
-      [&](int r, const SweepEntry &, const int *acc) {
-        w.ndom[r] = acc[0];
-        w.rank[r] = acc[0] == 0 ? 0 : -1;
-        if (acc[0] == 0) w.list[atomicAdd(&w.cnt[0], 1)] = r;
-      });
-  grid.sync();
-  // ---- 4: peel fronts until P rows are covered (every CTA reads the same counts, so all leave at the same round)
-  int start = 0, rc = -1, need = 0;
-  for (int r = 0; r < N; ++r) {
-    const int c = __ldcg(&w.cnt[r]);
-    if (c == 0) break;
-    if (start + c >= P) { rc = r; need = P - start; break; }
-    const int nxt = start + c;
+  if (threadIdx.x == 0) {
+    int nf = 0;
+    for (int b = 0; b < (int)gridDim.x; ++b) nf += __ldcg(w.fsum + b);
+    s_feas = nf;
+  }
+  __syncthreads();
+  const int nf = s_feas;
+  if (nf < P) {
+    // ---- 3': too few feasible rows: all of them survive, then the P - nf least infeasible (ascending G, ties by index)
+    auto cv_entry = [&](int j) {
+      SweepEntry e;
+      e.v[0] = feasible(j) ? __int_as_float(0x7FC00000) : __ldcg(w.g + j);   // NaN: a feasible row is never counted
+      e.v[1] = e.v[2] = 0.0f;
+      e.id = j;
+      return e;
+    };
+    // feasible rows are kept here, the infeasible ones get their keep from the sweep below: disjoint writers, no barrier
+    for (int i = gtid; i < N; i += gsz)
+      if (feasible(i)) w.keep[i] = 1;
     team_sweep(
-        tile, N, c,
-        [&](int i, SweepEntry &me) {
-          if (__ldcg(&w.rank[i]) >= 0) return false;
-          me = obj(i);
+        tile, N, N,
+        [&](int r, SweepEntry &me) {
+          if (feasible(r)) return false;
+          me = cv_entry(r);
           return true;
         },
-        [&](int t) { return obj(__ldcg(&w.list[start + t])); },
+        cv_entry,
+        [](const SweepEntry &me, const SweepEntry &o, int *acc) { acc[0] += before_asc(o.v[0], o.id, me.v[0], me.id) ? 1 : 0; },
+        [&](int r, const SweepEntry &, const int *acc) { w.keep[r] = acc[0] < P - nf ? 1 : 0; });
+    grid.sync();
+  } else {
+    // ---- 3: dominator counts among the feasible rows; front 0
+    auto live_entry = [&](int j) {
+      SweepEntry e = obj(j);
+      if (!feasible(j)) e.v[0] = e.v[1] = e.v[2] = __int_as_float(0x7FC00000);   // NaN never dominates
+      return e;
+    };
+    team_sweep(
+        tile, N, N,
+        [&](int r, SweepEntry &me) {
+          if (!feasible(r)) {
+            w.rank[r] = -2;
+            return false;
+          }
+          me = obj(r);
+          return true;
+        },
+        live_entry,
         [](const SweepEntry &me, const SweepEntry &o, int *acc) {
           acc[0] += dominates3(o.v[0], o.v[1], o.v[2], me.v[0], me.v[1], me.v[2]) ? 1 : 0;
         },
-        [&](int i, const SweepEntry &, const int *acc) {
-          if (acc[0] == 0) return;
-          const int nd = __ldcg(&w.ndom[i]) - acc[0];
-          w.ndom[i] = nd;
-          if (nd == 0) {
-            w.rank[i] = r + 1;
-            w.list[nxt + atomicAdd(&w.cnt[r + 1], 1)] = i;
+        [&](int r, const SweepEntry &, const int *acc) {
+          w.ndom[r] = acc[0];
+          w.rank[r] = acc[0] == 0 ? 0 : -1;
+          if (acc[0] == 0) w.list[atomicAdd(&w.cnt[0], 1)] = r;
+        });
+    grid.sync();
+    // ---- 4: peel fronts until P rows are covered (every CTA reads the same counts, so all leave at the same round)
+    int start = 0, rc = -1, need = 0;
+    for (int r = 0; r < N; ++r) {
+      const int c = __ldcg(&w.cnt[r]);
+      if (c == 0) break;
+      if (start + c >= P) { rc = r; need = P - start; break; }
+      const int nxt = start + c;
+      team_sweep(
+          tile, N, c,
+          [&](int i, SweepEntry &me) {
+            if (__ldcg(&w.rank[i]) != -1) return false;   // ranked or infeasible
+            me = obj(i);
+            return true;
+          },
+          [&](int t) { return obj(__ldcg(&w.list[start + t])); },
+          [](const SweepEntry &me, const SweepEntry &o, int *acc) {
+            acc[0] += dominates3(o.v[0], o.v[1], o.v[2], me.v[0], me.v[1], me.v[2]) ? 1 : 0;
+          },
+          [&](int i, const SweepEntry &, const int *acc) {
+            if (acc[0] == 0) return;
+            const int nd = __ldcg(&w.ndom[i]) - acc[0];
+            w.ndom[i] = nd;
+            if (nd == 0) {
+              w.rank[i] = r + 1;
+              w.list[nxt + atomicAdd(&w.cnt[r + 1], 1)] = i;
+            }
+          });
+      start = nxt;
+      grid.sync();
+    }
+    const int m = rc >= 0 ? __ldcg(&w.cnt[rc]) : 0;
+    const int *front = w.list + start;
+    // ---- 5: cut front: positions along f_0, f_1, f_2; whole fronts below the cut survive
+    for (int i = gtid; i < N; i += gsz) {
+      const int rk = __ldcg(&w.rank[i]);
+      w.keep[i] = (rc >= 0 && rk >= 0 && rk < rc) ? 1 : 0;
+    }
+    team_sweep(
+        tile, m, m, [&](int a, SweepEntry &me) { me = obj(__ldcg(front + a)); return true; },
+        [&](int t) { return obj(__ldcg(front + t)); },
+        [](const SweepEntry &me, const SweepEntry &o, int *acc) {
+#pragma unroll
+          for (int k = 0; k < 3; ++k) acc[k] += before_asc(o.v[k], o.id, me.v[k], me.id) ? 1 : 0;
+        },
+        [&](int a, const SweepEntry &me, const int *acc) {
+#pragma unroll
+          for (int k = 0; k < 3; ++k) {
+            w.pos[k * N + a] = acc[k];
+            w.order[k * N + acc[k]] = me.id;
           }
         });
-    start = nxt;
+    grid.sync();
+    // ---- 6: crowding, k = 0, 1, 2 in order, by the member itself
+    for (int a = gtid; a < m; a += gsz) {
+      float cr = 0.0f;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const float *fk = w.f + k * N;
+        const int *ok = w.order + k * N;
+        const int p = __ldcg(w.pos + k * N + a);
+        if (p == 0 || p == m - 1) cr = INFINITY;
+        else cr = crowd_interior(cr, __ldcg(fk + __ldcg(ok + p - 1)), __ldcg(fk + __ldcg(ok + p + 1)), __ldcg(fk + __ldcg(ok)),
+                                 __ldcg(fk + __ldcg(ok + m - 1)));
+      }
+      w.crowd[a] = cr;
+    }
+    grid.sync();
+    // ---- 7: the `need` members with the largest crowding survive
+    auto crowd_entry = [&](int a) {
+      SweepEntry e;
+      e.v[0] = __ldcg(w.crowd + a);
+      e.v[1] = e.v[2] = 0.0f;
+      e.id = __ldcg(front + a);
+      return e;
+    };
+    team_sweep(
+        tile, m, m, [&](int a, SweepEntry &me) { me = crowd_entry(a); return true; }, crowd_entry,
+        [](const SweepEntry &me, const SweepEntry &o, int *acc) { acc[0] += before_desc(o.v[0], o.id, me.v[0], me.id) ? 1 : 0; },
+        [&](int, const SweepEntry &me, const int *acc) {
+          if (acc[0] < need) w.keep[me.id] = 1;
+        });
     grid.sync();
   }
-  const int m = rc >= 0 ? __ldcg(&w.cnt[rc]) : 0;
-  const int *front = w.list + start;
-  // ---- 5: cut front: positions along f_0, f_1, f_2; whole fronts below the cut survive
-  for (int i = gtid; i < N; i += gsz) {
-    const int rk = __ldcg(&w.rank[i]);
-    w.keep[i] = (rc >= 0 && rk >= 0 && rk < rc) ? 1 : 0;
-  }
-  team_sweep(
-      tile, m, m, [&](int a, SweepEntry &me) { me = obj(__ldcg(front + a)); return true; },
-      [&](int t) { return obj(__ldcg(front + t)); },
-      [](const SweepEntry &me, const SweepEntry &o, int *acc) {
-#pragma unroll
-        for (int k = 0; k < 3; ++k) acc[k] += before_asc(o.v[k], o.id, me.v[k], me.id) ? 1 : 0;
-      },
-      [&](int a, const SweepEntry &me, const int *acc) {
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-          w.pos[k * N + a] = acc[k];
-          w.order[k * N + acc[k]] = me.id;
-        }
-      });
-  grid.sync();
-  // ---- 6: crowding, k = 0, 1, 2 in order, by the member itself
-  for (int a = gtid; a < m; a += gsz) {
-    float cr = 0.0f;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      const float *fk = w.f + k * N;
-      const int *ok = w.order + k * N;
-      const int p = __ldcg(w.pos + k * N + a);
-      if (p == 0 || p == m - 1) cr = INFINITY;
-      else cr = crowd_interior(cr, __ldcg(fk + __ldcg(ok + p - 1)), __ldcg(fk + __ldcg(ok + p + 1)), __ldcg(fk + __ldcg(ok)),
-                               __ldcg(fk + __ldcg(ok + m - 1)));
-    }
-    w.crowd[a] = cr;
-  }
-  grid.sync();
-  // ---- 7: the `need` members with the largest crowding survive
-  auto crowd_entry = [&](int a) {
-    SweepEntry e;
-    e.v[0] = __ldcg(w.crowd + a);
-    e.v[1] = e.v[2] = 0.0f;
-    e.id = __ldcg(front + a);
-    return e;
-  };
-  team_sweep(
-      tile, m, m, [&](int a, SweepEntry &me) { me = crowd_entry(a); return true; }, crowd_entry,
-      [](const SweepEntry &me, const SweepEntry &o, int *acc) { acc[0] += before_desc(o.v[0], o.id, me.v[0], me.id) ? 1 : 0; },
-      [&](int, const SweepEntry &me, const int *acc) {
-        if (acc[0] < need) w.keep[me.id] = 1;
-      });
-  grid.sync();
   // ---- 8: survivors -> ascending output rows (CTA b owns merged rows [b * chunk, (b + 1) * chunk))
   const int chunk = (int)ceil_div(N, gridDim.x);
   const int r0 = blockIdx.x * chunk, r1 = min(N, r0 + chunk);
@@ -597,6 +700,8 @@ __global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const fl
     const int r = (int)(q / 3), k = (int)(q % 3);
     Fn[q] = __ldcg(w.f + k * N + __ldcg(w.sel + r));
   }
+  if (Gn)
+    for (int q = gtid; q < total; q += gsz) Gn[q] = __ldcg(w.g + __ldcg(w.sel + q));
   for (int64_t q = gtid; q < (int64_t)total * d; q += gsz) {
     const int r = (int)(q / d), k = (int)(q % d);
     Xcn[q] = merged_row(X, C, P, D, __ldcg(w.sel + r))[k];
@@ -630,11 +735,13 @@ int64_t nsga_survive_ws_query(int64_t P, int64_t D) {
   return (int64_t)nsga_survive_ws_bytes(P);
 }
 
-int launch_nsga_survive(const float *X, const float *F, const float *C, const float *FC, int64_t P, int64_t D, int64_t d,
-                        float *Xn, float *Fn, float *Xcn, int32_t *Xen, void *ws, int64_t ws_bytes, cudaStream_t st) {
+int launch_nsga_survive(const float *X, const float *F, const float *G, const float *C, const float *FC, const float *GC,
+                        int64_t P, int64_t D, int64_t d, float *Xn, float *Fn, float *Gn, float *Xcn, int32_t *Xen, void *ws,
+                        int64_t ws_bytes, cudaStream_t st) {
   if (P <= 0 || P > NSGA_LARGE_MAX_POP || D <= 0 || d < 0 || d > D) return HB_ERR_INVALID;
+  if (!G != !GC) return HB_ERR_INVALID;
   if (2 * P <= NSGA_MAX) {
-    nsga_survive_kernel<<<1, NSGA_MAX, 0, st>>>(X, F, C, FC, (int)P, (int)D, (int)d, Xn, Fn, Xcn, Xen);
+    nsga_survive_kernel<<<1, NSGA_MAX, 0, st>>>(X, F, G, C, FC, GC, (int)P, (int)D, (int)d, Xn, Fn, Gn, Xcn, Xen);
     count_launches(1);
     HB_LAUNCH_CHECK("nsga_survive");
     return HB_OK;
@@ -660,7 +767,7 @@ int launch_nsga_survive(const float *X, const float *F, const float *C, const fl
   const int grid = (int)std::min<int64_t>({(int64_t)once.aux[dev], ceil_div(2 * P, NSGA_ROWS), (int64_t)NSGA_GRID_MAX});
   SurviveWs w = nsga_carve(ws, P);
   int Pi = (int)P, Di = (int)D, di = (int)d;
-  void *args[] = {&X, &F, &C, &FC, &Pi, &Di, &di, &Xn, &Fn, &Xcn, &Xen, &w};
+  void *args[] = {&X, &F, &G, &C, &FC, &GC, &Pi, &Di, &di, &Xn, &Fn, &Gn, &Xcn, &Xen, &w};
   HB_CUDA(cudaLaunchCooperativeKernel((const void *)nsga_survive_large_kernel, dim3(grid), dim3(NSGA_LT), args, 0, st));
   count_launches(1);
   HB_LAUNCH_CHECK("nsga_survive_large");

@@ -82,6 +82,61 @@ def rank_and_crowding_survival(F: np.ndarray, n_survive: int) -> np.ndarray:
     return np.asarray(keep, dtype=np.int64)
 
 
+def survive_host(X: np.ndarray, F: np.ndarray, C: np.ndarray, FC: np.ndarray, G: Optional[np.ndarray] = None,
+                 GC: Optional[np.ndarray] = None):
+    """numpy restatement of the device survival (hb_nsga2_survive_ex, and hb_nsga2_survive_cv when G / GC are given),
+    fp32 like the kernels so that the survivors agree bit for bit: sanitising, duplicate children, the constraint rule,
+    ranks, fp32 crowding of the cut front (see the rules in hebo_b200/csrc/nsga.cu).  Returns the merged indices of the
+    survivors in ascending order, and the sanitised objectives [2P, 3] and constraint [2P] of the merged rows."""
+    P = X.shape[0]
+    Xa = np.concatenate([X, C], 0).astype(np.float32)
+    f = np.concatenate([F, FC], 0).astype(np.float32)
+    f = np.where(np.isfinite(f), f, np.float32(np.inf))
+    cons = G is not None
+    g = np.zeros(2 * P, np.float32) if not cons else np.concatenate([G, GC]).astype(np.float32).reshape(-1)
+    g = np.where(np.isfinite(g), g, np.float32(np.inf))
+    for i in range(P, 2 * P):
+        if (np.abs(Xa[:i] - Xa[i]) <= np.float32(1e-16)).all(1).any():
+            f[i] = np.inf
+            if cons:
+                g[i] = np.inf
+    feas = g <= 0
+    nf = int(feas.sum())
+    keep = np.zeros(2 * P, bool)
+    if nf < P:
+        keep |= feas
+        inf_rows = np.flatnonzero(~feas)
+        keep[inf_rows[np.argsort(g[inf_rows], kind="stable")[:P - nf]]] = True
+        return np.flatnonzero(keep), f, g
+    rows = np.flatnonzero(feas)
+    fr = f[rows]
+    rank = fast_non_dominated_sort(fr)
+    cum = 0
+    for r in range(rank.max() + 1):
+        members = np.flatnonzero(rank == r)
+        if cum + members.size < P:
+            keep[rows[members]] = True
+            cum += members.size
+            continue
+        fm, m = fr[members], members.size
+        crowd = np.zeros(m, np.float32)
+        for k in range(3):
+            v = fm[:, k]
+            order = np.argsort(v, kind="stable")
+            pos = np.empty(m, np.int64)
+            pos[order] = np.arange(m)
+            fmin, fmax = v[order[0]], v[order[-1]]
+            ends = (pos == 0) | (pos == m - 1)
+            if fmax > fmin and np.isfinite(fmax - fmin):
+                with np.errstate(invalid="ignore", over="ignore"):
+                    step = (v[order[np.minimum(pos + 1, m - 1)]] - v[order[np.maximum(pos - 1, 0)]]) / (fmax - fmin)
+                crowd = np.where(ends, crowd, crowd + step).astype(np.float32)
+            crowd = np.where(ends, np.float32(np.inf), crowd).astype(np.float32)
+        keep[rows[members[np.argsort(-crowd, kind="stable")[:P - cum]]]] = True
+        break
+    return np.flatnonzero(keep), f, g
+
+
 class EvolutionOpt:
     def __init__(self, lb, ub, acq_fn: Callable[[np.ndarray], np.ndarray], pop: int = 100, iters: int = 100,
                  seed: Optional[int] = None, sbx_eta: float = 15.0, sbx_prob: float = 0.9, sbx_prob_var: float = 0.5,
@@ -190,13 +245,17 @@ class DeviceNSGA2:
     kinds [D]: 'real' | 'int' | 'choice' per optimisation column (numeric columns first, then the categorical ones:
     evolution_optimizer.py:26-41); lb / ub [D]; fixed: {column index: value} (fix_input, :97-101).  `score(Xc, Xe, gen)`
     returns the objectives F [pop, 3] of a batch as a device tensor (the fused posterior + MACE call).  2 <= pop <= 16384:
-    survival runs in one CTA up to pop 256 and in a cooperative multi-CTA kernel above, with the same results."""
+    survival runs in one CTA up to pop 256 and in a cooperative multi-CTA kernel above, with the same results.
+
+    constrained=True: `score` returns (F [pop, 3], G [pop]) with one constraint column (feasible iff G <= 0, the pymoo
+    constraint of evolution_optimizer.py:82,105); survival is hb_nsga2_survive_cv and the result is the feasible front
+    (hebo_b200.pareto.feasible_front).  The generation loop still never synchronises with the host."""
 
     KIND = {"real": 0, "int": 1, "choice": 2}
     MAX_POP = 16384                                 # hb_nsga2_survive_ex: single CTA up to 256, cooperative multi-CTA above
 
     def __init__(self, kinds, lb, ub, num_numeric: int, score: Callable, pop: int = 100, iters: int = 100,
-                 seed: Optional[int] = None, fixed: Optional[dict] = None, device="cuda"):
+                 seed: Optional[int] = None, fixed: Optional[dict] = None, device="cuda", constrained: bool = False):
         import torch
         self.torch = torch
         self.D, self.d, self.pop, self.iters = len(kinds), int(num_numeric), int(pop), int(iters)
@@ -212,6 +271,7 @@ class DeviceNSGA2:
             fx[k] = v
         self.fixed = torch.from_numpy(fx).to(dev)
         self.score = score
+        self.constrained = bool(constrained)
         self.seed = int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed)
         self.n_evals = 0
 
@@ -222,9 +282,9 @@ class DeviceNSGA2:
 
     def optimize(self, initial_suggest=None):
         """Returns (Xc [K, d] fp32, Xe [K, e] int32, F [K, 3]) of the non-dominated members of the final population
-        (res.X of evolution_optimizer.py:141-149), all on the device."""
+        (res.X of evolution_optimizer.py:141-149), all on the device; with constraints, of its feasible front."""
         from . import _lib
-        from .pareto import pareto_front
+        from .pareto import feasible_front, pareto_front
         t, lib, P, D, d = self.torch, _lib.lib(), self.pop, self.D, self.d
         st = _lib.stream_ptr
         X, Xc, Xe = self._bufs()
@@ -240,17 +300,32 @@ class DeviceNSGA2:
         with t.cuda.device(self.dev):
             _lib.check(lib.hb_nsga2_init(_lib.ptr(X), P, D, d, _lib.ptr(self.kind), _lib.ptr(self.lb), _lib.ptr(self.ub), _lib.ptr(self.fixed),
                                          _lib.ptr(init), n_init, self.seed, pc(Xc), pc(Xe), st()), "hb_nsga2_init")
-            F = self.score(Xc, Xe, 0).contiguous()
+            F, G = self._scored(Xc, Xe, 0)
             Fn = t.empty_like(F)
+            Gn = None if G is None else t.empty_like(G)
             self.n_evals = P
             for gen in range(1, self.iters):                       # ('n_gen', iters): generation 1 is the initial population
                 _lib.check(lib.hb_nsga2_mate(_lib.ptr(X), P, D, d, _lib.ptr(self.kind), _lib.ptr(self.lb), _lib.ptr(self.ub),
                                              _lib.ptr(self.fixed), self.seed, gen, _lib.ptr(C), pc(Cc), pc(Ce), st()), "hb_nsga2_mate")
-                FC = self.score(Cc, Ce, gen).contiguous()
-                _lib.check(lib.hb_nsga2_survive_ex(_lib.ptr(X), _lib.ptr(F), _lib.ptr(C), _lib.ptr(FC), P, D, d, _lib.ptr(Xn), _lib.ptr(Fn),
-                                                   pc(Xcn), pc(Xen), _lib.ptr(ws), ws_bytes, st()), "hb_nsga2_survive_ex")
+                FC, GC = self._scored(Cc, Ce, gen)
+                if G is None:
+                    _lib.check(lib.hb_nsga2_survive_ex(_lib.ptr(X), _lib.ptr(F), _lib.ptr(C), _lib.ptr(FC), P, D, d, _lib.ptr(Xn),
+                                                       _lib.ptr(Fn), pc(Xcn), pc(Xen), _lib.ptr(ws), ws_bytes, st()), "hb_nsga2_survive_ex")
+                else:
+                    _lib.check(lib.hb_nsga2_survive_cv(_lib.ptr(X), _lib.ptr(F), _lib.ptr(G), _lib.ptr(C), _lib.ptr(FC), _lib.ptr(GC), P, D,
+                                                       d, _lib.ptr(Xn), _lib.ptr(Fn), _lib.ptr(Gn), pc(Xcn), pc(Xen), _lib.ptr(ws),
+                                                       ws_bytes, st()), "hb_nsga2_survive_cv")
+                    G, Gn = Gn, G
                 X, Xn, Xc, Xcn, Xe, Xen, F, Fn = Xn, X, Xcn, Xc, Xen, Xe, Fn, F
                 self.n_evals += P
-        self.pop_X, self.pop_F = X, F
-        idx = pareto_front(F)
+        self.pop_X, self.pop_F, self.pop_G = X, F, G
+        idx = pareto_front(F) if G is None else feasible_front(F, G)
         return Xc[idx], Xe[idx], F[idx]
+
+    def _scored(self, Xc, Xe, gen):
+        """(F [n, 3], G [n] or None) of a batch, contiguous fp32 on the device."""
+        out = self.score(Xc, Xe, gen)
+        if not self.constrained:
+            return out.contiguous(), None
+        F, G = out
+        return F.contiguous(), G.reshape(-1).to(self.torch.float32).contiguous()

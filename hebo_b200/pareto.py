@@ -48,6 +48,21 @@ def pareto_front(F: torch.Tensor) -> torch.Tensor:
     return idx[:int(cnt.item())].to(torch.int64)
 
 
+def feasible_front(F: torch.Tensor, G: torch.Tensor) -> torch.Tensor:
+    """Rank-0 set under one constraint column: F [m,3], G [m] CUDA tensors -> ascending int64 indices (on the device).
+    A row is feasible iff G <= 0 (a non-finite G counts as +inf, as in hb_nsga2_survive_cv).  The result is the
+    non-dominated set of the feasible rows; with no feasible row it is the single least infeasible row (smallest G, lowest
+    index), which is what pymoo's filter_optimum(least_infeasible=True) is recalled to return -- not checked against
+    pymoo.  Infeasible rows are masked to NaN, which the device filter already excludes."""
+    G = G.reshape(-1).to(torch.float32)
+    G = torch.where(torch.isfinite(G), G, torch.full_like(G, float("inf")))
+    feas = G <= 0
+    idx = pareto_front(torch.where(feas[:, None], F.to(torch.float32), torch.full_like(F, float("nan"), dtype=torch.float32)))
+    if idx.numel() == 0 and G.numel() and not bool(feas.any()):
+        idx = torch.argmin(G).reshape(1)          # first of the minima: the lowest index on ties
+    return idx
+
+
 FRONT_W = 8     # floats per row of a front buffer (include/hebo_b200.h "multi-GPU front exchange")
 
 

@@ -25,7 +25,7 @@ from torch.quasirandom import SobolEngine
 
 from .acq import MACE
 from .gp import GP
-from .pareto import pareto_front
+from .pareto import feasible_front, pareto_front
 from .space import DesignSpace, box_space
 
 
@@ -61,7 +61,7 @@ class HEBO:
     def __init__(self, space=None, ub=None, model_config: Optional[dict] = None, rand_sample: Optional[int] = None,
                  scramble_seed: Optional[int] = None, n_candidates: int = 10000, device: str = "cuda",
                  n_refine: int = 0, refine_sigma: float = 0.05, acq_optimizer: str = "sobol", evo_pop: int = 100,
-                 evo_iters: int = 100, lb=None):
+                 evo_iters: int = 100, lb=None, _constraint=None):
         if lb is not None:
             space = lb
         if ub is not None:                                   # HEBO(lb, ub): continuous box, tensors in / out
@@ -87,6 +87,11 @@ class HEBO:
         self.n_refine = int(n_refine)
         self.refine_sigma = float(refine_sigma)
         self.device = device
+        # constraint hook (hebo_b200.embedding.HEBO_Embedding): Xc [m, d] on the device -> G [m], feasible iff G <= 0.  Both
+        # acquisition optimisers then return the feasible front (pareto.feasible_front); there is no constrained refinement
+        self._constraint = _constraint
+        if _constraint is not None and self.n_refine:
+            raise ValueError("n_refine is not supported together with a constraint")
         self._model_config = model_config
         self.last_timing = {}
 
@@ -208,11 +213,16 @@ class HEBO:
         def score(xc, xe, seed=0):
             return model.predict_mace(xc if self.d else None, tau, kappa, acq.eps, seed=seed, return_mu_var=True,
                                       Xe=xe if self.e else None, device_out=True)
+        cons = self._constraint
         if self.acq_optimizer == "nsga2" and candidates is None:
             from .evolution import DeviceNSGA2
-            evo = DeviceNSGA2(self.space.var_kinds, self.lb.numpy(), self.ub.numpy(), self.d,
-                              lambda xc, xe, gen: score(xc, xe, gen)[0], pop=self.evo_pop, iters=self.evo_iters,
-                              seed=int(np.random.randint(0, 2 ** 31 - 1)), fixed=fixed, device=dev)
+            if cons is None:
+                evo_score = lambda xc, xe, gen: score(xc, xe, gen)[0]
+            else:
+                evo_score = lambda xc, xe, gen: (score(xc, xe, gen)[0], cons(xc))
+            evo = DeviceNSGA2(self.space.var_kinds, self.lb.numpy(), self.ub.numpy(), self.d, evo_score, pop=self.evo_pop,
+                              iters=self.evo_iters, seed=int(np.random.randint(0, 2 ** 31 - 1)), fixed=fixed, device=dev,
+                              constrained=cons is not None)
             cand_c, cand_e, _ = evo.optimize(initial_suggest=torch.cat([bxc, bxe.float()], 1).numpy())
             cand_e = cand_e.long()
             mark("candidates_ms")
@@ -230,7 +240,7 @@ class HEBO:
             mark("candidates_ms")
             F, mu, var = score(cand_c, cand_e)
             mark("posterior_mace_ms")
-            idx = pareto_front(F)
+            idx = pareto_front(F) if cons is None else feasible_front(F, cons(cand_c))
         for _ in range(self.n_refine if self.d else 0):
             pc, pe = cand_c[idx], cand_e[idx]
             reps = max(1, (self.n_candidates // 4) // max(1, pc.shape[0]))

@@ -311,7 +311,15 @@ int32_t hb_pareto_front3(const float *F, int64_t m, int32_t *idx_out, int32_t *c
  *   larger populations run a cooperative multi-CTA kernel and need ws_bytes >= hb_nsga2_workspace_bytes(pop, D).
  *   Both give the same survivors, bit for bit, and are deterministic.
  * hb_nsga2_workspace_bytes: host only; < 0 if pop < 1, pop > 16384 or D < 1.
- * hb_nsga2_survive: the workspace-free entry, pop <= 256. */
+ * hb_nsga2_survive: the workspace-free entry, pop <= 256.
+ * hb_nsga2_survive_cv: the same survival with one constraint column (pymoo's survival with infeasible filtering, as
+ *   EvolutionOpt uses it with n_constr = 1: evolution_optimizer.py:82,105,135-140; the rule is recalled, not checked
+ *   against pymoo).  G [pop] / GC [pop] the population's / offspring's constraint, G_next [pop] out.  A row is feasible
+ *   iff G <= 0; a non-finite G and a duplicate child count as G = +inf.  With at least pop feasible merged rows only
+ *   those enter the rank-and-crowding survival; otherwise every feasible row survives and the remaining slots go to the
+ *   infeasible rows in ascending G, ties by the lower merged index.  Survivors keep ascending merged-row order.  Same
+ *   sizes, workspace, kernels and determinism as hb_nsga2_survive_ex; G = GC = 0 gives its result, except when the cut
+ *   front is the front of all-+inf rows and holds a duplicate child (which is infeasible here). */
 int32_t hb_nsga2_init(float *X, int64_t pop, int64_t D, int64_t d, const int32_t *kind, const float *lb, const float *ub,
                       const float *fixed, const float *init, int64_t n_init, uint64_t seed, float *Xc, int32_t *Xe, void *stream);
 int32_t hb_nsga2_mate(const float *X, int64_t pop, int64_t D, int64_t d, const int32_t *kind, const float *lb, const float *ub,
@@ -322,6 +330,20 @@ int64_t hb_nsga2_workspace_bytes(int64_t pop, int64_t D);
 int32_t hb_nsga2_survive_ex(const float *X, const float *F, const float *C, const float *FC, int64_t pop, int64_t D,
                             int64_t d, float *X_next, float *F_next, float *Xc_next, int32_t *Xe_next,
                             void *ws, int64_t ws_bytes, void *stream);
+int32_t hb_nsga2_survive_cv(const float *X, const float *F, const float *G, const float *C, const float *FC, const float *GC,
+                            int64_t pop, int64_t D, int64_t d, float *X_next, float *F_next, float *G_next, float *Xc_next,
+                            int32_t *Xe_next, void *ws, int64_t ws_bytes, void *stream);
+
+/* ---- bound violation of a random embedding  (MACE_Embedding.eval, optimizers/hebo_embedding.py:85-90, clip = False)
+ * Y [m, e] candidates in the embedding, B [e, D] projection matrix, both row-major fp32 on the device; G [m] out:
+ *   G[i] = sum_j max(|sum_k Y[i,k] B[k,j]| - 1, 0)   (hebo_embedding.py:88-89)
+ * without forming Y B.  Each projected coordinate is an fp32 sum over k ascending; the sums over j are reduced in fp64 in
+ * a fixed order (no float atomics), so G is bit-identical from run to run.  A NaN coordinate gives G = NaN (torch.clamp
+ * keeps NaN), which hb_nsga2_survive_cv and the feasible front treat as +inf, i.e. infeasible.  1 <= m, 1 <= e <= HB_MAX_FEATURES, 1 <= D.
+ * hb_embed_violation_workspace_bytes: host only; < 0 on bad sizes.  Two launches, no host synchronisation. */
+int64_t hb_embed_violation_workspace_bytes(int64_t m, int64_t e, int64_t D);
+int32_t hb_embed_violation(const float *Y, int64_t m, int64_t e, const float *B, int64_t D, float *G, void *ws,
+                           int64_t ws_bytes, void *stream);
 
 /* ---- multi-GPU front exchange  (candidate-sharded scoring, BASELINE config 5: every rank filters its shard, ONE
  * all-gather of fixed-capacity front buffers, every rank merges; no reference counterpart -- the reference is one process,
