@@ -13,6 +13,7 @@ LIB_PATH = os.path.join(HERE, "lib", "libhebo_b200.so")
 
 HB_OK, HB_ERR_INVALID, HB_ERR_NOT_PD, HB_ERR_CUDA = 0, 1, 2, 3
 KERNEL_IDS = {"matern32": 0, "matern52": 1, "rbf": 2}
+HB_ACQ1_LCB, HB_ACQ1_MEAN, HB_ACQ1_SIGMA, HB_ACQ1_ABS_ETA = 0, 1, 2, 3   # hb_acq1_epilogue modes
 HB_MAX_FEATURES = 4096   # d + sum(emb_sizes) a model may have (include/hebo_b200.h)
 HB_MAX_OUTPUTS = 32      # outputs one batched fit trains together (hb_fit_multi_ex)
 
@@ -87,6 +88,7 @@ SIGNATURES = {
     "hb_sample_y": (_i32, [_vp, _vp, _i64, _i64, _i64, _sp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _f32, _f32, _i32, _vp, _i32,
                            _vp, C.POINTER(C.c_float), _vp, _i64, _vp]),
     "hb_mace_epilogue": (_i32, [_vp, _vp, _i64, _f32, _f32, _f32, _f32, _vp, _vp, _u64, _vp, _vp]),
+    "hb_acq1_epilogue": (_i32, [_vp, _vp, _i64, _i32, _f32, _f32, _vp, _vp]),
     "hb_pareto_front3": (_i32, [_vp, _i64, _vp, _vp, _vp, _i64, _vp]),
     "hb_nsga2_init": (_i32, [_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _u64, _vp, _vp, _vp]),
     "hb_nsga2_mate": (_i32, [_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _u64, _i32, _vp, _vp, _vp, _vp]),
@@ -94,7 +96,8 @@ SIGNATURES = {
     "hb_nsga2_workspace_bytes": (_i64, [_i64, _i64]),
     "hb_nsga2_survive_ex": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
     "hb_nsga2_survive_cv": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
-    "hb_embed_violation_workspace_bytes": (_i64, [_i64, _i64, _i64]),
+    "hb_ga_survive": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
+    "hb_embed_violation_workspace_bytes":(_i64, [_i64, _i64, _i64]),
     "hb_embed_violation": (_i32, [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _vp]),
     "hb_front_merge_workspace_bytes": (_i64, [_i64, _i64]),
     "hb_front_pack": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp]),

@@ -810,6 +810,12 @@ int32_t hb_mace_epilogue(const float *mu, const float *var, int64_t m, float noi
   return launch_mace_only(mu, var, m, noise_var, tau, kappa, eps, xi1, xi2, seed, F, (cudaStream_t)stream);
 }
 
+int32_t hb_acq1_epilogue(const float *mu, const float *var, int64_t m, int32_t mode, float kappa, float eta, float *f,
+                         void *stream) {
+  if (!mu || !var || !f) return HB_ERR_INVALID;
+  return launch_acq1(mu, var, m, mode, kappa, eta, f, (cudaStream_t)stream);
+}
+
 int32_t hb_pareto_front3(const float *F, int64_t m, int32_t *idx_out, int32_t *count, void *ws, int64_t ws_bytes,
                          void *stream) {
   if (!F || !idx_out || !count || !ws) return HB_ERR_INVALID;
@@ -870,6 +876,12 @@ int32_t hb_nsga2_survive_cv(const float *X, const float *F, const float *G, cons
     return HB_ERR_INVALID;
   return launch_nsga_survive(X, F, G, C, FC, GC, pop, D, d, X_next, F_next, G_next, Xc_next, Xe_next, ws, ws_bytes,
                              (cudaStream_t)stream);
+}
+
+int32_t hb_ga_survive(const float *X, const float *F, const float *C, const float *FC, int64_t pop, int64_t D, int64_t d,
+                      float *X_next, float *F_next, float *Xc_next, int32_t *Xe_next, void *ws, int64_t ws_bytes, void *stream) {
+  if (!X || !F || !C || !FC || !X_next || !F_next || (d > 0 && !Xc_next) || (D > d && !Xe_next)) return HB_ERR_INVALID;
+  return launch_ga_survive(X, F, C, FC, pop, D, d, X_next, F_next, Xc_next, Xe_next, ws, ws_bytes, (cudaStream_t)stream);
 }
 
 int64_t hb_embed_violation_workspace_bytes(int64_t m, int64_t e, int64_t D) { return embed_violation_ws_query(m, e, D); }

@@ -133,6 +133,8 @@ size_t posterior_ws_bytes(int64_t np, int64_t d, int64_t m_chunk);
 int guard_stats(unsigned long long *out, int reset);
 int launch_mace_only(const float *mu, const float *var, int64_t m, float noise_var, float tau, float kappa, float eps,
                      const float *xi1, const float *xi2, uint64_t seed, float *F, cudaStream_t st);
+// f[m] of a single-objective acquisition (mode HB_ACQ1_*) over (mu, var)
+int launch_acq1(const float *mu, const float *var, int64_t m, int mode, float kappa, float eta, float *f, cudaStream_t st);
 int kstar_groups(int64_t np);
 int launch_kstar(const float *xs, const int32_t *xe, int64_t mc, const ModelSpec &sp, const float *tab_s, const float *x_mul,
                  const float *x_add, const float *Zt, const float *alpha, const float *hyp, int64_t n, int64_t np, int kern,
@@ -179,6 +181,9 @@ int64_t nsga_survive_ws_query(int64_t P, int64_t D);
 int launch_nsga_survive(const float *X, const float *F, const float *G, const float *C, const float *FC, const float *GC,
                         int64_t P, int64_t D, int64_t d, float *Xn, float *Fn, float *Gn, float *Xcn, int32_t *Xen, void *ws,
                         int64_t ws_bytes, cudaStream_t st);
+// single-objective survival: the P best merged rows by (f, index), best first; same sizes and workspace as above
+int launch_ga_survive(const float *X, const float *F, const float *C, const float *FC, int64_t P, int64_t D, int64_t d,
+                      float *Xn, float *Fn, float *Xcn, int32_t *Xen, void *ws, int64_t ws_bytes, cudaStream_t st);
 // embed.cu: G[i] = sum_j max(|sum_k Y[i,k] B[k,j]| - 1, 0)
 int64_t embed_violation_ws_query(int64_t m, int64_t e, int64_t D);
 int launch_embed_violation(const float *Y, int64_t m, int64_t e, const float *B, int64_t D, float *G, void *ws, int64_t ws_bytes,

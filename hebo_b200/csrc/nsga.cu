@@ -182,6 +182,14 @@ __device__ __forceinline__ const float *merged_row(const float *X, const float *
   return j < P ? X + (int64_t)j * D : C + (int64_t)(j - P) * D;
 }
 
+// merged row i (a child, i >= P) equals an earlier merged row j < i: the duplicate test of the single-CTA kernels
+__device__ __forceinline__ bool dup_of_earlier(const float *X, const float *C, int P, int D, int i) {
+  const float *me = C + (int64_t)(i - P) * D;
+  bool dup = false;
+  for (int j = 0; j < i && !dup; ++j) dup = same_row(merged_row(X, C, P, D, j), me, D);
+  return dup;
+}
+
 constexpr int NSGA_MAX = 512;
 __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__restrict__ X, const float *__restrict__ F,
                                                                 const float *__restrict__ G, const float *__restrict__ C,
@@ -207,10 +215,7 @@ __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__r
   __syncthreads();
   if (on && i >= P) {
     // duplicate elimination: a child equal to a population member or to an earlier child is discarded
-    const float *me = C + (int64_t)(i - P) * D;
-    bool dup = false;
-    for (int j = 0; j < i && !dup; ++j) dup = same_row(merged_row(X, C, P, D, j), me, D);
-    if (dup) {
+    if (dup_of_earlier(X, C, P, D, i)) {
       f[i][0] = f[i][1] = f[i][2] = INFINITY;
       if (G) g[i] = INFINITY;
     }
@@ -425,6 +430,43 @@ __device__ __forceinline__ uint32_t row_bucket(const float *row, int D, int H) {
   return h & (uint32_t)(H - 1);
 }
 
+// Steps shared by the multi-CTA survivals.  bucket_rows puts every merged row into its bucket (the bucket index is parked
+// in w.ndom); after a grid barrier dup_in_bucket tests child i with the exact predicate against the lower merged indices
+// of its bucket.
+__device__ __forceinline__ void bucket_rows(const float *X, const float *C, int P, int D, const SurviveWs &w, int gtid, int gsz) {
+  for (int i = gtid; i < 2 * P; i += gsz) {
+    const int b = (int)row_bucket(merged_row(X, C, P, D, i), D, w.H);
+    w.ndom[i] = b;
+    w.next[i] = atomicExch(&w.head[b], i);
+  }
+}
+
+__device__ __forceinline__ bool dup_in_bucket(const float *X, const float *C, int P, int D, const SurviveWs &w, int i) {
+  const float *me = C + (int64_t)(i - P) * D;
+  bool dup = false;
+  for (int j = __ldcg(&w.head[__ldcg(&w.ndom[i])]); j >= 0 && !dup; j = __ldcg(&w.next[j]))
+    dup = j < i && same_row(merged_row(X, C, P, D, j), me, D);
+  return dup;
+}
+
+// coalesced copy of the survivors: output row r < total is merged row sel[r], with its Xc / Xe split
+__device__ __forceinline__ void copy_survivors(const float *X, const float *C, int P, int D, int d, const int *sel, int total,
+                                               float *Xn, float *Xcn, int32_t *Xen, int gtid, int gsz) {
+  const int e = D - d;
+  for (int64_t q = gtid; q < (int64_t)total * D; q += gsz) {
+    const int r = (int)(q / D), k = (int)(q % D);
+    Xn[q] = merged_row(X, C, P, D, __ldcg(sel + r))[k];
+  }
+  for (int64_t q = gtid; q < (int64_t)total * d; q += gsz) {
+    const int r = (int)(q / d), k = (int)(q % d);
+    Xcn[q] = merged_row(X, C, P, D, __ldcg(sel + r))[k];
+  }
+  for (int64_t q = gtid; q < (int64_t)total * e; q += gsz) {
+    const int r = (int)(q / e), k = (int)(q % e);
+    Xen[q] = (int32_t)rintf(merged_row(X, C, P, D, __ldcg(sel + r))[d + k]);
+  }
+}
+
 // Tiled count: for every row r < nr (one 8-lane team each), acc[0..2] = sums of test(me, entry) over the nc entries of
 // the swept set, staged NSGA_TJ at a time in shared memory; out(r, me, acc) runs on the team's lane 0.  Every thread of
 // the CTA must call it (it holds __syncthreads and warp shuffles).
@@ -494,18 +536,11 @@ __global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const fl
   for (int r = gtid; r < N + 2; r += gsz) w.cnt[r] = 0;
   grid.sync();
   // ---- 1: bucket every merged row
-  for (int i = gtid; i < N; i += gsz) {
-    const int b = (int)row_bucket(merged_row(X, C, P, D, i), D, w.H);
-    w.ndom[i] = b;
-    w.next[i] = atomicExch(&w.head[b], i);
-  }
+  bucket_rows(X, C, P, D, w, gtid, gsz);
   grid.sync();
   // ---- 2: duplicate children
   for (int i = P + gtid; i < N; i += gsz) {
-    const float *me = C + (int64_t)(i - P) * D;
-    bool dup = false;
-    for (int j = __ldcg(&w.head[__ldcg(&w.ndom[i])]); j >= 0 && !dup; j = __ldcg(&w.next[j]))
-      dup = j < i && same_row(merged_row(X, C, P, D, j), me, D);
+    const bool dup = dup_in_bucket(X, C, P, D, w, i);
     float gi = __ldcg(w.g + i);
     if (dup) {
       f0[i] = f1[i] = f2[i] = INFINITY;
@@ -691,25 +726,114 @@ __global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const fl
   int total = 0;
   for (int b = 0; b < (int)gridDim.x; ++b) total += __ldcg(w.bsum + b);
   // ---- 9: coalesced copy of the survivors
-  const int e = D - d;
-  for (int64_t q = gtid; q < (int64_t)total * D; q += gsz) {
-    const int r = (int)(q / D), k = (int)(q % D);
-    Xn[q] = merged_row(X, C, P, D, __ldcg(w.sel + r))[k];
-  }
   for (int64_t q = gtid; q < (int64_t)total * 3; q += gsz) {
     const int r = (int)(q / 3), k = (int)(q % 3);
     Fn[q] = __ldcg(w.f + k * N + __ldcg(w.sel + r));
   }
   if (Gn)
     for (int q = gtid; q < total; q += gsz) Gn[q] = __ldcg(w.g + __ldcg(w.sel + q));
-  for (int64_t q = gtid; q < (int64_t)total * d; q += gsz) {
-    const int r = (int)(q / d), k = (int)(q % d);
-    Xcn[q] = merged_row(X, C, P, D, __ldcg(w.sel + r))[k];
+  copy_survivors(X, C, P, D, d, w.sel, total, Xn, Xcn, Xen, gtid, gsz);
+}
+
+// ---- single-objective survival (hb_ga_survive): pymoo's FitnessSurvival as MixedVariableGA runs it for a one-objective
+// acquisition (evolution_optimizer.py:123-124,132-133).  The ordering rule is recalled from pymoo 0.6 -- np.lexsort([F, cv])
+// then pop[S[:n_survive]], no constraint here -- and was not checked against pymoo.  On the merged rows (population
+// 0..P-1, offspring P..2P-1, one objective f each):
+//  * sanitising: a non-finite f becomes +inf;
+//  * duplicates: the predicate of the NSGA-II survival above (|o[k] - me[k]| <= 1e-16f in every column against any
+//    earlier merged row); a duplicate child gets f = +inf;
+//  * survivors: the P merged rows first in ascending (f, merged index) order, written in that order (row 0 = the best);
+//    F_next holds the sanitised f.
+// A row's output slot is its rank, the count of merged rows with a smaller (f, index) key.  The keys are distinct, so the
+// ranks are a permutation and a row with rank < P writes its slot directly: no scan, no float atomics, the same bytes from
+// both kernels and from run to run.
+__global__ void __launch_bounds__(NSGA_MAX) ga_survive_kernel(const float *__restrict__ X, const float *__restrict__ F,
+                                                              const float *__restrict__ C, const float *__restrict__ FC, int P,
+                                                              int D, int d, float *__restrict__ Xn, float *__restrict__ Fn,
+                                                              float *__restrict__ Xcn, int32_t *__restrict__ Xen) {
+  __shared__ float f[NSGA_MAX];
+  const int N = 2 * P, i = threadIdx.x;
+  const bool on = i < N;
+  if (on) {
+    f[i] = sanitize_obj(i < P ? F[i] : FC[i - P]);
+    if (i >= P && dup_of_earlier(X, C, P, D, i)) f[i] = INFINITY;
   }
-  for (int64_t q = gtid; q < (int64_t)total * e; q += gsz) {
-    const int r = (int)(q / e), k = (int)(q % e);
-    Xen[q] = (int32_t)rintf(merged_row(X, C, P, D, __ldcg(w.sel + r))[d + k]);
+  __syncthreads();
+  if (!on) return;
+  int rank = 0;
+  for (int j = 0; j < N; ++j) rank += before_asc(f[j], j, f[i], i) ? 1 : 0;
+  if (rank >= P) return;
+  const float *src = merged_row(X, C, P, D, i);
+  float *row = Xn + (int64_t)rank * D;
+  for (int k = 0; k < D; ++k) row[k] = src[k];
+  Fn[rank] = f[i];
+  split_row(src, d, D - d, Xcn + (int64_t)rank * d, Xen + (int64_t)rank * (D - d));
+}
+
+// multi-CTA form for 512 < 2P <= 32768: duplicates through the bucket table, ranks by the tiled count, then the copy
+__global__ void __launch_bounds__(NSGA_LT, 2) ga_survive_large_kernel(const float *__restrict__ X, const float *__restrict__ F,
+                                                                      const float *__restrict__ C, const float *__restrict__ FC,
+                                                                      int P, int D, int d, float *__restrict__ Xn,
+                                                                      float *__restrict__ Fn, float *__restrict__ Xcn,
+                                                                      int32_t *__restrict__ Xen, const SurviveWs w_arg) {
+  namespace cg = cooperative_groups;
+  SurviveWs w = w_arg;
+  cg::grid_group grid = cg::this_grid();
+  __shared__ SweepEntry tile[NSGA_TJ];
+  const int N = 2 * P;
+  const int gtid = blockIdx.x * blockDim.x + threadIdx.x, gsz = gridDim.x * blockDim.x;
+  // ---- 0: sanitise, clear the bucket table
+  for (int i = gtid; i < N; i += gsz) w.f[i] = sanitize_obj(i < P ? F[i] : FC[i - P]);
+  for (int h = gtid; h < w.H; h += gsz) w.head[h] = -1;
+  grid.sync();
+  // ---- 1: bucket every merged row
+  bucket_rows(X, C, P, D, w, gtid, gsz);
+  grid.sync();
+  // ---- 2: duplicate children
+  for (int i = P + gtid; i < N; i += gsz)
+    if (dup_in_bucket(X, C, P, D, w, i)) w.f[i] = INFINITY;
+  grid.sync();
+  // ---- 3: rank = count of smaller (f, index) keys; the survivors write their output slot
+  auto key = [&](int j) {
+    SweepEntry e;
+    e.v[0] = __ldcg(w.f + j);
+    e.v[1] = e.v[2] = 0.0f;
+    e.id = j;
+    return e;
+  };
+  team_sweep(
+      tile, N, N, [&](int r, SweepEntry &me) { me = key(r); return true; }, key,
+      [](const SweepEntry &me, const SweepEntry &o, int *acc) { acc[0] += before_asc(o.v[0], o.id, me.v[0], me.id) ? 1 : 0; },
+      [&](int r, const SweepEntry &, const int *acc) {
+        if (acc[0] < P) w.sel[acc[0]] = r;
+      });
+  grid.sync();
+  // ---- 4: coalesced copy of the survivors
+  for (int q = gtid; q < P; q += gsz) Fn[q] = __ldcg(w.f + __ldcg(w.sel + q));
+  copy_survivors(X, C, P, D, d, w.sel, P, Xn, Xcn, Xen, gtid, gsz);
+}
+
+// CTAs of a cooperative survival kernel: co-resident CTAs on the current device (at most 2 per SM, looked up once per
+// device), no more than row passes of the N-row sweeps, and no more than the per-CTA counts the workspace holds
+template <class Kernel>
+static int survive_grid(Kernel kernel, PerDevice &once, int64_t P, int *grid) {
+  bool fresh = false;
+  const int dev = once.slot(&fresh);
+  if (dev < 0) return HB_ERR_CUDA;
+  if (fresh) {
+    int sms = 0, per_sm = 0, coop = 0;
+    HB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    HB_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
+    HB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, NSGA_LT, 0));
+    if (!coop || per_sm < 1) {
+      set_error(cudaErrorNotSupported, "nsga_survive: cooperative launch unavailable");
+      return HB_ERR_CUDA;
+    }
+    once.aux[dev] = sms * min(per_sm, 2);
+    once.done[dev] = true;
   }
+  *grid = (int)std::min<int64_t>({(int64_t)once.aux[dev], ceil_div(2 * P, NSGA_ROWS), (int64_t)NSGA_GRID_MAX});
+  return HB_OK;
 }
 int launch_nsga_init(float *X, int64_t P, int64_t D, int64_t d, const int32_t *kind, const float *lb, const float *ub,
                      const float *fixed, const float *init, int64_t n_init, uint64_t seed, float *Xc, int32_t *Xe, cudaStream_t st) {
@@ -748,29 +872,38 @@ int launch_nsga_survive(const float *X, const float *F, const float *G, const fl
   }
   if (!ws || ws_bytes < (int64_t)nsga_survive_ws_bytes(P)) return HB_ERR_INVALID;
   static PerDevice once;   // aux[dev] = co-resident CTAs of the cooperative survival kernel on that device
-  bool fresh = false;
-  const int dev = once.slot(&fresh);
-  if (dev < 0) return HB_ERR_CUDA;
-  if (fresh) {
-    int sms = 0, per_sm = 0, coop = 0;
-    HB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    HB_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
-    HB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, nsga_survive_large_kernel, NSGA_LT, 0));
-    if (!coop || per_sm < 1) {
-      set_error(cudaErrorNotSupported, "nsga_survive: cooperative launch unavailable");
-      return HB_ERR_CUDA;
-    }
-    once.aux[dev] = sms * min(per_sm, 2);
-    once.done[dev] = true;
-  }
-  // no more CTAs than row passes of the N-row sweeps, and no more than the per-CTA survivor counts the workspace holds
-  const int grid = (int)std::min<int64_t>({(int64_t)once.aux[dev], ceil_div(2 * P, NSGA_ROWS), (int64_t)NSGA_GRID_MAX});
+  int grid = 0;
+  const int rc = survive_grid(nsga_survive_large_kernel, once, P, &grid);
+  if (rc != HB_OK) return rc;
   SurviveWs w = nsga_carve(ws, P);
   int Pi = (int)P, Di = (int)D, di = (int)d;
   void *args[] = {&X, &F, &G, &C, &FC, &GC, &Pi, &Di, &di, &Xn, &Fn, &Gn, &Xcn, &Xen, &w};
   HB_CUDA(cudaLaunchCooperativeKernel((const void *)nsga_survive_large_kernel, dim3(grid), dim3(NSGA_LT), args, 0, st));
   count_launches(1);
   HB_LAUNCH_CHECK("nsga_survive_large");
+  return HB_OK;
+}
+
+int launch_ga_survive(const float *X, const float *F, const float *C, const float *FC, int64_t P, int64_t D, int64_t d,
+                      float *Xn, float *Fn, float *Xcn, int32_t *Xen, void *ws, int64_t ws_bytes, cudaStream_t st) {
+  if (P <= 0 || P > NSGA_LARGE_MAX_POP || D <= 0 || d < 0 || d > D) return HB_ERR_INVALID;
+  if (2 * P <= NSGA_MAX) {
+    ga_survive_kernel<<<1, (int)round_up(2 * P, 32), 0, st>>>(X, F, C, FC, (int)P, (int)D, (int)d, Xn, Fn, Xcn, Xen);
+    count_launches(1);
+    HB_LAUNCH_CHECK("ga_survive");
+    return HB_OK;
+  }
+  if (!ws || ws_bytes < (int64_t)nsga_survive_ws_bytes(P)) return HB_ERR_INVALID;
+  static PerDevice once;   // aux[dev] = co-resident CTAs of the cooperative GA survival kernel on that device
+  int grid = 0;
+  const int rc = survive_grid(ga_survive_large_kernel, once, P, &grid);
+  if (rc != HB_OK) return rc;
+  SurviveWs w = nsga_carve(ws, P);
+  int Pi = (int)P, Di = (int)D, di = (int)d;
+  void *args[] = {&X, &F, &C, &FC, &Pi, &Di, &di, &Xn, &Fn, &Xcn, &Xen, &w};
+  HB_CUDA(cudaLaunchCooperativeKernel((const void *)ga_survive_large_kernel, dim3(grid), dim3(NSGA_LT), args, 0, st));
+  count_launches(1);
+  HB_LAUNCH_CHECK("ga_survive_large");
   return HB_OK;
 }
 

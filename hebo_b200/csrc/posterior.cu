@@ -322,6 +322,31 @@ int launch_mace_only(const float *mu, const float *var, int64_t m, float noise_v
   return HB_OK;
 }
 
+// single-objective acquisitions over (mu, var) (acq.py:55-82, nomr.py:32-34), each the reference's torch expression in
+// IEEE fp32 with every rounding explicit, so that no FMA contraction changes a bit
+__global__ void __launch_bounds__(256) acq1_kernel(const float *__restrict__ mu, const float *__restrict__ var, int64_t m,
+                                                   int mode, float kappa, float eta, float *__restrict__ f) {
+  const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= m) return;
+  const float py = mu[r], ps = __fsqrt_rn(var[r]);
+  float v;
+  switch (mode) {
+    case HB_ACQ1_LCB: v = __fsub_rn(py, __fmul_rn(kappa, ps)); break;                       // py - kappa * ps2.sqrt()
+    case HB_ACQ1_MEAN: v = py; break;                                                      // py
+    case HB_ACQ1_SIGMA: v = __fmul_rn(-1.0f, ps); break;                                   // -1 * ps2.sqrt()
+    default: v = __fsub_rn(fabsf(__fsub_rn(py, eta)), __fmul_rn(kappa, ps)); break;       // |py - eta| - kappa * ps2.sqrt()
+  }
+  f[r] = v;
+}
+
+int launch_acq1(const float *mu, const float *var, int64_t m, int mode, float kappa, float eta, float *f, cudaStream_t st) {
+  if (m <= 0 || mode < HB_ACQ1_LCB || mode > HB_ACQ1_ABS_ETA) return HB_ERR_INVALID;
+  acq1_kernel<<<(int)ceil_div(m, 256), 256, 0, st>>>(mu, var, m, mode, kappa, eta, f);
+  count_launches(1);
+  HB_LAUNCH_CHECK("acq1");
+  return HB_OK;
+}
+
 
 __global__ void __launch_bounds__(256) mace_kernel(const float *__restrict__ mupart, int ncg,
                                                    const float *__restrict__ vpart, int nt,

@@ -14,7 +14,9 @@ device), which replaces the per-individual marshalling of evolution_optimizer.py
 repair, duplicate elimination and rank-and-crowding survival in CUDA kernels, hebo_b200/csrc/nsga.cu; no per-generation
 host round trip); the numpy functions in this file restate the same operators on the host and serve as the checker of
 those kernels (tests/test_evolution.py, tests/test_gpu_nsga.py).  The default optimiser of suggest() is the one-pass Sobol
-mega-batch.
+mega-batch.  With a one-objective score `DeviceNSGA2` is the single-objective GA of the reference (pymoo's
+MixedVariableGA, evolution_optimizer.py:123-124,132-133): the same mating, the fitness survival of `hb_ga_survive`
+(restated by `ga_survive_host`); `hebo_b200.BO` runs it.
 """
 from __future__ import annotations
 
@@ -80,6 +82,27 @@ def rank_and_crowding_survival(F: np.ndarray, n_survive: int) -> np.ndarray:
         if len(keep) >= n_survive:
             break
     return np.asarray(keep, dtype=np.int64)
+
+
+def ga_survive_host(X: np.ndarray, F: np.ndarray, C: np.ndarray, FC: np.ndarray):
+    """numpy restatement of hb_ga_survive in fp32: a non-finite f becomes +inf, a duplicate child (the predicate of
+    survive_host) gets +inf, and the P merged rows first in ascending (f, merged index) order survive in that order.
+    Returns the merged indices of the survivors in output order (best first) and the sanitised f [2P]."""
+    P = X.shape[0]
+    Xa = np.concatenate([X, C], 0).astype(np.float32)
+    f = np.concatenate([np.asarray(F).reshape(-1), np.asarray(FC).reshape(-1)]).astype(np.float32)
+    f = np.where(np.isfinite(f), f, np.float32(np.inf))
+    # rows the predicate calls equal share a key (0 for |v| < 2^-20, else the bit pattern: the fp32 spacing above 2^-20
+    # exceeds 1e-16), so each child is tested against the earlier rows of its key only -- the exact predicate, in O(N D)
+    key = np.where(np.abs(Xa) < np.float32(2.0 ** -20), np.uint32(0), Xa.view(np.uint32))
+    earlier = {}
+    for i in range(2 * P):
+        rows = earlier.setdefault(key[i].tobytes(), [])
+        if i >= P and rows and (np.abs(Xa[rows] - Xa[i]) <= np.float32(1e-16)).all(1).any():
+            f[i] = np.inf
+        rows.append(i)
+    order = np.lexsort((np.arange(2 * P), f))          # primary f, ties by the lower merged index
+    return order[:P], f
 
 
 def survive_host(X: np.ndarray, F: np.ndarray, C: np.ndarray, FC: np.ndarray, G: Optional[np.ndarray] = None,
@@ -240,16 +263,21 @@ class EvolutionOpt:
 
 
 class DeviceNSGA2:
-    """NSGA-II over the MACE objectives with the population resident on the GPU (include/hebo_b200.h "device NSGA-II").
+    """The evolutionary acquisition optimiser with the population resident on the GPU (include/hebo_b200.h "device
+    NSGA-II"): NSGA-II over the MACE objectives, or the single-objective GA -- as in the reference, the algorithm follows
+    from the number of objectives (evolution_optimizer.py:123-124,132-133).
 
     kinds [D]: 'real' | 'int' | 'choice' per optimisation column (numeric columns first, then the categorical ones:
     evolution_optimizer.py:26-41); lb / ub [D]; fixed: {column index: value} (fix_input, :97-101).  `score(Xc, Xe, gen)`
-    returns the objectives F [pop, 3] of a batch as a device tensor (the fused posterior + MACE call).  2 <= pop <= 16384:
+    returns the objectives of a batch as a device tensor: F [pop, 3] (the fused posterior + MACE call; rank-and-crowding
+    survival, hb_nsga2_survive_ex) or one column, F [pop] or [pop, 1] (e.g. hebo_b200.acq.ga_score; fitness survival,
+    hb_ga_survive, and the result is the best row).  Any other column count raises ValueError.  2 <= pop <= 16384:
     survival runs in one CTA up to pop 256 and in a cooperative multi-CTA kernel above, with the same results.
 
     constrained=True: `score` returns (F [pop, 3], G [pop]) with one constraint column (feasible iff G <= 0, the pymoo
     constraint of evolution_optimizer.py:82,105); survival is hb_nsga2_survive_cv and the result is the feasible front
-    (hebo_b200.pareto.feasible_front).  The generation loop still never synchronises with the host."""
+    (hebo_b200.pareto.feasible_front).  The generation loop still never synchronises with the host.  There is no
+    constrained single-objective GA: constrained=True with a one-column score raises ValueError."""
 
     KIND = {"real": 0, "int": 1, "choice": 2}
     MAX_POP = 16384                                 # hb_nsga2_survive_ex: single CTA up to 256, cooperative multi-CTA above
@@ -274,6 +302,7 @@ class DeviceNSGA2:
         self.constrained = bool(constrained)
         self.seed = int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed)
         self.n_evals = 0
+        self.num_obj = None            # set by the first scored batch: 1 (GA) or 3 (NSGA-II)
 
     def _bufs(self):
         t, dev, P, D, d = self.torch, self.dev, self.pop, self.D, self.d
@@ -282,7 +311,9 @@ class DeviceNSGA2:
 
     def optimize(self, initial_suggest=None):
         """Returns (Xc [K, d] fp32, Xe [K, e] int32, F [K, 3]) of the non-dominated members of the final population
-        (res.X of evolution_optimizer.py:141-149), all on the device; with constraints, of its feasible front."""
+        (res.X of evolution_optimizer.py:141-149), all on the device; with constraints, of its feasible front.  With a
+        one-column score: (Xc [1, d], Xe [1, e], F [1, 1]) of the best member (the first minimum of the sanitised f, which
+        after a survival is row 0), res.X of a single-objective run."""
         from . import _lib
         from .pareto import feasible_front, pareto_front
         t, lib, P, D, d = self.torch, _lib.lib(), self.pop, self.D, self.d
@@ -308,7 +339,10 @@ class DeviceNSGA2:
                 _lib.check(lib.hb_nsga2_mate(_lib.ptr(X), P, D, d, _lib.ptr(self.kind), _lib.ptr(self.lb), _lib.ptr(self.ub),
                                              _lib.ptr(self.fixed), self.seed, gen, _lib.ptr(C), pc(Cc), pc(Ce), st()), "hb_nsga2_mate")
                 FC, GC = self._scored(Cc, Ce, gen)
-                if G is None:
+                if self.num_obj == 1:
+                    _lib.check(lib.hb_ga_survive(_lib.ptr(X), _lib.ptr(F), _lib.ptr(C), _lib.ptr(FC), P, D, d, _lib.ptr(Xn), _lib.ptr(Fn),
+                                                 pc(Xcn), pc(Xen), _lib.ptr(ws), ws_bytes, st()), "hb_ga_survive")
+                elif G is None:
                     _lib.check(lib.hb_nsga2_survive_ex(_lib.ptr(X), _lib.ptr(F), _lib.ptr(C), _lib.ptr(FC), P, D, d, _lib.ptr(Xn),
                                                        _lib.ptr(Fn), pc(Xcn), pc(Xen), _lib.ptr(ws), ws_bytes, st()), "hb_nsga2_survive_ex")
                 else:
@@ -319,13 +353,23 @@ class DeviceNSGA2:
                 X, Xn, Xc, Xcn, Xe, Xen, F, Fn = Xn, X, Xcn, Xc, Xen, Xe, Fn, F
                 self.n_evals += P
         self.pop_X, self.pop_F, self.pop_G = X, F, G
+        if self.num_obj == 1:
+            f = t.where(t.isfinite(F), F, t.full_like(F, float("inf")))
+            idx = t.argmin(f).reshape(1)
+            return Xc[idx], Xe[idx], F[idx].reshape(1, 1)
         idx = pareto_front(F) if G is None else feasible_front(F, G)
         return Xc[idx], Xe[idx], F[idx]
 
     def _scored(self, Xc, Xe, gen):
-        """(F [n, 3], G [n] or None) of a batch, contiguous fp32 on the device."""
+        """(F [n, 3] or [n], G [n] or None) of a batch, contiguous fp32 on the device."""
         out = self.score(Xc, Xe, gen)
-        if not self.constrained:
-            return out.contiguous(), None
-        F, G = out
-        return F.contiguous(), G.reshape(-1).to(self.torch.float32).contiguous()
+        F, G = out if self.constrained else (out, None)
+        F = F.reshape(self.pop, -1)
+        if F.shape[1] not in (1, 3):
+            raise ValueError(f"DeviceNSGA2: the score must have 1 or 3 columns, got {F.shape[1]}")
+        if F.shape[1] == 1 and self.constrained:
+            raise ValueError("DeviceNSGA2: constrained=True needs the 3 MACE columns; a one-column score has no constrained GA")
+        self.num_obj = F.shape[1]
+        F = F.reshape(-1) if self.num_obj == 1 else F
+        G = None if G is None else G.reshape(-1).to(self.torch.float32)
+        return F.to(self.torch.float32).contiguous(), None if G is None else G.contiguous()

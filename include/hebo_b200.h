@@ -293,6 +293,23 @@ int32_t hb_sample_y(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, 
 int32_t hb_mace_epilogue(const float *mu, const float *var, int64_t m, float noise_var, float tau, float kappa,
                          float eps, const float *xi1, const float *xi2, uint64_t seed, float *F, void *stream);
 
+/* ---- single-objective acquisitions  (LCB / Mean / Sigma.eval, acquisitions/acq.py:55-82, and AbsEtaDifference.eval,
+ * optimizers/nomr.py:25-34, over the mu / var that hb_posterior_mace_ex writes with F = NULL) ----
+ * mu, var [m] device; f [m] out, one launch.  Each mode is the reference's torch expression in fp32 (py = mu, ps2 = var):
+ *   HB_ACQ1_LCB      py - kappa * ps2.sqrt()
+ *   HB_ACQ1_MEAN     py
+ *   HB_ACQ1_SIGMA    -1 * ps2.sqrt()
+ *   HB_ACQ1_ABS_ETA  abs(py - eta) - kappa * ps2.sqrt()
+ * with correctly rounded sqrt, products and differences and no FMA contraction: bit-identical to the IEEE fp32 evaluation
+ * of the same expression on the same mu / var.  torch's CPU sqrt (MKL VML, < 1 ulp) is not always correctly rounded, so the
+ * reference's CPU eval may differ from it by one ulp.  kappa / eta are ignored by the modes that do not use them.  m >= 1. */
+#define HB_ACQ1_LCB        0
+#define HB_ACQ1_MEAN       1
+#define HB_ACQ1_SIGMA      2
+#define HB_ACQ1_ABS_ETA    3
+int32_t hb_acq1_epilogue(const float *mu, const float *var, int64_t m, int32_t mode, float kappa, float eta, float *f,
+                         void *stream);
+
 /* ---- 3-objective non-dominated filter  (the rank-0 set NSGA-II returns as res.X,
  * acq_optimizers/evolution_optimizer.py:141-149) ----------------------------------------------
  * F [m,3]; idx_out [m] int32 ascending indices of the non-dominated rows; count device int32.
@@ -333,6 +350,16 @@ int32_t hb_nsga2_survive_ex(const float *X, const float *F, const float *C, cons
 int32_t hb_nsga2_survive_cv(const float *X, const float *F, const float *G, const float *C, const float *FC, const float *GC,
                             int64_t pop, int64_t D, int64_t d, float *X_next, float *F_next, float *G_next, float *Xc_next,
                             int32_t *Xe_next, void *ws, int64_t ws_bytes, void *stream);
+/* hb_ga_survive: the survival of the single-objective GA (pymoo MixedVariableGA's FitnessSurvival, which EvolutionOpt runs
+ *   when the acquisition has one objective: evolution_optimizer.py:123-124,132-133; the order np.lexsort([F, cv]) then
+ *   pop[S[:n_survive]] is recalled from pymoo 0.6, not checked against it).  Mating is unchanged: hb_nsga2_init /
+ *   hb_nsga2_mate.  F [pop] / FC [pop] one objective per merged row (population rows 0..pop-1, offspring pop..2 pop-1).
+ *   A non-finite f counts as +inf; a duplicate child (the predicate of hb_nsga2_survive_ex) gets f = +inf.  The survivors
+ *   are the pop merged rows first in ascending (f, merged index) order, written in that order (row 0 is the best);
+ *   F_next [pop] holds their sanitised f, Xc_next / Xe_next the split rows.  Same sizes and workspace as
+ *   hb_nsga2_survive_ex (ws may be NULL when pop <= 256); both kernels give the same bytes, deterministic, one launch. */
+int32_t hb_ga_survive(const float *X, const float *F, const float *C, const float *FC, int64_t pop, int64_t D, int64_t d,
+                      float *X_next, float *F_next, float *Xc_next, int32_t *Xe_next, void *ws, int64_t ws_bytes, void *stream);
 
 /* ---- bound violation of a random embedding  (MACE_Embedding.eval, optimizers/hebo_embedding.py:85-90, clip = False)
  * Y [m, e] candidates in the embedding, B [e, D] projection matrix, both row-major fp32 on the device; G [m] out:
