@@ -87,6 +87,8 @@ SIGNATURES = {
     "hb_sample_workspace_bytes": (_i64, [_i64, _i64, _sp, _i64]),
     "hb_sample_y": (_i32, [_vp, _vp, _i64, _i64, _i64, _sp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _f32, _f32, _i32, _vp, _i32,
                            _vp, C.POINTER(C.c_float), _vp, _i64, _vp]),
+    "hb_sample_y_batch": (_i32, [_vp, _vp, _i64, _i64, _i64, _sp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _f32, _f32, _i32, _vp,
+                                 _u64, _u64, _vp, _vp, _vp, _vp, _i64, _vp]),
     "hb_mace_epilogue": (_i32, [_vp, _vp, _i64, _f32, _f32, _f32, _f32, _vp, _vp, _u64, _vp, _vp]),
     "hb_acq1_epilogue": (_i32, [_vp, _vp, _i64, _i32, _f32, _f32, _vp, _vp]),
     "hb_pareto_front3": (_i32, [_vp, _i64, _vp, _vp, _vp, _i64, _vp]),

@@ -80,16 +80,63 @@ class AbsEtaDifference(SingleObjectiveAcq):
         return torch.abs(py - self.eta) - self.kappa * ps2.sqrt()
 
 
+class NoisyAcq(Acquisition):
+    """acq.py:173-190: the acquisition is one joint posterior draw over the whole batch, ``model.sample_y(x, xe)``, which
+    is the CPU-tensor path for any model.  The device GA scores it through ``ga_score``."""
+
+    def __init__(self, model, num_obj, num_constr):
+        super().__init__(model)
+        self._num_obj = num_obj
+        self._num_constr = num_constr
+
+    @property
+    def num_obj(self):
+        return self._num_obj
+
+    @property
+    def num_constr(self):
+        return self._num_constr
+
+    def eval(self, x, xe):
+        with torch.no_grad():
+            return self.model.sample_y(x, xe).reshape(-1, self.num_obj + self.num_constr)
+
+
 # exact classes whose eval hb_acq1_epilogue restates; a subclass may override eval, so it takes the host path
 _ACQ1_MODES = {LCB: _lib.HB_ACQ1_LCB, Mean: _lib.HB_ACQ1_MEAN, Sigma: _lib.HB_ACQ1_SIGMA,
                AbsEtaDifference: _lib.HB_ACQ1_ABS_ETA}
 
 
-def ga_score(acq):
+def _noisy_device_score(model, seed: int):
+    """score(xc, xe, gen) of NoisyAcq over a fitted hebo_b200.GP: one hb_sample_y_batch per generation with counter = gen,
+    so every generation draws fresh N(0,1) values from the same seed.  The workspace is allocated at the first batch and
+    reused.  ``score.status`` is the device word a give-up of the jitter ladder sets to HB_ERR_NOT_PD; nothing in the
+    generation loop reads it."""
+    state = {}
+
+    def score(xc, xe, gen):
+        m = xc.shape[0] if model.d > 0 else xe.shape[0]
+        ws = state.get(m)
+        if ws is None:
+            ws = state[m] = torch.empty(model.sample_batch_workspace_bytes(m), dtype=torch.uint8, device=model.device)
+        return model.sample_y_batch(xc if model.d > 0 else None, xe if model.num_enum else None, seed, gen,
+                                    status=score.status, jitter=score.jitter, ws=ws)
+    score.status = torch.zeros(1, dtype=torch.int32, device=model.device)
+    score.jitter = torch.zeros(1, dtype=torch.float32, device=model.device)
+    return score
+
+
+def ga_score(acq, seed=None):
     """score(xc, xe, gen) -> f [m] fp32 on the device for DeviceNSGA2, of a single-objective acquisition.  xc [m, d] fp32
     and xe [m, e] int32 are device tensors.  With a hebo_b200.GP and one of the four acquisitions above: predict on the
-    device (hb_posterior_mace_ex with F = NULL) and hb_acq1_epilogue, no host synchronisation.  Otherwise: acq.eval on CPU
-    tensors (xe as int64, like the reference's BOProblem), its first column copied back to the device."""
+    device (hb_posterior_mace_ex with F = NULL) and hb_acq1_epilogue, no host synchronisation.  With a NoisyAcq of one
+    objective and no constraint over a fitted hebo_b200.GP: one joint draw per generation on the device
+    (``GP.sample_y_batch``, counter = the generation, ``seed`` drawn from numpy's global generator when None; batches of at
+    most 256 rows).  Otherwise: acq.eval on CPU tensors (xe as int64, like the reference's BOProblem), its first column
+    copied back to the device."""
+    if (type(acq) is NoisyAcq and acq.num_obj == 1 and acq.num_constr == 0 and isinstance(acq.model, GP)
+            and not acq.model._fit_failed):
+        return _noisy_device_score(acq.model, int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed))
     mode = _ACQ1_MODES.get(type(acq))
     if mode is not None and isinstance(acq.model, GP):
         kappa = float(getattr(acq, "kappa", 0.0))

@@ -804,6 +804,21 @@ int32_t hb_sample_y(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, 
                          y_std, pred_likeli, z, n_samples, out, jitter_used, ws, ws_bytes, (cudaStream_t)stream);
 }
 
+int32_t hb_sample_y_batch(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, int64_t d, const hb_model_spec_t *spec,
+                          const int32_t *emb_meta, const float *tab_s, const float *x_mul, const float *x_add, const float *Zt,
+                          const float *alpha, const float *Linv, const float *hyp, int32_t kern, float y_mean, float y_std,
+                          int32_t pred_likeli, const float *z, uint64_t seed, uint64_t counter, float *f, float *jitter,
+                          int32_t *status, void *ws, int64_t ws_bytes, void *stream) {
+  ModelSpec sp;
+  if (!build_spec(d, spec, sp)) return HB_ERR_INVALID;
+  if ((sp.d > 0 && (!Xs || !x_mul || !x_add)) || !Zt || !alpha || !Linv || !hyp || !f || !jitter || !status || !ws)
+    return HB_ERR_INVALID;
+  if (sp.e > 0 && (!Xe_s || !emb_meta || !tab_s)) return HB_ERR_INVALID;
+  bind_meta(sp, emb_meta, nullptr);
+  return launch_sample_y_batch(Xs, Xe_s, m, n, round_up(n, TILE), sp, tab_s, x_mul, x_add, Zt, alpha, Linv, hyp, kern, y_mean, y_std,
+                               pred_likeli, z, seed, counter, f, jitter, status, ws, ws_bytes, (cudaStream_t)stream);
+}
+
 int32_t hb_mace_epilogue(const float *mu, const float *var, int64_t m, float noise_var, float tau, float kappa,
                          float eps, const float *xi1, const float *xi2, uint64_t seed, float *F, void *stream) {
   if (!mu || !var || !F) return HB_ERR_INVALID;

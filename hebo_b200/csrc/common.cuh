@@ -175,6 +175,41 @@ __device__ __forceinline__ double warp_sum_d(double v) {
   return v;
 }
 
+// ---- Philox4x32-10 + Box-Muller: two N(0,1) draws per 64-bit counter `row` (the MACE epilogue's production noise and
+// the in-kernel draws of hb_sample_y_batch)
+__device__ __forceinline__ void philox_round(uint32_t (&c)[4], uint32_t k0, uint32_t k1) {
+  const uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u;
+  const uint32_t hi0 = __umulhi(M0, c[0]), lo0 = M0 * c[0];
+  const uint32_t hi1 = __umulhi(M1, c[2]), lo1 = M1 * c[2];
+  const uint32_t n0 = hi1 ^ c[1] ^ k0, n1 = lo1, n2 = hi0 ^ c[3] ^ k1, n3 = lo0;
+  c[0] = n0; c[1] = n1; c[2] = n2; c[3] = n3;
+}
+__device__ __forceinline__ void philox_normal2(uint64_t seed, uint64_t row, float &z0, float &z1) {
+  uint32_t c[4] = {(uint32_t)row, (uint32_t)(row >> 32), 0u, 0u};
+  uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    philox_round(c, k0, k1);
+    k0 += 0x9E3779B9u;
+    k1 += 0xBB67AE85u;
+  }
+  const float u0 = ((float)c[0] + 0.5f) * 2.3283064365386963e-10f;   // (0,1)
+  const float u1 = ((float)c[1] + 0.5f) * 2.3283064365386963e-10f;
+  const float rad = sqrtf(-2.0f * logf(u0));
+  float sn, cs;
+  sincospif(2.0f * u1, &sn, &cs);
+  z0 = rad * cs;
+  z1 = rad * sn;
+}
+
+// the duplicate predicate of the NSGA-II / GA survival (pymoo MixedVariableDuplicateElimination): |o[k] - me[k]| <= 1e-16f
+// in every one of the D columns
+__device__ __forceinline__ bool same_row(const float *o, const float *me, int D) {
+  bool same = true;
+  for (int k = 0; k < D && same; ++k) same = fabsf(o[k] - me[k]) <= 1e-16f;
+  return same;
+}
+
 // lower-triangular tile index decode: t -> (I >= J), t = I*(I+1)/2 + J
 __device__ __forceinline__ void tri_decode(int t, int &I, int &J) {
   int i = (int)((sqrtf(8.0f * (float)t + 1.0f) - 1.0f) * 0.5f);

@@ -169,6 +169,12 @@ int launch_sample_y(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, 
                     const float *x_mul, const float *x_add, const float *Zt, const float *alpha, const float *Linv, const float *hyp,
                     const float *hyp_host, int kern, float y_mean, float y_std, int pred_likeli, const float *z, int n_samples,
                     float *out, float *jitter_used, void *ws, int64_t ws_bytes, cudaStream_t st);
+// one joint draw f [m] over m <= 256 rows, duplicates dropped, jitter ladder on the device (hb_sample_y_batch)
+int launch_sample_y_batch(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, int64_t np, const ModelSpec &sp,
+                          const float *tab_s, const float *x_mul, const float *x_add, const float *Zt, const float *alpha,
+                          const float *Linv, const float *hyp, int kern, float y_mean, float y_std, int pred_likeli, const float *z,
+                          uint64_t seed, uint64_t counter, float *f, float *jitter_out, int32_t *status, void *ws, int64_t ws_bytes,
+                          cudaStream_t st);
 // nsga.cu
 int launch_nsga_init(float *X, int64_t P, int64_t D, int64_t d, const int32_t *kind, const float *lb, const float *ub,
                      const float *fixed, const float *init, int64_t n_init, uint64_t seed, float *Xc, int32_t *Xe, cudaStream_t st);

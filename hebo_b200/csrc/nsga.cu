@@ -163,11 +163,7 @@ __device__ __forceinline__ bool dominates3(float a0, float a1, float a2, float b
   return le && lt;
 }
 
-__device__ __forceinline__ bool same_row(const float *o, const float *me, int D) {
-  bool same = true;
-  for (int k = 0; k < D && same; ++k) same = fabsf(o[k] - me[k]) <= 1e-16f;
-  return same;
-}
+// (same_row, common.cuh: the duplicate predicate, shared with hb_sample_y_batch)
 
 // (fj, j) before (fi, i) in ascending f order, ties by index; in descending crowding order, ties by index
 __device__ __forceinline__ bool before_asc(float fj, int j, float fi, int i) { return fj < fi || (fj == fi && j < i); }

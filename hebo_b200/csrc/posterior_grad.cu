@@ -313,4 +313,164 @@ int launch_sample_y(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, 
   return HB_OK;
 }
 
+// ---- one joint draw over a GA batch, m <= SB_MAX rows, with no host round trip (hb_sample_y_batch; NoisyAcq.eval,
+// acq.py:173-190, once per generation).  K*, V, K** and the rank-n update are the stages above; cov_update_kernel runs with
+// diag_base = 0, so the diagonal holds -|v_i|^2 and the kernel below adds s (+ sigma_n^2) + jitter itself, the same fp32
+// sum as launch_sample_y's diag_base - |v_i|^2.  Then one CTA:
+//   1. row i is dropped when it duplicates an earlier row of the batch (same_row on the numeric columns, equal categories);
+//   2. the distinct rows' lower triangle goes to packed shared memory (row a at a (a + 1) / 2) and is factored in place by
+//      a right-looking fp32 Cholesky; a pivot that is not positive and finite reloads it with jitter x10, from 1e-6 until
+//      the jitter exceeds 10 (launch_sample_y's ladder, same fp32 arithmetic);
+//   3. f = (c + sum of the mean partials + R z) y_std + y_mean for the distinct rows, +inf for the dropped ones; on give-up
+//      f = NaN everywhere and *status = HB_ERR_NOT_PD.
+constexpr int SB_MAX = 256;
+constexpr int SB_THREADS = 1024;
+constexpr size_t SB_SMEM = ((size_t)SB_MAX * (SB_MAX + 1) / 2 + 2 * SB_MAX) * sizeof(float) + 2 * SB_MAX * sizeof(int);
+
+__global__ void __launch_bounds__(SB_THREADS, 1) sample_batch_kernel(
+    const float *__restrict__ Xs, const int32_t *__restrict__ Xe_s, int m, int d, int e, const float *__restrict__ cov, int64_t mp,
+    const float *__restrict__ mupart, int ncg, const float *__restrict__ hyp, int pred_likeli, float y_mean, float y_std,
+    const float *__restrict__ z, uint64_t seed, uint64_t counter, float *__restrict__ f, float *__restrict__ jitter_out,
+    int32_t *__restrict__ status) {
+  extern __shared__ float sb_smem[];
+  float *A = sb_smem;                                   // packed lower triangle of the distinct rows
+  float *col = A + SB_MAX * (SB_MAX + 1) / 2;           // column j of L below the pivot
+  float *zv = col + SB_MAX;                             // z by batch row
+  int *idx = reinterpret_cast<int *>(zv + SB_MAX);      // batch row of distinct row a
+  int *dup = idx + SB_MAX;
+  __shared__ int k_s;
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5, nw = SB_THREADS / 32;
+  if (t < m) {
+    bool dp = false;
+    for (int j = 0; j < t && !dp; ++j) {
+      dp = same_row(Xs + (int64_t)j * d, Xs + (int64_t)t * d, d);
+      for (int c = 0; c < e && dp; ++c) dp = Xe_s[(int64_t)j * e + c] == Xe_s[(int64_t)t * e + c];
+    }
+    dup[t] = dp ? 1 : 0;
+    if (z) zv[t] = z[t];
+  }
+  if (!z && 2 * t < m) {
+    float z0, z1;
+    philox_normal2(seed, (counter << 7) + (uint64_t)t, z0, z1);   // rows 2t, 2t + 1 of draw `counter`
+    zv[2 * t] = z0;
+    if (2 * t + 1 < m) zv[2 * t + 1] = z1;
+  }
+  __syncthreads();
+  if (t < m && !dup[t]) {
+    int a = 0;
+    for (int j = 0; j < t; ++j) a += 1 - dup[j];
+    idx[a] = t;
+  }
+  if (t == 0) {
+    int k = 0;
+    for (int j = 0; j < m; ++j) k += 1 - dup[j];
+    k_s = k;
+  }
+  __syncthreads();
+  const int k = k_s;
+  const float sn2 = hyp[0], s = hyp[2];
+  const float base = s + (pred_likeli ? sn2 : 0.0f);
+  float jitter = 1e-6f;   // gpytorch psd_safe_cholesky: fp32 jitter 1e-6, x10 per retry (launch_sample_y's ladder)
+  bool ok = false;
+  for (;;) {
+    const float diag = base + jitter;
+    for (int a = warp; a < k; a += nw) {
+      const float *src = cov + (int64_t)idx[a] * mp;
+      float *row = A + a * (a + 1) / 2;
+      for (int b = lane; b <= a; b += 32) row[b] = (b == a) ? diag + src[idx[b]] : src[idx[b]];
+    }
+    __syncthreads();
+    bool fail = false;
+    for (int j = 0; j < k; ++j) {
+      const int jj = j * (j + 1) / 2 + j;
+      const float pv = A[jj];                            // the same word in every thread: the branch is uniform
+      if (!(pv > 0.0f) || !isfinite(pv)) {
+        fail = true;
+        break;
+      }
+      const float ljj = sqrtf(pv);
+      for (int i = j + 1 + t; i < k; i += SB_THREADS) {
+        const float c = A[i * (i + 1) / 2 + j] / ljj;
+        A[i * (i + 1) / 2 + j] = c;
+        col[i] = c;
+      }
+      __syncthreads();
+      if (t == 0) A[jj] = ljj;
+      for (int i = j + 1 + warp; i < k; i += nw) {
+        const float ci = col[i];
+        float *row = A + i * (i + 1) / 2;
+        for (int l = j + 1 + lane; l <= i; l += 32) row[l] = fmaf(-ci, col[l], row[l]);
+      }
+      __syncthreads();
+    }
+    if (!fail) {
+      ok = true;
+      break;
+    }
+    __syncthreads();                                     // every thread has read the failed pivot before the reload
+    jitter *= 10.0f;
+    if (jitter > 10.0f) break;
+  }
+  if (t == 0) *jitter_out = jitter;
+  if (!ok) {
+    if (t == 0) *status = HB_ERR_NOT_PD;
+    if (t < m) f[t] = NAN;
+    return;
+  }
+  if (t < m && dup[t]) f[t] = INFINITY;
+  for (int a = warp; a < k; a += nw) {
+    const int r = idx[a];
+    const float *row = A + a * (a + 1) / 2;
+    float acc = 0.0f;
+    for (int b = lane; b <= a; b += 32) acc = fmaf(row[b], zv[idx[b]], acc);
+    acc = warp_sum(acc);
+    if (lane == 0) {
+      float mu = hyp[1];
+      for (int g = 0; g < ncg; ++g) mu += mupart[(int64_t)g * mp + r];
+      f[r] = __fadd_rn(__fmul_rn(mu + acc, y_std), y_mean);
+    }
+  }
+}
+
+int launch_sample_y_batch(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, int64_t np, const ModelSpec &sp,
+                          const float *tab_s, const float *x_mul, const float *x_add, const float *Zt, const float *alpha,
+                          const float *Linv, const float *hyp, int kern, float y_mean, float y_std, int pred_likeli, const float *z,
+                          uint64_t seed, uint64_t counter, float *f, float *jitter_out, int32_t *status, void *ws, int64_t ws_bytes,
+                          cudaStream_t st) {
+  if (m <= 0 || m > SB_MAX || n <= 0 || np % GT != 0 || kern < 0 || kern > 2) return HB_ERR_INVALID;
+  if ((size_t)ws_bytes < sample_ws_bytes(np, sp.dtot(), m)) return HB_ERR_INVALID;
+  static PerDevice once;   // the opt-in above 48 KB of dynamic shared memory is per device
+  bool fresh = false;
+  const int dev = once.slot(&fresh);
+  if (dev < 0) return HB_ERR_CUDA;
+  if (fresh) {
+    HB_CUDA(cudaFuncSetAttribute(sample_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SB_SMEM));
+    once.done[dev] = true;
+  }
+  const int64_t mp = round_up(m, GT);       // the row tiles that hold the m rows (sample_ws_bytes pads to 2 GT)
+  const int ncg = kstar_groups(np);
+  float *KS = reinterpret_cast<float *>(ws);
+  float *Vb = KS + mp * np;
+  float *mupart = Vb + mp * np;
+  float *cov = mupart + (int64_t)ncg * mp;
+  float *ZsT = cov + mp * mp;
+  HB_CUDA(cudaMemsetAsync(KS, 0, (size_t)mp * np * sizeof(float), st));     // rows m..mp of K* must be zero for the GEMMs
+  int s = launch_kstar(Xs, Xe_s, m, sp, tab_s, x_mul, x_add, Zt, alpha, hyp, n, np, kern, KS, nullptr, mupart, mp, nullptr, nullptr, st);
+  if (s != HB_OK) return s;
+  rows_gemm_kernel<0><<<dim3((unsigned)(np / GT), (unsigned)(mp / GT)), GTHREADS, 0, st>>>(KS, Linv, np, Vb);
+  cand_features_kernel<<<(int)ceil_div((int64_t)sp.dtot() * mp, 256), 256, 0, st>>>(Xs, Xe_s, m, mp, x_mul, x_add, hyp, tab_s, sp, ZsT);
+  count_launches(2);
+  ModelSpec sc = sp;
+  sc.warp = 1;                        // "prescaled features" switch of gram_kernel: ZsT is already warped and divided by l
+  s = launch_gram(ZsT, ZsT + (int64_t)sp.d * mp, m, mp, sc, hyp, kern, nullptr, 0.0f, cov, st);
+  if (s != HB_OK) return s;
+  const int nt = (int)(mp / GT);
+  cov_update_kernel<<<nt * (nt + 1) / 2, GTHREADS, 0, st>>>(cov, mp, m, Vb, np, 0.0f);
+  sample_batch_kernel<<<1, SB_THREADS, SB_SMEM, st>>>(Xs, Xe_s, (int)m, sp.d, sp.e, cov, mp, mupart, ncg, hyp, pred_likeli, y_mean,
+                                                      y_std, z, seed, counter, f, jitter_out, status);
+  count_launches(2);
+  HB_LAUNCH_CHECK("sample_y_batch");
+  return HB_OK;
+}
+
 }  // namespace hb

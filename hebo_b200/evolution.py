@@ -309,11 +309,13 @@ class DeviceNSGA2:
         return (t.empty(P, D, device=dev), t.empty(P, max(d, 1), device=dev)[:, :d].contiguous() if d else t.empty(P, 0, device=dev),
                 t.empty(P, D - d, dtype=t.int32, device=dev))
 
-    def optimize(self, initial_suggest=None):
+    def optimize(self, initial_suggest=None, return_pop: bool = False):
         """Returns (Xc [K, d] fp32, Xe [K, e] int32, F [K, 3]) of the non-dominated members of the final population
         (res.X of evolution_optimizer.py:141-149), all on the device; with constraints, of its feasible front.  With a
         one-column score: (Xc [1, d], Xe [1, e], F [1, 1]) of the best member (the first minimum of the sanitised f, which
-        after a survival is row 0), res.X of a single-objective run."""
+        after a survival is row 0), res.X of a single-objective run.  return_pop=True with a one-column score: the whole
+        final population (Xc [pop, d], Xe [pop, e], F [pop, 1]) in survival order, ascending (sanitised f, row), as res.pop
+        of evolution_optimizer.py:148-151; after a survival that is the population's own order."""
         from . import _lib
         from .pareto import feasible_front, pareto_front
         t, lib, P, D, d = self.torch, _lib.lib(), self.pop, self.D, self.d
@@ -353,8 +355,13 @@ class DeviceNSGA2:
                 X, Xn, Xc, Xcn, Xe, Xen, F, Fn = Xn, X, Xcn, Xc, Xen, Xe, Fn, F
                 self.n_evals += P
         self.pop_X, self.pop_F, self.pop_G = X, F, G
+        if return_pop and self.num_obj != 1:
+            raise ValueError("DeviceNSGA2: return_pop=True needs a one-column score")
         if self.num_obj == 1:
             f = t.where(t.isfinite(F), F, t.full_like(F, float("inf")))
+            if return_pop:
+                idx = t.sort(f, stable=True).indices
+                return Xc[idx], Xe[idx], F[idx].reshape(-1, 1)
             idx = t.argmin(f).reshape(1)
             return Xc[idx], Xe[idx], F[idx].reshape(1, 1)
         idx = pareto_front(F) if G is None else feasible_front(F, G)

@@ -655,6 +655,33 @@ class GP(BaseModel):
             self.sample_jitter = jit.value
             return out.cpu().view(n_samples, m, self.num_out)
 
+    def sample_y_batch(self, Xs_dev, Xe_dev, seed: int, counter: int, z=None, status=None, jitter=None, ws=None):
+        """One joint draw over a batch of m <= 256 rows on the device (``hb_sample_y_batch``): f [m] fp32, +inf at a row that
+        duplicates an earlier row of the batch.  Xs_dev [m, d] fp32 / Xe_dev [m, e] int32 device tensors; z [m] device draws
+        or None for the in-kernel Philox draws of (seed, counter).  status: a device int32 word the call sets to
+        HB_ERR_NOT_PD when the jitter ladder gives up (f is then NaN); jitter: a device float for the jitter used; ws: a
+        workspace of ``sample_batch_workspace_bytes(m)`` bytes.  Nothing synchronises with the host, so a caller may issue
+        many calls and read ``status`` once."""
+        lib, dev = _lib.lib(), self.device
+        m = self._rows(Xs_dev, Xe_dev)
+        f = torch.empty(m, dtype=torch.float32, device=dev)
+        status = torch.zeros(1, dtype=torch.int32, device=dev) if status is None else status
+        jitter = torch.empty(1, dtype=torch.float32, device=dev) if jitter is None else jitter
+        ws = torch.empty(self.sample_batch_workspace_bytes(m), dtype=torch.uint8, device=dev) if ws is None else ws
+        with torch.cuda.device(dev):
+            st = lib.hb_sample_y_batch(_lib.ptr(Xs_dev) if self.d > 0 else None, _lib.ptr(Xe_dev) if self.num_enum else None, m,
+                                       self.n, self.d, self._spec_ptr(), _lib.ptr(self._emb_meta_dev) if self.num_enum else None,
+                                       _lib.ptr(self.tab_s_dev) if self.num_enum else None, _lib.ptr(self._x_mul), _lib.ptr(self._x_add),
+                                       _lib.ptr(self.Zt_dev), _lib.ptr(self.alpha_dev), _lib.ptr(self.Linv_dev), _lib.ptr(self.hyp_dev),
+                                       self.kern_id, self._y_mean, self._y_std, int(bool(self.pred_likeli)), _lib.ptr(z), int(seed),
+                                       int(counter), _lib.ptr(f), _lib.ptr(jitter), _lib.ptr(status), _lib.ptr(ws), ws.numel(),
+                                       _lib.stream_ptr())
+        _lib.check(st, "hb_sample_y_batch")
+        return f
+
+    def sample_batch_workspace_bytes(self, m: int) -> int:
+        return int(_lib.lib().hb_sample_workspace_bytes(self.n, self.d, self._spec_ptr(), m))
+
     def sample_f(self):
         raise NotImplementedError("Thompson sampling is not supported for GP, use `sample_y` instead")
 

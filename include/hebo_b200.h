@@ -287,6 +287,28 @@ int32_t hb_sample_y(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, 
                     float y_std, int32_t pred_likeli, const float *z, int32_t n_samples, float *out, float *jitter_used, void *ws,
                     int64_t ws_bytes, void *stream);
 
+/* ---- one joint sample of a GA batch on the device  (NoisyAcq.eval, acquisitions/acq.py:173-190: model.sample_y(x, xe),
+ * one correlated draw per generation; GP.sample_y, models/gp/gp.py:166-177) ------------------------------------------
+ * The fitted state and inputs of hb_sample_y (no host copy of hyp: sigma_n^2 and s are read from hyp on the device), with
+ * 1 <= m <= 256 rows and ws_bytes >= hb_sample_workspace_bytes(n, d, spec, m).
+ *   z [m] device N(0,1) draws by batch row, or NULL: in-kernel Philox4x32-10 + Box-Muller draws keyed by (seed, counter),
+ *     e.g. counter = the generation index; the same (seed, counter) gives the same f bit for bit.
+ *   f [m] device out: f = (mu~ + R z) y_std + y_mean, as hb_sample_y, over the DISTINCT rows.  A row equal to an earlier
+ *     row of the batch (the duplicate predicate of hb_ga_survive: |a - b| <= 1e-16 in every numeric column, equal
+ *     categories) is left out of the joint covariance, so that it cannot make it singular, and gets f = +inf; a distinct
+ *     row's f is what the de-duplicated batch gives it.  R is a right-looking fp32 Cholesky of the distinct rows'
+ *     covariance in one CTA, so f differs from hb_sample_y's (tile-DAG Cholesky) by the rounding of the factorisation.
+ *   jitter [1] device out: the jitter of the accepted factorisation (ladder 1e-6 x10 per failed attempt, as hb_sample_y,
+ *     run on the device); on give-up the last one tried.
+ *   status [1] device int32: set to HB_ERR_NOT_PD when the ladder gives up (then f = NaN in every row), otherwise left
+ *     unchanged, so one word zeroed by the caller collects the outcome of many calls.
+ * No host read and no synchronisation: the call can be captured in a CUDA graph.  Six launches and one memset. */
+int32_t hb_sample_y_batch(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, int64_t d, const hb_model_spec_t *spec,
+                          const int32_t *emb_meta, const float *tab_s, const float *x_mul, const float *x_add, const float *Zt,
+                          const float *alpha, const float *Linv, const float *hyp, int32_t kern, float y_mean, float y_std,
+                          int32_t pred_likeli, const float *z, uint64_t seed, uint64_t counter, float *f, float *jitter,
+                          int32_t *status, void *ws, int64_t ws_bytes, void *stream);
+
 /* ---- MACE epilogue alone  (MACE.eval, acquisitions/acq.py:151-171, over any model's predict output) ----
  * mu, var [m] in original y units (device); noise_var = model.noise (gp.py:182-184); xi1/xi2 as above.
  * F [m,3] out = (LCB, -logEI, -logPI). */
