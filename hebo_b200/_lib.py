@@ -16,6 +16,7 @@ KERNEL_IDS = {"matern32": 0, "matern52": 1, "rbf": 2}
 HB_ACQ1_LCB, HB_ACQ1_MEAN, HB_ACQ1_SIGMA, HB_ACQ1_ABS_ETA = 0, 1, 2, 3   # hb_acq1_epilogue modes
 HB_MAX_FEATURES = 4096   # d + sum(emb_sizes) a model may have (include/hebo_b200.h)
 HB_MAX_OUTPUTS = 32      # outputs one batched fit trains together (hb_fit_multi_ex)
+HB_MAX_OBJ = 8           # objectives of hb_nsga2_survive_k / hb_pareto_front_k
 
 
 class HeboB200Error(RuntimeError):
@@ -91,7 +92,9 @@ SIGNATURES = {
                                  _u64, _u64, _vp, _vp, _vp, _vp, _i64, _vp]),
     "hb_mace_epilogue": (_i32, [_vp, _vp, _i64, _f32, _f32, _f32, _f32, _vp, _vp, _u64, _vp, _vp]),
     "hb_acq1_epilogue": (_i32, [_vp, _vp, _i64, _i32, _f32, _f32, _vp, _vp]),
+    "hb_general_acq_epilogue": (_i32, [_vp, _vp, _i64, _i64, _i64, _f32, _f32, _vp, _vp, _u64, _u64, _vp, _vp, _vp, _vp]),
     "hb_pareto_front3": (_i32, [_vp, _i64, _vp, _vp, _vp, _i64, _vp]),
+    "hb_pareto_front_k": (_i32, [_vp, _i64, _i64, _vp, _vp, _vp, _i64, _vp]),
     "hb_nsga2_init": (_i32, [_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _u64, _vp, _vp, _vp]),
     "hb_nsga2_mate": (_i32, [_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _u64, _i32, _vp, _vp, _vp, _vp]),
     "hb_nsga2_survive": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp]),
@@ -99,6 +102,9 @@ SIGNATURES = {
     "hb_nsga2_survive_ex": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
     "hb_nsga2_survive_cv": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
     "hb_ga_survive": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
+    "hb_ga_survive_cv": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
+    "hb_nsga2_workspace_bytes_k": (_i64, [_i64, _i64, _i64]),
+    "hb_nsga2_survive_k": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
     "hb_embed_violation_workspace_bytes":(_i64, [_i64, _i64, _i64]),
     "hb_embed_violation": (_i32, [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _vp]),
     "hb_front_merge_workspace_bytes": (_i64, [_i64, _i64]),

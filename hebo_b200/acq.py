@@ -11,6 +11,9 @@ its offspring through ``ga_score``: ``LCB``, ``Mean``, ``Sigma`` and ``AbsEtaDif
 posterior call with F = NULL plus one ``hb_acq1_epilogue`` on the device: the ``eval`` expression in IEEE fp32 on the same
 mu / var (torch's CPU sqrt, used by ``eval``, may differ from the correctly rounded one by one ulp).  Any other single-objective acquisition -- another model, or a user's own class, including a subclass of these
 four -- is scored through its own ``eval`` on CPU tensors, once per generation, as the reference's EvolutionOpt does.
+
+``GeneralAcq`` (acq.py:192-242) is the LCB of every objective and constraint of a multi-output model, for ``GeneralBO``.
+Its ``eval`` runs on any model through ``hb_general_acq_epilogue``; ``general_score`` scores it for the device GA.
 """
 from __future__ import annotations
 
@@ -19,7 +22,7 @@ import torch
 
 from . import _lib
 from .base import Acquisition
-from .gp import GP
+from .gp import GP, MultiTaskModel
 
 
 class SingleObjectiveAcq(Acquisition):
@@ -159,6 +162,105 @@ def ga_score(acq, seed=None):
             v = acq(xc.cpu(), xe.cpu().long())
         return torch.as_tensor(v).reshape(xc.shape[0], -1)[:, 0].to(xc.device, torch.float32).contiguous()
     return host_score
+
+
+class GeneralAcq(Acquisition):
+    """acq.py:192-242: minimise (py - kappa ps) of the num_obj objectives subject to (py - c_kappa ps) <= 0 of the
+    num_constr constraints, ps = sqrt(ps2) clamped at FLT_EPSILON, with py + noise^0.5 xi when use_noise.  ``eval`` takes
+    the N(0,1) draws from torch's CPU generator as ``torch.randn(py.shape)``, like the reference, and runs the arithmetic in
+    the CUDA epilogue ``hb_general_acq_epilogue`` (correctly rounded fp32: torch's CPU sqrt may differ by one ulp).
+    Returns [m, num_obj + num_constr] on the input's device."""
+
+    def __init__(self, model, num_obj, num_constr, **conf):
+        super().__init__(model, **conf)
+        self._num_obj = num_obj
+        self._num_constr = num_constr
+        self.kappa = conf.get("kappa", 2.0)
+        self.c_kappa = conf.get("c_kappa", 0.)
+        self.use_noise = conf.get("use_noise", True)
+        assert self.model.num_out == self.num_obj + self.num_constr
+        assert self.num_obj >= 1
+
+    @property
+    def num_obj(self):
+        return self._num_obj
+
+    @property
+    def num_constr(self):
+        return self._num_constr
+
+    def eval(self, x, xe):
+        with torch.no_grad():
+            py, ps2 = self.model.predict(x, xe)
+            xi = torch.randn(py.shape) if self.use_noise else None
+            dev = torch.device("cuda")
+            mu = torch.as_tensor(py).to(dev, torch.float32).t().contiguous()        # [K, m], output-major
+            var = torch.as_tensor(ps2).to(dev, torch.float32).t().contiguous()
+            noise_sd = self.model.noise.reshape(-1).float().sqrt().to(dev).contiguous() if self.use_noise else None
+            xi = None if xi is None else xi.to(dev, torch.float32).contiguous()
+            Fo, Fc, _ = _general_epilogue(mu, var, self.num_obj, self.num_constr, self.kappa, self.c_kappa, noise_sd, xi,
+                                          want_fc=True)
+            out = torch.cat([Fo, Fc], 1)
+        probe = x if torch.is_tensor(x) else xe
+        return out.to(probe.device if torch.is_tensor(probe) else "cpu")
+
+
+def _general_epilogue(mu, var, num_obj, num_constr, kappa, c_kappa, noise_sd, xi, seed=0, counter=0, want_fc=False,
+                      want_cv=False):
+    """(Fo [m, num_obj], Fc [m, num_constr] or None, cv [m] or None) of hb_general_acq_epilogue over mu / var [K, m]."""
+    m, dev = mu.shape[1], mu.device
+    Fo = torch.empty(m, num_obj, dtype=torch.float32, device=dev)
+    Fc = torch.empty(m, num_constr, dtype=torch.float32, device=dev) if want_fc else None
+    cv = torch.empty(m, dtype=torch.float32, device=dev) if want_cv else None
+    if m:
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().hb_general_acq_epilogue(_lib.ptr(mu), _lib.ptr(var), m, num_obj, num_constr, float(kappa),
+                                                          float(c_kappa), _lib.ptr(noise_sd), _lib.ptr(xi), int(seed), int(counter),
+                                                          _lib.ptr(Fo), _lib.ptr(Fc) if num_constr else None, _lib.ptr(cv),
+                                                          _lib.stream_ptr()), "hb_general_acq_epilogue")
+    return Fo, Fc, cv
+
+
+def general_score(acq, seed=None):
+    """score(xc, xe, gen) of a GeneralAcq for DeviceNSGA2(num_obj=acq.num_obj, constrained=acq.num_constr > 0): Fo
+    [m, num_obj] fp32 on the device, and with constraints (Fo, cv [m]), cv the summed positive parts of the constraint
+    columns.  Over a hebo_b200.MultiTaskModel of GPs, or one GP: one posterior call per output with F = NULL, writing row b
+    of [K, m] buffers, then hb_general_acq_epilogue with Philox draws keyed by (seed, gen) -- no host synchronisation
+    inside a generation; an output whose fit failed predicts N(y_mean, y_std^2) as GP.predict does.  ``seed`` is drawn from
+    numpy's global generator when None.  Any other acquisition or model: acq.eval on CPU tensors (xe as int64), once per
+    generation."""
+    no, nc = acq.num_obj, acq.num_constr
+    model = acq.model
+    gps = None
+    if isinstance(model, GP):
+        gps = [model]
+    elif isinstance(model, MultiTaskModel) and all(isinstance(g, GP) for g in model.models):
+        gps = model.models
+    if type(acq) is not GeneralAcq or gps is None:
+        def host_score(xc, xe, gen):
+            with torch.no_grad():
+                v = torch.as_tensor(acq(xc.cpu(), xe.cpu().long())).reshape(xc.shape[0], no + nc).to(xc.device, torch.float32)
+            Fo = v[:, :no].contiguous()
+            if nc == 0:
+                return Fo
+            c = v[:, no:]
+            return Fo, torch.where(torch.isnan(c), c, c.clamp_min(0)).sum(1).contiguous()
+        return host_score
+    seed = int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed)
+    dev = gps[0].device
+    noise_sd = model.noise.reshape(-1).float().sqrt().to(dev).contiguous() if acq.use_noise else None
+    kappa, c_kappa = float(acq.kappa), float(acq.c_kappa)
+
+    def device_score(xc, xe, gen):
+        m = xc.shape[0]
+        mu = torch.empty(no + nc, m, dtype=torch.float32, device=dev)
+        var = torch.empty_like(mu)
+        with torch.no_grad():
+            for b, gp in enumerate(gps):
+                gp._posterior(gp._to_dev(xc), False, Xe_dev=gp._xe_dev(xe, m), out=(mu[b], var[b]))
+        Fo, _, cv = _general_epilogue(mu, var, no, nc, kappa, c_kappa, noise_sd, None, seed, gen, want_cv=nc > 0)
+        return (Fo, cv) if nc else Fo
+    return device_score
 
 
 class MACE(Acquisition):

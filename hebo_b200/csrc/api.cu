@@ -831,10 +831,24 @@ int32_t hb_acq1_epilogue(const float *mu, const float *var, int64_t m, int32_t m
   return launch_acq1(mu, var, m, mode, kappa, eta, f, (cudaStream_t)stream);
 }
 
+int32_t hb_general_acq_epilogue(const float *mu, const float *var, int64_t m, int64_t num_obj, int64_t num_constr, float kappa,
+                                float c_kappa, const float *noise_sd, const float *xi, uint64_t seed, uint64_t counter, float *Fo,
+                                float *Fc, float *cv, void *stream) {
+  if (!mu || !var || !Fo) return HB_ERR_INVALID;
+  return launch_general_acq(mu, var, m, num_obj, num_constr, kappa, c_kappa, noise_sd, xi, seed, counter, Fo, Fc, cv,
+                            (cudaStream_t)stream);
+}
+
 int32_t hb_pareto_front3(const float *F, int64_t m, int32_t *idx_out, int32_t *count, void *ws, int64_t ws_bytes,
                          void *stream) {
   if (!F || !idx_out || !count || !ws) return HB_ERR_INVALID;
-  return launch_pareto3(F, m, idx_out, count, ws, ws_bytes, (cudaStream_t)stream);
+  return launch_pareto_k(F, m, 3, idx_out, count, ws, ws_bytes, (cudaStream_t)stream);
+}
+
+int32_t hb_pareto_front_k(const float *F, int64_t m, int64_t num_obj, int32_t *idx_out, int32_t *count, void *ws, int64_t ws_bytes,
+                          void *stream) {
+  if (!F || !idx_out || !count || !ws || num_obj < 1 || num_obj > HB_MAX_OBJ) return HB_ERR_INVALID;
+  return launch_pareto_k(F, m, num_obj, idx_out, count, ws, ws_bytes, (cudaStream_t)stream);
 }
 
 int64_t hb_front_merge_workspace_bytes(int64_t world, int64_t capacity) {
@@ -870,17 +884,19 @@ int32_t hb_nsga2_survive(const float *X, const float *F, const float *C, const f
                          float *X_next, float *F_next, float *Xc_next, int32_t *Xe_next, void *stream) {
   if (!X || !F || !C || !FC || !X_next || !F_next || (d > 0 && !Xc_next) || (D > d && !Xe_next)) return HB_ERR_INVALID;
   if (pop > 256) return HB_ERR_INVALID;   // the workspace-free entry keeps the single-CTA limit
-  return launch_nsga_survive(X, F, nullptr, C, FC, nullptr, pop, D, d, X_next, F_next, nullptr, Xc_next, Xe_next, nullptr, 0,
+  return launch_nsga_survive(X, F, nullptr, C, FC, nullptr, pop, D, d, 3, X_next, F_next, nullptr, Xc_next, Xe_next, nullptr, 0,
                              (cudaStream_t)stream);
 }
 
-int64_t hb_nsga2_workspace_bytes(int64_t pop, int64_t D) { return nsga_survive_ws_query(pop, D); }
+int64_t hb_nsga2_workspace_bytes(int64_t pop, int64_t D) { return nsga_survive_ws_query(pop, D, 3); }
+
+int64_t hb_nsga2_workspace_bytes_k(int64_t pop, int64_t D, int64_t num_obj) { return nsga_survive_ws_query(pop, D, num_obj); }
 
 int32_t hb_nsga2_survive_ex(const float *X, const float *F, const float *C, const float *FC, int64_t pop, int64_t D,
                             int64_t d, float *X_next, float *F_next, float *Xc_next, int32_t *Xe_next, void *ws,
                             int64_t ws_bytes, void *stream) {
   if (!X || !F || !C || !FC || !X_next || !F_next || (d > 0 && !Xc_next) || (D > d && !Xe_next)) return HB_ERR_INVALID;
-  return launch_nsga_survive(X, F, nullptr, C, FC, nullptr, pop, D, d, X_next, F_next, nullptr, Xc_next, Xe_next, ws, ws_bytes,
+  return launch_nsga_survive(X, F, nullptr, C, FC, nullptr, pop, D, d, 3, X_next, F_next, nullptr, Xc_next, Xe_next, ws, ws_bytes,
                              (cudaStream_t)stream);
 }
 
@@ -889,14 +905,33 @@ int32_t hb_nsga2_survive_cv(const float *X, const float *F, const float *G, cons
                             int32_t *Xe_next, void *ws, int64_t ws_bytes, void *stream) {
   if (!X || !F || !G || !C || !FC || !GC || !X_next || !F_next || !G_next || (d > 0 && !Xc_next) || (D > d && !Xe_next))
     return HB_ERR_INVALID;
-  return launch_nsga_survive(X, F, G, C, FC, GC, pop, D, d, X_next, F_next, G_next, Xc_next, Xe_next, ws, ws_bytes,
+  return launch_nsga_survive(X, F, G, C, FC, GC, pop, D, d, 3, X_next, F_next, G_next, Xc_next, Xe_next, ws, ws_bytes,
+                             (cudaStream_t)stream);
+}
+
+int32_t hb_nsga2_survive_k(const float *X, const float *F, const float *G, const float *C, const float *FC, const float *GC,
+                           int64_t pop, int64_t D, int64_t d, int64_t num_obj, float *X_next, float *F_next, float *G_next,
+                           float *Xc_next, int32_t *Xe_next, void *ws, int64_t ws_bytes, void *stream) {
+  if (!X || !F || !C || !FC || !X_next || !F_next || (d > 0 && !Xc_next) || (D > d && !Xe_next)) return HB_ERR_INVALID;
+  if (!G != !GC || !G != !G_next) return HB_ERR_INVALID;
+  return launch_nsga_survive(X, F, G, C, FC, GC, pop, D, d, num_obj, X_next, F_next, G_next, Xc_next, Xe_next, ws, ws_bytes,
                              (cudaStream_t)stream);
 }
 
 int32_t hb_ga_survive(const float *X, const float *F, const float *C, const float *FC, int64_t pop, int64_t D, int64_t d,
                       float *X_next, float *F_next, float *Xc_next, int32_t *Xe_next, void *ws, int64_t ws_bytes, void *stream) {
   if (!X || !F || !C || !FC || !X_next || !F_next || (d > 0 && !Xc_next) || (D > d && !Xe_next)) return HB_ERR_INVALID;
-  return launch_ga_survive(X, F, C, FC, pop, D, d, X_next, F_next, Xc_next, Xe_next, ws, ws_bytes, (cudaStream_t)stream);
+  return launch_ga_survive(X, F, nullptr, C, FC, nullptr, pop, D, d, X_next, F_next, nullptr, Xc_next, Xe_next, ws, ws_bytes,
+                           (cudaStream_t)stream);
+}
+
+int32_t hb_ga_survive_cv(const float *X, const float *F, const float *G, const float *C, const float *FC, const float *GC, int64_t pop,
+                         int64_t D, int64_t d, float *X_next, float *F_next, float *G_next, float *Xc_next, int32_t *Xe_next, void *ws,
+                         int64_t ws_bytes, void *stream) {
+  if (!X || !F || !G || !C || !FC || !GC || !X_next || !F_next || !G_next || (d > 0 && !Xc_next) || (D > d && !Xe_next))
+    return HB_ERR_INVALID;
+  return launch_ga_survive(X, F, G, C, FC, GC, pop, D, d, X_next, F_next, G_next, Xc_next, Xe_next, ws, ws_bytes,
+                           (cudaStream_t)stream);
 }
 
 int64_t hb_embed_violation_workspace_bytes(int64_t m, int64_t e, int64_t D) { return embed_violation_ws_query(m, e, D); }

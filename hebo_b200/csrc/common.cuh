@@ -184,8 +184,9 @@ __device__ __forceinline__ void philox_round(uint32_t (&c)[4], uint32_t k0, uint
   const uint32_t n0 = hi1 ^ c[1] ^ k0, n1 = lo1, n2 = hi0 ^ c[3] ^ k1, n3 = lo0;
   c[0] = n0; c[1] = n1; c[2] = n2; c[3] = n3;
 }
-__device__ __forceinline__ void philox_normal2(uint64_t seed, uint64_t row, float &z0, float &z1) {
-  uint32_t c[4] = {(uint32_t)row, (uint32_t)(row >> 32), 0u, 0u};
+// stream: the upper half of the 128-bit Philox counter (0 for the MACE epilogue and hb_sample_y_batch)
+__device__ __forceinline__ void philox_normal2(uint64_t seed, uint64_t row, uint64_t stream, float &z0, float &z1) {
+  uint32_t c[4] = {(uint32_t)row, (uint32_t)(row >> 32), (uint32_t)stream, (uint32_t)(stream >> 32)};
   uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
 #pragma unroll
   for (int r = 0; r < 10; ++r) {
@@ -200,6 +201,9 @@ __device__ __forceinline__ void philox_normal2(uint64_t seed, uint64_t row, floa
   sincospif(2.0f * u1, &sn, &cs);
   z0 = rad * cs;
   z1 = rad * sn;
+}
+__device__ __forceinline__ void philox_normal2(uint64_t seed, uint64_t row, float &z0, float &z1) {
+  philox_normal2(seed, row, 0, z0, z1);
 }
 
 // the duplicate predicate of the NSGA-II / GA survival (pymoo MixedVariableDuplicateElimination): |o[k] - me[k]| <= 1e-16f

@@ -135,6 +135,9 @@ int launch_mace_only(const float *mu, const float *var, int64_t m, float noise_v
                      const float *xi1, const float *xi2, uint64_t seed, float *F, cudaStream_t st);
 // f[m] of a single-objective acquisition (mode HB_ACQ1_*) over (mu, var)
 int launch_acq1(const float *mu, const float *var, int64_t m, int mode, float kappa, float eta, float *f, cudaStream_t st);
+int launch_general_acq(const float *mu, const float *var, int64_t m, int64_t num_obj, int64_t num_constr, float kappa,
+                       float c_kappa, const float *noise_sd, const float *xi, uint64_t seed, uint64_t counter, float *Fo,
+                       float *Fc, float *cv, cudaStream_t st);
 int kstar_groups(int64_t np);
 int launch_kstar(const float *xs, const int32_t *xe, int64_t mc, const ModelSpec &sp, const float *tab_s, const float *x_mul,
                  const float *x_add, const float *Zt, const float *alpha, const float *hyp, int64_t n, int64_t np, int kern,
@@ -155,8 +158,8 @@ int launch_vnorm_h16(const __half *ks_h0, const __half *ks_h1, int64_t ks_rows, 
                      cudaStream_t st);
 
 // pareto.cu
-int launch_pareto3(const float *F, int64_t m, int32_t *idx_out, int32_t *count, void *ws, int64_t ws_bytes,
-                   cudaStream_t st);
+int launch_pareto_k(const float *F, int64_t m, int64_t K, int32_t *idx_out, int32_t *count, void *ws, int64_t ws_bytes,
+                    cudaStream_t st);
 size_t pareto_ws_bytes(int64_t m);
 int launch_front_pack(const float *F, const float *mu, const float *var, const int32_t *idx, const int32_t *count,
                       int64_t row_offset, int64_t capacity, float *out, cudaStream_t st);
@@ -180,16 +183,18 @@ int launch_nsga_init(float *X, int64_t P, int64_t D, int64_t d, const int32_t *k
                      const float *fixed, const float *init, int64_t n_init, uint64_t seed, float *Xc, int32_t *Xe, cudaStream_t st);
 int launch_nsga_mate(const float *X, int64_t P, int64_t D, int64_t d, const int32_t *kind, const float *lb, const float *ub,
                      const float *fixed, uint64_t seed, int gen, float *C, float *Cc, int32_t *Ce, cudaStream_t st);
-// survival of the 2P merged rows: one CTA for 2P <= 512 (ws may be NULL), the cooperative multi-CTA kernel up to
-// P = 16384 (ws_bytes >= nsga_survive_ws_query(P, D)).  G / GC: constraint of the population / offspring (both NULL:
-// unconstrained); Gn (may be NULL): the survivors' constraint.
-int64_t nsga_survive_ws_query(int64_t P, int64_t D);
+// survival of the 2P merged rows with K objectives (2 <= K <= HB_MAX_OBJ): one CTA for 2P <= 512 (ws may be NULL), the
+// cooperative multi-CTA kernel up to P = 16384 (ws_bytes >= nsga_survive_ws_query(P, D, K)).  G / GC / Gn: constraint of
+// the population / offspring / survivors (all three NULL: unconstrained).
+int64_t nsga_survive_ws_query(int64_t P, int64_t D, int64_t K);
 int launch_nsga_survive(const float *X, const float *F, const float *G, const float *C, const float *FC, const float *GC,
-                        int64_t P, int64_t D, int64_t d, float *Xn, float *Fn, float *Gn, float *Xcn, int32_t *Xen, void *ws,
-                        int64_t ws_bytes, cudaStream_t st);
-// single-objective survival: the P best merged rows by (f, index), best first; same sizes and workspace as above
-int launch_ga_survive(const float *X, const float *F, const float *C, const float *FC, int64_t P, int64_t D, int64_t d,
-                      float *Xn, float *Fn, float *Xcn, int32_t *Xen, void *ws, int64_t ws_bytes, cudaStream_t st);
+                        int64_t P, int64_t D, int64_t d, int64_t K, float *Xn, float *Fn, float *Gn, float *Xcn, int32_t *Xen,
+                        void *ws, int64_t ws_bytes, cudaStream_t st);
+// single-objective survival: the P best merged rows by (f, index) -- (cv, f, index) with G / GC / Gn -- best first; the
+// workspace of the K = 3 survival
+int launch_ga_survive(const float *X, const float *F, const float *G, const float *C, const float *FC, const float *GC, int64_t P,
+                      int64_t D, int64_t d, float *Xn, float *Fn, float *Gn, float *Xcn, int32_t *Xen, void *ws, int64_t ws_bytes,
+                      cudaStream_t st);
 // embed.cu: G[i] = sum_j max(|sum_k Y[i,k] B[k,j]| - 1, 0)
 int64_t embed_violation_ws_query(int64_t m, int64_t e, int64_t D);
 int launch_embed_violation(const float *Y, int64_t m, int64_t e, const float *B, int64_t D, float *G, void *ws, int64_t ws_bytes,

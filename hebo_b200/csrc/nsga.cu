@@ -154,12 +154,20 @@ __global__ void nsga_mate_kernel(const float *__restrict__ X, int P, int D, int 
 // Without G (hb_nsga2_survive_ex) every row is feasible with G = 0, duplicates included, which is the rule above.  G = 0
 // everywhere gives the same survivors unless the cut reaches the front of all-+inf rows that holds a duplicate child:
 // with G the duplicate is infeasible and leaves that front.
+// Both kernels are templates on the objective count K (2 <= K <= HB_MAX_OBJ, hb_nsga2_survive_k): everything above holds
+// with K objectives in place of three, and crowding adds objective k = 0 .. K-1 in that order.  hb_nsga2_survive_ex / _cv
+// are the K = 3 instances.
 __device__ __forceinline__ float sanitize_obj(float v) { return isfinite(v) ? v : INFINITY; }
 
 // a dominates b (minimisation): all <=, at least one <
-__device__ __forceinline__ bool dominates3(float a0, float a1, float a2, float b0, float b1, float b2) {
-  const bool le = a0 <= b0 && a1 <= b1 && a2 <= b2;
-  const bool lt = a0 < b0 || a1 < b1 || a2 < b2;
+template <int K>
+__device__ __forceinline__ bool dominates(const float *a, const float *b) {
+  bool le = true, lt = false;
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    le = le && a[k] <= b[k];
+    lt = lt || a[k] < b[k];
+  }
   return le && lt;
 }
 
@@ -187,13 +195,14 @@ __device__ __forceinline__ bool dup_of_earlier(const float *X, const float *C, i
 }
 
 constexpr int NSGA_MAX = 512;
+template <int K>
 __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__restrict__ X, const float *__restrict__ F,
                                                                 const float *__restrict__ G, const float *__restrict__ C,
                                                                 const float *__restrict__ FC, const float *__restrict__ GC,
                                                                 int P, int D, int d, float *__restrict__ Xn,
                                                                 float *__restrict__ Fn, float *__restrict__ Gn,
                                                                 float *__restrict__ Xcn, int32_t *__restrict__ Xen) {
-  __shared__ float f[NSGA_MAX][3], g[NSGA_MAX];
+  __shared__ float f[NSGA_MAX][K], g[NSGA_MAX];
   __shared__ int ndom[NSGA_MAX], rank[NSGA_MAX], order[NSGA_MAX];
   __shared__ float crowd[NSGA_MAX];
   __shared__ unsigned char infront[NSGA_MAX], keep[NSGA_MAX];
@@ -201,8 +210,8 @@ __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__r
   const int N = 2 * P, i = threadIdx.x;
   const bool on = i < N;
   if (on) {
-    const float *src = i < P ? F + (int64_t)i * 3 : FC + (int64_t)(i - P) * 3;
-    for (int k = 0; k < 3; ++k) f[i][k] = sanitize_obj(src[k]);   // NaN / inf objectives never survive (evolution_optimizer.py:104 F)
+    const float *src = i < P ? F + (int64_t)i * K : FC + (int64_t)(i - P) * K;
+    for (int k = 0; k < K; ++k) f[i][k] = sanitize_obj(src[k]);   // NaN / inf objectives never survive (evolution_optimizer.py:104 F)
     g[i] = G ? sanitize_obj(i < P ? G[i] : GC[i - P]) : 0.0f;      // evolution_optimizer.py:105 G
     rank[i] = -1;
     keep[i] = 0;
@@ -212,7 +221,7 @@ __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__r
   if (on && i >= P) {
     // duplicate elimination: a child equal to a population member or to an earlier child is discarded
     if (dup_of_earlier(X, C, P, D, i)) {
-      f[i][0] = f[i][1] = f[i][2] = INFINITY;
+      for (int k = 0; k < K; ++k) f[i][k] = INFINITY;
       if (G) g[i] = INFINITY;
     }
   }
@@ -224,7 +233,7 @@ __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__r
       const float *src = merged_row(X, C, P, D, i);
       float *row = Xn + (int64_t)dst * D;
       for (int k = 0; k < D; ++k) row[k] = src[k];
-      for (int k = 0; k < 3; ++k) Fn[(int64_t)dst * 3 + k] = f[i][k];
+      for (int k = 0; k < K; ++k) Fn[(int64_t)dst * K + k] = f[i][k];
       if (Gn) Gn[dst] = g[i];
       split_row(src, d, D - d, Xcn + (int64_t)dst * d, Xen + (int64_t)dst * (D - d));
     }
@@ -245,7 +254,7 @@ __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__r
   }
   if (live) {
     int c = 0;
-    for (int j = 0; j < N; ++j) c += (g[j] <= 0.0f && dominates3(f[j][0], f[j][1], f[j][2], f[i][0], f[i][1], f[i][2])) ? 1 : 0;
+    for (int j = 0; j < N; ++j) c += (g[j] <= 0.0f && dominates<K>(f[j], f[i])) ? 1 : 0;
     ndom[i] = c;
   }
   if (i == 0) { cum = 0; r_cut = -1; need = 0; }
@@ -271,7 +280,7 @@ __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__r
     if (live && rank[i] < 0) {
       int sub = 0;
       for (int j = 0; j < N; ++j)
-        if (infront[j]) sub += dominates3(f[j][0], f[j][1], f[j][2], f[i][0], f[i][1], f[i][2]) ? 1 : 0;
+        if (infront[j]) sub += dominates<K>(f[j], f[i]) ? 1 : 0;
       ndom[i] -= sub;
     }
     __syncthreads();
@@ -286,7 +295,7 @@ __global__ void __launch_bounds__(NSGA_MAX) nsga_survive_kernel(const float *__r
   }
   __syncthreads();
   const bool mine = on && rc >= 0 && rank[i] == rc;
-  for (int k = 0; k < 3; ++k) {
+  for (int k = 0; k < K; ++k) {
     // position of i inside the cut front along objective k (counting sort, ties by index), then its neighbours
     int pos = 0, m = 0;
     float fmin = INFINITY, fmax = -INFINITY;
@@ -344,13 +353,15 @@ constexpr int NSGA_ROWS = NSGA_LT / NSGA_TEAM;     // rows per CTA pass
 constexpr int NSGA_TJ = 1024;                      // shared-memory tile of the swept set
 constexpr int NSGA_GRID_MAX = 1024;
 
-struct SweepEntry {
-  float v[3];
+template <int K>
+struct SweepEntryK {
+  float v[K];
   int id;
 };
+using SweepEntry = SweepEntryK<3>;
 
 struct SurviveWs {
-  float *f;       // [3][N] sanitised objectives (duplicates -> +inf)
+  float *f;       // [K][N] sanitised objectives (duplicates -> +inf)
   float *g;       // [N] sanitised constraint (0 without one; duplicates -> +inf with one)
   int *ndom;      // [N] dominator count; phase 1 parks the bucket index here
   int *rank;      // [N] front index, -1 = not yet ranked
@@ -358,8 +369,8 @@ struct SurviveWs {
   int *cnt;       // [N + 2] size of front r
   int *head;      // [H] bucket -> last inserted merged row
   int *next;      // [N] bucket chains
-  int *pos;       // [3][N] position of cut-front member a along f_k
-  int *order;     // [3][N] cut-front members sorted along f_k
+  int *pos;       // [K][N] position of cut-front member a along f_k
+  int *order;     // [K][N] cut-front members sorted along f_k
   float *crowd;   // [N] crowding of cut-front member a
   int *keep;      // [N]
   int *sel;       // [P] survivor r -> merged row
@@ -374,15 +385,16 @@ static int64_t nsga_buckets(int64_t P) {
   return H;
 }
 
-size_t nsga_survive_ws_bytes(int64_t P) {
+// K objectives per merged row (the single-objective GA survivals carve the K = 3 layout)
+size_t nsga_survive_ws_bytes(int64_t P, int64_t K = 3) {
   const int64_t N = 2 * P;
-  const int64_t words[] = {3 * N, N, N, N, N, N + 2, nsga_buckets(P), N, 3 * N, 3 * N, N, N, P, NSGA_GRID_MAX, NSGA_GRID_MAX};
+  const int64_t words[] = {K * N, N, N, N, N, N + 2, nsga_buckets(P), N, K * N, K * N, N, N, P, NSGA_GRID_MAX, NSGA_GRID_MAX};
   size_t total = 0;
   for (int64_t w : words) total += (size_t)round_up(w * 4, 256);
   return total;
 }
 
-static SurviveWs nsga_carve(void *ws, int64_t P) {
+static SurviveWs nsga_carve(void *ws, int64_t P, int64_t K = 3) {
   const int64_t N = 2 * P, H = nsga_buckets(P);
   char *p = (char *)ws;
   auto take = [&](int64_t words) {
@@ -391,7 +403,7 @@ static SurviveWs nsga_carve(void *ws, int64_t P) {
     return q;
   };
   SurviveWs w;
-  w.f = (float *)take(3 * N);
+  w.f = (float *)take(K * N);
   w.g = (float *)take(N);
   w.ndom = (int *)take(N);
   w.rank = (int *)take(N);
@@ -399,8 +411,8 @@ static SurviveWs nsga_carve(void *ws, int64_t P) {
   w.cnt = (int *)take(N + 2);
   w.head = (int *)take(H);
   w.next = (int *)take(N);
-  w.pos = (int *)take(3 * N);
-  w.order = (int *)take(3 * N);
+  w.pos = (int *)take(K * N);
+  w.order = (int *)take(K * N);
   w.crowd = (float *)take(N);
   w.keep = (int *)take(N);
   w.sel = (int *)take(P);
@@ -463,17 +475,17 @@ __device__ __forceinline__ void copy_survivors(const float *X, const float *C, i
   }
 }
 
-// Tiled count: for every row r < nr (one 8-lane team each), acc[0..2] = sums of test(me, entry) over the nc entries of
+// Tiled count: for every row r < nr (one 8-lane team each), acc[0..K-1] = sums of test(me, entry) over the nc entries of
 // the swept set, staged NSGA_TJ at a time in shared memory; out(r, me, acc) runs on the team's lane 0.  Every thread of
 // the CTA must call it (it holds __syncthreads and warp shuffles).
-template <class Row, class Col, class Test, class Out>
-__device__ __forceinline__ void team_sweep(SweepEntry *tile, int nr, int nc, Row row, Col col, Test test, Out out) {
+template <int K, class Row, class Col, class Test, class Out>
+__device__ __forceinline__ void team_sweep(SweepEntryK<K> *tile, int nr, int nc, Row row, Col col, Test test, Out out) {
   const int team = threadIdx.x / NSGA_TEAM, lane = threadIdx.x % NSGA_TEAM;
   for (int base = blockIdx.x * NSGA_ROWS; base < nr; base += gridDim.x * NSGA_ROWS) {
     const int r = base + team;
-    SweepEntry me;
+    SweepEntryK<K> me;
     const bool act = r < nr && row(r, me);
-    int acc[3] = {0, 0, 0};
+    int acc[K] = {};
     for (int c0 = 0; c0 < nc; c0 += NSGA_TJ) {
       const int ce = min(NSGA_TJ, nc - c0);
       __syncthreads();
@@ -485,11 +497,12 @@ __device__ __forceinline__ void team_sweep(SweepEntry *tile, int nr, int nc, Row
 #pragma unroll
     for (int o = NSGA_TEAM / 2; o > 0; o >>= 1)
 #pragma unroll
-      for (int k = 0; k < 3; ++k) acc[k] += __shfl_xor_sync(0xFFFFFFFFu, acc[k], o);
+      for (int k = 0; k < K; ++k) acc[k] += __shfl_xor_sync(0xFFFFFFFFu, acc[k], o);
     if (act && lane == 0) out(r, me, acc);
   }
 }
 
+template <int K>
 __global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const float *__restrict__ X, const float *__restrict__ F,
                                                                         const float *__restrict__ G, const float *__restrict__ C,
                                                                         const float *__restrict__ FC, const float *__restrict__ GC,
@@ -498,18 +511,17 @@ __global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const fl
                                                                         float *__restrict__ Xcn, int32_t *__restrict__ Xen,
                                                                         const SurviveWs w_arg) {
   namespace cg = cooperative_groups;
+  using Entry = SweepEntryK<K>;
   SurviveWs w = w_arg;
   cg::grid_group grid = cg::this_grid();
-  __shared__ SweepEntry tile[NSGA_TJ];
+  __shared__ Entry tile[NSGA_TJ];
   __shared__ int s_warp[NSGA_LT / 32], s_base, s_feas;
   const int N = 2 * P;
   const int gtid = blockIdx.x * blockDim.x + threadIdx.x, gsz = gridDim.x * blockDim.x;
-  float *f0 = w.f, *f1 = w.f + N, *f2 = w.f + 2 * N;
   auto obj = [&](int j) {   // written in this kernel: read through L2 after a grid barrier
-    SweepEntry e;
-    e.v[0] = __ldcg(f0 + j);
-    e.v[1] = __ldcg(f1 + j);
-    e.v[2] = __ldcg(f2 + j);
+    Entry e;
+#pragma unroll
+    for (int k = 0; k < K; ++k) e.v[k] = __ldcg(w.f + k * N + j);
     e.id = j;
     return e;
   };
@@ -520,10 +532,9 @@ __global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const fl
 
   // ---- 0: sanitise, clear the bucket table and the front sizes
   for (int i = gtid; i < N; i += gsz) {
-    const float *src = i < P ? F + (int64_t)i * 3 : FC + (int64_t)(i - P) * 3;
-    f0[i] = sanitize_obj(src[0]);
-    f1[i] = sanitize_obj(src[1]);
-    f2[i] = sanitize_obj(src[2]);
+    const float *src = i < P ? F + (int64_t)i * K : FC + (int64_t)(i - P) * K;
+#pragma unroll
+    for (int k = 0; k < K; ++k) w.f[k * N + i] = sanitize_obj(src[k]);
     const float gi = G ? sanitize_obj(i < P ? G[i] : GC[i - P]) : 0.0f;
     w.g[i] = gi;
     nfeas += (i < P && gi <= 0.0f) ? 1 : 0;
@@ -539,7 +550,8 @@ __global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const fl
     const bool dup = dup_in_bucket(X, C, P, D, w, i);
     float gi = __ldcg(w.g + i);
     if (dup) {
-      f0[i] = f1[i] = f2[i] = INFINITY;
+#pragma unroll
+      for (int k = 0; k < K; ++k) w.f[k * N + i] = INFINITY;
       if (G) w.g[i] = gi = INFINITY;
     }
     nfeas += gi <= 0.0f ? 1 : 0;
@@ -558,9 +570,10 @@ __global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const fl
   if (nf < P) {
     // ---- 3': too few feasible rows: all of them survive, then the P - nf least infeasible (ascending G, ties by index)
     auto cv_entry = [&](int j) {
-      SweepEntry e;
+      Entry e;
       e.v[0] = feasible(j) ? __int_as_float(0x7FC00000) : __ldcg(w.g + j);   // NaN: a feasible row is never counted
-      e.v[1] = e.v[2] = 0.0f;
+#pragma unroll
+      for (int k = 1; k < K; ++k) e.v[k] = 0.0f;
       e.id = j;
       return e;
     };
@@ -569,25 +582,27 @@ __global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const fl
       if (feasible(i)) w.keep[i] = 1;
     team_sweep(
         tile, N, N,
-        [&](int r, SweepEntry &me) {
+        [&](int r, Entry &me) {
           if (feasible(r)) return false;
           me = cv_entry(r);
           return true;
         },
         cv_entry,
-        [](const SweepEntry &me, const SweepEntry &o, int *acc) { acc[0] += before_asc(o.v[0], o.id, me.v[0], me.id) ? 1 : 0; },
-        [&](int r, const SweepEntry &, const int *acc) { w.keep[r] = acc[0] < P - nf ? 1 : 0; });
+        [](const Entry &me, const Entry &o, int *acc) { acc[0] += before_asc(o.v[0], o.id, me.v[0], me.id) ? 1 : 0; },
+        [&](int r, const Entry &, const int *acc) { w.keep[r] = acc[0] < P - nf ? 1 : 0; });
     grid.sync();
   } else {
     // ---- 3: dominator counts among the feasible rows; front 0
     auto live_entry = [&](int j) {
-      SweepEntry e = obj(j);
-      if (!feasible(j)) e.v[0] = e.v[1] = e.v[2] = __int_as_float(0x7FC00000);   // NaN never dominates
+      Entry e = obj(j);
+      if (!feasible(j))
+#pragma unroll
+        for (int k = 0; k < K; ++k) e.v[k] = __int_as_float(0x7FC00000);   // NaN never dominates
       return e;
     };
     team_sweep(
         tile, N, N,
-        [&](int r, SweepEntry &me) {
+        [&](int r, Entry &me) {
           if (!feasible(r)) {
             w.rank[r] = -2;
             return false;
@@ -596,10 +611,8 @@ __global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const fl
           return true;
         },
         live_entry,
-        [](const SweepEntry &me, const SweepEntry &o, int *acc) {
-          acc[0] += dominates3(o.v[0], o.v[1], o.v[2], me.v[0], me.v[1], me.v[2]) ? 1 : 0;
-        },
-        [&](int r, const SweepEntry &, const int *acc) {
+        [](const Entry &me, const Entry &o, int *acc) { acc[0] += dominates<K>(o.v, me.v) ? 1 : 0; },
+        [&](int r, const Entry &, const int *acc) {
           w.ndom[r] = acc[0];
           w.rank[r] = acc[0] == 0 ? 0 : -1;
           if (acc[0] == 0) w.list[atomicAdd(&w.cnt[0], 1)] = r;
@@ -614,16 +627,14 @@ __global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const fl
       const int nxt = start + c;
       team_sweep(
           tile, N, c,
-          [&](int i, SweepEntry &me) {
+          [&](int i, Entry &me) {
             if (__ldcg(&w.rank[i]) != -1) return false;   // ranked or infeasible
             me = obj(i);
             return true;
           },
           [&](int t) { return obj(__ldcg(&w.list[start + t])); },
-          [](const SweepEntry &me, const SweepEntry &o, int *acc) {
-            acc[0] += dominates3(o.v[0], o.v[1], o.v[2], me.v[0], me.v[1], me.v[2]) ? 1 : 0;
-          },
-          [&](int i, const SweepEntry &, const int *acc) {
+          [](const Entry &me, const Entry &o, int *acc) { acc[0] += dominates<K>(o.v, me.v) ? 1 : 0; },
+          [&](int i, const Entry &, const int *acc) {
             if (acc[0] == 0) return;
             const int nd = __ldcg(&w.ndom[i]) - acc[0];
             w.ndom[i] = nd;
@@ -637,31 +648,31 @@ __global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const fl
     }
     const int m = rc >= 0 ? __ldcg(&w.cnt[rc]) : 0;
     const int *front = w.list + start;
-    // ---- 5: cut front: positions along f_0, f_1, f_2; whole fronts below the cut survive
+    // ---- 5: cut front: positions along f_0 .. f_{K-1}; whole fronts below the cut survive
     for (int i = gtid; i < N; i += gsz) {
       const int rk = __ldcg(&w.rank[i]);
       w.keep[i] = (rc >= 0 && rk >= 0 && rk < rc) ? 1 : 0;
     }
     team_sweep(
-        tile, m, m, [&](int a, SweepEntry &me) { me = obj(__ldcg(front + a)); return true; },
+        tile, m, m, [&](int a, Entry &me) { me = obj(__ldcg(front + a)); return true; },
         [&](int t) { return obj(__ldcg(front + t)); },
-        [](const SweepEntry &me, const SweepEntry &o, int *acc) {
+        [](const Entry &me, const Entry &o, int *acc) {
 #pragma unroll
-          for (int k = 0; k < 3; ++k) acc[k] += before_asc(o.v[k], o.id, me.v[k], me.id) ? 1 : 0;
+          for (int k = 0; k < K; ++k) acc[k] += before_asc(o.v[k], o.id, me.v[k], me.id) ? 1 : 0;
         },
-        [&](int a, const SweepEntry &me, const int *acc) {
+        [&](int a, const Entry &me, const int *acc) {
 #pragma unroll
-          for (int k = 0; k < 3; ++k) {
+          for (int k = 0; k < K; ++k) {
             w.pos[k * N + a] = acc[k];
             w.order[k * N + acc[k]] = me.id;
           }
         });
     grid.sync();
-    // ---- 6: crowding, k = 0, 1, 2 in order, by the member itself
+    // ---- 6: crowding, k = 0 .. K-1 in order, by the member itself
     for (int a = gtid; a < m; a += gsz) {
       float cr = 0.0f;
 #pragma unroll
-      for (int k = 0; k < 3; ++k) {
+      for (int k = 0; k < K; ++k) {
         const float *fk = w.f + k * N;
         const int *ok = w.order + k * N;
         const int p = __ldcg(w.pos + k * N + a);
@@ -674,16 +685,17 @@ __global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const fl
     grid.sync();
     // ---- 7: the `need` members with the largest crowding survive
     auto crowd_entry = [&](int a) {
-      SweepEntry e;
+      Entry e;
       e.v[0] = __ldcg(w.crowd + a);
-      e.v[1] = e.v[2] = 0.0f;
+#pragma unroll
+      for (int k = 1; k < K; ++k) e.v[k] = 0.0f;
       e.id = __ldcg(front + a);
       return e;
     };
     team_sweep(
-        tile, m, m, [&](int a, SweepEntry &me) { me = crowd_entry(a); return true; }, crowd_entry,
-        [](const SweepEntry &me, const SweepEntry &o, int *acc) { acc[0] += before_desc(o.v[0], o.id, me.v[0], me.id) ? 1 : 0; },
-        [&](int, const SweepEntry &me, const int *acc) {
+        tile, m, m, [&](int a, Entry &me) { me = crowd_entry(a); return true; }, crowd_entry,
+        [](const Entry &me, const Entry &o, int *acc) { acc[0] += before_desc(o.v[0], o.id, me.v[0], me.id) ? 1 : 0; },
+        [&](int, const Entry &me, const int *acc) {
           if (acc[0] < need) w.keep[me.id] = 1;
         });
     grid.sync();
@@ -722,8 +734,8 @@ __global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const fl
   int total = 0;
   for (int b = 0; b < (int)gridDim.x; ++b) total += __ldcg(w.bsum + b);
   // ---- 9: coalesced copy of the survivors
-  for (int64_t q = gtid; q < (int64_t)total * 3; q += gsz) {
-    const int r = (int)(q / 3), k = (int)(q % 3);
+  for (int64_t q = gtid; q < (int64_t)total * K; q += gsz) {
+    const int r = (int)(q / K), k = (int)(q % K);
     Fn[q] = __ldcg(w.f + k * N + __ldcg(w.sel + r));
   }
   if (Gn)
@@ -731,47 +743,66 @@ __global__ void __launch_bounds__(NSGA_LT, 2) nsga_survive_large_kernel(const fl
   copy_survivors(X, C, P, D, d, w.sel, total, Xn, Xcn, Xen, gtid, gsz);
 }
 
-// ---- single-objective survival (hb_ga_survive): pymoo's FitnessSurvival as MixedVariableGA runs it for a one-objective
-// acquisition (evolution_optimizer.py:123-124,132-133).  The ordering rule is recalled from pymoo 0.6 -- np.lexsort([F, cv])
-// then pop[S[:n_survive]], no constraint here -- and was not checked against pymoo.  On the merged rows (population
+// ---- single-objective survival (hb_ga_survive, hb_ga_survive_cv): pymoo's FitnessSurvival as MixedVariableGA runs it for
+// a one-objective acquisition (evolution_optimizer.py:123-124,132-133).  The ordering rule is recalled from pymoo 0.6 --
+// np.lexsort([F, cv]) then pop[S[:n_survive]] -- and was not checked against pymoo.  On the merged rows (population
 // 0..P-1, offspring P..2P-1, one objective f each):
-//  * sanitising: a non-finite f becomes +inf;
+//  * sanitising: a non-finite f becomes +inf; with a constraint column (CV), cv = max(G, 0), a non-finite G becomes +inf;
 //  * duplicates: the predicate of the NSGA-II survival above (|o[k] - me[k]| <= 1e-16f in every column against any
-//    earlier merged row); a duplicate child gets f = +inf;
-//  * survivors: the P merged rows first in ascending (f, merged index) order, written in that order (row 0 = the best);
-//    F_next holds the sanitised f.
-// A row's output slot is its rank, the count of merged rows with a smaller (f, index) key.  The keys are distinct, so the
-// ranks are a permutation and a row with rank < P writes its slot directly: no scan, no float atomics, the same bytes from
-// both kernels and from run to run.
+//    earlier merged row); a duplicate child gets f = +inf (and cv = +inf);
+//  * survivors: the P merged rows first in ascending (f, merged index) order -- (cv, f, merged index) with CV -- written
+//    in that order (row 0 = the best); F_next holds the sanitised f, G_next the sanitised cv.
+// A row's output slot is its rank, the count of merged rows with a smaller key.  The keys are distinct, so the ranks are
+// a permutation and a row with rank < P writes its slot directly: no scan, no float atomics, the same bytes from both
+// kernels and from run to run.  With G = 0 everywhere the order is the unconstrained one, except among the f = +inf rows
+// when one of them is a duplicate child (cv = +inf here).
+__device__ __forceinline__ float sanitize_cv(float v) { return isfinite(v) ? (v > 0.0f ? v : 0.0f) : INFINITY; }
+
+// (gj, fj, j) before (gi, fi, i) in ascending lexicographic order
+__device__ __forceinline__ bool before_lex(float gj, float fj, int j, float gi, float fi, int i) {
+  return gj < gi || (gj == gi && before_asc(fj, j, fi, i));
+}
+
+template <bool CV>
 __global__ void __launch_bounds__(NSGA_MAX) ga_survive_kernel(const float *__restrict__ X, const float *__restrict__ F,
-                                                              const float *__restrict__ C, const float *__restrict__ FC, int P,
+                                                              const float *__restrict__ G, const float *__restrict__ C,
+                                                              const float *__restrict__ FC, const float *__restrict__ GC, int P,
                                                               int D, int d, float *__restrict__ Xn, float *__restrict__ Fn,
-                                                              float *__restrict__ Xcn, int32_t *__restrict__ Xen) {
-  __shared__ float f[NSGA_MAX];
+                                                              float *__restrict__ Gn, float *__restrict__ Xcn,
+                                                              int32_t *__restrict__ Xen) {
+  __shared__ float f[NSGA_MAX], g[CV ? NSGA_MAX : 1];
   const int N = 2 * P, i = threadIdx.x;
   const bool on = i < N;
   if (on) {
     f[i] = sanitize_obj(i < P ? F[i] : FC[i - P]);
-    if (i >= P && dup_of_earlier(X, C, P, D, i)) f[i] = INFINITY;
+    if (CV) g[i] = sanitize_cv(i < P ? G[i] : GC[i - P]);
+    if (i >= P && dup_of_earlier(X, C, P, D, i)) {
+      f[i] = INFINITY;
+      if (CV) g[i] = INFINITY;
+    }
   }
   __syncthreads();
   if (!on) return;
   int rank = 0;
-  for (int j = 0; j < N; ++j) rank += before_asc(f[j], j, f[i], i) ? 1 : 0;
+  for (int j = 0; j < N; ++j) rank += (CV ? before_lex(g[j], f[j], j, g[i], f[i], i) : before_asc(f[j], j, f[i], i)) ? 1 : 0;
   if (rank >= P) return;
   const float *src = merged_row(X, C, P, D, i);
   float *row = Xn + (int64_t)rank * D;
   for (int k = 0; k < D; ++k) row[k] = src[k];
   Fn[rank] = f[i];
+  if (CV) Gn[rank] = g[i];
   split_row(src, d, D - d, Xcn + (int64_t)rank * d, Xen + (int64_t)rank * (D - d));
 }
 
 // multi-CTA form for 512 < 2P <= 32768: duplicates through the bucket table, ranks by the tiled count, then the copy
+template <bool CV>
 __global__ void __launch_bounds__(NSGA_LT, 2) ga_survive_large_kernel(const float *__restrict__ X, const float *__restrict__ F,
-                                                                      const float *__restrict__ C, const float *__restrict__ FC,
+                                                                      const float *__restrict__ G, const float *__restrict__ C,
+                                                                      const float *__restrict__ FC, const float *__restrict__ GC,
                                                                       int P, int D, int d, float *__restrict__ Xn,
-                                                                      float *__restrict__ Fn, float *__restrict__ Xcn,
-                                                                      int32_t *__restrict__ Xen, const SurviveWs w_arg) {
+                                                                      float *__restrict__ Fn, float *__restrict__ Gn,
+                                                                      float *__restrict__ Xcn, int32_t *__restrict__ Xen,
+                                                                      const SurviveWs w_arg) {
   namespace cg = cooperative_groups;
   SurviveWs w = w_arg;
   cg::grid_group grid = cg::this_grid();
@@ -779,7 +810,10 @@ __global__ void __launch_bounds__(NSGA_LT, 2) ga_survive_large_kernel(const floa
   const int N = 2 * P;
   const int gtid = blockIdx.x * blockDim.x + threadIdx.x, gsz = gridDim.x * blockDim.x;
   // ---- 0: sanitise, clear the bucket table
-  for (int i = gtid; i < N; i += gsz) w.f[i] = sanitize_obj(i < P ? F[i] : FC[i - P]);
+  for (int i = gtid; i < N; i += gsz) {
+    w.f[i] = sanitize_obj(i < P ? F[i] : FC[i - P]);
+    if (CV) w.g[i] = sanitize_cv(i < P ? G[i] : GC[i - P]);
+  }
   for (int h = gtid; h < w.H; h += gsz) w.head[h] = -1;
   grid.sync();
   // ---- 1: bucket every merged row
@@ -787,25 +821,35 @@ __global__ void __launch_bounds__(NSGA_LT, 2) ga_survive_large_kernel(const floa
   grid.sync();
   // ---- 2: duplicate children
   for (int i = P + gtid; i < N; i += gsz)
-    if (dup_in_bucket(X, C, P, D, w, i)) w.f[i] = INFINITY;
+    if (dup_in_bucket(X, C, P, D, w, i)) {
+      w.f[i] = INFINITY;
+      if (CV) w.g[i] = INFINITY;
+    }
   grid.sync();
-  // ---- 3: rank = count of smaller (f, index) keys; the survivors write their output slot
+  // ---- 3: rank = count of smaller keys; the survivors write their output slot
   auto key = [&](int j) {
     SweepEntry e;
     e.v[0] = __ldcg(w.f + j);
-    e.v[1] = e.v[2] = 0.0f;
+    e.v[1] = CV ? __ldcg(w.g + j) : 0.0f;
+    e.v[2] = 0.0f;
     e.id = j;
     return e;
   };
   team_sweep(
       tile, N, N, [&](int r, SweepEntry &me) { me = key(r); return true; }, key,
-      [](const SweepEntry &me, const SweepEntry &o, int *acc) { acc[0] += before_asc(o.v[0], o.id, me.v[0], me.id) ? 1 : 0; },
+      [](const SweepEntry &me, const SweepEntry &o, int *acc) {
+        acc[0] += (CV ? before_lex(o.v[1], o.v[0], o.id, me.v[1], me.v[0], me.id) : before_asc(o.v[0], o.id, me.v[0], me.id)) ? 1 : 0;
+      },
       [&](int r, const SweepEntry &, const int *acc) {
         if (acc[0] < P) w.sel[acc[0]] = r;
       });
   grid.sync();
   // ---- 4: coalesced copy of the survivors
-  for (int q = gtid; q < P; q += gsz) Fn[q] = __ldcg(w.f + __ldcg(w.sel + q));
+  for (int q = gtid; q < P; q += gsz) {
+    const int s = __ldcg(w.sel + q);
+    Fn[q] = __ldcg(w.f + s);
+    if (CV) Gn[q] = __ldcg(w.g + s);
+  }
   copy_survivors(X, C, P, D, d, w.sel, P, Xn, Xcn, Xen, gtid, gsz);
 }
 
@@ -850,57 +894,83 @@ int launch_nsga_mate(const float *X, int64_t P, int64_t D, int64_t d, const int3
   return HB_OK;
 }
 
-int64_t nsga_survive_ws_query(int64_t P, int64_t D) {
-  if (P < 1 || P > NSGA_LARGE_MAX_POP || D < 1) return -1;
-  return (int64_t)nsga_survive_ws_bytes(P);
+int64_t nsga_survive_ws_query(int64_t P, int64_t D, int64_t K) {
+  if (P < 1 || P > NSGA_LARGE_MAX_POP || D < 1 || K < 2 || K > HB_MAX_OBJ) return -1;
+  return (int64_t)nsga_survive_ws_bytes(P, K);
 }
 
-int launch_nsga_survive(const float *X, const float *F, const float *G, const float *C, const float *FC, const float *GC,
-                        int64_t P, int64_t D, int64_t d, float *Xn, float *Fn, float *Gn, float *Xcn, int32_t *Xen, void *ws,
-                        int64_t ws_bytes, cudaStream_t st) {
-  if (P <= 0 || P > NSGA_LARGE_MAX_POP || D <= 0 || d < 0 || d > D) return HB_ERR_INVALID;
-  if (!G != !GC) return HB_ERR_INVALID;
+template <int K>
+static int launch_nsga_survive_t(const float *X, const float *F, const float *G, const float *C, const float *FC, const float *GC,
+                                 int64_t P, int64_t D, int64_t d, float *Xn, float *Fn, float *Gn, float *Xcn, int32_t *Xen,
+                                 void *ws, int64_t ws_bytes, cudaStream_t st) {
   if (2 * P <= NSGA_MAX) {
-    nsga_survive_kernel<<<1, NSGA_MAX, 0, st>>>(X, F, G, C, FC, GC, (int)P, (int)D, (int)d, Xn, Fn, Gn, Xcn, Xen);
+    nsga_survive_kernel<K><<<1, NSGA_MAX, 0, st>>>(X, F, G, C, FC, GC, (int)P, (int)D, (int)d, Xn, Fn, Gn, Xcn, Xen);
     count_launches(1);
     HB_LAUNCH_CHECK("nsga_survive");
     return HB_OK;
   }
-  if (!ws || ws_bytes < (int64_t)nsga_survive_ws_bytes(P)) return HB_ERR_INVALID;
-  static PerDevice once;   // aux[dev] = co-resident CTAs of the cooperative survival kernel on that device
+  if (!ws || ws_bytes < (int64_t)nsga_survive_ws_bytes(P, K)) return HB_ERR_INVALID;
+  static PerDevice once;   // aux[dev] = co-resident CTAs of this cooperative survival kernel on that device
   int grid = 0;
-  const int rc = survive_grid(nsga_survive_large_kernel, once, P, &grid);
+  const int rc = survive_grid(nsga_survive_large_kernel<K>, once, P, &grid);
   if (rc != HB_OK) return rc;
-  SurviveWs w = nsga_carve(ws, P);
+  SurviveWs w = nsga_carve(ws, P, K);
   int Pi = (int)P, Di = (int)D, di = (int)d;
   void *args[] = {&X, &F, &G, &C, &FC, &GC, &Pi, &Di, &di, &Xn, &Fn, &Gn, &Xcn, &Xen, &w};
-  HB_CUDA(cudaLaunchCooperativeKernel((const void *)nsga_survive_large_kernel, dim3(grid), dim3(NSGA_LT), args, 0, st));
+  HB_CUDA(cudaLaunchCooperativeKernel((const void *)nsga_survive_large_kernel<K>, dim3(grid), dim3(NSGA_LT), args, 0, st));
   count_launches(1);
   HB_LAUNCH_CHECK("nsga_survive_large");
   return HB_OK;
 }
 
-int launch_ga_survive(const float *X, const float *F, const float *C, const float *FC, int64_t P, int64_t D, int64_t d,
-                      float *Xn, float *Fn, float *Xcn, int32_t *Xen, void *ws, int64_t ws_bytes, cudaStream_t st) {
+int launch_nsga_survive(const float *X, const float *F, const float *G, const float *C, const float *FC, const float *GC,
+                        int64_t P, int64_t D, int64_t d, int64_t K, float *Xn, float *Fn, float *Gn, float *Xcn, int32_t *Xen,
+                        void *ws, int64_t ws_bytes, cudaStream_t st) {
   if (P <= 0 || P > NSGA_LARGE_MAX_POP || D <= 0 || d < 0 || d > D) return HB_ERR_INVALID;
+  if (!G != !GC || !G != !Gn) return HB_ERR_INVALID;
+  switch (K) {
+    case 2: return launch_nsga_survive_t<2>(X, F, G, C, FC, GC, P, D, d, Xn, Fn, Gn, Xcn, Xen, ws, ws_bytes, st);
+    case 3: return launch_nsga_survive_t<3>(X, F, G, C, FC, GC, P, D, d, Xn, Fn, Gn, Xcn, Xen, ws, ws_bytes, st);
+    case 4: return launch_nsga_survive_t<4>(X, F, G, C, FC, GC, P, D, d, Xn, Fn, Gn, Xcn, Xen, ws, ws_bytes, st);
+    case 5: return launch_nsga_survive_t<5>(X, F, G, C, FC, GC, P, D, d, Xn, Fn, Gn, Xcn, Xen, ws, ws_bytes, st);
+    case 6: return launch_nsga_survive_t<6>(X, F, G, C, FC, GC, P, D, d, Xn, Fn, Gn, Xcn, Xen, ws, ws_bytes, st);
+    case 7: return launch_nsga_survive_t<7>(X, F, G, C, FC, GC, P, D, d, Xn, Fn, Gn, Xcn, Xen, ws, ws_bytes, st);
+    case 8: return launch_nsga_survive_t<8>(X, F, G, C, FC, GC, P, D, d, Xn, Fn, Gn, Xcn, Xen, ws, ws_bytes, st);
+    default: return HB_ERR_INVALID;
+  }
+}
+
+template <bool CV>
+static int launch_ga_survive_t(const float *X, const float *F, const float *G, const float *C, const float *FC, const float *GC,
+                               int64_t P, int64_t D, int64_t d, float *Xn, float *Fn, float *Gn, float *Xcn, int32_t *Xen,
+                               void *ws, int64_t ws_bytes, cudaStream_t st) {
   if (2 * P <= NSGA_MAX) {
-    ga_survive_kernel<<<1, (int)round_up(2 * P, 32), 0, st>>>(X, F, C, FC, (int)P, (int)D, (int)d, Xn, Fn, Xcn, Xen);
+    ga_survive_kernel<CV><<<1, (int)round_up(2 * P, 32), 0, st>>>(X, F, G, C, FC, GC, (int)P, (int)D, (int)d, Xn, Fn, Gn, Xcn, Xen);
     count_launches(1);
     HB_LAUNCH_CHECK("ga_survive");
     return HB_OK;
   }
   if (!ws || ws_bytes < (int64_t)nsga_survive_ws_bytes(P)) return HB_ERR_INVALID;
-  static PerDevice once;   // aux[dev] = co-resident CTAs of the cooperative GA survival kernel on that device
+  static PerDevice once;   // aux[dev] = co-resident CTAs of this cooperative GA survival kernel on that device
   int grid = 0;
-  const int rc = survive_grid(ga_survive_large_kernel, once, P, &grid);
+  const int rc = survive_grid(ga_survive_large_kernel<CV>, once, P, &grid);
   if (rc != HB_OK) return rc;
   SurviveWs w = nsga_carve(ws, P);
   int Pi = (int)P, Di = (int)D, di = (int)d;
-  void *args[] = {&X, &F, &C, &FC, &Pi, &Di, &di, &Xn, &Fn, &Xcn, &Xen, &w};
-  HB_CUDA(cudaLaunchCooperativeKernel((const void *)ga_survive_large_kernel, dim3(grid), dim3(NSGA_LT), args, 0, st));
+  void *args[] = {&X, &F, &G, &C, &FC, &GC, &Pi, &Di, &di, &Xn, &Fn, &Gn, &Xcn, &Xen, &w};
+  HB_CUDA(cudaLaunchCooperativeKernel((const void *)ga_survive_large_kernel<CV>, dim3(grid), dim3(NSGA_LT), args, 0, st));
   count_launches(1);
   HB_LAUNCH_CHECK("ga_survive_large");
   return HB_OK;
+}
+
+int launch_ga_survive(const float *X, const float *F, const float *G, const float *C, const float *FC, const float *GC, int64_t P,
+                      int64_t D, int64_t d, float *Xn, float *Fn, float *Gn, float *Xcn, int32_t *Xen, void *ws, int64_t ws_bytes,
+                      cudaStream_t st) {
+  if (P <= 0 || P > NSGA_LARGE_MAX_POP || D <= 0 || d < 0 || d > D) return HB_ERR_INVALID;
+  if (!G != !GC || !G != !Gn) return HB_ERR_INVALID;
+  return G ? launch_ga_survive_t<true>(X, F, G, C, FC, GC, P, D, d, Xn, Fn, Gn, Xcn, Xen, ws, ws_bytes, st)
+           : launch_ga_survive_t<false>(X, F, G, C, FC, GC, P, D, d, Xn, Fn, Gn, Xcn, Xen, ws, ws_bytes, st);
 }
 
 }  // namespace hb

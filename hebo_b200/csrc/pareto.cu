@@ -1,4 +1,4 @@
-// 3-objective non-dominated filter (all objectives minimised): the rank-0 set that pymoo's NSGA-II hands back
+// K-objective non-dominated filter (1 <= K <= HB_MAX_OBJ, all objectives minimised; hb_pareto_front3 is K = 3): the rank-0 set that pymoo's NSGA-II hands back
 // as res.X in HEBO/hebo/acq_optimizers/evolution_optimizer.py:141-149, computed exactly on the device for
 // candidate batches of any size.
 //
@@ -34,12 +34,13 @@ __device__ __forceinline__ int64_t strided_row(int a, int stride) {
 // gridDim.y splits list B into segments (each block tests its 256 A rows against one segment and only ever CLEARS flags:
 // idempotent, no ordering needed), so a short list A against a long list B -- the 4096 x 4096 sample-front pass, 16 blocks
 // and 205 us when B was walked by one block per A tile -- still fills the machine.
+template <int K>
 __global__ void __launch_bounds__(PB) nondominated_kernel(const float *__restrict__ F, const int32_t *__restrict__ idxA,
                                                           const int32_t *__restrict__ nA_ptr, int nA_host, int strideA,
                                                           const int32_t *__restrict__ idxB,
                                                           const int32_t *__restrict__ nB_ptr, int nB_host, int strideB,
                                                           uint8_t *__restrict__ flags) {
-  __shared__ float b0[PB], b1[PB], b2[PB];
+  __shared__ float b[K][PB];
   const int nA = nA_ptr ? *nA_ptr : nA_host;
   const int nB = nB_ptr ? *nB_ptr : nB_host;
   if ((int)(blockIdx.x * PB) >= nA) return;
@@ -47,29 +48,36 @@ __global__ void __launch_bounds__(PB) nondominated_kernel(const float *__restric
   const int jbeg = blockIdx.y * seg, jend = min(nB, jbeg + seg);
   const int a = blockIdx.x * PB + threadIdx.x;
   const bool active = a < nA;
-  float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+  float av[K];
+  bool dominated = !active;
+#pragma unroll
+  for (int k = 0; k < K; ++k) av[k] = 0.f;
   if (active) {
     const int64_t ia = idxA ? idxA[a] : strided_row(a, strideA);
-    a0 = F[ia * 3 + 0];
-    a1 = F[ia * 3 + 1];
-    a2 = F[ia * 3 + 2];
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+      av[k] = F[ia * K + k];
+      dominated = dominated || isnan(av[k]);
+    }
   }
-  bool dominated = !active || isnan(a0) || isnan(a1) || isnan(a2);
   for (int j0 = jbeg; j0 < jend; j0 += PB) {
     const int j = j0 + threadIdx.x;
     if (j < jend) {
       const int64_t ib = idxB ? idxB[j] : strided_row(j, strideB);
-      b0[threadIdx.x] = F[ib * 3 + 0];
-      b1[threadIdx.x] = F[ib * 3 + 1];
-      b2[threadIdx.x] = F[ib * 3 + 2];
+#pragma unroll
+      for (int k = 0; k < K; ++k) b[k][threadIdx.x] = F[ib * K + k];
     }
     __syncthreads();
     const int lim = min(PB, jend - j0);
     if (!dominated) {
       for (int u = 0; u < lim; ++u) {
-        const float x0 = b0[u], x1 = b1[u], x2 = b2[u];
-        const bool le = (x0 <= a0) & (x1 <= a1) & (x2 <= a2);
-        const bool lt = (x0 < a0) | (x1 < a1) | (x2 < a2);
+        bool le = true, lt = false;
+#pragma unroll
+        for (int k = 0; k < K; ++k) {
+          const float x = b[k][u];
+          le = le & (x <= av[k]);
+          lt = lt | (x < av[k]);
+        }
         if (le & lt) {
           dominated = true;
           break;
@@ -176,8 +184,9 @@ static void compact(const uint8_t *flags, const int32_t *idxA, const int32_t *nA
   compact_scatter_kernel<<<nblocks, PB, 0, st>>>(flags, idxA, nA_ptr, nA_host, strideA, counts, out_idx);
 }
 
-int launch_pareto3(const float *F, int64_t m, int32_t *idx_out, int32_t *count, void *ws, int64_t ws_bytes,
-                   cudaStream_t st) {
+template <int K>
+static int launch_pareto_t(const float *F, int64_t m, int32_t *idx_out, int32_t *count, void *ws, int64_t ws_bytes,
+                           cudaStream_t st) {
   if (m <= 0 || m > 0x7fffffff) return HB_ERR_INVALID;
   if ((size_t)ws_bytes < pareto_ws_bytes(m)) return HB_ERR_INVALID;
   ParetoWs w = carve_pareto(ws, m);
@@ -191,7 +200,7 @@ int launch_pareto3(const float *F, int64_t m, int32_t *idx_out, int32_t *count, 
   };
   if (mi <= PARETO_DIRECT_MAX) {
     HB_CUDA(cudaMemsetAsync(w.flags, 1, (size_t)mi, st));
-    nondominated_kernel<<<dim3((unsigned)ceil_div(mi, PB), (unsigned)segs(mi, mi)), PB, 0, st>>>(F, nullptr, nullptr, mi, 1, nullptr, nullptr, mi, 1, w.flags);
+    nondominated_kernel<K><<<dim3((unsigned)ceil_div(mi, PB), (unsigned)segs(mi, mi)), PB, 0, st>>>(F, nullptr, nullptr, mi, 1, nullptr, nullptr, mi, 1, w.flags);
     compact(w.flags, nullptr, nullptr, mi, 1, w.counts, idx_out, count, st);
     count_launches(4);
   } else {
@@ -199,21 +208,36 @@ int launch_pareto3(const float *F, int64_t m, int32_t *idx_out, int32_t *count, 
     const int stride = (int)(m / PARETO_SAMPLE);
     const int ns = PARETO_SAMPLE;
     HB_CUDA(cudaMemsetAsync(w.flags, 1, (size_t)ns, st));
-    nondominated_kernel<<<dim3((unsigned)ceil_div(ns, PB), (unsigned)segs(ns, ns)), PB, 0, st>>>(F, nullptr, nullptr, ns, stride, nullptr, nullptr, ns, stride, w.flags);
+    nondominated_kernel<K><<<dim3((unsigned)ceil_div(ns, PB), (unsigned)segs(ns, ns)), PB, 0, st>>>(F, nullptr, nullptr, ns, stride, nullptr, nullptr, ns, stride, w.flags);
     compact(w.flags, nullptr, nullptr, ns, stride, w.counts, w.listS, w.nS, st);
     // (2) all points against the sample front (a short list: one segment)
     HB_CUDA(cudaMemsetAsync(w.flags, 1, (size_t)mi, st));
-    nondominated_kernel<<<(int)ceil_div(mi, PB), PB, 0, st>>>(F, nullptr, nullptr, mi, 1, w.listS, w.nS, 0, 1, w.flags);
+    nondominated_kernel<K><<<(int)ceil_div(mi, PB), PB, 0, st>>>(F, nullptr, nullptr, mi, 1, w.listS, w.nS, 0, 1, w.flags);
     compact(w.flags, nullptr, nullptr, mi, 1, w.counts, w.listA, w.nA, st);
     // (3) exact all-pairs among the survivors (count known only on the device: launch for the upper bound; blocks past the
     //     count exit at once; four B segments keep a long survivor list from serialising on a few SMs)
     HB_CUDA(cudaMemsetAsync(w.flags, 1, (size_t)mi, st));
-    nondominated_kernel<<<dim3((unsigned)ceil_div(mi, PB), 4), PB, 0, st>>>(F, w.listA, w.nA, 0, 1, w.listA, w.nA, 0, 1, w.flags);
+    nondominated_kernel<K><<<dim3((unsigned)ceil_div(mi, PB), 4), PB, 0, st>>>(F, w.listA, w.nA, 0, 1, w.listA, w.nA, 0, 1, w.flags);
     compact(w.flags, w.listA, w.nA, mi, 1, w.counts, idx_out, count, st);
     count_launches(12);
   }
-  HB_LAUNCH_CHECK("pareto3");
+  HB_LAUNCH_CHECK("pareto");
   return HB_OK;
+}
+
+int launch_pareto_k(const float *F, int64_t m, int64_t K, int32_t *idx_out, int32_t *count, void *ws, int64_t ws_bytes,
+                    cudaStream_t st) {
+  switch (K) {
+    case 1: return launch_pareto_t<1>(F, m, idx_out, count, ws, ws_bytes, st);
+    case 2: return launch_pareto_t<2>(F, m, idx_out, count, ws, ws_bytes, st);
+    case 3: return launch_pareto_t<3>(F, m, idx_out, count, ws, ws_bytes, st);
+    case 4: return launch_pareto_t<4>(F, m, idx_out, count, ws, ws_bytes, st);
+    case 5: return launch_pareto_t<5>(F, m, idx_out, count, ws, ws_bytes, st);
+    case 6: return launch_pareto_t<6>(F, m, idx_out, count, ws, ws_bytes, st);
+    case 7: return launch_pareto_t<7>(F, m, idx_out, count, ws, ws_bytes, st);
+    case 8: return launch_pareto_t<8>(F, m, idx_out, count, ws, ws_bytes, st);
+    default: return HB_ERR_INVALID;
+  }
 }
 
 // ================================================================================= multi-GPU front exchange
@@ -325,7 +349,7 @@ int launch_front_merge(const float *all, int64_t world, int64_t capacity, float 
   HB_CUDA(cudaMemsetAsync(cnt, 0, 2 * sizeof(int32_t), st));
   front_unpack_kernel<<<(int)ceil_div(R, 256), 256, 0, st>>>(all, (int)world, (int)capacity, Fm, ovf);
   count_launches(1);
-  const int s = launch_pareto3(Fm, R, idx, cnt, p, (int64_t)pareto_ws_bytes(R), st);
+  const int s = launch_pareto_k(Fm, R, 3, idx, cnt, p, (int64_t)pareto_ws_bytes(R), st);
   if (s != HB_OK) return s;
   front_gather_kernel<<<(int)ceil_div(R + 1, 256), 256, 0, st>>>(all, (int)world, (int)capacity, idx, cnt, ovf, out);
   count_launches(1);

@@ -324,6 +324,63 @@ int launch_acq1(const float *mu, const float *var, int64_t m, int mode, float ka
 }
 
 
+// GeneralAcq.eval (acq.py:211-242) over K = num_obj + num_constr outputs: mu / var [K, m] output-major (row b of output b,
+// as K single-output posterior calls write them).  Every operation is correctly rounded and nothing is contracted into an
+// FMA, so each column is bit-identical to the IEEE fp32 evaluation of the reference's torch expression:
+//   ps = sqrt(ps2).clamp(min = FLT_EPSILON)  (a NaN stays NaN, as torch.clamp keeps it)
+//   py = py + noise_sd * xi                  (when noise_sd != NULL, i.e. use_noise)
+//   Fo = py - kappa * ps (objectives),  Fc = py - c_kappa * ps (constraints)
+// cv = sum_j max(0, Fc[:, j]) in fp32, columns ascending (NaN propagates, so a NaN constraint is never feasible).
+// xi [m, K] (the reference's torch.randn(py.shape)) or NULL: Philox draws keyed by (seed, counter), element q = r K + b
+// takes half q % 2 of the pair q / 2.
+__global__ void __launch_bounds__(256) general_acq_kernel(const float *__restrict__ mu, const float *__restrict__ var, int64_t m,
+                                                          int num_obj, int num_constr, float kappa, float c_kappa,
+                                                          const float *__restrict__ noise_sd, const float *__restrict__ xi,
+                                                          uint64_t seed, uint64_t counter, float *__restrict__ Fo,
+                                                          float *__restrict__ Fc, float *__restrict__ cv) {
+  const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= m) return;
+  const int K = num_obj + num_constr;
+  float viol = 0.0f;
+  for (int b = 0; b < K; ++b) {
+    float py = mu[(int64_t)b * m + r];
+    const float s = __fsqrt_rn(var[(int64_t)b * m + r]);
+    const float ps = s < 1.1920929e-07f ? 1.1920929e-07f : s;
+    if (noise_sd) {
+      const int64_t q = r * K + b;
+      float z;
+      if (xi) {
+        z = xi[q];
+      } else {
+        float z0, z1;
+        philox_normal2(seed, (uint64_t)(q >> 1), counter, z0, z1);
+        z = (q & 1) ? z1 : z0;
+      }
+      py = __fadd_rn(py, __fmul_rn(noise_sd[b], z));
+    }
+    if (b < num_obj) {
+      Fo[r * num_obj + b] = __fsub_rn(py, __fmul_rn(kappa, ps));
+    } else {
+      const float c = __fsub_rn(py, __fmul_rn(c_kappa, ps));
+      if (Fc) Fc[r * num_constr + (b - num_obj)] = c;
+      viol = __fadd_rn(viol, isnan(c) ? c : fmaxf(c, 0.0f));
+    }
+  }
+  if (cv) cv[r] = viol;
+}
+
+int launch_general_acq(const float *mu, const float *var, int64_t m, int64_t num_obj, int64_t num_constr, float kappa,
+                       float c_kappa, const float *noise_sd, const float *xi, uint64_t seed, uint64_t counter, float *Fo,
+                       float *Fc, float *cv, cudaStream_t st) {
+  if (m <= 0 || num_obj < 1 || num_constr < 0 || num_obj + num_constr > HB_MAX_OUTPUTS) return HB_ERR_INVALID;
+  general_acq_kernel<<<(int)ceil_div(m, 256), 256, 0, st>>>(mu, var, m, (int)num_obj, (int)num_constr, kappa, c_kappa, noise_sd,
+                                                            xi, seed, counter, Fo, Fc, cv);
+  count_launches(1);
+  HB_LAUNCH_CHECK("general_acq");
+  return HB_OK;
+}
+
+
 __global__ void __launch_bounds__(256) mace_kernel(const float *__restrict__ mupart, int ncg,
                                                    const float *__restrict__ vpart, int nt,
                                                    const int32_t *__restrict__ fixmap,

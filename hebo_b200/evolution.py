@@ -84,14 +84,21 @@ def rank_and_crowding_survival(F: np.ndarray, n_survive: int) -> np.ndarray:
     return np.asarray(keep, dtype=np.int64)
 
 
-def ga_survive_host(X: np.ndarray, F: np.ndarray, C: np.ndarray, FC: np.ndarray):
+def ga_survive_host(X: np.ndarray, F: np.ndarray, C: np.ndarray, FC: np.ndarray, G: Optional[np.ndarray] = None,
+                    GC: Optional[np.ndarray] = None):
     """numpy restatement of hb_ga_survive in fp32: a non-finite f becomes +inf, a duplicate child (the predicate of
     survive_host) gets +inf, and the P merged rows first in ascending (f, merged index) order survive in that order.
-    Returns the merged indices of the survivors in output order (best first) and the sanitised f [2P]."""
+    With G / GC (hb_ga_survive_cv): cv = max(G, 0), a non-finite G becomes +inf, a duplicate child gets cv = +inf too, and
+    the order is ascending (cv, f, merged index).  Returns the merged indices of the survivors in output order (best first)
+    and the sanitised f [2P] (and cv [2P] when G is given)."""
     P = X.shape[0]
     Xa = np.concatenate([X, C], 0).astype(np.float32)
     f = np.concatenate([np.asarray(F).reshape(-1), np.asarray(FC).reshape(-1)]).astype(np.float32)
     f = np.where(np.isfinite(f), f, np.float32(np.inf))
+    cons = G is not None
+    if cons:
+        g = np.concatenate([np.asarray(G).reshape(-1), np.asarray(GC).reshape(-1)]).astype(np.float32)
+        g = np.where(np.isfinite(g), np.where(g > 0, g, np.float32(0)), np.float32(np.inf)).astype(np.float32)
     # rows the predicate calls equal share a key (0 for |v| < 2^-20, else the bit pattern: the fp32 spacing above 2^-20
     # exceeds 1e-16), so each child is tested against the earlier rows of its key only -- the exact predicate, in O(N D)
     key = np.where(np.abs(Xa) < np.float32(2.0 ** -20), np.uint32(0), Xa.view(np.uint32))
@@ -100,17 +107,22 @@ def ga_survive_host(X: np.ndarray, F: np.ndarray, C: np.ndarray, FC: np.ndarray)
         rows = earlier.setdefault(key[i].tobytes(), [])
         if i >= P and rows and (np.abs(Xa[rows] - Xa[i]) <= np.float32(1e-16)).all(1).any():
             f[i] = np.inf
+            if cons:
+                g[i] = np.inf
         rows.append(i)
+    if cons:
+        return np.lexsort((np.arange(2 * P), f, g))[:P], f, g     # primary cv, then f, then the lower merged index
     order = np.lexsort((np.arange(2 * P), f))          # primary f, ties by the lower merged index
     return order[:P], f
 
 
 def survive_host(X: np.ndarray, F: np.ndarray, C: np.ndarray, FC: np.ndarray, G: Optional[np.ndarray] = None,
                  GC: Optional[np.ndarray] = None):
-    """numpy restatement of the device survival (hb_nsga2_survive_ex, and hb_nsga2_survive_cv when G / GC are given),
-    fp32 like the kernels so that the survivors agree bit for bit: sanitising, duplicate children, the constraint rule,
-    ranks, fp32 crowding of the cut front (see the rules in hebo_b200/csrc/nsga.cu).  Returns the merged indices of the
-    survivors in ascending order, and the sanitised objectives [2P, 3] and constraint [2P] of the merged rows."""
+    """numpy restatement of the device survival (hb_nsga2_survive_ex, and hb_nsga2_survive_cv when G / GC are given;
+    hb_nsga2_survive_k for F with k = F.shape[1] columns), fp32 like the kernels so that the survivors agree bit for bit:
+    sanitising, duplicate children, the constraint rule, ranks, fp32 crowding of the cut front over the k objectives in
+    column order (see the rules in hebo_b200/csrc/nsga.cu).  Returns the merged indices of the survivors in ascending
+    order, and the sanitised objectives [2P, k] and constraint [2P] of the merged rows."""
     P = X.shape[0]
     Xa = np.concatenate([X, C], 0).astype(np.float32)
     f = np.concatenate([F, FC], 0).astype(np.float32)
@@ -143,7 +155,7 @@ def survive_host(X: np.ndarray, F: np.ndarray, C: np.ndarray, FC: np.ndarray, G:
             continue
         fm, m = fr[members], members.size
         crowd = np.zeros(m, np.float32)
-        for k in range(3):
+        for k in range(fm.shape[1]):
             v = fm[:, k]
             order = np.argsort(v, kind="stable")
             pos = np.empty(m, np.int64)
@@ -276,14 +288,22 @@ class DeviceNSGA2:
 
     constrained=True: `score` returns (F [pop, 3], G [pop]) with one constraint column (feasible iff G <= 0, the pymoo
     constraint of evolution_optimizer.py:82,105); survival is hb_nsga2_survive_cv and the result is the feasible front
-    (hebo_b200.pareto.feasible_front).  The generation loop still never synchronises with the host.  There is no
-    constrained single-objective GA: constrained=True with a one-column score raises ValueError."""
+    (hebo_b200.pareto.feasible_front).  The generation loop still never synchronises with the host.  Without `num_obj`
+    there is no constrained single-objective GA: constrained=True with a one-column score raises ValueError.
+
+    num_obj=k (1 <= k <= 8, GeneralBO): the score must have exactly k columns, with or without `constrained`.  k >= 2
+    survives with hb_nsga2_survive_k and returns the (feasible) front; k = 1 with a constraint survives with
+    hb_ga_survive_cv, (cv, f, row) ascending, and returns the first survivor: the best feasible row or, without one, the
+    least infeasible row (pymoo's filter_optimum); k = 1 without a constraint is the GA above.  num_obj=None keeps the
+    column count inferred from the score (1 or 3)."""
 
     KIND = {"real": 0, "int": 1, "choice": 2}
     MAX_POP = 16384                                 # hb_nsga2_survive_ex: single CTA up to 256, cooperative multi-CTA above
+    MAX_OBJ = 8                                     # HB_MAX_OBJ: objectives of hb_nsga2_survive_k
 
     def __init__(self, kinds, lb, ub, num_numeric: int, score: Callable, pop: int = 100, iters: int = 100,
-                 seed: Optional[int] = None, fixed: Optional[dict] = None, device="cuda", constrained: bool = False):
+                 seed: Optional[int] = None, fixed: Optional[dict] = None, device="cuda", constrained: bool = False,
+                 num_obj: Optional[int] = None):
         import torch
         self.torch = torch
         self.D, self.d, self.pop, self.iters = len(kinds), int(num_numeric), int(pop), int(iters)
@@ -302,7 +322,10 @@ class DeviceNSGA2:
         self.constrained = bool(constrained)
         self.seed = int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed)
         self.n_evals = 0
-        self.num_obj = None            # set by the first scored batch: 1 (GA) or 3 (NSGA-II)
+        self.num_obj = None            # set by the first scored batch: 1 (GA) or 3 (NSGA-II), or the given num_obj
+        if num_obj is not None and not 1 <= int(num_obj) <= self.MAX_OBJ:
+            raise ValueError(f"DeviceNSGA2: num_obj must lie in [1, {self.MAX_OBJ}], got {num_obj}")
+        self.k = None if num_obj is None else int(num_obj)
 
     def _bufs(self):
         t, dev, P, D, d = self.torch, self.dev, self.pop, self.D, self.d
@@ -326,7 +349,8 @@ class DeviceNSGA2:
         init = None if initial_suggest is None else t.as_tensor(np.asarray(initial_suggest, dtype=np.float32).reshape(-1, D)).to(self.dev)
         n_init = 0 if init is None else min(init.shape[0], P)
         pc = lambda x: _lib.ptr(x) if x.numel() else None
-        ws_bytes = int(lib.hb_nsga2_workspace_bytes(P, D))
+        k = self.k if self.k is not None and self.k >= 2 else 3          # the single-objective GA uses the 3-objective layout
+        ws_bytes = int(lib.hb_nsga2_workspace_bytes_k(P, D, k))
         if ws_bytes < 0:
             raise _lib.HeboB200Error(f"hb_nsga2_workspace_bytes: invalid size (pop {P}, D {D})")
         ws = t.empty(ws_bytes, dtype=t.uint8, device=self.dev)       # survival workspace, reused by every generation
@@ -341,9 +365,20 @@ class DeviceNSGA2:
                 _lib.check(lib.hb_nsga2_mate(_lib.ptr(X), P, D, d, _lib.ptr(self.kind), _lib.ptr(self.lb), _lib.ptr(self.ub),
                                              _lib.ptr(self.fixed), self.seed, gen, _lib.ptr(C), pc(Cc), pc(Ce), st()), "hb_nsga2_mate")
                 FC, GC = self._scored(Cc, Ce, gen)
-                if self.num_obj == 1:
+                if self.num_obj == 1 and G is not None:
+                    _lib.check(lib.hb_ga_survive_cv(_lib.ptr(X), _lib.ptr(F), _lib.ptr(G), _lib.ptr(C), _lib.ptr(FC), _lib.ptr(GC), P, D, d,
+                                                    _lib.ptr(Xn), _lib.ptr(Fn), _lib.ptr(Gn), pc(Xcn), pc(Xen), _lib.ptr(ws), ws_bytes,
+                                                    st()), "hb_ga_survive_cv")
+                    G, Gn = Gn, G
+                elif self.num_obj == 1:
                     _lib.check(lib.hb_ga_survive(_lib.ptr(X), _lib.ptr(F), _lib.ptr(C), _lib.ptr(FC), P, D, d, _lib.ptr(Xn), _lib.ptr(Fn),
                                                  pc(Xcn), pc(Xen), _lib.ptr(ws), ws_bytes, st()), "hb_ga_survive")
+                elif self.k is not None:
+                    _lib.check(lib.hb_nsga2_survive_k(_lib.ptr(X), _lib.ptr(F), _lib.ptr(G), _lib.ptr(C), _lib.ptr(FC), _lib.ptr(GC), P, D,
+                                                      d, k, _lib.ptr(Xn), _lib.ptr(Fn), _lib.ptr(Gn), pc(Xcn), pc(Xen), _lib.ptr(ws),
+                                                      ws_bytes, st()), "hb_nsga2_survive_k")
+                    if G is not None:
+                        G, Gn = Gn, G
                 elif G is None:
                     _lib.check(lib.hb_nsga2_survive_ex(_lib.ptr(X), _lib.ptr(F), _lib.ptr(C), _lib.ptr(FC), P, D, d, _lib.ptr(Xn),
                                                        _lib.ptr(Fn), pc(Xcn), pc(Xen), _lib.ptr(ws), ws_bytes, st()), "hb_nsga2_survive_ex")
@@ -357,6 +392,14 @@ class DeviceNSGA2:
         self.pop_X, self.pop_F, self.pop_G = X, F, G
         if return_pop and self.num_obj != 1:
             raise ValueError("DeviceNSGA2: return_pop=True needs a one-column score")
+        if self.num_obj == 1 and G is not None:
+            # (cv, f, row) ascending, as hb_ga_survive_cv orders its survivors; after a survival that is the population's order
+            f = np.where(np.isfinite(F.cpu().numpy()), F.cpu().numpy(), np.inf)
+            g = G.cpu().numpy()
+            g = np.where(np.isfinite(g), np.maximum(g, 0), np.inf)
+            order = t.from_numpy(np.lexsort((np.arange(P), f, g))).to(self.dev)
+            idx = order if return_pop else order[:1]
+            return Xc[idx], Xe[idx], F[idx].reshape(-1, 1)
         if self.num_obj == 1:
             f = t.where(t.isfinite(F), F, t.full_like(F, float("inf")))
             if return_pop:
@@ -372,9 +415,12 @@ class DeviceNSGA2:
         out = self.score(Xc, Xe, gen)
         F, G = out if self.constrained else (out, None)
         F = F.reshape(self.pop, -1)
-        if F.shape[1] not in (1, 3):
+        if self.k is not None:
+            if F.shape[1] != self.k:
+                raise ValueError(f"DeviceNSGA2: num_obj={self.k} needs a score with {self.k} columns, got {F.shape[1]}")
+        elif F.shape[1] not in (1, 3):
             raise ValueError(f"DeviceNSGA2: the score must have 1 or 3 columns, got {F.shape[1]}")
-        if F.shape[1] == 1 and self.constrained:
+        elif F.shape[1] == 1 and self.constrained:
             raise ValueError("DeviceNSGA2: constrained=True needs the 3 MACE columns; a one-column score has no constrained GA")
         self.num_obj = F.shape[1]
         F = F.reshape(-1) if self.num_obj == 1 else F

@@ -464,7 +464,9 @@ class GP(BaseModel):
         return self._side_stream
 
     def _posterior(self, Xs_dev: Optional[torch.Tensor], want_F: bool, tau=0.0, kappa=0.0, eps=0.0, xi1=None, xi2=None,
-                   seed: int = 0, want_mu_var: bool = True, Xe_dev: Optional[torch.Tensor] = None):
+                   seed: int = 0, want_mu_var: bool = True, Xe_dev: Optional[torch.Tensor] = None, out=None):
+        """(F, mu, var) of a batch.  out: optional (mu, var) contiguous fp32 [m] device views to write instead of new
+        tensors (a row of the [K, m] buffers of hebo_b200.acq.general_score)."""
         lib = _lib.lib()
         assert self._fitted or hasattr(self, "Linv_dev"), "fit() first"
         # a pinned host batch larger than one chunk is uploaded chunk by chunk under the scoring (same results)
@@ -479,14 +481,18 @@ class GP(BaseModel):
             return (torch.empty(0, 3, dtype=torch.float32, device=dev) if want_F else None,
                     e if want_mu_var else None, e.clone() if want_mu_var else None)
         F = torch.empty(m, 3, dtype=torch.float32, device=dev) if want_F else None
-        mu = torch.empty(m, dtype=torch.float32, device=dev) if want_mu_var else None
-        var = torch.empty(m, dtype=torch.float32, device=dev) if want_mu_var else None
+        if out is not None:
+            mu, var = out
+        else:
+            mu = torch.empty(m, dtype=torch.float32, device=dev) if want_mu_var else None
+            var = torch.empty(m, dtype=torch.float32, device=dev) if want_mu_var else None
         if self._fit_failed:
             # gp.py:152-154: "jitter is too large, output random predictions" = N(0, I) in the standardised space, pushed
             # through the same un-scaling and (for F) the MACE epilogue kernel -- never the leftovers of a failed factorisation
             print("jitter is too large, output random predictions")
-            mu_f = torch.full((m,), self._y_mean, dtype=torch.float32, device=dev)
-            var_f = torch.full((m,), max(self._y_std ** 2, EPS32), dtype=torch.float32, device=dev)
+            mu_f = torch.full((m,), self._y_mean, dtype=torch.float32, device=dev) if out is None else mu.fill_(self._y_mean)
+            var_f = (torch.full((m,), max(self._y_std ** 2, EPS32), dtype=torch.float32, device=dev) if out is None
+                     else var.fill_(max(self._y_std ** 2, EPS32)))
             if want_F:
                 with torch.cuda.device(dev):
                     _lib.check(lib.hb_mace_epilogue(_lib.ptr(mu_f), _lib.ptr(var_f), m, float(self.noise[0]), float(tau), float(kappa),

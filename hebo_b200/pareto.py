@@ -1,4 +1,4 @@
-"""Device non-dominated filter (3 objectives, minimised) through the C ABI.
+"""Device non-dominated filter (1 to 8 objectives, minimised) through the C ABI.
 
 Replaces the rank-0 extraction NSGA-II performs on the final population
 (HEBO/hebo/acq_optimizers/evolution_optimizer.py:141-149) for candidate batches of any size.
@@ -24,32 +24,38 @@ def _workspace(dev: torch.device, need: int, tag: str = "front") -> torch.Tensor
 
 
 def pareto_front_device(F: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
-    """F [m,3] float32 CUDA tensor -> (idx int32 [m] whose first `count` entries are the ascending indices of the
-    non-dominated rows, count int32 [1]), both on the device; NO host synchronisation."""
+    """F [m,k] float32 CUDA tensor, 1 <= k <= 8 -> (idx int32 [m] whose first `count` entries are the ascending indices
+    of the non-dominated rows, count int32 [1]), both on the device; NO host synchronisation.  k = 3 runs
+    hb_pareto_front3, any other k hb_pareto_front_k."""
     lib = _lib.lib()
-    assert F.is_cuda and F.dim() == 2 and F.shape[1] == 3
+    assert F.is_cuda and F.dim() == 2 and 1 <= F.shape[1] <= _lib.HB_MAX_OBJ
     F = F.to(torch.float32).contiguous()
     m = F.shape[0]
     dev = F.device
     ws = _workspace(dev, int(lib.hb_pareto_workspace_bytes(m)))
     idx = torch.empty(m, dtype=torch.int32, device=dev)
     cnt = torch.zeros(1, dtype=torch.int32, device=dev)
+    k = F.shape[1]
     with torch.cuda.device(dev):
-        st = lib.hb_pareto_front3(_lib.ptr(F), m, _lib.ptr(idx), _lib.ptr(cnt), _lib.ptr(ws), ws.numel(),
-                                  _lib.stream_ptr())
-    _lib.check(st, "hb_pareto_front3")
+        if k == 3:
+            st = lib.hb_pareto_front3(_lib.ptr(F), m, _lib.ptr(idx), _lib.ptr(cnt), _lib.ptr(ws), ws.numel(),
+                                      _lib.stream_ptr())
+        else:
+            st = lib.hb_pareto_front_k(_lib.ptr(F), m, k, _lib.ptr(idx), _lib.ptr(cnt), _lib.ptr(ws), ws.numel(),
+                                       _lib.stream_ptr())
+    _lib.check(st, "hb_pareto_front")
     return idx, cnt
 
 
 def pareto_front(F: torch.Tensor) -> torch.Tensor:
-    """F [m,3] float32 CUDA tensor -> ascending int64 indices (on the device) of the non-dominated rows
+    """F [m,k] float32 CUDA tensor -> ascending int64 indices (on the device) of the non-dominated rows
     (one host read of the count)."""
     idx, cnt = pareto_front_device(F)
     return idx[:int(cnt.item())].to(torch.int64)
 
 
 def feasible_front(F: torch.Tensor, G: torch.Tensor) -> torch.Tensor:
-    """Rank-0 set under one constraint column: F [m,3], G [m] CUDA tensors -> ascending int64 indices (on the device).
+    """Rank-0 set under one constraint column: F [m,k], G [m] CUDA tensors -> ascending int64 indices (on the device).
     A row is feasible iff G <= 0 (a non-finite G counts as +inf, as in hb_nsga2_survive_cv).  The result is the
     non-dominated set of the feasible rows; with no feasible row it is the single least infeasible row (smallest G, lowest
     index), which is what pymoo's filter_optimum(least_infeasible=True) is recalled to return -- not checked against

@@ -70,6 +70,9 @@ extern "C" {
 /* Most outputs one batched fit (hb_fit_multi_ex) trains together. */
 #define HB_MAX_OUTPUTS     32
 
+/* Most objectives the k-objective survival (hb_nsga2_survive_k) and front (hb_pareto_front_k) take. */
+#define HB_MAX_OBJ         8
+
 /* Model description beyond the numeric ARD default (HOST struct; NULL = numeric-only, ard_kernel=True). */
 typedef struct {
   int32_t        ard_kernel;  /* conf['ard_kernel'] (models/gp/gp.py:47, gp_util.py:45): 0 = one shared numeric lengthscale */
@@ -332,12 +335,36 @@ int32_t hb_mace_epilogue(const float *mu, const float *var, int64_t m, float noi
 int32_t hb_acq1_epilogue(const float *mu, const float *var, int64_t m, int32_t mode, float kappa, float eta, float *f,
                          void *stream);
 
+/* ---- GeneralAcq epilogue  (GeneralAcq.eval, acquisitions/acq.py:211-242: LCB of every objective and constraint of a
+ * multi-output model, used by GeneralBO, optimizers/general.py:65-158) ----
+ * mu, var [K, m] device, output-major (row b = output b, as K single-output posterior calls with F = NULL write them),
+ * K = num_obj + num_constr, 1 <= num_obj, 0 <= num_constr, K <= HB_MAX_OUTPUTS.  With py = mu, ps2 = var (per column b):
+ *   ps = sqrt(ps2).clamp(min = FLT_EPSILON)         (NaN stays NaN)
+ *   py = py + noise_sd[b] * xi                        only when noise_sd [K] != NULL (use_noise; noise_sd = model.noise.sqrt())
+ *   Fo [m, num_obj]    = py - kappa * ps              objectives
+ *   Fc [m, num_constr] = py - c_kappa * ps            constraints (may be NULL)
+ *   cv [m]             = sum_j max(0, Fc[:, j])       constraint violation, fp32, columns ascending (may be NULL; a NaN
+ *                                                     constraint gives cv = NaN, which the survivals treat as +inf)
+ * Correctly rounded operations, no FMA contraction: each column is bit-identical to the IEEE fp32 evaluation of the
+ * reference's torch expression on the same mu / var / draws.  xi [m, K] device draws (the reference's torch.randn(py.shape))
+ * or NULL: Philox4x32-10 + Box-Muller keyed by (seed, counter); element q = r K + b takes half q % 2 of pair q / 2, and the
+ * same (seed, counter) replays the same bits.  cv is pymoo's constraint violation as recalled from pymoo 0.6 (a sum of the
+ * positive parts), not checked against pymoo; feasibility (cv <= 0 exactly when every constraint is <= 0) and the order of
+ * the infeasible rows do not depend on the aggregation, so a sum and a mean give the same survivors.  One launch. */
+int32_t hb_general_acq_epilogue(const float *mu, const float *var, int64_t m, int64_t num_obj, int64_t num_constr, float kappa,
+                                float c_kappa, const float *noise_sd, const float *xi, uint64_t seed, uint64_t counter, float *Fo,
+                                float *Fc, float *cv, void *stream);
+
 /* ---- 3-objective non-dominated filter  (the rank-0 set NSGA-II returns as res.X,
  * acq_optimizers/evolution_optimizer.py:141-149) ----------------------------------------------
  * F [m,3]; idx_out [m] int32 ascending indices of the non-dominated rows; count device int32.
  * Rows with a NaN objective are excluded (they can neither dominate nor be dominated, and must never be recommended). */
 int32_t hb_pareto_front3(const float *F, int64_t m, int32_t *idx_out, int32_t *count,
                          void *ws, int64_t ws_bytes, void *stream);
+/* The same filter over F [m, num_obj], 1 <= num_obj <= HB_MAX_OBJ, same workspace (hb_pareto_workspace_bytes(m)) and rules;
+ * hb_pareto_front3 is num_obj = 3. */
+int32_t hb_pareto_front_k(const float *F, int64_t m, int64_t num_obj, int32_t *idx_out, int32_t *count,
+                          void *ws, int64_t ws_bytes, void *stream);
 
 /* ---- device NSGA-II  (acq_optimizers/evolution_optimizer.py:107-160: pymoo NSGA2 with MixedVariableMating over the MACE
  * objectives; variable typing :26-41).  The population lives on the device: X [pop, D] fp32 rows in the optimisation space
@@ -382,6 +409,26 @@ int32_t hb_nsga2_survive_cv(const float *X, const float *F, const float *G, cons
  *   hb_nsga2_survive_ex (ws may be NULL when pop <= 256); both kernels give the same bytes, deterministic, one launch. */
 int32_t hb_ga_survive(const float *X, const float *F, const float *C, const float *FC, int64_t pop, int64_t D, int64_t d,
                       float *X_next, float *F_next, float *Xc_next, int32_t *Xe_next, void *ws, int64_t ws_bytes, void *stream);
+/* hb_ga_survive_cv: the same survival with one constraint column (FitnessSurvival with constraints, np.lexsort([F, cv]),
+ *   which EvolutionOpt runs for a constrained one-objective acquisition, evolution_optimizer.py:132-133; recalled from
+ *   pymoo 0.6, not checked against it).  G [pop] / GC [pop]: the constraint of the population / offspring; cv = max(G, 0),
+ *   a non-finite G counts as +inf, a duplicate child gets cv = f = +inf.  The survivors are the pop merged rows first in
+ *   ascending (cv, f, merged index) order, best first, so row 0 is the best feasible row or, without one, the least
+ *   infeasible row (pymoo's filter_optimum).  G_next [pop] out: their cv.  Same sizes, workspace and determinism as
+ *   hb_ga_survive; G = GC = 0 gives its bytes except among the f = +inf rows when one of them is a duplicate child. */
+int32_t hb_ga_survive_cv(const float *X, const float *F, const float *G, const float *C, const float *FC, const float *GC, int64_t pop,
+                         int64_t D, int64_t d, float *X_next, float *F_next, float *G_next, float *Xc_next, int32_t *Xe_next, void *ws,
+                         int64_t ws_bytes, void *stream);
+/* hb_nsga2_survive_k: the rank-and-crowding survival of hb_nsga2_survive_ex / _cv over num_obj objectives,
+ *   2 <= num_obj <= HB_MAX_OBJ: F / FC [pop, num_obj], F_next [pop, num_obj]; crowding adds the num_obj objectives in
+ *   column order, each normalised by its own range.  G / GC / G_next all NULL: the unconstrained survival; all three given:
+ *   the constrained one.  ws_bytes >= hb_nsga2_workspace_bytes_k(pop, D, num_obj) when pop > 256.  hb_nsga2_survive_ex and
+ *   hb_nsga2_survive_cv are the num_obj = 3 instances (same kernels, same bytes), and hb_nsga2_workspace_bytes(pop, D) =
+ *   hb_nsga2_workspace_bytes_k(pop, D, 3). */
+int64_t hb_nsga2_workspace_bytes_k(int64_t pop, int64_t D, int64_t num_obj);
+int32_t hb_nsga2_survive_k(const float *X, const float *F, const float *G, const float *C, const float *FC, const float *GC,
+                           int64_t pop, int64_t D, int64_t d, int64_t num_obj, float *X_next, float *F_next, float *G_next,
+                           float *Xc_next, int32_t *Xe_next, void *ws, int64_t ws_bytes, void *stream);
 
 /* ---- bound violation of a random embedding  (MACE_Embedding.eval, optimizers/hebo_embedding.py:85-90, clip = False)
  * Y [m, e] candidates in the embedding, B [e, D] projection matrix, both row-major fp32 on the device; G [m] out:
