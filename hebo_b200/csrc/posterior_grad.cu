@@ -408,8 +408,9 @@ __global__ void __launch_bounds__(SB_THREADS, 1) sample_batch_kernel(
       break;
     }
     __syncthreads();                                     // every thread has read the failed pivot before the reload
-    jitter *= 10.0f;
-    if (jitter > 10.0f) break;
+    const float next = jitter * 10.0f;
+    if (next > 10.0f) break;                             // give up: `jitter` stays the last rung tried
+    jitter = next;
   }
   if (t == 0) *jitter_out = jitter;
   if (!ok) {
