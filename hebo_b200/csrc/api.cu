@@ -768,6 +768,8 @@ int32_t hb_posterior_grad_ex(const float *Xs, const int32_t *Xe_s, int64_t m, in
                              const float *Zt, const float *alpha, const float *Linv, const float *hyp, int32_t kern, float y_mean,
                              float y_std, int32_t pred_likeli, float *mu, float *var, float *dmu, float *dvar, void *ws,
                              int64_t ws_bytes, int64_t m_chunk, void *stream) {
+  // post_grad_kernel differentiates through x_mul / l only: a warp is the caller's, in front of this call
+  if (spec && spec->warp != 0) return HB_ERR_INVALID;
   ModelSpec sp;
   if (d <= 0 || !build_spec(d, spec, sp)) return HB_ERR_INVALID;
   if (!Xs || !x_mul || !x_add || !Zt || !alpha || !Linv || !hyp || !ws || !mu || !var || !dmu || !dvar) return HB_ERR_INVALID;

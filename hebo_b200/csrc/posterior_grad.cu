@@ -111,9 +111,10 @@ __global__ void __launch_bounds__(256) post_grad_kernel(const float *__restrict_
     w[i] = b;
   }
   __syncthreads();
-  // value path, exactly as mace_kernel
-  float mu_t = hyp[1];
+  // value path, exactly as mace_kernel: the mean partials first, the constant last
+  float mu_t = 0.0f;
   for (int g = 0; g < ncg; ++g) mu_t += mupart[(int64_t)g * mc_pad + r];
+  mu_t += hyp[1];
   float raw_var = s - s_vsq;
   if (pred_likeli) raw_var += hyp[0];           // lik(pred) adds the noise before the variance floor (gp.py:158-161)
   const float var_t = fmaxf(raw_var, 1e-6f);

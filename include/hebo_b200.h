@@ -262,7 +262,10 @@ int32_t hb_posterior_mace_ex(const float *Xs, const int32_t *Xe_s, int64_t m, in
  * models/gp/gp.py:137-164) -------------------------------------------------------------------------------------
  * Same inputs as hb_posterior_mace (FP32 SIMT contraction; Linv only).  mu, var [m] as above;
  * dmu, dvar [m, d] = d mu / d Xs, d var / d Xs (closed form; zero where a variance floor is active, like clamp_min).
- * ws: hb_posterior_workspace_bytes(n, d, m_chunk). */
+ * ws: hb_posterior_workspace_bytes(n, d, m_chunk).
+ * No input warp: hb_posterior_grad_ex returns HB_ERR_INVALID for spec->warp != 0.  A warped model's caller applies the
+ * Kumaraswamy warp in front, as hebo_b200.GP._predict_autograd does -- Xs = the warped MinMax-scaled rows, x_mul = 1,
+ * x_add = 0, spec->warp = 0 -- and chains dw/dx onto dmu / dvar itself. */
 int32_t hb_posterior_grad(const float *Xs, int64_t m, int64_t n, int64_t d,
                           const float *x_mul, const float *x_add,
                           const float *Zt, const float *alpha, const float *Linv, const float *hyp, int32_t kern,

@@ -20,8 +20,7 @@ from hebo_b200 import _lib
 from oracle import emb_oracle as E
 from oracle import gp_oracle as O
 from oracle import warp_oracle as W
-from tests.test_gpu_highdim import _emb_hypers
-from tests.util import seeded_problem
+from tests.util import emb_hypers, seeded_problem
 
 pytestmark = pytest.mark.gpu
 
@@ -243,7 +242,7 @@ def _family_ref(name, m, raw, dtype):
         loss, g = W.neg_mll_autograd(Xt, y, raw.to(dtype), NOISE_LB, "matern32", m.noise_guess)
         return float(loss), g.double()
     Xe = m.Xe.long().cpu() if m.Xe is not None else torch.zeros(m.n, 0, dtype=torch.long)
-    hp = _emb_hypers(m.owner, raw)
+    hp = emb_hypers(m.owner, raw)
     hp = E.EmbHypers(*(v.to(dtype) if torch.is_tensor(v) else [t.to(dtype) for t in v] if isinstance(v, list) else v
                        for v in (hp.raw_noise, hp.tables, hp.mean, hp.raw_os, hp.raw_ls, hp.raw_ls_e, hp.noise_lb)))
     loss, g = E.neg_mll_emb_closed_form(Xt, Xe, y, hp, m.noise_guess)

@@ -12,7 +12,7 @@ import hebo_b200
 from oracle import emb_oracle as E
 from oracle import gp_oracle as O
 from oracle import warp_oracle as W
-from tests.util import mu_sigma_errors, oracle_posterior, seeded_problem
+from tests.util import emb_hypers, mu_sigma_errors, oracle_posterior, scaled_xy, seeded_problem
 
 pytestmark = pytest.mark.gpu
 
@@ -37,12 +37,6 @@ def blocked_oracle(monkeypatch):
     monkeypatch.setattr(O, "kernel_matrix", _kernel_matrix_blocked)
 
 
-def _scaled(gp, X, y):
-    Xt64 = gp.xscaler.scale_.double() * X.double() + gp.xscaler.min_.double()
-    yt64 = (y.double().reshape(-1) - float(gp.yscaler.mean[0])) / float(gp.yscaler.std[0])
-    return Xt64, yt64
-
-
 @pytest.mark.parametrize("d", [128, 200])
 def test_fit_trajectory_past_the_former_shared_memory_limit(d):
     """d >= 128 used to be rejected by the MLL gradient launcher (per-warp accumulators of 8 (3 d + 3) floats)."""
@@ -58,7 +52,7 @@ def test_fit_trajectory_past_the_former_shared_memory_limit(d):
     raw0[1] += 0.5
     gp = hebo_b200.GP(d, 0, 1, num_epochs=5, init_raw=raw0, **conf)
     gp.fit(X, None, y)
-    Xt64, yt64 = _scaled(gp, X, y)
+    Xt64, yt64 = scaled_xy(gp, X, y)
     hp0 = O.Hypers.unpack(raw0.double(), 8e-4)
     hp, losses = O.fit_psgld(Xt64, yt64, hp0, "matern32", lr=0.01, num_epochs=5, record=True)
     dl = np.abs(gp.losses - np.array(losses))
@@ -87,7 +81,7 @@ def test_posterior_parity_at_high_d(n, d, kind, blocked_oracle):
     gp = hebo_b200.GP(d, 0, 1, kernel=kind, lr=0.01, num_epochs=3, noise_lb=8e-4, pred_likeli=False, langevin=False,
                       m_chunk=128)
     gp.fit(X, None, y)
-    Xt64, yt64 = _scaled(gp, X, y)
+    Xt64, yt64 = scaled_xy(gp, X, y)
     f = O.FittedGP(Xt64, O.Hypers.unpack(gp.raw.double(), 8e-4), kind, gp.xscaler.scale_.double(), gp.xscaler.min_.double(),
                    float(gp.yscaler.mean[0]), float(gp.yscaler.std[0]))
     f._yt = yt64
@@ -123,17 +117,6 @@ def _mixed_problem(n, d, num_uniqs, seed):
     return Xc, Xe, y.reshape(-1, 1)
 
 
-def _emb_hypers(gp, raw):
-    raw = raw.double()
-    lay = gp._param_layout()
-    tabs, o = [], lay["tab"]
-    for u, e in zip(gp.num_uniqs, gp.emb_sizes):
-        tabs.append(raw[o:o + u * e].reshape(u, e))
-        o += u * e
-    rle = raw[lay["le"]] if gp.num_enum else torch.zeros((), dtype=torch.float64)
-    return E.EmbHypers(raw[0], tabs, raw[lay["mean"]], raw[lay["os"]], raw[lay["ls"]:lay["ls"] + lay["n_ls"]], rle, gp.noise_lb)
-
-
 def _check_loss_grad(gp, oracle, what, steps=(0.0, 0.25)):
     P = gp._param_layout()["P"]
     g = torch.Generator().manual_seed(3)
@@ -160,8 +143,8 @@ def test_mixed_model_loss_gradient_posterior(name, n, d, nu):
     gp.fit(Xc, Xe, y)
     if name == "wide_embeddings":
         assert gp.De == 300
-    Xt, yt = _scaled(gp, Xc, y)
-    raw = _check_loss_grad(gp, lambda r: E.neg_mll_emb_closed_form(Xt, Xe.long(), yt, _emb_hypers(gp, r)), name)
+    Xt, yt = scaled_xy(gp, Xc, y)
+    raw = _check_loss_grad(gp, lambda r: E.neg_mll_emb_closed_form(Xt, Xe.long(), yt, emb_hypers(gp, r)), name)
     m = 300
     g = torch.Generator().manual_seed(9)
     Xs_c = torch.rand(m, d, generator=g) * 4.4 - 1.2
@@ -169,7 +152,7 @@ def test_mixed_model_loss_gradient_posterior(name, n, d, nu):
     Xs_c[:50], Xs_e[:50] = Xc[:50], Xe[:50]
     mu, var = gp.predict(Xs_c, Xs_e)
     Xs_t = gp.xscaler.scale_.double() * Xs_c.double() + gp.xscaler.min_.double()
-    mu_o, var_o = E.predict_emb(Xt, Xe.long(), yt, _emb_hypers(gp, raw), Xs_t, Xs_e.long())
+    mu_o, var_o = E.predict_emb(Xt, Xe.long(), yt, emb_hypers(gp, raw), Xs_t, Xs_e.long())
     ys, ym = float(gp.yscaler.std[0]), float(gp.yscaler.mean[0])
     mu_o, var_o = mu_o * ys + ym, var_o * ys ** 2
     emu = float(((mu.double().reshape(-1) - mu_o).abs() / mu_o.abs().clamp_min(ys)).max())
@@ -186,7 +169,7 @@ def test_learned_warp_loss_gradient_at_d300():
     torch.manual_seed(0)
     gp = hebo_b200.GP(d, 0, 1, lr=0.01, num_epochs=0, noise_lb=8e-4, pred_likeli=False, warp=True)
     gp.fit(X, None, y)
-    Xt, yt = _scaled(gp, X, y)
+    Xt, yt = scaled_xy(gp, X, y)
     _check_loss_grad(gp, lambda r: W.neg_mll_autograd(Xt, yt, r.double()), "warp d=300", steps=(0.0, 0.3))
 
 
@@ -197,8 +180,8 @@ def test_shared_lengthscale_loss_gradient_at_d1024():
     torch.manual_seed(0)
     gp = hebo_b200.GP(d, 0, 1, lr=0.01, num_epochs=0, noise_lb=8e-4, pred_likeli=False, ard_kernel=False)
     gp.fit(X, None, y)
-    Xt, yt = _scaled(gp, X, y)
-    _check_loss_grad(gp, lambda r: E.neg_mll_emb_closed_form(Xt, torch.zeros(n, 0).long(), yt, _emb_hypers(gp, r)),
+    Xt, yt = scaled_xy(gp, X, y)
+    _check_loss_grad(gp, lambda r: E.neg_mll_emb_closed_form(Xt, torch.zeros(n, 0).long(), yt, emb_hypers(gp, r)),
                      "ard_kernel=False d=1024")
 
 
@@ -217,7 +200,7 @@ def test_input_gradients_and_samples_at_d1024(blocked_oracle):
     mu1, var1 = gp.predict(xa, None)
     ((wm * mu1).sum() + (wv * var1).sum()).backward()
     dt = torch.float64
-    Xt, yt = _scaled(gp, X, y)
+    Xt, yt = scaled_xy(gp, X, y)
     xb = Xs.to(dt).clone().requires_grad_(True)
     f = O.FittedGP(Xt, O.Hypers.unpack(gp.raw.to(dt), 8e-4), "matern32", torch.ones(d, dtype=dt), torch.zeros(d, dtype=dt),
                    float(gp.yscaler.mean[0]), float(gp.yscaler.std[0]))

@@ -66,6 +66,26 @@ def seeded_problem(n, d, seed, dtype=torch.float32):
     return X.to(dtype), y.to(dtype).reshape(-1, 1)
 
 
+def scaled_xy(gp, X, y):
+    """fp64 training rows through the fitted GP's MinMax scaler and y through its standardisation."""
+    Xt64 = gp.xscaler.scale_.double() * X.double() + gp.xscaler.min_.double()
+    yt64 = (y.double().reshape(-1) - float(gp.yscaler.mean[0])) / float(gp.yscaler.std[0])
+    return Xt64, yt64
+
+
+def emb_hypers(gp, raw):
+    """oracle/emb_oracle.py EmbHypers of a GP's raw vector (fp64): noise, tables, mean, outputscale, lengthscales."""
+    from oracle import emb_oracle as E
+    raw = raw.double()
+    lay = gp._param_layout()
+    tabs, o = [], lay["tab"]
+    for u, e in zip(gp.num_uniqs, gp.emb_sizes):
+        tabs.append(raw[o:o + u * e].reshape(u, e))
+        o += u * e
+    rle = raw[lay["le"]] if gp.num_enum else torch.zeros((), dtype=torch.float64)
+    return E.EmbHypers(raw[0], tabs, raw[lay["mean"]], raw[lay["os"]], raw[lay["ls"]:lay["ls"] + lay["n_ls"]], rle, gp.noise_lb)
+
+
 def oracle_posterior(X, yt, raw, kind, Xs, dtype, warp=None, noise_diag=None, pred_likeli=False, noise_lb=8e-4):
     """Oracle predict() (mu, var in y units, flattened float64 numpy) in `dtype` at raw hypers `raw`.
 
