@@ -188,7 +188,7 @@ template <int K>
 static int launch_pareto_t(const float *F, int64_t m, int32_t *idx_out, int32_t *count, void *ws, int64_t ws_bytes,
                            cudaStream_t st) {
   if (m <= 0 || m > 0x7fffffff) return HB_ERR_INVALID;
-  if ((size_t)ws_bytes < pareto_ws_bytes(m)) return HB_ERR_INVALID;
+  if (ws_bytes < 0 || (size_t)ws_bytes < pareto_ws_bytes(m)) return HB_ERR_INVALID;
   ParetoWs w = carve_pareto(ws, m);
   const int mi = (int)m;
   // B-list segments per launch: enough blocks to fill the machine when list A is short
@@ -340,7 +340,7 @@ int launch_front_merge(const float *all, int64_t world, int64_t capacity, float 
                        cudaStream_t st) {
   const int64_t R = world * capacity;
   if (world <= 0 || capacity <= 0 || R > 0x3fffffff) return HB_ERR_INVALID;
-  if ((size_t)ws_bytes < front_merge_ws_bytes(world, capacity)) return HB_ERR_INVALID;
+  if (ws_bytes < 0 || (size_t)ws_bytes < front_merge_ws_bytes(world, capacity)) return HB_ERR_INVALID;
   unsigned char *p = reinterpret_cast<unsigned char *>(ws);
   float *Fm = reinterpret_cast<float *>(p);                 p += round_up(R * 3 * 4, 256);
   int32_t *idx = reinterpret_cast<int32_t *>(p);            p += round_up(R * 4, 256);

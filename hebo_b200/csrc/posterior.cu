@@ -472,7 +472,7 @@ int launch_posterior_mace(const float *Xs, const int32_t *Xe_s, int64_t m, int64
   const int64_t d = sp.d;
   if (m <= 0 || n <= 0 || sp.dtot() <= 0 || np % GT != 0 || n > np || m_chunk <= 0) return HB_ERR_INVALID;
   if (kern < 0 || kern > 2 || (sp.e > 0 && (!Xe_s || !tab_s))) return HB_ERR_INVALID;
-  if ((size_t)ws_bytes < posterior_ws_bytes(np, d, m_chunk)) return HB_ERR_INVALID;
+  if (ws_bytes < 0 || (size_t)ws_bytes < posterior_ws_bytes(np, d, m_chunk)) return HB_ERR_INVALID;
   const int64_t mc_pad_max = round_up(m_chunk, CHUNK_ROWS);
   const int ncg = (int)ceil_div(np, KS_GROUP);
   const int nt = (int)(np / GT);

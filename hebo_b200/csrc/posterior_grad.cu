@@ -154,7 +154,7 @@ int launch_posterior_grad(const float *Xs, const int32_t *Xe_s, int64_t m, int64
   if (m <= 0 || n <= 0 || d <= 0 || np % GT != 0 || n > np || m_chunk <= 0) return HB_ERR_INVALID;
   if (sp.e > 0 && (!Xe_s || !tab_s)) return HB_ERR_INVALID;
   if (kern < 0 || kern > 2 || !mu || !var || !dmu || !dvar) return HB_ERR_INVALID;
-  if ((size_t)ws_bytes < posterior_ws_bytes(np, d, m_chunk)) return HB_ERR_INVALID;
+  if (ws_bytes < 0 || (size_t)ws_bytes < posterior_ws_bytes(np, d, m_chunk)) return HB_ERR_INVALID;
   const int64_t mc_pad_max = round_up(m_chunk, 2 * GT);
   const int ncg = kstar_groups(np);
   const int nt = (int)(np / GT);
@@ -269,7 +269,7 @@ int launch_sample_y(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, 
                     const float *hyp_host, int kern, float y_mean, float y_std, int pred_likeli, const float *z, int n_samples,
                     float *out, float *jitter_used, void *ws, int64_t ws_bytes, cudaStream_t st) {
   if (m <= 0 || m > 8192 || n <= 0 || np % GT != 0 || n_samples <= 0 || kern < 0 || kern > 2 || !hyp_host) return HB_ERR_INVALID;
-  if ((size_t)ws_bytes < sample_ws_bytes(np, sp.dtot(), m)) return HB_ERR_INVALID;
+  if (ws_bytes < 0 || (size_t)ws_bytes < sample_ws_bytes(np, sp.dtot(), m)) return HB_ERR_INVALID;
   const int64_t mp = round_up(m, 2 * GT);
   const int ncg = kstar_groups(np);
   float *KS = reinterpret_cast<float *>(ws);
@@ -440,7 +440,7 @@ int launch_sample_y_batch(const float *Xs, const int32_t *Xe_s, int64_t m, int64
                           uint64_t seed, uint64_t counter, float *f, float *jitter_out, int32_t *status, void *ws, int64_t ws_bytes,
                           cudaStream_t st) {
   if (m <= 0 || m > SB_MAX || n <= 0 || np % GT != 0 || kern < 0 || kern > 2) return HB_ERR_INVALID;
-  if ((size_t)ws_bytes < sample_ws_bytes(np, sp.dtot(), m)) return HB_ERR_INVALID;
+  if (ws_bytes < 0 || (size_t)ws_bytes < sample_ws_bytes(np, sp.dtot(), m)) return HB_ERR_INVALID;
   static PerDevice once;   // the opt-in above 48 KB of dynamic shared memory is per device
   bool fresh = false;
   const int dev = once.slot(&fresh);

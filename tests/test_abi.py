@@ -70,6 +70,29 @@ def test_invalid_arguments_are_reported_not_crashed(lib):
     assert lib.hb_mll_fwd_bwd(None, None, None, 10, 2, None, None, 0, None, 0.0, 0.01, 0.0, None, None, None, None, 0, None) == _lib.HB_ERR_INVALID
 
 
+@pytest.mark.parametrize("ws_bytes", ["short", -1, -(1 << 40)])
+def test_workspace_size_is_checked_as_a_signed_count(lib, ws_bytes):
+    """A workspace one byte short, or of negative size, is refused before any launch.  A negative int64 must not pass the
+    check as a huge size_t.  The pointers are fake and never dereferenced."""
+    bad = _lib.HB_ERR_INVALID
+    p = ctypes.c_void_p(16)
+
+    def ws(need):
+        assert need > 0
+        return need - 1 if ws_bytes == "short" else ws_bytes
+    m = 5000
+    need = int(lib.hb_pareto_workspace_bytes(m))
+    assert lib.hb_pareto_front3(p, m, p, p, p, ws(need), None) == bad
+    for k in (1, 3, 8):
+        assert lib.hb_pareto_front_k(p, m, k, p, p, p, ws(need), None) == bad, k
+    need = int(lib.hb_front_merge_workspace_bytes(4, 64))
+    assert lib.hb_front_merge(p, 4, 64, p, p, ws(need), None) == bad
+    n, d = 300, 2
+    need = int(lib.hb_sample_workspace_bytes(n, d, None, 100))
+    assert lib.hb_sample_y(p, None, 100, n, d, None, None, None, p, p, p, p, p, p, p, 0, 0.0, 1.0, 0, p, 3, p, None, p,
+                           ws(need), None) == bad
+
+
 def test_missing_library_fails_loudly(monkeypatch, tmp_path):
     monkeypatch.setattr(_lib, "_lib", None)
     monkeypatch.setattr(_lib, "LIB_PATH", str(tmp_path / "nope.so"))

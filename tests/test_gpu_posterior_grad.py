@@ -57,78 +57,27 @@ import numpy as np
 import pytest
 import torch
 
-from hebo_b200 import GP, _lib
+from hebo_b200 import _lib
 from hebo_b200.scalers import kumaraswamy_warp
 from oracle import gp_oracle as O
-from tests.util import emb_hypers, scaled_xy, seeded_problem
+from tests.util import (DEV, RATE, VARIANTS, WIDTHS, candidates, features64, fit_model, gather_emb, kernel_parts, kmat64,
+                        true_model)
 
 pytestmark = pytest.mark.gpu
 
-DEV = torch.device("cuda")
 U = 2.0 ** -24
 C_MAX = 6.0             # the c of reference (a); the cases below need at most 1.7 on an H100
 CANCEL = 0.02           # sigma^2 / s below which the variance is cancellation residue (test_gpu_fullsize.py)
 EPS32 = float(np.finfo(np.float32).eps)
 SENTINEL = -777.25
 TAIL = 257
-RATE = {"matern32": math.sqrt(3.0), "matern52": math.sqrt(5.0)}
 FLUSH = 2.0 ** -102     # u FLUSH = 2^-126: fast_exp flushes results below it to zero
 
 
 # ---------------------------------------------------------------------------------------------------------------- models
-_MODELS = {}
-
-
-def _fit(key, n, d, num_uniqs=(), pred_likeli=True, seed=5, epochs=10, **conf):
-    if key in _MODELS:
-        return _MODELS[key]
-    X, y = seeded_problem(n, d, seed)
-    g = torch.Generator().manual_seed(seed + 100)
-    Xe = None
-    if num_uniqs:
-        Xe = torch.stack([torch.randint(u, (n,), generator=g) for u in num_uniqs], 1)
-        y = y + 0.4 * Xe[:, :1].float() - 0.2 * Xe[:, -1:].float()
-    if conf.get("noise_diag") == "hetero":
-        conf["noise_diag"] = (1e-2 * (1 + (X.double() ** 2).sum(1) / d)).float()
-    if conf.get("warp_a") == "fixed":
-        conf["warp_a"] = (torch.rand(d, generator=g) * 1.5 + 0.5).tolist()
-        conf["warp_b"] = (torch.rand(d, generator=g) * 1.5 + 0.5).tolist()
-    torch.manual_seed(seed)
-    np.random.seed(seed)
-    extra = dict(num_uniqs=list(num_uniqs)) if num_uniqs else {}
-    conf.setdefault("noise_lb", 8e-4)
-    gp = GP(d, len(num_uniqs), 1, lr=0.01, num_epochs=epochs, pred_likeli=pred_likeli, **extra, **conf)
-    gp.fit(X, Xe, y)
-    assert not gp._fit_failed
-    _MODELS[key] = (gp, X, Xe, y)
-    return _MODELS[key]
-
-
 def shape_model(n):
     """Numeric Matern-3/2 model, d = 8, with pred_likeli (the default of GP)."""
-    return _fit(("shape", n), n, 8, seed=n)
-
-
-def candidates(gp, X, Xe, m, seed, near=False):
-    """m rows in [-1.2, 1.2]^d (outside the training box in places) with random categories; the first rows are exact
-    training rows (r^2 = 0; none when m = 1) and the last ones duplicate rows 1, 2, 3.  near: training rows moved by 0.01 instead."""
-    g = torch.Generator().manual_seed(seed)
-    Xs = torch.rand(m, gp.d, generator=g) * 2.4 - 1.2
-    Xse = torch.stack([torch.randint(u, (m,), generator=g) for u in gp.num_uniqs], 1) if gp.num_enum else None
-    if near:
-        idx = torch.randint(X.shape[0], (m,), generator=g)
-        Xs = X[idx] + 0.01 * (torch.rand(m, gp.d, generator=g) * 2 - 1)
-        Xse = None if Xe is None else Xe[idx].clone()
-    k = min(5, m // 2, X.shape[0])
-    Xs[:k] = X[:k]
-    if Xse is not None:
-        Xse[:k] = Xe[:k]
-    dups = [(s, m - 4 + j) for j, s in enumerate((1, 2, 3)) if m >= 8]
-    for s, t in dups:
-        Xs[t] = Xs[s]
-        if Xse is not None:
-            Xse[t] = Xse[s]
-    return (Xs.float().to(DEV).contiguous(), None if Xse is None else Xse.to(DEV, torch.int32).contiguous(), dups)
+    return fit_model(("shape", n), n, 8, seed=n)
 
 
 def kernel_inputs(gp, Xs):
@@ -191,27 +140,6 @@ def gp_path(gp, Xs, Xe):
 
 
 # ---------------------------------------------------------------------------------------------------------------- (a) own state
-def _gather(gp, Xe, flat):
-    out, off = [], 0
-    for c, (u, e) in enumerate(zip(gp.num_uniqs, gp.emb_sizes)):
-        out.append(flat[off + Xe[:, c:c + 1].long() * e + torch.arange(e, device=DEV)])
-        off += u * e
-    return torch.cat(out, 1)
-
-
-def _kparts(r2, kind):
-    """k, h (dk/dr^2 = -h / 2), |exponent of fast_exp| and the rate of that exponent in the features."""
-    if kind == "rbf":
-        k = torch.exp(-0.5 * r2)
-        return k, k, 0.5 * r2, r2.clamp_min(0).sqrt()
-    a = RATE[kind]
-    r = r2.clamp_min(1e-30).sqrt()
-    e = torch.exp(-a * r)
-    if kind == "matern32":
-        return (1 + a * r) * e, 3.0 * e, a * r, torch.full_like(r, a)
-    return (1 + a * r + (5.0 / 3.0) * r2) * e, (5.0 / 3.0) * (1 + a * r) * e, a * r, torch.full_like(r, a)
-
-
 def own_state(gp, Xin, Xe, x_mul, x_add, y_std=None, dtype=torch.float64, bounds=True):
     """The closed form of the module docstring on the GP's own fp32 state, in `dtype`, with the bounds B in fp64."""
     dt = dtype
@@ -226,7 +154,7 @@ def own_state(gp, Xin, Xe, x_mul, x_add, y_std=None, dtype=torch.float64, bounds
     Zn = gp.Zt_dev[:d, :n].to(dt).t()
     emb = gp.num_enum > 0
     if emb:
-        zce = _gather(gp, Xe, gp.tab_s_dev.to(dt))
+        zce = gather_emb(gp, Xe, gp.tab_s_dev.to(dt))
         Ze = gp.Zt_dev[d:, :n].to(dt).t()
     L = gp.Linv_dev[:n, :n].to(dt).tril()
     alpha = gp.alpha_dev[:n].to(dt)
@@ -237,13 +165,13 @@ def own_state(gp, Xin, Xe, x_mul, x_add, y_std=None, dtype=torch.float64, bounds
         z = zc[r0:r0 + blk]
         Dz = z[:, None, :] - Zn[None]
         r2 = (Dz * Dz).sum(-1)
-        k, h, t, rate = _kparts(r2, gp.kernel)
+        k, h, t, rate = kernel_parts(r2, gp.kernel)
         zn = z.norm(dim=1)[:, None] + Zn.norm(dim=1)[None]
         grow = 2 + t + rate * zn
         if emb:
             ze = zce[r0:r0 + blk]
             De = ze[:, None, :] - Ze[None]
-            ke, _, te, _ = _kparts((De * De).sum(-1), "matern32")
+            ke, _, te, _ = kernel_parts((De * De).sum(-1), "matern32")
             keh = ke * (2 + te + math.sqrt(3.0) * (ze.norm(dim=1)[:, None] + Ze.norm(dim=1)[None]))
         else:
             ke = keh = torch.ones_like(k)
@@ -302,65 +230,13 @@ def check_own_state(name, gp, Xin, Xe, x_mul, x_add, got, y_std=None):
 
 
 # ---------------------------------------------------------------------------------------------------------------- (b) fp64 GP
-def _features(gp, X, Xe, hyp, tables):
-    parts = []
-    if gp.d:
-        xt = gp._x_mul.double() * X + gp._x_add.double()
-        if gp.warp_mode:
-            d, h = gp.d, gp._h_wa
-            xt = O.kumaraswamy_warp(xt, hyp[h:h + d], hyp[h + d:h + 2 * d])
-        parts.append(xt / hyp[3:3 + gp.d])
-    if gp.num_enum:
-        parts.append(_gather(gp, Xe, tables))
-    return torch.cat(parts, 1)
-
-
-def _kmat(gp, A, B, s):
-    """s k(A, B) in fp64 by direct differences, in row blocks; differentiable."""
-    d = gp.d
-    blk = max(1, (1 << 24) // max(1, B.shape[0] * A.shape[1]))
-    rows = []
-    for i0 in range(0, A.shape[0], blk):
-        a = A[i0:i0 + blk]
-        k = O.kernel_from_sqdist(((a[:, None, :d] - B[None, :, :d]) ** 2).sum(-1), gp.kernel)
-        if gp.num_enum:
-            k = k * O.kernel_from_sqdist(((a[:, None, d:] - B[None, :, d:]) ** 2).sum(-1), "matern32")
-        rows.append(s * k)
-    return torch.cat(rows)
-
-
-_TRUE = {}
-
-
-def true_model(gp, X, Xe, y):
-    """The fp64 GP at the hyper-parameters of `gp`: training features, K + sigma_n^2 I [+ noise_diag], Cholesky, alpha."""
-    key = id(gp)
-    if key in _TRUE and _TRUE[key]["raw"] is gp.raw:
-        return _TRUE[key]
-    hyp = gp.hyp.double().to(DEV)
-    tables = None
-    if gp.num_enum:
-        tables = torch.cat([t.reshape(-1) for t in emb_hypers(gp, gp.raw).tables]).to(DEV) / hyp[3 + gp.d]
-    _, yt64 = scaled_xy(gp, X, y)
-    Zt = _features(gp, X.double().to(DEV), None if Xe is None else Xe.to(DEV), hyp, tables)
-    K = _kmat(gp, Zt, Zt, float(hyp[2]))
-    K.diagonal().add_(float(hyp[0]))
-    if gp.noise_diag is not None:
-        K.diagonal().add_(torch.as_tensor(gp.noise_diag).double().to(DEV))
-    L = torch.linalg.cholesky(K)
-    c = float(hyp[1])
-    alpha = torch.cholesky_solve((yt64.to(DEV) - c).reshape(-1, 1), L).reshape(-1)
-    _TRUE[key] = dict(Zt=Zt, L=L, alpha=alpha, hyp=hyp, tables=tables, c=c, raw=gp.raw)
-    return _TRUE[key]
-
-
 def oracle_grad(gp, tm, Xs, Xe):
     """fp64 (mu, var, raw variance, dmu, dvar) of the candidates in original y units, by autograd."""
     hyp = tm["hyp"]
     s, sn2 = float(hyp[2]), float(hyp[0])
     X = Xs.double().clone().requires_grad_(True)
-    Zc = _features(gp, X, Xe, hyp, tm["tables"])
-    Ks = _kmat(gp, Zc, tm["Zt"], s)
+    Zc = features64(gp, X, Xe, hyp, tm["tables"])
+    Ks = kmat64(gp, Zc, tm["Zt"], s)
     mu_t = tm["c"] + Ks @ tm["alpha"]
     Vt = torch.linalg.solve_triangular(tm["L"], Ks.t(), upper=False)
     raw = s - (Vt * Vt).sum(0) + (sn2 if gp.pred_likeli else 0.0)
@@ -469,30 +345,9 @@ def test_gradients_through_gp_chunks(m):
     torch.cuda.empty_cache()
 
 
-VARIANTS = {
-    "matern32": dict(d=4, pred_likeli=False),
-    "matern32_pl": dict(d=4),
-    "matern52": dict(d=4, kernel="matern52", pred_likeli=False),
-    "matern52_pl": dict(d=4, kernel="matern52"),
-    "rbf": dict(d=4, kernel="rbf", pred_likeli=False),
-    "rbf_pl": dict(d=4, kernel="rbf"),
-    "mixed_e1": dict(d=3, num_uniqs=(4,)),
-    "mixed_e2": dict(d=3, num_uniqs=(3, 5), pred_likeli=False),
-    # De = 6 x 50 = 300.  The wide models are fitted without Langevin noise: with most lengthscale gradients vanishing,
-    # the noise of a short fit random-walks lengthscales towards zero (test_gpu_sample_root.py)
-    "wide_embeddings": dict(d=8, num_uniqs=(120,) * 6, langevin=False),
-    "no_ard": dict(d=4, ard_kernel=False),
-    "no_ard_mixed": dict(d=3, num_uniqs=(3, 5), ard_kernel=False),
-    "hetero": dict(d=4, pred_likeli=False, noise_diag="hetero"),
-    "warp": dict(d=4, warp=True),
-    "warp_mixed": dict(d=3, num_uniqs=(3, 5), warp=True),
-    "fixed_warp": dict(d=4, warp_a="fixed"),
-}
-
-
 def variant_model(name):
     conf = dict(VARIANTS[name])
-    return _fit(("variant", name), 300, seed=7, **conf)
+    return fit_model(("variant", name), 300, seed=7, **conf)
 
 
 @pytest.mark.parametrize("variant", list(VARIANTS))
@@ -506,17 +361,12 @@ def test_gradients_model_variants(variant):
     check_case(variant, gp, X, Xe, y, Xs, Xse, dups)
 
 
-WIDTHS = {1: dict(d=1), 33: dict(d=33), 300: dict(d=300, epochs=3, langevin=False),
-          # d + De = 4096 = HB_MAX_FEATURES, fitted without Langevin noise as the wide embeddings above
-          4096: dict(d=4000, num_uniqs=(5,), emb_sizes=[96], langevin=False, epochs=3)}
-
-
 @pytest.mark.parametrize("width", list(WIDTHS))
 def test_gradients_feature_widths(width):
     """d = 1, 33 (across kstar_kernel's 32-wide feature chunk), 300, and d + De = 4096; from d = 300 on, random rows
     are uncorrelated with the data, so the rows there sit next to training rows."""
     conf = dict(WIDTHS[width])
-    gp, X, Xe, y = _fit(("width", width), 300, seed=11, **conf)
+    gp, X, Xe, y = fit_model(("width", width), 300, seed=11, **conf)
     Xs, Xse, dups = candidates(gp, X, Xe, 64 if width == 4096 else 100, seed=width, near=width >= 300)
     check_case(f"width-{width}", gp, X, Xe, y, Xs, Xse, dups)
     torch.cuda.empty_cache()
@@ -544,7 +394,7 @@ def test_variance_floor_zeroes_dvar():
     """Rows within 1e-6 (raw units) of training rows, at a noise of 1e-9 and short lengthscales: the variance is under
     gpytorch's 1e-6 floor, so var is the floor exactly and dvar is exactly 0, while dmu is still checked.  Random rows of
     the same batch stay live."""
-    gp, X, Xe, y = _fit("floor", 129, 4, pred_likeli=False, epochs=2, noise_lb=1e-9)
+    gp, X, Xe, y = fit_model("floor", 129, 4, pred_likeli=False, epochs=2, noise_lb=1e-9)
     raw = gp.raw.clone()
     raw[0] = -30.0                                               # sigma_n^2 = noise_lb + softplus(-30)
     raw[3:3 + gp.d] = float(O.inv_softplus(torch.tensor(0.05, dtype=torch.float64)))

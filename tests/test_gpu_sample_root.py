@@ -612,3 +612,4 @@ def test_sample_y_rejects_bad_arguments(lib):
     assert call(n_samples=0) == bad
     assert call(hyp_host=None) == bad
     assert call(ws_bytes=need - 1) == bad
+    assert call(ws_bytes=-1) == bad

@@ -41,6 +41,7 @@ def test_sample_y_batch_rejects_bad_arguments(lib):
     for m in (0, -1, 257):
         assert call(m=m, ws_bytes=1 << 40) == bad, m
     assert call(ws_bytes=need - 1) == bad                                  # short workspace
+    assert call(ws_bytes=-1) == bad                                        # negative: not a huge unsigned size
     need256 = int(lib.hb_sample_workspace_bytes(n, d, None, 256))
     assert need256 >= need
     u, e = (ctypes.c_int32 * 1)(3), (ctypes.c_int32 * 1)(2)

@@ -65,6 +65,7 @@ def test_posterior_grad_rejects_bad_arguments(lib):
     need = int(lib.hb_posterior_workspace_bytes(N, D, 128))
     assert need > 0
     assert _call(lib, ws_bytes=need - 1) == bad                            # one byte short
+    assert _call(lib, ws_bytes=-1) == bad                                  # negative: not a huge unsigned size
     p = ctypes.c_void_p(16)
     mixed = _spec(0, num_enum=1)                                           # a categorical column needs Xe / meta / tables
     for Xe, meta, tab in ((None, p, p), (p, None, p), (p, p, None)):
@@ -83,4 +84,5 @@ def test_posterior_grad_null_spec_form_rejects_bad_arguments(lib):
     assert call(d=0, ws_bytes=1 << 40) == bad
     assert call(kern=3) == bad
     assert call(ws_bytes=need - 1) == bad
+    assert call(ws_bytes=-1) == bad
     assert call(dvar=None) == bad

@@ -183,3 +183,170 @@ def fullsize_oracle(c, gp, X, yt, Xs, xi1, xi2, extra, dtype=torch.float64):
     F = O.mace(mu, var, float(f.noise), tau, kappa, 1e-4, xi1, xi2)
     return dict(mu=mu.double().numpy().reshape(-1), var=var.double().numpy().reshape(-1), F=F.double().numpy(), tau=tau,
                 kappa=kappa, noise=float(f.noise), y_std=ys, s=float(f.hp.outputscale))
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# Fitted models, candidate rows and the fp64 posterior pieces shared by the per-element posterior tests
+# (test_gpu_posterior_grad.py, test_gpu_posterior_mace.py).  Models are cached by key for the whole session; a test
+# that changes a model's hypers fits its own key.
+DEV = torch.device("cuda")
+RATE = {"matern32": math.sqrt(3.0), "matern52": math.sqrt(5.0)}
+_MODELS = {}
+
+
+def fit_model(key, n, d, num_uniqs=(), pred_likeli=True, seed=5, epochs=10, **conf):
+    """(gp, X, Xe, y) of a GP fitted to seeded_problem(n, d, seed) (plus category effects); d = 0 is categorical-only
+    (X = None)."""
+    from hebo_b200 import GP
+    if key in _MODELS:
+        return _MODELS[key]
+    X, y = seeded_problem(n, max(d, 1), seed)
+    X = X if d else None
+    g = torch.Generator().manual_seed(seed + 100)
+    Xe = None
+    if num_uniqs:
+        Xe = torch.stack([torch.randint(u, (n,), generator=g) for u in num_uniqs], 1)
+        y = y + 0.4 * Xe[:, :1].float() - 0.2 * Xe[:, -1:].float()
+    if conf.get("noise_diag") == "hetero":
+        conf["noise_diag"] = (1e-2 * (1 + (X.double() ** 2).sum(1) / d)).float()
+    if conf.get("warp_a") == "fixed":
+        conf["warp_a"] = (torch.rand(d, generator=g) * 1.5 + 0.5).tolist()
+        conf["warp_b"] = (torch.rand(d, generator=g) * 1.5 + 0.5).tolist()
+    torch.manual_seed(seed)
+    np.random.seed(seed)
+    extra = dict(num_uniqs=list(num_uniqs)) if num_uniqs else {}
+    conf.setdefault("noise_lb", 8e-4)
+    gp = GP(d, len(num_uniqs), 1, lr=0.01, num_epochs=epochs, pred_likeli=pred_likeli, **extra, **conf)
+    gp.fit(X, Xe, y)
+    assert not gp._fit_failed
+    _MODELS[key] = (gp, X, Xe, y)
+    return _MODELS[key]
+
+
+VARIANTS = {
+    "matern32": dict(d=4, pred_likeli=False),
+    "matern32_pl": dict(d=4),
+    "matern52": dict(d=4, kernel="matern52", pred_likeli=False),
+    "matern52_pl": dict(d=4, kernel="matern52"),
+    "rbf": dict(d=4, kernel="rbf", pred_likeli=False),
+    "rbf_pl": dict(d=4, kernel="rbf"),
+    "mixed_e1": dict(d=3, num_uniqs=(4,)),
+    "mixed_e2": dict(d=3, num_uniqs=(3, 5), pred_likeli=False),
+    # De = 6 x 50 = 300.  The wide models are fitted without Langevin noise: with most lengthscale gradients vanishing,
+    # the noise of a short fit random-walks lengthscales towards zero (test_gpu_sample_root.py)
+    "wide_embeddings": dict(d=8, num_uniqs=(120,) * 6, langevin=False),
+    "no_ard": dict(d=4, ard_kernel=False),
+    "no_ard_mixed": dict(d=3, num_uniqs=(3, 5), ard_kernel=False),
+    "hetero": dict(d=4, pred_likeli=False, noise_diag="hetero"),
+    "warp": dict(d=4, warp=True),
+    "warp_mixed": dict(d=3, num_uniqs=(3, 5), warp=True),
+    "fixed_warp": dict(d=4, warp_a="fixed"),
+}
+
+WIDTHS = {1: dict(d=1), 33: dict(d=33), 300: dict(d=300, epochs=3, langevin=False),
+          # d + De = 4096 = HB_MAX_FEATURES, fitted without Langevin noise as the wide embeddings above
+          4096: dict(d=4000, num_uniqs=(5,), emb_sizes=[96], langevin=False, epochs=3)}
+
+
+def candidates(gp, X, Xe, m, seed, near=False):
+    """m rows in [-1.2, 1.2]^d (outside the training box in places) with random categories; the first rows are exact
+    training rows (r^2 = 0; none when m = 1) and the last ones duplicate rows 1, 2, 3.  near: training rows moved by 0.01
+    instead.  Returns (Xs [m, d] fp32, Xe int32 or None, [(row, its duplicate)]) on the device."""
+    g = torch.Generator().manual_seed(seed)
+    Xs = torch.rand(m, gp.d, generator=g) * 2.4 - 1.2
+    Xse = torch.stack([torch.randint(u, (m,), generator=g) for u in gp.num_uniqs], 1) if gp.num_enum else None
+    n = (X if X is not None else Xe).shape[0]
+    if near:
+        idx = torch.randint(n, (m,), generator=g)
+        Xs = X[idx] + 0.01 * (torch.rand(m, gp.d, generator=g) * 2 - 1)
+        Xse = None if Xe is None else Xe[idx].clone()
+    k = min(5, m // 2, n)
+    if X is not None:
+        Xs[:k] = X[:k]
+    if Xse is not None:
+        Xse[:k] = Xe[:k]
+    dups = [(s, m - 4 + j) for j, s in enumerate((1, 2, 3)) if m >= 8]
+    for s, t in dups:
+        Xs[t] = Xs[s]
+        if Xse is not None:
+            Xse[t] = Xse[s]
+    return (Xs.float().to(DEV).contiguous(), None if Xse is None else Xse.to(DEV, torch.int32).contiguous(), dups)
+
+
+def gather_emb(gp, Xe, flat):
+    """The embedding features of categories Xe [m, e] from the flat tables `flat` (tables / le), [m, De]."""
+    out, off = [], 0
+    for c, (u, e) in enumerate(zip(gp.num_uniqs, gp.emb_sizes)):
+        out.append(flat[off + Xe[:, c:c + 1].long() * e + torch.arange(e, device=flat.device)])
+        off += u * e
+    return torch.cat(out, 1)
+
+
+def kernel_parts(r2, kind):
+    """k, h (dk/dr^2 = -h / 2), |exponent of fast_exp| and the rate of that exponent in the features."""
+    if kind == "rbf":
+        k = torch.exp(-0.5 * r2)
+        return k, k, 0.5 * r2, r2.clamp_min(0).sqrt()
+    a = RATE[kind]
+    r = r2.clamp_min(1e-30).sqrt()
+    e = torch.exp(-a * r)
+    if kind == "matern32":
+        return (1 + a * r) * e, 3.0 * e, a * r, torch.full_like(r, a)
+    return (1 + a * r + (5.0 / 3.0) * r2) * e, (5.0 / 3.0) * (1 + a * r) * e, a * r, torch.full_like(r, a)
+
+
+def features64(gp, X, Xe, hyp, tables):
+    """fp64 features of rows X [m, d] (None when d = 0) / Xe at fp64 hypers: MinMax, [Kumaraswamy warp], 1 / l, then the
+    embedding features."""
+    from oracle import gp_oracle as O
+    parts = []
+    if gp.d:
+        xt = gp._x_mul.double() * X + gp._x_add.double()
+        if gp.warp_mode:
+            d, h = gp.d, gp._h_wa
+            xt = O.kumaraswamy_warp(xt, hyp[h:h + d], hyp[h + d:h + 2 * d])
+        parts.append(xt / hyp[3:3 + gp.d])
+    if gp.num_enum:
+        parts.append(gather_emb(gp, Xe, tables))
+    return torch.cat(parts, 1)
+
+
+def kmat64(gp, A, B, s):
+    """s k(A, B) in fp64 by direct differences, in row blocks; differentiable."""
+    from oracle import gp_oracle as O
+    d = gp.d
+    blk = max(1, (1 << 24) // max(1, B.shape[0] * A.shape[1]))
+    rows = []
+    for i0 in range(0, A.shape[0], blk):
+        a = A[i0:i0 + blk]
+        k = O.kernel_from_sqdist(((a[:, None, :d] - B[None, :, :d]) ** 2).sum(-1), gp.kernel)
+        if gp.num_enum:
+            k = k * O.kernel_from_sqdist(((a[:, None, d:] - B[None, :, d:]) ** 2).sum(-1), "matern32")
+        rows.append(s * k)
+    return torch.cat(rows)
+
+
+_TRUE = {}
+
+
+def true_model(gp, X, Xe, y):
+    """The fp64 GP at the hyper-parameters of `gp`: training features, K + sigma_n^2 I [+ noise_diag], Cholesky, alpha.
+    Rebuilt whenever gp's raw hypers are a new tensor (GP.set_hypers)."""
+    key = id(gp)
+    if key in _TRUE and _TRUE[key]["raw"] is gp.raw:
+        return _TRUE[key]
+    hyp = gp.hyp.double().to(DEV)
+    tables = None
+    if gp.num_enum:
+        tables = torch.cat([t.reshape(-1) for t in emb_hypers(gp, gp.raw).tables]).to(DEV) / hyp[3 + gp.d]
+    yt64 = (y.double().reshape(-1) - float(gp.yscaler.mean[0])) / float(gp.yscaler.std[0])
+    Zt = features64(gp, None if X is None else X.double().to(DEV), None if Xe is None else Xe.to(DEV), hyp, tables)
+    K = kmat64(gp, Zt, Zt, float(hyp[2]))
+    K.diagonal().add_(float(hyp[0]))
+    if gp.noise_diag is not None:
+        K.diagonal().add_(torch.as_tensor(gp.noise_diag).double().to(DEV))
+    L = torch.linalg.cholesky(K)
+    c = float(hyp[1])
+    alpha = torch.cholesky_solve((yt64.to(DEV) - c).reshape(-1, 1), L).reshape(-1)
+    _TRUE[key] = dict(Zt=Zt, L=L, alpha=alpha, hyp=hyp, tables=tables, c=c, raw=gp.raw)
+    return _TRUE[key]
