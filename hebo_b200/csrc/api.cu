@@ -427,7 +427,7 @@ int64_t hb_fit_workspace_bytes_ex(int64_t n, int64_t d, const hb_model_spec_t *s
 int64_t hb_fit_workspace_bytes(int64_t n, int64_t d) { return d <= 0 ? -1 : hb_fit_workspace_bytes_ex(n, d, nullptr); }
 int64_t hb_posterior_workspace_bytes(int64_t n, int64_t d, int64_t m_chunk) {
   if (n <= 0 || d < 0 || m_chunk <= 0) return -1;
-  return (int64_t)posterior_ws_bytes(round_up(n, TILE), d, m_chunk);
+  return (int64_t)carve_posterior_ws(nullptr, round_up(n, TILE), m_chunk).bytes;
 }
 int64_t hb_pareto_workspace_bytes(int64_t m) {
   if (m <= 0) return -1;
@@ -734,6 +734,22 @@ int32_t hb_fit(const float *Xt, const float *y, int64_t n, int64_t d, float *raw
                    ws, ws_bytes, stream);
 }
 
+// The fitted-model arguments that hb_posterior_mace_ex, hb_posterior_grad_ex, hb_sample_y and hb_sample_y_batch share,
+// validated and bound into `gp`; false: the call is invalid.  Xs / Xe_s are the candidates, checked here because which of
+// them a call needs follows from the same spec.
+static bool open_fitted(const float *Xs, const int32_t *Xe_s, int64_t n, int64_t d, const hb_model_spec_t *spec,
+                        const int32_t *emb_meta, const float *tab_s, const float *x_mul, const float *x_add, const float *Zt,
+                        const float *alpha, const float *Linv, const float *hyp, int32_t kern, float y_mean, float y_std,
+                        int32_t pred_likeli, Fitted &gp) {
+  ModelSpec sp;
+  if (!build_spec(d, spec, sp) || n <= 0 || kern < 0 || kern > 2) return false;
+  if ((sp.d > 0 && (!Xs || !x_mul || !x_add)) || !Zt || !alpha || !Linv || !hyp) return false;
+  if (sp.e > 0 && (!Xe_s || !emb_meta || !tab_s)) return false;
+  bind_meta(sp, emb_meta, nullptr);
+  gp = Fitted{sp, n, round_up(n, TILE), kern, Zt, alpha, Linv, hyp, tab_s, x_mul, x_add, y_mean, y_std, pred_likeli};
+  return true;
+}
+
 int32_t hb_posterior_mace_ex(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t rng_offset, int64_t n, int64_t d,
                              const hb_model_spec_t *spec,
                              const int32_t *emb_meta, const float *tab_s, const float *x_mul, const float *x_add,
@@ -741,16 +757,13 @@ int32_t hb_posterior_mace_ex(const float *Xs, const int32_t *Xe_s, int64_t m, in
                              const float *Linv_lo, const float *hyp, int32_t kern, float y_mean, float y_std, int32_t pred_likeli,
                              float tau, float kappa, float eps, const float *xi1, const float *xi2, uint64_t seed, float *F,
                              float *mu, float *var, void *ws, int64_t ws_bytes, int64_t m_chunk, void *stream) {
-  ModelSpec sp;
-  if (!build_spec(d, spec, sp)) return HB_ERR_INVALID;
-  if ((sp.d > 0 && (!Xs || !x_mul || !x_add)) || !Zt || !alpha || !Linv || !hyp || !ws) return HB_ERR_INVALID;
-  if (sp.e > 0 && (!Xe_s || !emb_meta || !tab_s)) return HB_ERR_INVALID;
-  if (!F && !mu && !var) return HB_ERR_INVALID;
+  Fitted gp;
+  if (!open_fitted(Xs, Xe_s, n, d, spec, emb_meta, tab_s, x_mul, x_add, Zt, alpha, Linv, hyp, kern, y_mean, y_std, pred_likeli, gp))
+    return HB_ERR_INVALID;
+  if (!ws || (!F && !mu && !var)) return HB_ERR_INVALID;
   if ((Linv_hi == nullptr) != (Linv_lo == nullptr)) return HB_ERR_INVALID;
-  bind_meta(sp, emb_meta, nullptr);
-  return launch_posterior_mace(Xs, Xe_s, m, rng_offset, n, round_up(n, TILE), sp, tab_s, x_mul, x_add, Zt, alpha, Linv, Linv_hi, Linv_lo, hyp,
-                               kern, y_mean, y_std, pred_likeli, tau, kappa, eps, xi1, xi2, seed, F, mu, var, ws, ws_bytes,
-                               m_chunk, (cudaStream_t)stream);
+  return launch_posterior_mace(gp, Xs, Xe_s, m, rng_offset, Linv_hi, Linv_lo, tau, kappa, eps, xi1, xi2, seed, F, mu, var, ws,
+                               ws_bytes, m_chunk, (cudaStream_t)stream);
 }
 int32_t hb_posterior_mace(const float *Xs, int64_t m, int64_t n, int64_t d, const float *x_mul, const float *x_add,
                           const float *Zt, const float *alpha, const float *Linv, const float *Linv_hi,
@@ -769,14 +782,12 @@ int32_t hb_posterior_grad_ex(const float *Xs, const int32_t *Xe_s, int64_t m, in
                              float y_std, int32_t pred_likeli, float *mu, float *var, float *dmu, float *dvar, void *ws,
                              int64_t ws_bytes, int64_t m_chunk, void *stream) {
   // post_grad_kernel differentiates through x_mul / l only: a warp is the caller's, in front of this call
-  if (spec && spec->warp != 0) return HB_ERR_INVALID;
-  ModelSpec sp;
-  if (d <= 0 || !build_spec(d, spec, sp)) return HB_ERR_INVALID;
-  if (!Xs || !x_mul || !x_add || !Zt || !alpha || !Linv || !hyp || !ws || !mu || !var || !dmu || !dvar) return HB_ERR_INVALID;
-  if (sp.e > 0 && (!Xe_s || !emb_meta || !tab_s)) return HB_ERR_INVALID;
-  bind_meta(sp, emb_meta, nullptr);
-  return launch_posterior_grad(Xs, Xe_s, m, n, round_up(n, TILE), sp, tab_s, x_mul, x_add, Zt, alpha, Linv, hyp, kern, y_mean, y_std,
-                               pred_likeli, mu, var, dmu, dvar, ws, ws_bytes, m_chunk, (cudaStream_t)stream);
+  if ((spec && spec->warp != 0) || d <= 0) return HB_ERR_INVALID;
+  Fitted gp;
+  if (!open_fitted(Xs, Xe_s, n, d, spec, emb_meta, tab_s, x_mul, x_add, Zt, alpha, Linv, hyp, kern, y_mean, y_std, pred_likeli, gp))
+    return HB_ERR_INVALID;
+  if (!ws || !mu || !var || !dmu || !dvar) return HB_ERR_INVALID;
+  return launch_posterior_grad(gp, Xs, Xe_s, m, mu, var, dmu, dvar, ws, ws_bytes, m_chunk, (cudaStream_t)stream);
 }
 int32_t hb_posterior_grad(const float *Xs, int64_t m, int64_t n, int64_t d, const float *x_mul, const float *x_add,
                           const float *Zt, const float *alpha, const float *Linv, const float *hyp, int32_t kern, float y_mean,
@@ -797,13 +808,11 @@ int32_t hb_sample_y(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, 
                     const float *alpha, const float *Linv, const float *hyp, const float *hyp_host, int32_t kern, float y_mean,
                     float y_std, int32_t pred_likeli, const float *z, int32_t n_samples, float *out, float *jitter_used, void *ws,
                     int64_t ws_bytes, void *stream) {
-  ModelSpec sp;
-  if (!build_spec(d, spec, sp)) return HB_ERR_INVALID;
-  if ((sp.d > 0 && (!Xs || !x_mul || !x_add)) || !Zt || !alpha || !Linv || !hyp || !hyp_host || !z || !out || !ws) return HB_ERR_INVALID;
-  if (sp.e > 0 && (!Xe_s || !emb_meta || !tab_s)) return HB_ERR_INVALID;
-  bind_meta(sp, emb_meta, nullptr);
-  return launch_sample_y(Xs, Xe_s, m, n, round_up(n, TILE), sp, tab_s, x_mul, x_add, Zt, alpha, Linv, hyp, hyp_host, kern, y_mean,
-                         y_std, pred_likeli, z, n_samples, out, jitter_used, ws, ws_bytes, (cudaStream_t)stream);
+  Fitted gp;
+  if (!open_fitted(Xs, Xe_s, n, d, spec, emb_meta, tab_s, x_mul, x_add, Zt, alpha, Linv, hyp, kern, y_mean, y_std, pred_likeli, gp))
+    return HB_ERR_INVALID;
+  if (!ws || !hyp_host || !z || !out) return HB_ERR_INVALID;
+  return launch_sample_y(gp, Xs, Xe_s, m, hyp_host, z, n_samples, out, jitter_used, ws, ws_bytes, (cudaStream_t)stream);
 }
 
 int32_t hb_sample_y_batch(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, int64_t d, const hb_model_spec_t *spec,
@@ -811,14 +820,11 @@ int32_t hb_sample_y_batch(const float *Xs, const int32_t *Xe_s, int64_t m, int64
                           const float *alpha, const float *Linv, const float *hyp, int32_t kern, float y_mean, float y_std,
                           int32_t pred_likeli, const float *z, uint64_t seed, uint64_t counter, float *f, float *jitter,
                           int32_t *status, void *ws, int64_t ws_bytes, void *stream) {
-  ModelSpec sp;
-  if (!build_spec(d, spec, sp)) return HB_ERR_INVALID;
-  if ((sp.d > 0 && (!Xs || !x_mul || !x_add)) || !Zt || !alpha || !Linv || !hyp || !f || !jitter || !status || !ws)
+  Fitted gp;
+  if (!open_fitted(Xs, Xe_s, n, d, spec, emb_meta, tab_s, x_mul, x_add, Zt, alpha, Linv, hyp, kern, y_mean, y_std, pred_likeli, gp))
     return HB_ERR_INVALID;
-  if (sp.e > 0 && (!Xe_s || !emb_meta || !tab_s)) return HB_ERR_INVALID;
-  bind_meta(sp, emb_meta, nullptr);
-  return launch_sample_y_batch(Xs, Xe_s, m, n, round_up(n, TILE), sp, tab_s, x_mul, x_add, Zt, alpha, Linv, hyp, kern, y_mean, y_std,
-                               pred_likeli, z, seed, counter, f, jitter, status, ws, ws_bytes, (cudaStream_t)stream);
+  if (!ws || !f || !jitter || !status) return HB_ERR_INVALID;
+  return launch_sample_y_batch(gp, Xs, Xe_s, m, z, seed, counter, f, jitter, status, ws, ws_bytes, (cudaStream_t)stream);
 }
 
 int32_t hb_mace_epilogue(const float *mu, const float *var, int64_t m, float noise_var, float tau, float kappa,

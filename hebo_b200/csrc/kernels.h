@@ -46,6 +46,29 @@ struct ModelSpec {
   __host__ __device__ int dtot() const { return d + De; }
 };
 
+// What candidate scoring reads of a fitted GP (GP.state_tensors() on the Python side), validated and bound once per entry
+// point (open_fitted, api.cu).  The launchers take it whole; kernels keep their __restrict__ pointer lists, unpacked where
+// the <<<...>>> is written.
+struct Fitted {
+  ModelSpec sp;                 // layout arrays bound (bind_meta)
+  int64_t n, np;                // training rows, np = round_up(n, TILE)
+  int kern;
+  const float *Zt, *alpha, *Linv, *hyp, *tab_s, *x_mul, *x_add;
+  float y_mean, y_std;
+  int pred_likeli;
+};
+
+// Consecutive float blocks of a workspace.  With base == nullptr it only counts, which is how a size query runs the same
+// carve as its launcher.
+struct Carver {
+  float *base;
+  int64_t used = 0;
+  float *take(int64_t count) {
+    used += count;
+    return base ? base + used - count : nullptr;
+  }
+};
+
 // ---- output dimension of the fit-loop kernels (DESIGN §3).  A batch of `nout` outputs that share one training set is
 // `nout` consecutive single-output workspaces `ws` bytes apart; output b reads its raw row at raw + b * P and its targets at
 // y + b * n, and shares the training inputs Xt / Xe.  Element-wise and tile kernels take b from blockIdx.z, the persistent
@@ -123,13 +146,20 @@ int launch_median_pdist(const float *Xt, int64_t np, int64_t d, const int32_t *i
                         float *out, cudaStream_t st);
 
 // posterior.cu
-int launch_posterior_mace(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t rng_offset, int64_t n, int64_t np, const ModelSpec &sp,
-                          const float *tab_s, const float *x_mul,
-                          const float *x_add, const float *Zt, const float *alpha, const float *Linv,
-                          const float *Linv_hi, const float *Linv_lo, const float *hyp, int kern, float y_mean, float y_std, int pred_likeli, float tau,
-                          float kappa, float eps, const float *xi1, const float *xi2, uint64_t seed, float *F,
-                          float *mu, float *var, void *ws, int64_t ws_bytes, int64_t m_chunk, cudaStream_t st);
-size_t posterior_ws_bytes(int64_t np, int64_t d, int64_t m_chunk);
+int launch_posterior_mace(const Fitted &gp, const float *Xs, const int32_t *Xe_s, int64_t m, int64_t rng_offset,
+                          const float *Linv_hi, const float *Linv_lo, float tau, float kappa, float eps, const float *xi1,
+                          const float *xi2, uint64_t seed, float *F, float *mu, float *var, void *ws, int64_t ws_bytes,
+                          int64_t m_chunk, cudaStream_t st);
+// The posterior workspace of one chunk of at most m_chunk candidates, rows padded to mc_pad = round_up(m_chunk, CHUNK_ROWS).
+// KS: fp32 K* rows (SIMT and guard passes); KS2: the fp16 two-level split h0 | h1 of the tensor path, or the V panel of the
+// gradient path, which then overwrites KS with W; mupart [groups, mc_pad]; vpart / vfix [np / GT, mc_pad]; the guard lists.
+struct PostWs {
+  float *KS, *KS2, *mupart, *vpart, *vfix;
+  int32_t *fixmap, *fixlist, *fixcount;
+  int64_t mc_pad;
+  size_t bytes;
+};
+PostWs carve_posterior_ws(void *ws, int64_t np, int64_t m_chunk);   // ws == nullptr: only .bytes, the size query
 int guard_stats(unsigned long long *out, int reset);
 int launch_mace_only(const float *mu, const float *var, int64_t m, float noise_var, float tau, float kappa, float eps,
                      const float *xi1, const float *xi2, uint64_t seed, float *F, cudaStream_t st);
@@ -139,17 +169,12 @@ int launch_general_acq(const float *mu, const float *var, int64_t m, int64_t num
                        float c_kappa, const float *noise_sd, const float *xi, uint64_t seed, uint64_t counter, float *Fo,
                        float *Fc, float *cv, cudaStream_t st);
 int kstar_groups(int64_t np);
-int launch_kstar(const float *xs, const int32_t *xe, int64_t mc, const ModelSpec &sp, const float *tab_s, const float *x_mul,
-                 const float *x_add, const float *Zt, const float *alpha, const float *hyp, int64_t n, int64_t np, int kern,
-                 float *KS, float *KS_h16, float *mupart, int64_t mc_pad, const int32_t *fixlist, const int32_t *fixcount,
-                 cudaStream_t st);
+int launch_kstar(const Fitted &gp, const float *xs, const int32_t *xe, int64_t mc, float *KS, float *KS_h16, float *mupart,
+                 int64_t mc_pad, const int32_t *fixlist, const int32_t *fixcount, cudaStream_t st);
 
 // posterior_grad.cu
-int launch_posterior_grad(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, int64_t np, const ModelSpec &sp,
-                          const float *tab_s, const float *x_mul, const float *x_add,
-                          const float *Zt, const float *alpha, const float *Linv, const float *hyp, int kern, float y_mean,
-                          float y_std, int pred_likeli, float *mu, float *var, float *dmu, float *dvar, void *ws,
-                          int64_t ws_bytes, int64_t m_chunk, cudaStream_t st);
+int launch_posterior_grad(const Fitted &gp, const float *Xs, const int32_t *Xe_s, int64_t m, float *mu, float *var, float *dmu,
+                          float *dvar, void *ws, int64_t ws_bytes, int64_t m_chunk, cudaStream_t st);
 
 // fp16 two-level split tensor path of the posterior (vnorm_h16.cu: wgmma / TMA / mbarrier)
 int launch_split_h16(const float *x, int64_t count, __half *h0, __half *h1, float *scale_slot, cudaStream_t st);
@@ -168,15 +193,11 @@ int launch_front_merge(const float *all, int64_t world, int64_t capacity, float 
                        cudaStream_t st);
 
 size_t sample_ws_bytes(int64_t np, int64_t dtot, int64_t m);
-int launch_sample_y(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, int64_t np, const ModelSpec &sp, const float *tab_s,
-                    const float *x_mul, const float *x_add, const float *Zt, const float *alpha, const float *Linv, const float *hyp,
-                    const float *hyp_host, int kern, float y_mean, float y_std, int pred_likeli, const float *z, int n_samples,
-                    float *out, float *jitter_used, void *ws, int64_t ws_bytes, cudaStream_t st);
+int launch_sample_y(const Fitted &gp, const float *Xs, const int32_t *Xe_s, int64_t m, const float *hyp_host, const float *z,
+                    int n_samples, float *out, float *jitter_used, void *ws, int64_t ws_bytes, cudaStream_t st);
 // one joint draw f [m] over m <= 256 rows, duplicates dropped, jitter ladder on the device (hb_sample_y_batch)
-int launch_sample_y_batch(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, int64_t np, const ModelSpec &sp,
-                          const float *tab_s, const float *x_mul, const float *x_add, const float *Zt, const float *alpha,
-                          const float *Linv, const float *hyp, int kern, float y_mean, float y_std, int pred_likeli, const float *z,
-                          uint64_t seed, uint64_t counter, float *f, float *jitter_out, int32_t *status, void *ws, int64_t ws_bytes,
+int launch_sample_y_batch(const Fitted &gp, const float *Xs, const int32_t *Xe_s, int64_t m, const float *z, uint64_t seed,
+                          uint64_t counter, float *f, float *jitter_out, int32_t *status, void *ws, int64_t ws_bytes,
                           cudaStream_t st);
 // nsga.cu
 int launch_nsga_init(float *X, int64_t P, int64_t D, int64_t d, const int32_t *kind, const float *lb, const float *ub,

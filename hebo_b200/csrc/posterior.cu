@@ -436,94 +436,89 @@ int kstar_groups(int64_t np) { return (int)ceil_div(np, KS_GROUP); }
 //   fixlist != nullptr: the guard pass: KS row `slot` is the exact fp32 row of candidate fixlist[slot], slot < *fixcount
 //                       (mupart nullptr);
 //   otherwise:          fp32 rows into KS, mean partials into mupart.
-int launch_kstar(const float *xs, const int32_t *xe, int64_t mc, const ModelSpec &sp, const float *tab_s, const float *x_mul,
-                 const float *x_add, const float *Zt, const float *alpha, const float *hyp, int64_t n, int64_t np, int kern,
-                 float *KS, float *KS_h16, float *mupart, int64_t mc_pad, const int32_t *fixlist, const int32_t *fixcount,
-                 cudaStream_t st) {
-  const dim3 grid((unsigned)ceil_div(mc, KS_ROWS), (unsigned)kstar_groups(np));
-  const int s = with_kernel(kern, sp.e > 0, [&](auto kk, auto ee) {
+int launch_kstar(const Fitted &gp, const float *xs, const int32_t *xe, int64_t mc, float *KS, float *KS_h16, float *mupart,
+                 int64_t mc_pad, const int32_t *fixlist, const int32_t *fixcount, cudaStream_t st) {
+  const ModelSpec &sp = gp.sp;
+  const dim3 grid((unsigned)ceil_div(mc, KS_ROWS), (unsigned)kstar_groups(gp.np));
+  const int s = with_kernel(gp.kern, sp.e > 0, [&](auto kk, auto ee) {
     constexpr int KERN = decltype(kk)::value;
     constexpr bool EMB = decltype(ee)::value;
     if (KS_h16)
-      kstar_kernel<KERN, 2, EMB><<<grid, 256, 0, st>>>(xs, mc, sp.d, x_mul, x_add, Zt, alpha, hyp, n, np, KS, KS_h16, mupart,
-                                                         mc_pad, fixlist, fixcount, xe, tab_s, sp);
+      kstar_kernel<KERN, 2, EMB><<<grid, 256, 0, st>>>(xs, mc, sp.d, gp.x_mul, gp.x_add, gp.Zt, gp.alpha, gp.hyp, gp.n, gp.np, KS,
+                                                         KS_h16, mupart, mc_pad, fixlist, fixcount, xe, gp.tab_s, sp);
     else
-      kstar_kernel<KERN, 0, EMB><<<grid, 256, 0, st>>>(xs, mc, sp.d, x_mul, x_add, Zt, alpha, hyp, n, np, KS, KS_h16, mupart,
-                                                         mc_pad, fixlist, fixcount, xe, tab_s, sp);
+      kstar_kernel<KERN, 0, EMB><<<grid, 256, 0, st>>>(xs, mc, sp.d, gp.x_mul, gp.x_add, gp.Zt, gp.alpha, gp.hyp, gp.n, gp.np, KS,
+                                                         KS_h16, mupart, mc_pad, fixlist, fixcount, xe, gp.tab_s, sp);
   });
   if (s != HB_OK) return s;
   count_launches(1);
   return HB_OK;
 }
 
-size_t posterior_ws_bytes(int64_t np, int64_t d, int64_t m_chunk) {
-  const int64_t mc_pad = round_up(m_chunk, CHUNK_ROWS);
-  const int64_t ncg = ceil_div(np, KS_GROUP);
+PostWs carve_posterior_ws(void *ws, int64_t np, int64_t m_chunk) {
+  PostWs w;
+  w.mc_pad = round_up(m_chunk, CHUNK_ROWS);
   const int64_t nt = np / GT;
-  return (size_t)(2 * mc_pad * np + ncg * mc_pad + 2 * nt * mc_pad + 2 * mc_pad) * sizeof(float) + 512;
+  Carver c{reinterpret_cast<float *>(ws)};
+  w.KS = c.take(w.mc_pad * np);
+  w.KS2 = c.take(w.mc_pad * np);
+  w.mupart = c.take(kstar_groups(np) * w.mc_pad);
+  w.vpart = c.take(nt * w.mc_pad);
+  w.vfix = c.take(nt * w.mc_pad);
+  w.fixmap = reinterpret_cast<int32_t *>(c.take(w.mc_pad));
+  w.fixlist = reinterpret_cast<int32_t *>(c.take(w.mc_pad));
+  w.fixcount = reinterpret_cast<int32_t *>(c.take(0));   // one word of the 512-byte tail
+  w.bytes = (size_t)c.used * sizeof(float) + 512;
+  return w;
 }
 
-int launch_posterior_mace(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t rng_offset, int64_t n, int64_t np, const ModelSpec &sp,
-                          const float *tab_s, const float *x_mul,
-                          const float *x_add, const float *Zt, const float *alpha, const float *Linv,
-                          const float *Linv_hi, const float *Linv_lo, const float *hyp, int kern, float y_mean, float y_std, int pred_likeli, float tau,
-                          float kappa, float eps, const float *xi1, const float *xi2, uint64_t seed, float *F,
-                          float *mu, float *var, void *ws, int64_t ws_bytes, int64_t m_chunk, cudaStream_t st) {
-  const int64_t d = sp.d;
-  if (m <= 0 || n <= 0 || sp.dtot() <= 0 || np % GT != 0 || n > np || m_chunk <= 0) return HB_ERR_INVALID;
-  if (kern < 0 || kern > 2 || (sp.e > 0 && (!Xe_s || !tab_s))) return HB_ERR_INVALID;
-  if (ws_bytes < 0 || (size_t)ws_bytes < posterior_ws_bytes(np, d, m_chunk)) return HB_ERR_INVALID;
-  const int64_t mc_pad_max = round_up(m_chunk, CHUNK_ROWS);
-  const int ncg = (int)ceil_div(np, KS_GROUP);
+int launch_posterior_mace(const Fitted &gp, const float *Xs, const int32_t *Xe_s, int64_t m, int64_t rng_offset,
+                          const float *Linv_hi, const float *Linv_lo, float tau, float kappa, float eps, const float *xi1,
+                          const float *xi2, uint64_t seed, float *F, float *mu, float *var, void *ws, int64_t ws_bytes,
+                          int64_t m_chunk, cudaStream_t st) {
+  const ModelSpec &sp = gp.sp;
+  const int64_t np = gp.np;
+  if (m <= 0 || m_chunk <= 0) return HB_ERR_INVALID;
+  const PostWs w = carve_posterior_ws(ws, np, m_chunk);
+  if (ws_bytes < 0 || (size_t)ws_bytes < w.bytes) return HB_ERR_INVALID;
   const int nt = (int)(np / GT);
   const bool tensor = Linv_hi != nullptr && Linv_lo != nullptr;   // wgmma path (two-level fp16 split), else FP32 SIMT
-  // workspace: the K* chunk (KS: fp32 rows of the SIMT / guard passes; KS2: the fp16 two-level split h0 | h1 of the
-  // tensor path), the mean partials and the per-chunk partial-sum buffers.  (Building chunk i+1 on a side stream under
-  // the tensor-core contraction of chunk i was measured and dropped: the contraction then drew ~all of the L2 -> SM
-  // bandwidth, the co-running CUDA-core kernel slowed it by 30 %.  Since the Linv multicast it draws 5/8 of those bytes
-  // per k-block; the overlap has not been measured again.)
-  float *KS = reinterpret_cast<float *>(ws);
-  float *KS2 = KS + mc_pad_max * np;
-  float *mupart = KS2 + mc_pad_max * np;
-  float *vpart = mupart + (int64_t)ncg * mc_pad_max;
-  float *vfix = vpart + (int64_t)nt * mc_pad_max;
-  int32_t *fixmap = reinterpret_cast<int32_t *>(vfix + (int64_t)nt * mc_pad_max);
-  int32_t *fixlist = fixmap + mc_pad_max;
-  int32_t *fixcount = fixlist + mc_pad_max;
+  // (Building chunk i+1 on a side stream under the tensor-core contraction of chunk i was measured and dropped: the
+  // contraction then drew ~all of the L2 -> SM bandwidth, the co-running CUDA-core kernel slowed it by 30 %.  Since the
+  // Linv multicast it draws 5/8 of those bytes per k-block; the overlap has not been measured again.)
   for (int64_t c0 = 0; c0 < m; c0 += m_chunk) {
     const int64_t mc = min(m_chunk, m - c0);
     const int64_t mc_pad = round_up(mc, GT);
-    const float *xs = Xs + c0 * d;
+    const float *xs = Xs + c0 * sp.d;
     const int32_t *xe = sp.e > 0 ? Xe_s + c0 * sp.e : nullptr;
-    int s = launch_kstar(xs, xe, mc, sp, tab_s, x_mul, x_add, Zt, alpha, hyp, n, np, kern, KS, tensor ? KS2 : nullptr, mupart,
-                         mc_pad_max, nullptr, nullptr, st);
+    int s = launch_kstar(gp, xs, xe, mc, w.KS, tensor ? w.KS2 : nullptr, w.mupart, w.mc_pad, nullptr, nullptr, st);
     if (s != HB_OK) return s;
     int nslots = nt;
     if (tensor) {
-      const __half *kh0 = reinterpret_cast<const __half *>(KS2), *kh1 = kh0 + mc_pad_max * np;
-      s = launch_vnorm_h16(kh0, kh1, mc_pad_max, reinterpret_cast<const __half *>(Linv_hi),
-                           reinterpret_cast<const __half *>(Linv_lo), Linv_lo + np * np / 2, hyp, np, mc_pad, mc_pad_max, vpart, st);
+      const __half *kh0 = reinterpret_cast<const __half *>(w.KS2), *kh1 = kh0 + w.mc_pad * np;
+      s = launch_vnorm_h16(kh0, kh1, w.mc_pad, reinterpret_cast<const __half *>(Linv_hi),
+                           reinterpret_cast<const __half *>(Linv_lo), Linv_lo + np * np / 2, gp.hyp, np, mc_pad, w.mc_pad, w.vpart, st);
       if (s != HB_OK) return s;
       nslots = (int)ceil_div(np, 128);
-      HB_CUDA(cudaMemsetAsync(fixcount, 0, sizeof(int32_t), st));
-      guard_kernel<<<(int)ceil_div(mc, 256), 256, 0, st>>>(vpart, nslots, mc, mc_pad_max, hyp, GUARD_THETA, fixmap, fixlist, fixcount);
+      HB_CUDA(cudaMemsetAsync(w.fixcount, 0, sizeof(int32_t), st));
+      guard_kernel<<<(int)ceil_div(mc, 256), 256, 0, st>>>(w.vpart, nslots, mc, w.mc_pad, gp.hyp, GUARD_THETA, w.fixmap, w.fixlist,
+                                                           w.fixcount);
       // exact fp32 K* rows of the flagged candidates only (compact, row = slot), then their FP32 contraction
-      s = launch_kstar(xs, xe, mc, sp, tab_s, x_mul, x_add, Zt, alpha, hyp, n, np, kern, KS, nullptr, nullptr, mc_pad_max, fixlist,
-                       fixcount, st);
+      s = launch_kstar(gp, xs, xe, mc, w.KS, nullptr, nullptr, w.mc_pad, w.fixlist, w.fixcount, st);
       if (s != HB_OK) return s;
       const dim3 gf((unsigned)nt, (unsigned)(mc_pad / GT));
-      vnorm_fix_kernel<<<gf, GTHREADS, 0, st>>>(KS, nullptr, Linv, np, mc_pad_max, fixlist, fixcount, vfix, 1);
+      vnorm_fix_kernel<<<gf, GTHREADS, 0, st>>>(w.KS, nullptr, gp.Linv, np, w.mc_pad, w.fixlist, w.fixcount, w.vfix, 1);
       count_launches(3);
     } else {
       const dim3 g2((unsigned)nt, (unsigned)(mc_pad / GT));
       prof_begin(st);
-      vnorm_kernel<<<g2, GTHREADS, 0, st>>>(KS, Linv, np, mc_pad_max, vpart);
+      vnorm_kernel<<<g2, GTHREADS, 0, st>>>(w.KS, gp.Linv, np, w.mc_pad, w.vpart);
       prof_end(st);
       count_launches(2);
     }
-    mace_kernel<<<(int)ceil_div(mc, 256), 256, 0, st>>>(mupart, ncg, vpart, nslots, tensor ? fixmap : nullptr, vfix, nt, mc,
-                                                        mc_pad_max, c0, rng_offset, hyp, y_mean, y_std,
-                                                        pred_likeli, tau, kappa, eps, xi1, xi2, seed, F, mu, var);
+    mace_kernel<<<(int)ceil_div(mc, 256), 256, 0, st>>>(w.mupart, kstar_groups(np), w.vpart, nslots, tensor ? w.fixmap : nullptr,
+                                                        w.vfix, nt, mc, w.mc_pad, c0, rng_offset, gp.hyp, gp.y_mean, gp.y_std,
+                                                        gp.pred_likeli, tau, kappa, eps, xi1, xi2, seed, F, mu, var);
   }
   HB_LAUNCH_CHECK("posterior_mace");
   return HB_OK;

@@ -145,37 +145,28 @@ __global__ void __launch_bounds__(256) post_grad_kernel(const float *__restrict_
   }
 }
 
-int launch_posterior_grad(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, int64_t np, const ModelSpec &sp,
-                          const float *tab_s, const float *x_mul, const float *x_add,
-                          const float *Zt, const float *alpha, const float *Linv, const float *hyp, int kern, float y_mean,
-                          float y_std, int pred_likeli, float *mu, float *var, float *dmu, float *dvar, void *ws,
-                          int64_t ws_bytes, int64_t m_chunk, cudaStream_t st) {
-  const int64_t d = sp.d;
-  if (m <= 0 || n <= 0 || d <= 0 || np % GT != 0 || n > np || m_chunk <= 0) return HB_ERR_INVALID;
-  if (sp.e > 0 && (!Xe_s || !tab_s)) return HB_ERR_INVALID;
-  if (kern < 0 || kern > 2 || !mu || !var || !dmu || !dvar) return HB_ERR_INVALID;
-  if (ws_bytes < 0 || (size_t)ws_bytes < posterior_ws_bytes(np, d, m_chunk)) return HB_ERR_INVALID;
-  const int64_t mc_pad_max = round_up(m_chunk, 2 * GT);
-  const int ncg = kstar_groups(np);
-  const int nt = (int)(np / GT);
-  // workspace layout of posterior.cu: [K* | second panel | mean partials] -- K* is later overwritten by W
-  float *KS = reinterpret_cast<float *>(ws);
-  float *Vb = KS + mc_pad_max * np;
-  float *mupart = Vb + mc_pad_max * np;
+int launch_posterior_grad(const Fitted &gp, const float *Xs, const int32_t *Xe_s, int64_t m, float *mu, float *var, float *dmu,
+                          float *dvar, void *ws, int64_t ws_bytes, int64_t m_chunk, cudaStream_t st) {
+  const ModelSpec &sp = gp.sp;
+  const int64_t d = sp.d, np = gp.np;
+  if (m <= 0 || m_chunk <= 0) return HB_ERR_INVALID;
+  const PostWs w = carve_posterior_ws(ws, np, m_chunk);
+  if (ws_bytes < 0 || (size_t)ws_bytes < w.bytes) return HB_ERR_INVALID;
+  float *V = w.KS2, *W = w.KS;   // W overwrites K* once V is built
   const size_t dyn = (2 * (size_t)d + sp.De) * sizeof(float);
   for (int64_t c0 = 0; c0 < m; c0 += m_chunk) {
     const int64_t mc = min(m_chunk, m - c0);
     const int64_t mc_pad = round_up(mc, GT);
-    int s = launch_kstar(Xs + c0 * d, sp.e > 0 ? Xe_s + c0 * sp.e : nullptr, mc, sp, tab_s, x_mul, x_add, Zt, alpha, hyp, n, np,
-                         kern, KS, nullptr, mupart, mc_pad_max, nullptr, nullptr, st);
+    int s = launch_kstar(gp, Xs + c0 * d, sp.e > 0 ? Xe_s + c0 * sp.e : nullptr, mc, w.KS, nullptr, w.mupart, w.mc_pad, nullptr,
+                         nullptr, st);
     if (s != HB_OK) return s;
-    const dim3 g((unsigned)nt, (unsigned)(mc_pad / GT));
-    rows_gemm_kernel<0><<<g, GTHREADS, 0, st>>>(KS, Linv, np, Vb);
-    rows_gemm_kernel<1><<<g, GTHREADS, 0, st>>>(Vb, Linv, np, KS);
-    s = with_kernel(kern, sp.e > 0, [&](auto kk, auto ee) {
+    const dim3 g((unsigned)(np / GT), (unsigned)(mc_pad / GT));
+    rows_gemm_kernel<0><<<g, GTHREADS, 0, st>>>(w.KS, gp.Linv, np, V);
+    rows_gemm_kernel<1><<<g, GTHREADS, 0, st>>>(V, gp.Linv, np, W);
+    s = with_kernel(gp.kern, sp.e > 0, [&](auto kk, auto ee) {
       post_grad_kernel<decltype(kk)::value, decltype(ee)::value><<<(unsigned)mc, 256, dyn, st>>>(
-          Xs, (int)d, x_mul, x_add, Zt, alpha, hyp, n, np, Vb, KS, mupart, ncg, mc_pad_max, c0, y_mean, y_std, pred_likeli, mu,
-          var, dmu, dvar, Xe_s, tab_s, sp);
+          Xs, (int)d, gp.x_mul, gp.x_add, gp.Zt, gp.alpha, gp.hyp, gp.n, np, V, W, w.mupart, kstar_groups(np), w.mc_pad, c0,
+          gp.y_mean, gp.y_std, gp.pred_likeli, mu, var, dmu, dvar, Xe_s, gp.tab_s, sp);
     });
     if (s != HB_OK) return s;
     count_launches(3);
@@ -259,56 +250,84 @@ __global__ void __launch_bounds__(256) sample_apply_kernel(const float *__restri
   }
 }
 
-size_t sample_ws_bytes(int64_t np, int64_t dtot, int64_t m) {
-  const int64_t mp = round_up(m, 2 * GT);
-  return (size_t)(2 * mp * np + kstar_groups(np) * mp + mp * mp + dtot * mp + GT * GT) * sizeof(float) + 1024;
+// The sampler workspace over mp padded candidate rows: K*, V [mp, np], the mean partials, cov [mp, mp], the transposed
+// candidate features, and the scratch tile and status word of launch_cholesky.
+struct SampleWs {
+  float *KS, *Vb, *mupart, *cov, *ZsT, *cholws;
+  int32_t *info;
+  int64_t mp;
+  size_t bytes;
+};
+static SampleWs carve_sample_ws(void *ws, int64_t np, int64_t dtot, int64_t mp) {
+  SampleWs w;
+  w.mp = mp;
+  Carver c{reinterpret_cast<float *>(ws)};
+  w.KS = c.take(mp * np);
+  w.Vb = c.take(mp * np);
+  w.mupart = c.take(kstar_groups(np) * mp);
+  w.cov = c.take(mp * mp);
+  w.ZsT = c.take(dtot * mp);
+  w.cholws = c.take(GT * GT);
+  w.info = reinterpret_cast<int32_t *>(c.take(0));   // one word of the 1024-byte tail
+  w.bytes = (size_t)c.used * sizeof(float) + 1024;
+  return w;
 }
 
-int launch_sample_y(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, int64_t np, const ModelSpec &sp, const float *tab_s,
-                    const float *x_mul, const float *x_add, const float *Zt, const float *alpha, const float *Linv, const float *hyp,
-                    const float *hyp_host, int kern, float y_mean, float y_std, int pred_likeli, const float *z, int n_samples,
-                    float *out, float *jitter_used, void *ws, int64_t ws_bytes, cudaStream_t st) {
-  if (m <= 0 || m > 8192 || n <= 0 || np % GT != 0 || n_samples <= 0 || kern < 0 || kern > 2 || !hyp_host) return HB_ERR_INVALID;
-  if (ws_bytes < 0 || (size_t)ws_bytes < sample_ws_bytes(np, sp.dtot(), m)) return HB_ERR_INVALID;
-  const int64_t mp = round_up(m, 2 * GT);
-  const int ncg = kstar_groups(np);
-  float *KS = reinterpret_cast<float *>(ws);
-  float *Vb = KS + mp * np;
-  float *mupart = Vb + mp * np;
-  float *cov = mupart + (int64_t)ncg * mp;
-  float *ZsT = cov + mp * mp;
-  float *cholws = ZsT + (int64_t)sp.dtot() * mp;
-  int32_t *info = reinterpret_cast<int32_t *>(cholws + GT * GT);
-  HB_CUDA(cudaMemsetAsync(KS, 0, (size_t)mp * np * sizeof(float), st));     // rows m..mp of K* must be zero for the GEMMs
-  int s = launch_kstar(Xs, Xe_s, m, sp, tab_s, x_mul, x_add, Zt, alpha, hyp, n, np, kern, KS, nullptr, mupart, mp, nullptr, nullptr, st);
+// both samplers share this size: launch_sample_y pads m to 2 GT, launch_sample_y_batch to GT
+size_t sample_ws_bytes(int64_t np, int64_t dtot, int64_t m) { return carve_sample_ws(nullptr, np, dtot, round_up(m, 2 * GT)).bytes; }
+
+// K* (+ mean partials), V = K* Linv^T and the candidates' own features of m rows padded to w.mp
+static int enqueue_sample_panels(const Fitted &gp, const float *Xs, const int32_t *Xe_s, int64_t m, const SampleWs &w, cudaStream_t st) {
+  const int64_t np = gp.np, mp = w.mp;
+  HB_CUDA(cudaMemsetAsync(w.KS, 0, (size_t)mp * np * sizeof(float), st));     // rows m..mp of K* must be zero for the GEMMs
+  const int s = launch_kstar(gp, Xs, Xe_s, m, w.KS, nullptr, w.mupart, mp, nullptr, nullptr, st);
   if (s != HB_OK) return s;
-  const dim3 g((unsigned)(np / GT), (unsigned)(mp / GT));
-  rows_gemm_kernel<0><<<g, GTHREADS, 0, st>>>(KS, Linv, np, Vb);
-  cand_features_kernel<<<(int)ceil_div((int64_t)sp.dtot() * mp, 256), 256, 0, st>>>(Xs, Xe_s, m, mp, x_mul, x_add, hyp, tab_s, sp, ZsT);
+  rows_gemm_kernel<0><<<dim3((unsigned)(np / GT), (unsigned)(mp / GT)), GTHREADS, 0, st>>>(w.KS, gp.Linv, np, w.Vb);
+  cand_features_kernel<<<(int)ceil_div((int64_t)gp.sp.dtot() * mp, 256), 256, 0, st>>>(Xs, Xe_s, m, mp, gp.x_mul, gp.x_add, gp.hyp,
+                                                                                      gp.tab_s, gp.sp, w.ZsT);
   count_launches(2);
-  ModelSpec sc = sp;
+  return HB_OK;
+}
+
+// cov = K** - V V^T over the lower tiles, diagonal diag_base - |v_i|^2
+static int enqueue_sample_cov(const Fitted &gp, int64_t m, const SampleWs &w, float diag_base, cudaStream_t st) {
+  const int64_t mp = w.mp;
+  ModelSpec sc = gp.sp;
   sc.warp = 1;                        // "prescaled features" switch of gram_kernel: ZsT is already warped and divided by l
-  const float sn2 = hyp_host[0], sv = hyp_host[2];
+  const int s = launch_gram(w.ZsT, w.ZsT + (int64_t)sc.d * mp, m, mp, sc, gp.hyp, gp.kern, nullptr, 0.0f, w.cov, st);
+  if (s != HB_OK) return s;
   const int nt = (int)(mp / GT);
+  cov_update_kernel<<<nt * (nt + 1) / 2, GTHREADS, 0, st>>>(w.cov, mp, m, w.Vb, gp.np, diag_base);
+  count_launches(1);
+  return HB_OK;
+}
+
+int launch_sample_y(const Fitted &gp, const float *Xs, const int32_t *Xe_s, int64_t m, const float *hyp_host, const float *z,
+                    int n_samples, float *out, float *jitter_used, void *ws, int64_t ws_bytes, cudaStream_t st) {
+  if (m <= 0 || m > 8192 || n_samples <= 0) return HB_ERR_INVALID;
+  if (ws_bytes < 0 || (size_t)ws_bytes < sample_ws_bytes(gp.np, gp.sp.dtot(), m)) return HB_ERR_INVALID;
+  const SampleWs w = carve_sample_ws(ws, gp.np, gp.sp.dtot(), round_up(m, 2 * GT));
+  int s = enqueue_sample_panels(gp, Xs, Xe_s, m, w, st);
+  if (s != HB_OK) return s;
+  const float sn2 = hyp_host[0], sv = hyp_host[2];
   float jitter = 1e-6f;               // gpytorch psd_safe_cholesky: fp32 jitter 1e-6, x10 per retry
   for (;;) {
-    s = launch_gram(ZsT, ZsT + (int64_t)sp.d * mp, m, mp, sc, hyp, kern, nullptr, 0.0f, cov, st);
+    s = enqueue_sample_cov(gp, m, w, sv + (gp.pred_likeli ? sn2 : 0.0f) + jitter, st);
     if (s != HB_OK) return s;
-    cov_update_kernel<<<nt * (nt + 1) / 2, GTHREADS, 0, st>>>(cov, mp, m, Vb, np, sv + (pred_likeli ? sn2 : 0.0f) + jitter);
-    count_launches(1);
-    HB_CUDA(cudaMemsetAsync(info, 0, sizeof(int32_t), st));
-    s = launch_cholesky(cov, mp, cholws, info, st);
+    HB_CUDA(cudaMemsetAsync(w.info, 0, sizeof(int32_t), st));
+    s = launch_cholesky(w.cov, w.mp, w.cholws, w.info, st);
     if (s != HB_OK) return s;
     int32_t h = 0;
-    HB_CUDA(cudaMemcpyAsync(&h, info, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    HB_CUDA(cudaMemcpyAsync(&h, w.info, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     HB_CUDA(cudaStreamSynchronize(st));
     if (h == 0) break;
     jitter *= 10.0f;
     if (jitter > 10.0f) return HB_ERR_NOT_PD;
   }
   if (jitter_used) *jitter_used = jitter;
-  sample_apply_kernel<<<(int)ceil_div((int64_t)n_samples * m * 32, 256), 256, 0, st>>>(cov, mp, m, z, n_samples, mupart, ncg, mp, hyp,
-                                                                                     y_mean, y_std, out);
+  sample_apply_kernel<<<(int)ceil_div((int64_t)n_samples * m * 32, 256), 256, 0, st>>>(w.cov, w.mp, m, z, n_samples, w.mupart,
+                                                                                     kstar_groups(gp.np), w.mp, gp.hyp, gp.y_mean,
+                                                                                     gp.y_std, out);
   count_launches(1);
   HB_LAUNCH_CHECK("sample_y");
   return HB_OK;
@@ -434,13 +453,11 @@ __global__ void __launch_bounds__(SB_THREADS, 1) sample_batch_kernel(
   }
 }
 
-int launch_sample_y_batch(const float *Xs, const int32_t *Xe_s, int64_t m, int64_t n, int64_t np, const ModelSpec &sp,
-                          const float *tab_s, const float *x_mul, const float *x_add, const float *Zt, const float *alpha,
-                          const float *Linv, const float *hyp, int kern, float y_mean, float y_std, int pred_likeli, const float *z,
-                          uint64_t seed, uint64_t counter, float *f, float *jitter_out, int32_t *status, void *ws, int64_t ws_bytes,
+int launch_sample_y_batch(const Fitted &gp, const float *Xs, const int32_t *Xe_s, int64_t m, const float *z, uint64_t seed,
+                          uint64_t counter, float *f, float *jitter_out, int32_t *status, void *ws, int64_t ws_bytes,
                           cudaStream_t st) {
-  if (m <= 0 || m > SB_MAX || n <= 0 || np % GT != 0 || kern < 0 || kern > 2) return HB_ERR_INVALID;
-  if (ws_bytes < 0 || (size_t)ws_bytes < sample_ws_bytes(np, sp.dtot(), m)) return HB_ERR_INVALID;
+  if (m <= 0 || m > SB_MAX) return HB_ERR_INVALID;
+  if (ws_bytes < 0 || (size_t)ws_bytes < sample_ws_bytes(gp.np, gp.sp.dtot(), m)) return HB_ERR_INVALID;
   static PerDevice once;   // the opt-in above 48 KB of dynamic shared memory is per device
   bool fresh = false;
   const int dev = once.slot(&fresh);
@@ -449,28 +466,15 @@ int launch_sample_y_batch(const float *Xs, const int32_t *Xe_s, int64_t m, int64
     HB_CUDA(cudaFuncSetAttribute(sample_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SB_SMEM));
     once.done[dev] = true;
   }
-  const int64_t mp = round_up(m, GT);       // the row tiles that hold the m rows (sample_ws_bytes pads to 2 GT)
-  const int ncg = kstar_groups(np);
-  float *KS = reinterpret_cast<float *>(ws);
-  float *Vb = KS + mp * np;
-  float *mupart = Vb + mp * np;
-  float *cov = mupart + (int64_t)ncg * mp;
-  float *ZsT = cov + mp * mp;
-  HB_CUDA(cudaMemsetAsync(KS, 0, (size_t)mp * np * sizeof(float), st));     // rows m..mp of K* must be zero for the GEMMs
-  int s = launch_kstar(Xs, Xe_s, m, sp, tab_s, x_mul, x_add, Zt, alpha, hyp, n, np, kern, KS, nullptr, mupart, mp, nullptr, nullptr, st);
+  const SampleWs w = carve_sample_ws(ws, gp.np, gp.sp.dtot(), round_up(m, GT));   // the row tiles that hold the m rows
+  int s = enqueue_sample_panels(gp, Xs, Xe_s, m, w, st);
   if (s != HB_OK) return s;
-  rows_gemm_kernel<0><<<dim3((unsigned)(np / GT), (unsigned)(mp / GT)), GTHREADS, 0, st>>>(KS, Linv, np, Vb);
-  cand_features_kernel<<<(int)ceil_div((int64_t)sp.dtot() * mp, 256), 256, 0, st>>>(Xs, Xe_s, m, mp, x_mul, x_add, hyp, tab_s, sp, ZsT);
-  count_launches(2);
-  ModelSpec sc = sp;
-  sc.warp = 1;                        // "prescaled features" switch of gram_kernel: ZsT is already warped and divided by l
-  s = launch_gram(ZsT, ZsT + (int64_t)sp.d * mp, m, mp, sc, hyp, kern, nullptr, 0.0f, cov, st);
+  s = enqueue_sample_cov(gp, m, w, 0.0f, st);
   if (s != HB_OK) return s;
-  const int nt = (int)(mp / GT);
-  cov_update_kernel<<<nt * (nt + 1) / 2, GTHREADS, 0, st>>>(cov, mp, m, Vb, np, 0.0f);
-  sample_batch_kernel<<<1, SB_THREADS, SB_SMEM, st>>>(Xs, Xe_s, (int)m, sp.d, sp.e, cov, mp, mupart, ncg, hyp, pred_likeli, y_mean,
-                                                      y_std, z, seed, counter, f, jitter_out, status);
-  count_launches(2);
+  sample_batch_kernel<<<1, SB_THREADS, SB_SMEM, st>>>(Xs, Xe_s, (int)m, gp.sp.d, gp.sp.e, w.cov, w.mp, w.mupart, kstar_groups(gp.np),
+                                                      gp.hyp, gp.pred_likeli, gp.y_mean, gp.y_std, z, seed, counter, f, jitter_out,
+                                                      status);
+  count_launches(1);
   HB_LAUNCH_CHECK("sample_y_batch");
   return HB_OK;
 }

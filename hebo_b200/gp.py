@@ -463,6 +463,16 @@ class GP(BaseModel):
             self._side_stream = torch.cuda.Stream(self.device)
         return self._side_stream
 
+    def _fitted_args(self, spec=None, x_mul=None, x_add=None):
+        """The fitted-model arguments shared by hb_posterior_mace_ex, hb_posterior_grad_ex, hb_sample_y and
+        hb_sample_y_batch, as the two runs (n ... Linv) and (kern ... pred_likeli); each call puts ``hyp`` and what it
+        alone takes between them."""
+        return ((self.n, self.d, self._spec_ptr() if spec is None else spec,
+                 _lib.ptr(self._emb_meta_dev) if self.num_enum else None, _lib.ptr(self.tab_s_dev) if self.num_enum else None,
+                 _lib.ptr(self._x_mul if x_mul is None else x_mul), _lib.ptr(self._x_add if x_add is None else x_add),
+                 _lib.ptr(self.Zt_dev), _lib.ptr(self.alpha_dev), _lib.ptr(self.Linv_dev)),
+                (self.kern_id, self._y_mean, self._y_std, int(bool(self.pred_likeli))))
+
     def _posterior(self, Xs_dev: Optional[torch.Tensor], want_F: bool, tau=0.0, kappa=0.0, eps=0.0, xi1=None, xi2=None,
                    seed: int = 0, want_mu_var: bool = True, Xe_dev: Optional[torch.Tensor] = None, out=None):
         """(F, mu, var) of a batch.  out: optional (mu, var) contiguous fp32 [m] device views to write instead of new
@@ -499,7 +509,7 @@ class GP(BaseModel):
                                                     float(eps), _lib.ptr(xi1), _lib.ptr(xi2), int(seed), _lib.ptr(F),
                                                     _lib.stream_ptr()), "hb_mace_epilogue")
             return F, (mu_f if want_mu_var else None), (var_f if want_mu_var else None)
-        x_mul, x_add = self._x_mul, self._x_add      # (an input warp is applied inside the K* load stage)
+        head, tail = self._fitted_args()      # (an input warp is applied inside the K* load stage)
         mc = min(self.m_chunk, max(128, -(-m // 128) * 128))
         need = int(lib.hb_posterior_workspace_bytes(self.n, self.d, mc))
         if self._post_ws is None or self._post_ws.numel() < need:
@@ -507,14 +517,10 @@ class GP(BaseModel):
 
         def call(xs, xe, rows, row0):
             off = lambda t, w=1: None if t is None else C.c_void_p(t.data_ptr() + row0 * w * 4)      # fp32 / int32 rows
-            return lib.hb_posterior_mace_ex(off(xs, self.d) if self.d > 0 else None, off(xe, self.num_enum), rows, row0, self.n, self.d,
-                                            self._spec_ptr(), _lib.ptr(self._emb_meta_dev) if self.num_enum else None,
-                                            _lib.ptr(self.tab_s_dev) if self.num_enum else None, _lib.ptr(x_mul), _lib.ptr(x_add),
-                                            _lib.ptr(self.Zt_dev), _lib.ptr(self.alpha_dev), _lib.ptr(self.Linv_dev),
+            return lib.hb_posterior_mace_ex(off(xs, self.d) if self.d > 0 else None, off(xe, self.num_enum), rows, row0, *head,
                                             _lib.ptr(self.Linv_hi_dev if self.tensor_cores else None),
                                             _lib.ptr(self.Linv_lo_dev if self.tensor_cores else None),
-                                            _lib.ptr(self.hyp_dev), self.kern_id, self._y_mean, self._y_std,
-                                            int(bool(self.pred_likeli)), float(tau), float(kappa), float(eps),
+                                            _lib.ptr(self.hyp_dev), *tail, float(tau), float(kappa), float(eps),
                                             off(xi1), off(xi2), int(seed), off(F, 3), off(mu), off(var),
                                             _lib.ptr(self._post_ws), self._post_ws.numel(), mc, _lib.stream_ptr())
         with torch.cuda.device(dev):
@@ -622,13 +628,9 @@ class GP(BaseModel):
             return mu, var, dmu, dvar
         with torch.cuda.device(dev):
             # (a warp stays in torch in front of this call so that autograd chains through it: the kernels get warp = 0)
-            st = lib.hb_posterior_grad_ex(_lib.ptr(Xin), _lib.ptr(self._grad_xe), m, self.n, self.d,
-                                          C.byref(self._spec_nowarp),
-                                          _lib.ptr(self._emb_meta_dev) if self.num_enum else None,
-                                          _lib.ptr(self.tab_s_dev) if self.num_enum else None, _lib.ptr(x_mul), _lib.ptr(x_add),
-                                          _lib.ptr(self.Zt_dev), _lib.ptr(self.alpha_dev), _lib.ptr(self.Linv_dev),
-                                          _lib.ptr(self.hyp_dev), self.kern_id, self._y_mean, self._y_std,
-                                          int(bool(self.pred_likeli)), _lib.ptr(mu), _lib.ptr(var), _lib.ptr(dmu), _lib.ptr(dvar),
+            head, tail = self._fitted_args(C.byref(self._spec_nowarp), x_mul, x_add)
+            st = lib.hb_posterior_grad_ex(_lib.ptr(Xin), _lib.ptr(self._grad_xe), m, *head, _lib.ptr(self.hyp_dev), *tail,
+                                          _lib.ptr(mu), _lib.ptr(var), _lib.ptr(dmu), _lib.ptr(dvar),
                                           _lib.ptr(self._post_ws), self._post_ws.numel(), mc, _lib.stream_ptr())
         _lib.check(st, "hb_posterior_grad")
         return mu, var, dmu, dvar
@@ -651,12 +653,10 @@ class GP(BaseModel):
             hyp_host = self.hyp.contiguous()
             jit = C.c_float(0.0)
             with torch.cuda.device(dev):
-                st = lib.hb_sample_y(_lib.ptr(Xs), _lib.ptr(xe), m, self.n, self.d, self._spec_ptr(),
-                                     _lib.ptr(self._emb_meta_dev) if self.num_enum else None,
-                                     _lib.ptr(self.tab_s_dev) if self.num_enum else None, _lib.ptr(self._x_mul), _lib.ptr(self._x_add),
-                                     _lib.ptr(self.Zt_dev), _lib.ptr(self.alpha_dev), _lib.ptr(self.Linv_dev), _lib.ptr(self.hyp_dev),
-                                     C.c_void_p(hyp_host.data_ptr()), self.kern_id, self._y_mean, self._y_std, int(bool(self.pred_likeli)),
-                                     _lib.ptr(z), int(n_samples), _lib.ptr(out), C.byref(jit), _lib.ptr(ws), ws.numel(), _lib.stream_ptr())
+                head, tail = self._fitted_args()
+                st = lib.hb_sample_y(_lib.ptr(Xs), _lib.ptr(xe), m, *head, _lib.ptr(self.hyp_dev),
+                                     C.c_void_p(hyp_host.data_ptr()), *tail, _lib.ptr(z), int(n_samples), _lib.ptr(out),
+                                     C.byref(jit), _lib.ptr(ws), ws.numel(), _lib.stream_ptr())
             _lib.check(st, "hb_sample_y")
             self.sample_jitter = jit.value
             return out.cpu().view(n_samples, m, self.num_out)
@@ -675,13 +675,10 @@ class GP(BaseModel):
         jitter = torch.empty(1, dtype=torch.float32, device=dev) if jitter is None else jitter
         ws = torch.empty(self.sample_batch_workspace_bytes(m), dtype=torch.uint8, device=dev) if ws is None else ws
         with torch.cuda.device(dev):
+            head, tail = self._fitted_args()
             st = lib.hb_sample_y_batch(_lib.ptr(Xs_dev) if self.d > 0 else None, _lib.ptr(Xe_dev) if self.num_enum else None, m,
-                                       self.n, self.d, self._spec_ptr(), _lib.ptr(self._emb_meta_dev) if self.num_enum else None,
-                                       _lib.ptr(self.tab_s_dev) if self.num_enum else None, _lib.ptr(self._x_mul), _lib.ptr(self._x_add),
-                                       _lib.ptr(self.Zt_dev), _lib.ptr(self.alpha_dev), _lib.ptr(self.Linv_dev), _lib.ptr(self.hyp_dev),
-                                       self.kern_id, self._y_mean, self._y_std, int(bool(self.pred_likeli)), _lib.ptr(z), int(seed),
-                                       int(counter), _lib.ptr(f), _lib.ptr(jitter), _lib.ptr(status), _lib.ptr(ws), ws.numel(),
-                                       _lib.stream_ptr())
+                                       *head, _lib.ptr(self.hyp_dev), *tail, _lib.ptr(z), int(seed), int(counter), _lib.ptr(f),
+                                       _lib.ptr(jitter), _lib.ptr(status), _lib.ptr(ws), ws.numel(), _lib.stream_ptr())
         _lib.check(st, "hb_sample_y_batch")
         return f
 
