@@ -72,8 +72,8 @@ template <class F> int with_kernel(int kern, bool emb, F &&f) {
 // ---------------------------------------------------------------- stationary kernels
 // k(r2) with unit outputscale.  KERN: 0 Matern-3/2, 1 Matern-5/2, 2 RBF (gpytorch MaternKernel/RBFKernel).
 // The radius and the exponential go through the SFU (MUFU.RSQ / MUFU.EX2: r = r2 * rsqrt(r2), exp(x) = ex2(x log2 e),
-// both ~2 ulp): the absolute error of k stays below ~1.5e-7 (it is largest where k ~ 1, i.e. no worse than the fp32
-// rounding of k itself), and the per-pair instruction count of the K* / Gram builders drops by about a third compared
+// both ~2 ulp): the absolute error of k at the r2 it receives stays below 3e-7, about four fp32 ulp of k ~ 1 (largest
+// measured 2.4e-7, Matern-5/2 near k ~ 1, on an H100; tests/test_gpu_fit_state.py), and the per-pair instruction count of the K* / Gram builders drops by about a third compared
 // with the IEEE sqrtf / expf sequences.  gram_kernel and kstar_kernel share these functions, so a candidate that
 // duplicates a training row reproduces that row of K bit for bit (r2 = 0 gives k = 1 exactly).
 __device__ __forceinline__ float fast_radius(float r2) {

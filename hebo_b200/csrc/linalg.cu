@@ -131,10 +131,14 @@ int launch_tri_inverse(const float *L, int64_t np, float *Linv, float *tmp, cuda
 // =============================================================================== refinement of L^-1 (prediction state)
 // One Newton step  X <- X + X (I - L X)  on the explicit inverse X = L^-1 the posterior contracts with.  The residual
 // R = I - L X is accumulated in fp64 (products of fp32 numbers are exact there), the correction X R in fp32 (R is
-// ~1e-5 small, so its relative accuracy is ample).  After the step every entry of X is the fp32 rounding of the exact
-// inverse of the fp32 factor L -- the explicit inverse then carries no more error than the triangular solve of the
-// reference (gp.py:148, gpytorch's cached prediction strategy), which matters exactly where sigma^2 = s - |L^-1 k*|^2
-// cancels (candidates on / next to training points).  Once per fit: ~n^3/3 DFMA + n^3/3 FFMA.
+// ~1e-5 small, so its relative accuracy is ample).  After the step X differs from the exact inverse Lambda of the fp32
+// factor L by at most u|X| + c u sqrt(NP) |X0||R| + |E0 L E0| (E0 = X0 - Lambda: exact Newton leaves -E0 L E0), with c
+// below 1.2 measured: on well-conditioned factors every entry is within 0-2 ulp of the fp32 rounding of Lambda, against up
+// to ~1e9 ulp (entries near zero) before the step; where cond_1(L) reaches 1e4 - 1e5 (d = 1, n = 4097, a factor after the
+// jitter ladder) the quadratic term leaves tens to a thousand ulp on some entries (tests/test_gpu_fit_state.py).  The
+// explicit inverse then carries about the error of the triangular solve of the reference (gp.py:148, gpytorch's cached
+// prediction strategy), which matters exactly where sigma^2 = s - |L^-1 k*|^2 cancels (candidates on / next to training
+// points).  Once per fit: ~n^3/3 DFMA + n^3/3 FFMA.
 // the Cholesky works in place on the lower triangle: the strict upper part of the diagonal tiles still holds Khat
 __global__ void __launch_bounds__(256) zero_upper_diag_kernel(float *__restrict__ L, int64_t np) {
   const int64_t o = (int64_t)blockIdx.x * GT;
@@ -345,7 +349,7 @@ size_t solve_ws_bytes(int64_t np) { return (size_t)np * sizeof(double) * (1 + (s
 
 int launch_solve_logdet(const float *L, const float *Linv, const float *y, int64_t n, int64_t np, const float *hyp,
                         float *alpha, double *scal, void *ws, cudaStream_t st, const Batch &bt) {
-  if (np <= 0 || np % GT != 0 || n > np) return HB_ERR_INVALID;
+  if (np <= 0 || np % GT != 0 || n <= 0 || n > np) return HB_ERR_INVALID;
   double *v = reinterpret_cast<double *>(ws);
   double *partial = v + np;
   const int nslab = (int)(np / GEMVT_ROWS);

@@ -145,7 +145,8 @@ int32_t hb_kinv(const float *Linv, int64_t np, float *Kinv, void *stream);
  * models/gp/gp.py:102,113; alpha is also the prediction-strategy mean cache, gp.py:148) --------
  * r = y - c (pad = 0).  alpha = Khat^-1 r, quad = r^T Khat^-1 r, logdet = 2 sum log L_ii.
  * scal[0] = quad, scal[1] = logdet (device, fp64 accumulated, stored as double[2]).
- * ws: >= 2*NP*sizeof(double) + 64*NP*sizeof(double). */
+ * 1 <= n <= NP, otherwise HB_ERR_INVALID before any launch.
+ * ws: >= (1 + NP/64)*NP*sizeof(double). */
 int32_t hb_solve_logdet(const float *L, const float *Linv, const float *y, int64_t n, int64_t np,
                         const float *hyp, float *alpha, double *scal, void *ws, void *stream);
 

@@ -70,6 +70,32 @@ def test_invalid_arguments_are_reported_not_crashed(lib):
     assert lib.hb_mll_fwd_bwd(None, None, None, 10, 2, None, None, 0, None, 0.0, 0.01, 0.0, None, None, None, None, 0, None) == _lib.HB_ERR_INVALID
 
 
+def test_linalg_stages_reject_bad_sizes_and_null_pointers(lib):
+    """hb_tri_inverse, hb_kinv and hb_solve_logdet refuse NP <= 0 or not a multiple of 128, n <= 0 or n > NP, and every
+    NULL pointer with HB_ERR_INVALID before any launch.  The pointers are fake and never dereferenced."""
+    bad = _lib.HB_ERR_INVALID
+    p = ctypes.c_void_p(16)
+    for np_ in (0, -128, 100, 129, 200):
+        assert lib.hb_tri_inverse(p, np_, p, p, None) == bad, np_
+        assert lib.hb_kinv(p, np_, p, None) == bad, np_
+        assert lib.hb_solve_logdet(p, p, p, 10, np_, p, p, p, p, None) == bad, np_
+    for n, np_ in ((0, 128), (-1, 128), (-(1 << 40), 256), (129, 128), (257, 256)):
+        assert lib.hb_solve_logdet(p, p, p, n, np_, p, p, p, p, None) == bad, (n, np_)
+    for k in range(3):
+        args = [p, p, p]
+        args[k] = None
+        assert lib.hb_tri_inverse(args[0], 128, args[1], args[2], None) == bad, k
+    for k in range(2):
+        args = [p, p]
+        args[k] = None
+        assert lib.hb_kinv(args[0], 128, args[1], None) == bad, k
+    for k in range(7):
+        args = [p] * 7                      # L, Linv, y, hyp, alpha, scal, ws
+        args[k] = None
+        L, Linv, y, hyp, alpha, scal, ws = args
+        assert lib.hb_solve_logdet(L, Linv, y, 10, 128, hyp, alpha, scal, ws, None) == bad, k
+
+
 @pytest.mark.parametrize("ws_bytes", ["short", -1, -(1 << 40)])
 def test_workspace_size_is_checked_as_a_signed_count(lib, ws_bytes):
     """A workspace one byte short, or of negative size, is refused before any launch.  A negative int64 must not pass the

@@ -61,7 +61,8 @@ import torch
 from hebo_b200 import _lib
 from oracle import gp_oracle as O
 from tests.util import (DEV, VARIANTS, WIDTHS, candidates, features64, fit_model, gather_emb, kernel_parts, kmat64,
-                        true_model)
+                        true_model, warp_error)
+from tests.util import reset_hypers as _set
 
 pytestmark = pytest.mark.gpu
 
@@ -146,25 +147,6 @@ def guard_stats(reset):
 
 
 # ---------------------------------------------------------------------------------------------------------------- (a) own state
-def warp_error(px, xt, a, b):
-    """W: the fp32 error of kumar_warp (common.cuh) at x_t = fl(px + x_add), px = x_mul x, in units of u (docstring)."""
-    eps = 1e-6
-    h = (xt + 1) * 0.5
-    uu = h.clamp(eps, 1 - eps)
-    clamped = (h < eps) | (h > 1 - eps)
-    e_u = torch.where(clamped, torch.ones_like(h), (px.abs() + xt.abs() + (xt + 1).abs()) / (2 * uu))
-    lu = uu.log()
-    e_lu = e_u + 2 * lu.abs() + 1
-    t = torch.exp(a * lu)
-    e_t = a * e_lu + (a * lu).abs() + 2
-    lom = torch.log1p(-t)
-    e_lom = t / (1 - t) * e_t + 2 * lom.abs() + 1
-    p = torch.exp(b * lom)
-    e_p = b * e_lom + (b * lom).abs() + 2
-    w = 2 * (1 - p) - 1
-    return 2 * p * e_p + 2 * (1 - p).abs() + w.abs()
-
-
 def own_state(gp, Xs, Xe, y_std=None, dtype=torch.float64, bounds=True):
     """The closed form of the module docstring on the GP's own fp32 state, in `dtype`, with the bounds B in fp64."""
     dt = dtype
@@ -530,21 +512,6 @@ def check_operand_split(gp):
 
 
 # ---------------------------------------------------------------------------------------------------------------- extremes
-def _set(gp, **kw):
-    """set_hypers on a copy of gp's raw vector: os (outputscale), noise (sigma_n^2 - noise_lb), ls (all lengthscales)."""
-    lay = gp._param_layout()
-    raw = gp.raw.clone()
-    inv = lambda v: float(O.inv_softplus(torch.tensor(v, dtype=torch.float64)))
-    if "os" in kw:
-        raw[lay["os"]] = inv(kw["os"])
-    if "noise" in kw:
-        raw[0] = kw["noise"]
-    if "ls" in kw:
-        raw[lay["ls"]:lay["ls"] + lay["n_ls"]] = inv(kw["ls"])
-    gp.set_hypers(raw)
-    assert not gp._fit_failed
-
-
 @pytest.mark.parametrize("outputscale", [1e-3, 1e3])
 def test_outputscale_extremes(outputscale):
     """s = 1e-3 and 1e3 move the K* operand scale 2^k far from 1."""

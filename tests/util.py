@@ -282,6 +282,42 @@ def gather_emb(gp, Xe, flat):
     return torch.cat(out, 1)
 
 
+def reset_hypers(gp, **kw):
+    """set_hypers on a copy of gp's raw vector: os (outputscale), noise (sigma_n^2 - noise_lb), ls (all lengthscales)."""
+    from oracle import gp_oracle as O
+    lay = gp._param_layout()
+    raw = gp.raw.clone()
+    inv = lambda v: float(O.inv_softplus(torch.tensor(v, dtype=torch.float64)))
+    if "os" in kw:
+        raw[lay["os"]] = inv(kw["os"])
+    if "noise" in kw:
+        raw[0] = kw["noise"]
+    if "ls" in kw:
+        raw[lay["ls"]:lay["ls"] + lay["n_ls"]] = inv(kw["ls"])
+    gp.set_hypers(raw)
+    assert not gp._fit_failed
+
+
+def warp_error(px, xt, a, b):
+    """W: the fp32 error of kumar_warp (common.cuh) at x_t = fl(px + x_add), px = x_mul x, in units of u
+    (test_gpu_posterior_mace.py docstring)."""
+    eps = 1e-6
+    h = (xt + 1) * 0.5
+    uu = h.clamp(eps, 1 - eps)
+    clamped = (h < eps) | (h > 1 - eps)
+    e_u = torch.where(clamped, torch.ones_like(h), (px.abs() + xt.abs() + (xt + 1).abs()) / (2 * uu))
+    lu = uu.log()
+    e_lu = e_u + 2 * lu.abs() + 1
+    t = torch.exp(a * lu)
+    e_t = a * e_lu + (a * lu).abs() + 2
+    lom = torch.log1p(-t)
+    e_lom = t / (1 - t) * e_t + 2 * lom.abs() + 1
+    p = torch.exp(b * lom)
+    e_p = b * e_lom + (b * lom).abs() + 2
+    w = 2 * (1 - p) - 1
+    return 2 * p * e_p + 2 * (1 - p).abs() + w.abs()
+
+
 def kernel_parts(r2, kind):
     """k, h (dk/dr^2 = -h / 2), |exponent of fast_exp| and the rate of that exponent in the features."""
     if kind == "rbf":
