@@ -15,128 +15,214 @@
 
 namespace hb {
 
-constexpr int KS_ROWS = 32;     // candidates per CTA in kstar_kernel
+constexpr int KS_ROWS = 128;    // candidates per kstar_kernel tile
 constexpr int KS_COLS = 128;    // training points per sub-tile
-constexpr int KS_GROUP = 512;   // training points per CTA (4 sub-tiles)
-constexpr int KS_DC = 32;
+constexpr int KS_GROUP = 512;   // training points per tile (4 sub-tiles; one mean partial per candidate and group)
+constexpr int KS_KC = 16;       // features per pipeline stage
+constexpr int KS_FSLOTS = 2;    // feature stages in shared memory; a tile with at most this many keeps them all
 // chunk rows of the workspace are rounded to whole clusters of 128-row bands: the tensor contraction pads the band count
 // of a chunk to a multiple of the cluster size
 constexpr int64_t CHUNK_ROWS = h16::CLUSTER * h16::BM;
 static_assert(CHUNK_ROWS % (2 * GT) == 0, "chunk rows: a multiple of 2 GT");
 
+// 16-byte global -> shared copy that bypasses the register file (L2 only)
+__device__ __forceinline__ void cp_async16(void *dst, const void *src) {
+  const unsigned ds = (unsigned)__cvta_generic_to_shared(dst);
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(ds), "l"(src) : "memory");
+}
+
+// acc[i][j] += (a_i - b_j)^2 over the kc features of one stage: a_i the feature of tile row (i < 4 ? 0 : 60) + ty*4 + i,
+// b_j the Zt entry of sub-tile column (j < 4 ? 0 : 60) + tx*4 + j.  Per k: two broadcast and two conflict-free LDS.128
+// against 64 FADD + 64 FFMA.
+__device__ __forceinline__ void ks_contract(const float (&zs)[KS_KC][KS_ROWS], const float (&zt)[KS_KC][KS_COLS], int kc,
+                                            float (&acc)[8][8]) {
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+#pragma unroll 4
+  for (int kk = 0; kk < kc; ++kk) {
+    const float4 a0 = *reinterpret_cast<const float4 *>(&zs[kk][ty * 4]);
+    const float4 a1 = *reinterpret_cast<const float4 *>(&zs[kk][64 + ty * 4]);
+    const float4 b0 = *reinterpret_cast<const float4 *>(&zt[kk][tx * 4]);
+    const float4 b1 = *reinterpret_cast<const float4 *>(&zt[kk][64 + tx * 4]);
+    const float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+    const float b[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float df = a[i] - b[j];
+        acc[i][j] = fmaf(df, df, acc[i][j]);
+      }
+  }
+}
+
 // SPLIT: 0 = plain fp32 K* in KS (SIMT contraction / guard pass); 2 = the two-level fp16 split in the KS_lo buffer
 // (h0 [mc_pad, np] halfs, then h1) and nothing else.
 // fixlist != nullptr (SPLIT 0 only): the guard's second pass -- output row `slot` is the exact fp32 K* row of candidate
-// fixlist[slot], for slot < *fixcount (blocks beyond the count exit at once); no mean partials.
+// fixlist[slot], for slot < *fixcount; no mean partials.  Its grid is at most one resident wave, whose CTAs walk the
+// tiles of the first *fixcount slots.
 // EMB: mixed model (gp_util.py:54-57): Zt holds d numeric rows followed by De embedding rows (both already divided by
 // their lengthscales); the candidate's embedding features are gathered from tab_s (tables / le) by its categories
 // Xe_s [m, e]; k* = s k_KERN(r over the numeric rows) Matern32(r over the embedding rows).
-// The candidates' features are staged one KS_DC chunk at a time next to the matching chunk of Zt, so shared memory is
-// fixed whatever d + De is; each 128-column sub-tile recomputes them (KS_DC features x KS_ROWS candidates per chunk).
+//
+// A tile is KS_ROWS candidates x one KS_GROUP column group, walked as four 128 x 128 sub-tiles, 8 x 8 pairs per thread
+// (two CTAs per SM for the tensor path's split rows; one, with room for r2e, for fp32 rows and the mixed model).
+// Features move in stages of KS_KC: while one stage is contracted, the next stage's Zt slab is in flight (cp.async) and
+// the next stage's candidate features are computed into the other slot, one barrier per stage.  A tile of at most
+// KS_FSLOTS stages (d + De <= 32) computes its candidates' features once for all four sub-tiles; a deeper one recomputes
+// them per sub-tile, so shared memory is 48 KB whatever d + De is.  Rows of the last tile past the candidate count get
+// the K* row of an all-zero feature vector.
+// Per pair the arithmetic is the Gram kernel's: fmaf(a - b, a - b, r2) in ascending k (numeric rows, then embedding rows),
+// then s k_KERN(r2) [* Matern32(r2e)], pad columns (index >= n) zeroed.  The K* alpha mean partial of a row is summed in
+// fmaf per 4-column lane of a sub-tile (a thread holds two lanes: columns tx*4.. and 64+tx*4..), sub-tiles then columns
+// ascending, and the 32 lanes of a group are added in the xor 16, 8, 4, 2, 1 butterfly order.
 template <int KERN, int SPLIT, bool EMB>
-__global__ void __launch_bounds__(256) kstar_kernel(const float *__restrict__ Xs, int64_t mc, int d,
-                                                    const float *__restrict__ x_mul, const float *__restrict__ x_add,
-                                                    const float *__restrict__ Zt, const float *__restrict__ alpha,
-                                                    const float *__restrict__ hyp, int64_t n, int64_t np,
-                                                    float *__restrict__ KS, float *__restrict__ KS_lo,
-                                                    float *__restrict__ mupart, int64_t mc_pad,
-                                                    const int32_t *__restrict__ fixlist, const int32_t *__restrict__ fixcount,
-                                                    const int32_t *__restrict__ Xe_s, const float *__restrict__ tab_s,
-                                                    ModelSpec sp) {
-  __shared__ float zs[KS_DC][KS_ROWS + 1];      // scaled candidate features of the chunk, transposed
-  __shared__ __align__(16) float zt[KS_DC][KS_COLS];
+__global__ void __launch_bounds__(256, (EMB || SPLIT == 0) ? 1 : 2) kstar_kernel(const float *__restrict__ Xs, int64_t mc, int d,
+                                                                 const float *__restrict__ x_mul, const float *__restrict__ x_add,
+                                                                 const float *__restrict__ Zt, const float *__restrict__ alpha,
+                                                                 const float *__restrict__ hyp, int64_t n, int64_t np,
+                                                                 float *__restrict__ KS, float *__restrict__ KS_lo,
+                                                                 float *__restrict__ mupart, int64_t mc_pad,
+                                                                 const int32_t *__restrict__ fixlist,
+                                                                 const int32_t *__restrict__ fixcount,
+                                                                 const int32_t *__restrict__ Xe_s, const float *__restrict__ tab_s,
+                                                                 ModelSpec sp) {
+  __shared__ __align__(16) float zs[KS_FSLOTS][KS_KC][KS_ROWS];   // candidate features of a stage, transposed
+  __shared__ __align__(16) float zt[2][KS_KC][KS_COLS];           // Zt slab of a stage, double-buffered
+  __shared__ float mu_acc[8][2][256];   // per thread and row: its lanes tx and tx + 16 of the 32 four-column lanes
   const int t = threadIdx.x;
-  const int tx = t & 31, ty = t >> 5;           // warp ty owns rows ty*4..+3, lane tx owns cols tx*4..+3
-  const int64_t r0 = (int64_t)blockIdx.x * KS_ROWS;
+  const int tx = t & 15, ty = t >> 4;
+  if (SPLIT != 0) fixlist = nullptr;   // (the guard pass writes fp32 rows)
   const int64_t nrows = fixlist ? (int64_t)*fixcount : mc;
-  if (r0 >= nrows) return;   // (block-uniform; only the guard pass launches more blocks than it needs)
+  const int nrt = (int)ceil_div(nrows, KS_ROWS);
+  const int ntiles = nrt * (int)ceil_div(np, KS_GROUP);
   const int De = EMB ? sp.De : 0;
+  const int nnum = (int)ceil_div(d, KS_KC);                  // stages of the numeric rows, then of the embedding rows
+  const int nst = nnum + (int)ceil_div(De, KS_KC);
+  const bool keep = nst <= KS_FSLOTS;                        // features staged once per tile
   const float s = hyp[2];
   const float sa = pow2_scale(s, 1);   // fp16 operand scale: K* <= s lands in [0, 2)
-  __half *KS_h0 = reinterpret_cast<__half *>(KS_lo), *KS_h1 = KS_h0 + mc_pad * np;
-  float mu_acc[4] = {0.f, 0.f, 0.f, 0.f};
-  const int64_t cg0 = (int64_t)blockIdx.y * KS_GROUP;
-  for (int sub = 0; sub < KS_GROUP / KS_COLS; ++sub) {
-    const int64_t c0 = cg0 + (int64_t)sub * KS_COLS;
-    if (c0 >= np) break;
-    float r2[4][4], r2e[4][4];   // (r2e dead unless EMB)
+  // feature rows [k0, k0 + kc) of stage c, and whether they are embedding rows
+  auto stage_rows = [&](int c, int &k0, int &kc) {
+    const bool emb = EMB && c >= nnum;
+    k0 = emb ? d + (c - nnum) * KS_KC : c * KS_KC;
+    kc = min(KS_KC, (emb ? d + De : d) - k0);
+    return emb;
+  };
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const int64_t r0 = (int64_t)(tile % nrt) * KS_ROWS;
+    const int grp = tile / nrt;
+    const int cg0 = grp * KS_GROUP;
+    const int nstage = min(KS_GROUP / KS_COLS, (int)(np - cg0) / KS_COLS) * nst;
+    // features: thread t computes those of tile row t % KS_ROWS
+    const int64_t frow = r0 + (t & (KS_ROWS - 1));
+    const bool flive = frow < nrows;
+    const int src = flive ? (fixlist ? fixlist[frow] : (int)frow) : 0;
+    // stage g of the tile is stage c of sub-tile sub (g = sub * nst + c)
+    auto load_zt = [&](int g, int sub, int c) {   // into buffer g & 1
+      int k0, kc;
+      stage_rows(c, k0, kc);
+      const float *base = Zt + cg0 + sub * KS_COLS;
 #pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) r2[i][j] = r2e[i][j] = 0.0f;
-#pragma unroll
-    for (int phase = 0; phase < (EMB ? 2 : 1); ++phase) {
-      const int kbeg = phase ? d : 0, kend = phase ? d + De : d;
-      float (&acc)[4][4] = phase ? r2e : r2;
-      for (int k0 = kbeg; k0 < kend; k0 += KS_DC) {
-        const int kc = min(KS_DC, kend - k0);
-        __syncthreads();
-        for (int f = t; f < kc * (KS_COLS / 4); f += 256) {
-          const int kk = f >> 5, c4 = f & 31;
-          *reinterpret_cast<float4 *>(&zt[kk][c4 * 4]) =
-              __ldg(reinterpret_cast<const float4 *>(Zt + (int64_t)(k0 + kk) * np + c0 + c4 * 4));
+      for (int q = 0; q < 2; ++q) {
+        const int f = t + q * 256, kk = f >> 5, c4 = f & 31;
+        if (kk < kc) cp_async16(&zt[g & 1][kk][c4 * 4], base + (int64_t)(k0 + kk) * np + c4 * 4);
+      }
+      asm volatile("cp.async.commit_group;\n" ::: "memory");
+    };
+    auto zslot = [&](int g, int c) { return keep ? c : g & 1; };
+    auto load_zs = [&](int g, int c) {
+      int k0, kc;
+      const bool emb = stage_rows(c, k0, kc);
+      float(&z)[KS_KC][KS_ROWS] = zs[zslot(g, c)];
+#pragma unroll 1
+      for (int q = 0; q < KS_KC / 2; ++q) {
+        const int kk = (t >> 7) + 2 * q;
+        if (kk < kc) {
+          float v = 0.0f;
+          if (flive)
+            v = emb ? tab_s[emb_entry(sp, Xe_s, src, k0 + kk - d)]
+                    : cand_feature(sp, sp.warp, Xs[(int64_t)src * d + k0 + kk], k0 + kk, x_mul, x_add, hyp);   // input warp fused here
+          z[kk][t & (KS_ROWS - 1)] = v;
         }
-        for (int f = t; f < KS_ROWS * KS_DC; f += 256) {
-          const int row = f / KS_DC, kk = f % KS_DC;
-          if (kk >= kc) continue;
-          float z = 0.0f;
-          if (r0 + row < nrows) {
-            const int64_t src = fixlist ? (int64_t)fixlist[r0 + row] : r0 + row;
-            z = phase ? tab_s[emb_entry(sp, Xe_s, src, k0 + kk - d)]
-                      : cand_feature(sp, sp.warp, Xs[src * d + k0 + kk], k0 + kk, x_mul, x_add, hyp);   // input warp fused here
-          }
-          zs[kk][row] = z;
-        }
-        __syncthreads();
-#pragma unroll 4
-        for (int kk = 0; kk < kc; ++kk) {
-          const float4 b4 = *reinterpret_cast<const float4 *>(&zt[kk][tx * 4]);
-          const float b[4] = {b4.x, b4.y, b4.z, b4.w};
-          const float *zr = &zs[kk][ty * 4];
-          const float a[4] = {zr[0], zr[1], zr[2], zr[3]};
+      }
+    };
+    float r2[8][8], r2e[8][8];   // (r2e dead unless EMB)
 #pragma unroll
-          for (int i = 0; i < 4; ++i)
+    for (int i = 0; i < 8; ++i) mu_acc[i][0][t] = mu_acc[i][1][t] = 0.0f;
+    load_zt(0, 0, 0);
+    load_zs(0, 0);
+    asm volatile("cp.async.wait_all;\n" ::: "memory");
+    __syncthreads();
+    for (int g = 0, sub = 0, c = 0; g < nstage; ++g) {
+      const int c1 = c + 1 == nst ? 0 : c + 1, sub1 = c1 ? sub : sub + 1;   // the next stage
+      if (c == 0) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+#pragma unroll
+          for (int j = 0; j < 8; ++j) r2[i][j] = r2e[i][j] = 0.0f;
+      }
+      if (g + 1 < nstage) load_zt(g + 1, sub1, c1);
+      {
+        int k0, kc;
+        const bool emb = stage_rows(c, k0, kc);
+        if (emb) ks_contract(zs[zslot(g, c)], zt[g & 1], kc, r2e);
+        else ks_contract(zs[zslot(g, c)], zt[g & 1], kc, r2);
+      }
+      if (g + 1 < nstage && (!keep || sub1 == 0)) load_zs(g + 1, c1);
+      if (c == nst - 1) {   // sub-tile done: K* rows, mean partials
+        const int c0 = cg0 + sub * KS_COLS;
+        float al[2][4];
+        int ncol[2];   // valid columns among each 4-column half (pad columns, training index >= n, must come out as exact
+                       // zeros: the pad block of Linv is the identity)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int cc = c0 + h * 64 + tx * 4;
+          const float4 a4 = __ldg(reinterpret_cast<const float4 *>(alpha + cc));
+          al[h][0] = a4.x; al[h][1] = a4.y; al[h][2] = a4.z; al[h][3] = a4.w;
+          ncol[h] = (int)min((int64_t)4, max((int64_t)0, n - cc));
+        }
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int64_t rowoff = (r0 + (i < 4 ? 0 : 60) + ty * 4 + i) * np + c0 + tx * 4;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float o[4], mu = mu_acc[i][h][t];
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
-              const float df = a[i] - b[j];
-              acc[i][j] = fmaf(df, df, acc[i][j]);
+              float kv = s * kern_eval<KERN>(r2[i][h * 4 + j]);
+              if (EMB) kv *= kern_eval<HB_KERN_MATERN32>(r2e[i][h * 4 + j]);
+              if (j >= ncol[h]) kv = 0.0f;
+              o[j] = kv;
+              mu = fmaf(kv, al[h][j], mu);
             }
+            mu_acc[i][h][t] = mu;
+            const int64_t off = rowoff + h * 64;
+            if (SPLIT == 2) {
+              unsigned int a01, a23, b01, b23;
+              split_h16x2(o[0] * sa, o[1] * sa, a01, b01);
+              split_h16x2(o[2] * sa, o[3] * sa, a23, b23);
+              __half *h0 = reinterpret_cast<__half *>(KS_lo) + off;   // h0 [mc_pad, np], then h1
+              *reinterpret_cast<uint2 *>(h0) = make_uint2(a01, a23);
+              *reinterpret_cast<uint2 *>(h0 + mc_pad * np) = make_uint2(b01, b23);
+            } else {
+              *reinterpret_cast<float4 *>(KS + off) = make_float4(o[0], o[1], o[2], o[3]);
+            }
+          }
         }
       }
+      asm volatile("cp.async.wait_all;\n" ::: "memory");
+      __syncthreads();
+      c = c1;
+      sub = sub1;
     }
-    const float4 al4 = __ldg(reinterpret_cast<const float4 *>(alpha + c0 + tx * 4));
-    const float al[4] = {al4.x, al4.y, al4.z, al4.w};
-    // pad columns (training index >= n) must come out as exact zeros: the pad block of Linv is the identity.  Only the
-    // last 128-column sub-tile can contain them, so the test is hoisted out of the per-pair code.
-    const int ncol = (int)min((int64_t)4, max((int64_t)0, n - (c0 + tx * 4)));   // valid columns among this thread's 4
-    const int64_t rowoff = (r0 + ty * 4) * np + c0 + tx * 4;
+    // lanes tx and tx + 16 first (the xor-16 step), then xor 8..1 across the 16 threads of this row group
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      float o[4];
+    for (int i = 0; i < 8; ++i) {
+      float v = mu_acc[i][0][t] + mu_acc[i][1][t];
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float kv = s * kern_eval<KERN>(r2[i][j]);
-        if (EMB) kv *= kern_eval<HB_KERN_MATERN32>(r2e[i][j]);
-        if (j >= ncol) kv = 0.0f;
-        o[j] = kv;
-        mu_acc[i] = fmaf(kv, al[j], mu_acc[i]);
-      }
-      const int64_t off = rowoff + (int64_t)i * np;
-      if (SPLIT == 2) {
-        unsigned int a01, a23, b01, b23;
-        split_h16x2(o[0] * sa, o[1] * sa, a01, b01);
-        split_h16x2(o[2] * sa, o[3] * sa, a23, b23);
-        *reinterpret_cast<uint2 *>(KS_h0 + off) = make_uint2(a01, a23);
-        *reinterpret_cast<uint2 *>(KS_h1 + off) = make_uint2(b01, b23);
-      } else {
-        *reinterpret_cast<float4 *>(KS + off) = make_float4(o[0], o[1], o[2], o[3]);
-      }
+      for (int o = 8; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      if (tx == 0 && mupart) mupart[(int64_t)grp * mc_pad + r0 + (i < 4 ? 0 : 60) + ty * 4 + i] = v;
     }
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const float v = warp_sum(mu_acc[i]);
-    if (tx == 0 && mupart) mupart[(int64_t)blockIdx.y * mc_pad + r0 + ty * 4 + i] = v;
   }
 }
 
@@ -212,31 +298,37 @@ __global__ void __launch_bounds__(GTHREADS, 1) vnorm_fix_kernel(const float *__r
                                                                 float *__restrict__ vfix, int compact) {
   __shared__ GemmSmem sm;
   const int cnt = *count;
-  const int64_t g = blockIdx.y;
-  if (g * GT >= cnt) return;
   const int nt = (int)(np / GT);
-  const int J = nt - 1 - (int)blockIdx.x;
-  int64_t rows[2];
-#pragma unroll
-  for (int q = 0; q < 2; ++q) {
-    const int64_t slot = g * GT + ((threadIdx.x + q * GTHREADS) >> 2);
-    rows[q] = compact ? (slot < cnt ? slot : 0) : fixlist[slot < cnt ? slot : 0];   // compact: KS_hi row = slot
-  }
-  double acc[8][8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) acc[i][j] = 0.0;
-  gemm_mainloop_gatherA(KS_hi, KS_lo, np, rows, Linv + (int64_t)J * GT * np, np, 0, (J + 1) * GT, acc, sm);
+  const int64_t ngr = ceil_div(cnt, GT);   // row groups of the flagged slots
   const int tx = threadIdx.x & 15;
+  // units (J, g) ordered by decreasing k range (J = nt - 1 first), dealt out in rounds of gridDim.x, every other round in
+  // reverse CTA order, so that every CTA gets about the same number of k-tiles
+  for (int64_t round = 0;; ++round) {
+    const int64_t u = round * gridDim.x + ((round & 1) ? gridDim.x - 1 - blockIdx.x : blockIdx.x);
+    if (u >= ngr * nt) break;
+    const int J = nt - 1 - (int)(u / ngr);
+    const int64_t g = u % ngr;
+    int64_t rows[2];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    double s = 0.0;
+    for (int q = 0; q < 2; ++q) {
+      const int64_t slot = g * GT + ((threadIdx.x + q * GTHREADS) >> 2);
+      rows[q] = compact ? (slot < cnt ? slot : 0) : fixlist[slot < cnt ? slot : 0];   // compact: KS_hi row = slot
+    }
+    double acc[8][8];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) s = fma(acc[i][j], acc[i][j], s);
+    for (int i = 0; i < 8; ++i)
 #pragma unroll
-    for (int o = 8; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (tx == 0) vfix[(int64_t)J * mc_pad + g * GT + gemm_row(i)] = (float)s;
+      for (int j = 0; j < 8; ++j) acc[i][j] = 0.0;
+    gemm_mainloop_gatherA(KS_hi, KS_lo, np, rows, Linv + (int64_t)J * GT * np, np, 0, (J + 1) * GT, acc, sm);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      double s = 0.0;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) s = fma(acc[i][j], acc[i][j], s);
+#pragma unroll
+      for (int o = 8; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+      if (tx == 0) vfix[(int64_t)J * mc_pad + g * GT + gemm_row(i)] = (float)s;
+    }
   }
 }
 
@@ -436,21 +528,55 @@ int kstar_groups(int64_t np) { return (int)ceil_div(np, KS_GROUP); }
 //   fixlist != nullptr: the guard pass: KS row `slot` is the exact fp32 row of candidate fixlist[slot], slot < *fixcount
 //                       (mupart nullptr);
 //   otherwise:          fp32 rows into KS, mean partials into mupart.
+// CTAs of `kernel` (256 threads) that are resident on the current device at once, looked up once per device
+template <class Kernel>
+static int resident_wave(Kernel kernel, PerDevice &once, int64_t *ctas) {
+  bool fresh = false;
+  const int dev = once.slot(&fresh);
+  if (dev < 0) return HB_ERR_CUDA;
+  if (fresh) {
+    int sms = 0, per_sm = 0;
+    HB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    HB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, 256, 0));
+    once.aux[dev] = sms * max(per_sm, 1);
+    once.done[dev] = true;
+  }
+  *ctas = once.aux[dev];
+  return HB_OK;
+}
+template <int KERN, bool EMB>
+static int kstar_guard_wave(int64_t *ctas) {
+  static PerDevice once;
+  return resident_wave(kstar_kernel<KERN, 0, EMB>, once, ctas);
+}
+
 int launch_kstar(const Fitted &gp, const float *xs, const int32_t *xe, int64_t mc, float *KS, float *KS_h16, float *mupart,
                  int64_t mc_pad, const int32_t *fixlist, const int32_t *fixcount, cudaStream_t st) {
   const ModelSpec &sp = gp.sp;
-  const dim3 grid((unsigned)ceil_div(mc, KS_ROWS), (unsigned)kstar_groups(gp.np));
+  const int64_t tiles = ceil_div(mc, KS_ROWS) * kstar_groups(gp.np);   // (the guard pass: the most its count can need)
+  int r = HB_OK;
   const int s = with_kernel(gp.kern, sp.e > 0, [&](auto kk, auto ee) {
     constexpr int KERN = decltype(kk)::value;
     constexpr bool EMB = decltype(ee)::value;
-    if (KS_h16)
-      kstar_kernel<KERN, 2, EMB><<<grid, 256, 0, st>>>(xs, mc, sp.d, gp.x_mul, gp.x_add, gp.Zt, gp.alpha, gp.hyp, gp.n, gp.np, KS,
-                                                         KS_h16, mupart, mc_pad, fixlist, fixcount, xe, gp.tab_s, sp);
-    else
-      kstar_kernel<KERN, 0, EMB><<<grid, 256, 0, st>>>(xs, mc, sp.d, gp.x_mul, gp.x_add, gp.Zt, gp.alpha, gp.hyp, gp.n, gp.np, KS,
-                                                         KS_h16, mupart, mc_pad, fixlist, fixcount, xe, gp.tab_s, sp);
+    if (KS_h16) {
+      kstar_kernel<KERN, 2, EMB><<<(unsigned)tiles, 256, 0, st>>>(xs, mc, sp.d, gp.x_mul, gp.x_add, gp.Zt, gp.alpha, gp.hyp, gp.n,
+                                                                  gp.np, KS, KS_h16, mupart, mc_pad, fixlist, fixcount, xe,
+                                                                  gp.tab_s, sp);
+    } else {
+      int64_t grid = tiles;
+      if (fixlist) {   // the flagged count is only known on the device: one resident wave walks its tiles
+        int64_t wave = 0;
+        r = kstar_guard_wave<KERN, EMB>(&wave);
+        if (r != HB_OK) return;
+        grid = min(grid, wave);
+      }
+      kstar_kernel<KERN, 0, EMB><<<(unsigned)grid, 256, 0, st>>>(xs, mc, sp.d, gp.x_mul, gp.x_add, gp.Zt, gp.alpha, gp.hyp, gp.n,
+                                                                 gp.np, KS, KS_h16, mupart, mc_pad, fixlist, fixcount, xe,
+                                                                 gp.tab_s, sp);
+    }
   });
   if (s != HB_OK) return s;
+  if (r != HB_OK) return r;
   count_launches(1);
   return HB_OK;
 }
@@ -506,7 +632,11 @@ int launch_posterior_mace(const Fitted &gp, const float *Xs, const int32_t *Xe_s
       // exact fp32 K* rows of the flagged candidates only (compact, row = slot), then their FP32 contraction
       s = launch_kstar(gp, xs, xe, mc, w.KS, nullptr, nullptr, w.mc_pad, w.fixlist, w.fixcount, st);
       if (s != HB_OK) return s;
-      const dim3 gf((unsigned)nt, (unsigned)(mc_pad / GT));
+      static PerDevice fix_once;
+      int64_t wave = 0;
+      s = resident_wave(vnorm_fix_kernel, fix_once, &wave);
+      if (s != HB_OK) return s;
+      const unsigned gf = (unsigned)min((int64_t)nt * (mc_pad / GT), wave);   // one resident wave walks the flagged rows
       vnorm_fix_kernel<<<gf, GTHREADS, 0, st>>>(w.KS, nullptr, gp.Linv, np, w.mc_pad, w.fixlist, w.fixcount, w.vfix, 1);
       count_launches(3);
     } else {
