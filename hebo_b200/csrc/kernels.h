@@ -151,10 +151,12 @@ int launch_posterior_mace(const Fitted &gp, const float *Xs, const int32_t *Xe_s
                           const float *xi2, uint64_t seed, float *F, float *mu, float *var, void *ws, int64_t ws_bytes,
                           int64_t m_chunk, cudaStream_t st);
 // The posterior workspace of one chunk of at most m_chunk candidates, rows padded to mc_pad = round_up(m_chunk, CHUNK_ROWS).
-// KS: fp32 K* rows (SIMT and guard passes); KS2: the fp16 two-level split h0 | h1 of the tensor path, or the V panel of the
-// gradient path, which then overwrites KS with W; mupart [groups, mc_pad]; vpart / vfix [np / GT, mc_pad]; the guard lists.
+// KS: fp32 K* rows (SIMT and guard passes); KS2[b]: the fp16 two-level split h0 | h1 of the tensor path, or (KS2[0]) the V
+// panel of the gradient path, which then overwrites KS with W; mupart[b] [groups, mc_pad]; vpart / vfix [np / GT, mc_pad];
+// the guard lists.  KS2 and mupart come twice so that the tensor path can build the K* of chunk i + 1 into one buffer while
+// chunk i is still contracted from the other (launch_posterior_mace).
 struct PostWs {
-  float *KS, *KS2, *mupart, *vpart, *vfix;
+  float *KS, *KS2[2], *mupart[2], *vpart, *vfix;
   int32_t *fixmap, *fixlist, *fixcount;
   int64_t mc_pad;
   size_t bytes;

@@ -581,14 +581,39 @@ int launch_kstar(const Fitted &gp, const float *xs, const int32_t *xe, int64_t m
   return HB_OK;
 }
 
+// The library's stream of the current device for the contraction stages of a pipelined posterior call, created once at
+// the highest priority, and the events that order it against the caller's stream.  Every call records the events
+// again; a wait orders against the record that precedes it.
+struct Pipeline {
+  cudaStream_t hi;
+  cudaEvent_t entry, kstar, started;
+};
+static int pipeline(Pipeline **out) {
+  static PerDevice once;
+  static Pipeline p[MAX_DEVICES];
+  bool fresh = false;
+  const int dev = once.slot(&fresh);
+  if (dev < 0) return HB_ERR_CUDA;
+  if (fresh) {
+    int least = 0, greatest = 0;
+    HB_CUDA(cudaDeviceGetStreamPriorityRange(&least, &greatest));
+    HB_CUDA(cudaStreamCreateWithPriority(&p[dev].hi, cudaStreamNonBlocking, greatest));
+    for (cudaEvent_t *e : {&p[dev].entry, &p[dev].kstar, &p[dev].started})
+      HB_CUDA(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    once.done[dev] = true;
+  }
+  *out = &p[dev];
+  return HB_OK;
+}
+
 PostWs carve_posterior_ws(void *ws, int64_t np, int64_t m_chunk) {
   PostWs w;
   w.mc_pad = round_up(m_chunk, CHUNK_ROWS);
   const int64_t nt = np / GT;
   Carver c{reinterpret_cast<float *>(ws)};
   w.KS = c.take(w.mc_pad * np);
-  w.KS2 = c.take(w.mc_pad * np);
-  w.mupart = c.take(kstar_groups(np) * w.mc_pad);
+  for (int b = 0; b < 2; ++b) w.KS2[b] = c.take(w.mc_pad * np);
+  for (int b = 0; b < 2; ++b) w.mupart[b] = c.take(kstar_groups(np) * w.mc_pad);
   w.vpart = c.take(nt * w.mc_pad);
   w.vfix = c.take(nt * w.mc_pad);
   w.fixmap = reinterpret_cast<int32_t *>(c.take(w.mc_pad));
@@ -609,47 +634,77 @@ int launch_posterior_mace(const Fitted &gp, const float *Xs, const int32_t *Xe_s
   if (ws_bytes < 0 || (size_t)ws_bytes < w.bytes) return HB_ERR_INVALID;
   const int nt = (int)(np / GT);
   const bool tensor = Linv_hi != nullptr && Linv_lo != nullptr;   // wgmma path (two-level fp16 split), else FP32 SIMT
-  // (Building chunk i+1 on a side stream under the tensor-core contraction of chunk i was measured and dropped: the
-  // contraction then drew ~all of the L2 -> SM bandwidth, the co-running CUDA-core kernel slowed it by 30 %.  Since the
-  // Linv multicast it draws 5/8 of those bytes per k-block; the overlap has not been measured again.)
-  for (int64_t c0 = 0; c0 < m; c0 += m_chunk) {
+  // A tensor-path call of two or more chunks is pipelined: K* of every chunk runs on the caller's stream `st`, the
+  // contraction, guard and MACE stages on the library's highest-priority stream `cs`, so that the K* of chunk i + 1 runs on
+  // the SMs the contraction of chunk i leaves free (it fills at most 30 clusters of 4 CTAs, 120 of an H100's 132 SMs, and
+  // its 193 KiB CTAs leave no room for a K* CTA beside them).  K* of chunk i + 1 waits until `cs` has reached the
+  // contraction of chunk i (event `started`), so that the contraction's clusters are dispatched before the K* CTAs can
+  // fill the SMs -- its schedule is static, one late cluster delays the whole launch -- and the stream's priority gives
+  // the guard and MACE stages the SMs as K* CTAs retire.  `started` also follows MACE of chunk i - 1, the last reader of
+  // the KS2 / mupart buffer that K* of chunk i + 1 writes (the other buffer holds chunk i).  The rest of the workspace is
+  // only touched on `cs`.  One-chunk calls and the SIMT path run everything on `st`.
+  const bool pipelined = tensor && m > m_chunk;
+  Pipeline *pl = nullptr;
+  cudaStream_t cs = st;
+  if (pipelined) {
+    const int s = pipeline(&pl);
+    if (s != HB_OK) return s;
+    cs = pl->hi;
+    HB_CUDA(cudaEventRecord(pl->entry, st));
+    HB_CUDA(cudaStreamWaitEvent(cs, pl->entry, 0));
+  }
+  auto chunk = [&](int64_t c0, int b) -> int {
     const int64_t mc = min(m_chunk, m - c0);
     const int64_t mc_pad = round_up(mc, GT);
     const float *xs = Xs + c0 * sp.d;
     const int32_t *xe = sp.e > 0 ? Xe_s + c0 * sp.e : nullptr;
-    int s = launch_kstar(gp, xs, xe, mc, w.KS, tensor ? w.KS2 : nullptr, w.mupart, w.mc_pad, nullptr, nullptr, st);
+    if (pipelined && c0 > 0) HB_CUDA(cudaStreamWaitEvent(st, pl->started, 0));
+    int s = launch_kstar(gp, xs, xe, mc, w.KS, tensor ? w.KS2[b] : nullptr, w.mupart[b], w.mc_pad, nullptr, nullptr, st);
     if (s != HB_OK) return s;
+    if (pipelined) {
+      HB_CUDA(cudaEventRecord(pl->kstar, st));
+      HB_CUDA(cudaStreamWaitEvent(cs, pl->kstar, 0));
+      HB_CUDA(cudaEventRecord(pl->started, cs));
+    }
     int nslots = nt;
     if (tensor) {
-      const __half *kh0 = reinterpret_cast<const __half *>(w.KS2), *kh1 = kh0 + w.mc_pad * np;
+      const __half *kh0 = reinterpret_cast<const __half *>(w.KS2[b]), *kh1 = kh0 + w.mc_pad * np;
       s = launch_vnorm_h16(kh0, kh1, w.mc_pad, reinterpret_cast<const __half *>(Linv_hi),
-                           reinterpret_cast<const __half *>(Linv_lo), Linv_lo + np * np / 2, gp.hyp, np, mc_pad, w.mc_pad, w.vpart, st);
+                           reinterpret_cast<const __half *>(Linv_lo), Linv_lo + np * np / 2, gp.hyp, np, mc_pad, w.mc_pad, w.vpart, cs);
       if (s != HB_OK) return s;
       nslots = (int)ceil_div(np, 128);
-      HB_CUDA(cudaMemsetAsync(w.fixcount, 0, sizeof(int32_t), st));
-      guard_kernel<<<(int)ceil_div(mc, 256), 256, 0, st>>>(w.vpart, nslots, mc, w.mc_pad, gp.hyp, GUARD_THETA, w.fixmap, w.fixlist,
+      HB_CUDA(cudaMemsetAsync(w.fixcount, 0, sizeof(int32_t), cs));
+      guard_kernel<<<(int)ceil_div(mc, 256), 256, 0, cs>>>(w.vpart, nslots, mc, w.mc_pad, gp.hyp, GUARD_THETA, w.fixmap, w.fixlist,
                                                            w.fixcount);
       // exact fp32 K* rows of the flagged candidates only (compact, row = slot), then their FP32 contraction
-      s = launch_kstar(gp, xs, xe, mc, w.KS, nullptr, nullptr, w.mc_pad, w.fixlist, w.fixcount, st);
+      s = launch_kstar(gp, xs, xe, mc, w.KS, nullptr, nullptr, w.mc_pad, w.fixlist, w.fixcount, cs);
       if (s != HB_OK) return s;
       static PerDevice fix_once;
       int64_t wave = 0;
       s = resident_wave(vnorm_fix_kernel, fix_once, &wave);
       if (s != HB_OK) return s;
       const unsigned gf = (unsigned)min((int64_t)nt * (mc_pad / GT), wave);   // one resident wave walks the flagged rows
-      vnorm_fix_kernel<<<gf, GTHREADS, 0, st>>>(w.KS, nullptr, gp.Linv, np, w.mc_pad, w.fixlist, w.fixcount, w.vfix, 1);
+      vnorm_fix_kernel<<<gf, GTHREADS, 0, cs>>>(w.KS, nullptr, gp.Linv, np, w.mc_pad, w.fixlist, w.fixcount, w.vfix, 1);
       count_launches(3);
     } else {
       const dim3 g2((unsigned)nt, (unsigned)(mc_pad / GT));
-      prof_begin(st);
-      vnorm_kernel<<<g2, GTHREADS, 0, st>>>(w.KS, gp.Linv, np, w.mc_pad, w.vpart);
-      prof_end(st);
+      prof_begin(cs);
+      vnorm_kernel<<<g2, GTHREADS, 0, cs>>>(w.KS, gp.Linv, np, w.mc_pad, w.vpart);
+      prof_end(cs);
       count_launches(2);
     }
-    mace_kernel<<<(int)ceil_div(mc, 256), 256, 0, st>>>(w.mupart, kstar_groups(np), w.vpart, nslots, tensor ? w.fixmap : nullptr,
+    mace_kernel<<<(int)ceil_div(mc, 256), 256, 0, cs>>>(w.mupart[b], kstar_groups(np), w.vpart, nslots, tensor ? w.fixmap : nullptr,
                                                         w.vfix, nt, mc, w.mc_pad, c0, rng_offset, gp.hyp, gp.y_mean, gp.y_std,
                                                         gp.pred_likeli, tau, kappa, eps, xi1, xi2, seed, F, mu, var);
+    return HB_OK;
+  };
+  int s = HB_OK;
+  for (int64_t c0 = 0, i = 0; c0 < m && s == HB_OK; c0 += m_chunk, ++i) s = chunk(c0, pipelined ? (int)(i & 1) : 0);
+  if (pipelined) {   // the caller's stream waits for the last stage (after an error too, so that nothing outlives the call)
+    HB_CUDA(cudaEventRecord(pl->entry, cs));
+    HB_CUDA(cudaStreamWaitEvent(st, pl->entry, 0));
   }
+  if (s != HB_OK) return s;
   HB_LAUNCH_CHECK("posterior_mace");
   return HB_OK;
 }

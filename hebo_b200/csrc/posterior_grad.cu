@@ -152,12 +152,12 @@ int launch_posterior_grad(const Fitted &gp, const float *Xs, const int32_t *Xe_s
   if (m <= 0 || m_chunk <= 0) return HB_ERR_INVALID;
   const PostWs w = carve_posterior_ws(ws, np, m_chunk);
   if (ws_bytes < 0 || (size_t)ws_bytes < w.bytes) return HB_ERR_INVALID;
-  float *V = w.KS2, *W = w.KS;   // W overwrites K* once V is built
+  float *V = w.KS2[0], *W = w.KS;   // W overwrites K* once V is built
   const size_t dyn = (2 * (size_t)d + sp.De) * sizeof(float);
   for (int64_t c0 = 0; c0 < m; c0 += m_chunk) {
     const int64_t mc = min(m_chunk, m - c0);
     const int64_t mc_pad = round_up(mc, GT);
-    int s = launch_kstar(gp, Xs + c0 * d, sp.e > 0 ? Xe_s + c0 * sp.e : nullptr, mc, w.KS, nullptr, w.mupart, w.mc_pad, nullptr,
+    int s = launch_kstar(gp, Xs + c0 * d, sp.e > 0 ? Xe_s + c0 * sp.e : nullptr, mc, w.KS, nullptr, w.mupart[0], w.mc_pad, nullptr,
                          nullptr, st);
     if (s != HB_OK) return s;
     const dim3 g((unsigned)(np / GT), (unsigned)(mc_pad / GT));
@@ -165,7 +165,7 @@ int launch_posterior_grad(const Fitted &gp, const float *Xs, const int32_t *Xe_s
     rows_gemm_kernel<1><<<g, GTHREADS, 0, st>>>(V, gp.Linv, np, W);
     s = with_kernel(gp.kern, sp.e > 0, [&](auto kk, auto ee) {
       post_grad_kernel<decltype(kk)::value, decltype(ee)::value><<<(unsigned)mc, 256, dyn, st>>>(
-          Xs, (int)d, gp.x_mul, gp.x_add, gp.Zt, gp.alpha, gp.hyp, gp.n, np, V, W, w.mupart, kstar_groups(np), w.mc_pad, c0,
+          Xs, (int)d, gp.x_mul, gp.x_add, gp.Zt, gp.alpha, gp.hyp, gp.n, np, V, W, w.mupart[0], kstar_groups(np), w.mc_pad, c0,
           gp.y_mean, gp.y_std, gp.pred_likeli, mu, var, dmu, dvar, Xe_s, gp.tab_s, sp);
     });
     if (s != HB_OK) return s;

@@ -209,6 +209,13 @@ static bool make_map(CUtensorMap *m, const __half *ptr, uint64_t rows, uint64_t 
 // ---- host side: schedule tables (device-resident, built once per shape and device) and the launcher
 namespace h16 {
 
+// The most clusters a contraction launch takes; the SMs it leaves free run the next chunk's K* (posterior.cu).  30 is
+// all that fit on a 132-SM H100 SXM.  Capping at 28 or 26 to give K* more SMs measured slower: scoring step 12.03 / 11.94
+// ms at 30, 12.41 / 12.37 at 28, 12.44 / 12.55 at 26 (bench.py, two runs each; H100 80GB HBM3, 700 W power limit, power-
+// capped at ~1.55-1.6 GHz): the contraction lost time in proportion to its SMs (2.60, 2.80, 2.93 ms per launch) while
+// the K* it let run alongside gained less.
+constexpr int MAX_CLUSTERS = 30;
+
 struct SchedEntry {
   int32_t *dev = nullptr;
   int len = 0;
@@ -287,7 +294,7 @@ int launch_vnorm_h16(const __half *ks_h0, const __half *ks_h1, int64_t ks_rows, 
   const int n_rt = (int)(mc_pad / BM);
   const int n_j = (int)ceil_div(np, BN);
   const int units = (int)(rows / BM / CLUSTER) * n_j;
-  const int clusters = std::min(once.aux[dev], units);
+  const int clusters = std::min({once.aux[dev], units, MAX_CLUSTERS});
   const SchedEntry *sc = get_schedule(dev, (int)np, n_rt, clusters, st);
   if (!sc) {
     set_error(cudaErrorMemoryAllocation, "vnorm_h16 schedule table");
