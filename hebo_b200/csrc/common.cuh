@@ -175,8 +175,8 @@ __device__ __forceinline__ double warp_sum_d(double v) {
   return v;
 }
 
-// ---- Philox4x32-10 + Box-Muller: two N(0,1) draws per 64-bit counter `row` (the MACE epilogue's production noise and
-// the in-kernel draws of hb_sample_y_batch)
+// ---- Philox4x32-10 (Salmon et al. 2011; cuRAND's curand_Philox4x32_10), the one generator of every device draw: the
+// Box-Muller pairs below and the NSGA-II operators (nsga.cu).  oracle/rng_oracle.py restates it and its known answers.
 __device__ __forceinline__ void philox_round(uint32_t (&c)[4], uint32_t k0, uint32_t k1) {
   const uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u;
   const uint32_t hi0 = __umulhi(M0, c[0]), lo0 = M0 * c[0];
@@ -184,9 +184,8 @@ __device__ __forceinline__ void philox_round(uint32_t (&c)[4], uint32_t k0, uint
   const uint32_t n0 = hi1 ^ c[1] ^ k0, n1 = lo1, n2 = hi0 ^ c[3] ^ k1, n3 = lo0;
   c[0] = n0; c[1] = n1; c[2] = n2; c[3] = n3;
 }
-// stream: the upper half of the 128-bit Philox counter (0 for the MACE epilogue and hb_sample_y_batch)
-__device__ __forceinline__ void philox_normal2(uint64_t seed, uint64_t row, uint64_t stream, float &z0, float &z1) {
-  uint32_t c[4] = {(uint32_t)row, (uint32_t)(row >> 32), (uint32_t)stream, (uint32_t)(stream >> 32)};
+// the 128-bit counter c is replaced by its block under the 64-bit key `seed`
+__device__ __forceinline__ void philox4x32_10(uint32_t (&c)[4], uint64_t seed) {
   uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
 #pragma unroll
   for (int r = 0; r < 10; ++r) {
@@ -194,8 +193,19 @@ __device__ __forceinline__ void philox_normal2(uint64_t seed, uint64_t row, uint
     k0 += 0x9E3779B9u;
     k1 += 0xBB67AE85u;
   }
-  const float u0 = ((float)c[0] + 0.5f) * 2.3283064365386963e-10f;   // (0,1)
-  const float u1 = ((float)c[1] + 0.5f) * 2.3283064365386963e-10f;
+}
+// a 32-bit word -> u = (c + 1/2) 2^-32 in fp32.  (float)c rounds to nearest, so a word >= 0xFFFFFF80 gives u = 1 exactly
+// (probability 2^-25); every consumer is written to take u = 1
+__device__ __forceinline__ float philox_uniform(uint32_t c) { return ((float)c + 0.5f) * 2.3283064365386963e-10f; }
+
+// ---- Box-Muller: two N(0,1) draws per 64-bit counter `row` (the MACE epilogue's production noise and the in-kernel
+// draws of hb_sample_y_batch)
+// stream: the upper half of the 128-bit Philox counter (0 for the MACE epilogue and hb_sample_y_batch)
+__device__ __forceinline__ void philox_normal2(uint64_t seed, uint64_t row, uint64_t stream, float &z0, float &z1) {
+  uint32_t c[4] = {(uint32_t)row, (uint32_t)(row >> 32), (uint32_t)stream, (uint32_t)(stream >> 32)};
+  philox4x32_10(c, seed);
+  const float u0 = philox_uniform(c[0]);   // (0, 1]: u0 = 1 gives z0 = z1 = 0
+  const float u1 = philox_uniform(c[1]);
   const float rad = sqrtf(-2.0f * logf(u0));
   float sn, cs;
   sincospif(2.0f * u1, &sn, &cs);

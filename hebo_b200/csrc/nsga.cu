@@ -17,21 +17,13 @@
 
 namespace hb {
 
+// four uniforms in (0, 1] from one Philox block (philox4x32_10, common.cuh).  Counter layouts, all keyed by `seed`:
+// init (p, 0xFFFFFFFF, k, 1), mating parents (t, gen, 0xFFFFFFF0, 2), mating column k (t, gen, k, 3) and (t, gen, k, 4)
 __device__ __forceinline__ void philox4(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint64_t seed, float (&u)[4]) {
   uint32_t c[4] = {c0, c1, c2, c3};
-  uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
-  const uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u;
+  philox4x32_10(c, seed);
 #pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    const uint32_t hi0 = __umulhi(M0, c[0]), lo0 = M0 * c[0];
-    const uint32_t hi1 = __umulhi(M1, c[2]), lo1 = M1 * c[2];
-    const uint32_t n0 = hi1 ^ c[1] ^ k0, n1 = lo1, n2 = hi0 ^ c[3] ^ k1, n3 = lo0;
-    c[0] = n0; c[1] = n1; c[2] = n2; c[3] = n3;
-    k0 += 0x9E3779B9u;
-    k1 += 0xBB67AE85u;
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) u[i] = ((float)c[i] + 0.5f) * 2.3283064365386963e-10f;   // (0, 1)
+  for (int i = 0; i < 4; ++i) u[i] = philox_uniform(c[i]);
 }
 
 __device__ __forceinline__ float repair(float v, int kind, float lo, float hi, float fixed) {
