@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "lib", "libhebo_b200.so")
 
 HB_OK, HB_ERR_INVALID, HB_ERR_NOT_PD, HB_ERR_CUDA = 0, 1, 2, 3
-KERNEL_IDS = {"matern32": 0, "matern52": 1, "rbf": 2}
+KERNEL_IDS = {"matern32": 0, "matern52": 1, "rbf": 2, "matern12": 4}   # HB_KERN_* of include/hebo_b200.h
 HB_ACQ1_LCB, HB_ACQ1_MEAN, HB_ACQ1_SIGMA, HB_ACQ1_ABS_ETA = 0, 1, 2, 3   # hb_acq1_epilogue modes
 HB_MAX_FEATURES = 4096   # d + sum(emb_sizes) a model may have (include/hebo_b200.h)
 HB_MAX_OUTPUTS = 32      # outputs one batched fit trains together (hb_fit_multi_ex)

@@ -315,7 +315,7 @@ template <class Attempt> static int jitter_ladder(Attempt &&attempt, float &jitt
 static int open_fit_ws(const float *Xt, const int32_t *Xe, const float *y, int64_t n, int64_t d, const hb_model_spec_t *spec,
                        const float *raw, int32_t kern, void *ws, int64_t ws_bytes, int64_t num_out, cudaStream_t st,
                        ModelSpec &sp, FitWs &w) {
-  if (!y || !raw || !ws || n <= 0 || kern < 0 || kern > 2 || !build_spec(d, spec, sp) || (sp.d > 0 && !Xt)) return HB_ERR_INVALID;
+  if (!y || !raw || !ws || n <= 0 || !kern_known(kern) || !build_spec(d, spec, sp) || (sp.d > 0 && !Xt)) return HB_ERR_INVALID;
   w = carve_fit(ws, n, sp);
   if (ws_bytes / num_out < (int64_t)w.total) return HB_ERR_INVALID;
   if (sp.e <= 0) return HB_OK;
@@ -742,7 +742,7 @@ static bool open_fitted(const float *Xs, const int32_t *Xe_s, int64_t n, int64_t
                         const float *alpha, const float *Linv, const float *hyp, int32_t kern, float y_mean, float y_std,
                         int32_t pred_likeli, Fitted &gp) {
   ModelSpec sp;
-  if (!build_spec(d, spec, sp) || n <= 0 || kern < 0 || kern > 2) return false;
+  if (!build_spec(d, spec, sp) || n <= 0 || !kern_known(kern)) return false;
   if ((sp.d > 0 && (!Xs || !x_mul || !x_add)) || !Zt || !alpha || !Linv || !hyp) return false;
   if (sp.e > 0 && (!Xe_s || !emb_meta || !tab_s)) return false;
   bind_meta(sp, emb_meta, nullptr);

@@ -58,8 +58,13 @@ template <class F> int with_kernel(int kern, F &&f) {
     case HB_KERN_MATERN32: f(std::integral_constant<int, HB_KERN_MATERN32>{}); return HB_OK;
     case HB_KERN_MATERN52: f(std::integral_constant<int, HB_KERN_MATERN52>{}); return HB_OK;
     case HB_KERN_RBF:      f(std::integral_constant<int, HB_KERN_RBF>{}); return HB_OK;
+    case HB_KERN_MATERN12: f(std::integral_constant<int, HB_KERN_MATERN12>{}); return HB_OK;
     default: return HB_ERR_INVALID;
   }
+}
+// the ids with_kernel dispatches: the argument checks of the entry points that validate kern before any launch
+inline bool kern_known(int kern) {
+  return kern == HB_KERN_MATERN32 || kern == HB_KERN_MATERN52 || kern == HB_KERN_RBF || kern == HB_KERN_MATERN12;
 }
 // ... and f(kk, ee) for kernels templated on <KERN, EMB> as well, ee = std::bool_constant<emb>
 template <class F> int with_kernel(int kern, bool emb, F &&f) {
@@ -70,17 +75,24 @@ template <class F> int with_kernel(int kern, bool emb, F &&f) {
 }
 
 // ---------------------------------------------------------------- stationary kernels
-// k(r2) with unit outputscale.  KERN: 0 Matern-3/2, 1 Matern-5/2, 2 RBF (gpytorch MaternKernel/RBFKernel).
+// k(r2) with unit outputscale.  KERN: 0 Matern-3/2, 1 Matern-5/2, 2 RBF, 4 Matern-1/2 (gpytorch MaternKernel/RBFKernel).
 // The radius and the exponential go through the SFU (MUFU.RSQ / MUFU.EX2: r = r2 * rsqrt(r2), exp(x) = ex2(x log2 e),
 // both ~2 ulp): the absolute error of k at the r2 it receives stays below 3e-7, about four fp32 ulp of k ~ 1 (largest
 // measured 2.4e-7, Matern-5/2 near k ~ 1, on an H100; tests/test_gpu_fit_state.py), and the per-pair instruction count of the K* / Gram builders drops by about a third compared
 // with the IEEE sqrtf / expf sequences.  gram_kernel and kstar_kernel share these functions, so a candidate that
 // duplicates a training row reproduces that row of K bit for bit (r2 = 0 gives k = 1 exactly).
-__device__ __forceinline__ float fast_radius(float r2) {
-  const float c = fmaxf(r2, 1e-30f);   // gpytorch: sqrt(clamp_min(sq_dist, 1e-30))
+// Matern-1/2, k = e^-r: the relative error of the radius (about 2^-22) moves k by at most 2^-22 r e^-r <= 2^-22 / e ~ 9e-8,
+// the rounding of the ex2 argument by at most 1.25 2^-24 r e^-r ~ 3e-8, and ex2 adds 2 ulp of k (2.4e-7 at k ~ 1, 0.9e-7
+// at r = 1), so the absolute error of k stays below 3e-7 as well (largest measured 1.1e-7, on an H100 at a 700 W power
+// limit; tests/test_gpu_matern12.py).
+__device__ __forceinline__ float fast_rsqrt(float c) {
   float q;
   asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(q) : "f"(c));   // c >= 1e-30 is a normal number: ftz changes nothing
-  return c * q;
+  return q;
+}
+__device__ __forceinline__ float fast_radius(float r2) {
+  const float c = fmaxf(r2, 1e-30f);   // gpytorch: sqrt(clamp_min(sq_dist, 1e-30))
+  return c * fast_rsqrt(c);
 }
 // exp(x) for x <= 0 as ex2(x log2 e); results below 2^-126 flush to zero (k ~ 1e-38 is zero for every purpose here)
 __device__ __forceinline__ float fast_exp(float x) {
@@ -92,6 +104,7 @@ template <int KERN>
 __device__ __forceinline__ float kern_eval(float r2) {
   if (KERN == HB_KERN_RBF) return fast_exp(-0.5f * r2);
   const float r = fast_radius(r2);
+  if (KERN == HB_KERN_MATERN12) return fast_exp(-r);
   if (KERN == HB_KERN_MATERN32) {
     const float a = 1.7320508075688772f;
     float ar = a * r;
@@ -104,12 +117,21 @@ __device__ __forceinline__ float kern_eval(float r2) {
 }
 
 // k and the radial factor h with  dk/dl_k = h * dz_k^2 / l_k  (dz = lengthscale-scaled difference),
-// SURVEY Appendix A.
+// SURVEY Appendix A.  Matern-1/2: h = e^-r / r is singular at r = 0; below the clamp (r2 < 1e-30) gpytorch's clamp_min
+// passes no gradient, so h = 0 there.  The clamped value (h ~ 1e15) would be harmless in the lengthscale terms
+// (h dz^2 <= r), but the posterior input gradient (h dz / l) and the warp-exponent terms (h dz (dZa - dZa')) of a pair
+// with 0 < r2 < 1e-30 would get a value of order 1 where autograd gives 0.
 template <int KERN>
 __device__ __forceinline__ void kern_eval_grad(float r2, float &k, float &h) {
   if (KERN == HB_KERN_RBF) {
     k = fast_exp(-0.5f * r2);
     h = k;
+    return;
+  }
+  if (KERN == HB_KERN_MATERN12) {
+    const float c = fmaxf(r2, 1e-30f), q = fast_rsqrt(c);   // r = c q as in fast_radius, and 1 / r = q
+    k = fast_exp(-(c * q));
+    h = c > r2 ? 0.0f : k * q;                               // c > r2 exactly when r2 < 1e-30
     return;
   }
   const float r = fast_radius(r2);

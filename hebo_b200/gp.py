@@ -7,8 +7,10 @@ sm_90a kernels of libhebo_b200.so through the C ABI -- no GPyTorch, no CPU fallb
 
 Extra conf keys (unknown keys are ignored by the reference's ``conf.get``, so they are safe to pass through
 ``HEBO(model_config=...)``):
-    kernel      'matern32' (reference default, gp_util.py:46) | 'matern52' | 'rbf'  (numeric dims; the embedding dims of a
-                mixed model always use Matern-3/2 with one lengthscale, gp_util.py:54-55)
+    kernel      'matern32' (reference default, gp_util.py:46) | 'matern52' | 'matern12' | 'rbf'  (numeric dims; the embedding
+                dims of a mixed model always use Matern-3/2 with one lengthscale, gp_util.py:54-55).  A gpytorch kernel
+                object in the reference's own key 'kern' (gp.py:201) maps by its ``nu``: 0.5, 1.5 or 2.5, the three values
+                gpytorch's MaternKernel accepts; an object without ``nu`` maps to 'rbf'
     num_uniqs / emb_sizes   categorical columns (the reference's own keys: hebo.py:99-100, layers.py:17-19)
     noise_diag  optional per-row extra noise variance [n] in *standardised* y units (BASELINE config 4)
     warp        True: Kumaraswamy input warp of the numeric dims with exponents a, b LEARNED inside the MLL (BASELINE config 3;
@@ -125,7 +127,7 @@ class GP(BaseModel):
             nu = getattr(base, "nu", None)
             if nu is None:
                 return "rbf"
-            return {1.5: "matern32", 2.5: "matern52"}[float(nu)]
+            return {0.5: "matern12", 1.5: "matern32", 2.5: "matern52"}[float(nu)]
         return "matern32"
 
     # ------------------------------------------------------------------ scaling (gp.py:51-71)

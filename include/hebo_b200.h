@@ -61,6 +61,8 @@ extern "C" {
 #define HB_KERN_MATERN32   0   /* reference default: models/gp/gp_util.py:46 (nu = 1.5) */
 #define HB_KERN_MATERN52   1   /* conf['kern'] injection, models/gp/gp.py:201            */
 #define HB_KERN_RBF        2
+#define HB_KERN_MATERN12   4   /* gpytorch MaternKernel(nu=0.5), through conf['kern'], models/gp/gp.py:201.
+                                  Ids 3 and 5-7 are not kernels: every entry point that takes kern rejects them. */
 
 /* Largest feature count d + De (numeric dims plus the summed embedding widths of the categorical columns) a model may
  * have.  Every entry point that takes a model description returns HB_ERR_INVALID above it (hb_num_params and the
