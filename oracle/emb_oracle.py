@@ -32,9 +32,7 @@ from typing import List, Tuple
 
 import torch
 
-from .gp_oracle import PSGLDState, inv_softplus, kernel_from_sqdist, psgld_step, softplus
-
-SQRT3 = math.sqrt(3.0)
+from .gp_oracle import KERNELS, PSGLDState, inv_softplus, kernel_from_sqdist, psgld_step, softplus
 
 
 def default_emb_sizes(num_uniqs: List[int]) -> List[int]:
@@ -105,20 +103,12 @@ def embed(Xe: torch.Tensor, tables: List[torch.Tensor]) -> torch.Tensor:
 
 def _phi_kind(r2: torch.Tensor, kind: str) -> Tuple[torch.Tensor, torch.Tensor]:
     """(k, h) of the numeric-dims kernel: k = kernel value, h with  dk / d r^2 = -h / 2  (SURVEY Appendix A)."""
-    if kind == "matern32":
-        return _phi(r2)
-    k = kernel_from_sqdist(r2, kind)
-    if kind == "rbf":
-        return k, k
-    a = math.sqrt(5.0)
-    r = torch.sqrt(torch.clamp_min(r2, 1e-30))
-    return k, (5.0 / 3.0) * (1.0 + a * r) * torch.exp(-a * r)
+    return kernel_from_sqdist(r2, kind), KERNELS[kind].h(r2)
 
 
 def _phi(r2: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
-    r = torch.sqrt(torch.clamp_min(r2, 1e-30))
-    e = torch.exp(-SQRT3 * r)
-    return (1.0 + SQRT3 * r) * e, 3.0 * e          # phi, h  (d phi / d r^2 = -h / 2)
+    """(phi, h) of the embedding-dims kernel, always Matern-3/2."""
+    return _phi_kind(r2, "matern32")
 
 
 def neg_mll_emb(Xt: torch.Tensor, Xe: torch.Tensor, yt: torch.Tensor, hp: EmbHypers, noise_guess: float = 0.01,

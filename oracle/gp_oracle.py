@@ -30,12 +30,11 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass, field
-from typing import Optional, Tuple
+from typing import Callable, Optional, Tuple
 
 import numpy as np
 import torch
 
-KERNELS = {"matern32": 0, "matern52": 1, "rbf": 2}
 MIN_VARIANCE_F32 = 1e-6          # gpytorch.settings.min_variance (float) -- MultivariateNormal.variance floor
 EPS_F32 = float(torch.finfo(torch.float32).eps)   # gp.py:164 clamp, acq.py:153 clamp
 
@@ -88,18 +87,66 @@ def scaled_sqdist(Z1: torch.Tensor, Z2: torch.Tensor) -> torch.Tensor:
     return (diff * diff).sum(-1)
 
 
+def _radius(r2: torch.Tensor) -> torch.Tensor:
+    """gpytorch MaternKernel's r = sqrt(clamp_min(r^2, 1e-30)); clamp_min passes no gradient below its bound."""
+    return torch.sqrt(torch.clamp_min(r2, 1e-30))
+
+
+def _matern12(r2):
+    return torch.exp(-_radius(r2))
+
+
+def _matern12_h(r2):
+    """e^-r / r is singular at r = 0; autograd through the clamp gives h = 0 below it, so a pair of equal rows
+    contributes nothing to any gradient."""
+    r = _radius(r2)
+    return torch.where(r2 < 1e-30, torch.zeros_like(r2), torch.exp(-r) / r)
+
+
+def _matern32(r2):
+    a, r = math.sqrt(3.0), _radius(r2)
+    return (1.0 + a * r) * torch.exp(-a * r)
+
+
+def _matern32_h(r2):
+    a, r = math.sqrt(3.0), _radius(r2)
+    return a * a * torch.exp(-a * r)
+
+
+def _matern52(r2):
+    a, r = math.sqrt(5.0), _radius(r2)
+    return (1.0 + a * r + (5.0 / 3.0) * r2) * torch.exp(-a * r)
+
+
+def _matern52_h(r2):
+    a, r = math.sqrt(5.0), _radius(r2)
+    return (a * a / 3.0) * (1.0 + a * r) * torch.exp(-a * r)
+
+
+def _rbf(r2):
+    return torch.exp(-0.5 * r2)
+
+
+@dataclass(frozen=True)
+class Kernel:
+    """One covariance kernel at unit outputscale as a function of the scaled squared distance r^2."""
+    id: int                # HB_KERN_* of include/hebo_b200.h
+    k: Callable[[torch.Tensor], torch.Tensor]
+    h: Callable[[torch.Tensor], torch.Tensor]      # radial factor, dk/dr^2 = -h / 2 (SURVEY Appendix A)
+
+
+# gpytorch MaternKernel(nu = 0.5, 1.5, 2.5).forward and RBFKernel.  The Matern-3/2 and -5/2 h keep a * a rather than 3:
+# the committed fixtures were computed with it.
+KERNELS = {
+    "matern32": Kernel(0, _matern32, _matern32_h),
+    "matern52": Kernel(1, _matern52, _matern52_h),
+    "rbf": Kernel(2, _rbf, _rbf),
+    "matern12": Kernel(4, _matern12, _matern12_h),
+}
+
+
 def kernel_from_sqdist(r2: torch.Tensor, kind: str) -> torch.Tensor:
-    """Matern-3/2, Matern-5/2 (gpytorch MaternKernel.forward) and RBF, unit outputscale."""
-    if kind == "rbf":
-        return torch.exp(-0.5 * r2)
-    r = torch.sqrt(torch.clamp_min(r2, 1e-30))
-    if kind == "matern32":
-        a = math.sqrt(3.0)
-        return (1.0 + a * r) * torch.exp(-a * r)
-    if kind == "matern52":
-        a = math.sqrt(5.0)
-        return (1.0 + a * r + (5.0 / 3.0) * r2) * torch.exp(-a * r)
-    raise ValueError(kind)
+    return KERNELS[kind].k(r2)
 
 
 KERNEL_FORM = "direct"   # "direct": sum((zi-zj)^2), used for parity; "mm": gpytorch's matmul form, used by the
@@ -272,16 +319,7 @@ def neg_mll_closed_form(Xt, yt, hp: Hypers, kind="matern32", noise_guess=0.01, n
     logdet = 2.0 * torch.log(torch.diagonal(L)).sum()
     W = torch.outer(alpha, alpha) - Kinv
     # radial derivative factor  h(r) with dk/dl_k = h * dz_k^2 / l_k   (dz = scaled difference)
-    r = torch.sqrt(torch.clamp_min(r2, 1e-30))
-    if kind == "matern32":
-        a = math.sqrt(3.0)
-        h = a * a * torch.exp(-a * r)
-    elif kind == "matern52":
-        a = math.sqrt(5.0)
-        h = (a * a / 3.0) * (1.0 + a * r) * torch.exp(-a * r)
-    else:
-        h = k
-    G = W * h * s                                            # [n,n]
+    G = W * KERNELS[kind].h(r2) * s                          # [n,n]
     g_ls = torch.zeros(d, dtype=dt)
     for i0 in range(0, n, block):
         dZ2 = (Z[i0:i0 + block, None, :] - Z[None, :, :]) ** 2   # [block,n,d]

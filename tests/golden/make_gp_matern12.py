@@ -4,7 +4,7 @@ repeats rows.
     python tests/golden/make_gp_matern12.py
 
 Reduced config: Ackley in 5 dimensions, n = 112 of which the last 12 rows repeat the first 12 (r^2 = 0 pairs), 256
-candidates, q = 4, seed 1240.  The Matern-1/2 oracle (tests/matern12_oracle.py) is installed for the call.
+candidates, q = 4, seed 1240.
 Test infrastructure; never imported by hebo_b200/.
 """
 from __future__ import annotations
@@ -18,7 +18,6 @@ if ROOT not in sys.path:
 
 from oracle import gp_oracle as O          # noqa: E402
 from oracle import make_golden             # noqa: E402
-from tests import matern12_oracle as M     # noqa: E402
 
 REPEATS = 12
 
@@ -32,8 +31,7 @@ def main():
         return X, y
     O.synthetic_problem = with_repeats
     try:
-        with M.installed():
-            make_golden.gen_gp(M.KIND, "ackley", 112, 5, 256, 4, M.KIND, 1240)
+        make_golden.gen_gp("matern12", "ackley", 112, 5, 256, 4, "matern12", 1240)
     finally:
         O.synthetic_problem = problem
     print("wrote", os.path.join(make_golden.OUT, "gp_matern12.npz"))

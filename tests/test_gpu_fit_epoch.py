@@ -147,7 +147,7 @@ def run_multi(m, Y, raws, E=1, lr=0.0, fill=0, XtT=None):
     return out, stride
 
 
-def run_simt(m, raw=None, fill=0, XtT=None):
+def run_simt(m, raw=None, fill=0, XtT=None, noise_diag=None):
     """hb_mll_fwd_bwd: one loss + gradient on the FP32 SIMT path."""
     lib = _lib.lib()
     wsb = int(lib.hb_fit_workspace_bytes_ex(m.n, m.d, m.spec))
@@ -157,8 +157,8 @@ def run_simt(m, raw=None, fill=0, XtT=None):
     loss = torch.full((1,), float("nan"), device="cuda")
     info = torch.full((1,), -7, dtype=torch.int32, device="cuda")
     _lib.check(lib.hb_mll_fwd_bwd(_lib.ptr(m.XtT if XtT is None else XtT), _lib.ptr(m.Xe), _lib.ptr(m.y), m.n, m.d, m.spec,
-                                  _lib.ptr(r), m.kern, None, NOISE_LB, m.noise_guess, 0.0, _lib.ptr(grad), _lib.ptr(loss),
-                                  _lib.ptr(info), _lib.ptr(ws), wsb, _lib.stream_ptr()), "hb_mll_fwd_bwd")
+                                  _lib.ptr(r), m.kern, _lib.ptr(noise_diag), NOISE_LB, m.noise_guess, 0.0, _lib.ptr(grad),
+                                  _lib.ptr(loss), _lib.ptr(info), _lib.ptr(ws), wsb, _lib.stream_ptr()), "hb_mll_fwd_bwd")
     torch.cuda.synchronize()
     assert int(info.item()) == 0
     st = _state(m, ws)
@@ -183,9 +183,10 @@ def run_factorize(m, raw=None, fill=0, XtT=None):
 
 
 # ---------------------------------------------------------------------------------------------- references
-def ref_numeric(m, raw, kind, dtype):
+def ref_numeric(m, raw, kind, dtype, noise_diag=None):
     hp = O.Hypers.unpack(raw.to(dtype), NOISE_LB)
-    loss, grad, _ = O.neg_mll_closed_form(m.Xt64().to(dtype), m.y64().to(dtype), hp, kind, m.noise_guess)
+    nd = None if noise_diag is None else noise_diag.to(dtype).cpu()
+    loss, grad, _ = O.neg_mll_closed_form(m.Xt64().to(dtype), m.y64().to(dtype), hp, kind, m.noise_guess, nd)
     return float(loss), grad.double()
 
 
@@ -207,8 +208,8 @@ def tc_at(m, raw):
     return float(r["losses"][0]), r["grad"]
 
 
-def simt_at(m, raw):
-    r = run_simt(m, raw)
+def simt_at(m, raw, noise_diag=None):
+    r = run_simt(m, raw, noise_diag=noise_diag)
     return float(r["loss"][0]), r["grad"]
 
 
@@ -236,16 +237,16 @@ FAMILIES = {
 }
 
 
-def _family_ref(name, m, raw, dtype):
+def _family_ref(name, m, raw, dtype, kind="matern32"):
     Xt, y = m.Xt64().to(dtype), m.y64().to(dtype)
     if name == "learned_warp":
-        loss, g = W.neg_mll_autograd(Xt, y, raw.to(dtype), NOISE_LB, "matern32", m.noise_guess)
+        loss, g = W.neg_mll_autograd(Xt, y, raw.to(dtype), NOISE_LB, kind, m.noise_guess)
         return float(loss), g.double()
     Xe = m.Xe.long().cpu() if m.Xe is not None else torch.zeros(m.n, 0, dtype=torch.long)
     hp = emb_hypers(m.owner, raw)
     hp = E.EmbHypers(*(v.to(dtype) if torch.is_tensor(v) else [t.to(dtype) for t in v] if isinstance(v, list) else v
                        for v in (hp.raw_noise, hp.tables, hp.mean, hp.raw_os, hp.raw_ls, hp.raw_ls_e, hp.noise_lb)))
-    loss, g = E.neg_mll_emb_closed_form(Xt, Xe, y, hp, m.noise_guess)
+    loss, g = E.neg_mll_emb_closed_form(Xt, Xe, y, hp, m.noise_guess, kind=kind)
     return float(loss), g.double()
 
 

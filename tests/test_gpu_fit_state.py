@@ -7,12 +7,13 @@ launch_linv_refine (one Newton step) -> fp16 split -> launch_solve_logdet -> sca
 the element-wise absolute value and |A||B| an fp64 matrix product of absolute values.  Each case prints the c it needs
 (max |error| / bound) and requires c <= C_MAX.
 
-1. hb_gram (numeric ARD features, all three kernels), n = 5 ... 4097 (NP up to 4224) and d = 1 ... 300 across the
+1. hb_gram (numeric ARD features, all four kernels), n = 5 ... 4097 (NP up to 4224) and d = 1 ... 300 across the
    32-wide feature chunks:
    - the kernel function itself: with s = 1, K_ij against k64(r^_ij^2), where r^^2 is the fp32 squared distance exactly
      as accum_sqdist forms it (df = fl(z_i - z_j), r2 = fma(df, df, r2) in feature order, emulated in fp64 with a
      rounding to fp32 per step) on the kernel's own fp32 features z = fl(Xt fl(1 / l)) (stage4).  Bound u eps_k:
        RBF        eps_k = k (E_EX2 + 1.25 t)
+       Matern-1/2 eps_k = k (E_EX2 + 1.25 t) + t e^-t (E_RSQ + 1.5)
        Matern-3/2 eps_k = k (E_EX2 + 1.25 t + 2) + t^2 e^-t (E_RSQ + 2.5)
        Matern-5/2 eps_k = k (E_EX2 + 1.25 t + 3.5) + t (t + t^2 / 3) e^-t (E_RSQ + 2.5)
      with t the exponent of fast_exp (kernel_parts).  E_EX2 = 4: ex2.approx.ftz.f32 is accurate to 2 ulp of its result
@@ -20,9 +21,10 @@ the element-wise absolute value and |A||B| an fp64 matrix product of absolute va
      rounding), i.e. 1.22 |x| u relative on exp(x), taken as 1.25 t.  E_RSQ = 2^-22.9 / u: rsqrt.approx.f32 (PTX ISA); r =
      c q and a r add one rounding each and a = fl(sqrt 3 | sqrt 5) half of one, so the exponent a r carries
      (E_RSQ + 2.5) u relative, which moves k by |dk/dt| t (E_RSQ + 2.5) u: t^2 e^-t for Matern-3/2, and for Matern-5/2,
-     whose r^2 term does not go through the radius, (t + t^2 / 3) e^-t t.  The last terms of the k factor are the
-     roundings of 1 + a r, (5/3) r^2, their sum and the product with the exponential.  Plus 2^-102 (results below
-     2^-126 flush to zero).  The largest |K - k64(r^^2)| is also checked against K_ABS = 3e-7, the absolute accuracy
+     whose r^2 term does not go through the radius, (t + t^2 / 3) e^-t t.  Matern-1/2 has t = r and no constant a: the
+     radius (E_RSQ and one rounding) moves k by |dk/dt| t = t e^-t times its relative error.  The last terms of the k
+     factor are the roundings of 1 + a r, (5/3) r^2, their sum and the product with the exponential.  Plus 2^-102
+     (results below 2^-126 flush to zero).  The largest |K - k64(r^^2)| is also checked against K_ABS = 3e-7, the absolute accuracy
      common.cuh states for k (largest measured 2.4e-7, Matern-5/2 near k ~ 1).
    - the Gram: |K - s k64(r^2)| <= s (h (d + 2) u r^2 / 2 + u eps_k) + u |K|, r^2 in fp64 from the same fp32 features:
      the direct-difference sum has non-negative terms, so its relative error is at most (d + 2) u (d accumulations, the
@@ -134,6 +136,8 @@ def eps_k(r2, kind):
     if kind == "rbf":
         return k * (E_EX2 + 1.25 * t) + FLUSH
     e = torch.exp(-t)
+    if kind == "matern12":
+        return k * (E_EX2 + 1.25 * t) + t * e * (E_RSQ + 1.5) + FLUSH
     if kind == "matern32":
         return k * (E_EX2 + 1.25 * t + 2) + t * t * e * (E_RSQ + 2.5) + FLUSH
     return k * (E_EX2 + 1.25 * t + 3.5) + t * (t + t * t / 3) * e * (E_RSQ + 2.5) + FLUSH
@@ -300,7 +304,7 @@ def gram_inputs(n, d, seed):
 
 @pytest.mark.parametrize("n,d", GRAM_SHAPES)
 def test_gram_per_element(n, d):
-    """hb_gram for the three kernels against k64 of the kernel's own fp32 features (docstring 1.)."""
+    """hb_gram for the four kernels against k64 of the kernel's own fp32 features (docstring 1.)."""
     Xt, ls, nd = gram_inputs(n, d, seed=1000 * d + n)
     NP = Xt.shape[1]
     inv = (np.float32(1.0) / ls.numpy().astype(np.float32)).astype(np.float32)          # fl(1 / l), IEEE
@@ -314,7 +318,7 @@ def test_gram_per_element(n, d):
     eye = torch.eye(NP, device=DEV)
     configs = [dict(s=1.0, sn2=1e-3, jitter=0.0, nd=None), dict(s=2.7, sn2=0.013, jitter=1e-5, nd=nd),
                dict(s=0.31, sn2=8e-4, jitter=1e-4, nd=None)]
-    for kind in ("matern32", "matern52", "rbf"):
+    for kind in ("matern32", "matern52", "rbf", "matern12"):
         kk = k64(r2, kind)
         kh = k64(r2h, kind)
         worst_abs = 0.0

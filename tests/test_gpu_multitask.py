@@ -24,6 +24,9 @@ FAMILIES = {
     "mixed": (3, 250, 3, {"num_uniqs": [4, 3]}),
     "learned_warp": (4, 230, 2, {"warp": True}),
     "fixed_warp": (3, 220, 2, {"warp_a": [0.7, 1.3, 2.0], "warp_b": [1.5, 0.8, 1.1]}),
+    "matern12": (4, 260, 3, {"kernel": "matern12"}),
+    "matern12_mixed": (3, 250, 2, {"kernel": "matern12", "num_uniqs": [4, 3]}),
+    "matern12_learned_warp": (4, 230, 2, {"kernel": "matern12", "warp": True}),
 }
 
 
@@ -106,7 +109,7 @@ def test_batched_fit_equals_per_output_fits(family, epochs):
     d, n, B, conf = FAMILIES[family]
     e = conf.get("num_uniqs", [])
     mt, singles, X, Xe, batched = _fit_both(d, e, n, B, conf, epochs)
-    assert batched
+    assert batched and all(g.kernel == conf.get("kernel", "matern32") for g in mt.models)
     _assert_equal_models(mt, singles, X, Xe)
 
 

@@ -24,7 +24,7 @@ from tests.util import assert_mace_close, load_golden, mu_sigma_errors, oracle_p
 
 pytestmark = pytest.mark.gpu
 
-GP_CASES = ["c1_branin", "c2_ackley", "c3_hartmann_warp", "c4_hetero", "rbf"]
+GP_CASES = ["c1_branin", "c2_ackley", "c3_hartmann_warp", "c4_hetero", "rbf", "matern12"]
 
 
 def _gp_from_golden(g, **extra):

@@ -25,7 +25,7 @@ def _setup(n, d, kernel="matern32", **conf):
     return gp, X, y, Xt, yt
 
 
-@pytest.mark.parametrize("n,d,kernel", [(300, 4, "matern32"), (260, 7, "matern52"), (200, 3, "rbf")])
+@pytest.mark.parametrize("n,d,kernel", [(300, 4, "matern32"), (260, 7, "matern52"), (200, 3, "rbf"), (260, 5, "matern12")])
 def test_learned_warp_loss_gradient_trajectory_posterior(n, d, kernel):
     gp, X, y, Xt, yt = _setup(n, d, kernel, warp=True)
     P = 3 + 3 * d

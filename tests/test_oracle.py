@@ -9,7 +9,7 @@ import torch
 from oracle import gp_oracle as O
 from tests.util import load_golden
 
-GP_CASES = ["c1_branin", "c2_ackley", "c3_hartmann_warp", "c4_hetero", "rbf"]
+GP_CASES = ["c1_branin", "c2_ackley", "c3_hartmann_warp", "c4_hetero", "rbf", "matern12"]
 
 
 def test_mace_restatement_matches_reference_vectors():

@@ -1,6 +1,6 @@
-"""Matern-1/2 (gpytorch MaternKernel(nu=0.5)), CPU only: the fp64 oracle extended by tests/matern12_oracle.py -- its
-closed-form MLL gradient against autograd on data with exact duplicate rows, the committed fixture -- the host's kernel
-mapping and the ABI's kernel-id checks."""
+"""Matern-1/2 (gpytorch MaternKernel(nu=0.5)), CPU only: the fp64 oracle's Matern-1/2 -- its closed-form MLL gradient
+against autograd on data with exact duplicate rows, the committed fixture -- the host's kernel mapping and the ABI's
+kernel-id checks."""
 import ctypes
 import os
 
@@ -11,18 +11,11 @@ import torch
 from hebo_b200 import _lib
 from oracle import emb_oracle as E
 from oracle import gp_oracle as O
-from tests import matern12_oracle as M
-from tests import test_oracle as TO
 from tests import test_posterior_grad_host as PG
 from tests import test_posterior_mace_host as PM
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BAD_IDS = (-1, 3, 5, 6, 7)
-
-
-@pytest.fixture(autouse=True)
-def _matern12_oracle(monkeypatch):
-    M.install(monkeypatch)
 
 
 def _with_duplicates(X, k=6):
@@ -36,21 +29,12 @@ def _close(ga, gc):
     return float((ga - gc).abs().max()) < 1e-10 * max(1.0, float(ga.abs().max()))
 
 
-def test_other_kernels_are_the_oracle_own():
-    """Installed, the extension leaves every other kind to oracle/'s own functions, which do not know Matern-1/2."""
-    r2 = torch.rand(6, 6, generator=torch.Generator().manual_seed(3), dtype=torch.float64)
-    for kind in ("matern32", "matern52", "rbf"):
-        assert torch.equal(O.kernel_from_sqdist(r2, kind), M._kernel_from_sqdist(r2, kind))
-    with pytest.raises(ValueError):
-        M._kernel_from_sqdist(r2, "matern12")
-
-
 def test_kernel_value_and_radial_factor():
     r2 = torch.tensor([0.0, 1e-31, 1e-30, 0.25, 4.0], dtype=torch.float64)
     k = O.kernel_from_sqdist(r2, "matern12")
     assert float(k[0]) == float(torch.exp(torch.tensor(-1e-15, dtype=torch.float64)))
     assert torch.allclose(k[3:], torch.exp(-r2[3:].sqrt()), rtol=0, atol=1e-16)
-    h = M.matern12_h(r2)
+    h = O.KERNELS["matern12"].h(r2)
     assert float(h[0]) == 0.0 and float(h[1]) == 0.0                       # below the clamp: no gradient
     assert torch.allclose(h[2:], torch.exp(-r2[2:].sqrt()) / r2[2:].sqrt(), rtol=1e-15, atol=0)
 
@@ -103,12 +87,12 @@ def test_learned_warp_autograd_is_finite_with_duplicates():
     assert torch.isfinite(loss) and torch.isfinite(grad).all() and float(grad[1:1 + 2 * d].abs().max()) > 0
 
 
-def test_oracle_reproduces_the_matern12_fixture():
+def test_the_fixture_is_a_matern12_model_with_duplicate_rows():
+    """tests/golden/gp_matern12.npz, which test_oracle.py and test_gpu_parity.py check as one of their GP cases."""
     g = np.load(os.path.join(ROOT, "tests", "golden", "gp_matern12.npz"))
     assert str(g["kind"]) == "matern12"
     X = g["X"]
-    assert any((X[i] == X[j]).all() for i in range(X.shape[0]) for j in range(i))   # the fixture holds duplicate rows
-    TO.test_oracle_reproduces_gp_goldens("matern12")
+    assert any((X[i] == X[j]).all() for i in range(X.shape[0]) for j in range(i))
 
 
 def test_host_maps_nu_one_half_and_the_kernel_key():
@@ -119,7 +103,7 @@ def test_host_maps_nu_one_half_and_the_kernel_key():
 
     class Scale:
         base_kernel = Matern()
-    assert _lib.KERNEL_IDS["matern12"] == M.ID == 4
+    assert _lib.KERNEL_IDS["matern12"] == O.KERNELS["matern12"].id == 4
     assert hebo_b200.GP(2, 0, 1, kern=Scale()).kernel == "matern12"
     assert hebo_b200.GP(2, 0, 1, kern=Matern()).kern_id == 4
     assert hebo_b200.GP(3, 0, 1, kernel="matern12").kern_id == 4
@@ -133,6 +117,7 @@ def test_header_defines_the_id():
     assert {k: int(v) for k, v in defs.items()} == {"HB_KERN_MATERN32": 0, "HB_KERN_MATERN52": 1, "HB_KERN_RBF": 2,
                                                      "HB_KERN_MATERN12": 4}
     assert sorted(_lib.KERNEL_IDS.values()) == [0, 1, 2, 4]
+    assert {k: v.id for k, v in O.KERNELS.items()} == _lib.KERNEL_IDS
 
 
 def test_entry_points_reject_every_id_that_is_not_a_kernel(lib):

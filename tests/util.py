@@ -190,7 +190,8 @@ def fullsize_oracle(c, gp, X, yt, Xs, xi1, xi2, extra, dtype=torch.float64):
 # (test_gpu_posterior_grad.py, test_gpu_posterior_mace.py).  Models are cached by key for the whole session; a test
 # that changes a model's hypers fits its own key.
 DEV = torch.device("cuda")
-RATE = {"matern32": math.sqrt(3.0), "matern52": math.sqrt(5.0)}
+RATE = {"matern12": 1.0, "matern32": math.sqrt(3.0), "matern52": math.sqrt(5.0)}
+COINCIDENT = 2.0 ** -20         # kernel_parts takes Matern-1/2's h as 0 below this r^2
 _MODELS = {}
 
 
@@ -319,16 +320,26 @@ def warp_error(px, xt, a, b):
 
 
 def kernel_parts(r2, kind):
-    """k, h (dk/dr^2 = -h / 2), |exponent of fast_exp| and the rate of that exponent in the features."""
+    """k, h (dk/dr^2 = -h / 2) of the oracle's kernel table, |exponent of fast_exp| and the rate of that exponent in the
+    features.
+
+    Matern-1/2's h is 0 for r^2 < COINCIDENT as well as below the oracle's clamp.  This is deliberately not the oracle's
+    rule; it covers the own-state references only.  They scale the candidate in fp64 from the fp32 row the kernel
+    receives, so a candidate equal to a training row lands within the fp32 roundings of the scaling (the MinMax shift's
+    absolute u |x_add| / l among them) of that row's fp32 feature vector, where the device, scaling both the same way in
+    fp32, has r = 0.  At the kink of e^-r that pair has h = 0 on the device and e^-r / r with an arbitrary direction
+    dz / r in fp64.  Those roundings stay below r = 2^-10 here; distinct candidates are at least 0.01 / l from the
+    data."""
+    from oracle import gp_oracle as O
+    kern = O.KERNELS[kind]
+    k, h = kern.k(r2), kern.h(r2)
     if kind == "rbf":
-        k = torch.exp(-0.5 * r2)
-        return k, k, 0.5 * r2, r2.clamp_min(0).sqrt()
+        return k, h, 0.5 * r2, r2.clamp_min(0).sqrt()
+    if kind == "matern12":
+        h = torch.where(r2 < COINCIDENT, torch.zeros_like(r2), h)
     a = RATE[kind]
-    r = r2.clamp_min(1e-30).sqrt()
-    e = torch.exp(-a * r)
-    if kind == "matern32":
-        return (1 + a * r) * e, 3.0 * e, a * r, torch.full_like(r, a)
-    return (1 + a * r + (5.0 / 3.0) * r2) * e, (5.0 / 3.0) * (1 + a * r) * e, a * r, torch.full_like(r, a)
+    t = a * r2.clamp_min(1e-30).sqrt()
+    return k, h, t, torch.full_like(t, a)
 
 
 def features64(gp, X, Xe, hyp, tables):
