@@ -6,9 +6,9 @@ from .embedding import HEBO_Embedding, MACE_Embedding  # noqa: F401
 from .bo import BO, NoMR_BO, HEBO_VectorContextual  # noqa: F401
 from .acq import NoisyAcq  # noqa: F401
 from .noisy import NoisyOpt  # noqa: F401
-from .acq import GeneralAcq  # noqa: F401
+from .acq import GeneralAcq, MOMeanSigmaLCB  # noqa: F401
 from .general import GeneralBO  # noqa: F401
 
 __all__ = ["GP", "B200GP", "MultiTaskModel", "MACE", "FusedMACE", "Mean", "Sigma", "LCB", "register", "HEBO_Embedding", "MACE_Embedding",
            "AbsEtaDifference", "BO", "NoMR_BO", "HEBO_VectorContextual", "NoisyOpt", "NoisyAcq",
-           "GeneralAcq", "GeneralBO"]
+           "GeneralAcq", "GeneralBO", "MOMeanSigmaLCB"]

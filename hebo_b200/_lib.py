@@ -93,6 +93,7 @@ SIGNATURES = {
     "hb_mace_epilogue": (_i32, [_vp, _vp, _i64, _f32, _f32, _f32, _f32, _vp, _vp, _u64, _vp, _vp]),
     "hb_acq1_epilogue": (_i32, [_vp, _vp, _i64, _i32, _f32, _f32, _vp, _vp]),
     "hb_general_acq_epilogue": (_i32, [_vp, _vp, _i64, _i64, _i64, _f32, _f32, _vp, _vp, _u64, _u64, _vp, _vp, _vp, _vp]),
+    "hb_mo_lcb_epilogue": (_i32, [_vp, _vp, _i64, _f32, _f32, _f32, _vp, _u64, _u64, _vp, _vp, _vp]),
     "hb_pareto_front3": (_i32, [_vp, _i64, _vp, _vp, _vp, _i64, _vp]),
     "hb_pareto_front_k": (_i32, [_vp, _i64, _i64, _vp, _vp, _vp, _i64, _vp]),
     "hb_nsga2_init": (_i32, [_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _u64, _vp, _vp, _vp]),

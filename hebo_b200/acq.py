@@ -221,16 +221,75 @@ def _general_epilogue(mu, var, num_obj, num_constr, kappa, c_kappa, noise_sd, xi
     return Fo, Fc, cv
 
 
+class MOMeanSigmaLCB(Acquisition):
+    """acq.py:99-129: minimise (py, -ps) subject to (py - kappa ps) - best_y <= 0, with py = mu + sqrt(model.noise) xi and
+    ps = sqrt(ps2) (no clamp), the acquisition ``HEBO(acq_cls=MOMeanSigmaLCB)`` optimises.  ``eval`` works over any
+    single-output model: it takes the N(0, 1) draws from torch's CPU generator as ``torch.randn(py.shape)``, like the
+    reference, and runs the arithmetic in the CUDA epilogue ``hb_mo_lcb_epilogue`` (correctly rounded fp32: torch's CPU
+    sqrt may differ by one ulp).  Returns [m, 3] on the input's device.  ``general_score`` scores it on the device."""
+
+    def __init__(self, model, best_y, **conf):
+        super().__init__(model, **conf)
+        self.best_y = best_y
+        self.kappa = conf.get("kappa", 2.0)
+        assert self.model.num_out == 1
+
+    @property
+    def num_obj(self):
+        return 2
+
+    @property
+    def num_constr(self):
+        return 1
+
+    def eval(self, x, xe):
+        with torch.no_grad():
+            py, ps2 = self.model.predict(x, xe)
+            xi = torch.randn(py.shape)
+            dev = torch.device("cuda")
+            up = lambda v: torch.as_tensor(v).reshape(-1).to(dev, torch.float32).contiguous()
+            F, G = _mo_lcb_epilogue(up(py), up(ps2), _noise_sd(self.model), _best_y(self), float(self.kappa), up(xi))
+            out = torch.cat([F, G[:, None]], 1)
+        probe = x if torch.is_tensor(x) else xe
+        return out.to(probe.device if torch.is_tensor(probe) else "cpu")
+
+
+def _noise_sd(model) -> float:
+    """np.sqrt(model.noise) as acq.py:119 takes it: a float32 noise gives its correctly rounded fp32 square root."""
+    return float(np.sqrt(np.asarray(model.noise)).reshape(-1)[0])
+
+
+def _best_y(acq) -> float:
+    return float(np.asarray(acq.best_y, dtype=np.float32).reshape(-1)[0])
+
+
+def _mo_lcb_epilogue(mu, var, noise_sd, best_y, kappa, xi, seed=0, counter=0):
+    """(F [m, 2], G [m]) of hb_mo_lcb_epilogue over mu / var [m]."""
+    m, dev = mu.shape[0], mu.device
+    F = torch.empty(m, 2, dtype=torch.float32, device=dev)
+    G = torch.empty(m, dtype=torch.float32, device=dev)
+    if m:
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().hb_mo_lcb_epilogue(_lib.ptr(mu), _lib.ptr(var), m, noise_sd, best_y, kappa, _lib.ptr(xi),
+                                                     int(seed), int(counter), _lib.ptr(F), _lib.ptr(G), _lib.stream_ptr()),
+                       "hb_mo_lcb_epilogue")
+    return F, G
+
+
 def general_score(acq, seed=None):
-    """score(xc, xe, gen) of a GeneralAcq for DeviceNSGA2(num_obj=acq.num_obj, constrained=acq.num_constr > 0): Fo
-    [m, num_obj] fp32 on the device, and with constraints (Fo, cv [m]), cv the summed positive parts of the constraint
-    columns.  Over a hebo_b200.MultiTaskModel of GPs, or one GP: one posterior call per output with F = NULL, writing row b
-    of [K, m] buffers, then hb_general_acq_epilogue with Philox draws keyed by (seed, gen) -- no host synchronisation
-    inside a generation; an output whose fit failed predicts N(y_mean, y_std^2) as GP.predict does.  ``seed`` is drawn from
-    numpy's global generator when None.  Any other acquisition or model: acq.eval on CPU tensors (xe as int64), once per
-    generation."""
+    """score(xc, xe, gen) of a multi-objective or constrained acquisition for DeviceNSGA2(num_obj=acq.num_obj,
+    constrained=acq.num_constr > 0): Fo [m, num_obj] fp32 on the device, and with constraints (Fo, cv [m]), cv the summed
+    positive parts of the constraint columns.  A GeneralAcq over a hebo_b200.MultiTaskModel of GPs, or one GP: one
+    posterior call per output with F = NULL, writing row b of [K, m] buffers, then hb_general_acq_epilogue with Philox
+    draws keyed by (seed, gen).  A MOMeanSigmaLCB over a hebo_b200.GP: one posterior call with F = NULL, then
+    hb_mo_lcb_epilogue with Philox draws keyed by (seed, gen), its G being the one constraint column.  Neither synchronises
+    with the host inside a generation; an output whose fit failed predicts N(y_mean, y_std^2) as GP.predict does.
+    ``seed`` is drawn from numpy's global generator when None.  Any other acquisition or model, including subclasses of
+    these two: acq.eval on CPU tensors (xe as int64), once per generation."""
     no, nc = acq.num_obj, acq.num_constr
     model = acq.model
+    if type(acq) is MOMeanSigmaLCB and isinstance(model, GP):
+        return _mo_lcb_device_score(acq, seed)
     gps = None
     if isinstance(model, GP):
         gps = [model]
@@ -260,6 +319,19 @@ def general_score(acq, seed=None):
                 gp._posterior(gp._to_dev(xc), False, Xe_dev=gp._xe_dev(xe, m), out=(mu[b], var[b]))
         Fo, _, cv = _general_epilogue(mu, var, no, nc, kappa, c_kappa, noise_sd, None, seed, gen, want_cv=nc > 0)
         return (Fo, cv) if nc else Fo
+    return device_score
+
+
+def _mo_lcb_device_score(acq, seed=None):
+    seed = int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed)
+    gp = acq.model
+    noise_sd, best_y, kappa = _noise_sd(gp), _best_y(acq), float(acq.kappa)
+
+    def device_score(xc, xe, gen):
+        m = xc.shape[0]
+        with torch.no_grad():
+            _, mu, var = gp._posterior(gp._to_dev(xc), False, Xe_dev=gp._xe_dev(xe, m))
+        return _mo_lcb_epilogue(mu, var, noise_sd, best_y, kappa, None, seed, gen)
     return device_score
 
 

@@ -847,6 +847,12 @@ int32_t hb_general_acq_epilogue(const float *mu, const float *var, int64_t m, in
                             (cudaStream_t)stream);
 }
 
+int32_t hb_mo_lcb_epilogue(const float *mu, const float *var, int64_t m, float noise_sd, float best_y, float kappa,
+                           const float *xi, uint64_t seed, uint64_t counter, float *F, float *G, void *stream) {
+  if (!mu || !var || !F || !G) return HB_ERR_INVALID;
+  return launch_mo_lcb(mu, var, m, noise_sd, best_y, kappa, xi, seed, counter, F, G, (cudaStream_t)stream);
+}
+
 int32_t hb_pareto_front3(const float *F, int64_t m, int32_t *idx_out, int32_t *count, void *ws, int64_t ws_bytes,
                          void *stream) {
   if (!F || !idx_out || !count || !ws) return HB_ERR_INVALID;

@@ -170,6 +170,9 @@ int launch_acq1(const float *mu, const float *var, int64_t m, int mode, float ka
 int launch_general_acq(const float *mu, const float *var, int64_t m, int64_t num_obj, int64_t num_constr, float kappa,
                        float c_kappa, const float *noise_sd, const float *xi, uint64_t seed, uint64_t counter, float *Fo,
                        float *Fc, float *cv, cudaStream_t st);
+// F [m, 2] and G [m] of MOMeanSigmaLCB over (mu, var)
+int launch_mo_lcb(const float *mu, const float *var, int64_t m, float noise_sd, float best_y, float kappa, const float *xi,
+                  uint64_t seed, uint64_t counter, float *F, float *G, cudaStream_t st);
 int kstar_groups(int64_t np);
 int launch_kstar(const Fitted &gp, const float *xs, const int32_t *xe, int64_t mc, float *KS, float *KS_h16, float *mupart,
                  int64_t mc_pad, const int32_t *fixlist, const int32_t *fixcount, cudaStream_t st);

@@ -472,6 +472,42 @@ int launch_general_acq(const float *mu, const float *var, int64_t m, int64_t num
   return HB_OK;
 }
 
+// MOMeanSigmaLCB.eval (acq.py:99-129) over one output's mu / var [m].  Correctly rounded operations, no FMA contraction, so
+// each column is bit-identical to the IEEE fp32 evaluation of the reference's torch expression:
+//   py = py + noise_sd * xi,  ps = sqrt(ps2)  (no clamp: a NaN or negative ps2 gives NaN)
+//   F [m, 2] = (py, -1 * ps),  G [m] = (py - kappa * ps) - best_y
+// xi [m] (the reference's torch.randn(py.shape)) or NULL: Philox draws keyed by (seed, counter), row r takes half r % 2 of
+// the pair r / 2 -- general_acq_kernel's layout with K = 1.
+__global__ void __launch_bounds__(256) mo_lcb_kernel(const float *__restrict__ mu, const float *__restrict__ var, int64_t m,
+                                                     float noise_sd, float best_y, float kappa, const float *__restrict__ xi,
+                                                     uint64_t seed, uint64_t counter, float *__restrict__ F,
+                                                     float *__restrict__ G) {
+  const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= m) return;
+  float z;
+  if (xi) {
+    z = xi[r];
+  } else {
+    float z0, z1;
+    philox_normal2(seed, (uint64_t)(r >> 1), counter, z0, z1);
+    z = (r & 1) ? z1 : z0;
+  }
+  const float py = __fadd_rn(mu[r], __fmul_rn(noise_sd, z));
+  const float ps = __fsqrt_rn(var[r]);
+  F[r * 2 + 0] = py;
+  F[r * 2 + 1] = __fmul_rn(-1.0f, ps);                                                     // exact: ps = 0 gives -0
+  G[r] = __fsub_rn(__fsub_rn(py, __fmul_rn(kappa, ps)), best_y);
+}
+
+int launch_mo_lcb(const float *mu, const float *var, int64_t m, float noise_sd, float best_y, float kappa, const float *xi,
+                  uint64_t seed, uint64_t counter, float *F, float *G, cudaStream_t st) {
+  if (m <= 0) return HB_ERR_INVALID;
+  mo_lcb_kernel<<<(int)ceil_div(m, 256), 256, 0, st>>>(mu, var, m, noise_sd, best_y, kappa, xi, seed, counter, F, G);
+  count_launches(1);
+  HB_LAUNCH_CHECK("mo_lcb");
+  return HB_OK;
+}
+
 
 __global__ void __launch_bounds__(256) mace_kernel(const float *__restrict__ mupart, int ncg,
                                                    const float *__restrict__ vpart, int nt,

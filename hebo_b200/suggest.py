@@ -8,6 +8,9 @@ either ONE big-batch device pass (default: m scrambled-Sobol candidates + the in
 non-dominated filter) or -- ``acq_optimizer="nsga2"`` -- a device-resident NSGA-II of the reference's shape
 (``hebo_b200.evolution.DeviceNSGA2``: pop 100 x 100 generations, typed variables, every generation scored by one fused call,
 no per-generation host round trip; evolution_optimizer.py:107-160).
+The acquisition is MACE unless ``acq_cls`` names another class (hebo.py:35-61,162), which is built per suggest as
+``acq_cls(model, best_y=py_best, kappa=kappa)``, scored by ``hebo_b200.acq.general_score`` and optimised over its own
+objective and constraint columns; such a class takes one suggestion per call, as in the reference.
 
 Two front ends:  ``HEBO(space)`` with a DesignSpace (or its list-of-dicts spec) speaks pandas DataFrames like the reference;
 ``HEBO(lb, ub)`` is the continuous-box shorthand that speaks tensors.  With a real HEBO install use
@@ -23,6 +26,7 @@ import pandas as pd
 import torch
 from torch.quasirandom import SobolEngine
 
+from . import _lib
 from .acq import MACE
 from .gp import GP
 from .pareto import feasible_front, pareto_front
@@ -61,7 +65,12 @@ class HEBO:
     def __init__(self, space=None, ub=None, model_config: Optional[dict] = None, rand_sample: Optional[int] = None,
                  scramble_seed: Optional[int] = None, n_candidates: int = 10000, device: str = "cuda",
                  n_refine: int = 0, refine_sigma: float = 0.05, acq_optimizer: str = "sobol", evo_pop: int = 100,
-                 evo_iters: int = 100, lb=None, _constraint=None):
+                 evo_iters: int = 100, lb=None, _constraint=None, model_name: str = "gp", acq_cls=MACE):
+        if model_name != "gp":
+            raise NotImplementedError(f"HEBO: model_name {model_name!r} is not supported, only 'gp'")
+        if acq_cls is not MACE and (n_refine or _constraint is not None):
+            raise ValueError("n_refine and the embedding constraint are defined for the MACE front only; an acq_cls other "
+                             "than MACE takes neither")
         if lb is not None:
             space = lb
         if ub is not None:                                   # HEBO(lb, ub): continuous box, tensors in / out
@@ -93,6 +102,10 @@ class HEBO:
         if _constraint is not None and self.n_refine:
             raise ValueError("n_refine is not supported together with a constraint")
         self._model_config = model_config
+        self.model_name = model_name
+        # the acquisition of hebo.py:162, built as acq_cls(model, best_y=py_best, kappa=kappa) in every suggest.  MACE keeps
+        # the fused posterior + MACE path; any other class is scored by hebo_b200.acq.general_score
+        self.acq_cls = acq_cls
         self.last_timing = {}
 
     # ------------------------------------------------------------------ config / data
@@ -185,7 +198,45 @@ class HEBO:
         except Exception:
             return build(torch.FloatTensor(self.y).clone())
 
+    def _acq_front(self, model, py_best, kappa, bxc, bxe, fix_input, fixed, candidates, mark):
+        """hebo.py:162-165 with an acquisition other than MACE: acq_cls(model, best_y=py_best, kappa=kappa), optimised by
+        DeviceNSGA2 with its objective count and constraint (evolution_optimizer.py:72-105), or scored on the Sobol batch
+        with the incumbent prepended.  Returns the (feasible) front (cand_c, cand_e) with its posterior mean and variance."""
+        from .acq import general_score
+        acq = self.acq_cls(model, best_y=py_best.numpy().squeeze(), kappa=kappa)
+        if acq.num_obj > _lib.HB_MAX_OBJ:
+            raise ValueError(f"HEBO: an acquisition with {acq.num_obj} objectives; at most {_lib.HB_MAX_OBJ} are supported")
+        dev, constrained = model.device, acq.num_constr > 0
+        seed = int(np.random.randint(0, 2 ** 31 - 1))
+        score = general_score(acq, seed ^ 0x5BD1E995)
+        if self.acq_optimizer == "nsga2" and candidates is None:
+            from .evolution import DeviceNSGA2
+            evo = DeviceNSGA2(self.space.var_kinds, self.lb.numpy(), self.ub.numpy(), self.d, score, pop=self.evo_pop,
+                              iters=self.evo_iters, seed=seed, fixed=fixed, device=dev, constrained=constrained,
+                              num_obj=acq.num_obj)
+            cand_c, cand_e, _ = evo.optimize(initial_suggest=torch.cat([bxc, bxe.float()], 1).numpy())
+            cand_e = cand_e.long()                                   # res.X is already the (feasible) rank-0 set
+            mark("candidates_ms")
+        else:
+            if candidates is None:
+                cc, ce = self.quasi_sample(self.n_candidates - 1, fix_input, self.cand_sobol, as_opt=True)
+                cand_c, cand_e = torch.cat([bxc, cc], 0), torch.cat([bxe, ce], 0)
+            else:
+                cand_c, cand_e = self._to_opt(candidates)
+            cand_c = cand_c.to(dev, torch.float32, non_blocking=True)
+            cand_e = cand_e.to(dev, non_blocking=True)
+            mark("candidates_ms")
+            F, G = (score(cand_c, cand_e, 0), None) if not constrained else score(cand_c, cand_e, 0)
+            idx = pareto_front(F) if G is None else feasible_front(F, G)
+            cand_c, cand_e = cand_c[idx], cand_e[idx]
+        with torch.no_grad():
+            mu, var = model.predict(cand_c if self.d else None, cand_e if self.e else None)
+        mark("posterior_ms")
+        return cand_c, cand_e, mu.reshape(-1), var.reshape(-1)
+
     def suggest(self, n_suggestions: int = 1, fix_input: Optional[dict] = None, candidates=None):
+        if self.acq_cls is not MACE and n_suggestions != 1:                 # hebo.py:120-121
+            raise RuntimeError("Parallel optimization is supported only for MACE acquisition")
         if self.Xc.shape[0] < self.rand_sample:
             return self.quasi_sample(n_suggestions, fix_input)
         t0 = time.perf_counter()
@@ -205,42 +256,47 @@ class HEBO:
         bxc, bxe = self.Xc[[best_id]], self.Xe[[best_id]]
         py_best, _ = model.predict(bxc if self.d else None, bxe if self.e else None)                  # hebo.py:152
         kappa = kappa_schedule(self.Xc.shape[0], n_suggestions, self.D)
-        acq = MACE(model, best_y=py_best.numpy().squeeze(), kappa=kappa)
-        tau = float(np.asarray(acq.tau).reshape(-1)[0])
-        mark("predict_best_ms")
         fixed = self._fixed_columns(fix_input)
-
-        def score(xc, xe, seed=0):
-            return model.predict_mace(xc if self.d else None, tau, kappa, acq.eps, seed=seed, return_mu_var=True,
-                                      Xe=xe if self.e else None, device_out=True)
-        cons = self._constraint
-        if self.acq_optimizer == "nsga2" and candidates is None:
-            from .evolution import DeviceNSGA2
-            if cons is None:
-                evo_score = lambda xc, xe, gen: score(xc, xe, gen)[0]
-            else:
-                evo_score = lambda xc, xe, gen: (score(xc, xe, gen)[0], cons(xc))
-            evo = DeviceNSGA2(self.space.var_kinds, self.lb.numpy(), self.ub.numpy(), self.d, evo_score, pop=self.evo_pop,
-                              iters=self.evo_iters, seed=int(np.random.randint(0, 2 ** 31 - 1)), fixed=fixed, device=dev,
-                              constrained=cons is not None)
-            cand_c, cand_e, _ = evo.optimize(initial_suggest=torch.cat([bxc, bxe.float()], 1).numpy())
-            cand_e = cand_e.long()
-            mark("candidates_ms")
-            F, mu, var = score(cand_c, cand_e.int())
-            mark("posterior_mace_ms")
-            idx = torch.arange(cand_c.shape[0], device=dev)          # res.X is already the rank-0 set
+        if self.acq_cls is not MACE:
+            mark("predict_best_ms")
+            cand_c, cand_e, mu, var = self._acq_front(model, py_best, kappa, bxc, bxe, fix_input, fixed, candidates, mark)
+            idx = torch.arange(cand_c.shape[0], device=dev)
         else:
-            if candidates is None:
-                cc, ce = self.quasi_sample(self.n_candidates - 1, fix_input, self.cand_sobol, as_opt=True)
-                cand_c, cand_e = torch.cat([bxc, cc], 0), torch.cat([bxe, ce], 0)
+            acq = MACE(model, best_y=py_best.numpy().squeeze(), kappa=kappa)
+            tau = float(np.asarray(acq.tau).reshape(-1)[0])
+            mark("predict_best_ms")
+
+            def score(xc, xe, seed=0):
+                return model.predict_mace(xc if self.d else None, tau, kappa, acq.eps, seed=seed, return_mu_var=True,
+                                          Xe=xe if self.e else None, device_out=True)
+            cons = self._constraint
+            if self.acq_optimizer == "nsga2" and candidates is None:
+                from .evolution import DeviceNSGA2
+                if cons is None:
+                    evo_score = lambda xc, xe, gen: score(xc, xe, gen)[0]
+                else:
+                    evo_score = lambda xc, xe, gen: (score(xc, xe, gen)[0], cons(xc))
+                evo = DeviceNSGA2(self.space.var_kinds, self.lb.numpy(), self.ub.numpy(), self.d, evo_score, pop=self.evo_pop,
+                                  iters=self.evo_iters, seed=int(np.random.randint(0, 2 ** 31 - 1)), fixed=fixed, device=dev,
+                                  constrained=cons is not None)
+                cand_c, cand_e, _ = evo.optimize(initial_suggest=torch.cat([bxc, bxe.float()], 1).numpy())
+                cand_e = cand_e.long()
+                mark("candidates_ms")
+                F, mu, var = score(cand_c, cand_e.int())
+                mark("posterior_mace_ms")
+                idx = torch.arange(cand_c.shape[0], device=dev)          # res.X is already the rank-0 set
             else:
-                cand_c, cand_e = self._to_opt(candidates)
-            cand_c = cand_c.to(dev, torch.float32, non_blocking=True)
-            cand_e = cand_e.to(dev, non_blocking=True)
-            mark("candidates_ms")
-            F, mu, var = score(cand_c, cand_e)
-            mark("posterior_mace_ms")
-            idx = pareto_front(F) if cons is None else feasible_front(F, cons(cand_c))
+                if candidates is None:
+                    cc, ce = self.quasi_sample(self.n_candidates - 1, fix_input, self.cand_sobol, as_opt=True)
+                    cand_c, cand_e = torch.cat([bxc, cc], 0), torch.cat([bxe, ce], 0)
+                else:
+                    cand_c, cand_e = self._to_opt(candidates)
+                cand_c = cand_c.to(dev, torch.float32, non_blocking=True)
+                cand_e = cand_e.to(dev, non_blocking=True)
+                mark("candidates_ms")
+                F, mu, var = score(cand_c, cand_e)
+                mark("posterior_mace_ms")
+                idx = pareto_front(F) if cons is None else feasible_front(F, cons(cand_c))
         for _ in range(self.n_refine if self.d else 0):
             pc, pe = cand_c[idx], cand_e[idx]
             reps = max(1, (self.n_candidates // 4) // max(1, pc.shape[0]))

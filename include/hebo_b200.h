@@ -361,6 +361,22 @@ int32_t hb_general_acq_epilogue(const float *mu, const float *var, int64_t m, in
                                 float c_kappa, const float *noise_sd, const float *xi, uint64_t seed, uint64_t counter, float *Fo,
                                 float *Fc, float *cv, void *stream);
 
+/* ---- MOMeanSigmaLCB epilogue  (MOMeanSigmaLCB.eval, acquisitions/acq.py:99-129: minimise (py, -ps) subject to
+ * LCB < best_y; the acquisition HEBO takes as acq_cls, optimizers/hebo.py:162) ----
+ * mu, var [m] device, in original y units (as hb_posterior_mace_ex writes them with F = NULL), m >= 1.  noise_sd =
+ * sqrt(model.noise), computed by the caller.  With py = mu, ps2 = var:
+ *   py = py + noise_sd * xi
+ *   ps = sqrt(ps2)                                    no clamp: a NaN or negative ps2 gives NaN, as torch.sqrt does
+ *   F [m, 2] = (py, -1 * ps)                          objectives; -1 * ps is an exact negation, so ps = 0 gives -0
+ *   G [m]    = (py - kappa * ps) - best_y             the constraint, feasible iff G <= 0 (a NaN G is infeasible)
+ * Correctly rounded operations, no FMA contraction: each column is bit-identical to the IEEE fp32 evaluation of the
+ * reference's torch expression on the same mu / var / draws.  xi [m] device draws (the reference's torch.randn(py.shape))
+ * or NULL: Philox4x32-10 + Box-Muller keyed by (seed, counter); row r takes half r % 2 of pair r / 2, which is
+ * hb_general_acq_epilogue's layout with K = 1, and the same (seed, counter) replays the same bits.  One launch, no host
+ * synchronisation. */
+int32_t hb_mo_lcb_epilogue(const float *mu, const float *var, int64_t m, float noise_sd, float best_y, float kappa,
+                           const float *xi, uint64_t seed, uint64_t counter, float *F, float *G, void *stream);
+
 /* ---- 3-objective non-dominated filter  (the rank-0 set NSGA-II returns as res.X,
  * acq_optimizers/evolution_optimizer.py:141-149) ----------------------------------------------
  * F [m,3]; idx_out [m] int32 ascending indices of the non-dominated rows; count device int32.
