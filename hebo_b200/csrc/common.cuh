@@ -174,15 +174,22 @@ __device__ __forceinline__ float softplus_f(float u) {
 __device__ __forceinline__ float sigmoid_f(float u) { return 1.0f / (1.0f + expf(-u)); }
 
 // pSGLD update of parameter i: torch.optim.RMSprop step followed by the Langevin term of HEBO/hebo/models/nn/sgld.py:57-70
-// (xi == nullptr: no Langevin term)
+// (xi == nullptr: no Langevin term).  Every operation is rounded on its own (no FMA contraction), in this order:
+//   v   = sq a + (1 - a) (g g)          square_avg.mul_(alpha).addcmul_(grad, grad, value=1 - alpha)
+//   avg = sqrt(v) + eps                 square_avg.sqrt().add_(eps)
+//   x   = raw + ((-lr) g) / avg         param.addcdiv_(grad, avg, value=-lr)
+//   x   = x + (factor sqrt((2 lr) / avg)) xi      sgld.py:64-70
+// so tests/test_fit_loop_host.py restates it bit for bit.  torch's CPU addcdiv has the same order; its CPU addcmul fuses
+// (value g) g into the sum, and it rounds 1 - alpha from fp64 where this forms it in fp32.  |g| > 2^64 overflows g g:
+// avg = inf and the step is 0.
 __device__ __forceinline__ void psgld_update(float *raw, const float *grad, float *sq, int i, float lr, float a, float eps,
                                              float factor, const float *xi) {
   const float g = grad[i];
-  const float v = a * sq[i] + (1.0f - a) * g * g;
+  const float v = __fadd_rn(__fmul_rn(sq[i], a), __fmul_rn(__fsub_rn(1.0f, a), __fmul_rn(g, g)));
   sq[i] = v;
-  const float avg = sqrtf(v) + eps;
-  float x = raw[i] - lr * g / avg;
-  if (xi) x += factor * sqrtf(2.0f * lr / avg) * xi[i];
+  const float avg = __fadd_rn(__fsqrt_rn(v), eps);
+  float x = __fadd_rn(raw[i], __fdiv_rn(__fmul_rn(-lr, g), avg));
+  if (xi) x = __fadd_rn(x, __fmul_rn(__fmul_rn(factor, __fsqrt_rn(__fdiv_rn(__fmul_rn(2.0f, lr), avg))), xi[i]));
   raw[i] = x;
 }
 

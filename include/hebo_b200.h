@@ -160,7 +160,9 @@ int32_t hb_mll_grad(const float *Xt, int64_t n, int64_t d, const float *raw, con
                     float noise_guess, float *grad, float *loss, void *ws, void *stream);
 
 /* ---- pSGLD update  (models/nn/sgld.py:49-70 on torch.optim.RMSprop) --------------------------
- * xi: [P] N(0,1) draws or NULL (= pretrain phase, no Langevin noise). */
+ * xi: [P] N(0,1) draws or NULL (= pretrain phase, no Langevin noise).  Per element, each operation rounded on its own
+ * (no FMA), a = rms_alpha:  v = sq a + (1 - a) (g g);  avg = sqrt(v) + eps;  raw += ((-lr) g) / avg;
+ * then raw += (factor sqrt((2 lr) / avg)) xi;  square_avg = v. */
 int32_t hb_psgld_step(float *raw, const float *grad, float *square_avg, int64_t p, float lr,
                       float rms_alpha, float rms_eps, float factor, const float *xi, void *stream);
 

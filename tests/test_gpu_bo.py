@@ -98,7 +98,7 @@ def fitted_gp():
 
 @pytest.mark.parametrize("cls,conf", [(LCB, {"kappa": 2.0}), (LCB, {"kappa": 0.6}), (Mean, {}), (Sigma, {}),
                                       (AbsEtaDifference, {}), (AbsEtaDifference, {"eta": 0.5, "kappa": 1.3})])
-def test_acq1_epilogue_equals_cpu_eval(fitted_gp, cls, conf):
+def test_acq1_cpu_eval_is_the_epilogue_expression_at_torch_sqrt(fitted_gp, cls, conf):
     rng = np.random.default_rng(1)
     m = 3000
     xc = torch.FloatTensor(rng.uniform(-3, 3, (m, 3)))
@@ -108,16 +108,20 @@ def test_acq1_epilogue_equals_cpu_eval(fitted_gp, cls, conf):
     ref = acq.eval(xc, xe).reshape(-1)
     got = ga_score(acq)(xc.cuda(), xe.cuda().int(), 0).cpu()
     # bit for bit against the same expression in IEEE fp32 (numpy: correctly rounded sqrt, products, differences) on the
-    # same mu / var; torch's CPU sqrt goes through MKL VML (< 1 ulp, not always correctly rounded), so the CPU eval itself
-    # may differ from that by one ulp in a few rows
-    mu, var = (t.reshape(-1).numpy() for t in fitted_gp.predict(xc, xe))
+    # same mu / var; torch's CPU sqrt goes through MKL VML (< 1 ulp, not always correctly rounded), so the CPU eval is
+    # that expression bit for bit at torch's own square root, which is within one ulp of the correctly rounded one (a
+    # one-ulp root can move a cancelling |mu - eta| - kappa s by more than one ulp of the result)
+    mu_t, var_t = fitted_gp.predict(xc, xe)
+    mu, var = (t.reshape(-1).numpy() for t in (mu_t, var_t))
+    s_cpu = var_t.sqrt().reshape(-1).numpy()
     k, e, s = np.float32(getattr(acq, "kappa", 0.0)), np.float32(getattr(acq, "eta", 0.0)), np.sqrt(var)
-    ieee = {LCB: lambda: mu - k * s, Mean: lambda: mu, Sigma: lambda: np.float32(-1) * s,
-            AbsEtaDifference: lambda: np.abs(mu - e) - k * s}[cls]()
+    expr = {LCB: lambda s: mu - k * s, Mean: lambda s: mu, Sigma: lambda s: np.float32(-1) * s,
+            AbsEtaDifference: lambda s: np.abs(mu - e) - k * s}[cls]
+    ieee = expr(s)
     assert ieee.dtype == np.float32
     assert np.array_equal(got.numpy().view(np.uint32), ieee.view(np.uint32))
-    ulp = np.abs(got.numpy().view(np.int32).astype(np.int64) - ref.numpy().view(np.int32).astype(np.int64))
-    assert ulp.max() <= (0 if cls is Mean else 1)
+    assert np.abs(s_cpu.view(np.int32).astype(np.int64) - s.view(np.int32).astype(np.int64)).max() <= 1
+    assert np.array_equal(ref.numpy().view(np.uint32), expr(s_cpu).view(np.uint32))
 
 
 def test_user_acquisition_scores_through_its_eval(fitted_gp):
