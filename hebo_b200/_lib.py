@@ -17,6 +17,10 @@ HB_ACQ1_LCB, HB_ACQ1_MEAN, HB_ACQ1_SIGMA, HB_ACQ1_ABS_ETA = 0, 1, 2, 3   # hb_ac
 HB_MAX_FEATURES = 4096   # d + sum(emb_sizes) a model may have (include/hebo_b200.h)
 HB_MAX_OUTPUTS = 32      # outputs one batched fit trains together (hb_fit_multi_ex)
 HB_MAX_OBJ = 8           # objectives of hb_nsga2_survive_k / hb_pareto_front_k
+# deep-ensemble envelope (HB_DE_MAX_* of include/hebo_b200.h)
+HB_DE_MAX_LAYERS, HB_DE_MAX_HIDDEN, HB_DE_MAX_OUT, HB_DE_MAX_IN, HB_DE_MAX_MEMBERS = 3, 256, 8, 256, 32
+HB_DE_MAX_BATCH_FLOATS = 56000
+HB_DE_EMBEDDING, HB_DE_ONEHOT = 0, 1
 
 
 class HeboB200Error(RuntimeError):
@@ -38,8 +42,15 @@ class ModelSpec(C.Structure):     # hb_model_spec_t
                 ("emb_sizes", C.POINTER(C.c_int32)), ("warp", C.c_int32)]
 
 
+class DeSpec(C.Structure):        # hb_de_spec_t
+    _fields_ = [("num_cont", C.c_int32), ("num_enum", C.c_int32), ("num_uniqs", C.POINTER(C.c_int32)),
+                ("enum_trans", C.c_int32), ("num_layers", C.c_int32), ("num_hiddens", C.c_int32), ("num_out", C.c_int32),
+                ("output_noise", C.c_int32), ("rand_prior", C.c_int32), ("noise_lb", C.c_float)]
+
+
 _vp, _i64, _i32, _f32, _u64 = C.c_void_p, C.c_int64, C.c_int32, C.c_float, C.c_uint64
 _sp = C.POINTER(ModelSpec)
+_dsp = C.POINTER(DeSpec)
 
 # name -> (restype, argtypes); must list every function declared in include/hebo_b200.h
 SIGNATURES = {
@@ -111,6 +122,11 @@ SIGNATURES = {
     "hb_front_merge_workspace_bytes": (_i64, [_i64, _i64]),
     "hb_front_pack": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp]),
     "hb_front_merge": (_i32, [_vp, _i64, _i64, _vp, _vp, _i64, _vp]),
+    "hb_de_num_params": (_i64, [_dsp]),
+    "hb_de_fit_workspace_bytes": (_i64, [_dsp, _i64]),
+    "hb_de_fit": (_i32, [_vp, _vp, _vp, _i64, _dsp, _i64, _vp, C.c_double, _f32, _i64, _i64, _vp, _u64, _vp, _vp, _i64, _vp]),
+    "hb_de_predict": (_i32, [_vp, _vp, _i64, _dsp, _i64, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
+    "hb_de_predict_grad": (_i32, [_vp, _vp, _i64, _dsp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
 }
 
 _lib = None

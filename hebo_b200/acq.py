@@ -22,6 +22,7 @@ import torch
 
 from . import _lib
 from .base import Acquisition
+from .ensemble import DeepEnsemble
 from .gp import GP, MultiTaskModel
 
 
@@ -141,7 +142,7 @@ def ga_score(acq, seed=None):
             and not acq.model._fit_failed):
         return _noisy_device_score(acq.model, int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed))
     mode = _ACQ1_MODES.get(type(acq))
-    if mode is not None and isinstance(acq.model, GP):
+    if mode is not None and isinstance(acq.model, (GP, DeepEnsemble)):
         kappa = float(getattr(acq, "kappa", 0.0))
         eta = float(getattr(acq, "eta", 0.0))
 

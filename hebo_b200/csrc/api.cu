@@ -956,4 +956,34 @@ int32_t hb_embed_violation(const float *Y, int64_t m, int64_t e, const float *B,
   return launch_embed_violation(Y, m, e, B, D, G, ws, ws_bytes, (cudaStream_t)stream);
 }
 
+// deep_ensemble.py:34-61 / BaseNet :183-221: P of one member
+int64_t hb_de_num_params(const hb_de_spec_t *spec) { return de_num_params(spec); }
+
+int64_t hb_de_fit_workspace_bytes(const hb_de_spec_t *spec, int64_t E) { return de_fit_ws_query(spec, E); }
+
+// deep_ensemble.py:71-93 (the member loop) and fit_one :151-181
+int32_t hb_de_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec, int64_t E,
+                  float *params, double lr, float l1, int64_t batch_size, int64_t num_epochs, const int32_t *perm,
+                  uint64_t seed, float *losses, void *ws, int64_t ws_bytes, void *stream) {
+  return launch_de_fit(Xc, Xe, y, n, spec, E, params, lr, l1, batch_size, num_epochs, perm, seed, losses, ws, ws_bytes,
+                       (cudaStream_t)stream);
+}
+
+// deep_ensemble.py:95-106 (predict) and :108-116 (sample_f, member >= 0)
+int32_t hb_de_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t E,
+                      const float *params, const float *x_mul, const float *x_add, const float *y_mean, const float *y_std,
+                      int32_t member, float *mu, float *var, void *stream) {
+  return launch_de_predict(Xs, Xe, m, spec, E, params, x_mul, x_add, y_mean, y_std, member, mu, var, nullptr, nullptr,
+                           (cudaStream_t)stream);
+}
+
+// autograd of deep_ensemble.py:95-106 with respect to Xc (the support_grad contract, base_model.py / test_base_model.py:94-108)
+int32_t hb_de_predict_grad(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t E,
+                           const float *params, const float *x_mul, const float *x_add, const float *y_mean,
+                           const float *y_std, float *mu, float *var, float *dmu, float *dvar, void *stream) {
+  if (!dmu || !dvar) return HB_ERR_INVALID;
+  return launch_de_predict(Xs, Xe, m, spec, E, params, x_mul, x_add, y_mean, y_std, -1, mu, var, dmu, dvar,
+                           (cudaStream_t)stream);
+}
+
 }  // extern "C"

@@ -225,5 +225,14 @@ int launch_ga_survive(const float *X, const float *F, const float *G, const floa
 int64_t embed_violation_ws_query(int64_t m, int64_t e, int64_t D);
 int launch_embed_violation(const float *Y, int64_t m, int64_t e, const float *B, int64_t D, float *G, void *ws, int64_t ws_bytes,
                            cudaStream_t st);
+// ensemble.cu: the deep-ensemble surrogate's fit (one CTA per member) and predict / input gradients (dmu == nullptr: none)
+int64_t de_num_params(const hb_de_spec_t *spec);
+int64_t de_fit_ws_query(const hb_de_spec_t *spec, int64_t E);
+int launch_de_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec, int64_t E,
+                  float *params, double lr, float l1, int64_t batch_size, int64_t num_epochs, const int32_t *perm,
+                  uint64_t seed, float *losses, void *ws, int64_t ws_bytes, cudaStream_t st);
+int launch_de_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t E, const float *params,
+                      const float *x_mul, const float *x_add, const float *y_mean, const float *y_std, int32_t member,
+                      float *mu, float *var, float *dmu, float *dvar, cudaStream_t st);
 
 }  // namespace hb

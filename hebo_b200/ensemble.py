@@ -1,0 +1,390 @@
+"""Deep-ensemble surrogate behind HEBO's ``BaseModel`` plugin surface.
+
+Drop-in for ``hebo.models.nn.deep_ensemble.DeepEnsemble`` (HEBO/hebo/models/nn/deep_ensemble.py:29-181): the same
+constructor keys and defaults, the same ``fit / predict / noise / sample_f`` contract with CPU tensors in and out, but the
+whole fit of every member runs in one launch of ``hb_de_fit`` and prediction in ``hb_de_predict`` /
+``hb_de_predict_grad`` (hebo_b200/csrc/ensemble.cu); nothing falls back to torch.
+
+Initial weights are drawn on the host from torch's global CPU generator in BaseNet's registration order and shapes
+(xavier_uniform_ with the ReLU gain for every weight, embedding tables included; zero biases) and uploaded once.  The
+minibatch order of each member's epochs is a keyed Philox bijection on the device, seeded from the same generator.
+
+Deliberate deviation: the reference calls ``torch.seed()`` at the start of every ``fit_one`` (:152), which makes each fit
+irreproducible and reseeds the caller's global generator.  This port does not reseed, so a fit is reproducible under
+``torch.manual_seed``.
+
+Extra conf key: ``device`` (default 'cuda').
+"""
+from __future__ import annotations
+
+import ctypes as C
+
+import numpy as np
+import torch
+import torch.nn as nn
+
+from . import _lib
+from .base import BaseModel
+from .scalers import MinMaxScaler, StandardScaler
+
+
+def param_layout(num_cont, num_uniqs, enum_trans, num_layers, num_hiddens, num_out, output_noise, rand_prior):
+    """[(state_dict name, shape)] of one BaseNet in registration order (deep_ensemble.py:183-221); the flat raw vector of
+    hb_de_fit is their concatenation."""
+    out = []
+    din = num_cont
+    if num_uniqs:
+        if enum_trans == "embedding":
+            for c, u in enumerate(num_uniqs):
+                w = min(50, 1 + u // 2)
+                out.append((f"enum_layer.emb.{c}.weight", (u, w)))
+                din += w
+        else:
+            din += sum(num_uniqs)
+
+    def mlp(prefix):
+        k = din
+        for l in range(num_layers):
+            out.append((f"{prefix}.{2 * l}.weight", (num_hiddens, k)))
+            out.append((f"{prefix}.{2 * l}.bias", (num_hiddens,)))
+            k = num_hiddens
+    mlp("hidden")
+    out += [("mu.weight", (num_out, num_hiddens)), ("mu.bias", (num_out,))]
+    if output_noise:
+        out += [("sigma2.0.weight", (num_out, num_hiddens)), ("sigma2.0.bias", (num_out,))]
+    if rand_prior:
+        mlp("prior_net")
+        out += [("prior_net.prior_net_out.weight", (num_out, num_hiddens)), ("prior_net.prior_net_out.bias", (num_out,))]
+    return out, din
+
+
+def init_params(layout) -> torch.Tensor:
+    """BaseNet's initialisation (:217-221) from torch's global CPU generator, in registration order."""
+    parts = []
+    for name, shape in layout:
+        t = torch.empty(shape)
+        if "bias" in name:
+            nn.init.zeros_(t)
+        else:
+            nn.init.xavier_uniform_(t, gain=nn.init.calculate_gain("relu"))
+        parts.append(t.reshape(-1))
+    return torch.cat(parts)
+
+
+def state_dict_to_raw(sd, layout) -> torch.Tensor:
+    return torch.cat([sd[name].detach().float().reshape(-1) for name, _ in layout])
+
+
+def raw_to_state_dict(raw: torch.Tensor, layout) -> dict:
+    out, o = {}, 0
+    for name, shape in layout:
+        k = int(np.prod(shape))
+        out[name] = raw[o:o + k].reshape(shape).clone()
+        o += k
+    return out
+
+
+def _reference_basenet():
+    """BaseNet of an installed HEBO, or None."""
+    try:  # pragma: no cover - depends on the environment
+        from hebo.models.nn.deep_ensemble import BaseNet
+        return BaseNet
+    except Exception:
+        return None
+
+
+def _is_basenet(cls, ref_basenet) -> bool:
+    """basenet_cls names the stock network: the installed reference's BaseNet itself when HEBO is importable; without it,
+    a class named BaseNet defined in a module named deep_ensemble (the reference file loaded some other way).  A subclass
+    or a look-alike elsewhere is not trained as BaseNet: it raises."""
+    if ref_basenet is not None:
+        return cls is ref_basenet
+    return getattr(cls, "__name__", "") == "BaseNet" and str(getattr(cls, "__module__", "")).rsplit(".", 1)[-1] == "deep_ensemble"
+
+
+def _check_categories(Xe, num_uniqs) -> None:
+    """nn.Embedding / F.one_hot raise on a category outside 0 .. num_uniq - 1 (layers.py:34, 50); so does this model."""
+    Xe = torch.as_tensor(Xe)
+    if Xe.numel() == 0:
+        return
+    hi = torch.as_tensor(num_uniqs, dtype=torch.int64, device=Xe.device)
+    if bool((Xe.long() < 0).any()) or bool((Xe.long() >= hi).any()):
+        raise IndexError("categorical index out of range")
+
+
+def _check_perm(perm, E: int, T: int, n: int) -> None:
+    """A caller-given minibatch order must be [E, T, n] with every row a permutation of 0 .. n - 1: hb_de_fit indexes the
+    training rows with it unchecked."""
+    p = torch.as_tensor(perm)
+    if tuple(p.shape) != (E, T, n):
+        raise ValueError(f"perm must be [num_ensembles, num_epochs, n] = [{E}, {T}, {n}], got {list(p.shape)}")
+    if p.numel() and not bool((torch.sort(p.reshape(-1, n).long(), dim=1).values == torch.arange(n, device=p.device)).all()):
+        raise ValueError("every row of perm must be a permutation of 0 .. n - 1")
+
+
+class _PredictWithGrad(torch.autograd.Function):
+    """DeepEnsemble.predict as an autograd node over ``hb_de_predict_grad``."""
+
+    @staticmethod
+    def forward(ctx, Xs, model, xe):
+        mu, var, dmu, dvar = model._predict_dev(Xs, xe, grad=True)
+        ctx.save_for_backward(dmu, dvar)
+        return mu, var
+
+    @staticmethod
+    def backward(ctx, gmu, gvar):
+        dmu, dvar = ctx.saved_tensors          # [m, O, d]
+        return (gmu.unsqueeze(2) * dmu + gvar.unsqueeze(2) * dvar).sum(1), None, None
+
+
+class DeepEnsemble(BaseModel):
+    support_ts = True
+    support_grad = True
+    support_multi_output = True
+    support_warm_start = True
+
+    def __init__(self, num_cont, num_enum, num_out, **conf):
+        super().__init__(num_cont, num_enum, num_out, **conf)
+        self.conf = conf
+        # deep_ensemble.py:36-51 (keys and defaults)
+        self.bootstrap = self.conf.setdefault("bootstrap", False)        # accepted, unused (as in the reference)
+        self.rand_prior = self.conf.setdefault("rand_prior", False)
+        self.output_noise = self.conf.setdefault("output_noise", True)
+        self.num_ensembles = self.conf.setdefault("num_ensembles", 5)
+        self.num_process = self.conf.setdefault("num_processes", 1)      # accepted; one launch trains every member
+        self.num_epochs = self.conf.setdefault("num_epochs", 500)
+        self.print_every = self.conf.setdefault("print_every", 50)
+        self.num_layers = self.conf.setdefault("num_layers", 1)
+        self.num_hiddens = self.conf.setdefault("num_hiddens", 128)
+        self.l1 = self.conf.setdefault("l1", 1e-3)
+        self.batch_size = self.conf.setdefault("batch_size", 32)
+        self.lr = self.conf.setdefault("lr", 5e-3)
+        self.adv_eps = self.conf.setdefault("adv_eps", 0.)              # accepted, unused (as in the reference)
+        self.verbose = self.conf.setdefault("verbose", False)
+        ref_basenet = _reference_basenet()
+        self.basenet_cls = self.conf.setdefault("basenet_cls", ref_basenet)
+        assert self.num_ensembles > 0
+        if self.basenet_cls is not None and not _is_basenet(self.basenet_cls, ref_basenet):
+            raise NotImplementedError("DeepEnsemble: only BaseNet members are supported (basenet_cls)")
+        act = self.conf.get("act", None)
+        if act is not None and type(act) is not nn.ReLU:
+            raise NotImplementedError("DeepEnsemble: only the nn.ReLU activation is supported (act)")
+        # BaseNet's own keys (:189-205)
+        self.noise_lb = float(self.conf.get("noise_lb", 1e-4))
+        self.enum_trans = self.conf.get("enum_trans", "embedding") if num_enum > 0 else "embedding"
+        if self.enum_trans not in ("embedding", "onehot"):
+            raise RuntimeError(f"Unknown enum processing type {self.enum_trans}, can only be [embedding|onehot]")
+        self.num_uniqs = [int(u) for u in self.conf["num_uniqs"]] if num_enum > 0 else []
+        self.device = torch.device(self.conf.get("device", "cuda"))
+        self.layout, self.din = param_layout(num_cont, self.num_uniqs, self.enum_trans, self.num_layers, self.num_hiddens,
+                                             num_out, self.output_noise, self.rand_prior)
+        self._check_envelope()
+        self._c_uniqs = (C.c_int32 * max(1, num_enum))(*self.num_uniqs)
+        self._spec = _lib.DeSpec(num_cont, num_enum, self._c_uniqs,
+                                 _lib.HB_DE_EMBEDDING if self.enum_trans == "embedding" else _lib.HB_DE_ONEHOT,
+                                 self.num_layers, self.num_hiddens, num_out, int(bool(self.output_noise)),
+                                 int(bool(self.rand_prior)), self.noise_lb)
+        self.P = sum(int(np.prod(s)) for _, s in self.layout)
+        self.xscaler = MinMaxScaler((-1, 1))
+        self.yscaler = StandardScaler()
+        self.loss_name = "NLL" if self.output_noise else "MSE"
+        self.params = None          # [E, P] device tensor once fitted (the reference's self.models)
+        self.sample_idx = 0
+        self.noise_est = torch.zeros(self.num_out)
+        self.losses = None
+
+    def _check_envelope(self):
+        L = _lib
+        for what, v, lim in (("num_layers", self.num_layers, L.HB_DE_MAX_LAYERS), ("num_hiddens", self.num_hiddens, L.HB_DE_MAX_HIDDEN),
+                             ("num_out", self.num_out, L.HB_DE_MAX_OUT),
+                             ("input width (num_cont + embedding / one-hot width)", self.din, L.HB_DE_MAX_IN),
+                             ("num_ensembles", self.num_ensembles, L.HB_DE_MAX_MEMBERS)):
+            if v > lim:
+                raise NotImplementedError(f"DeepEnsemble: {what} = {v} exceeds the limit of {lim}")
+        if self.num_layers < 1 or self.num_hiddens < 1:
+            raise NotImplementedError("DeepEnsemble: num_layers and num_hiddens must be at least 1")
+
+    def batch_floats(self, rows: int) -> int:
+        """Shared-memory floats a fit minibatch of `rows` rows needs (HB_DE_MAX_BATCH_FLOATS of include/hebo_b200.h)."""
+        h_ld = max(self.num_hiddens, self.din) | 1
+        return rows * ((self.din | 1) + (self.num_layers + 2) * h_ld + 5 * self.num_out + 1)
+
+    @property
+    def fitted(self):
+        return self.params is not None
+
+    @property
+    def noise(self) -> torch.Tensor:
+        return self.noise_est
+
+    # ------------------------------------------------------------------ scaling (deep_ensemble.py:118-138)
+    def fit_scaler(self, Xc, Xe, y):
+        if Xc is not None and Xc.shape[1] > 0:
+            self.xscaler.fit(Xc)
+        self.yscaler.fit(y)
+
+    def trans(self, Xc, Xe, y=None):
+        if Xc is not None and Xc.shape[1] > 0:
+            Xc_t = self.xscaler.transform(Xc)
+        else:
+            Xc_t = torch.zeros(Xe.shape[0], 0)
+        Xe_t = torch.zeros(Xc.shape[0], 0).long() if Xe is None else Xe.long()
+        if y is not None:
+            return Xc_t, Xe_t, self.yscaler.transform(y)
+        return Xc_t, Xe_t
+
+    # ------------------------------------------------------------------ fit (deep_ensemble.py:71-93, 151-181)
+    def fit(self, Xc_, Xe_, y_, perm=None):
+        """perm: optional [E, num_epochs, n] int32 minibatch order of each member's epochs over the filtered rows (tests);
+        otherwise the device's Philox order under a seed drawn from torch's generator."""
+        y_ = torch.as_tensor(y_).float()
+        if self.num_enum > 0:
+            _check_categories(Xe_, self.num_uniqs)
+        valid = torch.isfinite(y_).any(dim=1)
+        Xc = Xc_[valid] if Xc_ is not None else None
+        Xe = Xe_[valid] if Xe_ is not None else None
+        y = y_[valid]
+        if not self.yscaler.fitted:             # the first fit only: `if self.models is None: self.fit_scaler(...)`
+            self.fit_scaler(Xc, Xe, y)
+        Xc, Xe, y = self.trans(Xc, Xe, y)
+        n, E, dev = y.shape[0], self.num_ensembles, self.device
+        if perm is not None:
+            _check_perm(perm, E, int(self.num_epochs), n)
+        rows = min(n, int(self.batch_size))
+        if self.batch_floats(rows) > _lib.HB_DE_MAX_BATCH_FLOATS:
+            raise NotImplementedError(
+                f"DeepEnsemble: a minibatch of {rows} rows needs {self.batch_floats(rows)} floats of on-chip buffers, over "
+                f"the limit of {_lib.HB_DE_MAX_BATCH_FLOATS} (HB_DE_MAX_BATCH_FLOATS); use a smaller batch_size")
+        if self.params is None:
+            self.params = torch.stack([init_params(self.layout) for _ in range(E)]).to(dev).contiguous()
+        self.seed = int(torch.randint(0, 2 ** 62, (1,)).item())     # the Philox key of this fit's minibatch order
+        self._fit_dev(Xc, Xe, y, perm, self.seed)
+        self.sample_idx = 0
+        with torch.no_grad():
+            py, _ = self.predict(Xc_, Xe_)
+            err = (py - y_)[valid]
+            self.noise_est = (err ** 2).mean(dim=0).detach().clone()
+
+    def _fit_dev(self, Xc, Xe, y, perm, seed):
+        lib, dev, E = _lib.lib(), self.device, self.num_ensembles
+        n, T = y.shape[0], int(self.num_epochs)
+        xc = Xc.to(dev, torch.float32).contiguous() if self.num_cont > 0 else None
+        xe = Xe.to(dev, torch.int32).contiguous() if self.num_enum > 0 else None
+        yd = y.to(dev, torch.float32).contiguous()
+        pd_ = None if perm is None else torch.as_tensor(perm).to(dev, torch.int32).contiguous()
+        need = int(lib.hb_de_fit_workspace_bytes(C.byref(self._spec), E))
+        self.fit_ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        losses = torch.empty(E, max(1, T), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(lib.hb_de_fit(_lib.ptr(xc), _lib.ptr(xe), _lib.ptr(yd), n, C.byref(self._spec), E, _lib.ptr(self.params),
+                                     float(self.lr), float(self.l1), int(self.batch_size), T, _lib.ptr(pd_), seed & (2 ** 64 - 1),
+                                     _lib.ptr(losses), _lib.ptr(self.fit_ws), need, _lib.stream_ptr()), "hb_de_fit")
+        self.losses = losses[:, :T]
+        if self.verbose:
+            L = self.losses.cpu()
+            for i in range(E):
+                for ep in range(0, T, self.print_every):
+                    print("Epoch %d, %s loss = %g" % (ep, self.loss_name, float(L[i, ep])), flush=True)
+
+    def fit_state(self):
+        """Views of the fit workspace: Adam's exp_avg, exp_avg_sq and the last step's gradient, each [E, P]."""
+        w = self.fit_ws.view(torch.float32).view(3, self.num_ensembles, self.P)
+        return w[0], w[1], w[2]
+
+    # ------------------------------------------------------------------ predict (deep_ensemble.py:95-116)
+    def _scal_dev(self):
+        dev = self.device
+        if self.num_cont > 0:
+            xm, xa = self.xscaler.scale_.to(dev).contiguous(), self.xscaler.min_.to(dev).contiguous()
+        else:
+            xm = xa = None
+        return xm, xa, self.yscaler.mean.to(dev).contiguous(), self.yscaler.std.to(dev).contiguous()
+
+    def _inputs(self, Xc, Xe):
+        dev = self.device
+        m = (Xc if (Xc is not None and self.num_cont > 0) else Xe).shape[0]
+        xe = None
+        if self.num_enum > 0:
+            Xe = torch.as_tensor(Xe)
+            if not Xe.is_cuda:          # device categories are not read back (a GA batch is in range by construction);
+                _check_categories(Xe, self.num_uniqs)      # the kernels turn an out-of-range one into a NaN row
+            xe = Xe.to(dev, torch.int32).contiguous()
+        xs = torch.as_tensor(Xc).detach().to(dev, torch.float32).contiguous() if self.num_cont > 0 else None
+        return xs, xe, m
+
+    def _predict_dev(self, Xs, xe, grad=False, member=-1):
+        lib, dev = _lib.lib(), self.device
+        assert self.fitted, "fit() first"
+        m = (Xs if Xs is not None else xe).shape[0]
+        xm, xa, ym, ys = self._scal_dev()
+        mu = torch.empty(m, self.num_out, dtype=torch.float32, device=dev)
+        var = torch.empty(m, self.num_out, dtype=torch.float32, device=dev) if member < 0 else None
+        with torch.cuda.device(dev):
+            if grad:
+                dmu = torch.empty(m, self.num_out, self.num_cont, dtype=torch.float32, device=dev)
+                dvar = torch.empty_like(dmu)
+                _lib.check(lib.hb_de_predict_grad(_lib.ptr(Xs), _lib.ptr(xe), m, C.byref(self._spec), self.num_ensembles,
+                                                  _lib.ptr(self.params), _lib.ptr(xm), _lib.ptr(xa), _lib.ptr(ym), _lib.ptr(ys),
+                                                  _lib.ptr(mu), _lib.ptr(var), _lib.ptr(dmu), _lib.ptr(dvar),
+                                                  _lib.stream_ptr()), "hb_de_predict_grad")
+                return mu, var, dmu, dvar
+            _lib.check(lib.hb_de_predict(_lib.ptr(Xs), _lib.ptr(xe), m, C.byref(self._spec), self.num_ensembles,
+                                         _lib.ptr(self.params), _lib.ptr(xm), _lib.ptr(xa), _lib.ptr(ym), _lib.ptr(ys),
+                                         int(member), _lib.ptr(mu), _lib.ptr(var), _lib.stream_ptr()), "hb_de_predict")
+        return mu, var
+
+    def predict(self, Xc, Xe=None):
+        """(py, ps2) [m, num_out]: CPU tensors for CPU inputs, device tensors for device inputs; an input with
+        requires_grad goes through the input-gradient kernel."""
+        probe = Xc if (Xc is not None and self.num_cont > 0) else Xe
+        on_cpu = not (torch.is_tensor(probe) and probe.is_cuda)
+        xs, xe, m = self._inputs(Xc, Xe)
+        if torch.is_tensor(Xc) and Xc.requires_grad and self.num_cont > 0:
+            mu, var = _PredictWithGrad.apply(Xc.to(self.device, torch.float32).contiguous(), self, xe)
+            return mu.to(Xc.device), var.to(Xc.device)
+        mu, var = self._predict_dev(xs, xe)
+        return (mu.cpu(), var.cpu()) if on_cpu else (mu, var)
+
+    def predict_mace(self, Xc, tau: float, kappa: float, eps: float = 1e-4, xi1=None, xi2=None, seed: int = 0,
+                     return_mu_var: bool = False, Xe=None, device_out: bool = False):
+        """predict + MACE.eval (acq.py:146-171) through ``hb_mace_epilogue``: F [m, 3] = (LCB, -logEI, -logPI), on the
+        input's device (device_out=True: on the GPU for host inputs too).  Single-output models."""
+        assert self.num_out == 1, "MACE needs a single-output model"
+        probe = Xc if (Xc is not None and self.num_cont > 0) else Xe
+        on_cpu = not (torch.is_tensor(probe) and probe.is_cuda) and not device_out
+        xs, xe, m = self._inputs(Xc, Xe)
+        if xi1 is None:
+            xi1 = torch.randn(m, 1)          # acq.py:154-155
+            xi2 = torch.randn(m, 1)
+        dev = self.device
+        xi1 = torch.as_tensor(xi1).reshape(-1).to(dev, torch.float32).contiguous()
+        xi2 = torch.as_tensor(xi2).reshape(-1).to(dev, torch.float32).contiguous()
+        mu, var = self._predict_dev(xs, xe)
+        mu, var = mu.reshape(-1), var.reshape(-1)
+        F = torch.empty(m, 3, dtype=torch.float32, device=dev)
+        if m:
+            with torch.cuda.device(dev):
+                _lib.check(_lib.lib().hb_mace_epilogue(_lib.ptr(mu), _lib.ptr(var), m, float(self.noise[0]), float(tau),
+                                                       float(kappa), float(eps), _lib.ptr(xi1), _lib.ptr(xi2), int(seed),
+                                                       _lib.ptr(F), _lib.stream_ptr()), "hb_mace_epilogue")
+        if on_cpu:
+            F, mu, var = F.cpu(), mu.cpu(), var.cpu()
+        return (F, mu, var) if return_mu_var else F
+
+    def sample_f(self):
+        assert self.fitted
+        idx = self.sample_idx
+        self.sample_idx = (self.sample_idx + 1) % self.num_ensembles
+
+        def f(Xc, Xe):
+            probe = Xc if (Xc is not None and self.num_cont > 0) else Xe
+            on_cpu = not (torch.is_tensor(probe) and probe.is_cuda)
+            xs, xe, _ = self._inputs(Xc, Xe)
+            mu, _ = self._predict_dev(xs, xe, member=idx)
+            return mu.cpu() if on_cpu else mu
+        return f
+
+    def state_dicts(self):
+        """One BaseNet state_dict per member, from the device parameters."""
+        raw = self.params.cpu()
+        return [raw_to_state_dict(raw[i], self.layout) for i in range(self.num_ensembles)]

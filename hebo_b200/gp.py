@@ -741,8 +741,10 @@ def register(name: str = "gp_b200", override_gp: bool = False) -> bool:
         from hebo.models import model_factory
     except Exception:
         return False
+    from .ensemble import DeepEnsemble
     model_factory.model_dict[name] = GP
     model_factory.model_dict["multi_task_b200"] = MultiTaskModel
+    model_factory.model_dict["deep_ensemble_b200"] = DeepEnsemble
     if override_gp:
         model_factory.model_dict["gp"] = GP
     model_factory.model_names = list(model_factory.model_dict.keys())

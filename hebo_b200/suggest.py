@@ -28,6 +28,7 @@ from torch.quasirandom import SobolEngine
 
 from . import _lib
 from .acq import MACE
+from .ensemble import DeepEnsemble
 from .gp import GP
 from .pareto import feasible_front, pareto_front
 from .space import DesignSpace, box_space
@@ -66,8 +67,8 @@ class HEBO:
                  scramble_seed: Optional[int] = None, n_candidates: int = 10000, device: str = "cuda",
                  n_refine: int = 0, refine_sigma: float = 0.05, acq_optimizer: str = "sobol", evo_pop: int = 100,
                  evo_iters: int = 100, lb=None, _constraint=None, model_name: str = "gp", acq_cls=MACE):
-        if model_name != "gp":
-            raise NotImplementedError(f"HEBO: model_name {model_name!r} is not supported, only 'gp'")
+        if model_name not in ("gp", "deep_ensemble"):
+            raise NotImplementedError(f"HEBO: model_name {model_name!r} is not supported, only 'gp' and 'deep_ensemble'")
         if acq_cls is not MACE and (n_refine or _constraint is not None):
             raise ValueError("n_refine and the embedding constraint are defined for the MACE front only; an acq_cls other "
                              "than MACE takes neither")
@@ -111,8 +112,12 @@ class HEBO:
     # ------------------------------------------------------------------ config / data
     @property
     def model_config(self):
-        cfg = ({"lr": 0.01, "num_epochs": 100, "verbose": False, "noise_lb": 8e-4, "pred_likeli": False}       # hebo.py:80-87
-               if self._model_config is None else dict(self._model_config))
+        if self._model_config is not None:
+            cfg = dict(self._model_config)
+        elif self.model_name == "gp":
+            cfg = {"lr": 0.01, "num_epochs": 100, "verbose": False, "noise_lb": 8e-4, "pred_likeli": False}     # hebo.py:80-87
+        else:
+            cfg = {}                                                                                        # hebo.py:94-95
         if self.e > 0:
             cfg["num_uniqs"] = self.space.num_uniqs                                                         # hebo.py:99-100
         return cfg
@@ -189,8 +194,10 @@ class HEBO:
     # ------------------------------------------------------------------ suggest
     def _fit(self):
         """hebo.py:127-147: power-transformed y, and on ANY failure (transform or fit) a refit on the raw y."""
+        cls = GP if self.model_name == "gp" else DeepEnsemble
+
         def build(y):
-            model = GP(self.d, self.e, 1, device=self.device, **self.model_config)
+            model = cls(self.d, self.e, 1, device=self.device, **self.model_config)
             model.fit(self.Xc if self.d else None, self.Xe if self.e else None, y)
             return model
         try:

@@ -480,6 +480,82 @@ int32_t hb_front_pack(const float *F, const float *mu, const float *var, const i
 int32_t hb_front_merge(const float *all_buf, int64_t world, int64_t capacity, float *out, void *ws, int64_t ws_bytes,
                        void *stream);
 
+/* ---- deep-ensemble surrogate (models/nn/deep_ensemble.py: DeepEnsemble :29-181, BaseNet :183-238) -------------------
+ * E members, each BaseNet: inputs [numeric (MinMax-scaled) | embedding or one-hot of each categorical column]
+ * -> (Linear -> ReLU) x num_layers -> heads mu [num_out] (+ prior_net(inputs), not differentiated) and, with output_noise,
+ * sigma2 = noise_lb + softplus(Linear) [num_out].  One member's raw parameters are P = hb_de_num_params(spec) floats in
+ * BaseNet's registration order with torch's [out, in] weight layout, so a state_dict maps to them without permutation:
+ *   enum_layer.emb.{c}.weight [u_c, min(50, 1 + u_c / 2)] (embedding only; models/layers.py:19),
+ *   hidden.{2l}.weight [H, in_l], hidden.{2l}.bias [H] (l < num_layers), mu.weight [O, H], mu.bias [O],
+ *   sigma2.0.weight [O, H], sigma2.0.bias [O] (output_noise), prior_net.{2l}.weight / bias, prior_net.prior_net_out.weight
+ *   [O, H] / bias [O] (rand_prior).
+ * Envelope (HB_ERR_INVALID outside it, hb_de_num_params / hb_de_fit_workspace_bytes return -1): */
+#define HB_DE_MAX_LAYERS   3      /* num_layers                                                                      */
+#define HB_DE_MAX_HIDDEN   256    /* num_hiddens                                                                     */
+#define HB_DE_MAX_OUT      8      /* num_out                                                                         */
+#define HB_DE_MAX_IN       256    /* input width num_cont + sum of embedding (or one-hot) widths                     */
+#define HB_DE_MAX_MEMBERS  32     /* ensemble members E                                                              */
+/* A fit keeps one minibatch's activations on chip: rows B = min(n, batch_size) must satisfy
+ * B * (in_ld + (num_layers + 2) * hid_ld + 5 * num_out + 1) <= HB_DE_MAX_BATCH_FLOATS, with in_ld = in | 1 and
+ * hid_ld = max(num_hiddens, in) | 1 (odd leading dimensions).  BaseNet's defaults (batch 32) fit with room to spare at every
+ * layer / width / output count above. */
+#define HB_DE_MAX_BATCH_FLOATS 56000
+
+#define HB_DE_EMBEDDING    0      /* conf['enum_trans'] = 'embedding' (deep_ensemble.py:199-201) */
+#define HB_DE_ONEHOT       1      /* conf['enum_trans'] = 'onehot'    (deep_ensemble.py:202-203) */
+
+typedef struct {                  /* HOST struct */
+  int32_t        num_cont;        /* numeric columns                                                   */
+  int32_t        num_enum;        /* categorical columns                                               */
+  const int32_t *num_uniqs;       /* HOST [num_enum] categories per column (conf['num_uniqs'])         */
+  int32_t        enum_trans;      /* HB_DE_EMBEDDING | HB_DE_ONEHOT                                     */
+  int32_t        num_layers;      /* conf['num_layers'] (default 1)                                    */
+  int32_t        num_hiddens;     /* conf['num_hiddens'] (default 128)                                 */
+  int32_t        num_out;         /* outputs                                                           */
+  int32_t        output_noise;    /* conf['output_noise'] (default 1): sigma2 head and NLL loss, else MSE */
+  int32_t        rand_prior;      /* conf['rand_prior'] (default 0): fixed random prior network         */
+  float          noise_lb;        /* conf['noise_lb'] (default 1e-4)                                   */
+} hb_de_spec_t;
+
+/* P of one member, or -1 outside the envelope (HOST). */
+int64_t hb_de_num_params(const hb_de_spec_t *spec);
+/* Workspace of hb_de_fit: 3 E P floats laid out as Adam's exp_avg [E, P], exp_avg_sq [E, P] and the gradient of the last
+ * step [E, P] (data term + L1 term), all readable after the call.  -1 outside the envelope (HOST). */
+int64_t hb_de_fit_workspace_bytes(const hb_de_spec_t *spec, int64_t E);
+/* DeepEnsemble.fit's member loop (deep_ensemble.py:81-85) and fit_one (:151-181) for all E members in ONE launch, one CTA
+ * per member, with no host round trip: per epoch a permutation of the n rows, minibatches of batch_size rows (the last
+ * partial batch dropped iff n > batch_size; n <= batch_size gives one batch of n rows), per step forward, the data loss
+ * (NLL 0.5 (t - mu)^2 / sigma2 + 0.5 log sigma2, or MSE, over the finite entries of y), its backward, the L1 term
+ * l1 sum|p| / (n num_out) over all parameters, and torch.optim.Adam (0.9, 0.999, eps 1e-8; fresh moments; lr a double as
+ * torch keeps it, its bias corrections computed in double per step and rounded to fp32 where torch rounds them).
+ *   Xc [n, num_cont] MinMax-scaled (NULL iff num_cont = 0), Xe [n, num_enum] int32 (NULL iff num_enum = 0), y [n, num_out]
+ *   standardised (non-finite entries are masked out of the loss; every row needs one finite entry).
+ *   params [E, P] in/out.  perm: NULL, or [E, num_epochs, n] int32 rows of each member's epoch in order, for tests that
+ *   replay a given order; every row must be a permutation of 0..n-1, which the library does not check (the caller must:
+ *   hebo_b200.DeepEnsemble.fit does).  Categories outside 0 .. num_uniqs[c] - 1 load NaN (never a read outside a table).  With perm = NULL the order is a keyed Philox bijection of (seed, member, epoch): positions are
+ *   mapped through a 4-round Feistel network on 2h bits (2^(2h) >= n, round r keyed by word 0 of the Philox4x32-10 block
+ *   of counter (half, epoch, member, 0x44450000 + r) under `seed`) and cycle-walked into 0..n-1.
+ *   losses [E, num_epochs]: epoch_loss / n as the reference prints it (:176-179).
+ * Every reduction runs in a fixed order, so the result is bit-identical from run to run.  No host synchronisation. */
+int32_t hb_de_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec, int64_t E,
+                  float *params, double lr, float l1, int64_t batch_size, int64_t num_epochs, const int32_t *perm,
+                  uint64_t seed, float *losses, void *ws, int64_t ws_bytes, void *stream);
+/* DeepEnsemble.predict (deep_ensemble.py:95-106) of m candidates: Xs [m, num_cont] raw inputs scaled in the load as
+ * x * x_mul + x_add (the MinMax scaler's transform), Xe [m, num_enum] int32.  Members combine in index order:
+ *   output_noise: py = mean(mu), ps2 = var(mu, unbiased=False) + mean(sigma2); else py = mean(mu), ps2 = 1e-8 + var(mu)
+ * then py * y_std + y_mean, ps2 * y_std^2 (y_mean / y_std [num_out] device arrays).  mu / var [m, num_out].
+ * member >= 0: member's own mu, un-scaled, alone (sample_f, :108-116; var may be NULL).  A category outside
+ * 0 .. num_uniqs[c] - 1 gives that row NaN outputs.  No host synchronisation. */
+int32_t hb_de_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t E,
+                      const float *params, const float *x_mul, const float *x_add, const float *y_mean, const float *y_std,
+                      int32_t member, float *mu, float *var, void *stream);
+/* hb_de_predict (member = -1) and its input gradients dmu, dvar [m, num_out, num_cont] with respect to the raw numeric
+ * inputs, through the ReLU masks of every member (prior_net's output is a constant, as under the reference's no_grad).
+ * num_cont >= 1.  No host synchronisation. */
+int32_t hb_de_predict_grad(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t E,
+                           const float *params, const float *x_mul, const float *x_add, const float *y_mean,
+                           const float *y_std, float *mu, float *var, float *dmu, float *dvar, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
