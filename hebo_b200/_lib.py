@@ -73,6 +73,10 @@ SIGNATURES = {
     "hb_cholesky": (_i32, [_vp, _i64, _vp, _vp, _vp]),
     "hb_tri_inverse": (_i32, [_vp, _i64, _vp, _vp, _vp]),
     "hb_kinv": (_i32, [_vp, _i64, _vp, _vp]),
+    "hb_tc_workspace_bytes": (_i64, [_i64]),
+    "hb_cholesky_tc": (_i32, [_vp, _i64, _vp, _vp, _vp, _i64, _vp]),
+    "hb_tri_inverse_tc": (_i32, [_vp, _i64, _vp, _vp, _i64, _vp]),
+    "hb_kinv_tc": (_i32, [_i64, _vp, _vp, _i64, _vp]),
     "hb_solve_logdet": (_i32, [_vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp]),
     "hb_mll_grad": (_i32, [_vp, _i64, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _f32, _vp, _vp, _vp, _vp]),
     "hb_psgld_step": (_i32, [_vp, _vp, _vp, _i64, _f32, _f32, _f32, _f32, _vp, _vp]),

@@ -125,6 +125,39 @@ static void fill_meta_host(const hb_model_spec_t *c, const ModelSpec &sp, std::v
   }
 }
 
+// The hi/lo companion buffers of the tensor-core stages, in this order: Linv_hi, Linv_lo, L_hi, L_lo, U_hi, U_lo, T_hi, T_lo
+// ([NP, NP] each) and P_hi, P_lo ([NP, 512]), each block 256-byte aligned.  The fit workspace and the stand-alone
+// tensor-core entry points (hb_tc_workspace_bytes) both carve them here, so the two layouts are one.
+template <class Take> static TcBuffers carve_tc(Take &take, int64_t np) {
+  const size_t sq = (size_t)np * np * 4, panel = (size_t)np * 512 * 4;
+  TcBuffers tc;
+  tc.Linv_hi = (float *)take(sq);
+  tc.Linv_lo = (float *)take(sq);
+  tc.L_hi = (float *)take(sq);
+  tc.L_lo = (float *)take(sq);
+  tc.U_hi = (float *)take(sq);
+  tc.U_lo = (float *)take(sq);
+  tc.T_hi = (float *)take(sq);
+  tc.T_lo = (float *)take(sq);
+  tc.P_hi = (float *)take(panel);
+  tc.P_lo = (float *)take(panel);
+  return tc;
+}
+
+// TcBuffers of a stand-alone tensor-core workspace at `base` (nullptr: only counts); `bytes` = its size
+static TcBuffers carve_tc_ws(void *base, int64_t np, size_t &bytes) {
+  unsigned char *p = reinterpret_cast<unsigned char *>(base);
+  size_t off = 0;
+  auto take = [&](size_t b) {
+    void *r = p ? (void *)(p + off) : nullptr;
+    off += al256(b);
+    return r;
+  };
+  const TcBuffers tc = carve_tc(take, np);
+  bytes = off;
+  return tc;
+}
+
 static FitWs carve_fit(void *base, int64_t n, const ModelSpec &sp) {
   const int64_t np = round_up(n, TILE);
   const int64_t P = sp.P(), H = sp.H();
@@ -146,18 +179,9 @@ static FitWs carve_fit(void *base, int64_t n, const ModelSpec &sp) {
   w.L = (float *)take((size_t)np * np * 4);
   w.Linv = (float *)take((size_t)np * np * 4);
   w.tmp = (float *)take((size_t)np * np * 4);
-  w.Linv_hi = (float *)take((size_t)np * np * 4);
-  w.Linv_lo = (float *)take((size_t)np * np * 4);
-  w.tc.Linv_hi = w.Linv_hi;
-  w.tc.Linv_lo = w.Linv_lo;
-  w.tc.L_hi = (float *)take((size_t)np * np * 4);
-  w.tc.L_lo = (float *)take((size_t)np * np * 4);
-  w.tc.U_hi = (float *)take((size_t)np * np * 4);
-  w.tc.U_lo = (float *)take((size_t)np * np * 4);
-  w.tc.T_hi = (float *)take((size_t)np * np * 4);
-  w.tc.T_lo = (float *)take((size_t)np * np * 4);
-  w.tc.P_hi = (float *)take((size_t)np * 512 * 4);
-  w.tc.P_lo = (float *)take((size_t)np * 512 * 4);
+  w.tc = carve_tc(take, np);
+  w.Linv_hi = w.tc.Linv_hi;
+  w.Linv_lo = w.tc.Linv_lo;
   w.alpha = (float *)take((size_t)np * 4);
   w.Zt = (float *)take((size_t)sp.dtot() * np * 4);
   w.Ets = w.Zt ? w.Zt + (size_t)sp.d * np : nullptr;
@@ -466,6 +490,40 @@ int32_t hb_tri_inverse(const float *L, int64_t np, float *Linv, float *tmp, void
 int32_t hb_kinv(const float *Linv, int64_t np, float *Kinv, void *stream) {
   if (!Linv || !Kinv) return HB_ERR_INVALID;
   return launch_kinv(Linv, np, Kinv, (cudaStream_t)stream);
+}
+
+// the tensor-core twins: the same launchers the fit epoch runs (enqueue_mll with tc != nullptr), one stage at a time
+static bool tc_np_ok(int64_t np) { return np > 0 && np % TILE == 0; }
+static bool open_tc_ws(void *tc_ws, int64_t tc_ws_bytes, int64_t np, TcBuffers &tc) {
+  if (!tc_ws || !tc_np_ok(np)) return false;
+  size_t need = 0;
+  tc = carve_tc_ws(tc_ws, np, need);
+  return tc_ws_bytes >= 0 && (uint64_t)tc_ws_bytes >= need;
+}
+
+int64_t hb_tc_workspace_bytes(int64_t np) {
+  if (!tc_np_ok(np)) return -1;
+  size_t bytes = 0;
+  carve_tc_ws(nullptr, np, bytes);
+  return (int64_t)bytes;
+}
+
+int32_t hb_cholesky_tc(float *A, int64_t np, float *ws, int32_t *info, void *tc_ws, int64_t tc_ws_bytes, void *stream) {
+  TcBuffers tc;
+  if (!A || !ws || !info || !open_tc_ws(tc_ws, tc_ws_bytes, np, tc)) return HB_ERR_INVALID;
+  return launch_cholesky(A, np, ws, info, (cudaStream_t)stream, &tc);
+}
+
+int32_t hb_tri_inverse_tc(const float *L, int64_t np, float *Linv, void *tc_ws, int64_t tc_ws_bytes, void *stream) {
+  TcBuffers tc;
+  if (!L || !Linv || !open_tc_ws(tc_ws, tc_ws_bytes, np, tc)) return HB_ERR_INVALID;
+  return launch_tri_inverse_tc(L, np, Linv, tc, true, (cudaStream_t)stream, Batch());
+}
+
+int32_t hb_kinv_tc(int64_t np, float *Kinv, void *tc_ws, int64_t tc_ws_bytes, void *stream) {
+  TcBuffers tc;
+  if (!Kinv || !open_tc_ws(tc_ws, tc_ws_bytes, np, tc)) return HB_ERR_INVALID;
+  return launch_kinv_tc(np, Kinv, tc, (cudaStream_t)stream, Batch());
 }
 
 int32_t hb_solve_logdet(const float *L, const float *Linv, const float *y, int64_t n, int64_t np, const float *hyp,

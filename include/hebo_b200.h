@@ -143,6 +143,23 @@ int32_t hb_cholesky(float *A, int64_t np, float *ws, int32_t *info, void *stream
 int32_t hb_tri_inverse(const float *L, int64_t np, float *Linv, float *tmp, void *stream);
 int32_t hb_kinv(const float *Linv, int64_t np, float *Kinv, void *stream);
 
+/* ---- Tensor-core twins of hb_cholesky / hb_tri_inverse / hb_kinv: the stages every pSGLD epoch of hb_fit* runs, with
+ * their O(NP^3) GEMMs on the 3xTF32 tensor cores (each fp32 operand split hi + lo, products hi*hi + hi*lo + lo*hi).
+ * tc_ws: device workspace of >= hb_tc_workspace_bytes(np) bytes (tc_ws_bytes = its size), laid out like the fit
+ * workspace's own tensor-core block: the hi/lo copies of L, L^-1, U = L^-T, the doubling products and the Cholesky panel.
+ * NP > 0 and a multiple of 128, no NULL pointer and a large enough tc_ws, otherwise HB_ERR_INVALID before any launch.
+ * hb_cholesky_tc     as hb_cholesky; the trailing update right of each 512-column outer block on the tensor cores.
+ * hb_tri_inverse_tc  Linv = L^-1 (lower; Linv and the strict upper triangles of the hi/lo copies are zero-filled first).
+ *                    128 x 128 diagonal blocks on the FP32 pipe, the doubling levels on the tensor cores; also leaves
+ *                    the split of U = Linv^T in tc_ws.
+ * hb_kinv_tc         Kinv = U U^T from the U that the last hb_tri_inverse_tc left in the same tc_ws: every lower 128-tile,
+ *                    and an upper tile only where a 256-column output tile of its tile row overhangs the diagonal
+ *                    (columns < min(NP, round_up(r0 + 128, 256)) of tile row r0); nothing else is written. */
+int64_t hb_tc_workspace_bytes(int64_t np);
+int32_t hb_cholesky_tc(float *A, int64_t np, float *ws, int32_t *info, void *tc_ws, int64_t tc_ws_bytes, void *stream);
+int32_t hb_tri_inverse_tc(const float *L, int64_t np, float *Linv, void *tc_ws, int64_t tc_ws_bytes, void *stream);
+int32_t hb_kinv_tc(int64_t np, float *Kinv, void *tc_ws, int64_t tc_ws_bytes, void *stream);
+
 /* ---- alpha, quadratic form, log-det  (the data term of ExactMarginalLogLikelihood,
  * models/gp/gp.py:102,113; alpha is also the prediction-strategy mean cache, gp.py:148) --------
  * r = y - c (pad = 0).  alpha = Khat^-1 r, quad = r^T Khat^-1 r, logdet = 2 sum log L_ii.

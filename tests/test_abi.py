@@ -96,6 +96,40 @@ def test_linalg_stages_reject_bad_sizes_and_null_pointers(lib):
         assert lib.hb_solve_logdet(L, Linv, y, 10, 128, hyp, alpha, scal, ws, None) == bad, k
 
 
+def test_tensor_core_stages_reject_bad_sizes_null_pointers_and_short_workspaces(lib):
+    """hb_cholesky_tc, hb_tri_inverse_tc and hb_kinv_tc refuse NP <= 0 or not a multiple of 128, every NULL pointer, and a
+    tensor-core workspace one byte short or of negative size, with HB_ERR_INVALID before any launch.  The workspace size is
+    the fit workspace's tensor-core block: 8 NP^2 + 2 * 512 NP floats (every block a multiple of 256 bytes here).  The
+    pointers are fake and never dereferenced."""
+    bad = _lib.HB_ERR_INVALID
+    p = ctypes.c_void_p(16)
+    for np_ in (128, 640, 4224):
+        assert lib.hb_tc_workspace_bytes(np_) == 4 * (8 * np_ * np_ + 2 * 512 * np_), np_
+    big = lib.hb_tc_workspace_bytes(4224)
+    for np_ in (0, -128, 100, 129, 200):
+        assert lib.hb_tc_workspace_bytes(np_) < 0, np_
+        assert lib.hb_cholesky_tc(p, np_, p, p, p, big, None) == bad, np_
+        assert lib.hb_tri_inverse_tc(p, np_, p, p, big, None) == bad, np_
+        assert lib.hb_kinv_tc(np_, p, p, big, None) == bad, np_
+    for k in range(4):
+        args = [p] * 4                      # A, ws, info, tc_ws
+        args[k] = None
+        assert lib.hb_cholesky_tc(args[0], 128, args[1], args[2], args[3], big, None) == bad, k
+    for k in range(3):
+        args = [p] * 3                      # L, Linv, tc_ws
+        args[k] = None
+        assert lib.hb_tri_inverse_tc(args[0], 128, args[1], args[2], big, None) == bad, k
+    for k in range(2):
+        args = [p] * 2                      # Kinv, tc_ws
+        args[k] = None
+        assert lib.hb_kinv_tc(128, args[0], args[1], big, None) == bad, k
+    need = lib.hb_tc_workspace_bytes(640)
+    for short in (need - 1, -1, -(1 << 40)):
+        assert lib.hb_cholesky_tc(p, 640, p, p, p, short, None) == bad, short
+        assert lib.hb_tri_inverse_tc(p, 640, p, p, short, None) == bad, short
+        assert lib.hb_kinv_tc(640, p, p, short, None) == bad, short
+
+
 @pytest.mark.parametrize("ws_bytes", ["short", -1, -(1 << 40)])
 def test_workspace_size_is_checked_as_a_signed_count(lib, ws_bytes):
     """A workspace one byte short, or of negative size, is refused before any launch.  A negative int64 must not pass the
