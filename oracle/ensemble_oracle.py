@@ -200,3 +200,243 @@ def perm(seed: int, member: int, epoch: int, n: int) -> np.ndarray:
         bad = x >= n
         x[bad] = feistel(x[bad])
     return x.astype(np.int64)
+
+
+# ------------------------------------------------------------------------------------------------ fp32 restatement
+# hebo_b200/csrc/ensemble.cu operation by operation, each rounded as the device rounds it: every sum of products is a
+# sequential fmaf chain from 0 in the kernel's index order, everything else a single IEEE fp32 operation.  With
+# output_noise=False nothing else enters a fit step, predict or the input gradients, so these functions equal the device
+# bit for bit.  Arrays are numpy float32; the row-wise stages take only the rows they are given, so a caller may restate
+# chosen rows of a large predict.
+fma32 = rng_oracle.fma32
+f32 = np.float32
+
+
+class Net32:
+    """One member's DeNet: shapes, and the raw-vector slice of every parameter from OracleNet's registration order."""
+
+    def __init__(self, num_cont, num_uniqs, enum_trans="embedding", num_layers=1, num_hiddens=128, num_out=1,
+                 output_noise=False, rand_prior=False, noise_lb=1e-4):
+        ref = OracleNet(num_cont, num_uniqs, enum_trans, num_layers, num_hiddens, num_out, output_noise, rand_prior, noise_lb)
+        self.dc, self.uniqs, self.emb = num_cont, list(num_uniqs), enum_trans == "embedding"
+        self.L, self.H, self.O, self.noise, self.prior = num_layers, num_hiddens, num_out, output_noise, rand_prior
+        self.widths = [min(50, 1 + u // 2) if self.emb else u for u in self.uniqs]
+        self.din = num_cont + sum(self.widths)
+        self.slices, o = {}, 0
+        for name, p in ref.named_parameters():
+            self.slices[name] = (o, tuple(p.shape))
+            o += p.numel()
+        self.P = o
+        self.prior0 = min([s[0] for k, s in self.slices.items() if k.startswith("prior_net")], default=o)
+
+    def view(self, prm, name):
+        o, shape = self.slices[name]
+        return prm[o:o + int(np.prod(shape))].reshape(shape)
+
+
+def load_inputs32(net, prm, Xc, Xe, x_mul=None, x_add=None):
+    """de_load_inputs: numeric columns (x_mul x + x_add, two roundings, when x_mul is given), then the embedding rows or
+    one-hot codes of the categorical columns.  Xc [B, dc] fp32, Xe [B, ne] int."""
+    cols = []
+    if net.dc:
+        x = f32(Xc)
+        if x_mul is not None:
+            x = f32(x_mul) * x + f32(x_add)
+        cols.append(x)
+    for c, u in enumerate(net.uniqs):
+        cat = np.asarray(Xe)[:, c]
+        if net.emb:
+            cols.append(net.view(prm, f"enum_layer.emb.{c}.weight")[cat])
+        else:
+            cols.append((cat[:, None] == np.arange(u)[None, :]).astype(f32))
+    return np.concatenate(cols, 1).astype(f32)
+
+
+def dense32(x, W, b, relu, add=None):
+    """de_dense: acc = 0, fmaf over k ascending, + bias, ReLU (v < 0 -> 0), + add."""
+    acc = np.zeros((x.shape[0], W.shape[0]), f32)
+    for k in range(W.shape[1]):
+        acc = fma32(x[:, k:k + 1], W[None, :, k], acc)
+    v = acc + b
+    if relu:
+        v = np.where(v < 0, f32(0), v)
+    return v if add is None else v + add
+
+
+def forward32(net, prm, xin):
+    """de_forward: (hidden activations [L][B, H], mu head [B, O] with the prior net's output added, sigma2 head's
+    pre-softplus z [B, O] or None)."""
+    V = lambda name: net.view(prm, name)
+    pri = None
+    if net.prior:
+        h = xin
+        for l in range(net.L):
+            h = dense32(h, V(f"prior_net.{2 * l}.weight"), V(f"prior_net.{2 * l}.bias"), True)
+        pri = dense32(h, V("prior_net.prior_net_out.weight"), V("prior_net.prior_net_out.bias"), False)
+    acts, h = [], xin
+    for l in range(net.L):
+        h = dense32(h, V(f"hidden.{2 * l}.weight"), V(f"hidden.{2 * l}.bias"), True)
+        acts.append(h)
+    mu = dense32(h, V("mu.weight"), V("mu.bias"), False, pri)
+    z = dense32(h, V("sigma2.0.weight"), V("sigma2.0.bias"), False) if net.noise else None
+    return acts, mu, z
+
+
+def relu_mask32(a, d):
+    """The delta d where the layer's output a is positive, else +0."""
+    return np.where(a > 0, d, f32(0))
+
+
+def fma_over_rows32(d, x):
+    """sum_p d[p, :, None] x[p, None, :]: one fmaf chain per element over the rows p ascending."""
+    acc = np.zeros((d.shape[1], x.shape[1]), f32)
+    for p in range(d.shape[0]):
+        acc = fma32(d[p][:, None], x[p][None, :], acc)
+    return acc
+
+
+def sum_rows32(d):
+    acc = np.zeros(d.shape[1], f32)
+    for p in range(d.shape[0]):
+        acc = acc + d[p]
+    return acc
+
+
+def backward32(net, prm, xin, acts, dmu, dz, grads, k0=None):
+    """de_backward from head seeds dmu, dz [B, O]: ({name: gradient} when grads, else None; the input delta's columns
+    k0: of [B, din] when k0 is not None, else None)."""
+    V = lambda name: net.view(prm, name)
+    aL, g = acts[-1], {} if grads else None
+    if grads:
+        g["mu.weight"], g["mu.bias"] = fma_over_rows32(dmu, aL), sum_rows32(dmu)
+        if net.noise:
+            g["sigma2.0.weight"], g["sigma2.0.bias"] = fma_over_rows32(dz, aL), sum_rows32(dz)
+    acc = np.zeros_like(aL)
+    for o in range(net.O):
+        acc = fma32(dmu[:, o:o + 1], V("mu.weight")[None, o], acc)
+        if net.noise:
+            acc = fma32(dz[:, o:o + 1], V("sigma2.0.weight")[None, o], acc)
+    cur = relu_mask32(aL, acc)
+    for l in reversed(range(net.L)):
+        inp = xin if l == 0 else acts[l - 1]
+        W = V(f"hidden.{2 * l}.weight")
+        if grads:
+            g[f"hidden.{2 * l}.weight"], g[f"hidden.{2 * l}.bias"] = fma_over_rows32(cur, inp), sum_rows32(cur)
+        if l > 0 or k0 is not None:
+            kb = 0 if l > 0 else k0
+            acc = np.zeros((cur.shape[0], W.shape[1] - kb), f32)
+            for j in range(net.H):
+                acc = fma32(cur[:, j:j + 1], W[None, j, kb:], acc)
+            cur = relu_mask32(inp, acc) if l > 0 else acc
+    return g, (cur if k0 is not None else None)
+
+
+def scatter32(net, dx, Xe):
+    """The embedding tables' gradients: the input delta dx [B, din - dc] of each row added into the row of its
+    category, plain fp32 adds in minibatch-row order from +0 (categories never drawn keep +0)."""
+    out = {}
+    for c, (u, w) in enumerate(zip(net.uniqs, net.widths)):
+        c0 = sum(net.widths[:c])
+        tab = np.zeros((u, w), f32)
+        for p in range(dx.shape[0]):
+            cat = int(Xe[p, c])
+            tab[cat] = tab[cat] + dx[p, c0:c0 + w]
+        out[f"enum_layer.emb.{c}.weight"] = tab
+    return out
+
+
+def minibatch_rule(n: int, batch: int):
+    """(rows per step, steps per epoch): B = min(n, batch); drop_last = n > batch, so the partial minibatch is dropped."""
+    return min(n, batch), (n // batch if n > batch else 1)
+
+
+def step_grad32(net, prm, Xc, Xe, y, rows, n, l1):
+    """One minibatch's gradient as hb_de_fit forms it, output_noise=False: MSE seeds -2 (t - mu) / cnt over the finite
+    targets, de_backward, the embedding scatter, plus the L1 term (1 / (float)(n O)) l1 sign(p).  The prior net's
+    parameters get the L1 term only.  Returns the total gradient [P]."""
+    assert not net.noise, "the fp32 restatement covers output_noise=False (the NLL path goes through expf / log1pf / logf)"
+    rows = np.asarray(rows)
+    xc = f32(Xc)[rows] if net.dc else None
+    xe = np.asarray(Xe)[rows] if net.uniqs else None
+    xin = load_inputs32(net, prm, xc, xe)
+    acts, mu, _ = forward32(net, prm, xin)
+    t = f32(y)[rows]
+    fin = np.isfinite(t)
+    cnt = f32(fin.sum())
+    with np.errstate(invalid="ignore"):
+        gmu = np.where(fin, (f32(-2.0) * (t - mu)) / cnt, f32(0))
+    want_in = net.emb and len(net.uniqs) > 0
+    g, dx = backward32(net, prm, xin, acts, gmu, np.zeros_like(gmu), True, net.dc if want_in else None)
+    if want_in:
+        g.update(scatter32(net, dx, xe))
+    gd = np.zeros(net.P, f32)
+    for name, v in g.items():
+        o, shape = net.slices[name]
+        gd[o:o + v.size] = v.reshape(-1)
+    coef = (f32(1.0) / f32(n * net.O)) * f32(l1)
+    sg = np.where(prm > 0, f32(1), np.where(prm < 0, f32(-1), f32(0)))
+    return gd + coef * sg
+
+
+def fit32(net, prm0, Xc, Xe, y, orders, lr: float, l1: float, batch: int):
+    """One member of hb_de_fit over the given orders [epochs, n]: (params, exp_avg, exp_avg_sq, last gradient)."""
+    n = y.shape[0]
+    B, nb = minibatch_rule(n, batch)
+    p = f32(prm0).copy()
+    m1, m2, g = (np.zeros(net.P, f32) for _ in range(3))
+    step = 0
+    for order in orders:
+        for b in range(nb):
+            step += 1
+            g = step_grad32(net, p, Xc, Xe, y, order[b * B:(b + 1) * B], n, l1)
+            p, m1, m2 = adam_update_f32(p, g, m1, m2, step, lr)
+    return p, m1, m2, g
+
+
+def predict32(net, params, Xs, Xe, x_mul, x_add, y_mean, y_std, member=-1, grad=False):
+    """de_predict_kernel<grad> on the given rows: (mu, var) [B, O] un-scaled, and with grad (dmu, dvar) [B, O, dc].
+    params [E, P]; member >= 0 restates that member alone (var 0).  The members combine in the order of params."""
+    E = params.shape[0]
+    members = [member] if member >= 0 else list(range(E))
+    ne = f32(len(members))
+    ys, ym = f32(y_std), f32(y_mean)
+    state = []
+    for e in members:
+        xin = load_inputs32(net, params[e], Xs, Xe, x_mul, x_add)
+        state.append((params[e], xin) + forward32(net, params[e], xin))
+    mus = [s[3] for s in state]
+    if member >= 0:
+        mean, v = mus[0], np.zeros_like(mus[0])
+    else:
+        mean = np.zeros_like(mus[0])
+        for m in mus:
+            mean = mean + m
+        mean = mean / ne
+        v = np.zeros_like(mean)
+        for m in mus:
+            d = m - mean
+            v = fma32(d, d, v)
+        v = f32(1e-8) + v / ne
+    out = (mean * ys + ym, v * (ys * ys))
+    if not grad:
+        return out
+    B, O, dc = mean.shape[0], net.O, net.dc
+    dmu, dvar = np.zeros((B, O, dc), f32), np.zeros((B, O, dc), f32)
+    invE = f32(1.0) / ne
+    for prm, xin, acts, mu_e, _ in state:
+        for o in range(O):
+            for ps, dst in ((0, dmu), (1, dvar)):
+                seed = np.zeros((B, O), f32)
+                seed[:, o] = invE if ps == 0 else (f32(2.0) * invE) * (mu_e[:, o] - mean[:, o])
+                _, dx = backward32(net, prm, xin, acts, seed, np.zeros_like(seed), False, 0)
+                sc = ys[o] if ps == 0 else ys[o] * ys[o]
+                dst[:, o, :] = dst[:, o, :] + (dx[:, :dc] * f32(x_mul)) * sc
+    return out + (dmu, dvar)
+
+
+def mismatches(got, want) -> int:
+    """Elements whose bits differ (NaN equals NaN only with the same bits)."""
+    a = np.ascontiguousarray(np.asarray(got, dtype=np.float32)).view(np.uint32)
+    b = np.ascontiguousarray(np.asarray(want, dtype=np.float32)).view(np.uint32)
+    assert a.shape == b.shape, (a.shape, b.shape)
+    return int((a != b).sum())

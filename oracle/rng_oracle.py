@@ -174,11 +174,16 @@ def fma32(a, b, c) -> np.ndarray:
     return r.astype(np.float32)
 
 
+F32_OVERFLOW = Fraction(float(np.finfo(np.float32).max)) + Fraction(2) ** 103     # half an ulp above the largest float
+
+
 def fma32_exact(a: float, b: float, c: float) -> np.float32:
     """fmaf(a, b, c) by rational arithmetic, for checking fma32."""
     v = Fraction(float(a)) * Fraction(float(b)) + Fraction(float(c))
+    if abs(v) >= F32_OVERFLOW:                # ties to even round the midpoint above the largest float up to inf
+        return np.float32(np.inf if v > 0 else -np.inf)
     lo = np.float32(float(v))                 # float(Fraction) rounds correctly to fp64; step to the fp32 neighbours
-    cands = [np.nextafter(lo, np.float32(-np.inf)), lo, np.nextafter(lo, np.float32(np.inf))]
+    cands = [x for x in (np.nextafter(lo, np.float32(-np.inf)), lo, np.nextafter(lo, np.float32(np.inf))) if np.isfinite(x)]
     best = min(cands, key=lambda x: (abs(Fraction(float(x)) - v), int(np.float32(x).view(np.uint32)) & 1))
     return np.float32(best)
 

@@ -1,6 +1,8 @@
 """Shared helpers for the test-suite (test infrastructure; may import oracle/)."""
 from __future__ import annotations
 
+import contextlib
+import copy
 import math
 import os
 
@@ -397,3 +399,271 @@ def true_model(gp, X, Xe, y):
     alpha = torch.cholesky_solve((yt64.to(DEV) - c).reshape(-1, 1), L).reshape(-1)
     _TRUE[key] = dict(Zt=Zt, L=L, alpha=alpha, hyp=hyp, tables=tables, c=c, raw=gp.raw)
     return _TRUE[key]
+
+
+# ---------------------------------------------------------------------------------------------------- deep ensemble
+# The envelope of ensemble.cu at the shapes where its strided loops and leading dimensions matter (the row-float counts
+# follow HB_DE_MAX_BATCH_FLOATS of include/hebo_b200.h).  Each case: the net, its data (n rows, the minibatch size) and
+# the input generator's category range per column.
+DE_CASES = {
+    # 1583 floats per row: B = 35 is the largest admitted minibatch; n = 75 drops 5 rows per epoch
+    "corner": dict(net=dict(num_cont=256, num_uniqs=[], num_layers=3, num_hiddens=256, num_out=8, rand_prior=True),
+                   n=75, batch=35),
+    # din = 6 + 5 x 50 = 256 > H: the input delta runs on h_ld = 257; column 0 draws 40 of 120 categories (repeats within a
+    # minibatch, rows never drawn)
+    "emb-wide": dict(net=dict(num_cont=6, num_uniqs=[120] * 5, num_layers=3, num_hiddens=16, num_out=3), n=70, batch=32,
+                     cat_hi=[40, 120, 120, 120, 120]),
+    "onehot-wide": dict(net=dict(num_cont=2, num_uniqs=[200, 54], enum_trans="onehot", num_layers=2, num_hiddens=8,
+                                 num_out=2), n=70, batch=32),
+    "default": dict(net=dict(num_cont=5, num_uniqs=[]), n=70, batch=32, E=5),
+    "default-prior": dict(net=dict(num_cont=5, num_uniqs=[], rand_prior=True), n=70, batch=32, E=5),
+    # 10 floats per row: B = 5600 is exactly the limit; n = 11 201 drops one row per epoch
+    "big-batch": dict(net=dict(num_cont=1, num_uniqs=[], num_layers=1, num_hiddens=1), n=11201, batch=5600),
+    # output 5 is NaN on every row, and row i has i % 7 more NaN outputs: 1 ... 7 per row
+    "holes": dict(net=dict(num_cont=3, num_uniqs=[4, 7], num_layers=2, num_hiddens=64, num_out=8), n=70, batch=32,
+                  holes=True),
+    "small-n1": dict(net=dict(num_cont=2, num_uniqs=[3], num_layers=1, num_hiddens=8, num_out=2), n=1, batch=8),
+    "small-n8": dict(net=dict(num_cont=2, num_uniqs=[3], num_layers=1, num_hiddens=8, num_out=2), n=8, batch=8),
+    "small-n9": dict(net=dict(num_cont=2, num_uniqs=[3], num_layers=1, num_hiddens=8, num_out=2), n=9, batch=8),
+}
+
+
+def de_case(name, seed=0, output_noise=False, m=None):
+    """(net kwargs, Xc [n, dc] fp32, Xe [n, ne] int32, y [n, O] fp32) of DE_CASES[name]; m rows instead of n when given
+    (candidates for predict)."""
+    c = DE_CASES[name]
+    kw = dict(c["net"], output_noise=output_noise)
+    dc, uniqs, O = kw["num_cont"], kw["num_uniqs"], kw.get("num_out", 1)
+    n = c["n"] if m is None else m
+    g = np.random.default_rng(seed)
+    Xc = g.uniform(-1, 1, (n, dc)).astype(np.float32)
+    hi = c.get("cat_hi", uniqs)
+    Xe = np.stack([g.integers(0, h, n) for h in hi], 1).astype(np.int32) if uniqs else np.zeros((n, 0), np.int32)
+    base = Xc.sum(1, keepdims=True) / max(1, dc) ** 0.5 + (Xe.sum(1, keepdims=True) % 5 if uniqs else 0)
+    y = (np.sin(base + np.arange(O)) + 0.1 * g.standard_normal((n, O))).astype(np.float32)
+    if c.get("holes") and m is None:
+        y[:, 5] = np.nan
+        for i in range(n):
+            y[i, [k for k in range(O) if k != 5][:i % 7]] = np.nan
+    return kw, Xc, Xe, y
+
+
+U32 = 2.0 ** -24
+
+
+def gamma32(N):
+    return N * U32 / (1 - N * U32)
+
+
+def de_initial(kw, seed, E=1) -> torch.Tensor:
+    """[E, P] BaseNet initial weights of a DE_CASES net (xavier_uniform, zero biases) from torch's generator."""
+    from hebo_b200.ensemble import init_params, param_layout
+    lay, _ = param_layout(kw["num_cont"], kw["num_uniqs"], kw.get("enum_trans", "embedding"), kw.get("num_layers", 1),
+                          kw.get("num_hiddens", 128), kw.get("num_out", 1), kw["output_noise"], kw.get("rand_prior", False))
+    torch.manual_seed(seed)
+    return torch.stack([init_params(lay) for _ in range(E)])
+
+
+def de_abs_net(net):
+    """A copy of net with |W| and |b| and no forward hooks (a caller's kink hooks must not reach the magnitudes)."""
+    a = copy.deepcopy(net)
+    for m in a.modules():
+        m._forward_hooks.clear()
+    with torch.no_grad():
+        for p in a.parameters():
+            p.abs_()
+    return a
+
+
+def _hidden_linears(net):
+    return [m for m in net.hidden if isinstance(m, torch.nn.Linear)]
+
+
+def de_depth(net):
+    """(roundings of the forward chain to the heads, roundings of the backward chain from the heads to the input): a
+    dense output is a K-term fmaf chain plus the bias add, ReLU and the prior add."""
+    K = [net.din] + [net.H] * (net.L - 1)
+    return sum(k + 2 for k in K) + net.H + 3, net.O * 2 + net.H * net.L + 2
+
+
+def de_kink_units(net64, net32, run):
+    """{layer: [B, H] bool} of the hidden units whose fp64 pre-activation z lies within its fp32 error bound of 0, where
+    the device's ReLU may decide either way.  The bound is gamma_depth times z computed on |W|, |b| and the absolute
+    inputs through the fp64 ReLU masks (a unit that is off by more than its bound is 0 in fp32 too, and adds no error).
+    run(net) runs net64 on the rows."""
+    lins = _hidden_linears(net64)
+    z, xin = {}, []
+    hooks = [m.register_forward_hook(lambda m_, i_, o_, l=l: z.__setitem__(l, o_.detach())) for l, m in enumerate(lins)]
+    hooks.append(lins[0].register_forward_hook(lambda m_, i_, o_: xin.append(i_[0].detach())))
+    try:
+        run(net64)
+    finally:
+        for h in hooks:
+            h.remove()
+    a = xin[0].abs().numpy()
+    depth, out = 0, {}
+    for l, lin in enumerate(lins):
+        depth += lin.in_features + 2
+        zl = z[l].numpy()
+        za = a @ lin.weight.detach().abs().numpy().T + lin.bias.detach().abs().numpy()
+        out[l] = np.abs(zl) <= gamma32(depth) * za
+        a = np.where((zl > 0) | out[l], za, 0.0)
+    return out
+
+
+@contextlib.contextmanager
+def de_adopt_masks(net64, kinks, acts32):
+    """Within the block, net64's ReLU at each kink unit passes the gradient exactly when the fp32 activation acts32[l]
+    is positive (both are BaseNet's derivative there: the pre-activation is 0 within rounding); its value moves by
+    less than the unit's bound."""
+    def hook(l):
+        def f(mod, inp, out):
+            k = torch.from_numpy(kinks[l])
+            if not bool(k.any()):
+                return out
+            tiny = torch.tensor(1e-300, dtype=out.dtype)
+            s = torch.where(torch.from_numpy(acts32[l] > 0), tiny, -tiny)
+            return torch.where(k, s + (out - out.detach()), out)       # value exactly s, derivative 1
+        return f
+    hooks = [m.register_forward_hook(hook(l)) for l, m in enumerate(_hidden_linears(net64))]
+    try:
+        yield
+    finally:
+        for h in hooks:
+            h.remove()
+
+
+def de_step_grad_bound(net64, net32, Xc, Xe, y, rows, l1, n):
+    """(fp64 gradient, per-element bound on the fp32 step's error) of one minibatch, output_noise=False.  The bound is
+    gamma_N times the same gradient taken on |W|, |x| and the seeds' magnitudes 2 (|t| + |mu|) / cnt (every unit active),
+    plus the L1 coefficient's rounding; N is the longest chain of roundings from the inputs to a parameter's gradient."""
+    from oracle import ensemble_oracle as EO
+    rows = np.asarray(rows)
+    xc = torch.from_numpy(Xc[rows]).double()
+    xe = torch.from_numpy(Xe[rows]).long() if net32.uniqs else None
+    t = torch.from_numpy(y[rows]).double()
+    a = de_abs_net(net64)
+    _, g64 = EO.step_grad(net64, torch.from_numpy(Xc).double(), torch.from_numpy(Xe).long() if net32.uniqs else None,
+                          torch.from_numpy(y).double(), rows, l1, n)
+    a.zero_grad()
+    mu_a, _ = a(xc.abs(), xe)
+    fin = torch.isfinite(t)
+    seeds = torch.where(fin, 2 * (t.nan_to_num().abs() + mu_a.detach()) / fin.sum(), torch.zeros_like(t))
+    (seeds * mu_a).sum().backward()
+    ga = torch.cat([(p.grad if p.grad is not None else torch.zeros_like(p)).reshape(-1) for p in a.parameters()])
+    f, b = de_depth(net32)
+    coef = l1 / (n * net32.O)
+    return g64.numpy(), (gamma32(f + b + len(rows) + 6) * ga).numpy() + 4 * U32 * coef + 1e-300
+
+
+def _heads_and_input_grads(net, xc, xe, O):
+    """(mu, z or None, dmu/dxc [B, O, dc], dz/dxc or None) of net at the numeric inputs xc (rows are independent)."""
+    xc = xc.detach().clone().requires_grad_(True)
+    zs = []
+    h = net.sigma2[0].register_forward_hook(lambda m_, i_, o_: zs.append(o_)) if net.output_noise else None
+    mu, _ = net(xc, xe)
+    if h is not None:
+        h.remove()
+    heads = [mu] + zs
+    grads = [torch.stack([torch.autograd.grad(t[:, o].sum(), xc, retain_graph=True)[0] for o in range(O)], 1) for t in heads]
+    return mu.detach(), (zs[0].detach() if zs else None), grads[0], (grads[1] if zs else None)
+
+
+def de_predict_fp64(net32, params, Xs, Xe, x_mul, x_add, y_mean, y_std):
+    """BaseNet's ensemble predict in fp64 on the given rows and per-element bounds on the device's fp32 error:
+    ({'mu', 'var', 'dmu', 'dvar'}: (fp64 value, bound)), kink units, hidden units.  Values come from EO.ensemble_predict
+    and autograd.  Each bound restates the kernel's error chain: member heads within gamma_f of their |W|, |x| magnitude,
+    the member mean and variance sums, softplus and its derivative through expf / log1pf (2 and 1 ulp, CUDA C Programming
+    Guide, Mathematical Functions) on the NLL head, and the input-gradient backward within gamma_N of the |W| net's input
+    gradient times the seeds' magnitudes and errors.  At kink units the fp64 ReLU takes the fp32 decision (de_adopt_masks)."""
+    from oracle import ensemble_oracle as EO
+    E, O, dc, noise = params.shape[0], net32.O, net32.dc, net32.noise
+    f, b = de_depth(net32)
+    f += 2                                                      # x_mul x + x_add
+    gf, gN = gamma32(f + E + 4), gamma32(f + b + E + 6)
+    xm, xa = torch.from_numpy(x_mul).double(), torch.from_numpy(x_add).double()
+    ym, ys = torch.from_numpy(y_mean).double(), torch.from_numpy(y_std).double()
+    X64 = torch.from_numpy(Xs).double()
+    xe = torch.from_numpy(Xe).long() if net32.uniqs else None
+    xc, xc_a = X64 * xm + xa, X64.abs() * xm.abs() + xa.abs()
+    nets, kinks, per, stack = [], 0, [], contextlib.ExitStack()
+    for e in range(E):
+        net = EO.OracleNet(net32.dc, net32.uniqs, "embedding" if net32.emb else "onehot", net32.L, net32.H, O, noise,
+                           net32.prior).load_raw(params[e])
+        with torch.no_grad():
+            k = de_kink_units(net, net32, lambda n_: n_(xc, xe))
+        acts32, _, _ = EO.forward32(net32, params[e], EO.load_inputs32(net32, params[e], Xs, Xe, x_mul, x_add))
+        kinks += sum(int(v.sum()) for v in k.values())
+        a = de_abs_net(net)
+        stack.enter_context(de_adopt_masks(net, k, acts32))
+        nets.append(net)
+        mu, z, gmu, gz = _heads_and_input_grads(net, xc, xe, O)
+        mu_a, z_a, gmu_a, gz_a = _heads_and_input_grads(a, xc_a, xe, O)
+        per.append((mu, z, mu_a.abs(), None if z is None else z_a.abs(), gmu_a, gz_a))
+    with stack:
+        X = X64.clone().requires_grad_(True)
+        py, ps2 = EO.ensemble_predict(nets, X, xe, xm, xa, ym, ys, noise)
+        dmu = torch.stack([torch.autograd.grad(py[:, o].sum(), X, retain_graph=True)[0] for o in range(O)], 1)
+        dvar = torch.stack([torch.autograd.grad(ps2[:, o].sum(), X, retain_graph=True)[0] for o in range(O)], 1)
+    mean = sum(p_[0] for p_ in per) / E
+    mean_a = sum(p_[2] for p_ in per) / E
+    e_py = gf * mean_a
+    v_b, e_v, d_seed_mu, d_seed_z = 0.0, 0.0, [], []
+    for mu, z, mu_a, z_a, _, _ in per:
+        d = mu - mean
+        e_d = gf * mu_a + e_py + U32 * d.abs()
+        v_b = v_b + d * d / E
+        e_v = e_v + (2 * d.abs() * e_d + e_d ** 2) / E
+        d_seed_mu.append(2 / E * (e_d + gN * d.abs()))          # |error| of the pass-1 mu seed, backward rounding included
+        if noise:
+            sp = torch.nn.functional.softplus(z)
+            sig = torch.sigmoid(z)
+            e_z = gf * z_a
+            e_s2 = e_z * sig + 8 * U32 * (1e-4 + sp)
+            e_v = e_v + (e_s2 + gamma32(E + 2) * (1e-4 + sp)) / E
+            d_seed_z.append((e_z * sig * (1 - sig) + 8 * U32 * sig + gN * sig) / E)
+    v = ps2.detach() / ys ** 2
+    e_v = e_v + gamma32(E + 4) * v
+    x_scale = xm.abs()[None, None, :]
+    b_dmu = sum(gN / E * p_[4] for p_ in per) * x_scale * ys.abs()[None, :, None]
+    b_dvar = sum(s_[:, :, None] * p_[4] for s_, p_ in zip(d_seed_mu, per))
+    if noise:
+        b_dvar = b_dvar + sum(s_[:, :, None] * p_[5] for s_, p_ in zip(d_seed_z, per))
+    b_dvar = b_dvar * x_scale * (ys ** 2)[None, :, None]
+    out = {"mu": (py.detach(), gf * (mean_a * ys.abs() + ym.abs())),
+           "var": (ps2.detach(), e_v * ys ** 2),
+           "dmu": (dmu, b_dmu), "dvar": (dvar, b_dvar)}
+    return {k_: (v_.numpy(), b_.numpy() + 1e-300) for k_, (v_, b_) in out.items()}, kinks, Xs.shape[0] * net32.H * net32.L * E
+
+
+DE_PRED = [("holes", 1), ("holes", 2), ("holes", 32), ("corner", 2), ("emb-wide", 2), ("onehot-wide", 2), ("default-prior", 5)]
+
+
+def de_predict_case(case, E, output_noise=False):
+    """The predict set-up of tests/test_gpu_ensemble_envelope.py: perturbed initial weights (biases away from 0, members
+    apart), 4097 candidates, scalers away from the identity."""
+    from oracle import ensemble_oracle as EO
+    kw, _, _, _ = de_case(case, output_noise=output_noise)
+    _, Xs, Xe, _ = de_case(case, seed=21, m=4097)
+    net = EO.Net32(**kw)
+    g = np.random.default_rng(22)
+    params = de_initial(kw, 12, E).numpy()
+    params += (0.05 * g.standard_normal(params.shape)).astype(np.float32)
+    xm = g.uniform(0.5, 2, net.dc).astype(np.float32)
+    xa = g.uniform(-0.5, 0.5, net.dc).astype(np.float32)
+    ym = g.standard_normal(net.O).astype(np.float32)
+    ys = g.uniform(0.5, 3, net.O).astype(np.float32)
+    pick = np.unique(np.r_[0:16, 15:18, 4080:4097, np.random.default_rng(23).integers(0, 4097, 8)])
+    return kw, net, params, Xs, Xe, xm, xa, ym, ys, pick
+
+
+def de_check_against_fp64(got, ref, kinks, units, what):
+    """got (mu, var, dmu, dvar) against de_predict_fp64's values and bounds, per element; prints the largest ratio."""
+    assert kinks <= units // 20, (kinks, units)
+    ratios = []
+    for name, g in zip(("mu", "var", "dmu", "dvar"), got):
+        v, bnd = ref[name]
+        err = np.abs(np.asarray(g, np.float64) - v)
+        assert np.all(err <= bnd), f"{what} {name}: {int((err > bnd).sum())} over, worst {float(np.max(err / bnd)):.3g} x bound"
+        ratios.append(f"{name} {float(np.max(err / bnd)):.3g}")
+    print(f"{what}: error / bound " + ", ".join(ratios) + f"; kink units {kinks} of {units}")
