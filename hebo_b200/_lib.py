@@ -131,6 +131,10 @@ SIGNATURES = {
     "hb_de_fit": (_i32, [_vp, _vp, _vp, _i64, _dsp, _i64, _vp, C.c_double, _f32, _i64, _i64, _vp, _u64, _vp, _vp, _i64, _vp]),
     "hb_de_predict": (_i32, [_vp, _vp, _i64, _dsp, _i64, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
     "hb_de_predict_grad": (_i32, [_vp, _vp, _i64, _dsp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "hb_de_fit_batch": (_i32, [_vp, _vp, _vp, C.POINTER(C.c_int64), _i64, _dsp, _i64, _vp, C.c_double, _f32, _i64, _i64,
+                               C.POINTER(C.c_uint64), _vp, _vp, _i64, _vp]),
+    "hb_de_predict_batch": (_i32, [_vp, _vp, _i64, _dsp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _u64, _u64,
+                                   _vp, _vp]),
 }
 
 _lib = None

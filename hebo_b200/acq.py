@@ -13,7 +13,8 @@ mu / var (torch's CPU sqrt, used by ``eval``, may differ from the correctly roun
 four -- is scored through its own ``eval`` on CPU tensors, once per generation, as the reference's EvolutionOpt does.
 
 ``GeneralAcq`` (acq.py:192-242) is the LCB of every objective and constraint of a multi-output model, for ``GeneralBO``.
-Its ``eval`` runs on any model through ``hb_general_acq_epilogue``; ``general_score`` scores it for the device GA.
+Its ``eval`` runs on any model through ``hb_general_acq_epilogue``; ``general_score`` scores it for the device GA, over GPs
+and over deep ensembles.
 """
 from __future__ import annotations
 
@@ -22,7 +23,7 @@ import torch
 
 from . import _lib
 from .base import Acquisition
-from .ensemble import DeepEnsemble
+from .ensemble import DeepEnsemble, EnsembleBatch
 from .gp import GP, MultiTaskModel
 
 
@@ -130,17 +131,32 @@ def _noisy_device_score(model, seed: int):
     return score
 
 
+def _noisy_ensemble_score(model, seed: int):
+    """score(xc, xe, gen) of NoisyAcq over a fitted single-output DeepEnsemble: one hb_de_predict_batch per generation
+    with one independent draw per row (BaseModel.sample_y), keyed by (seed, counter = gen)."""
+    batch = EnsembleBatch([model])
+
+    def score(xc, xe, gen):
+        _, _, samp = batch.predict(xc if model.num_cont > 0 else None, xe if model.num_enum > 0 else None, n_samples=1,
+                                   seed=seed, counter=gen)
+        return samp.reshape(-1)
+    return score
+
+
 def ga_score(acq, seed=None):
     """score(xc, xe, gen) -> f [m] fp32 on the device for DeviceNSGA2, of a single-objective acquisition.  xc [m, d] fp32
     and xe [m, e] int32 are device tensors.  With a hebo_b200.GP and one of the four acquisitions above: predict on the
     device (hb_posterior_mace_ex with F = NULL) and hb_acq1_epilogue, no host synchronisation.  With a NoisyAcq of one
     objective and no constraint over a fitted hebo_b200.GP: one joint draw per generation on the device
     (``GP.sample_y_batch``, counter = the generation, ``seed`` drawn from numpy's global generator when None; batches of at
-    most 256 rows).  Otherwise: acq.eval on CPU tensors (xe as int64, like the reference's BOProblem), its first column
-    copied back to the device."""
-    if (type(acq) is NoisyAcq and acq.num_obj == 1 and acq.num_constr == 0 and isinstance(acq.model, GP)
-            and not acq.model._fit_failed):
-        return _noisy_device_score(acq.model, int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed))
+    most 256 rows); over a fitted single-output DeepEnsemble: one hb_de_predict_batch per generation with one
+    independent draw per row (counter = the generation, any batch size).  Otherwise: acq.eval on CPU tensors (xe as int64,
+    like the reference's BOProblem), its first column copied back to the device."""
+    if type(acq) is NoisyAcq and acq.num_obj == 1 and acq.num_constr == 0:
+        if isinstance(acq.model, GP) and not acq.model._fit_failed:
+            return _noisy_device_score(acq.model, int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed))
+        if isinstance(acq.model, DeepEnsemble) and acq.model.fitted and acq.model.num_out == 1:
+            return _noisy_ensemble_score(acq.model, int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed))
     mode = _ACQ1_MODES.get(type(acq))
     if mode is not None and isinstance(acq.model, (GP, DeepEnsemble)):
         kappa = float(getattr(acq, "kappa", 0.0))
@@ -283,14 +299,19 @@ def general_score(acq, seed=None):
     positive parts of the constraint columns.  A GeneralAcq over a hebo_b200.MultiTaskModel of GPs, or one GP: one
     posterior call per output with F = NULL, writing row b of [K, m] buffers, then hb_general_acq_epilogue with Philox
     draws keyed by (seed, gen).  A MOMeanSigmaLCB over a hebo_b200.GP: one posterior call with F = NULL, then
-    hb_mo_lcb_epilogue with Philox draws keyed by (seed, gen), its G being the one constraint column.  Neither synchronises
-    with the host inside a generation; an output whose fit failed predicts N(y_mean, y_std^2) as GP.predict does.
-    ``seed`` is drawn from numpy's global generator when None.  Any other acquisition or model, including subclasses of
-    these two: acq.eval on CPU tensors (xe as int64), once per generation."""
+    hb_mo_lcb_epilogue with Philox draws keyed by (seed, gen), its G being the one constraint column.  With deep
+    ensembles -- a GeneralAcq over one multi-output DeepEnsemble or a MultiTaskModel of them, a MOMeanSigmaLCB over one
+    DeepEnsemble -- the posterior is one hb_de_predict_batch (GeneralAcq, writing [K, m] directly) or hb_de_predict
+    (MOMeanSigmaLCB) call, followed by the same epilogue.  None of these synchronises with the host inside a generation;
+    an output whose GP fit failed predicts N(y_mean, y_std^2) as GP.predict does.  ``seed`` is drawn from numpy's global
+    generator when None.  Any other acquisition or model, including subclasses of these two: acq.eval on CPU tensors (xe as
+    int64), once per generation."""
     no, nc = acq.num_obj, acq.num_constr
     model = acq.model
-    if type(acq) is MOMeanSigmaLCB and isinstance(model, GP):
+    if type(acq) is MOMeanSigmaLCB and isinstance(model, (GP, DeepEnsemble)):
         return _mo_lcb_device_score(acq, seed)
+    if type(acq) is GeneralAcq and _ensembles_of(model) is not None:
+        return _general_ensemble_score(acq, _ensembles_of(model), seed)
     gps = None
     if isinstance(model, GP):
         gps = [model]
@@ -323,15 +344,43 @@ def general_score(acq, seed=None):
     return device_score
 
 
+def _ensembles_of(model):
+    """The DeepEnsembles behind a GeneralAcq's model as hb_de_predict_batch operands (one multi-output ensemble, or every
+    output's single-output ensemble of a MultiTaskModel), or None."""
+    if isinstance(model, DeepEnsemble):
+        return [model]
+    if isinstance(model, MultiTaskModel) and all(isinstance(m, DeepEnsemble) for m in model.models):
+        return model.models
+    return None
+
+
+def _general_ensemble_score(acq, models, seed=None):
+    seed = int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed)
+    no, nc, m0 = acq.num_obj, acq.num_constr, models[0]
+    batch = EnsembleBatch(models)
+    noise_sd = acq.model.noise.reshape(-1).float().sqrt().to(m0.device).contiguous() if acq.use_noise else None
+    kappa, c_kappa = float(acq.kappa), float(acq.c_kappa)
+
+    def device_score(xc, xe, gen):
+        mu, var, _ = batch.predict(xc if m0.num_cont > 0 else None, xe if m0.num_enum > 0 else None)
+        Fo, _, cv = _general_epilogue(mu, var, no, nc, kappa, c_kappa, noise_sd, None, seed, gen, want_cv=nc > 0)
+        return (Fo, cv) if nc else Fo
+    return device_score
+
+
 def _mo_lcb_device_score(acq, seed=None):
     seed = int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed)
-    gp = acq.model
-    noise_sd, best_y, kappa = _noise_sd(gp), _best_y(acq), float(acq.kappa)
+    model = acq.model
+    noise_sd, best_y, kappa = _noise_sd(model), _best_y(acq), float(acq.kappa)
 
     def device_score(xc, xe, gen):
         m = xc.shape[0]
         with torch.no_grad():
-            _, mu, var = gp._posterior(gp._to_dev(xc), False, Xe_dev=gp._xe_dev(xe, m))
+            if isinstance(model, GP):
+                _, mu, var = model._posterior(model._to_dev(xc), False, Xe_dev=model._xe_dev(xe, m))
+            else:
+                mu, var = model._predict_dev(xc if model.num_cont > 0 else None, xe if model.num_enum > 0 else None)
+                mu, var = mu.reshape(-1), var.reshape(-1)
         return _mo_lcb_epilogue(mu, var, noise_sd, best_y, kappa, None, seed, gen)
     return device_score
 

@@ -161,16 +161,17 @@ class NoMR_BO:
 
 class HEBO_VectorContextual:
     """hebo_contextual.py:20-50: HEBO with the named context ``self.context`` of ``context_dict`` ({name: {parameter:
-    value}}) passed as ``fix_input`` to every suggestion.  Only the 'gp' model is supported."""
+    value}}) passed as ``fix_input`` to every suggestion.  model_name: 'gp' or 'deep_ensemble', passed to HEBO."""
 
     support_parallel_opt = True
     support_combinatorial = True
     support_contextual = True
 
     def __init__(self, space, context_dict: dict, model_name: str = "gp", rand_sample: Optional[int] = None, **hebo_kwargs):
-        if model_name != "gp":
-            raise NotImplementedError(f"HEBO_VectorContextual: model_name {model_name!r} is not supported, only 'gp'")
-        self.hebo = HEBO(_design_space(space), rand_sample=rand_sample, **hebo_kwargs)
+        if model_name not in ("gp", "deep_ensemble"):
+            raise NotImplementedError(f"HEBO_VectorContextual: model_name {model_name!r} is not supported, only 'gp' and "
+                                      "'deep_ensemble'")
+        self.hebo = HEBO(_design_space(space), rand_sample=rand_sample, model_name=model_name, **hebo_kwargs)
         self.context_dict = context_dict
         self.context = None
 

@@ -1044,4 +1044,21 @@ int32_t hb_de_predict_grad(const float *Xs, const int32_t *Xe, int64_t m, const 
                            (cudaStream_t)stream);
 }
 
+// deep_ensemble.py:71-93 for the ensembles of a MultiTaskModel (model_factory.py:60-92), all in one launch
+int32_t hb_de_fit_batch(const float *Xc, const int32_t *Xe, const float *y, const int64_t *off, int64_t B,
+                        const hb_de_spec_t *spec, int64_t E, float *params, double lr, float l1, int64_t batch_size,
+                        int64_t num_epochs, const uint64_t *seeds, float *losses, void *ws, int64_t ws_bytes, void *stream) {
+  return launch_de_fit_batch(Xc, Xe, y, off, B, spec, E, params, lr, l1, batch_size, num_epochs, seeds, losses, ws, ws_bytes,
+                             (cudaStream_t)stream);
+}
+
+// deep_ensemble.py:95-106 for B ensembles, and BaseModel.sample_y (base_model.py:78-84)
+int32_t hb_de_predict_batch(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t B, int64_t E,
+                            const float *params, const float *x_mul, const float *x_add, const float *y_mean,
+                            const float *y_std, float *mu, float *var, int64_t n_samples, const float *xi, uint64_t seed,
+                            uint64_t counter, float *y_samp, void *stream) {
+  return launch_de_predict_batch(Xs, Xe, m, spec, B, E, params, x_mul, x_add, y_mean, y_std, mu, var, n_samples, xi, seed,
+                                 counter, y_samp, (cudaStream_t)stream);
+}
+
 }  // extern "C"

@@ -318,9 +318,9 @@ struct DeFitArgs {
   float coef;       // fp32 (1 / (n num_out)) * l1: the L1 term's gradient per unit sign
 };
 
-__global__ void __launch_bounds__(DE_FIT_THREADS) de_fit_kernel(const __grid_constant__ DeNet net, const DeFitArgs a) {
-  extern __shared__ float smem[];
-  const int member = blockIdx.x, B = a.B, O = net.O;
+// The whole fit of one member: a's pointers are its ensemble's (params [E, P], m1 / m2 / grad [E, P], losses [E, epochs])
+__device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs &a, int member, float *smem) {
+  const int B = a.B, O = net.O;
   const DeSmem s = de_carve(net, smem, B);
   float *prm = a.params + (size_t)member * net.P;
   float *m1 = a.m1 + (size_t)member * net.P, *m2 = a.m2 + (size_t)member * net.P, *g = a.grad + (size_t)member * net.P;
@@ -417,6 +417,50 @@ __global__ void __launch_bounds__(DE_FIT_THREADS) de_fit_kernel(const __grid_con
   }
 }
 
+__global__ void __launch_bounds__(DE_FIT_THREADS) de_fit_kernel(const __grid_constant__ DeNet net, const DeFitArgs a) {
+  extern __shared__ float smem[];
+  de_fit_member(net, a, blockIdx.x, smem);
+}
+
+// Per-ensemble arguments of hb_de_fit_batch: its rows [off, off + n) of the concatenated inputs and what follows from n
+struct DeFitSlot {
+  int64_t off;
+  uint64_t seed;
+  float coef;
+  int n, B, nb, h;
+};
+
+struct DeFitBatchArgs {
+  DeFitArgs a;         // concatenated Xc / Xe / y, params [nens, E, P], m1 = the workspace, losses [nens, E, epochs]
+  int E;
+  DeFitSlot slot[HB_MAX_OUTPUTS];
+};
+
+// CTA (b, member) = blockIdx.x = b E + member runs de_fit_kernel's member on ensemble b's slices
+__global__ void __launch_bounds__(DE_FIT_THREADS) de_fit_batch_kernel(const __grid_constant__ DeNet net,
+                                                                       const __grid_constant__ DeFitBatchArgs ba) {
+  extern __shared__ float smem[];
+  const int b = blockIdx.x / ba.E, member = blockIdx.x % ba.E;
+  const DeFitSlot &sl = ba.slot[b];
+  const size_t EP = (size_t)ba.E * net.P;
+  DeFitArgs a = ba.a;
+  a.Xc = a.Xc ? a.Xc + sl.off * net.dc : nullptr;
+  a.Xe = a.Xe ? a.Xe + sl.off * net.ne : nullptr;
+  a.y += sl.off * net.O;
+  a.params += b * EP;
+  a.m1 += 3 * b * EP;
+  a.m2 = a.m1 + EP;
+  a.grad = a.m2 + EP;
+  a.losses += (size_t)b * ba.E * a.epochs;
+  a.n = sl.n;
+  a.B = sl.B;
+  a.nb = sl.nb;
+  a.h = sl.h;
+  a.seed = sl.seed;
+  a.coef = sl.coef;
+  de_fit_member(net, a, member, smem);
+}
+
 // ------------------------------------------------------------------------------------------------ predict
 struct DePredArgs {
   const float *Xs, *params, *x_mul, *x_add, *y_mean, *y_std;
@@ -425,13 +469,11 @@ struct DePredArgs {
   int m, E, member;
 };
 
-template <bool GRAD>
-__global__ void __launch_bounds__(DE_PRED_THREADS) de_predict_kernel(const __grid_constant__ DeNet net, const DePredArgs a) {
-  extern __shared__ float smem[];
-  const int O = net.O, B = DE_TM, r0 = blockIdx.x * DE_TM;
-  const DeSmem s = de_carve(net, smem, B);
-  const int e0 = a.member >= 0 ? a.member : 0, e1 = a.member >= 0 ? a.member + 1 : a.E, ne = e1 - e0;
-  float *mus = s.red + DE_SCRATCH, *s2s = mus + ne * B * O, *py = s2s + ne * B * O;
+// Rows r0 .. r0 + DE_TM - 1 of the candidates (the last one repeated past m) through members e0 .. e1 - 1: the heads mu
+// into mus[e - e0][p, o] and, with output_noise, sigma2 into s2s[e - e0][p, o]
+__device__ __forceinline__ void de_member_heads(const DeNet &net, const DePredArgs &a, const DeSmem &s, int r0, int e0,
+                                                int e1, float *mus, float *s2s) {
+  const int O = net.O, B = DE_TM;
   for (int p = threadIdx.x; p < B; p += blockDim.x) s.rows[p] = min(r0 + p, a.m - 1);
   __syncthreads();
   for (int e = e0; e < e1; ++e) {
@@ -446,28 +488,47 @@ __global__ void __launch_bounds__(DE_PRED_THREADS) de_predict_kernel(const __gri
     }
     __syncthreads();
   }
-  // the ensemble combination in member order (deep_ensemble.py:97-106)
+}
+
+// the ensemble combination of tile entry i over ne members in member order (deep_ensemble.py:97-106); single: one
+// member's own mu
+__device__ __forceinline__ void de_combine(const DeNet &net, const float *mus, const float *s2s, int ne, int i, bool single,
+                                           float &mean, float &v) {
+  const int BO = DE_TM * net.O;
+  mean = 0.0f;
+  v = 0.0f;
+  if (single) {
+    mean = mus[i];
+    return;
+  }
+  for (int e = 0; e < ne; ++e) mean += mus[e * BO + i];
+  mean = mean / (float)ne;
+  for (int e = 0; e < ne; ++e) {
+    const float dlt = mus[e * BO + i] - mean;
+    v = fmaf(dlt, dlt, v);
+  }
+  v = v / (float)ne;
+  if (net.noise) {
+    float sm = 0.0f;
+    for (int e = 0; e < ne; ++e) sm += s2s[e * BO + i];
+    v = v + sm / (float)ne;
+  } else {
+    v = 1e-8f + v;
+  }
+}
+
+template <bool GRAD>
+__global__ void __launch_bounds__(DE_PRED_THREADS) de_predict_kernel(const __grid_constant__ DeNet net, const DePredArgs a) {
+  extern __shared__ float smem[];
+  const int O = net.O, B = DE_TM, r0 = blockIdx.x * DE_TM;
+  const DeSmem s = de_carve(net, smem, B);
+  const int e0 = a.member >= 0 ? a.member : 0, e1 = a.member >= 0 ? a.member + 1 : a.E, ne = e1 - e0;
+  float *mus = s.red + DE_SCRATCH, *s2s = mus + ne * B * O, *py = s2s + ne * B * O;
+  de_member_heads(net, a, s, r0, e0, e1, mus, s2s);
   for (int i = threadIdx.x; i < B * O; i += blockDim.x) {
     const int p = i / O, o = i % O, row = r0 + p;
-    float mean = 0.0f, v = 0.0f;
-    if (a.member >= 0) {
-      mean = mus[i];
-    } else {
-      for (int e = 0; e < ne; ++e) mean += mus[e * B * O + i];
-      mean = mean / (float)ne;
-      for (int e = 0; e < ne; ++e) {
-        const float dlt = mus[e * B * O + i] - mean;
-        v = fmaf(dlt, dlt, v);
-      }
-      v = v / (float)ne;
-      if (net.noise) {
-        float sm = 0.0f;
-        for (int e = 0; e < ne; ++e) sm += s2s[e * B * O + i];
-        v = v + sm / (float)ne;
-      } else {
-        v = 1e-8f + v;
-      }
-    }
+    float mean, v;
+    de_combine(net, mus, s2s, ne, i, a.member >= 0, mean, v);
     py[i] = mean;
     if (row < a.m) {
       const float sd = a.y_std[o];
@@ -518,6 +579,59 @@ __global__ void __launch_bounds__(DE_PRED_THREADS) de_predict_kernel(const __gri
           __syncthreads();
         }
       }
+    }
+  }
+}
+
+// B ensembles of one spec over one candidate batch: CTA (tile, b) = (blockIdx.x, blockIdx.y) runs de_predict_kernel's
+// member loop and combination on ensemble b's parameters and scalers, and writes mu / var output-major, [nens O, m]; with
+// nsamp > 0 also y_samp[t, row, b O + o] = py + sqrt(ps2) * xi (BaseModel.sample_y, base_model.py:78-84)
+struct DePredBatchArgs {
+  DePredArgs a;      // params [nens, E, P], x_mul / x_add [nens, dc], y_mean / y_std [nens, O]; mu / var [nens O, m]
+  int nens, nsamp;
+  const float *xi;   // [nsamp, m, nens O] or NULL: Philox pairs keyed by (seed, counter), element q takes half q % 2 of q / 2
+  float *ysamp;      // [nsamp, m, nens O]
+  uint64_t seed, counter;
+};
+
+__global__ void __launch_bounds__(DE_PRED_THREADS) de_predict_batch_kernel(const __grid_constant__ DeNet net,
+                                                                           const __grid_constant__ DePredBatchArgs ba) {
+  extern __shared__ float smem[];
+  const int O = net.O, B = DE_TM, r0 = blockIdx.x * DE_TM, b = blockIdx.y, ne = ba.a.E;
+  const DeSmem s = de_carve(net, smem, B);
+  DePredArgs a = ba.a;
+  a.params += (size_t)b * ne * net.P;
+  if (a.x_mul) {
+    a.x_mul += b * net.dc;
+    a.x_add += b * net.dc;
+  }
+  a.y_mean += b * O;
+  a.y_std += b * O;
+  float *mus = s.red + DE_SCRATCH, *s2s = mus + ne * B * O;
+  de_member_heads(net, a, s, r0, 0, ne, mus, s2s);
+  const int64_t m = a.m, KO = (int64_t)ba.nens * O;
+  for (int i = threadIdx.x; i < B * O; i += blockDim.x) {
+    const int p = i / O, o = i % O, row = r0 + p;
+    if (row >= a.m) continue;
+    float mean, v;
+    de_combine(net, mus, s2s, ne, i, false, mean, v);
+    const float sd = a.y_std[o];
+    const float py = __fadd_rn(__fmul_rn(mean, sd), a.y_mean[o]), ps2 = __fmul_rn(v, __fmul_rn(sd, sd));
+    const int64_t col = (int64_t)b * O + o;
+    a.mu[col * m + row] = py;
+    a.var[col * m + row] = ps2;
+    const float ps = __fsqrt_rn(ps2);
+    for (int t = 0; t < ba.nsamp; ++t) {
+      const int64_t q = ((int64_t)t * m + row) * KO + col;
+      float z;
+      if (ba.xi) {
+        z = ba.xi[q];
+      } else {
+        float z0, z1;
+        philox_normal2(ba.seed, (uint64_t)(q >> 1), ba.counter, z0, z1);
+        z = (q & 1) ? z1 : z0;
+      }
+      ba.ysamp[q] = __fadd_rn(py, __fmul_rn(ps, z));
     }
   }
 }
@@ -612,6 +726,95 @@ int launch_de_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de
   }
   count_launches(1);
   HB_LAUNCH_CHECK("de_predict_kernel");
+  return HB_OK;
+}
+
+int launch_de_fit_batch(const float *Xc, const int32_t *Xe, const float *y, const int64_t *off, int64_t nens,
+                        const hb_de_spec_t *spec, int64_t E, float *params, double lr, float l1, int64_t batch_size,
+                        int64_t num_epochs, const uint64_t *seeds, float *losses, void *ws, int64_t ws_bytes, cudaStream_t st) {
+  DeNet net;
+  if (!de_layout(spec, net) || E < 1 || E > HB_DE_MAX_MEMBERS || nens < 1 || nens > HB_MAX_OUTPUTS || batch_size < 1 ||
+      num_epochs < 0)
+    return HB_ERR_INVALID;
+  if (!off || !seeds || !y || !params || !ws || (num_epochs > 0 && !losses) || (net.dc > 0 && !Xc) || (net.ne > 0 && !Xe))
+    return HB_ERR_INVALID;
+  if (ws_bytes < nens * de_fit_ws_query(spec, E)) return HB_ERR_INVALID;
+  DeFitBatchArgs ba{};
+  int64_t Bmax = 0;
+  if (off[0] < 0) return HB_ERR_INVALID;
+  for (int64_t b = 0; b < nens; ++b) {
+    const int64_t n = off[b + 1] - off[b];
+    if (n < 1 || n > (1 << 30)) return HB_ERR_INVALID;
+    const int64_t B = n > batch_size ? batch_size : n;     // as launch_de_fit, per ensemble
+    DeFitSlot &sl = ba.slot[b];
+    sl.off = off[b];
+    sl.seed = seeds[b];
+    sl.coef = (1.0f / (float)(n * net.O)) * l1;
+    sl.n = (int)n;
+    sl.B = (int)B;
+    sl.nb = (int)(n > batch_size ? n / batch_size : 1);
+    int h = 1;
+    while ((int64_t(1) << (2 * h)) < n) ++h;
+    sl.h = h;
+    Bmax = B > Bmax ? B : Bmax;
+  }
+  if (de_rows_floats(net, Bmax) > HB_DE_MAX_BATCH_FLOATS) return HB_ERR_INVALID;
+  if (num_epochs == 0) return HB_OK;
+  DeFitArgs &a = ba.a;
+  a.Xc = Xc;
+  a.Xe = Xe;
+  a.y = y;
+  a.perm = nullptr;
+  a.params = params;
+  a.m1 = (float *)ws;
+  a.losses = losses;
+  a.epochs = (int)num_epochs;
+  a.lr = lr;
+  ba.E = (int)E;
+  const size_t smem = (size_t)(de_rows_floats(net, Bmax) + DE_SCRATCH) * sizeof(float);
+  HB_CUDA(cudaFuncSetAttribute(de_fit_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  de_fit_batch_kernel<<<(unsigned)(nens * E), DE_FIT_THREADS, smem, st>>>(net, ba);
+  count_launches(1);
+  HB_LAUNCH_CHECK("de_fit_batch_kernel");
+  return HB_OK;
+}
+
+int launch_de_predict_batch(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t nens, int64_t E,
+                            const float *params, const float *x_mul, const float *x_add, const float *y_mean,
+                            const float *y_std, float *mu, float *var, int64_t n_samples, const float *xi, uint64_t seed,
+                            uint64_t counter, float *y_samp, cudaStream_t st) {
+  DeNet net;
+  if (!de_layout(spec, net) || E < 1 || E > HB_DE_MAX_MEMBERS || nens < 1 || nens > HB_MAX_OUTPUTS || m < 0 ||
+      m > (int64_t(1) << 31) - DE_TM || n_samples < 0 || n_samples > (int64_t(1) << 31))
+    return HB_ERR_INVALID;
+  if (!params || !y_mean || !y_std || !mu || !var || (net.ne > 0 && !Xe) || (n_samples > 0 && !y_samp)) return HB_ERR_INVALID;
+  if (net.dc > 0 && (!Xs || !x_mul || !x_add)) return HB_ERR_INVALID;
+  if (m == 0) return HB_OK;
+  DePredBatchArgs ba{};
+  DePredArgs &a = ba.a;
+  a.Xs = Xs;
+  a.Xe = Xe;
+  a.params = params;
+  a.x_mul = x_mul;
+  a.x_add = x_add;
+  a.y_mean = y_mean;
+  a.y_std = y_std;
+  a.mu = mu;
+  a.var = var;
+  a.m = (int)m;
+  a.E = (int)E;
+  a.member = -1;
+  ba.nens = (int)nens;
+  ba.nsamp = (int)n_samples;
+  ba.xi = xi;
+  ba.ysamp = y_samp;
+  ba.seed = seed;
+  ba.counter = counter;
+  const size_t smem = (size_t)(de_rows_floats(net, DE_TM) + DE_SCRATCH + 2 * E * DE_TM * net.O) * sizeof(float);
+  HB_CUDA(cudaFuncSetAttribute(de_predict_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  de_predict_batch_kernel<<<dim3((unsigned)ceil_div(m, DE_TM), (unsigned)nens), DE_PRED_THREADS, smem, st>>>(net, ba);
+  count_launches(1);
+  HB_LAUNCH_CHECK("de_predict_batch_kernel");
   return HB_OK;
 }
 

@@ -234,5 +234,13 @@ int launch_de_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n,
 int launch_de_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t E, const float *params,
                       const float *x_mul, const float *x_add, const float *y_mean, const float *y_std, int32_t member,
                       float *mu, float *var, float *dmu, float *dvar, cudaStream_t st);
+// nens ensembles of one spec: the fit (one CTA per (ensemble, member)) and predict (mu / var output-major, optional draws)
+int launch_de_fit_batch(const float *Xc, const int32_t *Xe, const float *y, const int64_t *off, int64_t nens,
+                        const hb_de_spec_t *spec, int64_t E, float *params, double lr, float l1, int64_t batch_size,
+                        int64_t num_epochs, const uint64_t *seeds, float *losses, void *ws, int64_t ws_bytes, cudaStream_t st);
+int launch_de_predict_batch(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t nens, int64_t E,
+                            const float *params, const float *x_mul, const float *x_add, const float *y_mean,
+                            const float *y_std, float *mu, float *var, int64_t n_samples, const float *xi, uint64_t seed,
+                            uint64_t counter, float *y_samp, cudaStream_t st);
 
 }  // namespace hb

@@ -124,8 +124,9 @@ class HEBO_Embedding:
 
     def __init__(self, space, model_name: str = "gp", eff_dim: int = 1, scale: float = 1, strategy: str = "alebo",
                  clip: bool = False, rand_sample: Optional[int] = None, **hebo_kwargs):
-        if model_name != "gp":
-            raise NotImplementedError(f"HEBO_Embedding: model_name {model_name!r} is not supported, only 'gp'")
+        if model_name not in ("gp", "deep_ensemble"):
+            raise NotImplementedError(f"HEBO_Embedding: model_name {model_name!r} is not supported, only 'gp' and "
+                                      "'deep_ensemble'")
         self.space = space if isinstance(space, DesignSpace) else DesignSpace().parse(space)
         assert check_design_space(self.space)
         self.scale, self.eff_dim, self.clip = scale, eff_dim, clip
@@ -137,7 +138,7 @@ class HEBO_Embedding:
         self.device = hebo_kwargs.get("device", "cuda")
         self._B_dev = None
         constraint = None if clip else (lambda xc: embed_violation(xc, self.B_device))
-        self.mace = HEBO(self.eff_space, rand_sample=rand_sample, _constraint=constraint, **hebo_kwargs)
+        self.mace = HEBO(self.eff_space, rand_sample=rand_sample, _constraint=constraint, model_name=model_name, **hebo_kwargs)
         sobol_sample = self.mace.quasi_sample
 
         def quasi_sample(n, fix_input=None, engine=None, as_opt=False):

@@ -237,6 +237,13 @@ class DeepEnsemble(BaseModel):
     def fit(self, Xc_, Xe_, y_, perm=None):
         """perm: optional [E, num_epochs, n] int32 minibatch order of each member's epochs over the filtered rows (tests);
         otherwise the device's Philox order under a seed drawn from torch's generator."""
+        Xc, Xe, y, valid = self._prepare_fit(Xc_, Xe_, y_, perm)
+        self._fit_dev(Xc, Xe, y, perm, self.seed)
+        self._finish_fit(Xc_, Xe_, y_, valid)
+
+    def _prepare_fit(self, Xc_, Xe_, y_, perm=None):
+        """fit's host side up to the launch: the row filter, the scalers (first fit only), the initial weights (first fit
+        only) and then the seed, both from torch's generator.  Returns the filtered, scaled (Xc, Xe, y) and the row mask."""
         y_ = torch.as_tensor(y_).float()
         if self.num_enum > 0:
             _check_categories(Xe_, self.num_uniqs)
@@ -258,12 +265,21 @@ class DeepEnsemble(BaseModel):
         if self.params is None:
             self.params = torch.stack([init_params(self.layout) for _ in range(E)]).to(dev).contiguous()
         self.seed = int(torch.randint(0, 2 ** 62, (1,)).item())     # the Philox key of this fit's minibatch order
-        self._fit_dev(Xc, Xe, y, perm, self.seed)
+        return Xc, Xe, y, valid
+
+    def _finish_fit(self, Xc_, Xe_, y_, valid):
+        """fit's host side after the launch: the noise estimate on the kept rows (deep_ensemble.py:89-93)."""
         self.sample_idx = 0
         with torch.no_grad():
             py, _ = self.predict(Xc_, Xe_)
-            err = (py - y_)[valid]
+            err = (py - torch.as_tensor(y_).float())[valid]
             self.noise_est = (err ** 2).mean(dim=0).detach().clone()
+
+    def _print_losses(self):
+        L = self.losses.cpu()
+        for i in range(self.num_ensembles):
+            for ep in range(0, int(self.num_epochs), self.print_every):
+                print("Epoch %d, %s loss = %g" % (ep, self.loss_name, float(L[i, ep])), flush=True)
 
     def _fit_dev(self, Xc, Xe, y, perm, seed):
         lib, dev, E = _lib.lib(), self.device, self.num_ensembles
@@ -281,10 +297,7 @@ class DeepEnsemble(BaseModel):
                                      _lib.ptr(losses), _lib.ptr(self.fit_ws), need, _lib.stream_ptr()), "hb_de_fit")
         self.losses = losses[:, :T]
         if self.verbose:
-            L = self.losses.cpu()
-            for i in range(E):
-                for ep in range(0, T, self.print_every):
-                    print("Epoch %d, %s loss = %g" % (ep, self.loss_name, float(L[i, ep])), flush=True)
+            self._print_losses()
 
     def fit_state(self):
         """Views of the fit workspace: Adam's exp_avg, exp_avg_sq and the last step's gradient, each [E, P]."""
@@ -345,6 +358,18 @@ class DeepEnsemble(BaseModel):
         mu, var = self._predict_dev(xs, xe)
         return (mu.cpu(), var.cpu()) if on_cpu else (mu, var)
 
+    def sample_y(self, Xc, Xe=None, n_samples: int = 1):
+        """BaseModel.sample_y (base_model.py:78-84): py + sqrt(ps2) * N(0, 1), independent draws, [n_samples, m, num_out].
+        One hb_de_predict_batch launch with in-kernel Philox draws keyed by a seed from torch's global generator, so the
+        result is reproducible under torch.manual_seed (the reference draws torch.randn on the host).  CPU tensors for CPU
+        inputs."""
+        probe = Xc if (Xc is not None and self.num_cont > 0) else Xe
+        on_cpu = not (torch.is_tensor(probe) and probe.is_cuda)
+        xs, xe, _ = self._inputs(Xc, Xe)
+        seed = int(torch.randint(0, 2 ** 62, (1,)).item())
+        _, _, samp = EnsembleBatch([self]).predict(xs, xe, n_samples=n_samples, seed=seed)
+        return samp.cpu() if on_cpu else samp
+
     def predict_mace(self, Xc, tau: float, kappa: float, eps: float = 1e-4, xi1=None, xi2=None, seed: int = 0,
                      return_mu_var: bool = False, Xe=None, device_out: bool = False):
         """predict + MACE.eval (acq.py:146-171) through ``hb_mace_epilogue``: F [m, 3] = (LCB, -logEI, -logPI), on the
@@ -388,3 +413,84 @@ class DeepEnsemble(BaseModel):
         """One BaseNet state_dict per member, from the device parameters."""
         raw = self.params.cpu()
         return [raw_to_state_dict(raw[i], self.layout) for i in range(self.num_ensembles)]
+
+
+def _stacked_params(models) -> torch.Tensor:
+    """[B, E, P] device parameters of B ensembles: the common tensor when their params are consecutive slices of one
+    (as fit_ensembles leaves them), otherwise a stacked copy."""
+    base = models[0].params
+    step = base.numel() * base.element_size()
+    if all(m.params.is_contiguous() and m.params.data_ptr() == base.data_ptr() + b * step for b, m in enumerate(models)):
+        return torch.as_strided(base, (len(models),) + tuple(base.shape), (base.numel(), base.shape[1], 1))
+    return torch.stack([m.params for m in models]).contiguous()
+
+
+class EnsembleBatch:
+    """B fitted DeepEnsembles of one spec (one multi-output ensemble, or the single-output ensembles of a MultiTaskModel)
+    as one ``hb_de_predict_batch`` operand.  The stacked parameters and scalers are taken when it is built."""
+
+    def __init__(self, models):
+        m0 = models[0]
+        assert all(m.fitted for m in models), "fit() first"
+        self.models, self.spec, self.E, self.device = models, m0._spec, m0.num_ensembles, m0.device
+        self.num_cont, self.num_out = m0.num_cont, len(models) * m0.num_out
+        self.params = _stacked_params(models)
+        sc = [m._scal_dev() for m in models]
+        self.xm = torch.stack([t[0] for t in sc]).contiguous() if self.num_cont > 0 else None
+        self.xa = torch.stack([t[1] for t in sc]).contiguous() if self.num_cont > 0 else None
+        self.ym = torch.stack([t[2] for t in sc]).contiguous()
+        self.ys = torch.stack([t[3] for t in sc]).contiguous()
+
+    def predict(self, xs, xe, n_samples: int = 0, xi=None, seed: int = 0, counter: int = 0):
+        """(mu, var) [B num_out, m] output-major, and y_samp [n_samples, m, B num_out] (None when n_samples = 0), from
+        device inputs xs [m, num_cont] fp32 (None without numeric columns) and xe [m, num_enum] int32."""
+        m = (xs if xs is not None else xe).shape[0]
+        dev, K = self.device, self.num_out
+        mu = torch.empty(K, m, dtype=torch.float32, device=dev)
+        var = torch.empty_like(mu)
+        samp = torch.empty(n_samples, m, K, dtype=torch.float32, device=dev) if n_samples > 0 else None
+        xi = None if xi is None else torch.as_tensor(xi).to(dev, torch.float32).contiguous()
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().hb_de_predict_batch(
+                _lib.ptr(xs), _lib.ptr(xe), m, C.byref(self.spec), len(self.models), self.E, _lib.ptr(self.params),
+                _lib.ptr(self.xm), _lib.ptr(self.xa), _lib.ptr(self.ym), _lib.ptr(self.ys), _lib.ptr(mu), _lib.ptr(var),
+                int(n_samples), _lib.ptr(xi), int(seed) & (2 ** 64 - 1), int(counter), _lib.ptr(samp), _lib.stream_ptr()),
+                "hb_de_predict_batch")
+        return mu, var, samp
+
+
+def batch_offsets(ns) -> list:
+    """off [B + 1] of hb_de_fit_batch: ensemble b's rows are off[b] .. off[b + 1] - 1 of the concatenation."""
+    return [0] + np.cumsum(np.asarray(ns, dtype=np.int64)).tolist()
+
+
+def fit_ensembles(models, Xc, Xe, ys) -> None:
+    """model.fit(Xc, Xe, ys[b]) for every model b of B DeepEnsembles with one spec, in ONE hb_de_fit_batch launch.  The
+    host side runs model by model in the order the sequential loop draws from torch's generator (model b: its initial
+    weights on its first fit, then its seed), so every model ends bit-identical to its own fit.  Each model keeps its own
+    row filter and scalers; afterwards its params, fit workspace and losses are slices of the batch's tensors."""
+    m0 = models[0]
+    B, E, T, dev = len(models), m0.num_ensembles, int(m0.num_epochs), m0.device
+    if B > _lib.HB_MAX_OUTPUTS:
+        raise NotImplementedError(f"fit_ensembles: {B} ensembles exceed the limit of {_lib.HB_MAX_OUTPUTS} (HB_MAX_OUTPUTS)")
+    preps = [m._prepare_fit(Xc, Xe, y) for m, y in zip(models, ys)]
+    off = batch_offsets([p[2].shape[0] for p in preps])
+    xc = torch.cat([p[0] for p in preps]).to(dev, torch.float32).contiguous() if m0.num_cont > 0 else None
+    xe = torch.cat([p[1] for p in preps]).to(dev, torch.int32).contiguous() if m0.num_enum > 0 else None
+    yd = torch.cat([p[2] for p in preps]).to(dev, torch.float32).contiguous()
+    params = torch.stack([m.params for m in models]).contiguous()
+    lib = _lib.lib()
+    need = int(lib.hb_de_fit_workspace_bytes(C.byref(m0._spec), E))
+    ws = torch.empty(B * need, dtype=torch.uint8, device=dev)
+    losses = torch.empty(B, E, max(1, T), dtype=torch.float32, device=dev)
+    c_off = (C.c_int64 * (B + 1))(*off)
+    c_seed = (C.c_uint64 * B)(*[m.seed & (2 ** 64 - 1) for m in models])
+    with torch.cuda.device(dev):
+        _lib.check(lib.hb_de_fit_batch(_lib.ptr(xc), _lib.ptr(xe), _lib.ptr(yd), c_off, B, C.byref(m0._spec), E,
+                                       _lib.ptr(params), float(m0.lr), float(m0.l1), int(m0.batch_size), T, c_seed,
+                                       _lib.ptr(losses), _lib.ptr(ws), B * need, _lib.stream_ptr()), "hb_de_fit_batch")
+    for b, m in enumerate(models):
+        m.params, m.fit_ws, m.losses = params[b], ws[b * need:(b + 1) * need], losses[b, :, :T]
+        if m.verbose:
+            m._print_losses()
+        m._finish_fit(Xc, Xe, ys[b], preps[b][3])

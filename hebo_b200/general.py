@@ -1,7 +1,8 @@
 """Multi-objective and constrained Bayesian optimisation: ``GeneralBO`` (HEBO/hebo/optimizers/general.py:23-204).
 
 ``GeneralBO`` fits a ``hebo_b200.MultiTaskModel`` (one GP per objective and constraint column, trained in one batched
-device fit) on the raw y, scores ``GeneralAcq`` -- the LCB of every output -- with the device GA
+device fit; with ``model_config={'base_model_name': 'deep_ensemble'}`` one deep ensemble per column, trained in one
+launch), or with ``model_name='deep_ensemble'`` one multi-output ``hebo_b200.DeepEnsemble``, on the raw y, scores ``GeneralAcq`` -- the LCB of every output -- with the device GA
 (``hebo_b200.evolution.DeviceNSGA2`` with ``num_obj`` objectives and, when there are constraints, the summed constraint
 violation as its constraint column), and picks the suggestions from the resulting (feasible) front: at random with the
 most uncertain row kept, or by a Monte-Carlo expected hypervolume improvement when ``ref_point`` is given.
@@ -21,6 +22,7 @@ import torch
 
 from .acq import GeneralAcq, general_score
 from .bo import _design_space
+from .ensemble import DeepEnsemble
 from .gp import GP, MultiTaskModel
 
 
@@ -58,8 +60,11 @@ class GeneralBO:
     """general.py:23-204.  ``space``: a DesignSpace (or its list-of-dicts spec).  y has num_obj objective columns
     followed by num_constr constraint columns, all minimised; a row is feasible when every constraint is <= 0.
 
-    model_name: 'multi_task' (the default, ``hebo_b200.MultiTaskModel``) or 'gp' when num_obj + num_constr == 1; any
-    other surrogate raises NotImplementedError, and 'gp' with several outputs fails the reference's multi-output assertion.
+    model_name: 'multi_task' (the default, ``hebo_b200.MultiTaskModel``; model_config['base_model_name'] picks 'gp' or
+    'deep_ensemble' for its outputs), 'deep_ensemble' (one ``hebo_b200.DeepEnsemble`` with num_obj + num_constr outputs)
+    or 'gp' when num_obj + num_constr == 1; any other surrogate raises NotImplementedError, and 'gp' with several outputs
+    fails the reference's multi-output assertion.  Over deep ensembles the GA scores every generation with one
+    hb_de_predict_batch launch, and the EHVI selection (``ref_point``) draws its samples on the device.
     ``evo_pop`` / ``evo_iters`` are read when ``suggest`` runs, so they may be changed after construction.  As in the
     reference, ``fix_input`` only applies to the random start-up design: the model stage does not pass it to the GA."""
 
@@ -73,10 +78,11 @@ class GeneralBO:
                  model_name: str = "multi_task", model_config: Optional[dict] = None, kappa: Optional[float] = 2.0,
                  c_kappa: Optional[float] = 0.0, use_noise: bool = False, evo_pop: int = 100, evo_iters: int = 200,
                  ref_point: Optional[np.ndarray] = None, device: str = "cuda"):
-        if model_name not in ("multi_task", "gp"):
-            raise NotImplementedError(f"GeneralBO: model_name {model_name!r} is not supported, only 'multi_task' and 'gp'")
+        if model_name not in ("multi_task", "gp", "deep_ensemble"):
+            raise NotImplementedError(f"GeneralBO: model_name {model_name!r} is not supported, only 'multi_task', 'gp' and "
+                                      "'deep_ensemble'")
         if num_obj + num_constr > 1:
-            assert model_name == "multi_task", "GeneralBO: several outputs need a multi-output model"   # general.py:63-64
+            assert model_name != "gp", "GeneralBO: several outputs need a multi-output model"   # general.py:63-64
         self.space = _design_space(space)
         self.num_obj, self.num_constr = num_obj, num_constr
         self.rand_sample = 1 + self.space.num_paras if rand_sample is None else rand_sample
@@ -99,7 +105,8 @@ class GeneralBO:
         conf = {"device": self.device, **self.model_config}
         if e > 0:
             conf["num_uniqs"] = self.space.num_uniqs
-        model = MultiTaskModel(d, e, K, **conf) if self.model_name == "multi_task" else GP(d, e, 1, **conf)
+        cls = {"multi_task": MultiTaskModel, "deep_ensemble": DeepEnsemble}.get(self.model_name)
+        model = cls(d, e, K, **conf) if cls is not None else GP(d, e, 1, **conf)
         model.fit(Xc if d else None, Xe if e else None, torch.FloatTensor(self.y))
         torch.cuda.synchronize()
         return model

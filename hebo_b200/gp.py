@@ -780,15 +780,38 @@ def _fit_psgld(models, Xc, Xe, y) -> None:
 
 class MultiTaskModel(BaseModel):
     """Multi-output wrapper: one single-output model per column of y (HEBO/hebo/models/model_factory.py:60-92), the
-    building block of the reference's multi-objective / constrained optimisers (GeneralBO)."""
+    building block of the reference's multi-objective / constrained optimisers (GeneralBO).
+
+    conf['base_model_name']: 'gp' (the default), or 'deep_ensemble': one single-output ``DeepEnsemble`` per column, all
+    fitted in one ``hb_de_fit_batch`` launch (each with its own finite rows and scalers, bit-identical to fitting them one
+    after another) and scored in one ``hb_de_predict_batch`` launch.  Any other name raises NotImplementedError."""
     support_multi_output = True
 
     def __init__(self, num_cont, num_enum, num_out, **conf):
         super().__init__(num_cont, num_enum, num_out, **conf)
+        self.base_model_name = conf.get("base_model_name", "gp")
         self.model_conf = {k: v for k, v in conf.items() if k not in ("model_name", "base_model_name")}
-        self.models = [GP(num_cont, num_enum, 1, **self.model_conf) for _ in range(num_out)]
+        if self.base_model_name == "gp":
+            self.models = [GP(num_cont, num_enum, 1, **self.model_conf) for _ in range(num_out)]
+        elif self.base_model_name == "deep_ensemble":
+            from .ensemble import DeepEnsemble
+            if num_out > _lib.HB_MAX_OUTPUTS:
+                raise NotImplementedError(f"MultiTaskModel: {num_out} deep ensembles exceed the limit of {_lib.HB_MAX_OUTPUTS}")
+            self.models = [DeepEnsemble(num_cont, num_enum, 1, **self.model_conf) for _ in range(num_out)]
+        else:
+            raise NotImplementedError(f"MultiTaskModel: base_model_name {self.base_model_name!r} is not supported, only 'gp' "
+                                      "and 'deep_ensemble'")
+
+    @property
+    def _ensembles(self) -> bool:
+        return self.base_model_name == "deep_ensemble"
 
     def fit(self, Xc, Xe, y):
+        if self._ensembles:
+            from .ensemble import fit_ensembles
+            y = torch.as_tensor(y)
+            fit_ensembles(self.models, Xc, Xe, [y[:, [i]] for i in range(self.num_out)])
+            return
         if self._batched(y):
             self._fit_batched(Xc, Xe, y)
             return
@@ -807,8 +830,29 @@ class MultiTaskModel(BaseModel):
         _fit_psgld(self.models, Xc, Xe, y)
 
     def predict(self, Xc, Xe=None):
+        if self._ensembles and not (torch.is_tensor(Xc) and Xc.requires_grad):
+            return self._predict_ensembles(Xc, Xe)
         out = [m.predict(Xc, Xe) for m in self.models]
         return torch.cat([o[0] for o in out], dim=1), torch.cat([o[1] for o in out], dim=1)
+
+    def _predict_ensembles(self, Xc, Xe, n_samples: int = 0, seed: int = 0):
+        """(py, ps2) [m, num_out] (and the draws [n_samples, m, num_out]) of every output's ensemble in one
+        hb_de_predict_batch launch; CPU tensors for CPU inputs."""
+        from .ensemble import EnsembleBatch
+        m0 = self.models[0]
+        probe = Xc if (Xc is not None and self.num_cont > 0) else Xe
+        on_cpu = not (torch.is_tensor(probe) and probe.is_cuda)
+        xs, xe, _ = m0._inputs(Xc, Xe)
+        mu, var, samp = EnsembleBatch(self.models).predict(xs, xe, n_samples=n_samples, seed=seed)
+        out = (mu.t(), var.t()) if n_samples == 0 else (samp,)
+        return tuple(t.cpu() for t in out) if on_cpu else out
+
+    def sample_y(self, Xc, Xe=None, n_samples: int = 1):
+        """With deep ensembles: DeepEnsemble.sample_y over all outputs in one launch ([n_samples, m, num_out], seed from
+        torch's global generator).  With GPs: BaseModel.sample_y."""
+        if not self._ensembles:
+            return super().sample_y(Xc, Xe, n_samples)
+        return self._predict_ensembles(Xc, Xe, n_samples, int(torch.randint(0, 2 ** 62, (1,)).item()))[0]
 
     @property
     def noise(self):

@@ -1,11 +1,13 @@
 """``NoisyOpt`` (HEBO/hebo/optimizers/noisy_opt.py): HEBO's batch selection over the final population of a single-objective
 GA whose acquisition is one joint posterior draw per generation (``hebo_b200.acq.NoisyAcq``, acq.py:173-190).
 
-The GP is fitted on the raw y.  The device GA (``hebo_b200.evolution.DeviceNSGA2`` with a one-column score, pop 100 x 100
-generations) scores every generation with ``hb_sample_y_batch``: one correlated draw over the batch, with the jitter ladder
-on the device and duplicate rows left out of the joint covariance (they are +inf, which the GA survival gives a duplicate
-child anyway).  The generation loop never synchronises with the host; the status word of the ladder is read once, after
-the GA.  Suggestions follow noisy_opt.py:59-89: the final population in survival order, rows equal to an observation
+The model (a GP, or with ``model_name='deep_ensemble'`` a ``hebo_b200.DeepEnsemble``) is fitted on the raw y.  The device
+GA (``hebo_b200.evolution.DeviceNSGA2`` with a one-column score, pop 100 x 100 generations) scores every generation on the
+device.  Over the GP: ``hb_sample_y_batch``, one correlated draw over the batch, with the jitter ladder on the device and
+duplicate rows left out of the joint covariance (they are +inf, which the GA survival gives a duplicate child anyway); the
+status word of the ladder is read once, after the GA.  Over the deep ensemble: ``hb_de_predict_batch`` with one independent
+draw per row, as the reference's ``BaseModel.sample_y`` draws them.  The generation loop never synchronises with the
+host.  Suggestions follow noisy_opt.py:59-89: the final population in survival order, rows equal to an observation
 dropped, a Sobol top-up, then a random pick of q with the argmax-sigma / argmin-mu rows forced into slots 0 / 1 when
 q > 2.
 """
@@ -19,14 +21,16 @@ import torch
 
 from . import _lib
 from .acq import NoisyAcq, ga_score
+from .ensemble import DeepEnsemble
 from .evolution import DeviceNSGA2
 from .gp import GP
 from .suggest import HEBO
 
 
 class NoisyOpt(HEBO):
-    """noisy_opt.py:27-89.  ``space``: a DesignSpace (or its list-of-dicts spec); DataFrames in and out.  Only
-    ``model_name='gp'`` is supported.  ``evo_pop`` <= 256: the device sampler draws at most 256 rows jointly."""
+    """noisy_opt.py:27-89.  ``space``: a DesignSpace (or its list-of-dicts spec); DataFrames in and out.  model_name:
+    'gp' or 'deep_ensemble'.  With 'gp', ``evo_pop`` <= 256: the GP sampler draws at most 256 rows jointly; the deep
+    ensemble's draws are independent, so it takes any population the device GA takes (DeviceNSGA2.MAX_POP)."""
 
     support_parallel_opt = True
     support_combinatorial = True
@@ -35,12 +39,13 @@ class NoisyOpt(HEBO):
 
     def __init__(self, space, model_name: str = "gp", rand_sample: Optional[int] = None, model_config: Optional[dict] = None,
                  scramble_seed: Optional[int] = None, evo_pop: int = 100, evo_iters: int = 100, device: str = "cuda"):
-        if model_name != "gp":
-            raise NotImplementedError(f"NoisyOpt: model_name {model_name!r} is not supported, only 'gp'")
-        if not 2 <= int(evo_pop) <= self.MAX_POP:
-            raise ValueError(f"NoisyOpt: evo_pop must lie in [2, {self.MAX_POP}], got {evo_pop}")
+        if model_name not in ("gp", "deep_ensemble"):
+            raise NotImplementedError(f"NoisyOpt: model_name {model_name!r} is not supported, only 'gp' and 'deep_ensemble'")
+        max_pop = self.MAX_POP if model_name == "gp" else DeviceNSGA2.MAX_POP
+        if not 2 <= int(evo_pop) <= max_pop:
+            raise ValueError(f"NoisyOpt: evo_pop must lie in [2, {max_pop}], got {evo_pop}")
         super().__init__(space, model_config=model_config, rand_sample=rand_sample, scramble_seed=scramble_seed, device=device,
-                         acq_optimizer="nsga2", evo_pop=int(evo_pop), evo_iters=int(evo_iters))
+                         acq_optimizer="nsga2", evo_pop=int(evo_pop), evo_iters=int(evo_iters), model_name=model_name)
         self.acq_cls = NoisyAcq
 
     def suggest(self, n_suggestions: int = 1, fix_input: Optional[dict] = None):
@@ -48,7 +53,7 @@ class NoisyOpt(HEBO):
         if self.Xc.shape[0] < self.rand_sample:                    # noisy_opt.py:41-43: Sobol start-up design
             return self.quasi_sample(n_suggestions)
         t0 = time.perf_counter()
-        model = GP(self.d, self.e, 1, device=self.device, **self.model_config)
+        model = (GP if self.model_name == "gp" else DeepEnsemble)(self.d, self.e, 1, device=self.device, **self.model_config)
         model.fit(self.Xc if self.d else None, self.Xe if self.e else None, torch.FloatTensor(self.y).clone())   # raw y
         torch.cuda.synchronize()
         t1 = time.perf_counter()

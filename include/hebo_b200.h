@@ -572,6 +572,34 @@ int32_t hb_de_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de
 int32_t hb_de_predict_grad(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t E,
                            const float *params, const float *x_mul, const float *x_add, const float *y_mean,
                            const float *y_std, float *mu, float *var, float *dmu, float *dvar, void *stream);
+/* hb_de_fit for B ensembles of one spec in ONE launch (a MultiTaskModel of K single-output ensembles, model_factory.py:60-92),
+ * 1 <= B <= HB_MAX_OUTPUTS, grid B E CTAs: CTA (b, member) runs hb_de_fit's member on ensemble b.  B E > 132 takes more
+ * than one wave on a 132-SM H100.
+ *   off HOST [B + 1] int64: ensemble b trains on rows off[b] .. off[b + 1] - 1 (n_b >= 1 of them) of the concatenated
+ *   Xc [., num_cont], Xe [., num_enum] and y [., num_out], each slice filtered and scaled by its own ensemble.
+ *   seeds HOST [B]: ensemble b's Philox key; the minibatch order is always the keyed bijection of hb_de_fit (no perm).
+ *   params [B, E, P] in/out; losses [B, E, num_epochs]; L1 coefficient l1 / (n_b num_out) per ensemble; lr, l1,
+ *   batch_size and num_epochs shared.  The minibatch of min(n_b, batch_size) rows obeys HB_DE_MAX_BATCH_FLOATS for every b.
+ *   ws: ws_bytes >= B * hb_de_fit_workspace_bytes(spec, E); slice b (3 E P floats from ws + 3 b E P) is laid out as
+ *   hb_de_fit's workspace.
+ * Ensemble b's params, Adam moments, last gradient and losses are bit-identical to hb_de_fit on its slice alone with
+ * seed seeds[b].  No host synchronisation. */
+int32_t hb_de_fit_batch(const float *Xc, const int32_t *Xe, const float *y, const int64_t *off, int64_t B,
+                        const hb_de_spec_t *spec, int64_t E, float *params, double lr, float l1, int64_t batch_size,
+                        int64_t num_epochs, const uint64_t *seeds, float *losses, void *ws, int64_t ws_bytes, void *stream);
+/* hb_de_predict (member = -1) of B ensembles of one spec over one candidate batch, 1 <= B <= HB_MAX_OUTPUTS: params
+ * [B, E, P], x_mul / x_add [B, num_cont], y_mean / y_std [B, num_out].  mu / var [B num_out, m] OUTPUT-MAJOR (row
+ * b num_out + o is output o of ensemble b), the layout hb_general_acq_epilogue reads; each row is bit-identical to the
+ * matching column of hb_de_predict on ensemble b.
+ * n_samples > 0: the same launch also writes y_samp [n_samples, m, B num_out] = py + sqrt(ps2) * xi (BaseModel.sample_y,
+ * base_model.py:78-84: independent draws) with py / ps2 the mu / var above, correctly rounded fp32 without FMA
+ * contraction, so bit-identical to torch's fp32 expression on the same draws.  xi [n_samples, m, B num_out] device, or
+ * NULL: Philox4x32-10 + Box-Muller keyed by (seed, counter), element q (flat index of y_samp) takes half q % 2 of pair
+ * q / 2 (hb_general_acq_epilogue's convention); the same (seed, counter) replays the same bits.  No host synchronisation. */
+int32_t hb_de_predict_batch(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t B, int64_t E,
+                            const float *params, const float *x_mul, const float *x_add, const float *y_mean,
+                            const float *y_std, float *mu, float *var, int64_t n_samples, const float *xi, uint64_t seed,
+                            uint64_t counter, float *y_samp, void *stream);
 
 #ifdef __cplusplus
 }
