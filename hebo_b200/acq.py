@@ -24,6 +24,7 @@ import torch
 from . import _lib
 from .base import Acquisition
 from .ensemble import DeepEnsemble, EnsembleBatch
+from .forest import RF
 from .gp import GP, MultiTaskModel
 
 
@@ -143,6 +144,16 @@ def _noisy_ensemble_score(model, seed: int):
     return score
 
 
+def _noisy_forest_score(model, seed: int):
+    """score(xc, xe, gen) of NoisyAcq over a fitted RF: one hb_rf_predict per generation with one independent draw per row
+    (BaseModel.sample_y), keyed by (seed, counter = gen)."""
+    def score(xc, xe, gen):
+        _, _, samp = model._predict_dev(xc if model.num_cont > 0 else None, xe if model.num_enum > 0 else None, n_samples=1,
+                                        seed=seed, counter=gen)
+        return samp.reshape(-1)
+    return score
+
+
 def ga_score(acq, seed=None):
     """score(xc, xe, gen) -> f [m] fp32 on the device for DeviceNSGA2, of a single-objective acquisition.  xc [m, d] fp32
     and xe [m, e] int32 are device tensors.  With a hebo_b200.GP and one of the four acquisitions above: predict on the
@@ -150,15 +161,18 @@ def ga_score(acq, seed=None):
     objective and no constraint over a fitted hebo_b200.GP: one joint draw per generation on the device
     (``GP.sample_y_batch``, counter = the generation, ``seed`` drawn from numpy's global generator when None; batches of at
     most 256 rows); over a fitted single-output DeepEnsemble: one hb_de_predict_batch per generation with one
-    independent draw per row (counter = the generation, any batch size).  Otherwise: acq.eval on CPU tensors (xe as int64,
+    independent draw per row (counter = the generation, any batch size); over a fitted RF: one hb_rf_predict per generation
+    with the same draw layout.  The four acquisitions above over an RF score on the device as over a GP.  Otherwise: acq.eval on CPU tensors (xe as int64,
     like the reference's BOProblem), its first column copied back to the device."""
     if type(acq) is NoisyAcq and acq.num_obj == 1 and acq.num_constr == 0:
         if isinstance(acq.model, GP) and not acq.model._fit_failed:
             return _noisy_device_score(acq.model, int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed))
         if isinstance(acq.model, DeepEnsemble) and acq.model.fitted and acq.model.num_out == 1:
             return _noisy_ensemble_score(acq.model, int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed))
+        if isinstance(acq.model, RF) and acq.model.fitted:
+            return _noisy_forest_score(acq.model, int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed))
     mode = _ACQ1_MODES.get(type(acq))
-    if mode is not None and isinstance(acq.model, (GP, DeepEnsemble)):
+    if mode is not None and isinstance(acq.model, (GP, DeepEnsemble, RF)):
         kappa = float(getattr(acq, "kappa", 0.0))
         eta = float(getattr(acq, "eta", 0.0))
 
@@ -302,16 +316,18 @@ def general_score(acq, seed=None):
     hb_mo_lcb_epilogue with Philox draws keyed by (seed, gen), its G being the one constraint column.  With deep
     ensembles -- a GeneralAcq over one multi-output DeepEnsemble or a MultiTaskModel of them, a MOMeanSigmaLCB over one
     DeepEnsemble -- the posterior is one hb_de_predict_batch (GeneralAcq, writing [K, m] directly) or hb_de_predict
-    (MOMeanSigmaLCB) call, followed by the same epilogue.  None of these synchronises with the host inside a generation;
+    (MOMeanSigmaLCB) call, followed by the same epilogue; with an RF, one hb_rf_predict call and the same epilogues.  None of these synchronises with the host inside a generation;
     an output whose GP fit failed predicts N(y_mean, y_std^2) as GP.predict does.  ``seed`` is drawn from numpy's global
     generator when None.  Any other acquisition or model, including subclasses of these two: acq.eval on CPU tensors (xe as
     int64), once per generation."""
     no, nc = acq.num_obj, acq.num_constr
     model = acq.model
-    if type(acq) is MOMeanSigmaLCB and isinstance(model, (GP, DeepEnsemble)):
+    if type(acq) is MOMeanSigmaLCB and isinstance(model, (GP, DeepEnsemble, RF)):
         return _mo_lcb_device_score(acq, seed)
     if type(acq) is GeneralAcq and _ensembles_of(model) is not None:
         return _general_ensemble_score(acq, _ensembles_of(model), seed)
+    if type(acq) is GeneralAcq and isinstance(model, RF):
+        return _general_forest_score(acq, seed)
     gps = None
     if isinstance(model, GP):
         gps = [model]
@@ -368,6 +384,20 @@ def _general_ensemble_score(acq, models, seed=None):
     return device_score
 
 
+def _general_forest_score(acq, seed=None):
+    seed = int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed)
+    no, nc, model = acq.num_obj, acq.num_constr, acq.model
+    noise_sd = model.noise.reshape(-1).float().sqrt().to(model.device).contiguous() if acq.use_noise else None
+    kappa, c_kappa = float(acq.kappa), float(acq.c_kappa)
+
+    def device_score(xc, xe, gen):
+        mu, var, _ = model._predict_dev(xc if model.num_cont > 0 else None, xe if model.num_enum > 0 else None)
+        Fo, _, cv = _general_epilogue(mu.reshape(1, -1), var.reshape(1, -1), no, nc, kappa, c_kappa, noise_sd, None, seed, gen,
+                                      want_cv=nc > 0)
+        return (Fo, cv) if nc else Fo
+    return device_score
+
+
 def _mo_lcb_device_score(acq, seed=None):
     seed = int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed)
     model = acq.model
@@ -379,7 +409,7 @@ def _mo_lcb_device_score(acq, seed=None):
             if isinstance(model, GP):
                 _, mu, var = model._posterior(model._to_dev(xc), False, Xe_dev=model._xe_dev(xe, m))
             else:
-                mu, var = model._predict_dev(xc if model.num_cont > 0 else None, xe if model.num_enum > 0 else None)
+                mu, var = model._predict_dev(xc if model.num_cont > 0 else None, xe if model.num_enum > 0 else None)[:2]
                 mu, var = mu.reshape(-1), var.reshape(-1)
         return _mo_lcb_epilogue(mu, var, noise_sd, best_y, kappa, None, seed, gen)
     return device_score
@@ -405,6 +435,8 @@ class MACE(Acquisition):
         tau = float(np.asarray(self.tau).reshape(-1)[0])
         with torch.no_grad():
             if isinstance(self.model, GP):     # predict + MACE fused in ONE C-ABI call (a failed fit degrades inside it, gp.py:152-154)
+                return self.model.predict_mace(x, tau, float(self.kappa), float(self.eps), Xe=xe)
+            if isinstance(self.model, RF):     # predict + hb_mace_epilogue, draws as acq.py:154-155
                 return self.model.predict_mace(x, tau, float(self.kappa), float(self.eps), Xe=xe)
             return self._eval_any_model(x, xe, tau)
 

@@ -1061,4 +1061,36 @@ int32_t hb_de_predict_batch(const float *Xs, const int32_t *Xe, int64_t m, const
                                  counter, y_samp, (cudaStream_t)stream);
 }
 
+// rf.py:19-56: RF over sklearn's RandomForestRegressor (forest.cu)
+int64_t hb_rf_fit_workspace_bytes(int64_t n, const hb_rf_spec_t *spec, int64_t B, int64_t T) {
+  return rf_fit_ws_query(n, spec, B, T);
+}
+
+int64_t hb_rf_forest_bytes(const hb_rf_spec_t *spec, int64_t max_nodes, int64_t B, int64_t T) {
+  return rf_forest_bytes(spec, max_nodes, B, T);
+}
+
+// rf.py:37-43 (fit)
+int32_t hb_rf_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_rf_spec_t *spec, int64_t B,
+                  int64_t T, const int32_t *counts, uint64_t seed, void *forest, float *noise, void *ws, int64_t ws_bytes,
+                  void *stream) {
+  return launch_rf_fit(Xc, Xe, y, n, spec, B, T, counts, seed, forest, noise, ws, ws_bytes, (cudaStream_t)stream);
+}
+
+// rf.py:49-56 (predict) and BaseModel.sample_y (base_model.py:78-84)
+int32_t hb_rf_predict(const float *Xc, const int32_t *Xe, int64_t m, const hb_rf_spec_t *spec, const void *forest,
+                      int64_t B, int64_t T, const float *noise, float *mean, float *var, int64_t n_samples, uint64_t seed,
+                      uint64_t counter, float *samples, void *stream) {
+  return launch_rf_predict(Xc, Xe, m, spec, forest, B, T, noise, mean, var, n_samples, seed, counter, samples,
+                           (cudaStream_t)stream);
+}
+
+// a forest from per-tree node arrays (sklearn's tree_.children_left / children_right / feature / threshold / value)
+int32_t hb_rf_load(const int32_t *left, const int32_t *right, const int32_t *feature, const double *threshold,
+                   const double *value, const int32_t *node_counts, const hb_rf_spec_t *spec, int64_t T,
+                   int64_t max_nodes, void *forest, void *stream) {
+  return launch_rf_load(left, right, feature, threshold, value, node_counts, spec, T, max_nodes, forest,
+                        (cudaStream_t)stream);
+}
+
 }  // extern "C"

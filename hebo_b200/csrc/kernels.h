@@ -243,4 +243,17 @@ int launch_de_predict_batch(const float *Xs, const int32_t *Xe, int64_t m, const
                             const float *y_std, float *mu, float *var, int64_t n_samples, const float *xi, uint64_t seed,
                             uint64_t counter, float *y_samp, cudaStream_t st);
 
+// random-forest surrogate (forest.cu)
+int64_t rf_forest_bytes(const hb_rf_spec_t *spec, int64_t max_nodes, int64_t B, int64_t T);
+int64_t rf_fit_ws_query(int64_t n, const hb_rf_spec_t *spec, int64_t B, int64_t T);
+int launch_rf_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_rf_spec_t *spec, int64_t B,
+                  int64_t T, const int32_t *counts, uint64_t seed, void *forest, float *noise, void *ws, int64_t ws_bytes,
+                  cudaStream_t st);
+int launch_rf_predict(const float *Xc, const int32_t *Xe, int64_t m, const hb_rf_spec_t *spec, const void *forest,
+                      int64_t B, int64_t T, const float *noise, float *mean, float *var, int64_t n_samples, uint64_t seed,
+                      uint64_t counter, float *samples, cudaStream_t st);
+int launch_rf_load(const int32_t *left, const int32_t *right, const int32_t *feature, const double *thr,
+                   const double *value, const int32_t *node_counts, const hb_rf_spec_t *spec, int64_t T, int64_t max_nodes,
+                   void *forest, cudaStream_t st);
+
 }  // namespace hb

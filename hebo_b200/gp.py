@@ -734,19 +734,24 @@ class GP(BaseModel):
 B200GP = GP
 
 
-def register(name: str = "gp_b200", override_gp: bool = False) -> bool:
+def register(name: str = "gp_b200", override_gp: bool = False, override_rf: bool = False) -> bool:
     """Register into a real HEBO install's model registry (model_factory.py:30-58).  Returns False when
-    ``hebo`` is not importable."""
+    ``hebo`` is not importable.  The device random forest is always added as ``rf_b200``; ``override_rf`` also makes it the
+    install's ``'rf'``."""
     try:
         from hebo.models import model_factory
     except Exception:
         return False
     from .ensemble import DeepEnsemble
+    from .forest import RF
     model_factory.model_dict[name] = GP
     model_factory.model_dict["multi_task_b200"] = MultiTaskModel
     model_factory.model_dict["deep_ensemble_b200"] = DeepEnsemble
+    model_factory.model_dict["rf_b200"] = RF
     if override_gp:
         model_factory.model_dict["gp"] = GP
+    if override_rf:
+        model_factory.model_dict["rf"] = RF
     model_factory.model_names = list(model_factory.model_dict.keys())
     return True
 

@@ -601,6 +601,73 @@ int32_t hb_de_predict_batch(const float *Xs, const int32_t *Xe, int64_t m, const
                             const float *y_std, float *mu, float *var, int64_t n_samples, const float *xi, uint64_t seed,
                             uint64_t counter, float *y_samp, void *stream);
 
+/* ---- random-forest surrogate (models/rf/rf.py: RF :19-56 over sklearn's RandomForestRegressor defaults) ------------------
+ * T regression trees per output, each exact CART (squared error, every feature, min_samples_split 2, min_samples_leaf 1,
+ * unlimited depth) grown on bootstrap weights.  Tree inputs are NOT scaled: [Xc | one_hot(Xe)] (rf.py:27-35, layers.py:36),
+ * width = num_cont + sum(num_uniqs); one-hot column num_cont + j is category u of column c in column-major category order
+ * (c = 0 first).  Envelope (HB_ERR_INVALID before any launch outside it; the size queries return -1): */
+#define HB_RF_MAX_ROWS   8192     /* training rows n                                                                 */
+#define HB_RF_MAX_WIDTH  4096     /* num_cont + sum(num_uniqs) (= HB_MAX_FEATURES)                                  */
+#define HB_RF_MAX_TREES  1024     /* trees per output T (conf['n_estimators'])                                       */
+/* and 1 <= B <= HB_MAX_OUTPUTS outputs per fit.
+ *
+ * Forest (device bytes, hb_rf_forest_bytes): a 256-byte header {cap, B, T, woh, num_enum, 0, 0, 0} (int32; cap = node
+ * capacity per tree), then, each block 256-byte aligned: the decode tables int32 [num_enum] (categories per column) and
+ * [woh] ((c << 12) | u of one-hot column j); node counts int32 [B, T]; nodes int4 [B, T, cap]; thresholds double
+ * [B, T, cap]; node values double [B, T, cap].  Tree (b, t) is entry b T + t.  A node replaces one entry of sklearn's
+ * tree_ arrays (_tree.pyx): internal {feature, RD32(threshold) as fp32 bits, left, right}, leaf {-2, 0, value as the low and
+ * high words of its double}; the thresholds hold sklearn's fp64 threshold (-2 for a leaf) and the values
+ * tree_.value = sum(w y) / sum(w) of every node.  For fp32 x, x <= t exactly when x <= RD32(t) (t rounded toward -inf), so
+ * the fp32 traversal takes the fp64 decision of DecisionTreeRegressor.predict.  A fitted tree is numbered breadth first:
+ * the split nodes of a level, in index order, append their left then right child. */
+typedef struct {                  /* HOST struct */
+  int32_t        num_cont;        /* numeric columns                                                   */
+  int32_t        num_enum;        /* categorical columns                                               */
+  const int32_t *num_uniqs;       /* HOST [num_enum] categories per column (conf['num_uniqs'])         */
+} hb_rf_spec_t;
+
+/* Workspace of hb_rf_fit (HOST). */
+int64_t hb_rf_fit_workspace_bytes(int64_t n, const hb_rf_spec_t *spec, int64_t B, int64_t T);
+/* Bytes of a forest of B outputs x T trees with max_nodes node slots per tree (a fit of n rows: max_nodes = 2 n - 1)
+ * (HOST). */
+int64_t hb_rf_forest_bytes(const hb_rf_spec_t *spec, int64_t max_nodes, int64_t B, int64_t T);
+/* RF.fit (rf.py:37-43) of B outputs over one X, every tree of every output in one grow launch.
+ *   Xc [n, num_cont] fp32 (finite), Xe [n, num_enum] int32 in range, y [n, B] fp32: output b uses the rows with finite
+ *   y[:, b] (filter_nan(..., 'all') per column).
+ *   counts: NULL, or [B, T, n] int32 bootstrap counts (rows with non-finite y and negative counts weigh 0).  With NULL,
+ *   tree (b, t) draws n_b = #finite rows indices with replacement from output b's finite rows in row order: draw j is
+ *   row kept[umulhi(word j % 4 of Philox4x32-10 block (j / 4, t, b, 0x52460000) under `seed`, n_b)].
+ *   Growth: a node with fewer than 2 distinct in-bag rows, or impurity sum(w y^2)/W - (sum(w y)/W)^2 <= DBL_EPSILON, is a
+ *   leaf.  Each feature's in-bag rows are taken in the stable (value, row) order; a cut lies between sorted values
+ *   v[p-1] < v[p] with v[p] > v[p-1] + 1e-7 (fp64); the split maximises S_L^2/W_L + S_R^2/W_R (fp64), ties to the lowest
+ *   feature, then the lowest cut; threshold v[p-1]/2 + v[p]/2, or v[p-1] when that equals v[p] or is infinite; rows with
+ *   x <= threshold go left.  No feature with a cut: leaf.  Sums: the root's in row order; a node's left prefix
+ *   sums W_L, S_L = sum(w y), Q_L = sum((w y) y) sequentially in that sorted order; a child's totals are the split's left
+ *   sums and total - left for the right child.  Leaf value S / W.
+ *   forest: hb_rf_forest_bytes(spec, 2 n - 1, B, T) bytes; noise [B] fp32: est_noise = fp32(np.mean((forest mean -
+ *   y)^2)) over output b's finite rows, with the forest mean summed sequentially in tree order over fp64 leaf values, / T,
+ *   and numpy's pairwise sum.  Bit-identical from run to run.  Copies the spec's tables from the host and synchronises
+ *   the stream once before the launches. */
+int32_t hb_rf_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_rf_spec_t *spec, int64_t B,
+                  int64_t T, const int32_t *counts, uint64_t seed, void *forest, float *noise, void *ws, int64_t ws_bytes,
+                  void *stream);
+/* RF.predict (rf.py:49-56) of m candidates over a forest of B outputs x T trees: mean / var [m, B] with
+ *   mean = fp32(sum_t v_t / T), the sum sequential in tree order (RandomForestRegressor.predict);
+ *   var = fp32(np.var(v)) + noise[b] in fp32, np.var's mean and squared deviations both summed pairwise as numpy does.
+ * Bit-identical to the reference's fp32 outputs for the same trees.  A category outside 0 .. num_uniqs[c] - 1, or a forest
+ * whose header disagrees with (B, T, num_enum), gives NaN outputs.  n_samples > 0: samples [n_samples, m, B] =
+ * mean + sqrt(var) * xi, correctly rounded fp32, xi Philox4x32-10 + Box-Muller keyed by (seed, counter), element q (flat
+ * index of samples) takes half q % 2 of pair q / 2.  No host synchronisation. */
+int32_t hb_rf_predict(const float *Xc, const int32_t *Xe, int64_t m, const hb_rf_spec_t *spec, const void *forest,
+                      int64_t B, int64_t T, const float *noise, float *mean, float *var, int64_t n_samples, uint64_t seed,
+                      uint64_t counter, float *samples, void *stream);
+/* A one-output forest (B = 1) of T trees from device arrays [T, max_nodes] in sklearn's tree_ layout: children_left,
+ * children_right (-1 at a leaf), feature, threshold (fp64), value (fp64); node_counts [T] device int32.  For scoring a
+ * forest grown elsewhere.  Synchronises the stream once (header copy). */
+int32_t hb_rf_load(const int32_t *left, const int32_t *right, const int32_t *feature, const double *threshold,
+                   const double *value, const int32_t *node_counts, const hb_rf_spec_t *spec, int64_t T,
+                   int64_t max_nodes, void *forest, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
