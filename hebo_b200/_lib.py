@@ -23,6 +23,7 @@ HB_DE_MAX_BATCH_FLOATS = 56000
 HB_DE_EMBEDDING, HB_DE_ONEHOT = 0, 1
 # random-forest envelope (HB_RF_MAX_* of include/hebo_b200.h)
 HB_RF_MAX_ROWS, HB_RF_MAX_WIDTH, HB_RF_MAX_TREES = 8192, 4096, 1024
+HB_RF_NAN_LEFT = 1 << 30   # flag of an internal node's feature word: NaN inputs go left (sklearn's missing_go_to_left)
 
 
 class HeboB200Error(RuntimeError):

@@ -13,7 +13,9 @@
 //
 // Predict.  One thread per (candidate, output) walks the trees in index order, twice: the first walk sums the leaf values
 // sequentially (sklearn's forest mean) and pairwise (numpy's mean inside np.var), the second sums the squared deviations
-// pairwise.  Thresholds are compared in fp32 as RD32(t), which takes exactly the decisions of the fp64 comparison.
+// pairwise.  Thresholds are compared in fp32 as RD32(t), which takes exactly the decisions of the fp64 comparison.  A NaN
+// input goes to the child sklearn sends it to: for a tree trained without NaN, the one with more distinct training rows
+// (tree_.missing_go_to_left = n_left > n_right), the RF_NAN_LEFT bit of the node's feature word.
 #include <float.h>
 
 #include <algorithm>
@@ -30,6 +32,8 @@ constexpr int RF_SORT_THREADS = 1024;
 constexpr int RF_PRED_THREADS = 128;
 constexpr uint32_t RF_PHILOX_TAG = 0x52460000u;   // word 3 of the bootstrap counter ("RF")
 constexpr double RF_FEATURE_THRESHOLD = 1e-7;     // sklearn _splitter.pyx FEATURE_THRESHOLD
+constexpr int RF_NAN_LEFT = HB_RF_NAN_LEFT;       // bit of an internal node's feature word: NaN inputs go left
+constexpr int RF_FEATURE_MASK = RF_NAN_LEFT - 1;
 
 // ------------------------------------------------------------------------------------------------ forest layout
 // [header int32 x 8][uniq int32 [ne] | oh int32 [woh]][ncount int32 [B T]][nodes int4 [B T cap]][thr64 [B T cap]]
@@ -93,8 +97,8 @@ __device__ __forceinline__ double rf_tree_value(const int4 *nodes, const float *
                                                 const int32_t *oh, int64_t i) {
   int4 nd = nodes[0];
   while (nd.x >= 0) {
-    const float x = rf_x(Xc, Xe, dc, ne, oh, i, nd.x);
-    nd = nodes[x <= __int_as_float(nd.y) ? nd.z : nd.w];
+    const float x = rf_x(Xc, Xe, dc, ne, oh, i, nd.x & RF_FEATURE_MASK);
+    nd = nodes[x <= __int_as_float(nd.y) || (isnan(x) && (nd.x & RF_NAN_LEFT)) ? nd.z : nd.w];
   }
   return __hiloint2double(nd.w, nd.z);
 }
@@ -499,7 +503,9 @@ __global__ void __launch_bounds__(RF_THREADS) rf_grow_kernel(const __grid_consta
           const int l = nx, r = nx + 1;
           nx += 2;
           const double th = s.bthr[o];
-          F.nodes[nb0 + k] = make_int4(s.bfeat[o], __float_as_int(__double2float_rd(th)), l, r);
+          const bool nan_left = s.bcnt[o] > s.ncnt[k] - s.bcnt[o];
+          const int word = s.bfeat[o] | (nan_left ? RF_NAN_LEFT : 0);
+          F.nodes[nb0 + k] = make_int4(word, __float_as_int(__double2float_rd(th)), l, r);
           F.thr64[nb0 + k] = th;
           F.val64[nb0 + k] = S / W;
           const double WL = s.bWL[o], SL = s.bSL[o], QL = s.bQL[o];
@@ -521,7 +527,7 @@ __global__ void __launch_bounds__(RF_THREADS) rf_grow_kernel(const __grid_consta
         const int k = s.nid[i];
         if (k < lo || k >= hi || s.oidx[k] < 0) continue;
         const int4 nd = F.nodes[nb0 + k];
-        const float x = rf_x(a.Xc, a.Xe, dc, ne, F.oh, i, nd.x);
+        const float x = rf_x(a.Xc, a.Xe, dc, ne, F.oh, i, nd.x & RF_FEATURE_MASK);
         s.nid[i] = x <= __int_as_float(nd.y) ? nd.z : nd.w;
       }
       __syncthreads();

@@ -10,6 +10,11 @@ uses.  Where sklearn breaks ties at random, the device takes the highest proxy, 
 cut; this changes no in-bag partition, only where out-of-bag inputs fall.  ``predict`` reproduces the reference's fp32
 outputs bit for bit for the same trees (sklearn's sequential tree sum for the mean, numpy's pairwise sums for np.var).
 
+Candidates: a NaN is scored as sklearn scores it, going at each node to the child with more distinct training rows
+(``tree_.missing_go_to_left``).  Host candidates with +-inf raise ``ValueError``, as sklearn's input validation does.
+Device candidates are not read back (the GA scorers keep them on the device) and are not checked: there +inf goes right
+and -inf goes left at every node, the decisions of the threshold comparison.
+
 Deliberate deviation: the reference is unseeded (``RandomForestRegressor`` without ``random_state``).  This port draws its
 bootstrap key from torch's global generator, so a fit is reproducible under ``torch.manual_seed``.
 
@@ -92,8 +97,9 @@ class RF(BaseModel):
         self.est_noise = noise.cpu()
 
     def load_trees(self, trees, noise: float = 0.0):
-        """Take a fitted forest from sklearn-layout trees (``tree_.children_left / children_right / feature / threshold``
-        and ``value`` of each tree, as dicts of arrays), for scoring trees grown elsewhere."""
+        """Take a fitted forest from sklearn-layout trees (``tree_.children_left / children_right / feature / threshold``,
+        ``value`` and optionally ``missing_go_to_left`` of each tree, as dicts of arrays; without it NaN goes right), for
+        scoring trees grown elsewhere."""
         T = len(trees)
         assert T == self.n_estimators, "one tree per estimator"
         cap = max(int(np.asarray(t["feature"]).size) for t in trees)
@@ -102,11 +108,13 @@ class RF(BaseModel):
         def stack(key, dt, fill):
             a = np.full((T, cap), fill, dtype=dt)
             for i, t in enumerate(trees):
-                v = np.asarray(t[key]).reshape(-1)
+                v = np.asarray(t.get(key, fill)).reshape(-1)
                 a[i, :v.size] = v
             return torch.from_numpy(a).to(dev).contiguous()
         L, R, Fe = stack("left", np.int32, -1), stack("right", np.int32, -1), stack("feature", np.int32, -2)
         Th, V = stack("threshold", np.float64, -2.0), stack("value", np.float64, 0.0)
+        nan_left = (stack("missing_go_to_left", np.int32, 0) != 0) & (L >= 0)
+        Fe = torch.where(nan_left, Fe | _lib.HB_RF_NAN_LEFT, Fe)          # hb_rf_load reads the flag from the feature
         cnt = torch.tensor([int(np.asarray(t["feature"]).size) for t in trees], dtype=torch.int32, device=dev)
         lib = _lib.lib()
         forest = torch.empty(int(lib.hb_rf_forest_bytes(C.byref(self._spec), cap, 1, T)), dtype=torch.uint8, device=dev)
@@ -131,7 +139,12 @@ class RF(BaseModel):
             if not Xe.is_cuda:          # device categories are not read back; the kernel turns an out-of-range one into NaN
                 _check_categories(Xe, self.num_uniqs)
             xe = Xe.to(dev, torch.int32).contiguous()
-        xs = torch.as_tensor(Xc).detach().to(dev, torch.float32).contiguous() if self.num_cont > 0 else None
+        xs = None
+        if self.num_cont > 0:
+            Xc = torch.as_tensor(Xc).detach()
+            if not Xc.is_cuda and torch.isinf(Xc).any():          # sklearn's check_array(..., allow-nan)
+                raise ValueError("RF: input contains infinity")
+            xs = Xc.to(dev, torch.float32).contiguous()
         return xs, xe, m
 
     def _predict_dev(self, xs, xe, n_samples: int = 0, seed: int = 0, counter: int = 0):
@@ -194,8 +207,8 @@ class RF(BaseModel):
 
 def forest_trees(f: torch.Tensor) -> list:
     """The trees of a device forest (include/hebo_b200.h) as sklearn-layout dicts: feature (-2 at a leaf), threshold (-2 at
-    a leaf), left / right (-1 at a leaf), value, and thr32 (the fp32 threshold the traversal compares), tree b T + t at
-    index b T + t."""
+    a leaf), left / right (-1 at a leaf), value, missing_go_to_left (0 / 1), and thr32 (the fp32 threshold the traversal
+    compares), tree b T + t at index b T + t."""
     h = f[:32].cpu().view(torch.int32).numpy()
     cap, B, T, woh, ne = (int(v) for v in h[:5])
     align = lambda b: (b + 255) // 256 * 256
@@ -213,6 +226,9 @@ def forest_trees(f: torch.Tensor) -> list:
         k = int(cnt[t])
         nd = nodes[t, :k]
         leaf = nd[:, 0] < 0
-        out.append(dict(feature=nd[:, 0].copy(), threshold=thr[t, :k].copy(), left=np.where(leaf, -1, nd[:, 2]),
-                        right=np.where(leaf, -1, nd[:, 3]), value=val[t, :k].copy(), thr32=nd[:, 1].view(np.float32).copy()))
+        feature = np.where(leaf, nd[:, 0], nd[:, 0] & (_lib.HB_RF_NAN_LEFT - 1)).astype(np.int32)
+        out.append(dict(feature=feature, threshold=thr[t, :k].copy(), left=np.where(leaf, -1, nd[:, 2]),
+                        right=np.where(leaf, -1, nd[:, 3]), value=val[t, :k].copy(),
+                        missing_go_to_left=np.where(leaf, 0, (nd[:, 0] & _lib.HB_RF_NAN_LEFT) != 0).astype(np.int32),
+                        thr32=nd[:, 1].view(np.float32).copy()))
     return out

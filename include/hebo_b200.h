@@ -609,16 +609,21 @@ int32_t hb_de_predict_batch(const float *Xs, const int32_t *Xe, int64_t m, const
 #define HB_RF_MAX_ROWS   8192     /* training rows n                                                                 */
 #define HB_RF_MAX_WIDTH  4096     /* num_cont + sum(num_uniqs) (= HB_MAX_FEATURES)                                  */
 #define HB_RF_MAX_TREES  1024     /* trees per output T (conf['n_estimators'])                                       */
+#define HB_RF_NAN_LEFT   (1 << 30) /* flag of an internal node's feature word: NaN inputs go left (missing_go_to_left)    */
 /* and 1 <= B <= HB_MAX_OUTPUTS outputs per fit.
  *
  * Forest (device bytes, hb_rf_forest_bytes): a 256-byte header {cap, B, T, woh, num_enum, 0, 0, 0} (int32; cap = node
  * capacity per tree), then, each block 256-byte aligned: the decode tables int32 [num_enum] (categories per column) and
  * [woh] ((c << 12) | u of one-hot column j); node counts int32 [B, T]; nodes int4 [B, T, cap]; thresholds double
  * [B, T, cap]; node values double [B, T, cap].  Tree (b, t) is entry b T + t.  A node replaces one entry of sklearn's
- * tree_ arrays (_tree.pyx): internal {feature, RD32(threshold) as fp32 bits, left, right}, leaf {-2, 0, value as the low and
- * high words of its double}; the thresholds hold sklearn's fp64 threshold (-2 for a leaf) and the values
+ * tree_ arrays (_tree.pyx): internal {feature | HB_RF_NAN_LEFT if missing_go_to_left, RD32(threshold) as fp32 bits, left,
+ * right}, leaf
+ * {-2, 0, value as the low and high words of its double}; the thresholds hold sklearn's fp64 threshold (-2 for a leaf) and the values
  * tree_.value = sum(w y) / sum(w) of every node.  For fp32 x, x <= t exactly when x <= RD32(t) (t rounded toward -inf), so
- * the fp32 traversal takes the fp64 decision of DecisionTreeRegressor.predict.  A fitted tree is numbered breadth first:
+ * the fp32 traversal takes the fp64 decision of DecisionTreeRegressor.predict.  A NaN input goes left exactly where
+ * missing_go_to_left is set; sklearn sets it, for trees trained without NaN, where the split leaves more distinct in-bag
+ * rows left than right, and a fit here sets it so.  +inf goes right and -inf left, as any comparison takes them.  A
+ * fitted tree is numbered breadth first:
  * the split nodes of a level, in index order, append their left then right child. */
 typedef struct {                  /* HOST struct */
   int32_t        num_cont;        /* numeric columns                                                   */
@@ -662,8 +667,9 @@ int32_t hb_rf_predict(const float *Xc, const int32_t *Xe, int64_t m, const hb_rf
                       int64_t B, int64_t T, const float *noise, float *mean, float *var, int64_t n_samples, uint64_t seed,
                       uint64_t counter, float *samples, void *stream);
 /* A one-output forest (B = 1) of T trees from device arrays [T, max_nodes] in sklearn's tree_ layout: children_left,
- * children_right (-1 at a leaf), feature, threshold (fp64), value (fp64); node_counts [T] device int32.  For scoring a
- * forest grown elsewhere.  Synchronises the stream once (header copy). */
+ * children_right (-1 at a leaf), feature, threshold (fp64), value (fp64); node_counts [T] device int32.  An internal
+ * node's feature may carry HB_RF_NAN_LEFT (sklearn's tree_.missing_go_to_left): NaN inputs go left there, right at every
+ * node without it.  For scoring a forest grown elsewhere.  Synchronises the stream once (header copy). */
 int32_t hb_rf_load(const int32_t *left, const int32_t *right, const int32_t *feature, const double *threshold,
                    const double *value, const int32_t *node_counts, const hb_rf_spec_t *spec, int64_t T,
                    int64_t max_nodes, void *forest, void *stream);

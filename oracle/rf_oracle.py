@@ -6,9 +6,14 @@ equal it bit for bit; and it restates the reference's predict arithmetic (sklear
 sums inside np.var / np.mean), which must equal numpy bit for bit.
 
 A forest here is a list of trees; a tree is a dict of numpy arrays over its nodes: feature (int32, -2 at a leaf),
-threshold (fp64, -2 at a leaf), left / right (int32, -1 at a leaf) and value (fp64, S / W of every node).
+threshold (fp64, -2 at a leaf), left / right (int32, -1 at a leaf), value (fp64, S / W of every node) and, optionally,
+missing_go_to_left (int32, 1 where a NaN input goes left; sklearn sets it, for trees trained without NaN, where the split
+leaves more distinct in-bag rows left than right).
 """
 from __future__ import annotations
+
+import os
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
@@ -93,11 +98,12 @@ def grow_tree(X: np.ndarray, y: np.ndarray, w: np.ndarray) -> dict:
     w = np.asarray(w, dtype=np.int64)
     w64 = w.astype(np.float64)
     order = [np.argsort(X[:, f], kind="stable") for f in range(width)]
-    feat, thr, left, right, val = [], [], [], [], []
+    feat, thr, left, right, val, nanl = [], [], [], [], [], []
     Wn, Sn, Qn, Cn = [], [], [], []
 
     def add_node(W, S, Q, C):
-        for lst, v in ((feat, -2), (thr, -2.0), (left, -1), (right, -1), (val, 0.0), (Wn, W), (Sn, S), (Qn, Q), (Cn, C)):
+        for lst, v in ((feat, -2), (thr, -2.0), (left, -1), (right, -1), (val, 0.0), (nanl, 0), (Wn, W), (Sn, S), (Qn, Q),
+                       (Cn, C)):
             lst.append(v)
         return len(feat) - 1
 
@@ -155,7 +161,7 @@ def grow_tree(X: np.ndarray, y: np.ndarray, w: np.ndarray) -> dict:
             r = add_node(W - WL, S - SL, Q - QL, C - cl)
             assert (l, r) == (nx, nx + 1)
             nx += 2
-            feat[k], thr[k], left[k], right[k] = f, th, l, r
+            feat[k], thr[k], left[k], right[k], nanl[k] = f, th, l, r, int(cl > C - cl)
             sel = inbag & (nid == k)
             goes_left = X[:, f].astype(np.float64) <= th
             nid[sel & goes_left] = l
@@ -163,13 +169,175 @@ def grow_tree(X: np.ndarray, y: np.ndarray, w: np.ndarray) -> dict:
         lo, hi = hi, nx
     return dict(feature=np.array(feat, dtype=np.int32), threshold=np.array(thr, dtype=np.float64),
                 left=np.array(left, dtype=np.int32), right=np.array(right, dtype=np.int32),
-                value=np.array(val, dtype=np.float64))
+                value=np.array(val, dtype=np.float64), missing_go_to_left=np.array(nanl, dtype=np.int32))
+
+
+def grow_tree_level(X: np.ndarray, y: np.ndarray, w: np.ndarray, chunk_elems: int = 1 << 21) -> dict:
+    """grow_tree, level-synchronous and vectorised over features and nodes: the same tree, node numbering and bits.
+
+    Every in-bag row of the level's open nodes sits in G [width, nl]: row f is feature f's presorted order filtered to
+    those rows and grouped by node, the nodes' segments in node order at the same offsets for every feature.  A split
+    partitions each segment stably into its children's, so a segment stays the presorted order of its node's rows.
+    The split search pads the segments of a chunk of features into [features, nodes, L] blocks, one per power-of-two
+    length class L, and scans them with np.cumsum(axis=-1), which adds sequentially along each segment as grow_tree does
+    (trailing zero padding cannot change an earlier prefix).  Cut rule, proxy and tie rule are grow_tree's."""
+    X = np.asarray(X, dtype=np.float32) + np.float32(0.0)
+    n, width = X.shape
+    y64 = np.asarray(y, dtype=np.float32).astype(np.float64)
+    w = np.asarray(w, dtype=np.int64)
+    w64 = w.astype(np.float64)
+    inbag = w > 0
+    wy = w64 * np.where(inbag, y64, 0.0)
+    sq = wy * np.where(inbag, y64, 0.0)
+    Xt = np.ascontiguousarray(X.T)
+    feat, thr, left, right, val, nanl = [], [], [], [], [], []
+    Wn, Sn, Qn, Cn = [], [], [], []
+
+    def add_node(W, S, Q, C):
+        for lst, v in ((feat, -2), (thr, -2.0), (left, -1), (right, -1), (val, 0.0), (nanl, 0), (Wn, W), (Sn, S), (Qn, Q),
+                       (Cn, C)):
+            lst.append(v)
+        return len(feat) - 1
+
+    rows = np.nonzero(inbag)[0]
+    add_node(sequential_sum(w64[rows]), sequential_sum(wy[rows]), sequential_sum(sq[rows]), int(rows.size))
+    # root level: every feature's stable presort filtered to the in-bag rows; V [width, nl] holds G's values
+    order = np.argsort(Xt, axis=1, kind="stable").astype(np.int32)
+    G = order[inbag[order]].reshape(width, rows.size)
+    del order
+    V = np.take_along_axis(Xt, G, axis=1)
+    seg_nodes, seg_off = [0], [0]          # the level's nodes in order, and their column offsets in G
+    pool = ThreadPoolExecutor(os.cpu_count() or 1)          # numpy releases the GIL inside these array operations
+    lo, hi = 0, 1
+    while lo < hi:
+        open_nodes = []
+        for k in range(lo, hi):
+            W, S, Q = Wn[k], Sn[k], Qn[k]
+            mean = S / W if W != 0 else np.nan
+            imp = Q / W - mean * mean if W != 0 else np.nan
+            val[k] = mean
+            if Cn[k] < 2 or imp <= EPS:
+                continue
+            open_nodes.append(k)
+        if not open_nodes:
+            break
+        # keep only the open nodes' segments
+        off = dict(zip(seg_nodes, seg_off))
+        keep = np.concatenate([np.arange(off[k], off[k] + Cn[k]) for k in open_nodes])
+        G, V = np.ascontiguousarray(G[:, keep]), np.ascontiguousarray(V[:, keep])
+        no = len(open_nodes)
+        cnt = np.array([Cn[k] for k in open_nodes], dtype=np.int64)
+        segoff = np.concatenate([[0], np.cumsum(cnt)[:-1]])
+        Wv = np.array([Wn[k] for k in open_nodes], dtype=np.float64)
+        Sv = np.array([Sn[k] for k in open_nodes], dtype=np.float64)
+        nl = G.shape[1]
+        # length classes: open nodes whose count rounds up to the same power of two
+        L2 = 1 << np.ceil(np.log2(cnt)).astype(np.int64)
+        classes = []
+        for Lc in np.unique(L2):
+            ks = np.nonzero(L2 == Lc)[0]
+            j = np.arange(Lc)
+            valid = j[None, :] < cnt[ks, None]
+            idx = np.where(valid, segoff[ks, None] + j[None, :], 0)
+            classes.append((ks, idx, valid, valid[:, 1:] & valid[:, :-1], Sv[ks][None, :, None], Wv[ks][None, :, None]))
+
+        def search(f0, f1):
+            """per (feature, node) of features f0 .. f1 - 1: the proxy at the first arg-max over the cuts, and that cut"""
+            cp = np.full((f1 - f0, no), -np.inf)
+            cj = np.zeros((f1 - f0, no), dtype=np.int64)
+            with np.errstate(divide="ignore", invalid="ignore"):
+                for ks, idx, valid, cut, S, W in classes:
+                    r = G[f0:f1, idx]                                  # [features, nodes, Lc] rows
+                    v = V[f0:f1, idx].astype(np.float64)
+                    cw = np.cumsum(np.where(valid, w64[r], 0.0), axis=-1)
+                    cs = np.cumsum(np.where(valid, wy[r], 0.0), axis=-1)
+                    ok = cut & (v[..., 1:] > v[..., :-1] + FEATURE_THRESHOLD)
+                    WL, SL = cw[..., :-1], cs[..., :-1]
+                    SR = S - SL
+                    proxy = np.where(ok, SL * SL / WL + SR * SR / (W - WL), -np.inf)
+                    a = np.argmax(proxy, axis=-1)
+                    cp[:, ks] = np.take_along_axis(proxy, a[..., None], axis=-1)[..., 0]
+                    cj[:, ks] = a + 1
+            return cp, cj
+
+        fc = max(1, chunk_elems // (2 * nl))
+        bp = np.full(no, -np.inf)
+        bf = np.full(no, -1, dtype=np.int64)
+        bj = np.zeros(no, dtype=np.int64)
+        chunks = [(f0, min(width, f0 + fc)) for f0 in range(0, width, fc)]
+        for (f0, _), (cp, cj) in zip(chunks, pool.map(lambda c: search(*c), chunks)):
+            # ascending features, replace only on a strictly greater proxy (NaN never replaces)
+            for i in range(cp.shape[0]):
+                better = cp[i] > bp
+                bp = np.where(better, cp[i], bp)
+                bf = np.where(better, f0 + i, bf)
+                bj = np.where(better, cj[i], bj)
+        # children in breadth-first order, and each in-bag row's side
+        nx = hi
+        side = np.zeros(n, dtype=bool)
+        child = np.full(no, -1, dtype=np.int64)
+        for o, k in enumerate(open_nodes):
+            if bf[o] < 0:
+                continue
+            f, jj = int(bf[o]), int(bj[o])
+            seg = G[f, segoff[o]:segoff[o] + cnt[o]]
+            v = X[seg, f].astype(np.float64)
+            cw, cs, cq = np.cumsum(w64[seg]), np.cumsum(wy[seg]), np.cumsum(sq[seg])
+            th = v[jj - 1] / 2.0 + v[jj] / 2.0
+            if th == v[jj] or np.isinf(th):
+                th = v[jj - 1]
+            th, WL, SL, QL = float(th), float(cw[jj - 1]), float(cs[jj - 1]), float(cq[jj - 1])
+            W, S, Q, C = Wn[k], Sn[k], Qn[k], Cn[k]
+            l = add_node(WL, SL, QL, jj)
+            r = add_node(W - WL, S - SL, Q - QL, C - jj)
+            assert (l, r) == (nx, nx + 1)
+            nx += 2
+            feat[k], thr[k], left[k], right[k], nanl[k] = f, th, l, r, int(jj > C - jj)
+            child[o] = l
+            side[seg] = X[seg, f].astype(np.float64) <= th
+        if nx == hi:
+            break
+        # stable partition of every split node's segment into its children's, for every feature
+        nodeof = np.repeat(np.arange(no), cnt)
+        split = child[nodeof] >= 0
+        G, V = G[:, split], V[:, split]
+        nodeof = nodeof[split]
+        so = np.zeros(no, dtype=np.int64)                                       # split nodes' offsets in the new G
+        so[child >= 0] = np.concatenate([[0], np.cumsum(cnt[child >= 0])[:-1]])
+        lcnt = np.zeros(no, dtype=np.int64)
+        for o in np.nonzero(child >= 0)[0]:
+            lcnt[o] = Cn[int(child[o])]
+        start = so[nodeof]                                                       # segment start of each column
+        before = np.arange(G.shape[1]) - start
+        rstart = start + lcnt[nodeof]
+        Gn, Vn = np.empty_like(G), np.empty_like(V)
+
+        def partition(f0, f1):
+            sl = side[G[f0:f1]]
+            cl = np.cumsum(sl, axis=1, dtype=np.int64) - sl                     # left entries before, whole row
+            cl -= np.take_along_axis(cl, np.broadcast_to(start, cl.shape), axis=1)
+            dest = np.where(sl, start + cl, rstart + (before - cl))
+            np.put_along_axis(Gn[f0:f1], dest, G[f0:f1], axis=1)
+            np.put_along_axis(Vn[f0:f1], dest, V[f0:f1], axis=1)
+
+        fp = max(1, chunk_elems // G.shape[1])
+        list(pool.map(lambda c: partition(*c), [(f0, min(width, f0 + fp)) for f0 in range(0, width, fp)]))
+        G, V = Gn, Vn
+        seg_nodes = [int(child[o]) + s for o in np.nonzero(child >= 0)[0] for s in (0, 1)]
+        seg_off = [int(so[o]) + s * int(lcnt[o]) for o in np.nonzero(child >= 0)[0] for s in (0, 1)]
+        lo, hi = hi, nx
+    pool.shutdown()
+    return dict(feature=np.array(feat, dtype=np.int32), threshold=np.array(thr, dtype=np.float64),
+                left=np.array(left, dtype=np.int32), right=np.array(right, dtype=np.int32),
+                value=np.array(val, dtype=np.float64), missing_go_to_left=np.array(nanl, dtype=np.int32))
 
 
 def apply(tree: dict, X: np.ndarray) -> np.ndarray:
-    """Leaf index of every row of float32 X (DecisionTreeRegressor.apply: x <= threshold goes left, compared in fp64)."""
+    """Leaf index of every row of float32 X (DecisionTreeRegressor.apply: x <= threshold goes left, compared in fp64; NaN
+    goes left where missing_go_to_left is set, right elsewhere)."""
     X = np.asarray(X, dtype=np.float32)
     node = np.zeros(X.shape[0], dtype=np.int64)
+    nanl = np.asarray(tree.get("missing_go_to_left", np.zeros(tree["feature"].size, np.int32))) != 0
     while True:
         f = tree["feature"][node]
         inner = f >= 0
@@ -177,7 +345,8 @@ def apply(tree: dict, X: np.ndarray) -> np.ndarray:
             return node
         idx = np.nonzero(inner)[0]
         x = X[idx, f[idx]].astype(np.float64)
-        node[idx] = np.where(x <= tree["threshold"][node[idx]], tree["left"][node[idx]], tree["right"][node[idx]])
+        k = node[idx]
+        node[idx] = np.where((x <= tree["threshold"][k]) | (np.isnan(x) & nanl[k]), tree["left"][k], tree["right"][k])
 
 
 def tree_predict(tree: dict, X) -> np.ndarray:
@@ -185,11 +354,12 @@ def tree_predict(tree: dict, X) -> np.ndarray:
 
 
 # ---------------------------------------------------------------------------------------------------------------- forest
-def fit(X, y, counts):
-    """(trees, est_noise) of one output: X float32 [n, width], y float32 [n] (non-finite rows weigh 0), counts [T, n]."""
+def fit(X, y, counts, grow=grow_tree):
+    """(trees, est_noise) of one output: X float32 [n, width], y float32 [n] (non-finite rows weigh 0), counts [T, n].
+    grow: grow_tree, or grow_tree_level for large inputs (the same trees)."""
     y = np.asarray(y, dtype=np.float32)
     keep = np.isfinite(y)
-    trees = [grow_tree(X, np.where(keep, y, 0.0).astype(np.float32), np.where(keep, np.maximum(c, 0), 0))
+    trees = [grow(X, np.where(keep, y, 0.0).astype(np.float32), np.where(keep, np.maximum(c, 0), 0))
              for c in np.asarray(counts)]
     return trees, noise(trees, X[keep], y[keep])
 
@@ -219,3 +389,14 @@ def predict(trees, X, noise_b) -> tuple:
         d = P[i] - mu
         var[i] = np.float32(pairwise_sum(d * d) / T)
     return mean, var + np.float32(noise_b)
+
+
+def predict_fast(trees, X, noise_b) -> tuple:
+    """predict, vectorised over candidates with the reference's own expressions: P [m, T] of leaf values, the mean as
+    forest_mean64's sequential tree sum, the variance as np.var(P, axis=1) (rf.py:55), then fp32 and + noise in fp32."""
+    P = np.stack([tree_predict(t, X) for t in trees], axis=1)          # C-contiguous [m, T], as np.concatenate(axis=1)
+    s = np.zeros(P.shape[0], dtype=np.float64)
+    for t in range(P.shape[1]):
+        s = s + P[:, t]
+    mean = (s / P.shape[1]).astype(np.float32)
+    return mean, np.var(P, axis=1).astype(np.float32) + np.float32(noise_b)

@@ -9,7 +9,8 @@ n_estimators in {1, 20, 100}; the HEBO/test/test_acq.py setup X ~ N(0, 1) [10, 1
   - the data (Xc, Xe, y) and held-out rows;
   - each tree's bootstrap counts over the training rows, recovered with sklearn's own _generate_sample_indices from the
     tree's random_state (checked against tree_.weighted_n_node_samples[0] == n_kept);
-  - each tree's arrays (children_left / right, feature, threshold, value) and tree.apply on the training rows;
+  - each tree's arrays (children_left / right, feature, threshold, value, missing_go_to_left) and tree.apply on the
+    training rows (ref_rf.npz was generated before missing_go_to_left was recorded; its held-out rows have no NaN);
   - RF.predict (mean, var) on the held-out rows, and RF.noise.
 The sklearn version is stored with them.  Test infrastructure; never imported by hebo_b200/.
 """
@@ -62,6 +63,37 @@ def load_rf():
     return ref_loader._load("_hebo_ref.models.rf.rf", "models/rf/rf.py")
 
 
+def record_forest(model, keep, Xtr):
+    """(counts [T, n], tree arrays [T, cap], apply [T, n], node counts [T]) of a fitted reference RF: each tree's
+    bootstrap counts over the n training rows (keep: the rows filter_nan kept), recovered with sklearn's own
+    _generate_sample_indices from the tree's random_state and checked against tree_.weighted_n_node_samples[0]."""
+    from sklearn.ensemble._forest import _generate_sample_indices
+    kept = np.nonzero(keep)[0]
+    n, T = keep.size, len(model.rf.estimators_)
+    cap = max(e.tree_.node_count for e in model.rf.estimators_)
+    counts = np.zeros((T, n), dtype=np.int32)
+    arrs = {k: np.zeros((T, cap), dtype=dt) for k, dt in
+            (("left", np.int32), ("right", np.int32), ("feature", np.int32), ("threshold", np.float64), ("value", np.float64),
+             ("missing_go_to_left", np.int32))}
+    apply = np.zeros((T, n), dtype=np.int32)
+    ncount = np.zeros(T, dtype=np.int32)
+    for t, est in enumerate(model.rf.estimators_):
+        idx = _generate_sample_indices(est.random_state, kept.size, kept.size, None)
+        c = np.bincount(idx, minlength=kept.size)
+        assert est.tree_.weighted_n_node_samples[0] == kept.size
+        counts[t, kept] = c
+        k = est.tree_.node_count
+        ncount[t] = k
+        arrs["left"][t, :k] = est.tree_.children_left
+        arrs["right"][t, :k] = est.tree_.children_right
+        arrs["feature"][t, :k] = est.tree_.feature
+        arrs["threshold"][t, :k] = est.tree_.threshold
+        arrs["value"][t, :k] = est.tree_.value.reshape(-1)
+        arrs["missing_go_to_left"][t, :k] = est.tree_.missing_go_to_left
+        apply[t] = est.apply(Xtr.astype(np.float32))
+    return counts, arrs, apply, ncount
+
+
 def data(kind, n, dc, uniqs, seed):
     g = torch.Generator().manual_seed(seed)
     if kind == "acq":
@@ -80,7 +112,6 @@ def data(kind, n, dc, uniqs, seed):
 
 def main():
     import sklearn
-    from sklearn.ensemble._forest import _generate_sample_indices
     rf_mod = load_rf()
     out = {"sklearn_version": np.array(sklearn.__version__), "variants": np.array(list(VARIANTS))}
     for vi, (name, (kind, n, dc, uniqs, T)) in enumerate(VARIANTS.items()):
@@ -96,27 +127,8 @@ def main():
         model.fit(Xc_tr if dc > 0 else torch.zeros(n, 0), Xe_tr, y[tr])
         mean, var = model.predict(Xc[te] if dc > 0 else torch.zeros(M_TEST, 0), Xe[te] if uniqs else None)
         keep = torch.isfinite(y[tr]).all(1).numpy()
-        kept = np.nonzero(keep)[0]
         Xtr = model.xtrans(Xc_tr if dc > 0 else torch.zeros(n, 0), Xe_tr)
-        cap = max(e.tree_.node_count for e in model.rf.estimators_)
-        counts = np.zeros((T, n), dtype=np.int32)
-        arrs = {k: np.zeros((T, cap), dtype=dt) for k, dt in
-                (("left", np.int32), ("right", np.int32), ("feature", np.int32), ("threshold", np.float64), ("value", np.float64))}
-        apply = np.zeros((T, n), dtype=np.int32)
-        ncount = np.zeros(T, dtype=np.int32)
-        for t, est in enumerate(model.rf.estimators_):
-            idx = _generate_sample_indices(est.random_state, kept.size, kept.size, None)
-            c = np.bincount(idx, minlength=kept.size)
-            assert est.tree_.weighted_n_node_samples[0] == kept.size
-            counts[t, kept] = c
-            k = est.tree_.node_count
-            ncount[t] = k
-            arrs["left"][t, :k] = est.tree_.children_left
-            arrs["right"][t, :k] = est.tree_.children_right
-            arrs["feature"][t, :k] = est.tree_.feature
-            arrs["threshold"][t, :k] = est.tree_.threshold
-            arrs["value"][t, :k] = est.tree_.value.reshape(-1)
-            apply[t] = est.apply(Xtr.astype(np.float32))
+        counts, arrs, apply, ncount = record_forest(model, keep, Xtr)
         p = name + "/"
         out.update({p + "Xc": (Xc[tr] if dc > 0 else torch.zeros(n, 0)).numpy(), p + "y": y[tr].numpy(),
                     p + "Xc_test": (Xc[te] if dc > 0 else torch.zeros(M_TEST, 0)).numpy(),

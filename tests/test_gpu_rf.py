@@ -46,7 +46,7 @@ def rd32(th):
 def assert_same_forest(dev_trees, ref_trees):
     assert len(dev_trees) == len(ref_trees)
     for t, (a, b) in enumerate(zip(dev_trees, ref_trees)):
-        for k in ("feature", "left", "right"):
+        for k in ("feature", "left", "right", "missing_go_to_left"):
             assert np.array_equal(a[k], b[k]), (t, k)
         for k in ("threshold", "value"):
             assert a[k].tobytes() == b[k].tobytes(), (t, k)

@@ -48,6 +48,11 @@ def test_input_checks_before_any_launch():
         m.fit(torch.tensor([[0.0], [float("inf")]]), torch.zeros(2, 1).long(), torch.zeros(2, 1))
     with pytest.raises(IndexError):
         m.predict(torch.zeros(2, 1), torch.tensor([[0], [5]]))
+    for v in (float("inf"), float("-inf")):                  # sklearn refuses infinite candidates
+        with pytest.raises(ValueError):
+            m.predict(torch.tensor([[0.0], [v]]), torch.zeros(2, 1).long())
+        with pytest.raises(ValueError):
+            m.sample_y(torch.tensor([[v]]), torch.zeros(1, 1).long())
 
 
 def test_abi_rejects_outside_the_envelope():
