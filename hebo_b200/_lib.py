@@ -148,6 +148,8 @@ SIGNATURES = {
     "hb_rf_fit": (_i32, [_vp, _vp, _vp, _i64, _rsp, _i64, _i64, _vp, _u64, _vp, _vp, _vp, _i64, _vp]),
     "hb_rf_predict": (_i32, [_vp, _vp, _i64, _rsp, _vp, _i64, _i64, _vp, _vp, _vp, _i64, _u64, _u64, _vp, _vp]),
     "hb_rf_load": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _rsp, _i64, _i64, _vp, _vp]),
+    "hb_ehvi_workspace_bytes": (_i64, [_i64, _i64, _i64, _i64]),
+    "hb_ehvi": (_i32, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _i64, _vp]),
 }
 
 _lib = None

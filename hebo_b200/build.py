@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libhebo_b200.so")
-SOURCES = ["api.cu", "linalg.cu", "pairwise.cu", "posterior.cu", "pareto.cu", "cholesky.cu", "init.cu", "tcgemm.cu", "fit_tc.cu", "vnorm_h16.cu", "posterior_grad.cu", "nsga.cu", "embed.cu", "ensemble.cu", "forest.cu"]
+SOURCES = ["api.cu", "linalg.cu", "pairwise.cu", "posterior.cu", "pareto.cu", "cholesky.cu", "init.cu", "tcgemm.cu", "fit_tc.cu", "vnorm_h16.cu", "posterior_grad.cu", "nsga.cu", "embed.cu", "ensemble.cu", "forest.cu", "hypervolume.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr",

@@ -1093,4 +1093,13 @@ int32_t hb_rf_load(const int32_t *left, const int32_t *right, const int32_t *fea
                         (cudaStream_t)stream);
 }
 
+// general.py:116-140: the Monte-Carlo EHVI of one selection round (hypervolume.cu)
+int64_t hb_ehvi_workspace_bytes(int64_t n, int64_t K, int64_t m, int64_t n_mc) { return ehvi_ws_query(n, K, m, n_mc); }
+
+int32_t hb_ehvi(const double *front, int64_t n, int64_t K, const double *samples, int64_t m, int64_t n_mc, const double *ref,
+                double *base_hv, double *ehvi, void *ws, int64_t ws_bytes, void *stream) {
+  if ((n > 0 && !front) || !samples || !ref || !base_hv || !ehvi || !ws) return HB_ERR_INVALID;
+  return launch_ehvi(front, n, K, samples, m, n_mc, ref, base_hv, ehvi, ws, ws_bytes, (cudaStream_t)stream);
+}
+
 }  // extern "C"

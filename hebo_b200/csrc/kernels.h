@@ -243,6 +243,10 @@ int launch_de_predict_batch(const float *Xs, const int32_t *Xe, int64_t m, const
                             const float *y_std, float *mu, float *var, int64_t n_samples, const float *xi, uint64_t seed,
                             uint64_t counter, float *y_samp, cudaStream_t st);
 
+// hypervolume.cu: GeneralBO's Monte-Carlo EHVI selection round, bit for bit with general.hypervolume
+int64_t ehvi_ws_query(int64_t n, int64_t K, int64_t m, int64_t n_mc);
+int launch_ehvi(const double *front, int64_t n, int64_t K, const double *samples, int64_t m, int64_t n_mc, const double *ref,
+                double *base_hv, double *ehvi, void *ws, int64_t ws_bytes, cudaStream_t st);
 // random-forest surrogate (forest.cu)
 int64_t rf_forest_bytes(const hb_rf_spec_t *spec, int64_t max_nodes, int64_t B, int64_t T);
 int64_t rf_fit_ws_query(int64_t n, const hb_rf_spec_t *spec, int64_t B, int64_t T);

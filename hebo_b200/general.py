@@ -7,9 +7,11 @@ launch), or with ``model_name='deep_ensemble'`` one multi-output ``hebo_b200.Dee
 violation as its constraint column), and picks the suggestions from the resulting (feasible) front: at random with the
 most uncertain row kept, or by a Monte-Carlo expected hypervolume improvement when ``ref_point`` is given.
 
-Hypervolumes are computed exactly on the host (``hypervolume``), in any number of objectives.  The reference uses pymoo's
-``HV`` there; the selection only reads ``argmax`` and ``> 0`` of the improvements, so any exact hypervolume gives its
-choice.
+Hypervolumes are exact, in any number of objectives (``hypervolume``).  The reference uses pymoo's ``HV`` there; the
+selection only reads ``argmax`` and ``> 0`` of the improvements, so any exact hypervolume gives its choice.  On a CUDA
+device each EHVI round is one ``hb_ehvi`` call (``expected_hvi``), which returns the host loop's improvements bit for bit;
+the greedy rounds, the random fall-back, de-duplication and top-up stay on the host, so numpy's generator is consumed as
+before.  Without CUDA the round runs the host loop over ``hypervolume``.
 """
 from __future__ import annotations
 
@@ -56,6 +58,35 @@ def _nondominated(Y: np.ndarray) -> np.ndarray:
     return Y[~(le & lt).any(0)]
 
 
+def expected_hvi(front, samples, ref_point, device="cuda"):
+    """One Monte-Carlo EHVI round on the device (hb_ehvi): ``(base_hv, ehvi)`` with base_hv = hypervolume(front, ref_point)
+    and ehvi[j] = sum_k (hypervolume(vstack([front, samples[k, j]]), ref_point) - base_hv) / n_mc, bit for bit with that
+    host expression.  front [n, K]; samples [n_mc, m, K] (ndarray or tensor, converted to fp64 exactly); ehvi is an fp64
+    ndarray of m values."""
+    from . import _lib
+    dev = torch.device(device)
+    ref = np.asarray(ref_point, dtype=np.float64).reshape(-1)
+    K = ref.size
+    front = np.ascontiguousarray(np.asarray(front, dtype=np.float64).reshape(-1, K))
+    S = torch.as_tensor(samples).to(device=dev, dtype=torch.float64).contiguous()
+    if S.dim() != 3 or S.shape[2] != K:
+        raise ValueError(f"expected_hvi: samples must be [n_mc, m, {K}], got {tuple(S.shape)}")
+    n, (n_mc, m) = front.shape[0], S.shape[:2]
+    lib = _lib.lib()
+    need = lib.hb_ehvi_workspace_bytes(n, K, m, n_mc)
+    if need < 0:
+        raise ValueError(f"expected_hvi: unsupported sizes (n={n}, K={K}, m={m}, n_mc={n_mc})")
+    ws = torch.empty(need, dtype=torch.uint8, device=dev)
+    F = torch.from_numpy(front).to(dev) if n > 0 else None
+    r = torch.from_numpy(ref).to(dev)
+    base = torch.zeros(1, dtype=torch.float64, device=dev)
+    out = torch.empty(m, dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.hb_ehvi(_lib.ptr(F), n, K, _lib.ptr(S), m, n_mc, _lib.ptr(r), _lib.ptr(base), _lib.ptr(out), _lib.ptr(ws),
+                               need, _lib.stream_ptr()), "hb_ehvi")
+    return float(base.item()), out.cpu().numpy()
+
+
 class GeneralBO:
     """general.py:23-204.  ``space``: a DesignSpace (or its list-of-dicts spec).  y has num_obj objective columns
     followed by num_constr constraint columns, all minimised; a row is feasible when every constraint is <= 0.
@@ -64,7 +95,8 @@ class GeneralBO:
     'deep_ensemble' for its outputs), 'deep_ensemble' (one ``hebo_b200.DeepEnsemble`` with num_obj + num_constr outputs)
     or 'gp' when num_obj + num_constr == 1; any other surrogate raises NotImplementedError, and 'gp' with several outputs
     fails the reference's multi-output assertion.  Over deep ensembles the GA scores every generation with one
-    hb_de_predict_batch launch, and the EHVI selection (``ref_point``) draws its samples on the device.
+    hb_de_predict_batch launch, and the EHVI selection (``ref_point``) draws its samples on the device.  On a CUDA device
+    every EHVI round is one ``expected_hvi`` call.
     ``evo_pop`` / ``evo_iters`` are read when ``suggest`` runs, so they may be changed after construction.  As in the
     reference, ``fix_input`` only applies to the random start-up design: the model stage does not pass it to the GA."""
 
@@ -168,17 +200,24 @@ class GeneralBO:
         assert self.num_constr == 0
         n_mc = 10
         ref = np.asarray(self.ref_point, dtype=np.float64).reshape(-1)
+        on_device = torch.device(self.device).type == "cuda" and torch.cuda.is_available()
         with torch.no_grad():
-            y_samp = torch.as_tensor(model.sample_y(*self.space.transform(suggest), n_mc)).cpu().numpy()
+            y_samp = torch.as_tensor(model.sample_y(*self.space.transform(suggest), n_mc))
+        if on_device:
+            y_samp_dev = y_samp.to(device=self.device, dtype=torch.float64)
+        y_samp = y_samp.cpu().numpy()
         y_curr = self.get_pf(self.y).copy()
         select_id = []
         for _ in range(n_suggestions):
-            base_hv = hypervolume(y_curr, ref)
-            ehvi = []
-            for j in range(suggest.shape[0]):
-                samp = y_samp[:, j]
-                hvi = sum(hypervolume(np.vstack([y_curr, samp[[k]]]), ref) - base_hv for k in range(n_mc))
-                ehvi.append(hvi / n_mc)
+            if on_device:
+                _, ehvi = expected_hvi(y_curr, y_samp_dev, ref, self.device)
+            else:
+                base_hv = hypervolume(y_curr, ref)
+                ehvi = []
+                for j in range(suggest.shape[0]):
+                    samp = y_samp[:, j]
+                    hvi = sum(hypervolume(np.vstack([y_curr, samp[[k]]]), ref) - base_hv for k in range(n_mc))
+                    ehvi.append(hvi / n_mc)
             best_id = int(np.argmax(ehvi)) if max(ehvi) > 0 else np.random.choice(suggest.shape[0])
             y_curr = np.vstack([y_curr, y_samp[:, best_id].min(axis=0, keepdims=True)])
             select_id.append(best_id)

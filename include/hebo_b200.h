@@ -674,6 +674,21 @@ int32_t hb_rf_load(const int32_t *left, const int32_t *right, const int32_t *fea
                    const double *value, const int32_t *node_counts, const hb_rf_spec_t *spec, int64_t T,
                    int64_t max_nodes, void *forest, void *stream);
 
+/* ---- Monte-Carlo expected hypervolume improvement  (GeneralBO's ref_point selection, optimizers/general.py:116-140) ----
+ * One selection round, bit for bit with the host's exact hypervolume (hebo_b200.general.hypervolume, minimisation):
+ *   base_hv  = hypervolume(front, ref)
+ *   ehvi[j]  = (sum_k (hypervolume(vstack([front, samples[k, j]]), ref) - base_hv)) / n_mc,  the sum from 0.0, k ascending
+ * front [n, K], samples [n_mc, m, K], ref [K], base_hv [1], ehvi [m]: fp64 on the device.  A hypervolume keeps the rows
+ * strictly below ref in every coordinate (NaN rows drop out), sorts them stably by the last coordinate (a sample after the
+ * front rows it ties), and adds, over the slices with hi > y in ascending order, hv(nondominated(prefix[:, :-1]),
+ * ref[:-1]) * (hi - y) with base case ref[0] - min; every operation is one rounded fp64 operation (no FMA), so +-inf
+ * samples take the host's IEEE path.  Cost is exponential in K, as on the host.  2 <= K <= HB_MAX_OBJ, 0 <= n < 2^31 - 2,
+ * m >= 0, n_mc >= 1; front may be NULL when n == 0.  m == 0 launches nothing and leaves base_hv unwritten.
+ * hb_ehvi_workspace_bytes: host only, < 0 on bad sizes; non-decreasing in every argument.  No host synchronisation. */
+int64_t hb_ehvi_workspace_bytes(int64_t n, int64_t K, int64_t m, int64_t n_mc);
+int32_t hb_ehvi(const double *front, int64_t n, int64_t K, const double *samples, int64_t m, int64_t n_mc, const double *ref,
+                double *base_hv, double *ehvi, void *ws, int64_t ws_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
