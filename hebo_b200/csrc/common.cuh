@@ -152,18 +152,18 @@ __device__ __forceinline__ void kern_eval_grad(float r2, float &k, float &h) {
 // torch layer KumarWarp, HEBO/hebo/models/nn/mono_layers/layers.py:85-117, and GPy's InputWarpedGP in gpy_wgp.py:120-128):
 //   u = clamp((x + 1) / 2, eps, 1 - eps),  w = 1 - (1 - u^a)^b,  result 2 w - 1;   a, b in (0.01, 10)
 // da / db (optional): partial derivatives of the RESULT w.r.t. the exponents.
+// 1 - u^a is formed as -expm1(a log u): at the upper clamp a log u is about -1e-6 a, where expf(a log u) rounds to 1 for
+// a <= 0.031 and 1 - u^a would cancel to 0 (w = 1 instead of, say, 0.99972 at a = 0.02, b = 0.5, and lom = -inf, which
+// makes db NaN).  With a >= WARP_LO and log u <= -1e-6, -expm1f stays >= 1e-8 and lom finite.
 constexpr float WARP_LO = 0.01f, WARP_HI = 10.0f;
 __device__ __forceinline__ float kumar_warp(float x, float a, float b, float *da = nullptr, float *db = nullptr) {
   const float eps = 1e-6f;
   const float u = fminf(fmaxf((x + 1.0f) * 0.5f, eps), 1.0f - eps);
   const float lu = logf(u);
-  const float t = expf(a * lu);             // u^a
-  const float om = 1.0f - t;                // in (0, 1)
-  const float lom = log1pf(-t);
+  const float lom = logf(-expm1f(a * lu));  // log(1 - u^a)
   const float p = expf(b * lom);            // (1 - u^a)^b
-  if (da) *da = 2.0f * b * expf((b - 1.0f) * lom) * t * lu;
+  if (da) *da = 2.0f * b * expf((b - 1.0f) * lom) * expf(a * lu) * lu;
   if (db) *db = -2.0f * p * lom;
-  (void)om;
   return 2.0f * (1.0f - p) - 1.0f;
 }
 

@@ -85,7 +85,14 @@ def filter_nan(x, xe, y, keep_rule="any"):
 def kumaraswamy_warp(Xt: torch.Tensor, a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
     """Kumaraswamy-CDF input warp on MinMax(-1,1)-scaled inputs (BASELINE config 3); the reference's only
     definitions are KumarWarp (HEBO/hebo/models/nn/mono_layers/layers.py:85-117) and GPy's InputWarpedGP
-    (HEBO/hebo/models/gp/gpy_wgp.py:120-128): u in [eps, 1-eps], w = 1 - (1 - u^a)^b, mapped back to [-1,1]."""
+    (HEBO/hebo/models/gp/gpy_wgp.py:120-128): u in [eps, 1-eps], w = 1 - (1 - u^a)^b, mapped back to [-1,1].
+    1 - u^a is formed as -expm1(a log u) as kumar_warp (common.cuh) forms it: 1 - u ** a cancels to 0 in fp32 at the
+    upper clamp once a <= 0.031."""
     eps = 1e-6
     u = ((Xt + 1.0) * 0.5).clamp(eps, 1.0 - eps)
-    return 2.0 * (1.0 - (1.0 - u ** a) ** b) - 1.0
+    x = a * torch.log(u)
+    # the value is -expm1(x); its derivative is taken through -exp(x) (t.detach() - t adds exactly 0): torch
+    # differentiates expm1 as expm1(x) + 1, which rounds to 0 in fp32 once e^x < 2^-24 (a = 10 below u = 0.19)
+    t = torch.exp(x)
+    om = -torch.expm1(x).detach() + (t.detach() - t) if torch.is_grad_enabled() and x.requires_grad else -torch.expm1(x)
+    return 2.0 * (1.0 - torch.exp(b * torch.log(om))) - 1.0

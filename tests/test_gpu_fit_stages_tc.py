@@ -89,7 +89,7 @@ from hebo_b200 import _lib
 from oracle import gp_oracle as O
 from tests.test_gpu_fit_epoch import NOISE_LB, numeric_model, run_fit
 from tests.test_gpu_fit_state import E_EX2, E_RSQ, FLUSH, GT, U, _ratio, cholesky, cond1, eps_k, gram, lower_tiles
-from tests.util import DEV, kernel_parts
+from tests.util import DEV, kernel_parts, warp_derivs
 
 pytestmark = pytest.mark.gpu
 
@@ -351,8 +351,6 @@ def test_rbf_epoch_stages():
 
 # ---------------------------------------------------------------------------------------------------------------- e. gradient
 ACC = 83.0
-EPS32 = float(np.float32(1e-6))
-ONE_M_EPS32 = float(np.float32(1.0) - np.float32(1e-6))
 
 
 def h_err(r2, kind, d):
@@ -366,29 +364,6 @@ def k_err(r2, kind, d):
     """dk / u of kern_eval(_grad) at the fp32 r^2 (docstring e.)."""
     _, hh, _, _ = kernel_parts(r2, kind)
     return eps_k(r2, kind) + 0.5 * hh.abs() * (d + 2) * r2
-
-
-def warp_derivs(x, a, b, il):
-    """fp64 dZa, dZb of scale_zt_kernel (kumar_warp's da, db times fl(1 / l)) from the fp32 x, a, b, and their error in
-    units of u (docstring e.)."""
-    h = (x + 1) * 0.5
-    uu = h.clamp(EPS32, ONE_M_EPS32)
-    clamped = (h < EPS32) | (h > ONE_M_EPS32)
-    lu = uu.log()
-    t = torch.exp(a * lu)
-    lom = torch.log1p(-t)
-    da = 2 * b * torch.exp((b - 1) * lom) * t * lu * il
-    db = -2 * torch.exp(b * lom) * lom * il
-    # absolute errors of lu and lom, relative errors of t and p as tests/util.py warp_error derives them
-    e_u = torch.where(clamped, torch.ones_like(h), (x.abs() + (x + 1).abs()) / (2 * uu) + 1)
-    e_lu = e_u + 2 * lu.abs() + 1
-    e_t = a * e_lu + (a * lu).abs() + 2
-    e_lom = t / (1 - t) * e_t + 2 * lom.abs() + 1
-    e_q = (b - 1).abs() * e_lom + ((b - 1) * lom).abs() + 2
-    e_p = b * e_lom + (b * lom).abs() + 2
-    Ea = da.abs() * (e_q + e_t + e_lu / lu.abs().clamp_min(1e-300) + 6)
-    Eb = db.abs() * (e_p + e_lom / lom.abs().clamp_min(1e-300) + 4)
-    return da, db, Ea, Eb
 
 
 class Family:

@@ -23,8 +23,9 @@ is checked on both paths:
           (rate a: sqrt 3 / sqrt 5 for the Matern kernels, r_i for the RBF).  W_k is the fp32 error of the fused warp
           in units of u, propagated step by step through kumar_warp (common.cuh): the relative error of
           u = (x_t + 1) / 2 (the scaling's two roundings and the shift; 1 where the clamp is active), then
-          log u (+ 2 |log u| + 1), t = u^a (a x that + |a log u| + 2, relative), log1p(-t) (t / (1 - t) x that
-          + 2 |log(1 - t)| + 1), p = (1 - t)^b (b x that + |b log(1 - t)| + 2, relative) and 2 (1 - p) - 1
+          log u (+ 2 |log u| + 1), x = a log u (a x that + |x|, absolute), log(1 - u^a) = log(-expm1(x))
+          (u^a / (1 - u^a) x that + 2 |log(1 - u^a)| + 3), p = (1 - u^a)^b (b x that + |b log(1 - u^a)| + 2, relative) and
+          2 (1 - p) - 1
           (2 p x that + 2 |1 - p| + |w|); 0 without a warp;
         - sqrt(n), sqrt(NP): the fp32 sums over the training points (the K* alpha partials) and over the NP padded
           columns of the SIMT contraction (square-root growth, as in test_gpu_posterior_grad.py); |mu| and s: the final

@@ -311,14 +311,37 @@ def warp_error(px, xt, a, b):
     e_u = torch.where(clamped, torch.ones_like(h), (px.abs() + xt.abs() + (xt + 1).abs()) / (2 * uu))
     lu = uu.log()
     e_lu = e_u + 2 * lu.abs() + 1
-    t = torch.exp(a * lu)
-    e_t = a * e_lu + (a * lu).abs() + 2
-    lom = torch.log1p(-t)
-    e_lom = t / (1 - t) * e_t + 2 * lom.abs() + 1
+    e_x = a * e_lu + (a * lu).abs()                  # absolute error of fl(a log u)
+    lom = torch.log(-torch.expm1(a * lu))           # log(1 - u^a) = logf(-expm1f(a log u)): the relative error of
+    e_lom = torch.exp(a * lu) / -torch.expm1(a * lu) * e_x + 2 * lom.abs() + 3      # 1 - u^a, then logf's 2 |lom|
     p = torch.exp(b * lom)
     e_p = b * e_lom + (b * lom).abs() + 2
     w = 2 * (1 - p) - 1
     return 2 * p * e_p + 2 * (1 - p).abs() + w.abs()
+
+
+def warp_derivs(x, a, b, il=1.0):
+    """fp64 dZa, dZb of scale_zt_kernel (kumar_warp's da, db times fl(1 / l)) from the fp32 x, a, b, and their error in
+    units of u, carried term by term from the absolute errors of log u and log(1 - u^a) = log(-expm1(a log u)) and the
+    relative errors of u, u^a and the powers (test_gpu_fit_stages_tc.py docstring e.)."""
+    from oracle.warp_oracle import U32
+    h = (x + 1) * 0.5
+    uu = h.clamp(*U32)
+    clamped = (h < U32[0]) | (h > U32[1])
+    lu = uu.log()
+    t = torch.exp(a * lu)
+    lom = torch.log(-torch.expm1(a * lu))
+    da = 2 * b * torch.exp((b - 1) * lom) * t * lu * il
+    db = -2 * torch.exp(b * lom) * lom * il
+    e_u = torch.where(clamped, torch.ones_like(h), (x.abs() + (x + 1).abs()) / (2 * uu) + 1)
+    e_lu = e_u + 2 * lu.abs() + 1
+    e_t = a * e_lu + (a * lu).abs() + 2
+    e_lom = t / -torch.expm1(a * lu) * (e_t - 2) + 2 * lom.abs() + 3
+    e_q = (b - 1).abs() * e_lom + ((b - 1) * lom).abs() + 2
+    e_p = b * e_lom + (b * lom).abs() + 2
+    Ea = da.abs() * (e_q + e_t + e_lu / lu.abs().clamp_min(1e-300) + 6)
+    Eb = db.abs() * (e_p + e_lom / lom.abs().clamp_min(1e-300) + 4)
+    return da, db, Ea, Eb
 
 
 def kernel_parts(r2, kind):
