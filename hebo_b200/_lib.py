@@ -21,6 +21,7 @@ HB_MAX_OBJ = 8           # objectives of hb_nsga2_survive_k / hb_pareto_front_k
 HB_DE_MAX_LAYERS, HB_DE_MAX_HIDDEN, HB_DE_MAX_OUT, HB_DE_MAX_IN, HB_DE_MAX_MEMBERS = 3, 256, 8, 256, 32
 HB_DE_MAX_BATCH_FLOATS = 56000
 HB_DE_EMBEDDING, HB_DE_ONEHOT = 0, 1
+HB_FE_STG, HB_FE_CONCRETE, HB_FE_HARD_CONCRETE = 0, 1, 2
 # random-forest envelope (HB_RF_MAX_* of include/hebo_b200.h)
 HB_RF_MAX_ROWS, HB_RF_MAX_WIDTH, HB_RF_MAX_TREES = 8192, 4096, 1024
 HB_RF_NAN_LEFT = 1 << 30   # flag of an internal node's feature word: NaN inputs go left (sklearn's missing_go_to_left)
@@ -51,6 +52,11 @@ class DeSpec(C.Structure):        # hb_de_spec_t
                 ("output_noise", C.c_int32), ("rand_prior", C.c_int32), ("noise_lb", C.c_float)]
 
 
+class FeGate(C.Structure):        # hb_fe_gate_t
+    _fields_ = [("kind", C.c_int32), ("temperature", C.c_float), ("start_temp", C.c_double), ("end_temp", C.c_double),
+                ("anneal_base", C.c_double), ("mask_reg", C.c_float)]
+
+
 class RfSpec(C.Structure):        # hb_rf_spec_t
     _fields_ = [("num_cont", C.c_int32), ("num_enum", C.c_int32), ("num_uniqs", C.POINTER(C.c_int32))]
 
@@ -59,6 +65,7 @@ _vp, _i64, _i32, _f32, _u64 = C.c_void_p, C.c_int64, C.c_int32, C.c_float, C.c_u
 _sp = C.POINTER(ModelSpec)
 _dsp = C.POINTER(DeSpec)
 _rsp = C.POINTER(RfSpec)
+_fgp = C.POINTER(FeGate)
 
 # name -> (restype, argtypes); must list every function declared in include/hebo_b200.h
 SIGNATURES = {
@@ -143,6 +150,11 @@ SIGNATURES = {
                                C.POINTER(C.c_uint64), _vp, _vp, _i64, _vp]),
     "hb_de_predict_batch": (_i32, [_vp, _vp, _i64, _dsp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _u64, _u64,
                                    _vp, _vp]),
+    "hb_fe_num_params": (_i64, [_dsp]),
+    "hb_fe_fit_workspace_bytes": (_i64, [_dsp, _i64]),
+    "hb_fe_fit": (_i32, [_vp, _vp, _vp, _i64, _dsp, _fgp, _i64, _vp, C.c_double, _f32, _i64, _i64, _vp, _vp, _u64, _vp, _vp,
+                         _i64, _vp]),
+    "hb_fe_predict": (_i32, [_vp, _vp, _i64, _dsp, _fgp, _i64, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _u64, _u64, _vp, _vp, _vp]),
     "hb_rf_fit_workspace_bytes": (_i64, [_i64, _rsp, _i64, _i64]),
     "hb_rf_forest_bytes": (_i64, [_rsp, _i64, _i64, _i64]),
     "hb_rf_fit": (_i32, [_vp, _vp, _vp, _i64, _rsp, _i64, _i64, _vp, _u64, _vp, _vp, _vp, _i64, _vp]),

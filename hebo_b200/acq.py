@@ -23,7 +23,7 @@ import torch
 
 from . import _lib
 from .base import Acquisition
-from .ensemble import DeepEnsemble, EnsembleBatch
+from .ensemble import DeepEnsemble, EnsembleBatch, FeDeepEnsemble
 from .forest import RF
 from .gp import GP, MultiTaskModel
 
@@ -167,7 +167,7 @@ def ga_score(acq, seed=None):
     if type(acq) is NoisyAcq and acq.num_obj == 1 and acq.num_constr == 0:
         if isinstance(acq.model, GP) and not acq.model._fit_failed:
             return _noisy_device_score(acq.model, int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed))
-        if isinstance(acq.model, DeepEnsemble) and acq.model.fitted and acq.model.num_out == 1:
+        if _batchable(acq.model) and acq.model.fitted and acq.model.num_out == 1:
             return _noisy_ensemble_score(acq.model, int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed))
         if isinstance(acq.model, RF) and acq.model.fitted:
             return _noisy_forest_score(acq.model, int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed))
@@ -175,10 +175,12 @@ def ga_score(acq, seed=None):
     if mode is not None and isinstance(acq.model, (GP, DeepEnsemble, RF)):
         kappa = float(getattr(acq, "kappa", 0.0))
         eta = float(getattr(acq, "eta", 0.0))
+        fe = isinstance(acq.model, FeDeepEnsemble)     # fresh gate masks per generation, keyed by (fe_seed, gen)
+        fe_seed = (int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed)) if fe else 0
 
         def device_score(xc, xe, gen):
             with torch.no_grad():
-                mu, var = acq.model.predict(xc, xe)
+                mu, var = acq.model.predict(xc, xe, seed=fe_seed, counter=gen) if fe else acq.model.predict(xc, xe)
             mu, var = mu.reshape(-1), var.reshape(-1)
             f = torch.empty_like(mu)
             if f.numel():
@@ -363,11 +365,16 @@ def general_score(acq, seed=None):
 def _ensembles_of(model):
     """The DeepEnsembles behind a GeneralAcq's model as hb_de_predict_batch operands (one multi-output ensemble, or every
     output's single-output ensemble of a MultiTaskModel), or None."""
-    if isinstance(model, DeepEnsemble):
+    if _batchable(model):
         return [model]
-    if isinstance(model, MultiTaskModel) and all(isinstance(m, DeepEnsemble) for m in model.models):
+    if isinstance(model, MultiTaskModel) and all(_batchable(m) for m in model.models):
         return model.models
     return None
+
+
+def _batchable(model) -> bool:
+    """A DeepEnsemble that hb_de_predict_batch scores: not a FeDeepEnsemble, whose gate only hb_fe_predict applies."""
+    return isinstance(model, DeepEnsemble) and not isinstance(model, FeDeepEnsemble)
 
 
 def _general_ensemble_score(acq, models, seed=None):

@@ -1061,6 +1061,29 @@ int32_t hb_de_predict_batch(const float *Xs, const int32_t *Xe, int64_t m, const
                                  counter, y_samp, (cudaStream_t)stream);
 }
 
+// fe_deep_ensemble.py: FeNet / FeDeepEnsemble, P of one gated member
+int64_t hb_fe_num_params(const hb_de_spec_t *spec) { return fe_num_params(spec); }
+
+int64_t hb_fe_fit_workspace_bytes(const hb_de_spec_t *spec, int64_t E) { return fe_fit_ws_query(spec, E); }
+
+// deep_ensemble.py:71-93 (the member loop) and FeDeepEnsemble.fit_one (fe_deep_ensemble.py:46-75)
+int32_t hb_fe_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec,
+                  const hb_fe_gate_t *gate, int64_t E, float *params, double lr, float l1, int64_t batch_size,
+                  int64_t num_epochs, const int32_t *perm, const float *draws, uint64_t seed, float *losses, void *ws,
+                  int64_t ws_bytes, void *stream) {
+  return launch_fe_fit(Xc, Xe, y, n, spec, gate, E, params, lr, l1, batch_size, num_epochs, perm, draws, seed, losses, ws,
+                       ws_bytes, (cudaStream_t)stream);
+}
+
+// deep_ensemble.py:95-116 over FeNet members (fe_deep_ensemble.py:29-35), the gate in eval mode
+int32_t hb_fe_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, const hb_fe_gate_t *gate,
+                      int64_t E, const float *params, const float *x_mul, const float *x_add, const float *y_mean,
+                      const float *y_std, int32_t member, const float *draws, uint64_t seed, uint64_t counter, float *mu,
+                      float *var, void *stream) {
+  return launch_fe_predict(Xs, Xe, m, spec, gate, E, params, x_mul, x_add, y_mean, y_std, member, draws, seed, counter, mu,
+                           var, (cudaStream_t)stream);
+}
+
 // rf.py:19-56: RF over sklearn's RandomForestRegressor (forest.cu)
 int64_t hb_rf_fit_workspace_bytes(int64_t n, const hb_rf_spec_t *spec, int64_t B, int64_t T) {
   return rf_fit_ws_query(n, spec, B, T);

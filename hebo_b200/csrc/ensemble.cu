@@ -158,8 +158,10 @@ __device__ void de_dense(const float *x, int ldx, int B, int K, const float *W, 
 
 // The input rows of s.rows: numeric columns (scaled as x * x_mul + x_add when x_mul is given), then the embedding rows
 // or one-hot codes of the categorical columns.  A category outside 0 .. u - 1 loads NaN, so its row's outputs are NaN.
+// MASK: every input column k is then multiplied by gmask[k] (a feature gate's eval mask, shared by all rows).
+template <bool MASK = false>
 __device__ void de_load_inputs(const DeNet &net, const float *prm, const float *X, const int32_t *Xe, const float *x_mul,
-                               const float *x_add, const DeSmem &s, int B) {
+                               const float *x_add, const DeSmem &s, int B, const float *gmask = nullptr) {
   for (int idx = threadIdx.x; idx < B * net.din; idx += blockDim.x) {
     const int p = idx / net.din, k = idx % net.din;
     const int64_t r = s.rows[p];
@@ -175,14 +177,18 @@ __device__ void de_load_inputs(const DeNet &net, const float *prm, const float *
       else
         v = net.emb ? prm[net.col_tab[c] + (int64_t)cat * net.col_w[c] + q] : (cat == q ? 1.0f : 0.0f);
     }
+    if constexpr (MASK) v = __fmul_rn(v, gmask[k]);
     s.xin[p * net.in_ld + k] = v;
   }
 }
 
 // BaseNet.forward (deep_ensemble.py:229-238) of the B rows in s.xin: prior net into s.pri (through d0 / d1), hidden
 // activations into s.act, heads into s.head[p, 0:O] = mu (+ prior) and s.head[p, O:2O] = the sigma2 head's pre-softplus z.
+// GATE (FeNet.forward, fe_deep_ensemble.py:29-35): the prior net is built but not evaluated.
+template <int GATE = 0>
 __device__ void de_forward(const DeNet &net, const float *prm, const DeSmem &s, int B) {
-  if (net.prior) {
+  const bool prior = !GATE && net.prior;
+  if (prior) {
     const float *src = s.xin;
     int ld = net.in_ld, K = net.din;
     for (int l = 0; l < net.L; ++l) {
@@ -206,7 +212,7 @@ __device__ void de_forward(const DeNet &net, const float *prm, const DeSmem &s, 
     ld = net.h_ld;
     K = net.H;
   }
-  de_dense(src, ld, B, K, prm + net.mu_w, prm + net.mu_b, net.O, s.head, 2 * net.O, false, net.prior ? s.pri : nullptr, net.O);
+  de_dense(src, ld, B, K, prm + net.mu_w, prm + net.mu_b, net.O, s.head, 2 * net.O, false, prior ? s.pri : nullptr, net.O);
   if (net.noise) de_dense(src, ld, B, K, prm + net.sg_w, prm + net.sg_b, net.O, s.head + net.O, 2 * net.O, false);
   __syncthreads();
 }
@@ -307,6 +313,87 @@ __device__ __forceinline__ int de_perm(int pos, int n, int h, uint64_t seed, int
   return (int)x;
 }
 
+// ------------------------------------------------------------------------------------------------ feature gate
+// FeNet's gate (fe_layers.py) on the input columns: GATE = 1 + HB_FE_STG | HB_FE_CONCRETE | HB_FE_HARD_CONCRETE, 0 = none.
+// One gate parameter theta per input column, [din] after BaseNet's P: mu (stg) or logits (concrete layers).
+struct FeGate {
+  int off;               // first gate parameter (BaseNet's P); a member holds off + din floats
+  float T;               // stg: its temperature throughout; concrete layers: predict's (the last epoch's)
+  float mcoef;           // fp32 (1 / (n num_out)) * mask_reg, 0 without numeric columns (no mask penalty)
+  double t0, t1, tb;     // start_temp, end_temp, anneal_base of the concrete layers' schedule
+  const float *draws;    // fit [E, epochs, nb, B, din] / predict [E, din] raw draws, or NULL: Philox
+  uint64_t seed, counter;
+};
+
+constexpr uint32_t FE_TAG_FIT = 0x46454654u;      // upper word of the Philox counter of the training draws ('FEFT')
+constexpr uint32_t FE_TAG_EVAL = 0x46454556u;     // ... and of the eval draws ('FEEV')
+
+// Raw draw `half` of the Philox block (row, stream): N(0, 1) by philox_normal2 for stg, U(0, 1] word for the concrete layers
+template <int GATE>
+__device__ __forceinline__ float fe_draw(uint64_t seed, uint64_t row, uint64_t stream, int half) {
+  if constexpr (GATE == 1 + HB_FE_STG) {
+    float z0, z1;
+    philox_normal2(seed, row, stream, z0, z1);
+    return half ? z1 : z0;
+  } else {
+    uint32_t c[4] = {(uint32_t)row, (uint32_t)(row >> 32), (uint32_t)stream, (uint32_t)(stream >> 32)};
+    philox4x32_10(c, seed);
+    return philox_uniform(c[half]);
+  }
+}
+
+// sigmoid((logits + logit(u)) / T) with u clamped to [eps, 1 - eps] (ConcreteLayer.gumbel_sigmoid, fe_layers.py:44-50)
+__device__ __forceinline__ float fe_concrete(float theta, float r, float T) {
+  const float u = fminf(fmaxf(r, 1.1920928955078125e-07f), 0.99999988079071044921875f);
+  const float ul = logf(__fdiv_rn(u, __fsub_rn(1.0f, u)));
+  const float zt = __fdiv_rn(__fadd_rn(theta, ul), T);
+  return __frcp_rn(__fadd_rn(1.0f, expf(-zt)));
+}
+
+// The gate's state st of one element (stg: the pre-clamp mu + 0.5 + T r; concrete layers: the sigmoid) and its mask
+template <int GATE>
+__device__ __forceinline__ float fe_state(float theta, float r, float T) {
+  if constexpr (GATE == 1 + HB_FE_STG) return __fadd_rn(__fadd_rn(__fmul_rn(T, r), theta), 0.5f);
+  else return fe_concrete(theta, r, T);
+}
+template <int GATE>
+__device__ __forceinline__ float fe_mask(float st) {
+  if constexpr (GATE == 1 + HB_FE_CONCRETE) return st;
+  const float v = GATE == 1 + HB_FE_STG ? st : __fadd_rn(__fmul_rn(st, 1.2f), -0.1f);      // hard: stretch to [-0.1, 1.1]
+  return fminf(fmaxf(v, 0.0f), 1.0f);
+}
+// d loss / d theta of one element from gm = d loss / d mask, through torch.clamp's pass-through (inclusive at both bounds)
+template <int GATE>
+__device__ __forceinline__ float fe_dtheta(float st, float gm, float T) {
+  if constexpr (GATE == 1 + HB_FE_STG) return (st >= 0.0f && st <= 1.0f) ? gm : 0.0f;
+  if constexpr (GATE == 1 + HB_FE_HARD_CONCRETE) {
+    const float v = __fadd_rn(__fmul_rn(st, 1.2f), -0.1f);
+    gm = (v >= 0.0f && v <= 1.0f) ? __fmul_rn(gm, 1.2f) : 0.0f;
+  }
+  return __fdiv_rn(__fmul_rn(__fmul_rn(gm, __fsub_rn(1.0f, st)), st), T);
+}
+// d mask_loss / d theta: mcoef d mask_norm / d theta, mask_norm = sum Phi((mu + 0.5) / T) (stg) or sum sigmoid(logits)
+template <int GATE>
+__device__ __forceinline__ float fe_dnorm(float theta, float mcoef, float T) {
+  if constexpr (GATE == 1 + HB_FE_STG) {
+    const float w = __fdiv_rn(__fdiv_rn(__fadd_rn(theta, 0.5f), T), 1.41421356237309515f);
+    const float g = __fmul_rn(__fmul_rn(mcoef, 0.5f), __fmul_rn(1.12837916709551257f, expf(-__fmul_rn(w, w))));
+    return __fdiv_rn(__fdiv_rn(g, 1.41421356237309515f), T);
+  } else {
+    const float sg = __frcp_rn(__fadd_rn(1.0f, expf(-theta)));
+    return __fmul_rn(__fmul_rn(mcoef, __fsub_rn(1.0f, sg)), sg);
+  }
+}
+
+// parameter i is a weight (its state_dict name contains 'weight'): FeDeepEnsemble's L1 set (fe_deep_ensemble.py:62-64)
+__device__ __forceinline__ bool fe_is_weight(const DeNet &net, int i, int off) {
+  if (i >= off) return false;
+  const auto in = [i](int a, int n) { return i >= a && i < a + n; };
+  for (int l = 0; l < net.L; ++l)
+    if (in(net.b[l], net.H) || (net.prior && in(net.pb[l], net.H))) return false;
+  return !(in(net.mu_b, net.O) || (net.noise && in(net.sg_b, net.O)) || (net.prior && in(net.po_b, net.O)));
+}
+
 // ------------------------------------------------------------------------------------------------ fit
 struct DeFitArgs {
   const float *Xc, *y;
@@ -318,10 +405,15 @@ struct DeFitArgs {
   float coef;       // fp32 (1 / (n num_out)) * l1: the L1 term's gradient per unit sign
 };
 
-// The whole fit of one member: a's pointers are its ensemble's (params [E, P], m1 / m2 / grad [E, P], losses [E, epochs])
-__device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs &a, int member, float *smem) {
+// The whole fit of one member: a's pointers are its ensemble's (params [E, P], m1 / m2 / grad [E, P], losses [E, epochs]).
+// GATE: FeDeepEnsemble.fit_one (fe_deep_ensemble.py:46-75) with fe's gate; the unmasked inputs and the gate states of the
+// minibatch sit in two more [B, in_ld] buffers after the scratch.
+template <int GATE = 0>
+__device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs &a, int member, float *smem,
+                                              const FeGate *fe = nullptr) {
   const int B = a.B, O = net.O;
   const DeSmem s = de_carve(net, smem, B);
+  float *xraw = s.red + DE_SCRATCH, *gst = xraw + B * net.in_ld;
   float *prm = a.params + (size_t)member * net.P;
   float *m1 = a.m1 + (size_t)member * net.P, *m2 = a.m2 + (size_t)member * net.P, *g = a.grad + (size_t)member * net.P;
   for (int i = threadIdx.x; i < net.P; i += blockDim.x) {
@@ -332,6 +424,9 @@ __device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs 
   int step = 0;
   for (int ep = 0; ep < a.epochs; ++ep) {
     float epoch_loss = 0.0f;     // thread 0
+    float T = 0.0f;
+    if constexpr (GATE == 1 + HB_FE_STG) T = fe->T;
+    else if constexpr (GATE != 0) T = (float)fmax(fe->t0 * pow(fe->tb, (double)ep), fe->t1);     // torch.tensor(.).clamp(end)
     for (int bi = 0; bi < a.nb; ++bi) {
       ++step;
       for (int p = threadIdx.x; p < B; p += blockDim.x) {
@@ -341,7 +436,21 @@ __device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs 
       __syncthreads();
       de_load_inputs(net, prm, a.Xc, a.Xe, nullptr, nullptr, s, B);
       __syncthreads();
-      de_forward(net, prm, s, B);
+      if constexpr (GATE != 0) {       // x * mask with a fresh draw per row and column (the training mask of x.shape)
+        const size_t base = (((size_t)member * a.epochs + ep) * a.nb + bi) * (size_t)B * net.din;
+        for (int idx = threadIdx.x; idx < B * net.din; idx += blockDim.x) {
+          const int p = idx / net.din, k = idx % net.din;
+          const uint64_t q = (((uint64_t)ep * a.nb + bi) * B + p) * net.din + k;
+          const float r = fe->draws ? fe->draws[base + idx]
+                                    : fe_draw<GATE>(a.seed, q >> 1, ((uint64_t)FE_TAG_FIT << 32) | (uint32_t)member, (int)(q & 1));
+          const float x = s.xin[p * net.in_ld + k], st = fe_state<GATE>(prm[fe->off + k], r, T);
+          xraw[p * net.in_ld + k] = x;
+          gst[p * net.in_ld + k] = st;
+          s.xin[p * net.in_ld + k] = __fmul_rn(x, fe_mask<GATE>(st));
+        }
+        __syncthreads();
+      }
+      de_forward<GATE>(net, prm, s, B);
       // the loss over the finite entries of y (loss_likelihood / loss_mse, deep_ensemble.py:140-149)
       if (threadIdx.x < 32) {
         float cnt = 0.0f;
@@ -379,7 +488,23 @@ __device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs 
         sum = warp_sum(sum);
         if (threadIdx.x == 0) epoch_loss += sum / cnt * (float)B;      // epoch_loss += data_loss * bxc.shape[0]
       }
-      float *dx = de_backward(net, prm, s, B, g, net.emb && net.ne > 0, net.dc);
+      float *dx = GATE ? de_backward(net, prm, s, B, g, true, 0) : de_backward(net, prm, s, B, g, net.emb && net.ne > 0, net.dc);
+      if constexpr (GATE != 0) {
+        // column k: d loss / d theta_k = sum over rows in order of (dx x) through the mask, plus the mask penalty's;
+        // then dx becomes the delta of the unmasked input (dx mask) for the embedding tables
+        for (int k = threadIdx.x; k < net.din; k += blockDim.x) {
+          const float theta = prm[fe->off + k];
+          float acc = 0.0f;
+          for (int p = 0; p < B; ++p) {
+            float &d = dx[p * net.h_ld + k];
+            const float st = gst[p * net.in_ld + k];
+            acc += fe_dtheta<GATE>(st, __fmul_rn(d, xraw[p * net.in_ld + k]), T);
+            d = __fmul_rn(d, fe_mask<GATE>(st));
+          }
+          g[fe->off + k] = fe->mcoef != 0.0f ? __fadd_rn(acc, fe_dnorm<GATE>(theta, fe->mcoef, T)) : acc;
+        }
+        __syncthreads();
+      }
       // embedding tables: the input delta of each row added into the row of its category, rows in batch order
       if (net.emb) {
         for (int c = 0; c < net.ne; ++c) {
@@ -401,8 +526,14 @@ __device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs 
       for (int i = threadIdx.x; i < net.P; i += blockDim.x) {
         const float p = prm[i];
         const float sg = p > 0.0f ? 1.0f : (p < 0.0f ? -1.0f : 0.0f);
-        const float gd = i < net.prior0 ? g[i] : 0.0f;
-        const float gt = __fadd_rn(gd, __fmul_rn(a.coef, sg));
+        float gd, gt;
+        if constexpr (GATE != 0) {      // L1 over the weights only; the prior net's biases keep gt = 0 and do not move
+          gd = (i < net.prior0 || i >= fe->off) ? g[i] : 0.0f;
+          gt = fe_is_weight(net, i, fe->off) ? __fadd_rn(gd, __fmul_rn(a.coef, sg)) : gd;
+        } else {
+          gd = i < net.prior0 ? g[i] : 0.0f;
+          gt = __fadd_rn(gd, __fmul_rn(a.coef, sg));
+        }
         const float mm = __fadd_rn(m1[i], __fmul_rn(0.1f, __fsub_rn(gt, m1[i])));
         const float vv = __fadd_rn(__fmul_rn(m2[i], 0.999f), __fmul_rn(__fmul_rn(0.001f, gt), gt));
         const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(vv), bc2f), 1e-8f);
@@ -420,6 +551,13 @@ __device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs 
 __global__ void __launch_bounds__(DE_FIT_THREADS) de_fit_kernel(const __grid_constant__ DeNet net, const DeFitArgs a) {
   extern __shared__ float smem[];
   de_fit_member(net, a, blockIdx.x, smem);
+}
+
+template <int GATE>
+__global__ void __launch_bounds__(DE_FIT_THREADS) fe_fit_kernel(const __grid_constant__ DeNet net, const DeFitArgs a,
+                                                                const __grid_constant__ FeGate fe) {
+  extern __shared__ float smem[];
+  de_fit_member<GATE>(net, a, blockIdx.x, smem, &fe);
 }
 
 // Per-ensemble arguments of hb_de_fit_batch: its rows [off, off + n) of the concatenated inputs and what follows from n
@@ -470,17 +608,30 @@ struct DePredArgs {
 };
 
 // Rows r0 .. r0 + DE_TM - 1 of the candidates (the last one repeated past m) through members e0 .. e1 - 1: the heads mu
-// into mus[e - e0][p, o] and, with output_noise, sigma2 into s2s[e - e0][p, o]
+// into mus[e - e0][p, o] and, with output_noise, sigma2 into s2s[e - e0][p, o].  GATE: member e's eval mask [din] (one
+// draw per column, shared by every row) goes to gmask and multiplies the inputs in the load.
+template <int GATE = 0>
 __device__ __forceinline__ void de_member_heads(const DeNet &net, const DePredArgs &a, const DeSmem &s, int r0, int e0,
-                                                int e1, float *mus, float *s2s) {
+                                                int e1, float *mus, float *s2s, const FeGate *fe = nullptr,
+                                                float *gmask = nullptr) {
   const int O = net.O, B = DE_TM;
   for (int p = threadIdx.x; p < B; p += blockDim.x) s.rows[p] = min(r0 + p, a.m - 1);
   __syncthreads();
   for (int e = e0; e < e1; ++e) {
     const float *prm = a.params + (size_t)e * net.P;
-    de_load_inputs(net, prm, a.Xs, a.Xe, a.x_mul, a.x_add, s, B);
+    if constexpr (GATE != 0) {
+      for (int k = threadIdx.x; k < net.din; k += blockDim.x) {
+        const uint64_t stream = ((uint64_t)FE_TAG_EVAL << 32) | ((uint32_t)e << 16) | (uint32_t)(k >> 1);
+        const float r = fe->draws ? fe->draws[(size_t)e * net.din + k] : fe_draw<GATE>(fe->seed, fe->counter, stream, k & 1);
+        gmask[k] = fe_mask<GATE>(fe_state<GATE>(prm[fe->off + k], r, fe->T));
+      }
+      __syncthreads();
+      de_load_inputs<true>(net, prm, a.Xs, a.Xe, a.x_mul, a.x_add, s, B, gmask);
+    } else {
+      de_load_inputs(net, prm, a.Xs, a.Xe, a.x_mul, a.x_add, s, B);
+    }
     __syncthreads();
-    de_forward(net, prm, s, B);
+    de_forward<GATE>(net, prm, s, B);
     for (int i = threadIdx.x; i < B * O; i += blockDim.x) {
       const int p = i / O, o = i % O;
       mus[(e - e0) * B * O + i] = s.head[p * 2 * O + o];
@@ -517,14 +668,17 @@ __device__ __forceinline__ void de_combine(const DeNet &net, const float *mus, c
   }
 }
 
-template <bool GRAD>
-__global__ void __launch_bounds__(DE_PRED_THREADS) de_predict_kernel(const __grid_constant__ DeNet net, const DePredArgs a) {
+// GATE: fe's gate on every member (no input gradients: FeDeepEnsemble.support_grad = False); the eval mask sits after py
+template <bool GRAD, int GATE = 0>
+__global__ void __launch_bounds__(DE_PRED_THREADS) de_predict_kernel(const __grid_constant__ DeNet net, const DePredArgs a,
+                                                                     const __grid_constant__ FeGate fe) {
+  static_assert(!(GRAD && GATE), "the gated ensemble has no input gradients");
   extern __shared__ float smem[];
   const int O = net.O, B = DE_TM, r0 = blockIdx.x * DE_TM;
   const DeSmem s = de_carve(net, smem, B);
   const int e0 = a.member >= 0 ? a.member : 0, e1 = a.member >= 0 ? a.member + 1 : a.E, ne = e1 - e0;
   float *mus = s.red + DE_SCRATCH, *s2s = mus + ne * B * O, *py = s2s + ne * B * O;
-  de_member_heads(net, a, s, r0, e0, e1, mus, s2s);
+  de_member_heads<GATE>(net, a, s, r0, e0, e1, mus, s2s, &fe, py + B * O);
   for (int i = threadIdx.x; i < B * O; i += blockDim.x) {
     const int p = i / O, o = i % O, row = r0 + p;
     float mean, v;
@@ -719,10 +873,10 @@ int launch_de_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de
   const unsigned grid = (unsigned)ceil_div(m, DE_TM);
   if (grad) {
     HB_CUDA(cudaFuncSetAttribute(de_predict_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    de_predict_kernel<true><<<grid, DE_PRED_THREADS, smem, st>>>(net, a);
+    de_predict_kernel<true><<<grid, DE_PRED_THREADS, smem, st>>>(net, a, FeGate{});
   } else {
     HB_CUDA(cudaFuncSetAttribute(de_predict_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    de_predict_kernel<false><<<grid, DE_PRED_THREADS, smem, st>>>(net, a);
+    de_predict_kernel<false><<<grid, DE_PRED_THREADS, smem, st>>>(net, a, FeGate{});
   }
   count_launches(1);
   HB_LAUNCH_CHECK("de_predict_kernel");
@@ -815,6 +969,138 @@ int launch_de_predict_batch(const float *Xs, const int32_t *Xe, int64_t m, const
   de_predict_batch_kernel<<<dim3((unsigned)ceil_div(m, DE_TM), (unsigned)nens), DE_PRED_THREADS, smem, st>>>(net, ba);
   count_launches(1);
   HB_LAUNCH_CHECK("de_predict_batch_kernel");
+  return HB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ gated launchers
+// FeDeepEnsemble's member: BaseNet's layout (net.P = its P + din afterwards) with the gate [din] last
+static bool fe_layout(const hb_de_spec_t *spec, const hb_fe_gate_t *gate, DeNet &net, FeGate &fe) {
+  if (!gate || gate->kind < HB_FE_STG || gate->kind > HB_FE_HARD_CONCRETE || !(gate->temperature > 0.0f)) return false;
+  if (!de_layout(spec, net)) return false;
+  fe = FeGate{};
+  fe.off = net.P;
+  net.P += net.din;
+  fe.T = gate->temperature;
+  fe.t0 = gate->start_temp;
+  fe.t1 = gate->end_temp;
+  fe.tb = gate->anneal_base;
+  return true;
+}
+
+// floats of a gated fit's minibatch buffers: BaseNet's plus the unmasked inputs and the gate states, B in_ld each
+static int64_t fe_rows_floats(const DeNet &net, int64_t B) { return de_rows_floats(net, B) + 2 * B * net.in_ld; }
+
+int64_t fe_num_params(const hb_de_spec_t *spec) {
+  DeNet net;
+  return de_layout(spec, net) ? net.P + net.din : -1;
+}
+
+int64_t fe_fit_ws_query(const hb_de_spec_t *spec, int64_t E) {
+  const int64_t P = fe_num_params(spec);
+  if (P < 0 || E < 1 || E > HB_DE_MAX_MEMBERS) return -1;
+  return 3 * E * P * (int64_t)sizeof(float);
+}
+
+template <int GATE>
+static int fe_fit_launch(const DeNet &net, const DeFitArgs &a, const FeGate &fe, int64_t E, size_t smem, cudaStream_t st) {
+  HB_CUDA(cudaFuncSetAttribute(fe_fit_kernel<GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  fe_fit_kernel<GATE><<<(unsigned)E, DE_FIT_THREADS, smem, st>>>(net, a, fe);
+  return HB_OK;
+}
+
+int launch_fe_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec,
+                  const hb_fe_gate_t *gate, int64_t E, float *params, double lr, float l1, int64_t batch_size,
+                  int64_t num_epochs, const int32_t *perm, const float *draws, uint64_t seed, float *losses, void *ws,
+                  int64_t ws_bytes, cudaStream_t st) {
+  DeNet net;
+  FeGate fe;
+  if (!fe_layout(spec, gate, net, fe) || E < 1 || E > HB_DE_MAX_MEMBERS || n < 1 || n > (1 << 30) || batch_size < 1 ||
+      num_epochs < 0)
+    return HB_ERR_INVALID;
+  if (!y || !params || !ws || (num_epochs > 0 && !losses) || (net.dc > 0 && !Xc) || (net.ne > 0 && !Xe)) return HB_ERR_INVALID;
+  if (ws_bytes < fe_fit_ws_query(spec, E)) return HB_ERR_INVALID;
+  const int64_t B = n > batch_size ? batch_size : n;     // as launch_de_fit
+  if (fe_rows_floats(net, B) > HB_DE_MAX_BATCH_FLOATS) return HB_ERR_INVALID;
+  if (num_epochs == 0) return HB_OK;
+  DeFitArgs a;
+  a.Xc = Xc;
+  a.Xe = Xe;
+  a.y = y;
+  a.perm = perm;
+  a.params = params;
+  a.m1 = (float *)ws;
+  a.m2 = a.m1 + E * net.P;
+  a.grad = a.m2 + E * net.P;
+  a.losses = losses;
+  a.n = (int)n;
+  a.B = (int)B;
+  a.nb = (int)(n > batch_size ? n / batch_size : 1);
+  a.epochs = (int)num_epochs;
+  int h = 1;
+  while ((int64_t(1) << (2 * h)) < n) ++h;
+  a.h = h;
+  a.seed = seed;
+  a.lr = lr;
+  a.coef = (1.0f / (float)(n * net.O)) * l1;
+  fe.mcoef = net.dc > 0 ? (1.0f / (float)(n * net.O)) * gate->mask_reg : 0.0f;     // mask_loss only when Xc.shape[1] > 0
+  fe.draws = draws;
+  const size_t smem = (size_t)(fe_rows_floats(net, B) + DE_SCRATCH) * sizeof(float);
+  const int rc = gate->kind == HB_FE_STG        ? fe_fit_launch<1 + HB_FE_STG>(net, a, fe, E, smem, st)
+                 : gate->kind == HB_FE_CONCRETE ? fe_fit_launch<1 + HB_FE_CONCRETE>(net, a, fe, E, smem, st)
+                                                : fe_fit_launch<1 + HB_FE_HARD_CONCRETE>(net, a, fe, E, smem, st);
+  if (rc != HB_OK) return rc;
+  count_launches(1);
+  HB_LAUNCH_CHECK("fe_fit_kernel");
+  return HB_OK;
+}
+
+template <int GATE>
+static int fe_predict_launch(const DeNet &net, const DePredArgs &a, const FeGate &fe, unsigned grid, size_t smem,
+                              cudaStream_t st) {
+  HB_CUDA(cudaFuncSetAttribute(de_predict_kernel<false, GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  de_predict_kernel<false, GATE><<<grid, DE_PRED_THREADS, smem, st>>>(net, a, fe);
+  return HB_OK;
+}
+
+int launch_fe_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, const hb_fe_gate_t *gate,
+                      int64_t E, const float *params, const float *x_mul, const float *x_add, const float *y_mean,
+                      const float *y_std, int32_t member, const float *draws, uint64_t seed, uint64_t counter, float *mu,
+                      float *var, cudaStream_t st) {
+  DeNet net;
+  FeGate fe;
+  if (!fe_layout(spec, gate, net, fe) || E < 1 || E > HB_DE_MAX_MEMBERS || m < 0 || m > (int64_t(1) << 31) - DE_TM)
+    return HB_ERR_INVALID;
+  if (member < -1 || member >= E) return HB_ERR_INVALID;
+  if (!params || !y_mean || !y_std || !mu || (member < 0 && !var) || (net.ne > 0 && !Xe)) return HB_ERR_INVALID;
+  if (net.dc > 0 && (!Xs || !x_mul || !x_add)) return HB_ERR_INVALID;
+  if (m == 0) return HB_OK;
+  DePredArgs a;
+  a.Xs = Xs;
+  a.Xe = Xe;
+  a.params = params;
+  a.x_mul = x_mul;
+  a.x_add = x_add;
+  a.y_mean = y_mean;
+  a.y_std = y_std;
+  a.mu = mu;
+  a.var = var;
+  a.dmu = a.dvar = nullptr;
+  a.m = (int)m;
+  a.E = (int)E;
+  a.member = member;
+  fe.draws = draws;
+  fe.seed = seed;
+  fe.counter = counter;
+  const int64_t ne = member >= 0 ? 1 : E;
+  const size_t smem =
+      (size_t)(de_rows_floats(net, DE_TM) + DE_SCRATCH + (2 * ne + 1) * DE_TM * net.O + net.din) * sizeof(float);
+  const unsigned grid = (unsigned)ceil_div(m, DE_TM);
+  const int rc = gate->kind == HB_FE_STG        ? fe_predict_launch<1 + HB_FE_STG>(net, a, fe, grid, smem, st)
+                 : gate->kind == HB_FE_CONCRETE ? fe_predict_launch<1 + HB_FE_CONCRETE>(net, a, fe, grid, smem, st)
+                                                : fe_predict_launch<1 + HB_FE_HARD_CONCRETE>(net, a, fe, grid, smem, st);
+  if (rc != HB_OK) return rc;
+  count_launches(1);
+  HB_LAUNCH_CHECK("de_predict_kernel (gated)");
   return HB_OK;
 }
 

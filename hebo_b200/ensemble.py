@@ -59,11 +59,14 @@ def param_layout(num_cont, num_uniqs, enum_trans, num_layers, num_hiddens, num_o
 
 
 def init_params(layout) -> torch.Tensor:
-    """BaseNet's initialisation (:217-221) from torch's global CPU generator, in registration order."""
+    """BaseNet's initialisation (:217-221) from torch's global CPU generator, in registration order; a feature gate's
+    parameter (FeNet's feature_select, last) is 0.01 randn (fe_layers.py:26, 82)."""
     parts = []
     for name, shape in layout:
         t = torch.empty(shape)
-        if "bias" in name:
+        if name.startswith("feature_select."):
+            t = 0.01 * torch.randn(shape)
+        elif "bias" in name:
             nn.init.zeros_(t)
         else:
             nn.init.xavier_uniform_(t, gain=nn.init.calculate_gain("relu"))
@@ -267,11 +270,12 @@ class DeepEnsemble(BaseModel):
         self.seed = int(torch.randint(0, 2 ** 62, (1,)).item())     # the Philox key of this fit's minibatch order
         return Xc, Xe, y, valid
 
-    def _finish_fit(self, Xc_, Xe_, y_, valid):
-        """fit's host side after the launch: the noise estimate on the kept rows (deep_ensemble.py:89-93)."""
+    def _finish_fit(self, Xc_, Xe_, y_, valid, **predict_kw):
+        """fit's host side after the launch: the noise estimate on the kept rows (deep_ensemble.py:89-93); predict_kw
+        goes to that predict."""
         self.sample_idx = 0
         with torch.no_grad():
-            py, _ = self.predict(Xc_, Xe_)
+            py, _ = self.predict(Xc_, Xe_, **predict_kw)
             err = (py - torch.as_tensor(y_).float())[valid]
             self.noise_est = (err ** 2).mean(dim=0).detach().clone()
 
@@ -432,6 +436,8 @@ class EnsembleBatch:
     def __init__(self, models):
         m0 = models[0]
         assert all(m.fitted for m in models), "fit() first"
+        if any(isinstance(m, FeDeepEnsemble) for m in models):
+            raise TypeError("EnsembleBatch: a FeDeepEnsemble predicts through hb_fe_predict, which applies its gate")
         self.models, self.spec, self.E, self.device = models, m0._spec, m0.num_ensembles, m0.device
         self.num_cont, self.num_out = m0.num_cont, len(models) * m0.num_out
         self.params = _stacked_params(models)
@@ -494,3 +500,153 @@ def fit_ensembles(models, Xc, Xe, ys) -> None:
         if m.verbose:
             m._print_losses()
         m._finish_fit(Xc, Xe, ys[b], preps[b][3])
+
+
+_FE_KINDS = {"stg": _lib.HB_FE_STG, "concrete": _lib.HB_FE_CONCRETE, "hard_concrete": _lib.HB_FE_HARD_CONCRETE}
+_FE_DEFAULT_T = {"stg": 1.0, "concrete": 0.1, "hard_concrete": 0.1}      # the layers' constructor defaults
+
+
+def fe_epoch_temperature(start_temp: float, end_temp: float, anneal_base: float, epoch: int) -> float:
+    """The concrete layers' temperature of an epoch as fe_deep_ensemble.py:59-60 rounds it: the product in double, then
+    torch.tensor (fp32) clamped below at end_temp."""
+    return float(np.float32(max(start_temp * anneal_base ** epoch, end_temp)))
+
+
+class FeDeepEnsemble(DeepEnsemble):
+    """Drop-in for ``hebo.models.nn.fe_deep_ensemble.FeDeepEnsemble``: a DeepEnsemble whose members gate their input
+    columns with a learned feature-selection layer (``fe_layer``: 'stg' (default), 'concrete' or 'hard_concrete') before
+    the first hidden layer, so irrelevant inputs can be switched off.  The fit runs in one ``hb_fe_fit`` launch and
+    prediction in ``hb_fe_predict`` (hebo_b200/csrc/ensemble.cu, the deep ensemble's kernels with the gate compiled in).
+
+    Extra conf keys and defaults: fe_layer 'stg', temperature None (the layer's own: 1.0 for stg, 0.1 otherwise),
+    mask_reg 0.1, start_temp 1.0, end_temp 0.1, anneal_base 0.99.  A member's parameters are FeNet's state_dict in
+    registration order: BaseNet's, then ``feature_select.mu`` (stg) or ``feature_select.logits`` [din] last.  The L1 term
+    covers weights only, the mask penalty applies when there are numeric columns, and the random prior net (rand_prior)
+    is built but not evaluated, all as the reference does.
+
+    Masks are random in predict too (the reference redraws them on every forward): each call draws fresh eval masks from
+    a Philox key taken from torch's global generator, or from the given ``seed`` / ``counter``, so a call is reproducible
+    under ``torch.manual_seed``.  No input gradients (``support_grad = False``).  Like DeepEnsemble, the fit does not
+    call ``torch.seed()``, a deliberate deviation that keeps it reproducible under ``torch.manual_seed``."""
+    support_grad = False
+
+    def __init__(self, num_cont, num_enum, num_out, **conf):
+        fe_layer = conf.get("fe_layer", "stg")
+        if fe_layer not in _FE_KINDS:
+            raise KeyError(f"FeDeepEnsemble: unknown fe_layer {fe_layer!r}, can only be [stg|concrete|hard_concrete]")
+        conf.pop("basenet_cls", None)
+        super().__init__(num_cont, num_enum, num_out, **conf)
+        self.basenet_cls = _reference_fenet()
+        self.conf["basenet_cls"] = self.basenet_cls
+        self.fe_layer = fe_layer
+        self.temperature = self.conf.get("temperature")
+        self.mask_reg = self.conf.get("mask_reg", 0.1)
+        self.end_temp = self.conf.get("end_temp", 0.1)
+        self.start_temp = self.conf.get("start_temp", 1.0)
+        self.anneal_base = self.conf.get("anneal_base", 0.99)
+        t = self.temperature if self.temperature else _FE_DEFAULT_T[fe_layer]      # FeNet: `if self.temperature:`
+        self.gate_temperature = float(np.float32(t))        # stg's T throughout; the concrete layers' until a fit
+        self.layout = self.layout + [("feature_select.mu" if fe_layer == "stg" else "feature_select.logits", (self.din,))]
+        self.P += self.din
+
+    def batch_floats(self, rows: int) -> int:
+        """On-chip floats of a gated minibatch: the deep ensemble's plus the unmasked inputs and gate states."""
+        return super().batch_floats(rows) + 2 * rows * (self.din | 1)
+
+    def _gate(self):
+        return _lib.FeGate(_FE_KINDS[self.fe_layer], self.gate_temperature, float(self.start_temp), float(self.end_temp),
+                           float(self.anneal_base), float(self.mask_reg))
+
+    def draws_shape(self, n: int):
+        """Shape of fit's explicit training draws for n kept rows: [E, num_epochs, minibatches, rows, din]."""
+        bs = int(self.batch_size)
+        return (self.num_ensembles, int(self.num_epochs), n // bs if n > bs else 1, min(n, bs), self.din)
+
+    # ------------------------------------------------------------------ fit (fe_deep_ensemble.py:46-75)
+    def fit(self, Xc_, Xe_, y_, perm=None, draws=None, eval_draws=None):
+        """perm: as DeepEnsemble.fit.  draws: optional training draws (``draws_shape``): N(0, 1) for stg, U(0, 1) for the
+        concrete layers; otherwise Philox draws on the device.  eval_draws: optional [E, din] draws of the noise
+        estimate's predict (tests replaying the reference's own draws)."""
+        Xc, Xe, y, valid = self._prepare_fit(Xc_, Xe_, y_, perm)
+        if draws is not None:
+            draws = torch.as_tensor(draws, dtype=torch.float32)
+            if tuple(draws.shape) != self.draws_shape(y.shape[0]):
+                raise ValueError(f"draws must be {list(self.draws_shape(y.shape[0]))}, got {list(draws.shape)}")
+        self._fit_dev(Xc, Xe, y, perm, self.seed, draws)
+        self._finish_fit(Xc_, Xe_, y_, valid, draws=eval_draws)
+
+    def _fit_dev(self, Xc, Xe, y, perm, seed, draws=None):
+        lib, dev, E = _lib.lib(), self.device, self.num_ensembles
+        n, T = y.shape[0], int(self.num_epochs)
+        xc = Xc.to(dev, torch.float32).contiguous() if self.num_cont > 0 else None
+        xe = Xe.to(dev, torch.int32).contiguous() if self.num_enum > 0 else None
+        yd = y.to(dev, torch.float32).contiguous()
+        pd_ = None if perm is None else torch.as_tensor(perm).to(dev, torch.int32).contiguous()
+        dd = None if draws is None else draws.to(dev, torch.float32).contiguous()
+        need = int(lib.hb_fe_fit_workspace_bytes(C.byref(self._spec), E))
+        self.fit_ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        losses = torch.empty(E, max(1, T), dtype=torch.float32, device=dev)
+        gate = self._gate()
+        with torch.cuda.device(dev):
+            _lib.check(lib.hb_fe_fit(_lib.ptr(xc), _lib.ptr(xe), _lib.ptr(yd), n, C.byref(self._spec), C.byref(gate), E,
+                                     _lib.ptr(self.params), float(self.lr), float(self.l1), int(self.batch_size), T,
+                                     _lib.ptr(pd_), _lib.ptr(dd), seed & (2 ** 64 - 1), _lib.ptr(losses),
+                                     _lib.ptr(self.fit_ws), need, _lib.stream_ptr()), "hb_fe_fit")
+        self.losses = losses[:, :T]
+        if T > 0 and self.fe_layer != "stg":       # predict uses the last epoch's temperature
+            self.gate_temperature = fe_epoch_temperature(self.start_temp, self.end_temp, self.anneal_base, T - 1)
+        if self.verbose:
+            self._print_losses()
+
+    # ------------------------------------------------------------------ predict
+    def _predict_dev(self, Xs, xe, grad=False, member=-1, draws=None, seed=None, counter=0):
+        if grad:
+            raise NotImplementedError("FeDeepEnsemble: no input gradients (support_grad = False)")
+        lib, dev = _lib.lib(), self.device
+        assert self.fitted, "fit() first"
+        m = (Xs if Xs is not None else xe).shape[0]
+        xm, xa, ym, ys = self._scal_dev()
+        mu = torch.empty(m, self.num_out, dtype=torch.float32, device=dev)
+        var = torch.empty(m, self.num_out, dtype=torch.float32, device=dev) if member < 0 else None
+        if draws is not None:
+            draws = torch.as_tensor(draws).to(dev, torch.float32).contiguous()
+            if tuple(draws.shape) != (self.num_ensembles, self.din):
+                raise ValueError(f"eval draws must be [{self.num_ensembles}, {self.din}], got {list(draws.shape)}")
+        elif seed is None:
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
+        gate = self._gate()
+        with torch.cuda.device(dev):
+            _lib.check(lib.hb_fe_predict(_lib.ptr(Xs), _lib.ptr(xe), m, C.byref(self._spec), C.byref(gate),
+                                         self.num_ensembles, _lib.ptr(self.params), _lib.ptr(xm), _lib.ptr(xa), _lib.ptr(ym),
+                                         _lib.ptr(ys), int(member), _lib.ptr(draws), int(seed or 0) & (2 ** 64 - 1),
+                                         int(counter) & (2 ** 64 - 1), _lib.ptr(mu), _lib.ptr(var), _lib.stream_ptr()),
+                       "hb_fe_predict")
+        return mu, var
+
+    def predict(self, Xc, Xe=None, draws=None, seed=None, counter=0):
+        """(py, ps2) [m, num_out] under fresh eval masks: CPU tensors for CPU inputs, device tensors for device inputs.
+        draws [E, din]: the masks' raw draws (tests); otherwise Philox keyed by (seed, counter), seed from torch's
+        generator when None."""
+        probe = Xc if (Xc is not None and self.num_cont > 0) else Xe
+        on_cpu = not (torch.is_tensor(probe) and probe.is_cuda)
+        xs, xe, _ = self._inputs(Xc, Xe)
+        mu, var = self._predict_dev(xs, xe, draws=draws, seed=seed, counter=counter)
+        return (mu.cpu(), var.cpu()) if on_cpu else (mu, var)
+
+    def sample_y(self, Xc, Xe=None, n_samples: int = 1):
+        """BaseModel.sample_y (base_model.py:78-84): one predict, then py + sqrt(ps2) * torch.randn per sample."""
+        py, ps2 = self.predict(Xc, Xe)
+        ps = ps2.sqrt()
+        samp = torch.zeros(n_samples, py.shape[0], self.num_out, device=py.device)
+        for i in range(n_samples):
+            samp[i] = py + ps * torch.randn(py.shape).to(py.device)
+        return samp
+
+
+def _reference_fenet():
+    """FeNet of an installed HEBO, or None."""
+    try:  # pragma: no cover - depends on the environment
+        from hebo.models.nn.fe_deep_ensemble import FeNet
+        return FeNet
+    except Exception:
+        return None

@@ -601,6 +601,68 @@ int32_t hb_de_predict_batch(const float *Xs, const int32_t *Xe, int64_t m, const
                             const float *y_std, float *mu, float *var, int64_t n_samples, const float *xi, uint64_t seed,
                             uint64_t counter, float *y_samp, void *stream);
 
+/* ---- feature-selecting deep ensemble (models/nn/fe_deep_ensemble.py: FeNet, FeDeepEnsemble; fe_layers.py) ---------------
+ * The deep ensemble above whose members multiply their input row x [din] (numeric columns, then the embedding or one-hot
+ * columns) by a learned gate mask before the first hidden layer.  The prior net, when rand_prior is set, is built and takes
+ * the L1 term but is not evaluated (FeNet.forward).  One member's raw parameters are P_fe = hb_fe_num_params(spec) =
+ * hb_de_num_params(spec) + din floats: BaseNet's layout, then the gate's feature_select.mu (stg) or feature_select.logits
+ * (concrete layers) [din] LAST, so a FeNet state_dict maps to them without permutation.  Masks of parameter theta, draw r
+ * and temperature T, in IEEE fp32 without FMA contraction:
+ *   HB_FE_STG            clamp((T r + theta) + 0.5, 0, 1),                     r ~ N(0, 1)
+ *   HB_FE_CONCRETE       sigmoid((theta + log(u / (1 - u))) / T),              u = clamp(r, eps, 1 - eps), r ~ U(0, 1]
+ *   HB_FE_HARD_CONCRETE  clamp(concrete * 1.2 + (-0.1), 0, 1)                  (stretched to [-0.1, 1.1])
+ * eps = FLT_EPSILON; the clamps pass the gradient at both bounds inclusive, as torch.clamp does. */
+#define HB_FE_STG            0    /* conf['fe_layer'] = 'stg' (the default)  */
+#define HB_FE_CONCRETE       1    /* conf['fe_layer'] = 'concrete'           */
+#define HB_FE_HARD_CONCRETE  2    /* conf['fe_layer'] = 'hard_concrete'      */
+
+typedef struct {                  /* HOST struct */
+  int32_t kind;                   /* HB_FE_*                                                                            */
+  float   temperature;            /* > 0.  stg: its T in fit and predict (conf['temperature'], default 1.0).  Concrete
+                                     layers: predict's T, the last epoch's of the fit's schedule (the constructor's,
+                                     default 0.1, before any epoch)                                                      */
+  double  start_temp;             /* concrete layers: epoch e of a fit uses T = fp32(max(start_temp anneal_base^e,      */
+  double  end_temp;               /*   end_temp)), computed in double and rounded once, as torch.tensor(.).clamp(.)     */
+  double  anneal_base;            /*   rounds it (defaults 1.0, 0.1, 0.99); unused by stg                               */
+  float   mask_reg;               /* conf['mask_reg'] (default 0.1)                                                      */
+} hb_fe_gate_t;
+
+/* P_fe of one gated member, or -1 outside the deep ensemble's envelope (HOST). */
+int64_t hb_fe_num_params(const hb_de_spec_t *spec);
+/* Workspace of hb_fe_fit: 3 E P_fe floats, laid out as hb_de_fit's (Adam's exp_avg, exp_avg_sq, last gradient). */
+int64_t hb_fe_fit_workspace_bytes(const hb_de_spec_t *spec, int64_t E);
+/* hb_de_fit of FeDeepEnsemble (fe_deep_ensemble.py:46-75) in ONE launch, one CTA per member: hb_de_fit's minibatches,
+ * data loss and Adam, with
+ *   - the training mask drawn per minibatch row and input column, applied after the inputs are loaded; the backward
+ *     carries the input delta through the mask into the gate (rows summed in order) and into the embedding tables;
+ *   - the L1 term l1 sum|w| / (n num_out) over the WEIGHTS only (parameters whose name contains 'weight': embedding
+ *     tables, hidden / heads / prior-net weights), not biases or the gate;
+ *   - mask_loss = mask_reg mask_norm / (n num_out) when num_cont > 0 (none otherwise), mask_norm = sum Phi((mu + 0.5) / T)
+ *     (stg) or sum sigmoid(logits) (concrete layers);
+ *   - the concrete layers' temperature set at the start of every epoch (see hb_fe_gate_t).
+ * The rows B = min(n, batch_size) must satisfy, on top of hb_de_fit's formula, the unmasked inputs and gate states:
+ *   B * (in_ld + (num_layers + 2) * hid_ld + 5 * num_out + 1) + 2 * B * in_ld <= HB_DE_MAX_BATCH_FLOATS.
+ *   params [E, P_fe] in/out; perm as hb_de_fit.  draws: NULL, or [E, num_epochs, nb, B, din] raw draws r (nb minibatches
+ *   per epoch) for tests that replay given draws.  With draws = NULL, element q = ((epoch nb + step) B + row) din + column
+ *   of member e's fit takes half q % 2 of the Philox4x32-10 block of counter (q / 2 as 64 bits, member, 0x46454654) under
+ *   `seed` (words 0-1, 2, 3), as a Box-Muller normal (stg, hb_de_predict_batch's pair convention) or the word as a uniform
+ *   (concrete layers); the minibatch order's counters end in 0x44450000 + r, so the two streams never share a block.
+ * Bit-identical from run to run.  No host synchronisation. */
+int32_t hb_fe_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec,
+                  const hb_fe_gate_t *gate, int64_t E, float *params, double lr, float l1, int64_t batch_size,
+                  int64_t num_epochs, const int32_t *perm, const float *draws, uint64_t seed, float *losses, void *ws,
+                  int64_t ws_bytes, void *stream);
+/* hb_de_predict over gated members (member = -1: the ensemble; member >= 0: sample_f's one member, var may be NULL).  Each
+ * member's eval mask is one draw per input column, shared by every candidate row: draws [E, din] device raw draws, or
+ * NULL: column k of member e takes half k % 2 of the Philox4x32-10 block of counter (counter as 64 bits,
+ * (e << 16) | (k / 2), 0x46454556) under `seed`.  A new counter (a GA generation) gives fresh masks, as the reference
+ * redraws them on every call; the same (seed, counter) replays the same bits.  No input gradients.  No host
+ * synchronisation. */
+int32_t hb_fe_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, const hb_fe_gate_t *gate,
+                      int64_t E, const float *params, const float *x_mul, const float *x_add, const float *y_mean,
+                      const float *y_std, int32_t member, const float *draws, uint64_t seed, uint64_t counter, float *mu,
+                      float *var, void *stream);
+
 /* ---- random-forest surrogate (models/rf/rf.py: RF :19-56 over sklearn's RandomForestRegressor defaults) ------------------
  * T regression trees per output, each exact CART (squared error, every feature, min_samples_split 2, min_samples_leaf 1,
  * unlimited depth) grown on bootstrap weights.  Tree inputs are NOT scaled: [Xc | one_hot(Xe)] (rf.py:27-35, layers.py:36),
