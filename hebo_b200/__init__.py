@@ -8,9 +8,9 @@ from .acq import NoisyAcq  # noqa: F401
 from .noisy import NoisyOpt  # noqa: F401
 from .acq import GeneralAcq, MOMeanSigmaLCB  # noqa: F401
 from .general import GeneralBO  # noqa: F401
-from .ensemble import DeepEnsemble, FeDeepEnsemble  # noqa: F401
+from .ensemble import DeepEnsemble, FeDeepEnsemble, GumbelDeepEnsemble  # noqa: F401
 from .forest import RF  # noqa: F401
 
 __all__ = ["GP", "B200GP", "MultiTaskModel", "MACE", "FusedMACE", "Mean", "Sigma", "LCB", "register", "HEBO_Embedding", "MACE_Embedding",
            "AbsEtaDifference", "BO", "NoMR_BO", "HEBO_VectorContextual", "NoisyOpt", "NoisyAcq",
-           "GeneralAcq", "GeneralBO", "MOMeanSigmaLCB", "DeepEnsemble", "FeDeepEnsemble", "RF"]
+           "GeneralAcq", "GeneralBO", "MOMeanSigmaLCB", "DeepEnsemble", "FeDeepEnsemble", "GumbelDeepEnsemble", "RF"]

@@ -155,6 +155,12 @@ SIGNATURES = {
     "hb_fe_fit": (_i32, [_vp, _vp, _vp, _i64, _dsp, _fgp, _i64, _vp, C.c_double, _f32, _i64, _i64, _vp, _vp, _u64, _vp, _vp,
                          _i64, _vp]),
     "hb_fe_predict": (_i32, [_vp, _vp, _i64, _dsp, _fgp, _i64, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _u64, _u64, _vp, _vp, _vp]),
+    "hb_gumbel_num_params": (_i64, [_dsp, _i64]),
+    "hb_gumbel_fit_workspace_bytes": (_i64, [_dsp, _i64, _i64]),
+    "hb_gumbel_fit": (_i32, [_vp, _vp, _vp, _i64, _dsp, _i64, _i64, _vp, C.c_double, _f32, _i64, _i64, _vp, _vp, _u64, _vp,
+                             _vp, _i64, _vp]),
+    "hb_gumbel_predict": (_i32, [_vp, _vp, _i64, _dsp, _i64, _f32, _i64, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _u64, _u64, _vp,
+                                 _vp, _vp, _i64, _vp]),
     "hb_rf_fit_workspace_bytes": (_i64, [_i64, _rsp, _i64, _i64]),
     "hb_rf_forest_bytes": (_i64, [_rsp, _i64, _i64, _i64]),
     "hb_rf_fit": (_i32, [_vp, _vp, _vp, _i64, _rsp, _i64, _i64, _vp, _u64, _vp, _vp, _vp, _i64, _vp]),

@@ -1084,6 +1084,31 @@ int32_t hb_fe_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de
                            var, (cudaStream_t)stream);
 }
 
+// gumbel_linear.py: GumbelNet / GumbelDeepEnsemble, P of one member
+int64_t hb_gumbel_num_params(const hb_de_spec_t *spec, int64_t reduced_dim) { return gb_num_params(spec, reduced_dim); }
+
+int64_t hb_gumbel_fit_workspace_bytes(const hb_de_spec_t *spec, int64_t reduced_dim, int64_t E) {
+  return gb_fit_ws_query(spec, reduced_dim, E);
+}
+
+// deep_ensemble.py:71-93 (the member loop) and GumbelDeepEnsemble.fit_one (gumbel_linear.py:69-100)
+int32_t hb_gumbel_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec,
+                      int64_t reduced_dim, int64_t E, float *params, double lr, float l1, int64_t batch_size,
+                      int64_t num_epochs, const int32_t *perm, const float *draws, uint64_t seed, float *losses, void *ws,
+                      int64_t ws_bytes, void *stream) {
+  return launch_gb_fit(Xc, Xe, y, n, spec, reduced_dim, E, params, lr, l1, batch_size, num_epochs, perm, draws, seed, losses,
+                       ws, ws_bytes, (cudaStream_t)stream);
+}
+
+// deep_ensemble.py:95-116 over GumbelNet members (gumbel_linear.py:58-61)
+int32_t hb_gumbel_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t reduced_dim,
+                          float temperature, int64_t E, const float *params, const float *x_mul, const float *x_add,
+                          const float *y_mean, const float *y_std, int32_t member, const float *draws, uint64_t seed,
+                          uint64_t counter, float *mu, float *var, void *ws, int64_t ws_bytes, void *stream) {
+  return launch_gb_predict(Xs, Xe, m, spec, reduced_dim, temperature, E, params, x_mul, x_add, y_mean, y_std, member, draws,
+                           seed, counter, mu, var, ws, ws_bytes, (cudaStream_t)stream);
+}
+
 // rf.py:19-56: RF over sklearn's RandomForestRegressor (forest.cu)
 int64_t hb_rf_fit_workspace_bytes(int64_t n, const hb_rf_spec_t *spec, int64_t B, int64_t T) {
   return rf_fit_ws_query(n, spec, B, T);

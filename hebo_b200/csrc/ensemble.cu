@@ -139,8 +139,8 @@ __device__ __forceinline__ float de_softplus_d(float z) {
   return e / (e + 1.0f);
 }
 
-// y[p, j] = act(bias[j] + sum_k x[p, k] W[j, k]) (+ add[p, j]) for p < B, j < N; W [N, K] row-major (torch's layout).
-// Lanes run over rows p, so W[j, k] is one broadcast load per warp.
+// y[p, j] = act(bias[j] + sum_k x[p, k] W[j, k]) (+ add[p, j]) for p < B, j < N; W [N, K] row-major (torch's layout);
+// bias NULL: no bias term (F.linear(x, W)).  Lanes run over rows p, so W[j, k] is one broadcast load per warp.
 __device__ void de_dense(const float *x, int ldx, int B, int K, const float *W, const float *bias, int N, float *y, int ldy,
                          bool relu, const float *add = nullptr, int ld_add = 0) {
   for (int idx = threadIdx.x; idx < B * N; idx += blockDim.x) {
@@ -149,7 +149,7 @@ __device__ void de_dense(const float *x, int ldx, int B, int K, const float *W, 
     const float *wr = W + (size_t)j * K;
     float acc = 0.0f;
     for (int k = 0; k < K; ++k) acc = fmaf(xr[k], wr[k], acc);
-    float v = acc + bias[j];
+    float v = bias ? acc + bias[j] : acc;
     if (relu) v = v < 0.0f ? 0.0f : v;
     if (add) v += add[p * ld_add + j];
     y[p * ldy + j] = v;
@@ -159,11 +159,13 @@ __device__ void de_dense(const float *x, int ldx, int B, int K, const float *W, 
 // The input rows of s.rows: numeric columns (scaled as x * x_mul + x_add when x_mul is given), then the embedding rows
 // or one-hot codes of the categorical columns.  A category outside 0 .. u - 1 loads NaN, so its row's outputs are NaN.
 // MASK: every input column k is then multiplied by gmask[k] (a feature gate's eval mask, shared by all rows).
+// Only columns k0 .. din - 1 are loaded (the Gumbel selection writes its columns 0 .. k0 - 1 itself).
 template <bool MASK = false>
 __device__ void de_load_inputs(const DeNet &net, const float *prm, const float *X, const int32_t *Xe, const float *x_mul,
-                               const float *x_add, const DeSmem &s, int B, const float *gmask = nullptr) {
-  for (int idx = threadIdx.x; idx < B * net.din; idx += blockDim.x) {
-    const int p = idx / net.din, k = idx % net.din;
+                               const float *x_add, const DeSmem &s, int B, const float *gmask = nullptr, int k0 = 0) {
+  const int w = net.din - k0;
+  for (int idx = threadIdx.x; idx < B * w; idx += blockDim.x) {
+    const int p = idx / w, k = k0 + idx % w;
     const int64_t r = s.rows[p];
     float v;
     if (k < net.dc) {
@@ -184,10 +186,12 @@ __device__ void de_load_inputs(const DeNet &net, const float *prm, const float *
 
 // BaseNet.forward (deep_ensemble.py:229-238) of the B rows in s.xin: prior net into s.pri (through d0 / d1), hidden
 // activations into s.act, heads into s.head[p, 0:O] = mu (+ prior) and s.head[p, O:2O] = the sigma2 head's pre-softplus z.
-// GATE (FeNet.forward, fe_deep_ensemble.py:29-35): the prior net is built but not evaluated.
+// GATE (FeNet.forward, fe_deep_ensemble.py:29-35): the prior net is built but not evaluated.  DE_GUMBEL (GumbelNet,
+// gumbel_linear.py:58-61) evaluates it on the selected inputs.
+constexpr int DE_GUMBEL = 2 + HB_FE_HARD_CONCRETE;      // the GATE value of the Gumbel selection layer
 template <int GATE = 0>
 __device__ void de_forward(const DeNet &net, const float *prm, const DeSmem &s, int B) {
-  const bool prior = !GATE && net.prior;
+  const bool prior = (GATE == 0 || GATE == DE_GUMBEL) && net.prior;
   if (prior) {
     const float *src = s.xin;
     int ld = net.in_ld, K = net.din;
@@ -394,6 +398,88 @@ __device__ __forceinline__ bool fe_is_weight(const DeNet &net, int i, int off) {
   return !(in(net.mu_b, net.O) || (net.noise && in(net.sg_b, net.O)) || (net.prior && in(net.po_b, net.O)));
 }
 
+// ------------------------------------------------------------------------------------------------ Gumbel selection
+// GumbelNet's feature_select (gumbel_linear.py:21-40) on the dx numeric columns: x_sel = x_num W^T [B, r] with
+// W = RelaxedOneHotCategorical(T, logits).rsample() [r, dx], one W per forward shared by every row.  The member's DeNet is
+// BaseNet's layout with num_cont = r (its input row is [x_sel | embedding or one-hot]); the logits [r, dx] follow it.
+struct GbSel {
+  int off;               // first logit (the selected-width BaseNet's P); a member holds off + r dx floats
+  int dx, r, x_ld;       // numeric columns of the data, selected columns, leading dimension of the on-chip numeric rows
+  float T;               // predict's temperature (the last trained epoch's)
+  const float *draws;    // fit [E, epochs, nb, r, dx] / predict [E, r, dx] uniforms, or NULL: Philox
+  float *w;              // [E, r, dx] each member's W of the current step (fit) or call (predict)
+  uint64_t seed, counter;
+};
+
+constexpr uint32_t GB_TAG_FIT = 0x47424654u;      // upper word of the Philox counter of the training draws ('GBFT')
+constexpr uint32_t GB_TAG_EVAL = 0x47424556u;     // ... and of the eval draws ('GBEV')
+
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// torch.logsumexp of v[0 .. n - 1] over one warp: max, a max of +-inf taken as 0, log(sum exp(v - max)) + max
+__device__ __forceinline__ float gb_warp_lse(const float *v, int n) {
+  const int lane = threadIdx.x & 31;
+  float mx = -INFINITY;
+  for (int k = lane; k < n; k += 32) mx = fmaxf(mx, v[k]);
+  mx = warp_max(mx);
+  if (isinf(mx)) mx = 0.0f;
+  float sm = 0.0f;
+  for (int k = lane; k < n; k += 32) sm += expf(__fsub_rn(v[k], mx));
+  return __fadd_rn(logf(warp_sum(sm)), mx);
+}
+
+// W [r, dx] of one member from its logits and uniforms draw(j, k), one warp per row j, in ExpRelaxedCategorical.rsample's
+// order: L = logits - lse(logits) (Categorical), g = -log(-log(clamp(u, eps, 1 - eps))), s = (L + g) / T (fp32 division
+// by fp32(T), as torch divides an fp32 tensor by a Python float), W = exp(s - lse(s)).
+template <class Draw>
+__device__ void gb_build_w(const float *theta, int r, int dx, float T, float *W, Draw draw) {
+  const int lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  for (int j = threadIdx.x >> 5; j < r; j += nw) {
+    const float *th = theta + (size_t)j * dx;
+    float *w = W + (size_t)j * dx;
+    const float lse = gb_warp_lse(th, dx);
+    for (int k = lane; k < dx; k += 32) {
+      const float u = fminf(fmaxf(draw(j, k), 1.1920928955078125e-07f), 0.99999988079071044921875f);
+      const float g = -logf(-logf(u));
+      w[k] = __fdiv_rn(__fadd_rn(__fsub_rn(th[k], lse), g), T);
+    }
+    __syncwarp();
+    const float ls = gb_warp_lse(w, dx);
+    __syncwarp();
+    for (int k = lane; k < dx; k += 32) w[k] = expf(__fsub_rn(w[k], ls));
+  }
+}
+
+// In place, row by row (one warp each): d = dW [r, dx] -> d loss / d logits through W = exp(s - lse(s)), s = (L + g) / T
+// and L = logits - lse(logits), each logsumexp's backward included (the normalisation terms are not dropped).
+__device__ void gb_logits_grad(const float *theta, const float *W, float *d, int r, int dx, float T) {
+  const int lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  for (int j = threadIdx.x >> 5; j < r; j += nw) {
+    const float *th = theta + (size_t)j * dx, *w = W + (size_t)j * dx;
+    float *dr = d + (size_t)j * dx;
+    float s1 = 0.0f;
+    for (int k = lane; k < dx; k += 32) {
+      const float dz = __fmul_rn(dr[k], w[k]);      // exp's backward
+      dr[k] = dz;
+      s1 += dz;
+    }
+    s1 = -warp_sum(s1);
+    float s2 = 0.0f;
+    for (int k = lane; k < dx; k += 32) {
+      const float dl = __fdiv_rn(__fadd_rn(dr[k], __fmul_rn(s1, w[k])), T);
+      dr[k] = dl;
+      s2 += dl;
+    }
+    s2 = -warp_sum(s2);
+    const float lse = gb_warp_lse(th, dx);
+    for (int k = lane; k < dx; k += 32) dr[k] = __fadd_rn(dr[k], __fmul_rn(s2, expf(__fsub_rn(th[k], lse))));
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ fit
 struct DeFitArgs {
   const float *Xc, *y;
@@ -406,14 +492,20 @@ struct DeFitArgs {
 };
 
 // The whole fit of one member: a's pointers are its ensemble's (params [E, P], m1 / m2 / grad [E, P], losses [E, epochs]).
+// Step bi takes rows bi B .. min((bi + 1) B, n) - 1 of the epoch's order, so a.nb decides whether a partial last
+// minibatch is trained (a.nb = ceil(n / B)) or dropped.
 // GATE: FeDeepEnsemble.fit_one (fe_deep_ensemble.py:46-75) with fe's gate; the unmasked inputs and the gate states of the
-// minibatch sit in two more [B, in_ld] buffers after the scratch.
+// minibatch sit in two more [B, in_ld] buffers after the scratch.  DE_GUMBEL: GumbelDeepEnsemble.fit_one
+// (gumbel_linear.py:69-100) with gb's selection layer; the numeric rows sit in one [B, x_ld] buffer after the scratch.
 template <int GATE = 0>
 __device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs &a, int member, float *smem,
-                                              const FeGate *fe = nullptr) {
+                                              const FeGate *fe = nullptr, const GbSel *gb = nullptr) {
   const int B = a.B, O = net.O;
   const DeSmem s = de_carve(net, smem, B);
   float *xraw = s.red + DE_SCRATCH, *gst = xraw + B * net.in_ld;
+  constexpr bool GUMBEL = GATE == DE_GUMBEL;
+  const int wsz = GUMBEL ? gb->r * gb->dx : 0;
+  float *W = GUMBEL ? gb->w + (size_t)member * wsz : nullptr;
   float *prm = a.params + (size_t)member * net.P;
   float *m1 = a.m1 + (size_t)member * net.P, *m2 = a.m2 + (size_t)member * net.P, *g = a.grad + (size_t)member * net.P;
   for (int i = threadIdx.x; i < net.P; i += blockDim.x) {
@@ -426,17 +518,38 @@ __device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs 
     float epoch_loss = 0.0f;     // thread 0
     float T = 0.0f;
     if constexpr (GATE == 1 + HB_FE_STG) T = fe->T;
+    else if constexpr (GUMBEL) T = (float)(pow(0.8, (double)ep) + 0.1);     // 0.8**epoch + 0.1, a double, used as fp32
     else if constexpr (GATE != 0) T = (float)fmax(fe->t0 * pow(fe->tb, (double)ep), fe->t1);     // torch.tensor(.).clamp(end)
     for (int bi = 0; bi < a.nb; ++bi) {
       ++step;
-      for (int p = threadIdx.x; p < B; p += blockDim.x) {
+      const int Bs = min(B, a.n - bi * B);      // rows of this step
+      for (int p = threadIdx.x; p < Bs; p += blockDim.x) {
         const int pos = bi * B + p;
         s.rows[p] = a.perm ? a.perm[((size_t)member * a.epochs + ep) * a.n + pos] : de_perm(pos, a.n, a.h, a.seed, ep, member);
       }
       __syncthreads();
-      de_load_inputs(net, prm, a.Xc, a.Xe, nullptr, nullptr, s, B);
+      if constexpr (GUMBEL) {
+        if (gb->dx > 0) {       // this step's W from fresh uniforms, then x_sel = x_num W^T; x_num stays for the backward
+          const int dx = gb->dx, r = gb->r;
+          const size_t base = (((size_t)member * a.epochs + ep) * a.nb + bi) * (size_t)wsz;
+          const uint64_t q0 = ((uint64_t)ep * a.nb + bi) * (uint64_t)wsz;
+          gb_build_w(prm + gb->off, r, dx, T, W, [&](int j, int k) {
+            const uint64_t q = q0 + (uint64_t)j * dx + k;
+            return gb->draws ? gb->draws[base + (size_t)j * dx + k]
+                             : fe_draw<1 + HB_FE_CONCRETE>(a.seed, q >> 1, ((uint64_t)GB_TAG_FIT << 32) | (uint32_t)member,
+                                                           (int)(q & 1));
+          });
+          for (int idx = threadIdx.x; idx < Bs * dx; idx += blockDim.x)
+            xraw[(idx / dx) * gb->x_ld + idx % dx] = a.Xc[(int64_t)s.rows[idx / dx] * dx + idx % dx];
+          __syncthreads();
+          de_dense(xraw, gb->x_ld, Bs, dx, W, nullptr, r, s.xin, net.in_ld, false);
+        }
+        de_load_inputs(net, prm, a.Xc, a.Xe, nullptr, nullptr, s, Bs, nullptr, net.dc);
+      } else {
+        de_load_inputs(net, prm, a.Xc, a.Xe, nullptr, nullptr, s, Bs);
+      }
       __syncthreads();
-      if constexpr (GATE != 0) {       // x * mask with a fresh draw per row and column (the training mask of x.shape)
+      if constexpr (GATE != 0 && !GUMBEL) {       // x * mask with a fresh draw per row and column (the training mask of x.shape)
         const size_t base = (((size_t)member * a.epochs + ep) * a.nb + bi) * (size_t)B * net.din;
         for (int idx = threadIdx.x; idx < B * net.din; idx += blockDim.x) {
           const int p = idx / net.din, k = idx % net.din;
@@ -450,17 +563,17 @@ __device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs 
         }
         __syncthreads();
       }
-      de_forward<GATE>(net, prm, s, B);
+      de_forward<GATE>(net, prm, s, Bs);
       // the loss over the finite entries of y (loss_likelihood / loss_mse, deep_ensemble.py:140-149)
       if (threadIdx.x < 32) {
         float cnt = 0.0f;
-        for (int i = threadIdx.x; i < B * O; i += 32) cnt += isfinite(a.y[(int64_t)s.rows[i / O] * O + i % O]) ? 1.0f : 0.0f;
+        for (int i = threadIdx.x; i < Bs * O; i += 32) cnt += isfinite(a.y[(int64_t)s.rows[i / O] * O + i % O]) ? 1.0f : 0.0f;
         cnt = warp_sum(cnt);
         if (threadIdx.x == 0) s.red[0] = cnt;
       }
       __syncthreads();
       const float cnt = s.red[0];
-      for (int i = threadIdx.x; i < B * O; i += blockDim.x) {
+      for (int i = threadIdx.x; i < Bs * O; i += blockDim.x) {
         const int p = i / O, o = i % O;
         const float t = a.y[(int64_t)s.rows[p] * O + o];
         float el = 0.0f, gmu = 0.0f, gz = 0.0f;
@@ -484,12 +597,27 @@ __device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs 
       __syncthreads();
       if (threadIdx.x < 32) {
         float sum = 0.0f;
-        for (int i = threadIdx.x; i < B * O; i += 32) sum += s.pri[i];
+        for (int i = threadIdx.x; i < Bs * O; i += 32) sum += s.pri[i];
         sum = warp_sum(sum);
-        if (threadIdx.x == 0) epoch_loss += sum / cnt * (float)B;      // epoch_loss += data_loss * bxc.shape[0]
+        if (threadIdx.x == 0) epoch_loss += sum / cnt * (float)Bs;      // epoch_loss += data_loss * bxc.shape[0]
       }
-      float *dx = GATE ? de_backward(net, prm, s, B, g, true, 0) : de_backward(net, prm, s, B, g, net.emb && net.ne > 0, net.dc);
-      if constexpr (GATE != 0) {
+      const bool sel = GUMBEL && gb->dx > 0;
+      float *dx = GATE && !GUMBEL ? de_backward(net, prm, s, Bs, g, true, 0)
+                                  : de_backward(net, prm, s, Bs, g, sel || (net.emb && net.ne > 0), sel ? 0 : net.dc);
+      if (sel) {
+        // d loss / d W [j, k] = sum over the rows in order of delta_sel[p, j] x_num[p, k], then through the softmax
+        const int dx_ = gb->dx;
+        for (int idx = threadIdx.x; idx < wsz; idx += blockDim.x) {
+          const int j = idx / dx_, k = idx % dx_;
+          float acc = 0.0f;
+          for (int p = 0; p < Bs; ++p) acc = fmaf(dx[p * net.h_ld + j], xraw[p * gb->x_ld + k], acc);
+          g[gb->off + idx] = acc;
+        }
+        __syncthreads();
+        gb_logits_grad(prm + gb->off, W, g + gb->off, gb->r, dx_, T);
+        __syncthreads();
+      }
+      if constexpr (GATE != 0 && !GUMBEL) {
         // column k: d loss / d theta_k = sum over rows in order of (dx x) through the mask, plus the mask penalty's;
         // then dx becomes the delta of the unmasked input (dx mask) for the embedding tables
         for (int k = threadIdx.x; k < net.din; k += blockDim.x) {
@@ -512,7 +640,7 @@ __device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs 
           for (int idx = threadIdx.x; idx < tab; idx += blockDim.x) {
             const int u = idx / wc, q = idx % wc;
             float acc = 0.0f;
-            for (int p = 0; p < B; ++p)
+            for (int p = 0; p < Bs; ++p)
               if (a.Xe[(int64_t)s.rows[p] * net.ne + c] == u) acc += dx[p * net.h_ld + net.dc + net.col_in[c] + q];
             g[net.col_tab[c] + idx] = acc;
           }
@@ -528,8 +656,9 @@ __device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs 
         const float sg = p > 0.0f ? 1.0f : (p < 0.0f ? -1.0f : 0.0f);
         float gd, gt;
         if constexpr (GATE != 0) {      // L1 over the weights only; the prior net's biases keep gt = 0 and do not move
-          gd = (i < net.prior0 || i >= fe->off) ? g[i] : 0.0f;
-          gt = fe_is_weight(net, i, fe->off) ? __fadd_rn(gd, __fmul_rn(a.coef, sg)) : gd;
+          const int off = GUMBEL ? gb->off : fe->off;
+          gd = (i < net.prior0 || i >= off) ? g[i] : 0.0f;
+          gt = fe_is_weight(net, i, off) ? __fadd_rn(gd, __fmul_rn(a.coef, sg)) : gd;
         } else {
           gd = i < net.prior0 ? g[i] : 0.0f;
           gt = __fadd_rn(gd, __fmul_rn(a.coef, sg));
@@ -558,6 +687,12 @@ __global__ void __launch_bounds__(DE_FIT_THREADS) fe_fit_kernel(const __grid_con
                                                                 const __grid_constant__ FeGate fe) {
   extern __shared__ float smem[];
   de_fit_member<GATE>(net, a, blockIdx.x, smem, &fe);
+}
+
+__global__ void __launch_bounds__(DE_FIT_THREADS) gb_fit_kernel(const __grid_constant__ DeNet net, const DeFitArgs a,
+                                                                const __grid_constant__ GbSel gb) {
+  extern __shared__ float smem[];
+  de_fit_member<DE_GUMBEL>(net, a, blockIdx.x, smem, nullptr, &gb);
 }
 
 // Per-ensemble arguments of hb_de_fit_batch: its rows [off, off + n) of the concatenated inputs and what follows from n
@@ -609,17 +744,29 @@ struct DePredArgs {
 
 // Rows r0 .. r0 + DE_TM - 1 of the candidates (the last one repeated past m) through members e0 .. e1 - 1: the heads mu
 // into mus[e - e0][p, o] and, with output_noise, sigma2 into s2s[e - e0][p, o].  GATE: member e's eval mask [din] (one
-// draw per column, shared by every row) goes to gmask and multiplies the inputs in the load.
+// draw per column, shared by every row) goes to gmask and multiplies the inputs in the load.  DE_GUMBEL: the tile's
+// scaled numeric rows go to gmask [B, x_ld] once, and member e's x_sel takes its W of the call, gb->w [e].
 template <int GATE = 0>
 __device__ __forceinline__ void de_member_heads(const DeNet &net, const DePredArgs &a, const DeSmem &s, int r0, int e0,
                                                 int e1, float *mus, float *s2s, const FeGate *fe = nullptr,
-                                                float *gmask = nullptr) {
+                                                float *gmask = nullptr, const GbSel *gb = nullptr) {
   const int O = net.O, B = DE_TM;
   for (int p = threadIdx.x; p < B; p += blockDim.x) s.rows[p] = min(r0 + p, a.m - 1);
   __syncthreads();
+  if constexpr (GATE == DE_GUMBEL) {
+    const int dx = gb->dx;
+    for (int idx = threadIdx.x; idx < B * dx; idx += blockDim.x) {
+      const int p = idx / dx, k = idx % dx;
+      gmask[p * gb->x_ld + k] = __fadd_rn(__fmul_rn(a.x_mul[k], a.Xs[(int64_t)s.rows[p] * dx + k]), a.x_add[k]);
+    }
+    __syncthreads();
+  }
   for (int e = e0; e < e1; ++e) {
     const float *prm = a.params + (size_t)e * net.P;
-    if constexpr (GATE != 0) {
+    if constexpr (GATE == DE_GUMBEL) {
+      if (gb->dx > 0) de_dense(gmask, gb->x_ld, B, gb->dx, gb->w + (size_t)e * gb->r * gb->dx, nullptr, gb->r, s.xin, net.in_ld, false);
+      de_load_inputs(net, prm, a.Xs, a.Xe, a.x_mul, a.x_add, s, B, nullptr, net.dc);
+    } else if constexpr (GATE != 0) {
       for (int k = threadIdx.x; k < net.din; k += blockDim.x) {
         const uint64_t stream = ((uint64_t)FE_TAG_EVAL << 32) | ((uint32_t)e << 16) | (uint32_t)(k >> 1);
         const float r = fe->draws ? fe->draws[(size_t)e * net.din + k] : fe_draw<GATE>(fe->seed, fe->counter, stream, k & 1);
@@ -668,17 +815,19 @@ __device__ __forceinline__ void de_combine(const DeNet &net, const float *mus, c
   }
 }
 
-// GATE: fe's gate on every member (no input gradients: FeDeepEnsemble.support_grad = False); the eval mask sits after py
+// GATE: fe's gate on every member (no input gradients: FeDeepEnsemble.support_grad = False); the eval mask sits after py.
+// DE_GUMBEL: gb's selection on every member (no input gradients either); the numeric rows sit after py.
 template <bool GRAD, int GATE = 0>
 __global__ void __launch_bounds__(DE_PRED_THREADS) de_predict_kernel(const __grid_constant__ DeNet net, const DePredArgs a,
-                                                                     const __grid_constant__ FeGate fe) {
+                                                                     const __grid_constant__ FeGate fe,
+                                                                     const __grid_constant__ GbSel gb) {
   static_assert(!(GRAD && GATE), "the gated ensemble has no input gradients");
   extern __shared__ float smem[];
   const int O = net.O, B = DE_TM, r0 = blockIdx.x * DE_TM;
   const DeSmem s = de_carve(net, smem, B);
   const int e0 = a.member >= 0 ? a.member : 0, e1 = a.member >= 0 ? a.member + 1 : a.E, ne = e1 - e0;
   float *mus = s.red + DE_SCRATCH, *s2s = mus + ne * B * O, *py = s2s + ne * B * O;
-  de_member_heads<GATE>(net, a, s, r0, e0, e1, mus, s2s, &fe, py + B * O);
+  de_member_heads<GATE>(net, a, s, r0, e0, e1, mus, s2s, &fe, py + B * O, &gb);
   for (int i = threadIdx.x; i < B * O; i += blockDim.x) {
     const int p = i / O, o = i % O, row = r0 + p;
     float mean, v;
@@ -873,10 +1022,10 @@ int launch_de_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de
   const unsigned grid = (unsigned)ceil_div(m, DE_TM);
   if (grad) {
     HB_CUDA(cudaFuncSetAttribute(de_predict_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    de_predict_kernel<true><<<grid, DE_PRED_THREADS, smem, st>>>(net, a, FeGate{});
+    de_predict_kernel<true><<<grid, DE_PRED_THREADS, smem, st>>>(net, a, FeGate{}, GbSel{});
   } else {
     HB_CUDA(cudaFuncSetAttribute(de_predict_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    de_predict_kernel<false><<<grid, DE_PRED_THREADS, smem, st>>>(net, a, FeGate{});
+    de_predict_kernel<false><<<grid, DE_PRED_THREADS, smem, st>>>(net, a, FeGate{}, GbSel{});
   }
   count_launches(1);
   HB_LAUNCH_CHECK("de_predict_kernel");
@@ -1058,7 +1207,7 @@ template <int GATE>
 static int fe_predict_launch(const DeNet &net, const DePredArgs &a, const FeGate &fe, unsigned grid, size_t smem,
                               cudaStream_t st) {
   HB_CUDA(cudaFuncSetAttribute(de_predict_kernel<false, GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  de_predict_kernel<false, GATE><<<grid, DE_PRED_THREADS, smem, st>>>(net, a, fe);
+  de_predict_kernel<false, GATE><<<grid, DE_PRED_THREADS, smem, st>>>(net, a, fe, GbSel{});
   return HB_OK;
 }
 
@@ -1101,6 +1250,147 @@ int launch_fe_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de
   if (rc != HB_OK) return rc;
   count_launches(1);
   HB_LAUNCH_CHECK("de_predict_kernel (gated)");
+  return HB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ Gumbel launchers
+// GumbelDeepEnsemble's member: BaseNet's layout over the selected width (num_cont -> r when num_cont > 0), then the
+// logits [r, num_cont] last.  The random prior net keeps the original width, so it only runs when r = num_cont or there
+// are no numeric columns; anything else is rejected (the reference fails with a shape error in forward).
+static bool gb_layout(const hb_de_spec_t *spec, int64_t r, DeNet &net, GbSel &gb) {
+  if (!spec || r < 1 || r > HB_DE_MAX_IN || spec->num_cont < 0 || spec->num_cont > HB_DE_MAX_IN) return false;
+  const int dx = spec->num_cont;
+  if (spec->rand_prior && dx > 0 && r != dx) return false;
+  hb_de_spec_t sel = *spec;
+  if (dx > 0) sel.num_cont = (int32_t)r;
+  if (!de_layout(&sel, net)) return false;
+  gb = GbSel{};
+  gb.off = net.P;
+  gb.dx = dx;
+  gb.r = dx > 0 ? (int)r : 0;      // without numeric columns the logits [r, 0] are empty and nothing is drawn
+  gb.x_ld = dx > 0 ? (dx | 1) : 0;
+  net.P += gb.r * dx;
+  return true;
+}
+
+// floats of a Gumbel fit's minibatch buffers: BaseNet's over the selected width plus the numeric rows, B x_ld
+static int64_t gb_rows_floats(const DeNet &net, const GbSel &gb, int64_t B) { return de_rows_floats(net, B) + B * gb.x_ld; }
+
+int64_t gb_num_params(const hb_de_spec_t *spec, int64_t reduced_dim) {
+  DeNet net;
+  GbSel gb;
+  return gb_layout(spec, reduced_dim, net, gb) ? net.P : -1;
+}
+
+int64_t gb_fit_ws_query(const hb_de_spec_t *spec, int64_t reduced_dim, int64_t E) {
+  DeNet net;
+  GbSel gb;
+  if (!gb_layout(spec, reduced_dim, net, gb) || E < 1 || E > HB_DE_MAX_MEMBERS) return -1;
+  return (3 * E * (int64_t)net.P + E * (int64_t)gb.r * gb.dx) * (int64_t)sizeof(float);
+}
+
+int launch_gb_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec,
+                  int64_t reduced_dim, int64_t E, float *params, double lr, float l1, int64_t batch_size, int64_t num_epochs,
+                  const int32_t *perm, const float *draws, uint64_t seed, float *losses, void *ws, int64_t ws_bytes,
+                  cudaStream_t st) {
+  DeNet net;
+  GbSel gb;
+  if (!gb_layout(spec, reduced_dim, net, gb) || E < 1 || E > HB_DE_MAX_MEMBERS || n < 1 || n > (1 << 30) ||
+      batch_size < 1 || num_epochs < 0)
+    return HB_ERR_INVALID;
+  if (!y || !params || !ws || (num_epochs > 0 && !losses) || (gb.dx > 0 && !Xc) || (net.ne > 0 && !Xe)) return HB_ERR_INVALID;
+  if (ws_bytes < gb_fit_ws_query(spec, reduced_dim, E)) return HB_ERR_INVALID;
+  const int64_t B = n > batch_size ? batch_size : n;
+  if (gb_rows_floats(net, gb, B) > HB_DE_MAX_BATCH_FLOATS) return HB_ERR_INVALID;
+  if (num_epochs == 0) return HB_OK;
+  DeFitArgs a;
+  a.Xc = Xc;
+  a.Xe = Xe;
+  a.y = y;
+  a.perm = perm;
+  a.params = params;
+  a.m1 = (float *)ws;
+  a.m2 = a.m1 + E * net.P;
+  a.grad = a.m2 + E * net.P;
+  a.losses = losses;
+  a.n = (int)n;
+  a.B = (int)B;
+  a.nb = (int)((n + B - 1) / B);      // no drop_last (gumbel_linear.py:72): the partial last minibatch is trained
+  a.epochs = (int)num_epochs;
+  int h = 1;
+  while ((int64_t(1) << (2 * h)) < n) ++h;
+  a.h = h;
+  a.seed = seed;
+  a.lr = lr;
+  a.coef = (1.0f / (float)(n * net.O)) * l1;
+  gb.draws = draws;
+  gb.w = a.grad + E * net.P;
+  const size_t smem = (size_t)(gb_rows_floats(net, gb, B) + DE_SCRATCH) * sizeof(float);
+  HB_CUDA(cudaFuncSetAttribute(gb_fit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  gb_fit_kernel<<<(unsigned)E, DE_FIT_THREADS, smem, st>>>(net, a, gb);
+  count_launches(1);
+  HB_LAUNCH_CHECK("gb_fit_kernel");
+  return HB_OK;
+}
+
+// W of members e0 + blockIdx.x for one predict call: uniforms from gb.draws [E, r, dx] or Philox keyed by
+// (seed, counter, member), so every candidate tile of the call uses the same W
+__global__ void __launch_bounds__(DE_PRED_THREADS) gb_weights_kernel(const float *params, int P, int e0,
+                                                                     const __grid_constant__ GbSel gb) {
+  const int e = e0 + blockIdx.x, wsz = gb.r * gb.dx;
+  gb_build_w(params + (size_t)e * P + gb.off, gb.r, gb.dx, gb.T, gb.w + (size_t)e * wsz, [&](int j, int k) {
+    const int q = j * gb.dx + k;
+    const uint64_t stream = ((uint64_t)GB_TAG_EVAL << 32) | ((uint32_t)e << 16) | (uint32_t)(q >> 1);
+    return gb.draws ? gb.draws[(size_t)e * wsz + q] : fe_draw<1 + HB_FE_CONCRETE>(gb.seed, gb.counter, stream, q & 1);
+  });
+}
+
+int launch_gb_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t reduced_dim,
+                      float temperature, int64_t E, const float *params, const float *x_mul, const float *x_add,
+                      const float *y_mean, const float *y_std, int32_t member, const float *draws, uint64_t seed,
+                      uint64_t counter, float *mu, float *var, void *ws, int64_t ws_bytes, cudaStream_t st) {
+  DeNet net;
+  GbSel gb;
+  if (!gb_layout(spec, reduced_dim, net, gb) || !(temperature > 0.0f) || E < 1 || E > HB_DE_MAX_MEMBERS || m < 0 ||
+      m > (int64_t(1) << 31) - DE_TM)
+    return HB_ERR_INVALID;
+  if (member < -1 || member >= E) return HB_ERR_INVALID;
+  if (!params || !y_mean || !y_std || !mu || (member < 0 && !var) || (net.ne > 0 && !Xe)) return HB_ERR_INVALID;
+  if (gb.dx > 0 && (!Xs || !x_mul || !x_add || !ws || ws_bytes < E * (int64_t)gb.r * gb.dx * (int64_t)sizeof(float)))
+    return HB_ERR_INVALID;
+  if (m == 0) return HB_OK;
+  DePredArgs a;
+  a.Xs = Xs;
+  a.Xe = Xe;
+  a.params = params;
+  a.x_mul = x_mul;
+  a.x_add = x_add;
+  a.y_mean = y_mean;
+  a.y_std = y_std;
+  a.mu = mu;
+  a.var = var;
+  a.dmu = a.dvar = nullptr;
+  a.m = (int)m;
+  a.E = (int)E;
+  a.member = member;
+  gb.T = temperature;
+  gb.draws = draws;
+  gb.seed = seed;
+  gb.counter = counter;
+  gb.w = (float *)ws;
+  const int64_t ne = member >= 0 ? 1 : E;
+  if (gb.dx > 0) {
+    gb_weights_kernel<<<(unsigned)ne, DE_PRED_THREADS, 0, st>>>(params, net.P, member >= 0 ? member : 0, gb);
+    count_launches(1);
+    HB_LAUNCH_CHECK("gb_weights_kernel");
+  }
+  const size_t smem =
+      (size_t)(de_rows_floats(net, DE_TM) + DE_SCRATCH + (2 * ne + 1) * DE_TM * net.O + DE_TM * gb.x_ld) * sizeof(float);
+  const unsigned grid = (unsigned)ceil_div(m, DE_TM);
+  HB_CUDA(cudaFuncSetAttribute(de_predict_kernel<false, DE_GUMBEL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  de_predict_kernel<false, DE_GUMBEL><<<grid, DE_PRED_THREADS, smem, st>>>(net, a, FeGate{}, gb);
+  count_launches(1);
+  HB_LAUNCH_CHECK("de_predict_kernel (Gumbel)");
   return HB_OK;
 }
 

@@ -253,6 +253,17 @@ int launch_fe_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de
                       int64_t E, const float *params, const float *x_mul, const float *x_add, const float *y_mean,
                       const float *y_std, int32_t member, const float *draws, uint64_t seed, uint64_t counter, float *mu,
                       float *var, cudaStream_t st);
+// the Gumbel-selection ensemble (GumbelDeepEnsemble): the same fit and predict kernels with the selection layer compiled in
+int64_t gb_num_params(const hb_de_spec_t *spec, int64_t reduced_dim);
+int64_t gb_fit_ws_query(const hb_de_spec_t *spec, int64_t reduced_dim, int64_t E);
+int launch_gb_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec,
+                  int64_t reduced_dim, int64_t E, float *params, double lr, float l1, int64_t batch_size, int64_t num_epochs,
+                  const int32_t *perm, const float *draws, uint64_t seed, float *losses, void *ws, int64_t ws_bytes,
+                  cudaStream_t st);
+int launch_gb_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t reduced_dim,
+                      float temperature, int64_t E, const float *params, const float *x_mul, const float *x_add,
+                      const float *y_mean, const float *y_std, int32_t member, const float *draws, uint64_t seed,
+                      uint64_t counter, float *mu, float *var, void *ws, int64_t ws_bytes, cudaStream_t st);
 
 // hypervolume.cu: GeneralBO's Monte-Carlo EHVI selection round, bit for bit with general.hypervolume
 int64_t ehvi_ws_query(int64_t n, int64_t K, int64_t m, int64_t n_mc);

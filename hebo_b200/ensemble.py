@@ -266,9 +266,13 @@ class DeepEnsemble(BaseModel):
                 f"DeepEnsemble: a minibatch of {rows} rows needs {self.batch_floats(rows)} floats of on-chip buffers, over "
                 f"the limit of {_lib.HB_DE_MAX_BATCH_FLOATS} (HB_DE_MAX_BATCH_FLOATS); use a smaller batch_size")
         if self.params is None:
-            self.params = torch.stack([init_params(self.layout) for _ in range(E)]).to(dev).contiguous()
+            self.params = torch.stack([self.init_member() for _ in range(E)]).to(dev).contiguous()
         self.seed = int(torch.randint(0, 2 ** 62, (1,)).item())     # the Philox key of this fit's minibatch order
         return Xc, Xe, y, valid
+
+    def init_member(self) -> torch.Tensor:
+        """One member's initial raw parameters [P] from torch's global generator."""
+        return init_params(self.layout)
 
     def _finish_fit(self, Xc_, Xe_, y_, valid, **predict_kw):
         """fit's host side after the launch: the noise estimate on the kept rows (deep_ensemble.py:89-93); predict_kw
@@ -438,6 +442,9 @@ class EnsembleBatch:
         assert all(m.fitted for m in models), "fit() first"
         if any(isinstance(m, FeDeepEnsemble) for m in models):
             raise TypeError("EnsembleBatch: a FeDeepEnsemble predicts through hb_fe_predict, which applies its gate")
+        if any(isinstance(m, GumbelDeepEnsemble) for m in models):
+            raise TypeError("EnsembleBatch: a GumbelDeepEnsemble predicts through hb_gumbel_predict, which applies its "
+                            "selection layer")
         self.models, self.spec, self.E, self.device = models, m0._spec, m0.num_ensembles, m0.device
         self.num_cont, self.num_out = m0.num_cont, len(models) * m0.num_out
         self.params = _stacked_params(models)
@@ -648,5 +655,158 @@ def _reference_fenet():
     try:  # pragma: no cover - depends on the environment
         from hebo.models.nn.fe_deep_ensemble import FeNet
         return FeNet
+    except Exception:
+        return None
+
+
+def gumbel_epoch_temperature(epoch: int) -> float:
+    """GumbelDeepEnsemble.fit_one's temperature of an epoch (gumbel_linear.py:81), a double that torch uses as fp32(T)."""
+    return float(np.float32(0.8 ** epoch + 0.1))
+
+
+class GumbelDeepEnsemble(DeepEnsemble):
+    """Drop-in for ``hebo.models.nn.gumbel_linear.GumbelDeepEnsemble``: a DeepEnsemble whose members map their numeric
+    columns to ``reduced_dim`` learned soft selections of them (a Gumbel-softmax selection layer, one draw of its
+    [reduced_dim, num_cont] matrix per forward) before the first hidden layer.  The fit runs in one ``hb_gumbel_fit``
+    launch and prediction in ``hb_gumbel_predict`` (hebo_b200/csrc/ensemble.cu, the deep ensemble's kernels with the
+    selection layer compiled in).
+
+    Extra conf key and default: reduced_dim = num_cont // 2 + 1.  A member's parameters are GumbelNet's state_dict in
+    order: BaseNet's over the selected width, then ``feature_select.logits`` [reduced_dim, num_cont] last.  The hidden
+    layers (rebuilt by GumbelNet when num_cont > 0) keep torch's default nn.Linear initialisation, the logits start at
+    zero.  Every epoch's minibatches cover all rows (no drop_last); the L1 term covers weights only; the temperature is
+    0.8**epoch + 0.1.  The random prior net (rand_prior) needs reduced_dim == num_cont or no numeric columns.
+
+    The selection is random in predict too (the reference redraws it on every forward): each call draws one matrix per
+    member from a Philox key taken from torch's global generator, or from the given ``seed`` / ``counter``, at the last
+    trained epoch's temperature.  No input gradients (``support_grad = False``).  Like DeepEnsemble, the fit does not
+    call ``torch.seed()``, a deliberate deviation that keeps it reproducible under ``torch.manual_seed``."""
+    support_grad = False
+
+    def __init__(self, num_cont, num_enum, num_out, **conf):
+        conf.pop("basenet_cls", None)
+        self.reduced_dim = int(conf.setdefault("reduced_dim", num_cont // 2 + 1))
+        if self.reduced_dim < 1:
+            raise NotImplementedError("GumbelDeepEnsemble: reduced_dim must be at least 1")
+        if conf.get("rand_prior", False) and num_cont > 0 and self.reduced_dim != num_cont:
+            raise NotImplementedError("GumbelDeepEnsemble: rand_prior needs reduced_dim == num_cont (the prior net keeps the "
+                                      "unselected input width, so the reference fails in forward)")
+        if num_cont > _lib.HB_DE_MAX_IN:
+            raise NotImplementedError(f"GumbelDeepEnsemble: num_cont = {num_cont} exceeds the limit of {_lib.HB_DE_MAX_IN}")
+        super().__init__(num_cont, num_enum, num_out, **conf)
+        self.basenet_cls = _reference_gumbelnet()
+        self.conf["basenet_cls"] = self.basenet_cls
+        self.temperature = 0.1          # GumbelSelectionLayer's default until a fit sets the last epoch's
+
+    def _check_envelope(self):
+        """GumbelNet's layout replaces BaseNet's here, before DeepEnsemble's envelope check and parameter count read it:
+        BaseNet's over the selected width (num_cont -> reduced_dim when num_cont > 0), then the logits."""
+        sel = self.reduced_dim if self.num_cont > 0 else 0
+        lay, self.din = param_layout(sel, self.num_uniqs, self.enum_trans, self.num_layers, self.num_hiddens, self.num_out,
+                                     self.output_noise, self.rand_prior)
+        self.layout = lay + [("feature_select.logits", (self.reduced_dim, self.num_cont))]
+        super()._check_envelope()
+
+    def batch_floats(self, rows: int) -> int:
+        """On-chip floats of a minibatch: the deep ensemble's over the selected width plus the numeric rows."""
+        return super().batch_floats(rows) + (rows * (self.num_cont | 1) if self.num_cont > 0 else 0)
+
+    def draws_shape(self, n: int):
+        """Shape of fit's explicit training uniforms for n kept rows: [E, num_epochs, ceil(n / batch), r, num_cont]."""
+        bs = min(n, int(self.batch_size))
+        return (self.num_ensembles, int(self.num_epochs), -(-n // bs), self.reduced_dim, self.num_cont)
+
+    def init_member(self) -> torch.Tensor:
+        """GumbelNet's initialisation from torch's global generator: BaseNet's (xavier with the ReLU gain, zero biases) over
+        its own layout; with numeric columns the hidden layers are then rebuilt with nn.Linear's default initialisation
+        (kaiming-uniform weights, U(+-1/sqrt(fan_in)) biases), and the logits are zeros."""
+        full, _ = param_layout(self.num_cont, self.num_uniqs, self.enum_trans, self.num_layers, self.num_hiddens,
+                               self.num_out, self.output_noise, self.rand_prior)
+        base = raw_to_state_dict(init_params(full), full)
+        if self.num_cont > 0:
+            k = self.din
+            for l in range(self.num_layers):
+                lin = nn.Linear(k, self.num_hiddens)
+                base[f"hidden.{2 * l}.weight"], base[f"hidden.{2 * l}.bias"] = lin.weight.detach(), lin.bias.detach()
+                k = self.num_hiddens
+        base["feature_select.logits"] = torch.zeros(self.reduced_dim, self.num_cont)
+        return state_dict_to_raw(base, self.layout)
+
+    # ------------------------------------------------------------------ fit (gumbel_linear.py:69-100)
+    def fit(self, Xc_, Xe_, y_, perm=None, draws=None, eval_draws=None):
+        """perm: as DeepEnsemble.fit.  draws: optional training uniforms (``draws_shape``); otherwise Philox draws on the
+        device.  eval_draws: optional [E, reduced_dim, num_cont] uniforms of the noise estimate's predict (tests replaying
+        the reference's own draws)."""
+        Xc, Xe, y, valid = self._prepare_fit(Xc_, Xe_, y_, perm)
+        if draws is not None:
+            draws = torch.as_tensor(draws, dtype=torch.float32)
+            if tuple(draws.shape) != self.draws_shape(y.shape[0]):
+                raise ValueError(f"draws must be {list(self.draws_shape(y.shape[0]))}, got {list(draws.shape)}")
+        self._fit_dev(Xc, Xe, y, perm, self.seed, draws)
+        self._finish_fit(Xc_, Xe_, y_, valid, draws=eval_draws)
+
+    def _fit_dev(self, Xc, Xe, y, perm, seed, draws=None):
+        lib, dev, E = _lib.lib(), self.device, self.num_ensembles
+        n, T = y.shape[0], int(self.num_epochs)
+        xc = Xc.to(dev, torch.float32).contiguous() if self.num_cont > 0 else None
+        xe = Xe.to(dev, torch.int32).contiguous() if self.num_enum > 0 else None
+        yd = y.to(dev, torch.float32).contiguous()
+        pd_ = None if perm is None else torch.as_tensor(perm).to(dev, torch.int32).contiguous()
+        dd = None if draws is None else draws.to(dev, torch.float32).contiguous()
+        r = self.reduced_dim
+        need = int(lib.hb_gumbel_fit_workspace_bytes(C.byref(self._spec), r, E))
+        self.fit_ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        losses = torch.empty(E, max(1, T), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(lib.hb_gumbel_fit(_lib.ptr(xc), _lib.ptr(xe), _lib.ptr(yd), n, C.byref(self._spec), r, E,
+                                         _lib.ptr(self.params), float(self.lr), float(self.l1), int(self.batch_size), T,
+                                         _lib.ptr(pd_), _lib.ptr(dd), seed & (2 ** 64 - 1), _lib.ptr(losses),
+                                         _lib.ptr(self.fit_ws), need, _lib.stream_ptr()), "hb_gumbel_fit")
+        self.losses = losses[:, :T]
+        if T > 0:               # predict uses the last trained epoch's temperature
+            self.temperature = gumbel_epoch_temperature(T - 1)
+        if self.verbose:
+            self._print_losses()
+
+    def fit_state(self):
+        """Views of the fit workspace: Adam's exp_avg, exp_avg_sq and the last step's gradient, each [E, P]."""
+        E, P = self.num_ensembles, self.P
+        return tuple(self.fit_ws.view(torch.float32)[:3 * E * P].view(3, E, P))
+
+    # ------------------------------------------------------------------ predict
+    def _predict_dev(self, Xs, xe, grad=False, member=-1, draws=None, seed=None, counter=0):
+        if grad:
+            raise NotImplementedError("GumbelDeepEnsemble: no input gradients (support_grad = False)")
+        lib, dev = _lib.lib(), self.device
+        assert self.fitted, "fit() first"
+        m = (Xs if Xs is not None else xe).shape[0]
+        E, r = self.num_ensembles, self.reduced_dim
+        xm, xa, ym, ys = self._scal_dev()
+        mu = torch.empty(m, self.num_out, dtype=torch.float32, device=dev)
+        var = torch.empty(m, self.num_out, dtype=torch.float32, device=dev) if member < 0 else None
+        if draws is not None:
+            draws = torch.as_tensor(draws).to(dev, torch.float32).contiguous()
+            if tuple(draws.shape) != (E, r, self.num_cont):
+                raise ValueError(f"eval draws must be [{E}, {r}, {self.num_cont}], got {list(draws.shape)}")
+        elif seed is None:
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
+        ws = torch.empty(max(1, E * r * self.num_cont), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(lib.hb_gumbel_predict(_lib.ptr(Xs), _lib.ptr(xe), m, C.byref(self._spec), r, float(self.temperature),
+                                             E, _lib.ptr(self.params), _lib.ptr(xm), _lib.ptr(xa), _lib.ptr(ym), _lib.ptr(ys),
+                                             int(member), _lib.ptr(draws), int(seed or 0) & (2 ** 64 - 1),
+                                             int(counter) & (2 ** 64 - 1), _lib.ptr(mu), _lib.ptr(var), _lib.ptr(ws),
+                                             ws.numel() * 4, _lib.stream_ptr()), "hb_gumbel_predict")
+        return mu, var
+
+    predict = FeDeepEnsemble.predict
+    sample_y = FeDeepEnsemble.sample_y
+
+
+def _reference_gumbelnet():
+    """GumbelNet of an installed HEBO, or None."""
+    try:  # pragma: no cover - depends on the environment
+        from hebo.models.nn.gumbel_linear import GumbelNet
+        return GumbelNet
     except Exception:
         return None

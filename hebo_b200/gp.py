@@ -742,12 +742,13 @@ def register(name: str = "gp_b200", override_gp: bool = False, override_rf: bool
         from hebo.models import model_factory
     except Exception:
         return False
-    from .ensemble import DeepEnsemble, FeDeepEnsemble
+    from .ensemble import DeepEnsemble, FeDeepEnsemble, GumbelDeepEnsemble
     from .forest import RF
     model_factory.model_dict[name] = GP
     model_factory.model_dict["multi_task_b200"] = MultiTaskModel
     model_factory.model_dict["deep_ensemble_b200"] = DeepEnsemble
     model_factory.model_dict["fe_deep_ensemble_b200"] = FeDeepEnsemble
+    model_factory.model_dict["gumbel_b200"] = GumbelDeepEnsemble
     model_factory.model_dict["rf_b200"] = RF
     if override_gp:
         model_factory.model_dict["gp"] = GP

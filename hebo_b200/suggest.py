@@ -28,7 +28,7 @@ from torch.quasirandom import SobolEngine
 
 from . import _lib
 from .acq import MACE
-from .ensemble import DeepEnsemble, FeDeepEnsemble
+from .ensemble import DeepEnsemble, FeDeepEnsemble, GumbelDeepEnsemble
 from .gp import GP
 from .pareto import feasible_front, pareto_front
 from .space import DesignSpace, box_space
@@ -67,9 +67,9 @@ class HEBO:
                  scramble_seed: Optional[int] = None, n_candidates: int = 10000, device: str = "cuda",
                  n_refine: int = 0, refine_sigma: float = 0.05, acq_optimizer: str = "sobol", evo_pop: int = 100,
                  evo_iters: int = 100, lb=None, _constraint=None, model_name: str = "gp", acq_cls=MACE):
-        if model_name not in ("gp", "deep_ensemble", "fe_deep_ensemble"):
-            raise NotImplementedError(f"HEBO: model_name {model_name!r} is not supported, only 'gp', 'deep_ensemble' and "
-                                      "'fe_deep_ensemble'")
+        if model_name not in ("gp", "deep_ensemble", "fe_deep_ensemble", "gumbel"):
+            raise NotImplementedError(f"HEBO: model_name {model_name!r} is not supported, only 'gp', 'deep_ensemble', "
+                                      "'fe_deep_ensemble' and 'gumbel'")
         if acq_cls is not MACE and (n_refine or _constraint is not None):
             raise ValueError("n_refine and the embedding constraint are defined for the MACE front only; an acq_cls other "
                              "than MACE takes neither")
@@ -195,7 +195,8 @@ class HEBO:
     # ------------------------------------------------------------------ suggest
     def _fit(self):
         """hebo.py:127-147: power-transformed y, and on ANY failure (transform or fit) a refit on the raw y."""
-        cls = {"gp": GP, "deep_ensemble": DeepEnsemble, "fe_deep_ensemble": FeDeepEnsemble}[self.model_name]
+        cls = {"gp": GP, "deep_ensemble": DeepEnsemble, "fe_deep_ensemble": FeDeepEnsemble,
+               "gumbel": GumbelDeepEnsemble}[self.model_name]
 
         def build(y):
             model = cls(self.d, self.e, 1, device=self.device, **self.model_config)

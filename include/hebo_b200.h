@@ -515,7 +515,9 @@ int32_t hb_front_merge(const float *all_buf, int64_t world, int64_t capacity, fl
 /* A fit keeps one minibatch's activations on chip: rows B = min(n, batch_size) must satisfy
  * B * (in_ld + (num_layers + 2) * hid_ld + 5 * num_out + 1) <= HB_DE_MAX_BATCH_FLOATS, with in_ld = in | 1 and
  * hid_ld = max(num_hiddens, in) | 1 (odd leading dimensions).  BaseNet's defaults (batch 32) fit with room to spare at every
- * layer / width / output count above. */
+ * layer / width / output count above.  The feature-gated ensemble (hb_fe_fit) adds 2 * B * in_ld to the left side; the
+ * Gumbel ensemble (hb_gumbel_fit) takes in_ld and hid_ld of the SELECTED width r + enum width and adds B * (num_cont | 1)
+ * for the minibatch's numeric rows when num_cont > 0. */
 #define HB_DE_MAX_BATCH_FLOATS 56000
 
 #define HB_DE_EMBEDDING    0      /* conf['enum_trans'] = 'embedding' (deep_ensemble.py:199-201) */
@@ -662,6 +664,57 @@ int32_t hb_fe_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de
                       int64_t E, const float *params, const float *x_mul, const float *x_add, const float *y_mean,
                       const float *y_std, int32_t member, const float *draws, uint64_t seed, uint64_t counter, float *mu,
                       float *var, void *stream);
+
+/* ---- Gumbel feature-selection deep ensemble (models/nn/gumbel_linear.py: GumbelNet, GumbelDeepEnsemble) ----------------
+ * The deep ensemble above whose members first map their num_cont numeric inputs to r = reduced_dim selected ones,
+ * x_sel = x_num W^T, W [r, num_cont] = RelaxedOneHotCategorical(T, logits).rsample() (softmax over the numeric columns),
+ * ONE W per forward shared by every row.  The member's input row is [x_sel | embedding or one-hot]; with num_cont = 0
+ * nothing is drawn and the member is a BaseNet.  One member's raw parameters are P_gb = hb_gumbel_num_params(spec, r)
+ * floats: BaseNet's layout for spec with num_cont replaced by r (when num_cont > 0), then feature_select.logits
+ * [r, num_cont] LAST (GumbelNet's state_dict order).  W from logits theta, uniforms u and temperature T, in fp32:
+ *   L = theta - lse(theta),  g = -log(-log(clamp(u, eps, 1 - eps))),  s = (L + g) / T,  W = exp(s - lse(s))
+ * with lse(v) = log(sum exp(v - max v)) + max v over the row, eps = FLT_EPSILON, and (L + g) / T one IEEE fp32 division by
+ * fp32(T), as torch divides an fp32 tensor by a Python float.
+ * Envelope, on top of the deep ensemble's: num_cont <= HB_DE_MAX_IN, 1 <= r, r + embedding / one-hot width <= HB_DE_MAX_IN;
+ * rand_prior needs r = num_cont or num_cont = 0 (the prior net keeps the unselected width).  The numeric rows of the
+ * minibatch stay on chip next to BaseNet's buffers of the selected width (in_ld, hid_ld of r + enum width):
+ *   B * (in_ld + (num_layers + 2) * hid_ld + 5 * num_out + 1) + B * (num_cont | 1) <= HB_DE_MAX_BATCH_FLOATS
+ * (the last term only when num_cont > 0).  W and d loss / d W live in global memory (the fit's workspace).  Outside the
+ * envelope: HB_ERR_INVALID before any launch, and -1 from the two queries. */
+int64_t hb_gumbel_num_params(const hb_de_spec_t *spec, int64_t reduced_dim);
+/* Workspace of hb_gumbel_fit: 3 E P_gb floats laid out as hb_de_fit's (exp_avg, exp_avg_sq, last gradient), then each
+ * member's W of its last step [E, r, num_cont]. */
+int64_t hb_gumbel_fit_workspace_bytes(const hb_de_spec_t *spec, int64_t reduced_dim, int64_t E);
+/* GumbelDeepEnsemble.fit_one (gumbel_linear.py:69-100) for all E members in ONE launch, one CTA per member: hb_de_fit's
+ * minibatch order, data loss and Adam, with
+ *   - NO drop_last: ceil(n / batch_size) steps per epoch, the last one of the remaining rows; each step's loss is the mean
+ *     over its own minibatch, the L1 divisor stays n num_out;
+ *   - per step a fresh W from uniforms, x_sel = x_num W^T, and the backward through W, the softmax and the logits'
+ *     normalisation into the logits (d loss / d W sums the minibatch rows in order);
+ *   - the L1 term over the WEIGHTS only (embedding tables, hidden / heads / prior-net weights), not biases or logits;
+ *   - the random prior net (rand_prior) evaluated without gradient; its weights take the L1 term, its biases do not move;
+ *   - T = fp32(0.8^epoch + 0.1) (the double rounded once) throughout epoch `epoch`.
+ *   perm as hb_de_fit (rows of each epoch in order).  draws: NULL, or [E, num_epochs, nb, r, num_cont] uniforms, nb the
+ *   steps per epoch, for tests that replay given draws.  With draws = NULL, element q = ((epoch nb + step) r + j) num_cont
+ *   + k of member e's fit takes the word q % 2 of the Philox4x32-10 block of counter (q / 2 as 64 bits, e, 0x47424654)
+ *   under `seed`, as the uniform (w + 0.5) 2^-32; the minibatch order's counters end in 0x44450000 + r and the fe
+ *   ensemble's in 0x4645..., so no two streams share a block.
+ * Bit-identical from run to run.  No host synchronisation. */
+int32_t hb_gumbel_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec,
+                      int64_t reduced_dim, int64_t E, float *params, double lr, float l1, int64_t batch_size,
+                      int64_t num_epochs, const int32_t *perm, const float *draws, uint64_t seed, float *losses, void *ws,
+                      int64_t ws_bytes, void *stream);
+/* hb_de_predict over GumbelNet members (member = -1: the ensemble; member >= 0: sample_f's one member, var may be NULL) at
+ * temperature T = `temperature` (the last trained epoch's; 0.1 before any epoch).  Each member's W is built ONCE per call
+ * into ws (ws_bytes >= 4 E r num_cont; unused when num_cont = 0) and shared by every candidate tile: draws [E, r, num_cont]
+ * device uniforms, or NULL: element q = j num_cont + k of member e takes the word q % 2 of the Philox4x32-10 block of
+ * counter (counter as 64 bits, (e << 16) | (q / 2), 0x47424556) under `seed`.  A new counter (a GA generation) gives a
+ * fresh W, as the reference redraws it on every forward; the same (seed, counter) replays the same bits, so a call split
+ * over candidate rows equals the whole call.  No input gradients.  Two launches, no host synchronisation. */
+int32_t hb_gumbel_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t reduced_dim,
+                          float temperature, int64_t E, const float *params, const float *x_mul, const float *x_add,
+                          const float *y_mean, const float *y_std, int32_t member, const float *draws, uint64_t seed,
+                          uint64_t counter, float *mu, float *var, void *ws, int64_t ws_bytes, void *stream);
 
 /* ---- random-forest surrogate (models/rf/rf.py: RF :19-56 over sklearn's RandomForestRegressor defaults) ------------------
  * T regression trees per output, each exact CART (squared error, every feature, min_samples_split 2, min_samples_leaf 1,
