@@ -23,7 +23,7 @@ import torch
 
 from . import _lib
 from .base import Acquisition
-from .ensemble import DeepEnsemble, EnsembleBatch, FeDeepEnsemble, GumbelDeepEnsemble
+from .ensemble import DeepEnsemble, EnsembleBatch, FeatureSelectionEnsemble
 from .forest import RF
 from .gp import GP, MultiTaskModel
 
@@ -175,7 +175,7 @@ def ga_score(acq, seed=None):
     if mode is not None and isinstance(acq.model, (GP, DeepEnsemble, RF)):
         kappa = float(getattr(acq, "kappa", 0.0))
         eta = float(getattr(acq, "eta", 0.0))
-        fe = isinstance(acq.model, (FeDeepEnsemble, GumbelDeepEnsemble))     # fresh draws per generation: (fe_seed, gen)
+        fe = isinstance(acq.model, FeatureSelectionEnsemble)     # fresh draws per generation: (fe_seed, gen)
         fe_seed = (int(np.random.randint(0, 2 ** 31 - 1)) if seed is None else int(seed)) if fe else 0
 
         def device_score(xc, xe, gen):
@@ -373,9 +373,9 @@ def _ensembles_of(model):
 
 
 def _batchable(model) -> bool:
-    """A DeepEnsemble that hb_de_predict_batch scores: not a FeDeepEnsemble or a GumbelDeepEnsemble, whose gate or
-    selection layer only hb_fe_predict / hb_gumbel_predict apply."""
-    return isinstance(model, DeepEnsemble) and not isinstance(model, (FeDeepEnsemble, GumbelDeepEnsemble))
+    """A DeepEnsemble that hb_de_predict_batch scores: not a FeatureSelectionEnsemble, whose selection layer only its
+    own predict entry point applies."""
+    return isinstance(model, DeepEnsemble) and not isinstance(model, FeatureSelectionEnsemble)
 
 
 def _general_ensemble_score(acq, models, seed=None):

@@ -18,10 +18,9 @@ import pandas as pd
 import torch
 
 from .acq import LCB, AbsEtaDifference, ga_score  # noqa: F401  (AbsEtaDifference: nomr.py exports it next to NoMR_BO)
-from .ensemble import DeepEnsemble, FeDeepEnsemble, GumbelDeepEnsemble
 from .gp import GP
 from .space import DesignSpace
-from .suggest import HEBO
+from .suggest import HEBO, MODELS, check_model_name
 
 
 def _design_space(space) -> DesignSpace:
@@ -39,9 +38,7 @@ class BO:
 
     def __init__(self, space, model_name: str = "gp", rand_sample: Optional[int] = None, acq_cls=None,
                  acq_conf: Optional[dict] = None, pop: int = 100, iters: int = 100, device: str = "cuda"):
-        if model_name not in ("gp", "deep_ensemble", "fe_deep_ensemble", "gumbel"):
-            raise NotImplementedError(f"BO: model_name {model_name!r} is not supported, only 'gp', 'deep_ensemble', "
-                                      "'fe_deep_ensemble' and 'gumbel'")
+        check_model_name("BO", model_name)
         self.space = _design_space(space)
         sp = self.space
         self.d, self.e = sp.num_numeric, sp.num_categorical
@@ -78,8 +75,9 @@ class BO:
         conf = {"warp": False, "device": self.device}              # bo.py:62-69: the GP's own defaults, raw y
         if self.e > 0:
             conf["num_uniqs"] = self.space.num_uniqs
-        model = {"gp": GP, "deep_ensemble": DeepEnsemble, "fe_deep_ensemble": FeDeepEnsemble,
-                 "gumbel": GumbelDeepEnsemble}[self.model_name](self.d, self.e, 1, **conf)
+        # GP is read from this module at call time, so replacing hebo_b200.bo.GP replaces the GP that BO fits
+        cls = GP if self.model_name == "gp" else MODELS[self.model_name]
+        model = cls(self.d, self.e, 1, **conf)
         model.fit(self.Xc if self.d else None, self.Xe if self.e else None, torch.FloatTensor(self.y))
         acq = self.acq_cls(model, **self.acq_conf)
         if acq.num_obj != 1 or acq.num_constr != 0:

@@ -1015,24 +1015,24 @@ int32_t hb_embed_violation(const float *Y, int64_t m, int64_t e, const float *B,
 }
 
 // deep_ensemble.py:34-61 / BaseNet :183-221: P of one member
-int64_t hb_de_num_params(const hb_de_spec_t *spec) { return de_num_params(spec); }
+int64_t hb_de_num_params(const hb_de_spec_t *spec) { return de_num_params(spec, DeVariant{}); }
 
-int64_t hb_de_fit_workspace_bytes(const hb_de_spec_t *spec, int64_t E) { return de_fit_ws_query(spec, E); }
+int64_t hb_de_fit_workspace_bytes(const hb_de_spec_t *spec, int64_t E) { return de_fit_ws_query(spec, DeVariant{}, E); }
 
 // deep_ensemble.py:71-93 (the member loop) and fit_one :151-181
 int32_t hb_de_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec, int64_t E,
                   float *params, double lr, float l1, int64_t batch_size, int64_t num_epochs, const int32_t *perm,
                   uint64_t seed, float *losses, void *ws, int64_t ws_bytes, void *stream) {
-  return launch_de_fit(Xc, Xe, y, n, spec, E, params, lr, l1, batch_size, num_epochs, perm, seed, losses, ws, ws_bytes,
-                       (cudaStream_t)stream);
+  return launch_de_fit(Xc, Xe, y, n, spec, DeVariant{}, E, params, lr, l1, batch_size, num_epochs, perm, nullptr, seed, losses,
+                       ws, ws_bytes, (cudaStream_t)stream);
 }
 
 // deep_ensemble.py:95-106 (predict) and :108-116 (sample_f, member >= 0)
 int32_t hb_de_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t E,
                       const float *params, const float *x_mul, const float *x_add, const float *y_mean, const float *y_std,
                       int32_t member, float *mu, float *var, void *stream) {
-  return launch_de_predict(Xs, Xe, m, spec, E, params, x_mul, x_add, y_mean, y_std, member, mu, var, nullptr, nullptr,
-                           (cudaStream_t)stream);
+  return launch_de_predict(Xs, Xe, m, spec, DeVariant{}, E, params, x_mul, x_add, y_mean, y_std, member, nullptr, 0, 0, mu, var,
+                           nullptr, nullptr, nullptr, 0, (cudaStream_t)stream);
 }
 
 // autograd of deep_ensemble.py:95-106 with respect to Xc (the support_grad contract, base_model.py / test_base_model.py:94-108)
@@ -1040,8 +1040,8 @@ int32_t hb_de_predict_grad(const float *Xs, const int32_t *Xe, int64_t m, const 
                            const float *params, const float *x_mul, const float *x_add, const float *y_mean,
                            const float *y_std, float *mu, float *var, float *dmu, float *dvar, void *stream) {
   if (!dmu || !dvar) return HB_ERR_INVALID;
-  return launch_de_predict(Xs, Xe, m, spec, E, params, x_mul, x_add, y_mean, y_std, -1, mu, var, dmu, dvar,
-                           (cudaStream_t)stream);
+  return launch_de_predict(Xs, Xe, m, spec, DeVariant{}, E, params, x_mul, x_add, y_mean, y_std, -1, nullptr, 0, 0, mu, var,
+                           dmu, dvar, nullptr, 0, (cudaStream_t)stream);
 }
 
 // deep_ensemble.py:71-93 for the ensembles of a MultiTaskModel (model_factory.py:60-92), all in one launch
@@ -1061,18 +1061,27 @@ int32_t hb_de_predict_batch(const float *Xs, const int32_t *Xe, int64_t m, const
                                  counter, y_samp, (cudaStream_t)stream);
 }
 
-// fe_deep_ensemble.py: FeNet / FeDeepEnsemble, P of one gated member
-int64_t hb_fe_num_params(const hb_de_spec_t *spec) { return fe_num_params(spec); }
+// The gated and Gumbel layouts depend on neither the gate's kind and temperatures nor predict's temperature: the
+// queries, and the Gumbel fit (which anneals its own temperature), pass any valid one
+static const hb_fe_gate_t ANY_GATE = {HB_FE_STG, 1.0f, 1.0, 0.1, 0.99, 0.1f};
+static DeVariant gumbel_variant(int64_t reduced_dim, float temperature = 1.0f) {
+  return {DeVariant::GUMBEL, nullptr, reduced_dim, temperature};
+}
 
-int64_t hb_fe_fit_workspace_bytes(const hb_de_spec_t *spec, int64_t E) { return fe_fit_ws_query(spec, E); }
+// fe_deep_ensemble.py: FeNet / FeDeepEnsemble, P of one gated member
+int64_t hb_fe_num_params(const hb_de_spec_t *spec) { return de_num_params(spec, {DeVariant::GATED, &ANY_GATE}); }
+
+int64_t hb_fe_fit_workspace_bytes(const hb_de_spec_t *spec, int64_t E) {
+  return de_fit_ws_query(spec, {DeVariant::GATED, &ANY_GATE}, E);
+}
 
 // deep_ensemble.py:71-93 (the member loop) and FeDeepEnsemble.fit_one (fe_deep_ensemble.py:46-75)
 int32_t hb_fe_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec,
                   const hb_fe_gate_t *gate, int64_t E, float *params, double lr, float l1, int64_t batch_size,
                   int64_t num_epochs, const int32_t *perm, const float *draws, uint64_t seed, float *losses, void *ws,
                   int64_t ws_bytes, void *stream) {
-  return launch_fe_fit(Xc, Xe, y, n, spec, gate, E, params, lr, l1, batch_size, num_epochs, perm, draws, seed, losses, ws,
-                       ws_bytes, (cudaStream_t)stream);
+  return launch_de_fit(Xc, Xe, y, n, spec, {DeVariant::GATED, gate}, E, params, lr, l1, batch_size, num_epochs, perm, draws,
+                       seed, losses, ws, ws_bytes, (cudaStream_t)stream);
 }
 
 // deep_ensemble.py:95-116 over FeNet members (fe_deep_ensemble.py:29-35), the gate in eval mode
@@ -1080,15 +1089,17 @@ int32_t hb_fe_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de
                       int64_t E, const float *params, const float *x_mul, const float *x_add, const float *y_mean,
                       const float *y_std, int32_t member, const float *draws, uint64_t seed, uint64_t counter, float *mu,
                       float *var, void *stream) {
-  return launch_fe_predict(Xs, Xe, m, spec, gate, E, params, x_mul, x_add, y_mean, y_std, member, draws, seed, counter, mu,
-                           var, (cudaStream_t)stream);
+  return launch_de_predict(Xs, Xe, m, spec, {DeVariant::GATED, gate}, E, params, x_mul, x_add, y_mean, y_std, member, draws,
+                           seed, counter, mu, var, nullptr, nullptr, nullptr, 0, (cudaStream_t)stream);
 }
 
 // gumbel_linear.py: GumbelNet / GumbelDeepEnsemble, P of one member
-int64_t hb_gumbel_num_params(const hb_de_spec_t *spec, int64_t reduced_dim) { return gb_num_params(spec, reduced_dim); }
+int64_t hb_gumbel_num_params(const hb_de_spec_t *spec, int64_t reduced_dim) {
+  return de_num_params(spec, gumbel_variant(reduced_dim));
+}
 
 int64_t hb_gumbel_fit_workspace_bytes(const hb_de_spec_t *spec, int64_t reduced_dim, int64_t E) {
-  return gb_fit_ws_query(spec, reduced_dim, E);
+  return de_fit_ws_query(spec, gumbel_variant(reduced_dim), E);
 }
 
 // deep_ensemble.py:71-93 (the member loop) and GumbelDeepEnsemble.fit_one (gumbel_linear.py:69-100)
@@ -1096,8 +1107,8 @@ int32_t hb_gumbel_fit(const float *Xc, const int32_t *Xe, const float *y, int64_
                       int64_t reduced_dim, int64_t E, float *params, double lr, float l1, int64_t batch_size,
                       int64_t num_epochs, const int32_t *perm, const float *draws, uint64_t seed, float *losses, void *ws,
                       int64_t ws_bytes, void *stream) {
-  return launch_gb_fit(Xc, Xe, y, n, spec, reduced_dim, E, params, lr, l1, batch_size, num_epochs, perm, draws, seed, losses,
-                       ws, ws_bytes, (cudaStream_t)stream);
+  return launch_de_fit(Xc, Xe, y, n, spec, gumbel_variant(reduced_dim), E, params, lr, l1, batch_size, num_epochs, perm, draws,
+                       seed, losses, ws, ws_bytes, (cudaStream_t)stream);
 }
 
 // deep_ensemble.py:95-116 over GumbelNet members (gumbel_linear.py:58-61)
@@ -1105,8 +1116,8 @@ int32_t hb_gumbel_predict(const float *Xs, const int32_t *Xe, int64_t m, const h
                           float temperature, int64_t E, const float *params, const float *x_mul, const float *x_add,
                           const float *y_mean, const float *y_std, int32_t member, const float *draws, uint64_t seed,
                           uint64_t counter, float *mu, float *var, void *ws, int64_t ws_bytes, void *stream) {
-  return launch_gb_predict(Xs, Xe, m, spec, reduced_dim, temperature, E, params, x_mul, x_add, y_mean, y_std, member, draws,
-                           seed, counter, mu, var, ws, ws_bytes, (cudaStream_t)stream);
+  return launch_de_predict(Xs, Xe, m, spec, gumbel_variant(reduced_dim, temperature), E, params, x_mul, x_add, y_mean, y_std,
+                           member, draws, seed, counter, mu, var, nullptr, nullptr, ws, ws_bytes, (cudaStream_t)stream);
 }
 
 // rf.py:19-56: RF over sklearn's RandomForestRegressor (forest.cu)

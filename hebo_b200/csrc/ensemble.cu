@@ -317,18 +317,24 @@ __device__ __forceinline__ int de_perm(int pos, int n, int h, uint64_t seed, int
   return (int)x;
 }
 
-// ------------------------------------------------------------------------------------------------ feature gate
-// FeNet's gate (fe_layers.py) on the input columns: GATE = 1 + HB_FE_STG | HB_FE_CONCRETE | HB_FE_HARD_CONCRETE, 0 = none.
-// One gate parameter theta per input column, [din] after BaseNet's P: mu (stg) or logits (concrete layers).
-struct FeGate {
-  int off;               // first gate parameter (BaseNet's P); a member holds off + din floats
-  float T;               // stg: its temperature throughout; concrete layers: predict's (the last epoch's)
-  float mcoef;           // fp32 (1 / (n num_out)) * mask_reg, 0 without numeric columns (no mask penalty)
-  double t0, t1, tb;     // start_temp, end_temp, anneal_base of the concrete layers' schedule
-  const float *draws;    // fit [E, epochs, nb, B, din] / predict [E, din] raw draws, or NULL: Philox
-  uint64_t seed, counter;
+// ------------------------------------------------------------------------------------------------ selection
+// A member's selection layer.  GATE = 0: none (BaseNet).  GATE = 1 + HB_FE_STG | HB_FE_CONCRETE | HB_FE_HARD_CONCRETE:
+// FeNet's gate (fe_layers.py) on the input columns, one parameter theta per column, [din] after BaseNet's P: mu (stg) or
+// logits (concrete layers).  GATE = DE_GUMBEL: GumbelNet's selection of the numeric columns (below).
+struct DeSel {
+  int off;               // first selection parameter (BaseNet's P); a member holds off + din (gate) or off + r dx floats
+  float T;               // stg: its temperature throughout; concrete layers and Gumbel: predict's (the last epoch's)
+  float mcoef;           // gate: fp32 (1 / (n num_out)) * mask_reg, 0 without numeric columns (no mask penalty)
+  int gate;              // GATE
+  double t0, t1, tb;     // gate: start_temp, end_temp, anneal_base of the concrete layers' schedule
+  const float *draws;    // raw draws, or NULL: Philox.  Gate: fit [E, epochs, nb, B, din] / predict [E, din]; Gumbel:
+                         // fit [E, epochs, nb, r, dx] / predict [E, r, dx] uniforms
+  uint64_t seed, counter;      // predict's Philox key
+  int dx, r, x_ld;       // Gumbel: numeric columns of the data, selected columns, leading dimension of the on-chip numeric rows
+  float *w;              // Gumbel: [E, r, dx] each member's W of the current step (fit) or call (predict)
 };
 
+// ------------------------------------------------------------------------------------------------ feature gate
 constexpr uint32_t FE_TAG_FIT = 0x46454654u;      // upper word of the Philox counter of the training draws ('FEFT')
 constexpr uint32_t FE_TAG_EVAL = 0x46454556u;     // ... and of the eval draws ('FEEV')
 
@@ -402,15 +408,6 @@ __device__ __forceinline__ bool fe_is_weight(const DeNet &net, int i, int off) {
 // GumbelNet's feature_select (gumbel_linear.py:21-40) on the dx numeric columns: x_sel = x_num W^T [B, r] with
 // W = RelaxedOneHotCategorical(T, logits).rsample() [r, dx], one W per forward shared by every row.  The member's DeNet is
 // BaseNet's layout with num_cont = r (its input row is [x_sel | embedding or one-hot]); the logits [r, dx] follow it.
-struct GbSel {
-  int off;               // first logit (the selected-width BaseNet's P); a member holds off + r dx floats
-  int dx, r, x_ld;       // numeric columns of the data, selected columns, leading dimension of the on-chip numeric rows
-  float T;               // predict's temperature (the last trained epoch's)
-  const float *draws;    // fit [E, epochs, nb, r, dx] / predict [E, r, dx] uniforms, or NULL: Philox
-  float *w;              // [E, r, dx] each member's W of the current step (fit) or call (predict)
-  uint64_t seed, counter;
-};
-
 constexpr uint32_t GB_TAG_FIT = 0x47424654u;      // upper word of the Philox counter of the training draws ('GBFT')
 constexpr uint32_t GB_TAG_EVAL = 0x47424556u;     // ... and of the eval draws ('GBEV')
 
@@ -494,18 +491,18 @@ struct DeFitArgs {
 // The whole fit of one member: a's pointers are its ensemble's (params [E, P], m1 / m2 / grad [E, P], losses [E, epochs]).
 // Step bi takes rows bi B .. min((bi + 1) B, n) - 1 of the epoch's order, so a.nb decides whether a partial last
 // minibatch is trained (a.nb = ceil(n / B)) or dropped.
-// GATE: FeDeepEnsemble.fit_one (fe_deep_ensemble.py:46-75) with fe's gate; the unmasked inputs and the gate states of the
-// minibatch sit in two more [B, in_ld] buffers after the scratch.  DE_GUMBEL: GumbelDeepEnsemble.fit_one
-// (gumbel_linear.py:69-100) with gb's selection layer; the numeric rows sit in one [B, x_ld] buffer after the scratch.
+// GATE: FeDeepEnsemble.fit_one (fe_deep_ensemble.py:46-75) with sel's gate; the unmasked inputs and the gate states of
+// the minibatch sit in two more [B, in_ld] buffers after the scratch.  DE_GUMBEL: GumbelDeepEnsemble.fit_one
+// (gumbel_linear.py:69-100) with sel's selection layer; the numeric rows sit in one [B, x_ld] buffer after the scratch.
 template <int GATE = 0>
 __device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs &a, int member, float *smem,
-                                              const FeGate *fe = nullptr, const GbSel *gb = nullptr) {
+                                              const DeSel *sel = nullptr) {
   const int B = a.B, O = net.O;
   const DeSmem s = de_carve(net, smem, B);
   float *xraw = s.red + DE_SCRATCH, *gst = xraw + B * net.in_ld;
   constexpr bool GUMBEL = GATE == DE_GUMBEL;
-  const int wsz = GUMBEL ? gb->r * gb->dx : 0;
-  float *W = GUMBEL ? gb->w + (size_t)member * wsz : nullptr;
+  const int wsz = GUMBEL ? sel->r * sel->dx : 0;
+  float *W = GUMBEL ? sel->w + (size_t)member * wsz : nullptr;
   float *prm = a.params + (size_t)member * net.P;
   float *m1 = a.m1 + (size_t)member * net.P, *m2 = a.m2 + (size_t)member * net.P, *g = a.grad + (size_t)member * net.P;
   for (int i = threadIdx.x; i < net.P; i += blockDim.x) {
@@ -517,9 +514,9 @@ __device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs 
   for (int ep = 0; ep < a.epochs; ++ep) {
     float epoch_loss = 0.0f;     // thread 0
     float T = 0.0f;
-    if constexpr (GATE == 1 + HB_FE_STG) T = fe->T;
+    if constexpr (GATE == 1 + HB_FE_STG) T = sel->T;
     else if constexpr (GUMBEL) T = (float)(pow(0.8, (double)ep) + 0.1);     // 0.8**epoch + 0.1, a double, used as fp32
-    else if constexpr (GATE != 0) T = (float)fmax(fe->t0 * pow(fe->tb, (double)ep), fe->t1);     // torch.tensor(.).clamp(end)
+    else if constexpr (GATE != 0) T = (float)fmax(sel->t0 * pow(sel->tb, (double)ep), sel->t1);     // torch.tensor(.).clamp(end)
     for (int bi = 0; bi < a.nb; ++bi) {
       ++step;
       const int Bs = min(B, a.n - bi * B);      // rows of this step
@@ -529,20 +526,20 @@ __device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs 
       }
       __syncthreads();
       if constexpr (GUMBEL) {
-        if (gb->dx > 0) {       // this step's W from fresh uniforms, then x_sel = x_num W^T; x_num stays for the backward
-          const int dx = gb->dx, r = gb->r;
+        if (sel->dx > 0) {       // this step's W from fresh uniforms, then x_sel = x_num W^T; x_num stays for the backward
+          const int dx = sel->dx, r = sel->r;
           const size_t base = (((size_t)member * a.epochs + ep) * a.nb + bi) * (size_t)wsz;
           const uint64_t q0 = ((uint64_t)ep * a.nb + bi) * (uint64_t)wsz;
-          gb_build_w(prm + gb->off, r, dx, T, W, [&](int j, int k) {
+          gb_build_w(prm + sel->off, r, dx, T, W, [&](int j, int k) {
             const uint64_t q = q0 + (uint64_t)j * dx + k;
-            return gb->draws ? gb->draws[base + (size_t)j * dx + k]
-                             : fe_draw<1 + HB_FE_CONCRETE>(a.seed, q >> 1, ((uint64_t)GB_TAG_FIT << 32) | (uint32_t)member,
-                                                           (int)(q & 1));
+            return sel->draws ? sel->draws[base + (size_t)j * dx + k]
+                              : fe_draw<1 + HB_FE_CONCRETE>(a.seed, q >> 1, ((uint64_t)GB_TAG_FIT << 32) | (uint32_t)member,
+                                                            (int)(q & 1));
           });
           for (int idx = threadIdx.x; idx < Bs * dx; idx += blockDim.x)
-            xraw[(idx / dx) * gb->x_ld + idx % dx] = a.Xc[(int64_t)s.rows[idx / dx] * dx + idx % dx];
+            xraw[(idx / dx) * sel->x_ld + idx % dx] = a.Xc[(int64_t)s.rows[idx / dx] * dx + idx % dx];
           __syncthreads();
-          de_dense(xraw, gb->x_ld, Bs, dx, W, nullptr, r, s.xin, net.in_ld, false);
+          de_dense(xraw, sel->x_ld, Bs, dx, W, nullptr, r, s.xin, net.in_ld, false);
         }
         de_load_inputs(net, prm, a.Xc, a.Xe, nullptr, nullptr, s, Bs, nullptr, net.dc);
       } else {
@@ -554,9 +551,9 @@ __device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs 
         for (int idx = threadIdx.x; idx < B * net.din; idx += blockDim.x) {
           const int p = idx / net.din, k = idx % net.din;
           const uint64_t q = (((uint64_t)ep * a.nb + bi) * B + p) * net.din + k;
-          const float r = fe->draws ? fe->draws[base + idx]
-                                    : fe_draw<GATE>(a.seed, q >> 1, ((uint64_t)FE_TAG_FIT << 32) | (uint32_t)member, (int)(q & 1));
-          const float x = s.xin[p * net.in_ld + k], st = fe_state<GATE>(prm[fe->off + k], r, T);
+          const float r = sel->draws ? sel->draws[base + idx]
+                                     : fe_draw<GATE>(a.seed, q >> 1, ((uint64_t)FE_TAG_FIT << 32) | (uint32_t)member, (int)(q & 1));
+          const float x = s.xin[p * net.in_ld + k], st = fe_state<GATE>(prm[sel->off + k], r, T);
           xraw[p * net.in_ld + k] = x;
           gst[p * net.in_ld + k] = st;
           s.xin[p * net.in_ld + k] = __fmul_rn(x, fe_mask<GATE>(st));
@@ -601,27 +598,27 @@ __device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs 
         sum = warp_sum(sum);
         if (threadIdx.x == 0) epoch_loss += sum / cnt * (float)Bs;      // epoch_loss += data_loss * bxc.shape[0]
       }
-      const bool sel = GUMBEL && gb->dx > 0;
+      const bool selw = GUMBEL && sel->dx > 0;
       float *dx = GATE && !GUMBEL ? de_backward(net, prm, s, Bs, g, true, 0)
-                                  : de_backward(net, prm, s, Bs, g, sel || (net.emb && net.ne > 0), sel ? 0 : net.dc);
-      if (sel) {
+                                  : de_backward(net, prm, s, Bs, g, selw || (net.emb && net.ne > 0), selw ? 0 : net.dc);
+      if (selw) {
         // d loss / d W [j, k] = sum over the rows in order of delta_sel[p, j] x_num[p, k], then through the softmax
-        const int dx_ = gb->dx;
+        const int dx_ = sel->dx;
         for (int idx = threadIdx.x; idx < wsz; idx += blockDim.x) {
           const int j = idx / dx_, k = idx % dx_;
           float acc = 0.0f;
-          for (int p = 0; p < Bs; ++p) acc = fmaf(dx[p * net.h_ld + j], xraw[p * gb->x_ld + k], acc);
-          g[gb->off + idx] = acc;
+          for (int p = 0; p < Bs; ++p) acc = fmaf(dx[p * net.h_ld + j], xraw[p * sel->x_ld + k], acc);
+          g[sel->off + idx] = acc;
         }
         __syncthreads();
-        gb_logits_grad(prm + gb->off, W, g + gb->off, gb->r, dx_, T);
+        gb_logits_grad(prm + sel->off, W, g + sel->off, sel->r, dx_, T);
         __syncthreads();
       }
       if constexpr (GATE != 0 && !GUMBEL) {
         // column k: d loss / d theta_k = sum over rows in order of (dx x) through the mask, plus the mask penalty's;
         // then dx becomes the delta of the unmasked input (dx mask) for the embedding tables
         for (int k = threadIdx.x; k < net.din; k += blockDim.x) {
-          const float theta = prm[fe->off + k];
+          const float theta = prm[sel->off + k];
           float acc = 0.0f;
           for (int p = 0; p < B; ++p) {
             float &d = dx[p * net.h_ld + k];
@@ -629,7 +626,7 @@ __device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs 
             acc += fe_dtheta<GATE>(st, __fmul_rn(d, xraw[p * net.in_ld + k]), T);
             d = __fmul_rn(d, fe_mask<GATE>(st));
           }
-          g[fe->off + k] = fe->mcoef != 0.0f ? __fadd_rn(acc, fe_dnorm<GATE>(theta, fe->mcoef, T)) : acc;
+          g[sel->off + k] = sel->mcoef != 0.0f ? __fadd_rn(acc, fe_dnorm<GATE>(theta, sel->mcoef, T)) : acc;
         }
         __syncthreads();
       }
@@ -656,7 +653,7 @@ __device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs 
         const float sg = p > 0.0f ? 1.0f : (p < 0.0f ? -1.0f : 0.0f);
         float gd, gt;
         if constexpr (GATE != 0) {      // L1 over the weights only; the prior net's biases keep gt = 0 and do not move
-          const int off = GUMBEL ? gb->off : fe->off;
+          const int off = sel->off;
           gd = (i < net.prior0 || i >= off) ? g[i] : 0.0f;
           gt = fe_is_weight(net, i, off) ? __fadd_rn(gd, __fmul_rn(a.coef, sg)) : gd;
         } else {
@@ -677,22 +674,11 @@ __device__ __forceinline__ void de_fit_member(const DeNet &net, const DeFitArgs 
   }
 }
 
-__global__ void __launch_bounds__(DE_FIT_THREADS) de_fit_kernel(const __grid_constant__ DeNet net, const DeFitArgs a) {
-  extern __shared__ float smem[];
-  de_fit_member(net, a, blockIdx.x, smem);
-}
-
 template <int GATE>
-__global__ void __launch_bounds__(DE_FIT_THREADS) fe_fit_kernel(const __grid_constant__ DeNet net, const DeFitArgs a,
-                                                                const __grid_constant__ FeGate fe) {
+__global__ void __launch_bounds__(DE_FIT_THREADS) de_fit_kernel(const __grid_constant__ DeNet net, const DeFitArgs a,
+                                                                const __grid_constant__ DeSel sel) {
   extern __shared__ float smem[];
-  de_fit_member<GATE>(net, a, blockIdx.x, smem, &fe);
-}
-
-__global__ void __launch_bounds__(DE_FIT_THREADS) gb_fit_kernel(const __grid_constant__ DeNet net, const DeFitArgs a,
-                                                                const __grid_constant__ GbSel gb) {
-  extern __shared__ float smem[];
-  de_fit_member<DE_GUMBEL>(net, a, blockIdx.x, smem, nullptr, &gb);
+  de_fit_member<GATE>(net, a, blockIdx.x, smem, &sel);
 }
 
 // Per-ensemble arguments of hb_de_fit_batch: its rows [off, off + n) of the concatenated inputs and what follows from n
@@ -709,7 +695,7 @@ struct DeFitBatchArgs {
   DeFitSlot slot[HB_MAX_OUTPUTS];
 };
 
-// CTA (b, member) = blockIdx.x = b E + member runs de_fit_kernel's member on ensemble b's slices
+// CTA (b, member) = blockIdx.x = b E + member runs de_fit_kernel<0>'s member on ensemble b's slices
 __global__ void __launch_bounds__(DE_FIT_THREADS) de_fit_batch_kernel(const __grid_constant__ DeNet net,
                                                                        const __grid_constant__ DeFitBatchArgs ba) {
   extern __shared__ float smem[];
@@ -745,32 +731,32 @@ struct DePredArgs {
 // Rows r0 .. r0 + DE_TM - 1 of the candidates (the last one repeated past m) through members e0 .. e1 - 1: the heads mu
 // into mus[e - e0][p, o] and, with output_noise, sigma2 into s2s[e - e0][p, o].  GATE: member e's eval mask [din] (one
 // draw per column, shared by every row) goes to gmask and multiplies the inputs in the load.  DE_GUMBEL: the tile's
-// scaled numeric rows go to gmask [B, x_ld] once, and member e's x_sel takes its W of the call, gb->w [e].
+// scaled numeric rows go to gmask [B, x_ld] once, and member e's x_sel takes its W of the call, sel->w [e].
 template <int GATE = 0>
 __device__ __forceinline__ void de_member_heads(const DeNet &net, const DePredArgs &a, const DeSmem &s, int r0, int e0,
-                                                int e1, float *mus, float *s2s, const FeGate *fe = nullptr,
-                                                float *gmask = nullptr, const GbSel *gb = nullptr) {
+                                                int e1, float *mus, float *s2s, const DeSel *sel = nullptr,
+                                                float *gmask = nullptr) {
   const int O = net.O, B = DE_TM;
   for (int p = threadIdx.x; p < B; p += blockDim.x) s.rows[p] = min(r0 + p, a.m - 1);
   __syncthreads();
   if constexpr (GATE == DE_GUMBEL) {
-    const int dx = gb->dx;
+    const int dx = sel->dx;
     for (int idx = threadIdx.x; idx < B * dx; idx += blockDim.x) {
       const int p = idx / dx, k = idx % dx;
-      gmask[p * gb->x_ld + k] = __fadd_rn(__fmul_rn(a.x_mul[k], a.Xs[(int64_t)s.rows[p] * dx + k]), a.x_add[k]);
+      gmask[p * sel->x_ld + k] = __fadd_rn(__fmul_rn(a.x_mul[k], a.Xs[(int64_t)s.rows[p] * dx + k]), a.x_add[k]);
     }
     __syncthreads();
   }
   for (int e = e0; e < e1; ++e) {
     const float *prm = a.params + (size_t)e * net.P;
     if constexpr (GATE == DE_GUMBEL) {
-      if (gb->dx > 0) de_dense(gmask, gb->x_ld, B, gb->dx, gb->w + (size_t)e * gb->r * gb->dx, nullptr, gb->r, s.xin, net.in_ld, false);
+      if (sel->dx > 0) de_dense(gmask, sel->x_ld, B, sel->dx, sel->w + (size_t)e * sel->r * sel->dx, nullptr, sel->r, s.xin, net.in_ld, false);
       de_load_inputs(net, prm, a.Xs, a.Xe, a.x_mul, a.x_add, s, B, nullptr, net.dc);
     } else if constexpr (GATE != 0) {
       for (int k = threadIdx.x; k < net.din; k += blockDim.x) {
         const uint64_t stream = ((uint64_t)FE_TAG_EVAL << 32) | ((uint32_t)e << 16) | (uint32_t)(k >> 1);
-        const float r = fe->draws ? fe->draws[(size_t)e * net.din + k] : fe_draw<GATE>(fe->seed, fe->counter, stream, k & 1);
-        gmask[k] = fe_mask<GATE>(fe_state<GATE>(prm[fe->off + k], r, fe->T));
+        const float r = sel->draws ? sel->draws[(size_t)e * net.din + k] : fe_draw<GATE>(sel->seed, sel->counter, stream, k & 1);
+        gmask[k] = fe_mask<GATE>(fe_state<GATE>(prm[sel->off + k], r, sel->T));
       }
       __syncthreads();
       de_load_inputs<true>(net, prm, a.Xs, a.Xe, a.x_mul, a.x_add, s, B, gmask);
@@ -815,19 +801,18 @@ __device__ __forceinline__ void de_combine(const DeNet &net, const float *mus, c
   }
 }
 
-// GATE: fe's gate on every member (no input gradients: FeDeepEnsemble.support_grad = False); the eval mask sits after py.
-// DE_GUMBEL: gb's selection on every member (no input gradients either); the numeric rows sit after py.
+// GATE: sel's gate on every member (no input gradients: FeDeepEnsemble.support_grad = False); the eval mask sits after
+// py.  DE_GUMBEL: sel's selection on every member (no input gradients either); the numeric rows sit after py.
 template <bool GRAD, int GATE = 0>
 __global__ void __launch_bounds__(DE_PRED_THREADS) de_predict_kernel(const __grid_constant__ DeNet net, const DePredArgs a,
-                                                                     const __grid_constant__ FeGate fe,
-                                                                     const __grid_constant__ GbSel gb) {
+                                                                     const __grid_constant__ DeSel sel) {
   static_assert(!(GRAD && GATE), "the gated ensemble has no input gradients");
   extern __shared__ float smem[];
   const int O = net.O, B = DE_TM, r0 = blockIdx.x * DE_TM;
   const DeSmem s = de_carve(net, smem, B);
   const int e0 = a.member >= 0 ? a.member : 0, e1 = a.member >= 0 ? a.member + 1 : a.E, ne = e1 - e0;
   float *mus = s.red + DE_SCRATCH, *s2s = mus + ne * B * O, *py = s2s + ne * B * O;
-  de_member_heads<GATE>(net, a, s, r0, e0, e1, mus, s2s, &fe, py + B * O, &gb);
+  de_member_heads<GATE>(net, a, s, r0, e0, e1, mus, s2s, &sel, py + B * O);
   for (int i = threadIdx.x; i < B * O; i += blockDim.x) {
     const int p = i / O, o = i % O, row = r0 + p;
     float mean, v;
@@ -939,29 +924,127 @@ __global__ void __launch_bounds__(DE_PRED_THREADS) de_predict_batch_kernel(const
   }
 }
 
+// W of members e0 + blockIdx.x for one Gumbel predict call: uniforms from sel.draws [E, r, dx] or Philox keyed by
+// (seed, counter, member), so every candidate tile of the call uses the same W
+__global__ void __launch_bounds__(DE_PRED_THREADS) gb_weights_kernel(const float *params, int P, int e0,
+                                                                     const __grid_constant__ DeSel sel) {
+  const int e = e0 + blockIdx.x, wsz = sel.r * sel.dx;
+  gb_build_w(params + (size_t)e * P + sel.off, sel.r, sel.dx, sel.T, sel.w + (size_t)e * wsz, [&](int j, int k) {
+    const int q = j * sel.dx + k;
+    const uint64_t stream = ((uint64_t)GB_TAG_EVAL << 32) | ((uint32_t)e << 16) | (uint32_t)(q >> 1);
+    return sel.draws ? sel.draws[(size_t)e * wsz + q] : fe_draw<1 + HB_FE_CONCRETE>(sel.seed, sel.counter, stream, q & 1);
+  });
+}
+
 // ------------------------------------------------------------------------------------------------ launchers
-int64_t de_num_params(const hb_de_spec_t *spec) {
-  DeNet net;
-  return de_layout(spec, net) ? net.P : -1;
+// A member's layout and selection constants: BaseNet's; FeNet's, BaseNet's with the gate [din] last; or GumbelNet's,
+// BaseNet's over the selected width (num_cont -> r when num_cont > 0) with the logits [r, num_cont] last.  GumbelNet's
+// random prior net keeps the original width, so it only runs when r = num_cont or there are no numeric columns; anything
+// else is rejected (the reference fails with a shape error in forward).
+static bool de_sel_layout(const hb_de_spec_t *spec, const DeVariant &v, DeNet &net, DeSel &sel) {
+  sel = DeSel{};
+  if (v.kind == DeVariant::GUMBEL) {
+    if (!spec || v.r < 1 || v.r > HB_DE_MAX_IN || spec->num_cont < 0 || spec->num_cont > HB_DE_MAX_IN || !(v.T > 0.0f))
+      return false;
+    const int dx = spec->num_cont;
+    if (spec->rand_prior && dx > 0 && v.r != dx) return false;
+    hb_de_spec_t narrow = *spec;
+    if (dx > 0) narrow.num_cont = (int32_t)v.r;
+    if (!de_layout(&narrow, net)) return false;
+    sel.gate = DE_GUMBEL;
+    sel.off = net.P;
+    sel.T = v.T;
+    sel.dx = dx;
+    sel.r = dx > 0 ? (int)v.r : 0;      // without numeric columns the logits [r, 0] are empty and nothing is drawn
+    sel.x_ld = dx > 0 ? (dx | 1) : 0;
+    net.P += sel.r * dx;
+    return true;
+  }
+  if (!de_layout(spec, net)) return false;
+  sel.off = net.P;
+  if (v.kind == DeVariant::GATED) {
+    const hb_fe_gate_t *g = v.gate;
+    if (!g || g->kind < HB_FE_STG || g->kind > HB_FE_HARD_CONCRETE || !(g->temperature > 0.0f)) return false;
+    sel.gate = 1 + g->kind;
+    sel.T = g->temperature;
+    sel.t0 = g->start_temp;
+    sel.t1 = g->end_temp;
+    sel.tb = g->anneal_base;
+    net.P += net.din;
+  }
+  return true;
 }
 
-int64_t de_fit_ws_query(const hb_de_spec_t *spec, int64_t E) {
-  DeNet net;
-  if (!de_layout(spec, net) || E < 1 || E > HB_DE_MAX_MEMBERS) return -1;
-  return 3 * E * (int64_t)net.P * (int64_t)sizeof(float);
+// floats of a fit's per-row buffers of B rows: BaseNet's, plus a gate's unmasked inputs and gate states (B in_ld each)
+// or a Gumbel selection's numeric rows (B x_ld)
+static int64_t de_fit_rows_floats(const DeNet &net, const DeSel &sel, int64_t B) {
+  const int64_t extra = sel.gate == DE_GUMBEL ? B * sel.x_ld : sel.gate != 0 ? 2 * B * net.in_ld : 0;
+  return de_rows_floats(net, B) + extra;
 }
 
-int launch_de_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec, int64_t E,
-                  float *params, double lr, float l1, int64_t batch_size, int64_t num_epochs, const int32_t *perm,
-                  uint64_t seed, float *losses, void *ws, int64_t ws_bytes, cudaStream_t st) {
+// a predict tile's shared floats after the combination's: a gate's eval mask [din] or a Gumbel tile's numeric rows
+static int64_t de_predict_sel_floats(const DeNet &net, const DeSel &sel) {
+  return sel.gate == DE_GUMBEL ? (int64_t)DE_TM * sel.x_ld : sel.gate != 0 ? net.din : 0;
+}
+
+// a fit's workspace: Adam's exp_avg, exp_avg_sq and the last step's gradient, [E, P] each, then Gumbel's W [E, r, dx]
+static int64_t de_fit_ws_bytes(const DeNet &net, const DeSel &sel, int64_t E) {
+  return (3 * E * (int64_t)net.P + E * (int64_t)sel.r * sel.dx) * (int64_t)sizeof(float);
+}
+
+// The minibatches of a fit over n rows: B rows a step and nb steps an epoch (drop_last: a partial last minibatch is
+// dropped, deep_ensemble.py:154; otherwise it is trained, gumbel_linear.py:72), the Feistel half-width h of the epoch's
+// order of n, and coef = fp32 (1 / (n num_out)) * l1
+struct DeFitShape {
+  int B, nb, h;
+  float coef;
+};
+
+static DeFitShape de_fit_shape(int64_t n, int64_t batch_size, bool drop_last, int O, float l1) {
+  DeFitShape f;
+  const int64_t B = n > batch_size ? batch_size : n;
+  f.B = (int)B;
+  f.nb = (int)(!drop_last ? (n + B - 1) / B : n > batch_size ? n / batch_size : 1);
+  f.h = 1;
+  while ((int64_t(1) << (2 * f.h)) < n) ++f.h;
+  f.coef = (1.0f / (float)(n * O)) * l1;
+  return f;
+}
+
+// every variant's kernel instance, indexed by GATE
+static_assert(HB_FE_STG == 0 && HB_FE_CONCRETE == 1 && HB_FE_HARD_CONCRETE == 2, "GATE 0 .. DE_GUMBEL indexes the tables");
+static decltype(&de_fit_kernel<0>) const DE_FIT_KERNELS[] = {de_fit_kernel<0>, de_fit_kernel<1 + HB_FE_STG>,
+                                                              de_fit_kernel<1 + HB_FE_CONCRETE>,
+                                                              de_fit_kernel<1 + HB_FE_HARD_CONCRETE>, de_fit_kernel<DE_GUMBEL>};
+static decltype(&de_predict_kernel<false>) const DE_PREDICT_KERNELS[] = {
+    de_predict_kernel<false>, de_predict_kernel<false, 1 + HB_FE_STG>, de_predict_kernel<false, 1 + HB_FE_CONCRETE>,
+    de_predict_kernel<false, 1 + HB_FE_HARD_CONCRETE>, de_predict_kernel<false, DE_GUMBEL>};
+
+int64_t de_num_params(const hb_de_spec_t *spec, const DeVariant &v) {
   DeNet net;
-  if (!de_layout(spec, net) || E < 1 || E > HB_DE_MAX_MEMBERS || n < 1 || n > (1 << 30) || batch_size < 1 || num_epochs < 0)
+  DeSel sel;
+  return de_sel_layout(spec, v, net, sel) ? net.P : -1;
+}
+
+int64_t de_fit_ws_query(const hb_de_spec_t *spec, const DeVariant &v, int64_t E) {
+  DeNet net;
+  DeSel sel;
+  if (!de_sel_layout(spec, v, net, sel) || E < 1 || E > HB_DE_MAX_MEMBERS) return -1;
+  return de_fit_ws_bytes(net, sel, E);
+}
+
+int launch_de_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec, const DeVariant &v,
+                  int64_t E, float *params, double lr, float l1, int64_t batch_size, int64_t num_epochs, const int32_t *perm,
+                  const float *draws, uint64_t seed, float *losses, void *ws, int64_t ws_bytes, cudaStream_t st) {
+  DeNet net;
+  DeSel sel;
+  if (!de_sel_layout(spec, v, net, sel) || E < 1 || E > HB_DE_MAX_MEMBERS || n < 1 || n > (1 << 30) || batch_size < 1 ||
+      num_epochs < 0)
     return HB_ERR_INVALID;
   if (!y || !params || !ws || (num_epochs > 0 && !losses) || (net.dc > 0 && !Xc) || (net.ne > 0 && !Xe)) return HB_ERR_INVALID;
-  const int64_t need = de_fit_ws_query(spec, E);
-  if (ws_bytes < need) return HB_ERR_INVALID;
-  const int64_t B = n > batch_size ? batch_size : n;     // drop_last = n > batch_size (deep_ensemble.py:154)
-  if (de_rows_floats(net, B) > HB_DE_MAX_BATCH_FLOATS) return HB_ERR_INVALID;
+  if (ws_bytes < de_fit_ws_bytes(net, sel, E)) return HB_ERR_INVALID;
+  const DeFitShape f = de_fit_shape(n, batch_size, sel.gate != DE_GUMBEL, net.O, l1);
+  if (de_fit_rows_floats(net, sel, f.B) > HB_DE_MAX_BATCH_FLOATS) return HB_ERR_INVALID;
   if (num_epochs == 0) return HB_OK;
   DeFitArgs a;
   a.Xc = Xc;
@@ -974,33 +1057,40 @@ int launch_de_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n,
   a.grad = a.m2 + E * net.P;
   a.losses = losses;
   a.n = (int)n;
-  a.B = (int)B;
-  a.nb = (int)(n > batch_size ? n / batch_size : 1);
+  a.B = f.B;
+  a.nb = f.nb;
   a.epochs = (int)num_epochs;
-  int h = 1;
-  while ((int64_t(1) << (2 * h)) < n) ++h;
-  a.h = h;
+  a.h = f.h;
   a.seed = seed;
   a.lr = lr;
-  a.coef = (1.0f / (float)(n * net.O)) * l1;
-  const size_t smem = (size_t)(de_rows_floats(net, B) + DE_SCRATCH) * sizeof(float);
-  HB_CUDA(cudaFuncSetAttribute(de_fit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  de_fit_kernel<<<(unsigned)E, DE_FIT_THREADS, smem, st>>>(net, a);
+  a.coef = f.coef;
+  if (v.kind == DeVariant::GATED)      // mask_loss only when Xc.shape[1] > 0
+    sel.mcoef = net.dc > 0 ? (1.0f / (float)(n * net.O)) * v.gate->mask_reg : 0.0f;
+  if (sel.gate == DE_GUMBEL) sel.w = a.grad + E * net.P;
+  sel.draws = draws;
+  const size_t smem = (size_t)(de_fit_rows_floats(net, sel, f.B) + DE_SCRATCH) * sizeof(float);
+  const auto kernel = DE_FIT_KERNELS[sel.gate];
+  HB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kernel<<<(unsigned)E, DE_FIT_THREADS, smem, st>>>(net, a, sel);
   count_launches(1);
   HB_LAUNCH_CHECK("de_fit_kernel");
   return HB_OK;
 }
 
-int launch_de_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t E, const float *params,
-                      const float *x_mul, const float *x_add, const float *y_mean, const float *y_std, int32_t member,
-                      float *mu, float *var, float *dmu, float *dvar, cudaStream_t st) {
+int launch_de_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, const DeVariant &v, int64_t E,
+                      const float *params, const float *x_mul, const float *x_add, const float *y_mean, const float *y_std,
+                      int32_t member, const float *draws, uint64_t seed, uint64_t counter, float *mu, float *var,
+                      float *dmu, float *dvar, void *ws, int64_t ws_bytes, cudaStream_t st) {
   DeNet net;
-  if (!de_layout(spec, net) || E < 1 || E > HB_DE_MAX_MEMBERS || m < 0 || m > (int64_t(1) << 31) - DE_TM) return HB_ERR_INVALID;
+  DeSel sel;
+  if (!de_sel_layout(spec, v, net, sel) || E < 1 || E > HB_DE_MAX_MEMBERS || m < 0 || m > (int64_t(1) << 31) - DE_TM)
+    return HB_ERR_INVALID;
   if (member < -1 || member >= E) return HB_ERR_INVALID;
   const bool grad = dmu != nullptr;
   if (!params || !y_mean || !y_std || !mu || (member < 0 && !var) || (net.ne > 0 && !Xe)) return HB_ERR_INVALID;
   if (net.dc > 0 && (!Xs || !x_mul || !x_add)) return HB_ERR_INVALID;
-  if (grad && (!dvar || net.dc < 1 || member >= 0)) return HB_ERR_INVALID;
+  if (sel.dx > 0 && (!ws || ws_bytes < E * (int64_t)sel.r * sel.dx * (int64_t)sizeof(float))) return HB_ERR_INVALID;
+  if (grad && (!dvar || net.dc < 1 || member >= 0 || sel.gate != 0)) return HB_ERR_INVALID;
   if (m == 0) return HB_OK;
   DePredArgs a;
   a.Xs = Xs;
@@ -1017,16 +1107,21 @@ int launch_de_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de
   a.m = (int)m;
   a.E = (int)E;
   a.member = member;
+  sel.draws = draws;
+  sel.seed = seed;
+  sel.counter = counter;
+  sel.w = (float *)ws;
   const int64_t ne = member >= 0 ? 1 : E;
-  const size_t smem = (size_t)(de_rows_floats(net, DE_TM) + DE_SCRATCH + (2 * ne + 1) * DE_TM * net.O) * sizeof(float);
-  const unsigned grid = (unsigned)ceil_div(m, DE_TM);
-  if (grad) {
-    HB_CUDA(cudaFuncSetAttribute(de_predict_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    de_predict_kernel<true><<<grid, DE_PRED_THREADS, smem, st>>>(net, a, FeGate{}, GbSel{});
-  } else {
-    HB_CUDA(cudaFuncSetAttribute(de_predict_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    de_predict_kernel<false><<<grid, DE_PRED_THREADS, smem, st>>>(net, a, FeGate{}, GbSel{});
+  if (sel.dx > 0) {
+    gb_weights_kernel<<<(unsigned)ne, DE_PRED_THREADS, 0, st>>>(params, net.P, member >= 0 ? member : 0, sel);
+    count_launches(1);
+    HB_LAUNCH_CHECK("gb_weights_kernel");
   }
+  const size_t smem = (size_t)(de_rows_floats(net, DE_TM) + DE_SCRATCH + (2 * ne + 1) * DE_TM * net.O +
+                               de_predict_sel_floats(net, sel)) * sizeof(float);
+  const auto kernel = grad ? de_predict_kernel<true> : DE_PREDICT_KERNELS[sel.gate];
+  HB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kernel<<<(unsigned)ceil_div(m, DE_TM), DE_PRED_THREADS, smem, st>>>(net, a, sel);
   count_launches(1);
   HB_LAUNCH_CHECK("de_predict_kernel");
   return HB_OK;
@@ -1041,25 +1136,23 @@ int launch_de_fit_batch(const float *Xc, const int32_t *Xe, const float *y, cons
     return HB_ERR_INVALID;
   if (!off || !seeds || !y || !params || !ws || (num_epochs > 0 && !losses) || (net.dc > 0 && !Xc) || (net.ne > 0 && !Xe))
     return HB_ERR_INVALID;
-  if (ws_bytes < nens * de_fit_ws_query(spec, E)) return HB_ERR_INVALID;
+  if (ws_bytes < nens * de_fit_ws_bytes(net, DeSel{}, E)) return HB_ERR_INVALID;
   DeFitBatchArgs ba{};
   int64_t Bmax = 0;
   if (off[0] < 0) return HB_ERR_INVALID;
   for (int64_t b = 0; b < nens; ++b) {
     const int64_t n = off[b + 1] - off[b];
     if (n < 1 || n > (1 << 30)) return HB_ERR_INVALID;
-    const int64_t B = n > batch_size ? batch_size : n;     // as launch_de_fit, per ensemble
+    const DeFitShape f = de_fit_shape(n, batch_size, true, net.O, l1);
     DeFitSlot &sl = ba.slot[b];
     sl.off = off[b];
     sl.seed = seeds[b];
-    sl.coef = (1.0f / (float)(n * net.O)) * l1;
+    sl.coef = f.coef;
     sl.n = (int)n;
-    sl.B = (int)B;
-    sl.nb = (int)(n > batch_size ? n / batch_size : 1);
-    int h = 1;
-    while ((int64_t(1) << (2 * h)) < n) ++h;
-    sl.h = h;
-    Bmax = B > Bmax ? B : Bmax;
+    sl.B = f.B;
+    sl.nb = f.nb;
+    sl.h = f.h;
+    Bmax = f.B > Bmax ? f.B : Bmax;
   }
   if (de_rows_floats(net, Bmax) > HB_DE_MAX_BATCH_FLOATS) return HB_ERR_INVALID;
   if (num_epochs == 0) return HB_OK;
@@ -1118,279 +1211,6 @@ int launch_de_predict_batch(const float *Xs, const int32_t *Xe, int64_t m, const
   de_predict_batch_kernel<<<dim3((unsigned)ceil_div(m, DE_TM), (unsigned)nens), DE_PRED_THREADS, smem, st>>>(net, ba);
   count_launches(1);
   HB_LAUNCH_CHECK("de_predict_batch_kernel");
-  return HB_OK;
-}
-
-// ------------------------------------------------------------------------------------------------ gated launchers
-// FeDeepEnsemble's member: BaseNet's layout (net.P = its P + din afterwards) with the gate [din] last
-static bool fe_layout(const hb_de_spec_t *spec, const hb_fe_gate_t *gate, DeNet &net, FeGate &fe) {
-  if (!gate || gate->kind < HB_FE_STG || gate->kind > HB_FE_HARD_CONCRETE || !(gate->temperature > 0.0f)) return false;
-  if (!de_layout(spec, net)) return false;
-  fe = FeGate{};
-  fe.off = net.P;
-  net.P += net.din;
-  fe.T = gate->temperature;
-  fe.t0 = gate->start_temp;
-  fe.t1 = gate->end_temp;
-  fe.tb = gate->anneal_base;
-  return true;
-}
-
-// floats of a gated fit's minibatch buffers: BaseNet's plus the unmasked inputs and the gate states, B in_ld each
-static int64_t fe_rows_floats(const DeNet &net, int64_t B) { return de_rows_floats(net, B) + 2 * B * net.in_ld; }
-
-int64_t fe_num_params(const hb_de_spec_t *spec) {
-  DeNet net;
-  return de_layout(spec, net) ? net.P + net.din : -1;
-}
-
-int64_t fe_fit_ws_query(const hb_de_spec_t *spec, int64_t E) {
-  const int64_t P = fe_num_params(spec);
-  if (P < 0 || E < 1 || E > HB_DE_MAX_MEMBERS) return -1;
-  return 3 * E * P * (int64_t)sizeof(float);
-}
-
-template <int GATE>
-static int fe_fit_launch(const DeNet &net, const DeFitArgs &a, const FeGate &fe, int64_t E, size_t smem, cudaStream_t st) {
-  HB_CUDA(cudaFuncSetAttribute(fe_fit_kernel<GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  fe_fit_kernel<GATE><<<(unsigned)E, DE_FIT_THREADS, smem, st>>>(net, a, fe);
-  return HB_OK;
-}
-
-int launch_fe_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec,
-                  const hb_fe_gate_t *gate, int64_t E, float *params, double lr, float l1, int64_t batch_size,
-                  int64_t num_epochs, const int32_t *perm, const float *draws, uint64_t seed, float *losses, void *ws,
-                  int64_t ws_bytes, cudaStream_t st) {
-  DeNet net;
-  FeGate fe;
-  if (!fe_layout(spec, gate, net, fe) || E < 1 || E > HB_DE_MAX_MEMBERS || n < 1 || n > (1 << 30) || batch_size < 1 ||
-      num_epochs < 0)
-    return HB_ERR_INVALID;
-  if (!y || !params || !ws || (num_epochs > 0 && !losses) || (net.dc > 0 && !Xc) || (net.ne > 0 && !Xe)) return HB_ERR_INVALID;
-  if (ws_bytes < fe_fit_ws_query(spec, E)) return HB_ERR_INVALID;
-  const int64_t B = n > batch_size ? batch_size : n;     // as launch_de_fit
-  if (fe_rows_floats(net, B) > HB_DE_MAX_BATCH_FLOATS) return HB_ERR_INVALID;
-  if (num_epochs == 0) return HB_OK;
-  DeFitArgs a;
-  a.Xc = Xc;
-  a.Xe = Xe;
-  a.y = y;
-  a.perm = perm;
-  a.params = params;
-  a.m1 = (float *)ws;
-  a.m2 = a.m1 + E * net.P;
-  a.grad = a.m2 + E * net.P;
-  a.losses = losses;
-  a.n = (int)n;
-  a.B = (int)B;
-  a.nb = (int)(n > batch_size ? n / batch_size : 1);
-  a.epochs = (int)num_epochs;
-  int h = 1;
-  while ((int64_t(1) << (2 * h)) < n) ++h;
-  a.h = h;
-  a.seed = seed;
-  a.lr = lr;
-  a.coef = (1.0f / (float)(n * net.O)) * l1;
-  fe.mcoef = net.dc > 0 ? (1.0f / (float)(n * net.O)) * gate->mask_reg : 0.0f;     // mask_loss only when Xc.shape[1] > 0
-  fe.draws = draws;
-  const size_t smem = (size_t)(fe_rows_floats(net, B) + DE_SCRATCH) * sizeof(float);
-  const int rc = gate->kind == HB_FE_STG        ? fe_fit_launch<1 + HB_FE_STG>(net, a, fe, E, smem, st)
-                 : gate->kind == HB_FE_CONCRETE ? fe_fit_launch<1 + HB_FE_CONCRETE>(net, a, fe, E, smem, st)
-                                                : fe_fit_launch<1 + HB_FE_HARD_CONCRETE>(net, a, fe, E, smem, st);
-  if (rc != HB_OK) return rc;
-  count_launches(1);
-  HB_LAUNCH_CHECK("fe_fit_kernel");
-  return HB_OK;
-}
-
-template <int GATE>
-static int fe_predict_launch(const DeNet &net, const DePredArgs &a, const FeGate &fe, unsigned grid, size_t smem,
-                              cudaStream_t st) {
-  HB_CUDA(cudaFuncSetAttribute(de_predict_kernel<false, GATE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  de_predict_kernel<false, GATE><<<grid, DE_PRED_THREADS, smem, st>>>(net, a, fe, GbSel{});
-  return HB_OK;
-}
-
-int launch_fe_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, const hb_fe_gate_t *gate,
-                      int64_t E, const float *params, const float *x_mul, const float *x_add, const float *y_mean,
-                      const float *y_std, int32_t member, const float *draws, uint64_t seed, uint64_t counter, float *mu,
-                      float *var, cudaStream_t st) {
-  DeNet net;
-  FeGate fe;
-  if (!fe_layout(spec, gate, net, fe) || E < 1 || E > HB_DE_MAX_MEMBERS || m < 0 || m > (int64_t(1) << 31) - DE_TM)
-    return HB_ERR_INVALID;
-  if (member < -1 || member >= E) return HB_ERR_INVALID;
-  if (!params || !y_mean || !y_std || !mu || (member < 0 && !var) || (net.ne > 0 && !Xe)) return HB_ERR_INVALID;
-  if (net.dc > 0 && (!Xs || !x_mul || !x_add)) return HB_ERR_INVALID;
-  if (m == 0) return HB_OK;
-  DePredArgs a;
-  a.Xs = Xs;
-  a.Xe = Xe;
-  a.params = params;
-  a.x_mul = x_mul;
-  a.x_add = x_add;
-  a.y_mean = y_mean;
-  a.y_std = y_std;
-  a.mu = mu;
-  a.var = var;
-  a.dmu = a.dvar = nullptr;
-  a.m = (int)m;
-  a.E = (int)E;
-  a.member = member;
-  fe.draws = draws;
-  fe.seed = seed;
-  fe.counter = counter;
-  const int64_t ne = member >= 0 ? 1 : E;
-  const size_t smem =
-      (size_t)(de_rows_floats(net, DE_TM) + DE_SCRATCH + (2 * ne + 1) * DE_TM * net.O + net.din) * sizeof(float);
-  const unsigned grid = (unsigned)ceil_div(m, DE_TM);
-  const int rc = gate->kind == HB_FE_STG        ? fe_predict_launch<1 + HB_FE_STG>(net, a, fe, grid, smem, st)
-                 : gate->kind == HB_FE_CONCRETE ? fe_predict_launch<1 + HB_FE_CONCRETE>(net, a, fe, grid, smem, st)
-                                                : fe_predict_launch<1 + HB_FE_HARD_CONCRETE>(net, a, fe, grid, smem, st);
-  if (rc != HB_OK) return rc;
-  count_launches(1);
-  HB_LAUNCH_CHECK("de_predict_kernel (gated)");
-  return HB_OK;
-}
-
-// ------------------------------------------------------------------------------------------------ Gumbel launchers
-// GumbelDeepEnsemble's member: BaseNet's layout over the selected width (num_cont -> r when num_cont > 0), then the
-// logits [r, num_cont] last.  The random prior net keeps the original width, so it only runs when r = num_cont or there
-// are no numeric columns; anything else is rejected (the reference fails with a shape error in forward).
-static bool gb_layout(const hb_de_spec_t *spec, int64_t r, DeNet &net, GbSel &gb) {
-  if (!spec || r < 1 || r > HB_DE_MAX_IN || spec->num_cont < 0 || spec->num_cont > HB_DE_MAX_IN) return false;
-  const int dx = spec->num_cont;
-  if (spec->rand_prior && dx > 0 && r != dx) return false;
-  hb_de_spec_t sel = *spec;
-  if (dx > 0) sel.num_cont = (int32_t)r;
-  if (!de_layout(&sel, net)) return false;
-  gb = GbSel{};
-  gb.off = net.P;
-  gb.dx = dx;
-  gb.r = dx > 0 ? (int)r : 0;      // without numeric columns the logits [r, 0] are empty and nothing is drawn
-  gb.x_ld = dx > 0 ? (dx | 1) : 0;
-  net.P += gb.r * dx;
-  return true;
-}
-
-// floats of a Gumbel fit's minibatch buffers: BaseNet's over the selected width plus the numeric rows, B x_ld
-static int64_t gb_rows_floats(const DeNet &net, const GbSel &gb, int64_t B) { return de_rows_floats(net, B) + B * gb.x_ld; }
-
-int64_t gb_num_params(const hb_de_spec_t *spec, int64_t reduced_dim) {
-  DeNet net;
-  GbSel gb;
-  return gb_layout(spec, reduced_dim, net, gb) ? net.P : -1;
-}
-
-int64_t gb_fit_ws_query(const hb_de_spec_t *spec, int64_t reduced_dim, int64_t E) {
-  DeNet net;
-  GbSel gb;
-  if (!gb_layout(spec, reduced_dim, net, gb) || E < 1 || E > HB_DE_MAX_MEMBERS) return -1;
-  return (3 * E * (int64_t)net.P + E * (int64_t)gb.r * gb.dx) * (int64_t)sizeof(float);
-}
-
-int launch_gb_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec,
-                  int64_t reduced_dim, int64_t E, float *params, double lr, float l1, int64_t batch_size, int64_t num_epochs,
-                  const int32_t *perm, const float *draws, uint64_t seed, float *losses, void *ws, int64_t ws_bytes,
-                  cudaStream_t st) {
-  DeNet net;
-  GbSel gb;
-  if (!gb_layout(spec, reduced_dim, net, gb) || E < 1 || E > HB_DE_MAX_MEMBERS || n < 1 || n > (1 << 30) ||
-      batch_size < 1 || num_epochs < 0)
-    return HB_ERR_INVALID;
-  if (!y || !params || !ws || (num_epochs > 0 && !losses) || (gb.dx > 0 && !Xc) || (net.ne > 0 && !Xe)) return HB_ERR_INVALID;
-  if (ws_bytes < gb_fit_ws_query(spec, reduced_dim, E)) return HB_ERR_INVALID;
-  const int64_t B = n > batch_size ? batch_size : n;
-  if (gb_rows_floats(net, gb, B) > HB_DE_MAX_BATCH_FLOATS) return HB_ERR_INVALID;
-  if (num_epochs == 0) return HB_OK;
-  DeFitArgs a;
-  a.Xc = Xc;
-  a.Xe = Xe;
-  a.y = y;
-  a.perm = perm;
-  a.params = params;
-  a.m1 = (float *)ws;
-  a.m2 = a.m1 + E * net.P;
-  a.grad = a.m2 + E * net.P;
-  a.losses = losses;
-  a.n = (int)n;
-  a.B = (int)B;
-  a.nb = (int)((n + B - 1) / B);      // no drop_last (gumbel_linear.py:72): the partial last minibatch is trained
-  a.epochs = (int)num_epochs;
-  int h = 1;
-  while ((int64_t(1) << (2 * h)) < n) ++h;
-  a.h = h;
-  a.seed = seed;
-  a.lr = lr;
-  a.coef = (1.0f / (float)(n * net.O)) * l1;
-  gb.draws = draws;
-  gb.w = a.grad + E * net.P;
-  const size_t smem = (size_t)(gb_rows_floats(net, gb, B) + DE_SCRATCH) * sizeof(float);
-  HB_CUDA(cudaFuncSetAttribute(gb_fit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  gb_fit_kernel<<<(unsigned)E, DE_FIT_THREADS, smem, st>>>(net, a, gb);
-  count_launches(1);
-  HB_LAUNCH_CHECK("gb_fit_kernel");
-  return HB_OK;
-}
-
-// W of members e0 + blockIdx.x for one predict call: uniforms from gb.draws [E, r, dx] or Philox keyed by
-// (seed, counter, member), so every candidate tile of the call uses the same W
-__global__ void __launch_bounds__(DE_PRED_THREADS) gb_weights_kernel(const float *params, int P, int e0,
-                                                                     const __grid_constant__ GbSel gb) {
-  const int e = e0 + blockIdx.x, wsz = gb.r * gb.dx;
-  gb_build_w(params + (size_t)e * P + gb.off, gb.r, gb.dx, gb.T, gb.w + (size_t)e * wsz, [&](int j, int k) {
-    const int q = j * gb.dx + k;
-    const uint64_t stream = ((uint64_t)GB_TAG_EVAL << 32) | ((uint32_t)e << 16) | (uint32_t)(q >> 1);
-    return gb.draws ? gb.draws[(size_t)e * wsz + q] : fe_draw<1 + HB_FE_CONCRETE>(gb.seed, gb.counter, stream, q & 1);
-  });
-}
-
-int launch_gb_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t reduced_dim,
-                      float temperature, int64_t E, const float *params, const float *x_mul, const float *x_add,
-                      const float *y_mean, const float *y_std, int32_t member, const float *draws, uint64_t seed,
-                      uint64_t counter, float *mu, float *var, void *ws, int64_t ws_bytes, cudaStream_t st) {
-  DeNet net;
-  GbSel gb;
-  if (!gb_layout(spec, reduced_dim, net, gb) || !(temperature > 0.0f) || E < 1 || E > HB_DE_MAX_MEMBERS || m < 0 ||
-      m > (int64_t(1) << 31) - DE_TM)
-    return HB_ERR_INVALID;
-  if (member < -1 || member >= E) return HB_ERR_INVALID;
-  if (!params || !y_mean || !y_std || !mu || (member < 0 && !var) || (net.ne > 0 && !Xe)) return HB_ERR_INVALID;
-  if (gb.dx > 0 && (!Xs || !x_mul || !x_add || !ws || ws_bytes < E * (int64_t)gb.r * gb.dx * (int64_t)sizeof(float)))
-    return HB_ERR_INVALID;
-  if (m == 0) return HB_OK;
-  DePredArgs a;
-  a.Xs = Xs;
-  a.Xe = Xe;
-  a.params = params;
-  a.x_mul = x_mul;
-  a.x_add = x_add;
-  a.y_mean = y_mean;
-  a.y_std = y_std;
-  a.mu = mu;
-  a.var = var;
-  a.dmu = a.dvar = nullptr;
-  a.m = (int)m;
-  a.E = (int)E;
-  a.member = member;
-  gb.T = temperature;
-  gb.draws = draws;
-  gb.seed = seed;
-  gb.counter = counter;
-  gb.w = (float *)ws;
-  const int64_t ne = member >= 0 ? 1 : E;
-  if (gb.dx > 0) {
-    gb_weights_kernel<<<(unsigned)ne, DE_PRED_THREADS, 0, st>>>(params, net.P, member >= 0 ? member : 0, gb);
-    count_launches(1);
-    HB_LAUNCH_CHECK("gb_weights_kernel");
-  }
-  const size_t smem =
-      (size_t)(de_rows_floats(net, DE_TM) + DE_SCRATCH + (2 * ne + 1) * DE_TM * net.O + DE_TM * gb.x_ld) * sizeof(float);
-  const unsigned grid = (unsigned)ceil_div(m, DE_TM);
-  HB_CUDA(cudaFuncSetAttribute(de_predict_kernel<false, DE_GUMBEL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  de_predict_kernel<false, DE_GUMBEL><<<grid, DE_PRED_THREADS, smem, st>>>(net, a, FeGate{}, gb);
-  count_launches(1);
-  HB_LAUNCH_CHECK("de_predict_kernel (Gumbel)");
   return HB_OK;
 }
 

@@ -225,15 +225,25 @@ int launch_ga_survive(const float *X, const float *F, const float *G, const floa
 int64_t embed_violation_ws_query(int64_t m, int64_t e, int64_t D);
 int launch_embed_violation(const float *Y, int64_t m, int64_t e, const float *B, int64_t D, float *G, void *ws, int64_t ws_bytes,
                            cudaStream_t st);
-// ensemble.cu: the deep-ensemble surrogate's fit (one CTA per member) and predict / input gradients (dmu == nullptr: none)
-int64_t de_num_params(const hb_de_spec_t *spec);
-int64_t de_fit_ws_query(const hb_de_spec_t *spec, int64_t E);
-int launch_de_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec, int64_t E,
-                  float *params, double lr, float l1, int64_t batch_size, int64_t num_epochs, const int32_t *perm,
-                  uint64_t seed, float *losses, void *ws, int64_t ws_bytes, cudaStream_t st);
-int launch_de_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t E, const float *params,
-                      const float *x_mul, const float *x_add, const float *y_mean, const float *y_std, int32_t member,
-                      float *mu, float *var, float *dmu, float *dvar, cudaStream_t st);
+// ensemble.cu: the deep ensembles' fit (one CTA per member) and predict / input gradients (dmu == nullptr: none).  The
+// variant: DeepEnsemble's BaseNet members (DeVariant{}), FeDeepEnsemble's gated ones (GATED, the gate) or
+// GumbelDeepEnsemble's (GUMBEL, r = reduced_dim and T = predict's temperature); draws, seed / counter and ws are the
+// selection layer's (NULL / 0 for BaseNet)
+struct DeVariant {
+  enum Kind { BASE, GATED, GUMBEL } kind;
+  const hb_fe_gate_t *gate;
+  int64_t r;
+  float T;
+};
+int64_t de_num_params(const hb_de_spec_t *spec, const DeVariant &v);
+int64_t de_fit_ws_query(const hb_de_spec_t *spec, const DeVariant &v, int64_t E);
+int launch_de_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec, const DeVariant &v,
+                  int64_t E, float *params, double lr, float l1, int64_t batch_size, int64_t num_epochs, const int32_t *perm,
+                  const float *draws, uint64_t seed, float *losses, void *ws, int64_t ws_bytes, cudaStream_t st);
+int launch_de_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, const DeVariant &v, int64_t E,
+                      const float *params, const float *x_mul, const float *x_add, const float *y_mean, const float *y_std,
+                      int32_t member, const float *draws, uint64_t seed, uint64_t counter, float *mu, float *var,
+                      float *dmu, float *dvar, void *ws, int64_t ws_bytes, cudaStream_t st);
 // nens ensembles of one spec: the fit (one CTA per (ensemble, member)) and predict (mu / var output-major, optional draws)
 int launch_de_fit_batch(const float *Xc, const int32_t *Xe, const float *y, const int64_t *off, int64_t nens,
                         const hb_de_spec_t *spec, int64_t E, float *params, double lr, float l1, int64_t batch_size,
@@ -242,28 +252,6 @@ int launch_de_predict_batch(const float *Xs, const int32_t *Xe, int64_t m, const
                             const float *params, const float *x_mul, const float *x_add, const float *y_mean,
                             const float *y_std, float *mu, float *var, int64_t n_samples, const float *xi, uint64_t seed,
                             uint64_t counter, float *y_samp, cudaStream_t st);
-// the feature-gated ensemble (FeDeepEnsemble): the same fit and predict kernels with the gate compiled in
-int64_t fe_num_params(const hb_de_spec_t *spec);
-int64_t fe_fit_ws_query(const hb_de_spec_t *spec, int64_t E);
-int launch_fe_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec,
-                  const hb_fe_gate_t *gate, int64_t E, float *params, double lr, float l1, int64_t batch_size,
-                  int64_t num_epochs, const int32_t *perm, const float *draws, uint64_t seed, float *losses, void *ws,
-                  int64_t ws_bytes, cudaStream_t st);
-int launch_fe_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, const hb_fe_gate_t *gate,
-                      int64_t E, const float *params, const float *x_mul, const float *x_add, const float *y_mean,
-                      const float *y_std, int32_t member, const float *draws, uint64_t seed, uint64_t counter, float *mu,
-                      float *var, cudaStream_t st);
-// the Gumbel-selection ensemble (GumbelDeepEnsemble): the same fit and predict kernels with the selection layer compiled in
-int64_t gb_num_params(const hb_de_spec_t *spec, int64_t reduced_dim);
-int64_t gb_fit_ws_query(const hb_de_spec_t *spec, int64_t reduced_dim, int64_t E);
-int launch_gb_fit(const float *Xc, const int32_t *Xe, const float *y, int64_t n, const hb_de_spec_t *spec,
-                  int64_t reduced_dim, int64_t E, float *params, double lr, float l1, int64_t batch_size, int64_t num_epochs,
-                  const int32_t *perm, const float *draws, uint64_t seed, float *losses, void *ws, int64_t ws_bytes,
-                  cudaStream_t st);
-int launch_gb_predict(const float *Xs, const int32_t *Xe, int64_t m, const hb_de_spec_t *spec, int64_t reduced_dim,
-                      float temperature, int64_t E, const float *params, const float *x_mul, const float *x_add,
-                      const float *y_mean, const float *y_std, int32_t member, const float *draws, uint64_t seed,
-                      uint64_t counter, float *mu, float *var, void *ws, int64_t ws_bytes, cudaStream_t st);
 
 // hypervolume.cu: GeneralBO's Monte-Carlo EHVI selection round, bit for bit with general.hypervolume
 int64_t ehvi_ws_query(int64_t n, int64_t K, int64_t m, int64_t n_mc);

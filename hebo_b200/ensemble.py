@@ -18,6 +18,7 @@ Extra conf key: ``device`` (default 'cuda').
 from __future__ import annotations
 
 import ctypes as C
+from importlib import import_module
 
 import numpy as np
 import torch
@@ -87,11 +88,10 @@ def raw_to_state_dict(raw: torch.Tensor, layout) -> dict:
     return out
 
 
-def _reference_basenet():
-    """BaseNet of an installed HEBO, or None."""
+def _reference_net(module: str, name: str):
+    """Class `name` of an installed HEBO's hebo.models.nn.`module`, or None."""
     try:  # pragma: no cover - depends on the environment
-        from hebo.models.nn.deep_ensemble import BaseNet
-        return BaseNet
+        return getattr(import_module(f"hebo.models.nn.{module}"), name)
     except Exception:
         return None
 
@@ -164,7 +164,7 @@ class DeepEnsemble(BaseModel):
         self.lr = self.conf.setdefault("lr", 5e-3)
         self.adv_eps = self.conf.setdefault("adv_eps", 0.)              # accepted, unused (as in the reference)
         self.verbose = self.conf.setdefault("verbose", False)
-        ref_basenet = _reference_basenet()
+        ref_basenet = _reference_net("deep_ensemble", "BaseNet")
         self.basenet_cls = self.conf.setdefault("basenet_cls", ref_basenet)
         assert self.num_ensembles > 0
         if self.basenet_cls is not None and not _is_basenet(self.basenet_cls, ref_basenet):
@@ -309,8 +309,8 @@ class DeepEnsemble(BaseModel):
 
     def fit_state(self):
         """Views of the fit workspace: Adam's exp_avg, exp_avg_sq and the last step's gradient, each [E, P]."""
-        w = self.fit_ws.view(torch.float32).view(3, self.num_ensembles, self.P)
-        return w[0], w[1], w[2]
+        E, P = self.num_ensembles, self.P
+        return tuple(self.fit_ws.view(torch.float32)[:3 * E * P].view(3, E, P))
 
     # ------------------------------------------------------------------ predict (deep_ensemble.py:95-116)
     def _scal_dev(self):
@@ -440,11 +440,10 @@ class EnsembleBatch:
     def __init__(self, models):
         m0 = models[0]
         assert all(m.fitted for m in models), "fit() first"
-        if any(isinstance(m, FeDeepEnsemble) for m in models):
-            raise TypeError("EnsembleBatch: a FeDeepEnsemble predicts through hb_fe_predict, which applies its gate")
-        if any(isinstance(m, GumbelDeepEnsemble) for m in models):
-            raise TypeError("EnsembleBatch: a GumbelDeepEnsemble predicts through hb_gumbel_predict, which applies its "
-                            "selection layer")
+        for m in models:
+            if isinstance(m, FeatureSelectionEnsemble):
+                raise TypeError(f"EnsembleBatch: a {type(m).__name__} predicts through {m._C_PREDICT}, which applies its "
+                                "selection layer")
         self.models, self.spec, self.E, self.device = models, m0._spec, m0.num_ensembles, m0.device
         self.num_cont, self.num_out = m0.num_cont, len(models) * m0.num_out
         self.params = _stacked_params(models)
@@ -509,6 +508,100 @@ def fit_ensembles(models, Xc, Xe, ys) -> None:
         m._finish_fit(Xc, Xe, ys[b], preps[b][3])
 
 
+class FeatureSelectionEnsemble(DeepEnsemble):
+    """The host side shared by FeDeepEnsemble and GumbelDeepEnsemble: a DeepEnsemble whose members pass their inputs
+    through a random selection layer, after BaseNet's parameters, before the first hidden layer.  A subclass names its C
+    entry points (_C_FIT, _C_FIT_WS, _C_PREDICT), the variant arguments they take after the spec (_layout_args,
+    _fit_args, _predict_args, the last with predict's workspace tensor or None) and what a fit of T epochs leaves for
+    predict (_trained_epochs).
+
+    The selection is random in predict too (the reference redraws it on every forward): each call draws afresh from a
+    Philox key taken from torch's global generator, or from the given ``seed`` / ``counter``, so a call is reproducible
+    under ``torch.manual_seed``.  No input gradients (``support_grad = False``).  Like DeepEnsemble, the fit does not call
+    ``torch.seed()``, a deliberate deviation that keeps it reproducible under ``torch.manual_seed``."""
+    support_grad = False
+
+    def fit(self, Xc_, Xe_, y_, perm=None, draws=None, eval_draws=None):
+        """perm: as DeepEnsemble.fit.  draws: optional training draws (``draws_shape``); otherwise Philox draws on the
+        device.  eval_draws: optional draws of the noise estimate's predict (``eval_draws_shape``; tests replaying the
+        reference's own draws)."""
+        Xc, Xe, y, valid = self._prepare_fit(Xc_, Xe_, y_, perm)
+        if draws is not None:
+            draws = torch.as_tensor(draws, dtype=torch.float32)
+            if tuple(draws.shape) != self.draws_shape(y.shape[0]):
+                raise ValueError(f"draws must be {list(self.draws_shape(y.shape[0]))}, got {list(draws.shape)}")
+        self._fit_dev(Xc, Xe, y, perm, self.seed, draws)
+        self._finish_fit(Xc_, Xe_, y_, valid, draws=eval_draws)
+
+    def _fit_dev(self, Xc, Xe, y, perm, seed, draws=None):
+        lib, dev, E = _lib.lib(), self.device, self.num_ensembles
+        n, T = y.shape[0], int(self.num_epochs)
+        xc = Xc.to(dev, torch.float32).contiguous() if self.num_cont > 0 else None
+        xe = Xe.to(dev, torch.int32).contiguous() if self.num_enum > 0 else None
+        yd = y.to(dev, torch.float32).contiguous()
+        pd_ = None if perm is None else torch.as_tensor(perm).to(dev, torch.int32).contiguous()
+        dd = None if draws is None else draws.to(dev, torch.float32).contiguous()
+        need = int(getattr(lib, self._C_FIT_WS)(C.byref(self._spec), *self._layout_args(), E))
+        self.fit_ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        losses = torch.empty(E, max(1, T), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(getattr(lib, self._C_FIT)(_lib.ptr(xc), _lib.ptr(xe), _lib.ptr(yd), n, C.byref(self._spec),
+                                                 *self._fit_args(), E, _lib.ptr(self.params), float(self.lr), float(self.l1),
+                                                 int(self.batch_size), T, _lib.ptr(pd_), _lib.ptr(dd), seed & (2 ** 64 - 1),
+                                                 _lib.ptr(losses), _lib.ptr(self.fit_ws), need, _lib.stream_ptr()),
+                       self._C_FIT)
+        self.losses = losses[:, :T]
+        if T > 0:
+            self._trained_epochs(T)
+        if self.verbose:
+            self._print_losses()
+
+    def _predict_dev(self, Xs, xe, grad=False, member=-1, draws=None, seed=None, counter=0):
+        if grad:
+            raise NotImplementedError(f"{type(self).__name__}: no input gradients (support_grad = False)")
+        lib, dev = _lib.lib(), self.device
+        assert self.fitted, "fit() first"
+        m = (Xs if Xs is not None else xe).shape[0]
+        xm, xa, ym, ys = self._scal_dev()
+        mu = torch.empty(m, self.num_out, dtype=torch.float32, device=dev)
+        var = torch.empty(m, self.num_out, dtype=torch.float32, device=dev) if member < 0 else None
+        if draws is not None:
+            draws = torch.as_tensor(draws).to(dev, torch.float32).contiguous()
+            if tuple(draws.shape) != self.eval_draws_shape():
+                raise ValueError(f"eval draws must be {list(self.eval_draws_shape())}, got {list(draws.shape)}")
+        elif seed is None:
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
+        head, ws = self._predict_args()
+        tail = () if ws is None else (_lib.ptr(ws), ws.numel() * ws.element_size())
+        with torch.cuda.device(dev):
+            _lib.check(getattr(lib, self._C_PREDICT)(_lib.ptr(Xs), _lib.ptr(xe), m, C.byref(self._spec), *head,
+                                                     self.num_ensembles, _lib.ptr(self.params), _lib.ptr(xm), _lib.ptr(xa),
+                                                     _lib.ptr(ym), _lib.ptr(ys), int(member), _lib.ptr(draws),
+                                                     int(seed or 0) & (2 ** 64 - 1), int(counter) & (2 ** 64 - 1),
+                                                     _lib.ptr(mu), _lib.ptr(var), *tail, _lib.stream_ptr()),
+                       self._C_PREDICT)
+        return mu, var
+
+    def predict(self, Xc, Xe=None, draws=None, seed=None, counter=0):
+        """(py, ps2) [m, num_out] under a fresh selection: CPU tensors for CPU inputs, device tensors for device inputs.
+        draws (``eval_draws_shape``): the selection's raw draws (tests); otherwise Philox keyed by (seed, counter), seed
+        from torch's generator when None."""
+        probe = Xc if (Xc is not None and self.num_cont > 0) else Xe
+        on_cpu = not (torch.is_tensor(probe) and probe.is_cuda)
+        xs, xe, _ = self._inputs(Xc, Xe)
+        mu, var = self._predict_dev(xs, xe, draws=draws, seed=seed, counter=counter)
+        return (mu.cpu(), var.cpu()) if on_cpu else (mu, var)
+
+    def sample_y(self, Xc, Xe=None, n_samples: int = 1):
+        """BaseModel.sample_y (base_model.py:78-84): one predict, then py + sqrt(ps2) * torch.randn per sample."""
+        py, ps2 = self.predict(Xc, Xe)
+        ps = ps2.sqrt()
+        samp = torch.zeros(n_samples, py.shape[0], self.num_out, device=py.device)
+        for i in range(n_samples):
+            samp[i] = py + ps * torch.randn(py.shape).to(py.device)
+        return samp
+
+
 _FE_KINDS = {"stg": _lib.HB_FE_STG, "concrete": _lib.HB_FE_CONCRETE, "hard_concrete": _lib.HB_FE_HARD_CONCRETE}
 _FE_DEFAULT_T = {"stg": 1.0, "concrete": 0.1, "hard_concrete": 0.1}      # the layers' constructor defaults
 
@@ -519,7 +612,7 @@ def fe_epoch_temperature(start_temp: float, end_temp: float, anneal_base: float,
     return float(np.float32(max(start_temp * anneal_base ** epoch, end_temp)))
 
 
-class FeDeepEnsemble(DeepEnsemble):
+class FeDeepEnsemble(FeatureSelectionEnsemble):
     """Drop-in for ``hebo.models.nn.fe_deep_ensemble.FeDeepEnsemble``: a DeepEnsemble whose members gate their input
     columns with a learned feature-selection layer (``fe_layer``: 'stg' (default), 'concrete' or 'hard_concrete') before
     the first hidden layer, so irrelevant inputs can be switched off.  The fit runs in one ``hb_fe_fit`` launch and
@@ -529,13 +622,8 @@ class FeDeepEnsemble(DeepEnsemble):
     mask_reg 0.1, start_temp 1.0, end_temp 0.1, anneal_base 0.99.  A member's parameters are FeNet's state_dict in
     registration order: BaseNet's, then ``feature_select.mu`` (stg) or ``feature_select.logits`` [din] last.  The L1 term
     covers weights only, the mask penalty applies when there are numeric columns, and the random prior net (rand_prior)
-    is built but not evaluated, all as the reference does.
-
-    Masks are random in predict too (the reference redraws them on every forward): each call draws fresh eval masks from
-    a Philox key taken from torch's global generator, or from the given ``seed`` / ``counter``, so a call is reproducible
-    under ``torch.manual_seed``.  No input gradients (``support_grad = False``).  Like DeepEnsemble, the fit does not
-    call ``torch.seed()``, a deliberate deviation that keeps it reproducible under ``torch.manual_seed``."""
-    support_grad = False
+    is built but not evaluated, all as the reference does.  Predict draws fresh eval masks on every call."""
+    _C_FIT, _C_FIT_WS, _C_PREDICT = "hb_fe_fit", "hb_fe_fit_workspace_bytes", "hb_fe_predict"
 
     def __init__(self, num_cont, num_enum, num_out, **conf):
         fe_layer = conf.get("fe_layer", "stg")
@@ -543,7 +631,7 @@ class FeDeepEnsemble(DeepEnsemble):
             raise KeyError(f"FeDeepEnsemble: unknown fe_layer {fe_layer!r}, can only be [stg|concrete|hard_concrete]")
         conf.pop("basenet_cls", None)
         super().__init__(num_cont, num_enum, num_out, **conf)
-        self.basenet_cls = _reference_fenet()
+        self.basenet_cls = _reference_net("fe_deep_ensemble", "FeNet")
         self.conf["basenet_cls"] = self.basenet_cls
         self.fe_layer = fe_layer
         self.temperature = self.conf.get("temperature")
@@ -565,98 +653,27 @@ class FeDeepEnsemble(DeepEnsemble):
                            float(self.anneal_base), float(self.mask_reg))
 
     def draws_shape(self, n: int):
-        """Shape of fit's explicit training draws for n kept rows: [E, num_epochs, minibatches, rows, din]."""
+        """Shape of fit's explicit training draws for n kept rows: [E, num_epochs, minibatches, rows, din]; N(0, 1) for
+        stg, U(0, 1) for the concrete layers."""
         bs = int(self.batch_size)
         return (self.num_ensembles, int(self.num_epochs), n // bs if n > bs else 1, min(n, bs), self.din)
 
-    # ------------------------------------------------------------------ fit (fe_deep_ensemble.py:46-75)
-    def fit(self, Xc_, Xe_, y_, perm=None, draws=None, eval_draws=None):
-        """perm: as DeepEnsemble.fit.  draws: optional training draws (``draws_shape``): N(0, 1) for stg, U(0, 1) for the
-        concrete layers; otherwise Philox draws on the device.  eval_draws: optional [E, din] draws of the noise
-        estimate's predict (tests replaying the reference's own draws)."""
-        Xc, Xe, y, valid = self._prepare_fit(Xc_, Xe_, y_, perm)
-        if draws is not None:
-            draws = torch.as_tensor(draws, dtype=torch.float32)
-            if tuple(draws.shape) != self.draws_shape(y.shape[0]):
-                raise ValueError(f"draws must be {list(self.draws_shape(y.shape[0]))}, got {list(draws.shape)}")
-        self._fit_dev(Xc, Xe, y, perm, self.seed, draws)
-        self._finish_fit(Xc_, Xe_, y_, valid, draws=eval_draws)
+    def eval_draws_shape(self):
+        """Shape of predict's explicit draws: one per member and input column, [E, din]."""
+        return (self.num_ensembles, self.din)
 
-    def _fit_dev(self, Xc, Xe, y, perm, seed, draws=None):
-        lib, dev, E = _lib.lib(), self.device, self.num_ensembles
-        n, T = y.shape[0], int(self.num_epochs)
-        xc = Xc.to(dev, torch.float32).contiguous() if self.num_cont > 0 else None
-        xe = Xe.to(dev, torch.int32).contiguous() if self.num_enum > 0 else None
-        yd = y.to(dev, torch.float32).contiguous()
-        pd_ = None if perm is None else torch.as_tensor(perm).to(dev, torch.int32).contiguous()
-        dd = None if draws is None else draws.to(dev, torch.float32).contiguous()
-        need = int(lib.hb_fe_fit_workspace_bytes(C.byref(self._spec), E))
-        self.fit_ws = torch.empty(need, dtype=torch.uint8, device=dev)
-        losses = torch.empty(E, max(1, T), dtype=torch.float32, device=dev)
-        gate = self._gate()
-        with torch.cuda.device(dev):
-            _lib.check(lib.hb_fe_fit(_lib.ptr(xc), _lib.ptr(xe), _lib.ptr(yd), n, C.byref(self._spec), C.byref(gate), E,
-                                     _lib.ptr(self.params), float(self.lr), float(self.l1), int(self.batch_size), T,
-                                     _lib.ptr(pd_), _lib.ptr(dd), seed & (2 ** 64 - 1), _lib.ptr(losses),
-                                     _lib.ptr(self.fit_ws), need, _lib.stream_ptr()), "hb_fe_fit")
-        self.losses = losses[:, :T]
-        if T > 0 and self.fe_layer != "stg":       # predict uses the last epoch's temperature
+    def _layout_args(self):
+        return ()
+
+    def _fit_args(self):
+        return (C.byref(self._gate()),)
+
+    def _predict_args(self):
+        return (C.byref(self._gate()),), None
+
+    def _trained_epochs(self, T: int):
+        if self.fe_layer != "stg":       # predict uses the last epoch's temperature
             self.gate_temperature = fe_epoch_temperature(self.start_temp, self.end_temp, self.anneal_base, T - 1)
-        if self.verbose:
-            self._print_losses()
-
-    # ------------------------------------------------------------------ predict
-    def _predict_dev(self, Xs, xe, grad=False, member=-1, draws=None, seed=None, counter=0):
-        if grad:
-            raise NotImplementedError("FeDeepEnsemble: no input gradients (support_grad = False)")
-        lib, dev = _lib.lib(), self.device
-        assert self.fitted, "fit() first"
-        m = (Xs if Xs is not None else xe).shape[0]
-        xm, xa, ym, ys = self._scal_dev()
-        mu = torch.empty(m, self.num_out, dtype=torch.float32, device=dev)
-        var = torch.empty(m, self.num_out, dtype=torch.float32, device=dev) if member < 0 else None
-        if draws is not None:
-            draws = torch.as_tensor(draws).to(dev, torch.float32).contiguous()
-            if tuple(draws.shape) != (self.num_ensembles, self.din):
-                raise ValueError(f"eval draws must be [{self.num_ensembles}, {self.din}], got {list(draws.shape)}")
-        elif seed is None:
-            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-        gate = self._gate()
-        with torch.cuda.device(dev):
-            _lib.check(lib.hb_fe_predict(_lib.ptr(Xs), _lib.ptr(xe), m, C.byref(self._spec), C.byref(gate),
-                                         self.num_ensembles, _lib.ptr(self.params), _lib.ptr(xm), _lib.ptr(xa), _lib.ptr(ym),
-                                         _lib.ptr(ys), int(member), _lib.ptr(draws), int(seed or 0) & (2 ** 64 - 1),
-                                         int(counter) & (2 ** 64 - 1), _lib.ptr(mu), _lib.ptr(var), _lib.stream_ptr()),
-                       "hb_fe_predict")
-        return mu, var
-
-    def predict(self, Xc, Xe=None, draws=None, seed=None, counter=0):
-        """(py, ps2) [m, num_out] under fresh eval masks: CPU tensors for CPU inputs, device tensors for device inputs.
-        draws [E, din]: the masks' raw draws (tests); otherwise Philox keyed by (seed, counter), seed from torch's
-        generator when None."""
-        probe = Xc if (Xc is not None and self.num_cont > 0) else Xe
-        on_cpu = not (torch.is_tensor(probe) and probe.is_cuda)
-        xs, xe, _ = self._inputs(Xc, Xe)
-        mu, var = self._predict_dev(xs, xe, draws=draws, seed=seed, counter=counter)
-        return (mu.cpu(), var.cpu()) if on_cpu else (mu, var)
-
-    def sample_y(self, Xc, Xe=None, n_samples: int = 1):
-        """BaseModel.sample_y (base_model.py:78-84): one predict, then py + sqrt(ps2) * torch.randn per sample."""
-        py, ps2 = self.predict(Xc, Xe)
-        ps = ps2.sqrt()
-        samp = torch.zeros(n_samples, py.shape[0], self.num_out, device=py.device)
-        for i in range(n_samples):
-            samp[i] = py + ps * torch.randn(py.shape).to(py.device)
-        return samp
-
-
-def _reference_fenet():
-    """FeNet of an installed HEBO, or None."""
-    try:  # pragma: no cover - depends on the environment
-        from hebo.models.nn.fe_deep_ensemble import FeNet
-        return FeNet
-    except Exception:
-        return None
 
 
 def gumbel_epoch_temperature(epoch: int) -> float:
@@ -664,7 +681,7 @@ def gumbel_epoch_temperature(epoch: int) -> float:
     return float(np.float32(0.8 ** epoch + 0.1))
 
 
-class GumbelDeepEnsemble(DeepEnsemble):
+class GumbelDeepEnsemble(FeatureSelectionEnsemble):
     """Drop-in for ``hebo.models.nn.gumbel_linear.GumbelDeepEnsemble``: a DeepEnsemble whose members map their numeric
     columns to ``reduced_dim`` learned soft selections of them (a Gumbel-softmax selection layer, one draw of its
     [reduced_dim, num_cont] matrix per forward) before the first hidden layer.  The fit runs in one ``hb_gumbel_fit``
@@ -675,13 +692,9 @@ class GumbelDeepEnsemble(DeepEnsemble):
     order: BaseNet's over the selected width, then ``feature_select.logits`` [reduced_dim, num_cont] last.  The hidden
     layers (rebuilt by GumbelNet when num_cont > 0) keep torch's default nn.Linear initialisation, the logits start at
     zero.  Every epoch's minibatches cover all rows (no drop_last); the L1 term covers weights only; the temperature is
-    0.8**epoch + 0.1.  The random prior net (rand_prior) needs reduced_dim == num_cont or no numeric columns.
-
-    The selection is random in predict too (the reference redraws it on every forward): each call draws one matrix per
-    member from a Philox key taken from torch's global generator, or from the given ``seed`` / ``counter``, at the last
-    trained epoch's temperature.  No input gradients (``support_grad = False``).  Like DeepEnsemble, the fit does not
-    call ``torch.seed()``, a deliberate deviation that keeps it reproducible under ``torch.manual_seed``."""
-    support_grad = False
+    0.8**epoch + 0.1.  The random prior net (rand_prior) needs reduced_dim == num_cont or no numeric columns.  Predict
+    draws one matrix per member on every call, at the last trained epoch's temperature."""
+    _C_FIT, _C_FIT_WS, _C_PREDICT = "hb_gumbel_fit", "hb_gumbel_fit_workspace_bytes", "hb_gumbel_predict"
 
     def __init__(self, num_cont, num_enum, num_out, **conf):
         conf.pop("basenet_cls", None)
@@ -694,7 +707,7 @@ class GumbelDeepEnsemble(DeepEnsemble):
         if num_cont > _lib.HB_DE_MAX_IN:
             raise NotImplementedError(f"GumbelDeepEnsemble: num_cont = {num_cont} exceeds the limit of {_lib.HB_DE_MAX_IN}")
         super().__init__(num_cont, num_enum, num_out, **conf)
-        self.basenet_cls = _reference_gumbelnet()
+        self.basenet_cls = _reference_net("gumbel_linear", "GumbelNet")
         self.conf["basenet_cls"] = self.basenet_cls
         self.temperature = 0.1          # GumbelSelectionLayer's default until a fit sets the last epoch's
 
@@ -716,6 +729,10 @@ class GumbelDeepEnsemble(DeepEnsemble):
         bs = min(n, int(self.batch_size))
         return (self.num_ensembles, int(self.num_epochs), -(-n // bs), self.reduced_dim, self.num_cont)
 
+    def eval_draws_shape(self):
+        """Shape of predict's explicit uniforms: one matrix per member, [E, reduced_dim, num_cont]."""
+        return (self.num_ensembles, self.reduced_dim, self.num_cont)
+
     def init_member(self) -> torch.Tensor:
         """GumbelNet's initialisation from torch's global generator: BaseNet's (xavier with the ReLU gain, zero biases) over
         its own layout; with numeric columns the hidden layers are then rebuilt with nn.Linear's default initialisation
@@ -732,81 +749,17 @@ class GumbelDeepEnsemble(DeepEnsemble):
         base["feature_select.logits"] = torch.zeros(self.reduced_dim, self.num_cont)
         return state_dict_to_raw(base, self.layout)
 
-    # ------------------------------------------------------------------ fit (gumbel_linear.py:69-100)
-    def fit(self, Xc_, Xe_, y_, perm=None, draws=None, eval_draws=None):
-        """perm: as DeepEnsemble.fit.  draws: optional training uniforms (``draws_shape``); otherwise Philox draws on the
-        device.  eval_draws: optional [E, reduced_dim, num_cont] uniforms of the noise estimate's predict (tests replaying
-        the reference's own draws)."""
-        Xc, Xe, y, valid = self._prepare_fit(Xc_, Xe_, y_, perm)
-        if draws is not None:
-            draws = torch.as_tensor(draws, dtype=torch.float32)
-            if tuple(draws.shape) != self.draws_shape(y.shape[0]):
-                raise ValueError(f"draws must be {list(self.draws_shape(y.shape[0]))}, got {list(draws.shape)}")
-        self._fit_dev(Xc, Xe, y, perm, self.seed, draws)
-        self._finish_fit(Xc_, Xe_, y_, valid, draws=eval_draws)
+    def _layout_args(self):
+        return (self.reduced_dim,)
 
-    def _fit_dev(self, Xc, Xe, y, perm, seed, draws=None):
-        lib, dev, E = _lib.lib(), self.device, self.num_ensembles
-        n, T = y.shape[0], int(self.num_epochs)
-        xc = Xc.to(dev, torch.float32).contiguous() if self.num_cont > 0 else None
-        xe = Xe.to(dev, torch.int32).contiguous() if self.num_enum > 0 else None
-        yd = y.to(dev, torch.float32).contiguous()
-        pd_ = None if perm is None else torch.as_tensor(perm).to(dev, torch.int32).contiguous()
-        dd = None if draws is None else draws.to(dev, torch.float32).contiguous()
-        r = self.reduced_dim
-        need = int(lib.hb_gumbel_fit_workspace_bytes(C.byref(self._spec), r, E))
-        self.fit_ws = torch.empty(need, dtype=torch.uint8, device=dev)
-        losses = torch.empty(E, max(1, T), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(lib.hb_gumbel_fit(_lib.ptr(xc), _lib.ptr(xe), _lib.ptr(yd), n, C.byref(self._spec), r, E,
-                                         _lib.ptr(self.params), float(self.lr), float(self.l1), int(self.batch_size), T,
-                                         _lib.ptr(pd_), _lib.ptr(dd), seed & (2 ** 64 - 1), _lib.ptr(losses),
-                                         _lib.ptr(self.fit_ws), need, _lib.stream_ptr()), "hb_gumbel_fit")
-        self.losses = losses[:, :T]
-        if T > 0:               # predict uses the last trained epoch's temperature
-            self.temperature = gumbel_epoch_temperature(T - 1)
-        if self.verbose:
-            self._print_losses()
+    def _fit_args(self):
+        return (self.reduced_dim,)
 
-    def fit_state(self):
-        """Views of the fit workspace: Adam's exp_avg, exp_avg_sq and the last step's gradient, each [E, P]."""
-        E, P = self.num_ensembles, self.P
-        return tuple(self.fit_ws.view(torch.float32)[:3 * E * P].view(3, E, P))
+    def _predict_args(self):
+        """reduced_dim and the temperature, and the workspace of each member's W [E, reduced_dim, num_cont]."""
+        ws = torch.empty(max(1, self.num_ensembles * self.reduced_dim * self.num_cont), dtype=torch.float32,
+                         device=self.device)
+        return (self.reduced_dim, float(self.temperature)), ws
 
-    # ------------------------------------------------------------------ predict
-    def _predict_dev(self, Xs, xe, grad=False, member=-1, draws=None, seed=None, counter=0):
-        if grad:
-            raise NotImplementedError("GumbelDeepEnsemble: no input gradients (support_grad = False)")
-        lib, dev = _lib.lib(), self.device
-        assert self.fitted, "fit() first"
-        m = (Xs if Xs is not None else xe).shape[0]
-        E, r = self.num_ensembles, self.reduced_dim
-        xm, xa, ym, ys = self._scal_dev()
-        mu = torch.empty(m, self.num_out, dtype=torch.float32, device=dev)
-        var = torch.empty(m, self.num_out, dtype=torch.float32, device=dev) if member < 0 else None
-        if draws is not None:
-            draws = torch.as_tensor(draws).to(dev, torch.float32).contiguous()
-            if tuple(draws.shape) != (E, r, self.num_cont):
-                raise ValueError(f"eval draws must be [{E}, {r}, {self.num_cont}], got {list(draws.shape)}")
-        elif seed is None:
-            seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-        ws = torch.empty(max(1, E * r * self.num_cont), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(lib.hb_gumbel_predict(_lib.ptr(Xs), _lib.ptr(xe), m, C.byref(self._spec), r, float(self.temperature),
-                                             E, _lib.ptr(self.params), _lib.ptr(xm), _lib.ptr(xa), _lib.ptr(ym), _lib.ptr(ys),
-                                             int(member), _lib.ptr(draws), int(seed or 0) & (2 ** 64 - 1),
-                                             int(counter) & (2 ** 64 - 1), _lib.ptr(mu), _lib.ptr(var), _lib.ptr(ws),
-                                             ws.numel() * 4, _lib.stream_ptr()), "hb_gumbel_predict")
-        return mu, var
-
-    predict = FeDeepEnsemble.predict
-    sample_y = FeDeepEnsemble.sample_y
-
-
-def _reference_gumbelnet():
-    """GumbelNet of an installed HEBO, or None."""
-    try:  # pragma: no cover - depends on the environment
-        from hebo.models.nn.gumbel_linear import GumbelNet
-        return GumbelNet
-    except Exception:
-        return None
+    def _trained_epochs(self, T: int):
+        self.temperature = gumbel_epoch_temperature(T - 1)      # predict uses the last trained epoch's temperature

@@ -55,6 +55,16 @@ def hebo_y_transform(y: np.ndarray, strict: bool = False) -> torch.Tensor:
         return torch.FloatTensor(y).clone()
 
 
+# the surrogate of each model_name that HEBO and BO take
+MODELS = {"gp": GP, "deep_ensemble": DeepEnsemble, "fe_deep_ensemble": FeDeepEnsemble, "gumbel": GumbelDeepEnsemble}
+
+
+def check_model_name(owner: str, model_name: str) -> None:
+    if model_name not in MODELS:
+        raise NotImplementedError(f"{owner}: model_name {model_name!r} is not supported, only "
+                                  + ", ".join(map(repr, MODELS)))
+
+
 def kappa_schedule(n_obs: int, q: int, D: int) -> float:
     """hebo.py:156-160."""
     it = max(1, n_obs // q)
@@ -67,9 +77,7 @@ class HEBO:
                  scramble_seed: Optional[int] = None, n_candidates: int = 10000, device: str = "cuda",
                  n_refine: int = 0, refine_sigma: float = 0.05, acq_optimizer: str = "sobol", evo_pop: int = 100,
                  evo_iters: int = 100, lb=None, _constraint=None, model_name: str = "gp", acq_cls=MACE):
-        if model_name not in ("gp", "deep_ensemble", "fe_deep_ensemble", "gumbel"):
-            raise NotImplementedError(f"HEBO: model_name {model_name!r} is not supported, only 'gp', 'deep_ensemble', "
-                                      "'fe_deep_ensemble' and 'gumbel'")
+        check_model_name("HEBO", model_name)
         if acq_cls is not MACE and (n_refine or _constraint is not None):
             raise ValueError("n_refine and the embedding constraint are defined for the MACE front only; an acq_cls other "
                              "than MACE takes neither")
@@ -195,8 +203,7 @@ class HEBO:
     # ------------------------------------------------------------------ suggest
     def _fit(self):
         """hebo.py:127-147: power-transformed y, and on ANY failure (transform or fit) a refit on the raw y."""
-        cls = {"gp": GP, "deep_ensemble": DeepEnsemble, "fe_deep_ensemble": FeDeepEnsemble,
-               "gumbel": GumbelDeepEnsemble}[self.model_name]
+        cls = MODELS[self.model_name]
 
         def build(y):
             model = cls(self.d, self.e, 1, device=self.device, **self.model_config)
