@@ -246,6 +246,7 @@ int launch_pareto_k(const float *F, int64_t m, int64_t K, int32_t *idx_out, int3
 //   buffer [(capacity + 1), FRONT_W] floats.  row 0 = (count, overflow flag, 0...);  row 1 + j = (F0, F1, F2, mu, sigma,
 //   id_lo, id_hi, 0) of front row j, the global candidate id split in two fp32-exact 24-bit halves; unused rows = +inf.
 constexpr int FRONT_W = 8;
+constexpr int64_t FRONT_MAX_ROW_OFFSET = (int64_t(1) << 48) - (int64_t(1) << 31);
 
 __global__ void __launch_bounds__(256) front_pack_kernel(const float *__restrict__ F, const float *__restrict__ mu,
                                                          const float *__restrict__ var, const int32_t *__restrict__ idx,
@@ -280,7 +281,9 @@ __global__ void __launch_bounds__(256) front_pack_kernel(const float *__restrict
   o[1] = make_float4(v[4], v[5], v[6], v[7]);
 }
 
-// gathered buffers [world][capacity + 1][FRONT_W] -> objective matrix [world * capacity, 3] (+inf beyond each rank's count)
+// gathered buffers [world][capacity + 1][FRONT_W] -> objective matrix [world * capacity, 3], NaN beyond each rank's count:
+// the filter excludes a NaN row, whereas +inf rows do not dominate one another and, with every rank's front empty, would
+// all come back as front rows
 __global__ void __launch_bounds__(256) front_unpack_kernel(const float *__restrict__ all, int world, int capacity,
                                                            float *__restrict__ Fm, int32_t *__restrict__ overflow) {
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
@@ -291,9 +294,9 @@ __global__ void __launch_bounds__(256) front_unpack_kernel(const float *__restri
   if (j == 0 && (k > capacity || hdr[1] != 0.0f)) atomicOr(overflow, 1);
   const float *row = hdr + (int64_t)(j + 1) * FRONT_W;
   const bool valid = j < min(k, capacity);
-  Fm[(int64_t)p * 3 + 0] = valid ? row[0] : INFINITY;
-  Fm[(int64_t)p * 3 + 1] = valid ? row[1] : INFINITY;
-  Fm[(int64_t)p * 3 + 2] = valid ? row[2] : INFINITY;
+  Fm[(int64_t)p * 3 + 0] = valid ? row[0] : NAN;
+  Fm[(int64_t)p * 3 + 1] = valid ? row[1] : NAN;
+  Fm[(int64_t)p * 3 + 2] = valid ? row[2] : NAN;
 }
 
 __global__ void __launch_bounds__(256) front_gather_kernel(const float *__restrict__ all, int world, int capacity,
@@ -325,6 +328,8 @@ __global__ void __launch_bounds__(256) front_gather_kernel(const float *__restri
 int launch_front_pack(const float *F, const float *mu, const float *var, const int32_t *idx, const int32_t *count,
                       int64_t row_offset, int64_t capacity, float *out, cudaStream_t st) {
   if (capacity <= 0 || capacity > 0x3fffffff) return HB_ERR_INVALID;
+  // global ids row_offset + idx (idx < 2^31) must stay below 2^48, the range of the two 24-bit fp32 halves
+  if (row_offset < 0 || row_offset > FRONT_MAX_ROW_OFFSET) return HB_ERR_INVALID;
   front_pack_kernel<<<(int)ceil_div(capacity + 1, 256), 256, 0, st>>>(F, mu, var, idx, count, row_offset, (int)capacity, out);
   count_launches(1);
   HB_LAUNCH_CHECK("front_pack");

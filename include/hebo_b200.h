@@ -489,8 +489,11 @@ int32_t hb_embed_violation(const float *Y, int64_t m, int64_t e, const float *B,
  * id_lo, id_hi, 0) with the global candidate id = id_lo + 2^24 id_hi; unused rows hold +inf objectives.
  * hb_front_pack : F [m,3], mu / var [m] (or NULL), idx / count from hb_pareto_front3, row_offset = first global id of
  *                 this shard -> out.  A front larger than `capacity` sets the overflow flag (never silently truncated).
+ *                 0 <= row_offset <= 2^48 - 2^31 (ids of int32 rows stay below 2^48, exact in the two halves), else
+ *                 HB_ERR_INVALID before any launch.
  * hb_front_merge: all_buf [world][capacity + 1][8] (the all-gathered buffers) -> out [(world * capacity + 1), 8]: the
- *                 non-dominated rows of the union in ascending global-id order.  No host synchronisation in either call. */
+ *                 non-dominated rows of the union in ascending global-id order; rows beyond a rank's count never take
+ *                 part, so ranks whose fronts are all empty merge to count 0.  No host synchronisation in either call. */
 int64_t hb_front_merge_workspace_bytes(int64_t world, int64_t capacity);
 int32_t hb_front_pack(const float *F, const float *mu, const float *var, const int32_t *idx, const int32_t *count,
                       int64_t row_offset, int64_t capacity, float *out, void *stream);

@@ -130,6 +130,17 @@ def test_tensor_core_stages_reject_bad_sizes_null_pointers_and_short_workspaces(
         assert lib.hb_kinv_tc(640, p, p, short, None) == bad, short
 
 
+def test_front_pack_rejects_row_offsets_outside_the_id_range(lib):
+    """hb_front_pack stores a global id row_offset + row (row < 2^31) as two 24-bit fp32 halves, exact below 2^48: a
+    negative row_offset, or one above 2^48 - 2^31, is refused before any launch.  The pointers are fake and never
+    dereferenced."""
+    bad = _lib.HB_ERR_INVALID
+    p = ctypes.c_void_p(16)
+    top = (1 << 48) - (1 << 31)
+    for off in (-1, -(1 << 31), top + 1, 1 << 48, (1 << 62)):
+        assert lib.hb_front_pack(p, p, p, p, p, off, 64, p, None) == bad, off
+
+
 @pytest.mark.parametrize("ws_bytes", ["short", -1, -(1 << 40)])
 def test_workspace_size_is_checked_as_a_signed_count(lib, ws_bytes):
     """A workspace one byte short, or of negative size, is refused before any launch.  A negative int64 must not pass the

@@ -56,7 +56,8 @@ def merge_fn_torch(all_buf, world, capacity):
     over = bool((counts > capacity).any()) or bool((all_buf[:, 0, 1] != 0).any())
     body = all_buf[:, 1:, :].reshape(world * capacity, FRONT_W)
     valid = (torch.arange(capacity)[None, :] < counts.clamp(max=capacity)[:, None]).reshape(-1)
-    Fm = torch.where(valid[:, None], body[:, :3], torch.full_like(body[:, :3], float("inf")))
+    # rows beyond a rank's count are NaN, which the filter excludes: +inf rows would not dominate one another
+    Fm = torch.where(valid[:, None], body[:, :3], torch.full_like(body[:, :3], float("nan")))
     keep = torch.from_numpy(O.pareto_front(Fm.numpy()))
     out = torch.zeros(world * capacity + 1, FRONT_W)
     out[1:, :3] = float("inf")
@@ -138,3 +139,37 @@ def test_single_process_path_is_the_local_buffer():
     # ids above 2^24 survive the two-halves encoding
     buf2 = pack_fn_torch(F, mu, var, idx, cnt, (1 << 30) + 5, 64)
     assert np.array_equal(front_read(buf2)[0].numpy(), ref + (1 << 30) + 5)
+
+
+def _rank_buffers(counts, capacity, m=400, offset_step=1000):
+    """One packed buffer per rank whose local front has counts[r] rows (0: every objective of the shard is NaN)."""
+    bufs = []
+    for r, want in enumerate(counts):
+        F, mu, var = _fake_objectives(m, seed=r + 1)
+        idx, cnt = front_fn_torch(F)
+        if want == 0:
+            F = torch.full_like(F, float("nan"))
+            idx, cnt = front_fn_torch(F)
+            assert int(cnt[0]) == 0
+        bufs.append(pack_fn_torch(F, mu, var, idx, cnt, r * offset_step, capacity))
+    return torch.stack(bufs)
+
+
+def test_merge_of_empty_fronts_is_empty():
+    """Ranks whose local fronts are all empty merge to an empty front, not to world * capacity padding rows."""
+    for world, capacity in ((2, 4), (8, 64)):
+        out = merge_fn_torch(_rank_buffers([0] * world, capacity), world, capacity)
+        assert int(out[0, 0]) == 0 and int(out[0, 1]) == 0
+        gidx, Ff, extra = front_read(out)
+        assert gidx.numel() == 0 and Ff.shape == (0, 3)
+
+
+def test_merge_ignores_empty_ranks():
+    """A merge in which some ranks are empty equals the merge of the non-empty ranks alone."""
+    capacity = 256
+    all_buf = _rank_buffers([1, 0, 1, 0], capacity)
+    full = merge_fn_torch(all_buf, 4, capacity)
+    part = merge_fn_torch(all_buf[[0, 2]], 2, capacity)
+    assert int(full[0, 0]) == int(part[0, 0]) > 0
+    for a, b in zip(front_read(full), front_read(part)):
+        assert torch.equal(a, b)
