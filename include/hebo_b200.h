@@ -99,7 +99,8 @@ int32_t     hb_profile_collect(double *total_ms, int32_t *n_launches);
 /* rows_flagged[0] = candidate rows that went through the tensor path since the last reset, [1] = how many of them the
  * precision guard re-contracted on the FP32 pipe (synchronises the device; current device only). */
 int32_t     hb_guard_stats(uint64_t *rows_flagged, int32_t reset);
-/* Workspace sizes in BYTES for the fused calls below. */
+/* Workspace sizes in BYTES for the fused calls below.
+ * The fit workspace is about 44 NP^2 bytes (eleven fp32 [NP, NP] arrays), 47.9 GB at NP = 32 896. */
 int64_t     hb_fit_workspace_bytes(int64_t n, int64_t d);
 int64_t     hb_fit_workspace_bytes_ex(int64_t n, int64_t d, const hb_model_spec_t *spec);
 int64_t     hb_num_params(int64_t d, const hb_model_spec_t *spec);      /* P: length of raw / grad / a Langevin row */
